@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- stereo pairs/sec for GwcNet @256x512, D=192 (BASELINE.json metric), 1..8 x B200.
+"""bench.py -- stereo pairs/sec for GwcNet @256x512, D=192 (BASELINE.json metric), 1..8 x H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch 8]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch 8] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one GwcNet inference forward (2D backbone -> cost volume -> 3D aggregation -> soft-argmin) over one batch
@@ -13,17 +13,20 @@ Reported in one JSON line (rank 0):
   value      pairs/s, inputs already resident in HBM, CUDA-event timed, max over ranks
   e2e        same metric through the public model call with PINNED HOST inputs: H2D copy of the images + ground truth
              and D2H read-back of the per-image EPE inside the timed region, every step
-  roofline   the DOMINANT kernel family of the step (3x3x3 Conv3d / ConvTranspose3d on tcgen05, split-operand fp32-accurate
+  roofline   the DOMINANT kernel family of the step (3x3x3 Conv3d / ConvTranspose3d on wgmma, split-operand fp32-accurate
              MMAs; tensor-bound), timed live with CUDA events around every launch inside the timed steps
-  roofline_volume  the cost-volume kernel the metric names (HBM-bound) against MEASURED_PEAKS.json hbm_gbs and the 8 TB/s nominal;
+  roofline_volume  the cost-volume kernel the metric names (HBM-bound) against MEASURED_PEAKS.json hbm_gbs and the 3.35 TB/s nominal;
              roofline_cuda_core = the fp32 layers still on CUDA cores
   cpu_baseline  the UNMODIFIED reference GwcNet (oracle/_ref, staged by oracle/make_ref.py; kind "reference") on the host
              cores, bounded sample -- the oracle port (kind "port") only when the staged reference is absent
   parity_epe_px  mean |disparity - reference| of one pair of the timed batch: this library on the GPU vs that CPU forward
   dropin     the same step through the reference's OWN GwcNet class + openstereo_b200.patch.patch() (what a maintainer gets)
-  comparators  the unmodified reference on the same B200 (cuDNN fp32, TF32 off) and its Triton gwc kernel
+  comparators  the unmodified reference on the same GPU (cuDNN fp32, TF32 off) and its Triton gwc kernel
                (fast_foundationstereo/core/submodule.py:443-478) against this library's gwc volume kernel
 --impl reference times the reference's own CPU implementation as the reference arm.
+--dump-outputs DIR writes what the last timed step returned (rank 0): DIR/disp_pred.npy, the (B, 256, 512) float32 disparity
+  maps, and DIR/epe_partial.npy, the (B, 2) float32 per-image EPE partial sums.  Inputs and weights are seeded, so two builds
+  run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -41,9 +44,9 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 METRIC = "stereo_pairs_per_sec_gwcnet_256x512_d192"
-# dram__bytes_read.sum + dram__bytes_write.sum per launch at B = 8 from `ncu --set full` captures of this command
-# (profiles/README.md names the capture each figure comes from); None = not captured for the current kernel version
-NCU_TRAFFIC = {"volume_kernel": 919946496, "conv3d_tc_kernel": 765931264}
+# dram__bytes_read.sum + dram__bytes_write.sum per launch at B = 8, by kernel name, where a capture of the current kernel version
+# exists; a missing name reports traffic None
+NCU_TRAFFIC = {}
 CFG = {"MAX_DISP": 192, "USE_CONCAT_VOLUME": True, "CONCAT_CHANNELS": 12, "DOWNSAMPLE": 4, "NUM_GROUPS": 40}
 H, W = 256, 512
 
@@ -53,8 +56,8 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             d = json.load(f)
-        return float(d.get("hbm_gbs", 6650.0)), "measured (MEASURED_PEAKS.json)", float(d.get("sm_max_mhz", 1965.0))
-    return 6650.0, "fallback (B200_PROFILING.md)", 1965.0
+        return float(d.get("hbm_gbs", 3350.0)), "measured (MEASURED_PEAKS.json)", float(d.get("sm_max_mhz", 1980.0))
+    return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s, 1980 MHz max SM clock)", 1980.0
 
 
 def synthetic_weights(model, seed=1):
@@ -253,7 +256,7 @@ def run_ours(args):
     B = args.batch
     model = synthetic_weights(host_models.GwcNet(CFG)).eval().to(dev)
     gen = torch.Generator().manual_seed(1234 + rank)
-    rot = args.rotate                                               # distinct input batches: rot * 12.6 MB > L2 (126 MB)
+    rot = args.rotate                                               # distinct input batches: rot * 12.6 MB > L2 (50 MB)
     host_left = [torch.randn(B, 3, H, W, generator=gen).pin_memory() for _ in range(rot)]
     host_right = [torch.randn(B, 3, H, W, generator=gen).pin_memory() for _ in range(rot)]
     host_gt = [(torch.rand(B, H, W, generator=gen) * 190 + 1).pin_memory() for _ in range(rot)]
@@ -262,11 +265,15 @@ def run_ours(args):
     dev_gt = [t.to(dev) for t in host_gt]
     host_epe = torch.empty(B, 2).pin_memory()
 
+    last = {}                                                       # what the most recent resident step returned
+
     def step_resident(i):
         k = i % rot
         with torch.no_grad():
             disp = model({"left": dev_left[k], "right": dev_right[k]})["disp_pred"]
-            return ops.epe_partial(disp, dev_gt[k], CFG["MAX_DISP"])
+            part = ops.epe_partial(disp, dev_gt[k], CFG["MAX_DISP"])
+            last["disp_pred"], last["epe_partial"] = disp, part
+            return part
 
     def step_e2e(i):
         k = i % rot
@@ -326,6 +333,8 @@ def run_ours(args):
     ms, launches, prof, parts = timed(step_resident, args.steps, profile=True)
     if os.environ.get("OSB_NCU_RANGE"):
         torch.cuda.cudart().cudaProfilerStop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     ms_e2e, _, _, _ = timed(step_e2e, args.steps, profile=False)
     clocks = sampler.stop(args.gpus) if rank == 0 else None
     if rank != 0:
@@ -352,7 +361,7 @@ def run_ours(args):
     if vol_ms:
         ach = vol_bytes / vol_ms / 1e6
         roof_vol = {"kernel": "volume_kernel (gwc+concat fused)", "bound": "hbm", "achieved": round(ach, 1), "peak": hbm_peak,
-                    "unit": "GB/s", "frac": round(ach / hbm_peak, 4), "frac_of_8TBs_nominal": round(ach / 8000.0, 4),
+                    "unit": "GB/s", "frac": round(ach / hbm_peak, 4), "frac_of_nominal": round(ach / 3350.0, 4),
                     "peak_source": peak_src, "alg_bytes_per_launch": vol_bytes, "ms_per_launch": round(vol_ms, 4),
                     "traffic": NCU_TRAFFIC.get("volume_kernel") if B == 8 else None, "share_of_step": round(vol_total / ms, 4)}
     # ---- 3D aggregation (SURVEY.md section 8a row a6): MACs per pair of GwcNet-gc at D'=48, H'=64, W'=128
@@ -379,7 +388,7 @@ def run_ours(args):
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             bf16_peak = float(json.load(f).get("bf16_tflops_sustained"))
     except Exception:
-        bf16_peak = 1400.0
+        bf16_peak = 989.0                                           # H100 SXM data sheet, dense 16-bit
     mma_kind = ops.tc_operand_kind()                                # "tf32" (3xTF32) or "f16" (3xFP16 split)
     tc_peak = bf16_peak / (2.0 if mma_kind == "tf32" else 1.0)      # dense tf32 = half the 16-bit rate
     roofline = None
@@ -393,7 +402,7 @@ def run_ours(args):
                           "useful_tflops": round(2 * macs[n] * B * args.steps / (tot / 1e3) / 1e12, 1)}
         ran = [n for n in tc_names if kernel_stats(n)[2] > 0]
         useful = 2 * sum(macs[n] for n in ran) * B * args.steps / (tc_total / 1e3) / 1e12
-        roofline = {"kernel": "tcgen05 conv family (conv3d_tc / tcg / tcs2 / tcdc kernels: 3x3x3 s1, s2, transposed; the backbone's 3x3 "
+        roofline = {"kernel": "wgmma conv family (conv3d_tc / tcg / tcs2 / tcdc kernels: 3x3x3 s1, s2, transposed; the backbone's 3x3 "
                               "blocks as one-plane volumes), kind::%s, 3 split-operand MMAs per fp32-accurate product" % mma_kind,
                     "bound": "tensor", "achieved": round(3 * useful, 1), "peak": round(tc_peak, 1), "unit": "TFLOP/s",
                     "frac": round(3 * useful / tc_peak, 4), "useful_fp32_equivalent_tflops": round(useful, 1),
@@ -404,14 +413,14 @@ def run_ours(args):
     cc_names = ["osb_conv3d_k3_bn_act_fwd", "osb_deconv3d_bn_act_fwd", "osb_conv3d_1x1_bn_act_fwd", "osb_conv1x1_ndhwc_fwd",
                 "osb_conv3d_k3_c1_ndhwc_fwd"]
     cc_total = sum(kernel_stats(n)[2] for n in cc_names)
-    fp32_peak = 148 * 128 * 2 * sm_max * 1e6 / 1e12                 # derived: SMs x fp32 lanes x 2 x max clock
+    fp32_peak = 132 * 128 * 2 * sm_max * 1e6 / 1e12                 # derived: SMs x fp32 lanes x 2 x max clock
     roof_cc = None
     if cc_total > 0:
         cc_flops = 2 * (agg_macs - (sum(macs[n] for n in tc_names[:3]) if tc_total > 0 else 0)) * B
         ach = cc_flops * args.steps / (cc_total / 1e3) / 1e12
         roof_cc = {"kernel": "fp32 CUDA-core layers left in the aggregation", "bound": "fp32_fma", "achieved": round(ach, 2),
                    "peak": round(fp32_peak, 1), "unit": "TFLOP/s", "frac": round(ach / fp32_peak, 4),
-                   "peak_source": "derived 148 SM x 128 lanes x 2 x %.0f MHz" % sm_max,
+                   "peak_source": "derived 132 SM x 128 lanes x 2 x %.0f MHz" % sm_max,
                    "alg_flops_per_step": cc_flops, "share_of_step": round(cc_total / ms, 4), "traffic": None}
     shares = {}
     for name, ev in prof.items():
@@ -446,7 +455,7 @@ def run_ours(args):
         "config": {"workload": "GwcNet cfgs/gwcnet/gwcnet_sceneflow.yaml, batch %d/GPU @256x512 D=192 (BASELINE configs[1])" % B,
                    "global_batch": B * world, "parallelism": "dp%d batch-shard, 1 all_gather of per-image EPE" % world,
                    "model_path": "openstereo_b200.host_models.GwcNet (state_dict-compatible mirror; `dropin` = the reference's class + patch())",
-                   "l2": "inputs rotate over %d distinct batches (%.0f MB > 126 MB L2); per-step activations ~6 GB" % (rot, rot * 2 * B * 3 * H * W * 4 / 1e6),
+                   "l2": "inputs rotate over %d distinct batches (%.0f MB > 50 MB L2); per-step activations ~6 GB" % (rot, rot * 2 * B * 3 * H * W * 4 / 1e6),
                    "weights": "synthetic seeded init (no checkpoints ship with the reference)"},
         "clocks": clocks,
         "e2e": {"value": round(e2e_value, 3), "unit": "pairs/s", "ms_per_step": round(ms_e2e / args.steps, 4),
@@ -467,7 +476,7 @@ def run_comparators(args, dev, B, dev_left, dev_right, dev_gt, mirror_value):
     """N = 1 legs that need the staged reference (oracle/_ref).  Each is CUDA-event timed after warm-up, resident inputs, same
     synthetic weights and batches as the main arm.
       dropin                     the reference's own GwcNet class + patch(): pairs/s and its ratio to the mirror's value
-      reference_gpu_cudnn_fp32   the UNMODIFIED reference forward on this B200 (cuDNN fp32, TF32 off) -- SURVEY.md section 8d's GPU bar
+      reference_gpu_cudnn_fp32   the UNMODIFIED reference forward on this GPU (cuDNN fp32, TF32 off) -- SURVEY.md section 8d's GPU bar
       triton_gwc                 the reference's Triton gwc kernel (normalize=False, / K to match build_gwc_volume's mean)
                                  against osb_gwc_volume_fwd at the config-2 shape (8, 320, 64, 128), D' = 48, G = 40"""
     from oracle import _reference_shim as shim
@@ -539,6 +548,29 @@ def run_comparators(args, dev, B, dev_left, dev_right, dev_gt, mirror_value):
     return dropin, comp
 
 
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each output of the last timed step as <out_dir>/<name>.npy (float32), at most DUMP_CAP_BYTES in all.  An output
+    that does not fit (large --batch) is replaced by a fixed sample: the values at flat indices drawn with seed 0 (sorted) in
+    <name>.npy and those indices, as float64, in <name>_index.npy."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    host = {name: t.detach().float().cpu().numpy() for name, t in arrays.items()}
+    small = sum(a.nbytes for a in host.values() if a.nbytes <= 1 << 20)       # small outputs are always written whole
+    budget = DUMP_CAP_BYTES - small - 4096 * len(host)                       # .npy headers
+    big = [name for name, a in host.items() if a.nbytes > 1 << 20]
+    for name, a in host.items():
+        if name in big and sum(host[n].nbytes for n in big) > budget:
+            k = budget // len(big) // 12                                   # 4 bytes of value + 8 bytes of index per sample
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=k, replace=False))
+            np.save(os.path.join(out_dir, name + ".npy"), a.reshape(-1)[idx])
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+        else:
+            np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -549,6 +581,8 @@ def main():
     ap.add_argument("--rotate", type=int, default=12)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-comparators", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * openstereo_b200.h -- C ABI of the B200-native cost-volume hot path for OpenStereo.
+ * openstereo_b200.h -- C ABI of the H100-native cost-volume hot path for OpenStereo.
  *
  * Drop-in boundary.  The reference (XiandaGuo/OpenStereo) has no operator registry: the hot path is
  * a set of plain Python callables on torch.Tensor (SURVEY.md section 8b).  The reference's own
@@ -55,9 +55,10 @@ int osb_tc_overflow_count(osb_stream_t stream, int reset, unsigned int* count);
  * reads *host_pinned after an event recorded behind it has completed; the Python engines do that at the start of their next call). */
 int osb_tc_overflow_poll(osb_stream_t stream, unsigned int* host_pinned);
 const unsigned int* osb_tc_overflow_flag(void);
-/* Expected round-towards-zero loss per accumulating tcgen05.mma, undone by the conv epilogues (csrc/tc_common.cuh: rz_kappa;
- * DESIGN.md section 4.3).  Process-wide; returns the previous value; 0 switches the correction off.  The default is the
- * constant measured on B200 (profiles/r2_parity_bisect.md); the setter exists for that calibration. */
+/* Expected round-towards-zero loss per accumulating tensor-core MMA, undone by the conv epilogues (csrc/tc_common.cuh: rz_kappa;
+ * DESIGN.md section 4.3).  Process-wide; returns the previous value; 0 switches the correction off.  The default has not been
+ * calibrated separately for H100; with it the full-size GwcNet / PSMNet tests stay within their 1e-3 px EPE bar there.  The
+ * setter exists for calibration (tools/parity_bisect.py). */
 float osb_set_rz_kappa(float kappa);
 
 /* ---------------------------------------------------------------- cost-volume constructors --- */
@@ -145,9 +146,9 @@ int osb_conv3d_1x1_bn_act_fwd(const float* x0, const float* x1, int Cin0, const 
                               const float* gate, float* y, int B, int Cin, int Cout, int D, int H,
                               int W, int act, int sigmoid_out, osb_stream_t stream);
 
-/* ------------------------------------------------------- tensor-core (tcgen05) variant of the 3x3x3 conv ----- */
+/* ------------------------------------------------------- tensor-core (wgmma) variant of the 3x3x3 conv ----- */
 
-/* Same operator as osb_conv3d_k3_bn_act_fwd (stride 1) for the full-resolution layers, computed on the 5th-gen tensor
+/* Same operator as osb_conv3d_k3_bn_act_fwd (stride 1) for the full-resolution layers, computed on the Hopper (wgmma) tensor
  * cores with 3xFP16 operand splitting (fp32-accurate, see csrc/tc_common.cuh, conv3d_tc.cu, conv3d_tcg.cu).  Supported shapes:
  * osb_conv3d_tc_supported / osb_conv3d_tc_kc.  x is CHANNELS-LAST (B,D,H,W,Cin) fp32; w_split is the host-split fp16 weight
  * tensor [3 kd][Cin/kc][3 kh][3*Cout (kw-major)][kc hi | kc lo] of w * 2^e_c (ops.pack_tc_weight; e_c per output channel);

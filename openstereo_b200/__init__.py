@@ -1,4 +1,4 @@
-"""B200-native cost-volume hot path for OpenStereo (sm_100a CUDA kernels behind a C ABI).
+"""H100-native cost-volume hot path for OpenStereo (sm_90a CUDA kernels behind a C ABI).
 
 Sub-modules are loaded on first access (``openstereo_b200.ops`` etc.) so that ``python -m openstereo_b200.build`` can
 run before the shared library exists.  The first access to ``ops`` / ``_lib`` loads ``lib/libopenstereo_b200.so`` and

@@ -1,4 +1,4 @@
-"""Hot-path engines: run the reference's 3D aggregation modules with the sm_100a kernels.
+"""Hot-path engines: run the reference's 3D aggregation modules with the sm_90a kernels.
 
 Each engine is built FROM an existing module tree (the reference's own ``GwcDispProcessor`` /
 ``PSMAggregator`` / StereoBase ``Hourglass``, or the host mirrors in host_models.py): it reads the
@@ -24,7 +24,7 @@ class _Packed:
     __slots__ = ("w", "scale", "shift", "stride", "kernel", "transposed", "cin", "cout", "_w5", "_tc")
 
     def __init__(self, conv, bn=None):
-        self._tc = {}                                           # K-chunk -> hi/lo split weight for the tcgen05 kernels
+        self._tc = {}                                           # K-chunk -> hi/lo split weight for the wgmma kernels
         self._w5 = conv.weight.detach() if conv.weight.dim() == 5 else None
         self.cin, self.cout = (conv.in_channels, conv.out_channels)
         self.transposed = isinstance(conv, (torch.nn.ConvTranspose3d, torch.nn.ConvTranspose2d))
@@ -427,7 +427,7 @@ class StereoBaseAggregation(_Engine):
         return (c + 31) // 32 * 32
 
     def tc_route_ok(self, shape):
-        """True when the 1/8 and 1/16 levels and the two upper transposed convs of this hourglass have tcgen05 variants for an
+        """True when the 1/8 and 1/16 levels and the two upper transposed convs of this hourglass have wgmma variants for an
         input volume of `shape` (B, C, D', H', W'); the 1/32 level (6 % of the MACs at config 3) stays on the CUDA-core kernels."""
         if not USE_TENSOR_CORES:
             return False
@@ -488,7 +488,7 @@ class StereoBaseAggregation(_Engine):
         for name in ("conv2_up", "conv1_up"):
             t[name] = deconv(self.up[name][0])
         # 1/32 level: 6c = 144 runs as 160 = 96 + 64 output-channel slices (N = 3 * 160 exceeds one CTA's weight buffers), the
-        # transposed conv back to 4c = 96 as 64 + 32 (N = 4 * 96 exceeds the UMMA N limit): separately packed weight slices
+        # transposed conv back to 4c = 96 as 64 + 32 (N = 4 * 96 exceeds the wgmma N limit of 256): separately packed weight slices
         (l0, _), (l1, _) = self.conv["conv3"]
         lu = self.up["conv3_up"][0]
         if P(l0.cout) == 160 and P(l0.cin) == 96 and lu.kernel == 4 and all(l._w5 is not None for l in (l0, l1, lu)):
@@ -610,7 +610,7 @@ class StereoBaseCostHead(_Engine):
         if (USE_TENSOR_CORES and lay.cout == 1 and lay._w5 is not None and lay.kernel == 3 and lay.stride == 1
                 and ops.conv3d_tc_kc(cp, 1, geo.shape[-1]) == 32):
             # 24 -> 1 head on the narrow tensor-core variant: channels zero-padded to 32 while the layout changes (one pass), the
-            # generic CUDA-core conv took 0.71 ms at config 3 (profiles/r2_c3_launches.csv)
+            # generic CUDA-core conv is the slow path at config 3
             if "head" not in lay._tc:
                 w = lay._w5.new_zeros((1, cp) + tuple(lay._w5.shape[2:]))
                 w[:, :lay.cin] = lay._w5

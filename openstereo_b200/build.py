@@ -1,10 +1,10 @@
-"""Build libopenstereo_b200.so (sm_100a) in-tree with nvcc.
+"""Build libopenstereo_b200.so (sm_90a, H100) in-tree with nvcc.
 
     python -m openstereo_b200.build [--force] [--verbose]
 
 The shared library is the whole native product: hand-written CUDA kernels behind the C ABI of
-include/openstereo_b200.h.  It is built IN-TREE (openstereo_b200/lib/) so that it travels to the
-GPU box with the repository snapshot; nvcc cross-compiles without a GPU.
+include/openstereo_b200.h.  It is built IN-TREE (openstereo_b200/lib/) so that the package imports
+from the repository tree; nvcc cross-compiles without a GPU.
 """
 import argparse
 import glob
@@ -22,7 +22,7 @@ LIB = os.path.join(LIBDIR, "libopenstereo_b200.so")
 STAMP = os.path.join(LIBDIR, "build.stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -51,7 +51,7 @@ def _fingerprint():
 
 
 def build(force=False, verbose=False):
-    """Compile every csrc/*.cu for sm_100a and link the shared library.  Returns its path."""
+    """Compile every csrc/*.cu for sm_90a and link the shared library.  Returns its path."""
     os.makedirs(LIBDIR, exist_ok=True)
     fp = _fingerprint()
     if not force and os.path.exists(LIB) and os.path.exists(STAMP) and open(STAMP).read().strip() == fp:
@@ -71,7 +71,7 @@ def build(force=False, verbose=False):
         if proc.returncode != 0:
             sys.stderr.write("\n".join(logs))
             raise RuntimeError("nvcc failed on %s" % src)
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-o", LIB] + objs
+    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-o", LIB] + objs
     res = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if res.returncode != 0:
         sys.stderr.write(res.stdout)

@@ -17,7 +17,7 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-static std::atomic<float> g_rz_kappa{1.57e-8f};   // measured on B200: profiles/r2_parity_bisect.md
+static std::atomic<float> g_rz_kappa{1.57e-8f};   // default of osb_set_rz_kappa (include/openstereo_b200.h)
 float rz_kappa() { return g_rz_kappa.load(std::memory_order_relaxed); }
 
 // Sticky fp16-range counter of the tensor-core convolutions (tc_common.cuh): one zero-initialised unsigned int per device,
@@ -56,7 +56,7 @@ int sm_count() {
   if (n > 0) return n;
   if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
     (void)cudaGetLastError();
-    n = 148;
+    n = 132;
   }
   cache[dev & 63].store(n, std::memory_order_relaxed);
   return n;

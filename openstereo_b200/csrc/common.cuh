@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of the OpenStereo cost-volume hot path.
+// Shared helpers for the sm_90a kernels of the OpenStereo cost-volume hot path.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Direct (im2col-free) fp32 3D convolutions for the hourglass aggregation, sm_100a.
+// Direct (im2col-free) fp32 3D convolutions for the hourglass aggregation, sm_90a.
 //
 //   Conv3d k3 s1/s2 + BN + act (+residual, +gate)   convbn_3d gwcnet/hourglass.py:5-16, gwcnet_disp_processor.py:8-19
 //                                                   conv3d_bn(_relu) psmnet/submodule.py:68-83,160-177
@@ -858,7 +858,7 @@ int osb_conv1x1_ndhwc_fwd(const float* x, const float* w_packed, const float* sc
   OSB_REQUIRE(act >= 0 && act <= 2, "conv1x1_ndhwc: unknown activation %d", act);
   OSB_REQUIRE(aligned16(x) && aligned16(y), "conv1x1_ndhwc: pointers must be 16-byte aligned");
   const long long groups = (voxels + 31) / 32;
-  const unsigned blocks = (unsigned)std::min<long long>((groups + 1) / 2, 148ll * 16);   // 2 warps per CTA, grid-stride over 32-voxel groups
+  const unsigned blocks = (unsigned)std::min<long long>((groups + 1) / 2, (long long)osb::sm_count() * 16);   // 2 warps per CTA, grid-stride over 32-voxel groups
   cudaStream_t s = (cudaStream_t)stream;
   if (Cin == 32 && Cout == 32) conv1x1_ndhwc_32_kernel<<<blocks, 64, 0, s>>>(x, w_packed, scale, shift, y, (size_t)voxels, act);
   else if (Cin == 64 && Cout == 64) conv1x1_ndhwc_kernel<64, 64><<<blocks, 64, 0, s>>>(x, w_packed, scale, shift, y, (size_t)voxels, act);

@@ -1,9 +1,9 @@
-// Tensor-core (tcgen05 / TMEM) implicit-GEMM Conv3d 3x3x3, stride 1, pad 1, for the full-resolution layers of the
-// hourglass aggregation (W = 128 output columns = one UMMA M tile).  fp32-accurate through 3xFP16 operand splitting
-// (tc_common.cuh):   a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi   on tcgen05.mma.kind::f16, fp32 accumulation in TMEM.
+// Tensor-core (Hopper wgmma) implicit-GEMM Conv3d 3x3x3, stride 1, pad 1, for the full-resolution layers of the hourglass
+// aggregation (W = 128 output columns = one 128-row M tile).  fp32-accurate through 3xFP16 operand splitting (tc_common.cuh):
+//   a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi   on wgmma (fp16 operands), fp32 accumulation in registers.
 // Activations are split while they are staged (fp32 in HBM -> [hi | lo] fp16 rows in shared memory); weights are split
-// and pre-scaled once on the host.  Plain TF32 / BF16 / FP16 operands break the north star's 1e-3 px EPE bar
-// (SURVEY.md section 4.3: 2.2e-2 px for TF32); the split keeps it (tests/test_zz_fullsize_gpu.py).
+// and pre-scaled once on the host.  Plain TF32 / BF16 / FP16 operands break the 1e-3 px EPE bar (SURVEY.md section 4.3);
+// the split keeps it (tests/test_zz_fullsize_gpu.py).
 //
 // Replaces the same reference modules as conv3d.cu (convbn_3d + ReLU of gwcnet/hourglass.py:5-16,
 // gwcnet_disp_processor.py:40-81; conv3d_bn(_relu) psmnet/submodule.py:68-83,160-177) for layers with W == 128.
@@ -13,40 +13,39 @@
 //   * the three kw taps are NOT realised by shifting A (that would need halo columns and unaligned tiles); instead the
 //     three weight slices are stacked along N -- one MMA of N = 3*Cout produces P_kw[m] = A[m] . B_kw for kw = 0,1,2 --
 //     and the epilogue forms D[m] = P_0[m-1] + P_1[m] + P_2[m+1] with warp shuffles (zero padding at m = -1 / 128 is
-//     implicit because a row tile spans the whole image width).  N = 96 also lifts the MMA above the ~55-cycle floor
-//     that small-N tf32 MMAs hit (tools/tc_probe.cu: N=32, 64 and 96 all take 54-56 cycles).
-//   * kh taps: output row t of the block needs input rows t-1, t, t+1: input rows stream through a shared-memory ring
-//     and each staged row feeds up to three accumulator tiles.
+//     implicit because a row tile spans the whole image width).
+//   * kh taps: output row h needs input rows h-1, h, h+1, staged through a shared-memory ring; row r of a phase meets weight
+//     slice kh = r.
 //   * an operand row is 128 bytes = [32 channels hi | 32 channels lo] fp16, SWIZZLE_128B; a K = 16 MMA step is 32 bytes, so
 //     the hi k-steps sit at descriptor offsets +0, +2 and the lo ones at +4, +6 (16-byte units) of the SAME tile.
-//   * kd taps and 32-channel Cin chunks are phases of one work item; the three kh weight slices of a phase are
-//     refilled just in time (slice kh is free after row 4+kh of a phase and needed again at row kh of the next one).
-// Work item = (image b, output plane d, block of 5 output rows); 5 accumulator tiles x 96 columns = 480 TMEM columns.
+//   * kd taps and 32-channel Cin chunks are phases of one work item; the three kh weight slices of a phase are double-buffered.
+// Work item = (image b, output plane d, output row h): ONE accumulator tile of 128 x 3*Cout fp32, held in the registers of the
+// consumer warpgroup as two m64 halves (96 registers per thread for Cout = 32).  Register capacity is what sets one tile per
+// item: the tile of the next output row cannot be live at the same time, so an input row is staged for every output row it
+// feeds (3 stagings per output row).
 //
-// Operand staging.  A first version fed the ring with TMA (cp.async.bulk.tensor, SWIZZLE_64B boxes of 64-byte rows;
-// kept as profiles/r1_conv3d_tc_tma_variant.cu.txt): correct, but ncu showed the TMA unit request-rate bound (~9 cycles
-// per 64-byte row, 7 B/clk/SM) and the tensor pipe only 34 % busy (profiles/r1_ncu_summary.md) -- and fp32 data needs
-// the split anyway.  Here the loader warps read coalesced float4 from global/L2, convert to the hi/lo fp16 pair, write
-// both halves of the row with the 128-byte swizzle applied by hand (two conflict-free STS.64) and publish the tile to the
-// tensor core through fence.proxy.async + mbarrier; arbitrary gathers (stride 2, multi-row tiles) come for free.
+// Operand staging.  The loader warps read coalesced float4 from global/L2 (or the raw rows a bulk-copy producer staged), convert
+// to the hi/lo fp16 pair, write both halves of the row with the 128-byte swizzle applied by hand (two conflict-free STS.64) and
+// publish the tile to the tensor core through fence.proxy.async + mbarrier.
 //
-// Warp roles (352 threads, 1 CTA/SM, persistent): warp 0 = MMA issuer (+ TMEM allocator), warps 1-4 = A-row loaders,
-// warps 5-8 = epilogue (TMEM -> registers -> BN/residual/ReLU -> global), warp 9 = weight-slice producer (one elected lane issuing
-// 1-D TMA bulk copies of the pre-swizzled slices into two buffer sets), warp 10 idle.
+// Warp roles (320 threads, 1 CTA/SM, persistent): warps 0-3 = consumer warpgroup (wgmma issue, then the epilogue of the finished
+// tile: registers -> shared staging -> one voxel per thread -> BN/residual/ReLU -> global), warps 4-7 = A-row loaders, warp 8 =
+// weight-slice producer (one elected lane issuing 1-D bulk copies of the pre-swizzled slices into two buffer sets), warp 9 =
+// raw-row producer (bulk copies of whole fp32 input rows ahead of the converters).
 #include <cstdlib>
 
 #include "tc_common.cuh"
 
 namespace osb {
 
-constexpr int TC_W = 128;          // image width handled (UMMA M)
+constexpr int TC_W = 128;          // image width handled (M tile)
 constexpr int TC_KC = 32;          // input channels per phase: 128-byte K-major rows [32 hi | 32 lo] fp16, SWIZZLE_128B
-constexpr int TC_TILES = 5;        // output rows (accumulator tiles) per work item
+constexpr int TC_TILES = 1;        // output rows (accumulator tiles) per work item
 constexpr int TC_ROWS = TC_TILES + 2;
 constexpr int TC_STAGES = 4;       // A-row ring depth (converted fp16 hi|lo tiles)
-constexpr int TC_RAW = 4;          // raw fp32 rows staged by 1-D TMA bulk copies ahead of the converters (Cin = 32 channels-last layers)
+constexpr int TC_RAW = 2;          // raw fp32 rows staged by 1-D TMA bulk copies ahead of the converters (Cin = 32 channels-last layers)
 constexpr int TC_ROW_BYTES = TC_W * TC_KC * 4;     // 16384: one staged input row (hi and lo halves of every voxel)
-constexpr int TC_THREADS = 352;
+constexpr int TC_THREADS = 320;
 
 struct TcParams {
   const float* x;          // (B, D, H, W, Cin) channels-last
@@ -67,36 +66,43 @@ struct TcParams {
 };
 
 template <int COUT>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams p) {
-  constexpr int N3 = 3 * COUT;                      // kw-stacked MMA N
-  constexpr int B_SLICE = N3 * TC_KC * 4;           // one kh weight slice, rows [hi | lo] (12288 B for Cout = 32)
+struct TcCfg {
+  static constexpr int N3 = 3 * COUT;                      // kw-stacked MMA N
+  static constexpr int B_SLICE = N3 * TC_KC * 4;           // one kh weight slice, rows [hi | lo] (12288 B for Cout = 32)
+  static constexpr int LD = N3 + 4;                        // floats per row of the staged accumulator tile
+  static constexpr int A_OFF = 0;
+  static constexpr int B_OFF = A_OFF + TC_STAGES * TC_ROW_BYTES;      // [2][3 kh]
+  static constexpr int RAW_OFF = B_OFF + TC_BSLOTS * 3 * B_SLICE;    // [TC_RAW] raw fp32 input rows
+  static constexpr int STAGE_OFF = RAW_OFF + TC_RAW * TC_ROW_BYTES;  // [128][LD] fp32 accumulator tile
+  static constexpr int BAR_OFF = STAGE_OFF + 128 * LD * 4;
+  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 256 + 2 * 4 * 2 * COUT * 4 + 3 * COUT * 4;
   static_assert(B_SLICE % 1024 == 0, "weight slices must stay 1024-byte aligned");
-  static_assert(TC_TILES * N3 <= 512, "accumulators exceed TMEM");
-  constexpr int A_OFF = 0;
-  constexpr int B_OFF = A_OFF + TC_STAGES * TC_ROW_BYTES;      // [3 kh]
-  constexpr int RAW_OFF = B_OFF + TC_BSLOTS * 3 * B_SLICE;    // [TC_RAW] raw fp32 input rows
-  constexpr int BAR_OFF = RAW_OFF + TC_RAW * TC_ROW_BYTES;
+  static_assert(TC_TILES == 1, "the consumer warpgroup holds one accumulator tile");
+  static_assert(SMEM <= 232448, "shared memory budget of one CTA exceeded");
+};
+
+template <int COUT>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams p) {
+  using C = TcCfg<COUT>;
+  constexpr int N3 = C::N3;
+  constexpr int B_SLICE = C::B_SLICE;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* a_buf = smem + A_OFF;
-  uint8_t* b_buf = smem + B_OFF;
-  uint8_t* raw_buf = smem + RAW_OFF;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BAR_OFF);
-  uint64_t* a_ready = bars;                         // [STAGES] loaders -> MMA        (128 arrivals)
-  uint64_t* a_empty = a_ready + TC_STAGES;          // [STAGES] MMA -> loaders        (tcgen05.commit)
-  uint64_t* b_full = a_empty + TC_STAGES;           // [2][3]   weight producer -> MMA (expect_tx + TMA bytes)
-  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   MMA -> weight producer (tcgen05.commit)
-  uint64_t* acc_full = b_empty + TC_BSLOTS * 3;     // [TILES]  MMA -> epilogue, one per accumulator tile
-  uint64_t* acc_empty = acc_full + TC_TILES;        // [TILES]  epilogue -> MMA       (128 arrivals)
-  uint64_t* raw_full = acc_empty + TC_TILES;        // [RAW]    row producer -> converters (expect_tx + TMA bytes, or a plain arrive)
+  uint8_t* a_buf = smem + C::A_OFF;
+  uint8_t* b_buf = smem + C::B_OFF;
+  uint8_t* raw_buf = smem + C::RAW_OFF;
+  float* stage = reinterpret_cast<float*>(smem + C::STAGE_OFF);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
+  uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumer   (128 arrivals)
+  uint64_t* a_empty = a_ready + TC_STAGES;          // [STAGES] consumer -> loaders   (4 arrivals: one per consumer warp)
+  uint64_t* b_full = a_empty + TC_STAGES;           // [2][3]   weight producer -> consumer (expect_tx + bulk-copy bytes)
+  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   consumer -> weight producer (4 arrivals)
+  uint64_t* raw_full = b_empty + TC_BSLOTS * 3;     // [RAW]    row producer -> converters (expect_tx + bulk-copy bytes, or a plain arrive)
   uint64_t* raw_empty = raw_full + TC_RAW;          // [RAW]    converters -> row producer (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(raw_empty + TC_RAW);
-  float* xchg = reinterpret_cast<float*>(tmem_slot + 4);   // 16-byte aligned
-  //   // [2 tile parities][4 warps][2][COUT] boundary exchange
+  float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 256);   // [2 tile parities][4 warps][2][COUT] boundary exchange
   float* s_scale = xchg + 2 * 4 * 2 * COUT;                // [COUT]
   float* s_shift = s_scale + COUT;
   float* zeros = s_shift + COUT;                           // [COUT] of 0.f (image-edge neighbours)
-  float* tpose = zeros + COUT;                      // [4 warps][32][TP_STRIDE] transpose tiles of the epilogue
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nchunk = p.Cin / TC_KC;
@@ -104,15 +110,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_STAGES; ++s) {
       mbar_init(&a_ready[s], 128);
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 4);
     }
     for (int k = 0; k < TC_BSLOTS * 3; ++k) {
       mbar_init(&b_full[k], 1);
-      mbar_init(&b_empty[k], 1);
-    }
-    for (int t = 0; t < TC_TILES; ++t) {
-      mbar_init(&acc_full[t], 1);
-      mbar_init(&acc_empty[t], 128);
+      mbar_init(&b_empty[k], 4);
     }
     for (int k = 0; k < TC_RAW; ++k) {
       mbar_init(&raw_full[k], 1);
@@ -120,18 +122,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
     }
     fence_mbar_init();
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   for (int c = threadIdx.x; c < COUT; c += blockDim.x) {
     s_scale[c] = p.scale ? p.scale[c] : 1.f;
     s_shift[c] = p.shift ? p.shift[c] : 0.f;
     zeros[c] = 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   // The rows a CTA stages form one flat sequence (item, kd, chunk, r).  `RowIter` walks it; loads run TWO rows ahead of
   // the stores (software pipeline in registers) so that a full L2/HBM round trip is always in flight.
   struct RowIter {
@@ -156,76 +152,147 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
       s.kd = (d2 == 0) ? 1 : 0;                     // first input plane that exists
     }
   };
-  const uint32_t tmem = *tmem_slot;
-
-  // ---------------------------------------------------------------------------------------------- MMA issuer
-  if (warp == 0) {
-    {
-      const uint32_t idesc = idesc_f16(128, N3);
-      constexpr uint32_t LO = TcK<TC_KC>::LO_OFF;     // descriptor offset of the lo half of an operand row
-      const uint64_t dbase = desc_sw128_base();
-      // Descriptors differ only in their 14-bit start-address field (bits 0-13, units of 16 bytes).
-      const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
-      uint32_t rowc = 0, phc = 0, itc = 0;
-      for (int it = blockIdx.x; it < p.items; it += gridDim.x, ++itc) {
-        const int hb = it % p.hblocks;
+  // ---------------------------------------------------------------------------------------------- consumer warpgroup
+  if (warp < 4) {
+    constexpr uint32_t LO = TcK<TC_KC>::LO_OFF;     // descriptor offset of the lo half of an operand row
+    constexpr uint32_t A_HALF = 64 * TC_KC * 4 / 16;  // descriptor offset of operand rows 64..127
+    const uint64_t dbase = desc_sw128_base();
+    // Descriptors differ only in their 14-bit start-address field (bits 0-13, units of 16 bytes).
+    const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
+    const int q = warp;                              // epilogue: this warp owns tile rows 32q .. 32q + 31
+    const int m = q * 32 + lane;                     // voxel (image column) owned by this thread
+    uint32_t rowc = 0, phc = 0, tilec = 0;
+    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+      {
         const int d = (it / p.hblocks) % p.D;
-        const int ntiles = min(TC_TILES, p.H - hb * TC_TILES);
-        const int last_kd = (d + 1 < p.D) ? 2 : 1;    // last input plane that exists for this output plane
-        uint32_t started = 0;
+        float acc[2][N3 / 2];
+        uint32_t accum = 0;
         for (int kd = 0; kd < 3; ++kd) {
           const int din = d + kd - 1;
           if (din < 0 || din >= p.D) continue;
           for (int ch = 0; ch < nchunk; ++ch, ++phc) {
-            const bool last_phase = (kd == last_kd) && (ch == nchunk - 1);
+            const uint32_t bslot = (phc & 1) * 3;   // weight buffers alternate between phases
 #pragma unroll
-            for (int r = 0; r < TC_ROWS; ++r) {
+            for (int r = 0; r < TC_ROWS; ++r) {     // one output row: input row r of the phase meets weight slice kh = r
               const uint32_t s = rowc % TC_STAGES, par = (rowc / TC_STAGES) & 1;
               mbar_wait(&a_ready[s], par);
-              const uint32_t bslot = (phc & 1) * 3;           // weight buffers alternate between phases
-              if (r < 3) mbar_wait(&b_full[bslot + r], (phc >> 1) & 1);   // slice kh = r is first needed by row r (tile 0)
-              tc_fence_after();
+              mbar_wait(&b_full[bslot + r], (phc >> 1) & 1);
               const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + s * TC_ROW_BYTES) & 0x3FFFF) >> 4);
+              const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot + r) * (B_SLICE / 16));
+              wg_fence();
 #pragma unroll
-              for (int kh = 0; kh < 3; ++kh) {
-                const int t = r - kh;                 // output row tile fed by input row r through tap kh (compile time)
-                if (t < 0 || t >= TC_TILES) continue;
-                const uint32_t accum = (started >> t) & 1;
-                if (!accum) {                         // first touch of this tile in this item: the previous item's epilogue
-                  mbar_wait(&acc_empty[t], (itc & 1) ^ 1);     // must have drained it.  Taken for UNUSED tiles too: otherwise
-                  tc_fence_after();                            // acc_full[t] could complete twice before the epilogue looks
-                  started |= 1u << t;                          // and the mbarrier parity would alias (deadlock).
-                }
-                if (t < ntiles) {
-                  const uint32_t acc = tmem + t * N3;
-                  const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot + kh) * (B_SLICE / 16));
-                  if (elect_one()) {
-#pragma unroll
-                    for (int ks = 0; ks < TcK<TC_KC>::KSTEPS; ++ks) {
-                      mma_f16(acc, da0 + LO + 2 * ks, db0 + 2 * ks, idesc, ks > 0 ? 1u : accum);   // small terms first
-                      mma_f16(acc, da0 + 2 * ks, db0 + LO + 2 * ks, idesc, 1);
-                      mma_f16(acc, da0 + 2 * ks, db0 + 2 * ks, idesc, 1);
-                    }
-                  }
-                  __syncwarp();
-                }
-                if (t == TC_TILES - 1 && elect_one()) mma_commit(&b_empty[bslot + kh]);   // row 4+kh: last user of slice kh
-              }
-              if (elect_one()) {
-                mma_commit(&a_empty[s]);              // ring slot reusable once these MMAs have read it
-                if (last_phase && r >= 2) mma_commit(&acc_full[r - 2]);   // tile r-2 has received its last tap
-              }
-              __syncwarp();
+              for (int ks = 0; ks < TcK<TC_KC>::KSTEPS; ++ks)
+                wg_mma_split<N3>(acc, da0 + 2 * ks, A_HALF, db0 + 2 * ks, LO, ks > 0 ? 1u : accum);
+              wg_commit();
+              wg_wait_all();
+              accum = 1;
+              wg_release(&a_empty[s], lane);        // ring slot and weight slice are free once these MMAs have read them
+              wg_release(&b_empty[bslot + r], lane);
               ++rowc;
             }
           }
+        }
+        named_bar_sync(2, 128);                      // every warp is done with the previous tile's staged rows
+        wg_stage<N3>(stage, C::LD, acc, warp, lane);
+        named_bar_sync(2, 128);
+      }
+      const int hb = it % p.hblocks;
+      const int d = (it / p.hblocks) % p.D;
+      const int b = it / (p.hblocks * p.D);
+      const int h0 = hb * TC_TILES;
+      const int ntiles = min(TC_TILES, p.H - h0);
+      // MMAs each P_kw accumulator received: (existing kd planes) x chunks x 3 kh x k-steps x 3 split terms
+      const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * TcK<TC_KC>::KSTEPS * 3);
+      // D[m] = P0[m-1] + P1[m] + P2[m+1], from the staged tile
+      for (int t = 0; t < ntiles; ++t) {           // ntiles == TC_TILES == 1
+        const int h = h0 + t;
+        const size_t vox = (((size_t)b * p.D + d) * p.H + h) * TC_W + m;           // NDHWC voxel index
+        const size_t plane = (size_t)p.D * p.H * TC_W;                             // NCDHW channel stride
+        const size_t ncdhw0 = (size_t)b * p.Cout * plane + ((size_t)d * p.H + h) * TC_W + m;   // p.Cout <= COUT real channels
+        // all 3*COUT accumulator columns of this voxel from the staged tile
+        uint32_t raw[3][COUT];
+#pragma unroll
+        for (int kw = 0; kw < 3; ++kw)
+#pragma unroll
+          for (int c0 = 0; c0 < COUT; c0 += 16) stage_ld16(stage + m * C::LD + kw * COUT + c0, &raw[kw][c0]);
+        // lanes at the warp edges need the neighbour quadrant's values: exchange through shared memory (double-buffered
+        // by tile parity so one named barrier per tile suffices)
+        float* xb = xchg + (tilec & 1) * (4 * 2 * COUT);
+        ++tilec;                                      // running tile count: consecutive tiles never share a buffer
+        if (lane == 31) {
+#pragma unroll
+          for (int i = 0; i < COUT; ++i) xb[(q * 2) * COUT + i] = __uint_as_float(raw[0][i]);
+        }
+        if (lane == 0) {
+#pragma unroll
+          for (int i = 0; i < COUT; ++i) xb[(q * 2 + 1) * COUT + i] = __uint_as_float(raw[2][i]);
+        }
+        named_bar_sync(1, 128);
+        const float* xl = (q > 0) ? xb + ((q - 1) * 2) * COUT : zeros;
+        const float* xr = (q < 3) ? xb + ((q + 1) * 2 + 1) * COUT : zeros;
+        float out[COUT];
+        // The neighbour-quadrant values are loaded UNCONDITIONALLY (warp-uniform addresses: broadcast LDS.128) and merged with
+        // selects: the `lane == 0 ? xl[i] : left` form compiles to a branch around a load per element.
+#pragma unroll
+        for (int i0 = 0; i0 < COUT; i0 += 4) {
+          const float4 l4 = *reinterpret_cast<const float4*>(xl + i0);
+          const float4 r4 = *reinterpret_cast<const float4*>(xr + i0);
+          const float le[4] = {l4.x, l4.y, l4.z, l4.w}, re[4] = {r4.x, r4.y, r4.z, r4.w};
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int i = i0 + k;
+            float left = __shfl_up_sync(0xffffffffu, __uint_as_float(raw[0][i]), 1);
+            float right = __shfl_down_sync(0xffffffffu, __uint_as_float(raw[2][i]), 1);
+            left = (lane == 0) ? le[k] : left;        // m-1 lives in the previous quadrant (zero at the image edge)
+            right = (lane == 31) ? re[k] : right;     // m+1 lives in the next quadrant
+            out[i] = ((left + __uint_as_float(raw[1][i])) + right) * corr;
+          }
+        }
+        if constexpr (COUT == 32) {
+          if (p.out_ndhwc && (!p.residual || p.res_ndhwc)) {     // coalesced channels-last path (BN/residual/act inside)
+            store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, out, p.y + (vox - lane) * COUT,
+                                p.residual ? p.residual + (vox - lane) * COUT : nullptr, COUT, s_scale, s_shift, p.act);
+            continue;
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < COUT; ++i) out[i] = fmaf(out[i], s_scale[i], s_shift[i]);
+        if (p.residual) {
+          if (p.res_ndhwc) {
+            const float4* rp = reinterpret_cast<const float4*>(p.residual + vox * COUT);
+#pragma unroll
+            for (int i = 0; i < COUT / 4; ++i) {
+              const float4 rv = __ldg(rp + i);
+              out[4 * i] += rv.x, out[4 * i + 1] += rv.y, out[4 * i + 2] += rv.z, out[4 * i + 3] += rv.w;
+            }
+          } else {
+#pragma unroll
+            for (int i = 0; i < COUT; ++i)
+              if (i < p.Cout) out[i] += __ldg(p.residual + ncdhw0 + (size_t)i * plane);
+          }
+        }
+        if (p.act == OSB_ACT_RELU) {
+#pragma unroll
+          for (int i = 0; i < COUT; ++i) out[i] = fmaxf(out[i], 0.f);
+        } else if (p.act == OSB_ACT_LEAKY) {
+#pragma unroll
+          for (int i = 0; i < COUT; ++i) out[i] = out[i] > 0.f ? out[i] : 0.01f * out[i];
+        }
+        if (p.out_ndhwc) {
+          float4* yp = reinterpret_cast<float4*>(p.y + vox * COUT);
+#pragma unroll
+          for (int i = 0; i < COUT / 4; ++i) yp[i] = make_float4(out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
+        } else {
+#pragma unroll
+          for (int i = 0; i < COUT; ++i)
+            if (i < p.Cout) p.y[ncdhw0 + (size_t)i * plane] = out[i];                 // 128-byte rows per warp
         }
       }
     }
   }
   // ---------------------------------------------------------------------------------------------- A-row loaders
-  else if (warp < 5) {
-    const int lt = threadIdx.x - 32;                 // 0..127
+  else if (warp < 8) {
+    const int lt = threadIdx.x - 128;                // 0..127
     const int vsel = lt >> 3, c16 = lt & 7;          // this thread's voxel (mod 16) and fp32 16-byte chunk of the 32-channel slice
     // voxel order inside a half-warp alternates bit 2 of the column so that the STS.64 pairs of stage_f16_split hit disjoint banks
     const int vcol = ((vsel & 1) << 2) | ((vsel >> 1) & 3) | (vsel & 8);
@@ -275,7 +342,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
     RowIter ld{(int)blockIdx.x, 0, 0, -1};
     if (ld.it < p.items) ld.kd = (((ld.it / p.hblocks) % p.D) == 0) ? 1 : 0;
     if (p.bulk_rows) {
-      // The row producer (warp 10) keeps TC_RAW rows of raw fp32 in flight with 16 KB TMA bulk copies; these four warps only
+      // The row producer (warp 9) keeps TC_RAW rows of raw fp32 in flight with 16 KB TMA bulk copies; these four warps only
       // convert: LDS.128 (a warp reads 512 contiguous bytes) -> fp16 hi|lo -> swizzled STS.64.  No load latency on this path.
       uint32_t rawc = 0;
       while (advance(ld)) {
@@ -322,122 +389,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
     }
     tc_report_overflow(p.overflow, amax);
   }
-  // ---------------------------------------------------------------------------------------------- epilogue
-  else if (warp < 9) {
-    const int q = warp & 3;                          // TMEM lane quadrant this warp may read
-    const int m = q * 32 + lane;                     // voxel (image column) owned by this thread
-    uint32_t itc = 0, tilec = 0;
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x, ++itc) {
-      const int hb = it % p.hblocks;
-      const int d = (it / p.hblocks) % p.D;
-      const int b = it / (p.hblocks * p.D);
-      const int h0 = hb * TC_TILES;
-      const int ntiles = min(TC_TILES, p.H - h0);
-      // MMAs each P_kw accumulator received: (existing kd planes) x chunks x 3 kh x k-steps x 3 split terms
-      const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * TcK<TC_KC>::KSTEPS * 3);
-      // D[m] = P0[m-1] + P1[m] + P2[m+1], tile by tile as the MMA warp releases them
-      for (int t = 0; t < ntiles; ++t) {
-        mbar_wait_relaxed(&acc_full[t], itc & 1);
-        tc_fence_after();
-        const int h = h0 + t;
-        const size_t vox = (((size_t)b * p.D + d) * p.H + h) * TC_W + m;           // NDHWC voxel index
-        const size_t plane = (size_t)p.D * p.H * TC_W;                             // NCDHW channel stride
-        const size_t ncdhw0 = (size_t)b * p.Cout * plane + ((size_t)d * p.H + h) * TC_W + m;   // p.Cout <= COUT real channels
-        const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16) + t * N3;
-        // all 3*COUT accumulator columns of this voxel in one go: loads back to back, a single wait
-        uint32_t raw[3][COUT];
-#pragma unroll
-        for (int kw = 0; kw < 3; ++kw)
-#pragma unroll
-          for (int c0 = 0; c0 < COUT; c0 += 16) tmem_ld16_nowait(trow + kw * COUT + c0, &raw[kw][c0]);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(&acc_empty[t]);                   // the tile is in registers: hand it back to the MMA warp
-        // lanes at the warp edges need the neighbour quadrant's values: exchange through shared memory (double-buffered
-        // by tile parity so one named barrier per tile suffices)
-        float* xb = xchg + (tilec & 1) * (4 * 2 * COUT);
-        ++tilec;                                      // running tile count: consecutive tiles never share a buffer
-        if (lane == 31) {
-#pragma unroll
-          for (int i = 0; i < COUT; ++i) xb[(q * 2) * COUT + i] = __uint_as_float(raw[0][i]);
-        }
-        if (lane == 0) {
-#pragma unroll
-          for (int i = 0; i < COUT; ++i) xb[(q * 2 + 1) * COUT + i] = __uint_as_float(raw[2][i]);
-        }
-        named_bar_sync(1, 128);
-        const float* xl = (q > 0) ? xb + ((q - 1) * 2) * COUT : zeros;
-        const float* xr = (q < 3) ? xb + ((q + 1) * 2 + 1) * COUT : zeros;
-        float out[COUT];
-        // The neighbour-quadrant values are loaded UNCONDITIONALLY (warp-uniform addresses: broadcast LDS.128) and merged with
-        // selects: the `lane == 0 ? xl[i] : left` form compiled to a branch around a load per element -- 32 % of the kernel's
-        // stall samples sat on it (branch_resolving; profiles/r2_step_summary.md) and the MMA warp waited for acc_empty.
-#pragma unroll
-        for (int i0 = 0; i0 < COUT; i0 += 4) {
-          const float4 l4 = *reinterpret_cast<const float4*>(xl + i0);
-          const float4 r4 = *reinterpret_cast<const float4*>(xr + i0);
-          const float le[4] = {l4.x, l4.y, l4.z, l4.w}, re[4] = {r4.x, r4.y, r4.z, r4.w};
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int i = i0 + k;
-            float left = __shfl_up_sync(0xffffffffu, __uint_as_float(raw[0][i]), 1);
-            float right = __shfl_down_sync(0xffffffffu, __uint_as_float(raw[2][i]), 1);
-            left = (lane == 0) ? le[k] : left;        // m-1 lives in the previous quadrant (zero at the image edge)
-            right = (lane == 31) ? re[k] : right;     // m+1 lives in the next quadrant
-            out[i] = ((left + __uint_as_float(raw[1][i])) + right) * corr;
-          }
-        }
-        if constexpr (COUT == 32) {
-          if (p.out_ndhwc && (!p.residual || p.res_ndhwc)) {     // coalesced channels-last path (BN/residual/act inside)
-            store_ndhwc_chunk32(tpose + q * TP_WARP_FLOATS, lane, out, p.y + (vox - lane) * COUT,
-                                p.residual ? p.residual + (vox - lane) * COUT : nullptr, COUT, s_scale, s_shift, p.act);
-            continue;
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < COUT; ++i) out[i] = fmaf(out[i], s_scale[i], s_shift[i]);
-        if (p.residual) {
-          if (p.res_ndhwc) {
-            const float4* rp = reinterpret_cast<const float4*>(p.residual + vox * COUT);
-#pragma unroll
-            for (int i = 0; i < COUT / 4; ++i) {
-              const float4 rv = __ldg(rp + i);
-              out[4 * i] += rv.x, out[4 * i + 1] += rv.y, out[4 * i + 2] += rv.z, out[4 * i + 3] += rv.w;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < COUT; ++i)
-              if (i < p.Cout) out[i] += __ldg(p.residual + ncdhw0 + (size_t)i * plane);
-          }
-        }
-        if (p.act == OSB_ACT_RELU) {
-#pragma unroll
-          for (int i = 0; i < COUT; ++i) out[i] = fmaxf(out[i], 0.f);
-        } else if (p.act == OSB_ACT_LEAKY) {
-#pragma unroll
-          for (int i = 0; i < COUT; ++i) out[i] = out[i] > 0.f ? out[i] : 0.01f * out[i];
-        }
-        if (p.out_ndhwc) {
-          float4* yp = reinterpret_cast<float4*>(p.y + vox * COUT);
-#pragma unroll
-          for (int i = 0; i < COUT / 4; ++i) yp[i] = make_float4(out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < COUT; ++i)
-            if (i < p.Cout) p.y[ncdhw0 + (size_t)i * plane] = out[i];                 // 128-byte rows per warp
-        }
-      }
-      // tiles this (short) block never used still take part in the hand-shake so barrier phases stay in step
-      for (int t = ntiles; t < TC_TILES; ++t) {
-        mbar_wait(&acc_full[t], itc & 1);
-        mbar_arrive(&acc_empty[t]);
-      }
-    }
-  }
   // ---------------------------------------------------------------------------------------------- weight-slice producer
-  // One elected lane streams the pre-swizzled (kd, chunk, kh) slices with 1-D TMA bulk copies into the two buffer sets; it runs up
-  // to a whole phase ahead of the MMAs (the other 63 threads of warps 9-10 idle: the slot they used to fill by LDG/STS is gone).
-  else if (warp == 9) {
+  // One elected lane streams the pre-swizzled (kd, chunk, kh) slices with 1-D bulk copies into the two buffer sets; it runs up
+  // to a whole phase ahead of the MMAs.
+  else if (warp == 8) {
     if (elect_one()) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w);
       uint32_t phc = 0;
@@ -461,7 +416,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
     __syncwarp();
   }
   // ---------------------------------------------------------------------------------------------- raw-row producer
-  else if (warp == 10 && p.bulk_rows) {
+  else if (warp == 9 && p.bulk_rows) {
     if (elect_one()) {
       RowIter ld{(int)blockIdx.x, 0, 0, -1};
       if (ld.it < p.items) ld.kd = (((ld.it / p.hblocks) % p.D) == 0) ? 1 : 0;
@@ -491,9 +446,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
     }
     __syncwarp();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 // ---------------------------------------------------------------------------------------- layout conversion kernels
@@ -520,9 +472,7 @@ __global__ void __launch_bounds__(256) ncdhw_to_ndhwc_kernel(const float* __rest
 
 template <int COUT>
 static int launch_tc(const TcParams& p, cudaStream_t stream) {
-  constexpr int N3 = 3 * COUT;
-  const size_t smem = 1024 + (size_t)(TC_STAGES + TC_RAW) * TC_ROW_BYTES + TC_BSLOTS * 3 * (size_t)(N3 * TC_KC * 4) + 512 + 2 * 4 * 2 * COUT * 4 +
-                      3 * COUT * 4 + TP_BYTES;
+  const size_t smem = TcCfg<COUT>::SMEM;
   auto kernel = conv3d_tc_kernel<COUT>;
   static PerDeviceFlag configured;
   if (!configured.here()) {
@@ -534,7 +484,7 @@ static int launch_tc(const TcParams& p, cudaStream_t stream) {
     configured.here() = true;
   }
   const int sms = sm_count();
-  const int grid = p.items < sms ? p.items : sms;   // persistent: one CTA per SM (it owns all 512 TMEM columns)
+  const int grid = p.items < sms ? p.items : sms;   // persistent: one CTA per SM (its shared memory is taken)
   kernel<<<grid, TC_THREADS, smem, stream>>>(p);
   count_launch();
   return check_launch("conv3d_tc_kernel");

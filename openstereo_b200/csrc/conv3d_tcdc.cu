@@ -1,9 +1,10 @@
-// Tensor-core (tcgen05) ConvTranspose3d k=3, stride 2, padding 1, output_padding 1: the up-sampling convs of the hourglasses
+// Tensor-core (Hopper wgmma) ConvTranspose3d k=3, stride 2, padding 1, output_padding 1: the up-sampling convs of the hourglasses
 //   conv5 128->64 / 64->64 (1/16 -> 1/8 res) and conv6 64->32 (1/8 -> 1/4 res): gwcnet/hourglass.py:35-41,
 //   psmnet/psmnet_cost_processor.py:99-106 (deconv3d_bn).
 // Per dimension an output index o gathers  o even (=2m): tap k=1 from input m;  o odd (=2m+1): k=0 from m+1 and k=2 from m.
 // Same machinery as conv3d_tcg.cu / conv3d_tcs2.cu (3xFP16 split, LDG-staged swizzled operands, warp-specialised
-// persistent CTA).  An accumulator tile holds the output rows of ONE parity class: plane od, rows oh = 2j + ph for
+// persistent CTA with a consumer warpgroup, one accumulator tile of G = 32 output channels per work item).  An accumulator tile
+// holds the output rows of ONE parity class: plane od, rows oh = 2j + ph for
 // R = 128/Win consecutive j, all 2*Win output columns.  For each valid tap pair (kd, kh) the operand tile is the R input
 // rows j (+1 for k=0) of input plane id, un-shifted in w, and one MMA with the kw slices stacked along N gives
 //   E[m] = A[m].W1 -> output column 2m,      P2[m] = A[m].W2 and P0[m] = A[m].W0 -> output column 2m+1 = P2[m] + P0[m+1];
@@ -16,8 +17,6 @@
 //   o = 2m: taps k=1 (input m) and k=3 (input m-1);   o = 2m+1: taps k=2 (input m) and k=0 (input m+1)
 // -- every parity class has 2 x 2 (kd, kh) tap pairs, the four kw slices are stacked along N as [W1 | W3 | W2 | W0] and the
 // epilogue forms  even[m] = P1[m] + P3[m-1],  odd[m] = P2[m] + P0[m+1]  (one left and one right shift).
-#include <cstdlib>
-
 #include "tc_common.cuh"
 
 namespace osb {
@@ -51,14 +50,17 @@ struct TcdcCfg {
   static constexpr int ROWB = KC * 4;                       // bytes per K-major operand row: [KC fp16 hi | KC fp16 lo]
   static constexpr int UNIT_BYTES = 128 * ROWB;
   static constexpr int N3 = KS_ * COUT;                     // kw slices stacked along N
-  static constexpr int B_SLICE = N3 * ROWB;                 // one kh weight slice (hi and lo halves of every row)
-  // A-unit ring.  NLW loader warps (1-4 and 10) fill the units round-robin (unit u belongs to warp u mod NLW) into a ring as deep as
-  // shared memory allows (at most 10 units).  Each loader warp enumerates ONLY ITS OWN units: when every warp walked the whole
-  // (tile, tap) sequence and picked every NLW-th unit, that scalar control flow was the bound of these kernels -- a conv6 run with
-  // loads, conversions, MMAs and stores all disabled still took 0.37 of 0.69 ms, two thirds of the loader warps' stall samples on
-  // the loop lines (profiles/r2_conv6_barrier_skeleton_stalls.txt).
+  static constexpr int G = 32;                              // output channels per work item
+  static constexpr int NG = COUT / G;                       // channel groups
+  static constexpr int NGK = KS_ * G;                       // wgmma N: the KS kw blocks of one channel group
+  static constexpr int B_SLICE = N3 * ROWB;                 // one kh weight slice in global memory (hi and lo halves of every row)
+  static constexpr int B_SUB = NGK * ROWB;                  // the part of it one item reads
+  static constexpr int LD = NGK + 4;                        // floats per row of the staged accumulator tile
+  // A-unit ring.  NLW loader warps (4-7 and 9) fill the units round-robin (unit u belongs to loader u mod NLW) into a ring as deep as
+  // shared memory allows (at most 10 units).  Each loader warp enumerates ONLY ITS OWN units: a walk over the whole (tile, tap)
+  // sequence by every warp, picking every NLW-th unit, makes that scalar control flow the bound of these kernels.
   static constexpr int NLW = 5;
-  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * KS_ * B_SLICE + 1024 + 2 * 4 * 2 * 32 * 4 + 3 * COUT * 4 + TP_BYTES;
+  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * KS_ * B_SUB + 128 * LD * 4 + 1024 + 2 * 4 * 2 * 32 * 4 + 3 * COUT * 4;
   static constexpr int STAGES = (232448 - FIXED_SMEM) / UNIT_BYTES < 10 ? (232448 - FIXED_SMEM) / UNIT_BYTES : 10;
   static_assert(STAGES >= NLW, "the ring must hold at least one unit per loader warp");
   static constexpr int HBLK = TILES * R;                    // output rows per work item
@@ -66,13 +68,14 @@ struct TcdcCfg {
   static constexpr int LO = KC / 8;                         // descriptor offset (16-byte units) of the lo half of a row
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + STAGES * UNIT_BYTES;
-  static constexpr int BAR_OFF = B_OFF + TC_BSLOTS * KS_ * B_SLICE;
-  static constexpr int THREADS = 32 + 128 + 128 + 64;       // MMA | A loaders | epilogue | weight loaders (11 warps)
-  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + 2 * 4 * 2 * 32 * 4 + 3 * COUT * 4 + TP_BYTES;
+  static constexpr int STAGE_OFF = B_OFF + TC_BSLOTS * KS_ * B_SUB;   // [128][LD] fp32 accumulator tile
+  static constexpr int BAR_OFF = STAGE_OFF + 128 * LD * 4;
+  static constexpr int THREADS = 128 + 128 + 64;            // consumer warpgroup | A loaders | weight producer + 5th loader (10 warps)
+  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + 2 * 4 * 2 * 32 * 4 + 3 * COUT * 4;
   static_assert(SMEM <= 232448, "shared memory budget of one CTA exceeded");
-  static_assert(TILES * N3 <= 512, "accumulators exceed TMEM");
-  static_assert(B_SLICE % 1024 == 0 && UNIT_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
-  static_assert(N3 % 16 == 0 && N3 <= 256, "invalid UMMA N");
+  static_assert(TILES == 1, "the consumer warpgroup holds one accumulator tile");
+  static_assert(COUT % G == 0, "output channels come in groups of 32");
+  static_assert(B_SUB % 1024 == 0 && UNIT_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
 };
 
 // work item = (image b, output plane od, row parity ph, block of TILES*R input rows); parity bits vary fastest so that the
@@ -118,19 +121,16 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* a_buf = smem + C::A_OFF;
   uint8_t* b_buf = smem + C::B_OFF;
+  float* stage = reinterpret_cast<float*>(smem + C::STAGE_OFF);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
-  uint64_t* a_ready = bars;                         // [STAGES] loaders -> MMA        (32 arrivals: one warp)
-  uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] MMA -> loaders        (tcgen05.commit)
-  uint64_t* b_full = a_empty + C::STAGES;           // [2][KS]  weight producer -> MMA (expect_tx + TMA bytes)
-  uint64_t* b_empty = b_full + TC_BSLOTS * KS;      // [2][KS]  MMA -> weight producer (tcgen05.commit)
-  uint64_t* acc_full = b_empty + TC_BSLOTS * KS;                // [TILES]
-  uint64_t* acc_empty = acc_full + TILES;           // [TILES]  (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + TILES);
+  uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumer   (32 arrivals: one warp)
+  uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] consumer -> loaders   (4 arrivals: one per consumer warp)
+  uint64_t* b_full = a_empty + C::STAGES;           // [2][KS]  weight producer -> consumer (expect_tx + bulk-copy bytes)
+  uint64_t* b_empty = b_full + TC_BSLOTS * KS;      // [2][KS]  consumer -> weight producer (4 arrivals)
   float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 1024);   // [2][4 quadrants][2 sides][32]
   float* s_scale = xchg + 2 * 4 * 2 * 32;
   float* s_shift = s_scale + COUT;
   float* zeros = s_shift + COUT;
-  float* tpose = zeros + COUT;                      // [4 warps][32][TP_STRIDE] transpose tiles of the epilogue
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nchunk = p.Cin / KC;
@@ -140,169 +140,72 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&a_ready[s], 32);                     // one loader warp fills a unit
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 4);
     }
     for (int k = 0; k < TC_BSLOTS * KS; ++k) {
       mbar_init(&b_full[k], 1);
-      mbar_init(&b_empty[k], 1);
-    }
-    for (int t = 0; t < TILES; ++t) {
-      mbar_init(&acc_full[t], 1);
-      mbar_init(&acc_empty[t], 128);
+      mbar_init(&b_empty[k], 4);
     }
     fence_mbar_init();
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   for (int c = threadIdx.x; c < COUT; c += blockDim.x) {
     s_scale[c] = p.scale ? p.scale[c] : 1.f;
     s_shift[c] = p.shift ? p.shift[c] : 0.f;
     zeros[c] = 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  // ---------------------------------------------------------------------------------------------- MMA issuer
-  if (warp == 0) {
-    const uint32_t idesc = idesc_f16(128, C::N3);
+  // ---------------------------------------------------------------------------------------------- consumer warpgroup
+  // wgmma issue into one 128 x KS*G register tile (output channels cg .. cg + 31 of every kw tap), then the epilogue of that tile.
+  if (warp < 4) {
     const uint64_t dbase = (KC == 32) ? desc_sw128_base() : desc_sw64_base();
+    constexpr uint32_t A_HALF = 64 * C::ROWB / 16;  // descriptor offset of operand rows 64..127
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
-    uint32_t unitc = 0, itc = 0;
-    uint32_t bph[KS] = {};                            // per-slice use counters (slices are loaded only for valid kh)
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x, ++itc) {
-      const ItemDc w = decode_dc<C>(p, it);
-      const int ntiles = min(TILES, (p.H - w.j0 + C::R - 1) / C::R);
-      uint32_t started = 0;
-      for (int kd = 0; kd < KS; ++kd) {
-        if (!kd_valid(w.od, kd, p.D)) continue;
-        for (int ch = 0; ch < nchunk; ++ch) {
-          const bool last_phase = (kd == w.last_kd) && (ch == nchunk - 1);
-#pragma unroll
-          for (int t = 0; t < TILES; ++t) {
-#pragma unroll
-            for (int kh = 0; kh < KS; ++kh) {
-              if (!kh_valid(w.ph, kh)) continue;        // warp-uniform
-              const uint32_t slot = unitc % C::STAGES, ph = (unitc / C::STAGES) & 1;
-              mbar_wait(&a_ready[slot], ph);
-              const uint32_t bslot = (bph[kh] & 1) * KS + kh;  // the buffers of tap kh alternate between its uses
-              if (t == 0) mbar_wait(&b_full[bslot], (bph[kh] >> 1) & 1);   // first use of slice kh in this phase
-              tc_fence_after();
-              const uint32_t accum = (started >> t) & 1;
-              if (!accum) {                             // hand-shake taken for unused tiles too (parity must not alias)
-                mbar_wait(&acc_empty[t], (itc & 1) ^ 1);
-                tc_fence_after();
-                started |= 1u << t;
-              }
-              if (t < ntiles) {
-                if (elect_one()) {
-                  const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
-                  const uint32_t acc = tmem + t * C::N3;
-                  const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SLICE) / 16);
-#pragma unroll
-                  for (int ks = 0; ks < C::KSTEPS; ++ks) {
-                    mma_f16(acc, da0 + C::LO + 2 * ks, db0 + 2 * ks, idesc, ks > 0 ? 1u : accum);   // small terms first
-                    mma_f16(acc, da0 + 2 * ks, db0 + C::LO + 2 * ks, idesc, 1);
-                    mma_f16(acc, da0 + 2 * ks, db0 + 2 * ks, idesc, 1);
-                  }
-                }
-                __syncwarp();
-              }
-              if (elect_one()) {
-                mma_commit(&a_empty[slot]);
-                if (t == TILES - 1) mma_commit(&b_empty[bslot]);                 // last user of slice kh in this phase
-                if (last_phase && kh == w.last_kh) mma_commit(&acc_full[t]);     // tile t has received its last tap
-              }
-              __syncwarp();
-              if (t == TILES - 1) ++bph[kh];
-              ++unitc;
-            }
-          }
-        }
-      }
-    }
-  }
-  // ---------------------------------------------------------------------------------------------- A-unit loaders
-  // One loader WARP per unit, units round-robin over the NLW loader warps (unit u -> warp u % NLW, ring slot u % STAGES), so NLW
-  // units' global loads are in flight per SM; a slot is refilled in unit order (the a_empty wait of use n cannot be overtaken: use
-  // n + 1 of that slot belongs to a warp that has not filled it yet, so no mbarrier phase is skipped).  ncu
-  // (profiles/r1_ncu_summary.md, r1_tcdc_conv6): with all four warps on one unit at a time the loaders sat on the load latency and
-  // the tensor pipe was 17 % busy.  Each warp enumerates ONLY its own units (see the Cfg note): one runtime loop, one copy of the
-  // body (unrolled bodies took the kernel to 254 KB of code).
-  else if (warp < 5 || warp == 10) {
-    const int lw = warp < 5 ? warp - 1 : 4;
-    static_assert(KC == 16, "lane_voxel / unit-row mapping below is written for 64-byte operand rows");
-    constexpr int CPR = KC / 4;                      // fp32 16-byte chunks per voxel of the K chunk
-    constexpr int VPL = 32 / CPR;                    // voxels covered by one warp-wide LDG.128
-    constexpr int NLD = 128 / VPL;                   // loads per lane per unit
-    static_assert(W % VPL == 0, "a load instruction must not straddle image rows");
-    const int v0 = lane_voxel<KC>(lane), c = lane % CPR;   // permuted voxel order: conflict-free STS.64 (tc_common.cuh)
-    float amax = 0.f;
-    uint32_t ubase = 0;                              // global index of the current phase's first unit
-    int first = lw;                                  // this warp's first local unit index in the current phase: (ubase + first) % NLW == lw
-    auto fill = [&](const float* base, size_t rstride, size_t cstride, int h_first, int h_step, uint32_t u, int col0) {
-      // base: this lane's address for load 0; load j covers operand rows VPL*j .. VPL*j + VPL - 1 = columns (VPL*j) % W ..
-      // of tile row (VPL*j) / W, read from image row h_first + h_step * tile row (rstride / cstride floats per tile row / column).
-      // General widths: col0 = INPUT column of load 0 (columns >= Wp are zero: beyond the image).
-      float4 v[NLD];
-#pragma unroll
-      for (int j = 0; j < NLD; ++j) {
-        const int hin = h_first + h_step * ((VPL * j) / W);
-        const size_t off = (size_t)((VPL * j) / W) * rstride + (size_t)((VPL * j) % W) * cstride;
-        bool ok = hin >= 0 && hin < p.H;
-        if (GW) ok = ok && (unsigned)(col0 + VPL * j) < (unsigned)Wp;
-        v[j] = ok ? __ldg(reinterpret_cast<const float4*>(base + (ptrdiff_t)off)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      const uint32_t slot = u % C::STAGES, ph = (u / C::STAGES) & 1;   // u = global unit index
-      mbar_wait_relaxed(&a_empty[slot], ph ^ 1);
-      uint8_t* tile = a_buf + slot * C::UNIT_BYTES;
-#pragma unroll
-      for (int j = 0; j < NLD; ++j) stage_f16_split<KC>(tile, v0 + VPL * j, c, v[j], amax);
-      fence_proxy_async();
-      mbar_arrive(&a_ready[slot]);
-    };
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
-      const ItemDc w = decode_dc<C>(p, it);
-      for (int kd = 0; kd < KS; ++kd) {
-        if (!kd_valid(w.od, kd, p.D)) continue;
-        const int id = (w.od + 1 - kd) >> 1;         // input plane feeding output plane od through tap kd
-        const float* plane = p.x + ((size_t)w.b * p.D + id) * p.H * (size_t)Wp * p.Cin;
-        const int col0 = w.ct * C::CSTEP + v0;       // INPUT column of this lane's first load (whole-row kernels: v0)
-        // valid kh taps of this row parity in issue order: k3: ph 0 -> {1}, ph 1 -> {0, 2};  k4: ph 0 -> {1, 3}, ph 1 -> {0, 2}
-        const int nkh = (KS == 4 || w.ph) ? 2 : 1, kh0 = w.ph ? 0 : 1;
-        const int upp = TILES * nkh;                 // units per (kd, chunk) phase, local index = t * nkh + tap index
-        for (int ch = 0; ch < nchunk; ++ch) {
-#pragma unroll 1
-          for (int j = first; j < upp; j += C::NLW) {
-            const int t = nkh == 2 ? (j >> 1) : j, kh = kh0 + 2 * (nkh == 2 ? (j & 1) : 0);
-            // operand row v = input voxel (row j0 + t*R + v / W + (ph + 1 - kh) / 2, column v % W): output row 2j + ph gathers
-            // tap kh from input row j + (ph + 1 - kh) / 2  (k3: +1 for kh = 0; k4: +1 for kh = 0, -1 for kh = 3)
-            const int h_first = w.j0 + t * C::R + ((w.ph + 1 - kh) >> 1);
-            const float* base = plane + ((ptrdiff_t)h_first * Wp + col0) * p.Cin + ch * KC + c * 4;
-            fill(base, (size_t)Wp * p.Cin, (size_t)p.Cin, h_first, 1, ubase + j, col0);
-          }
-          ubase += upp;
-          first = (first + C::NLW - upp % C::NLW) % C::NLW;
-        }
-      }
-    }
-    tc_report_overflow(p.overflow, amax);
-  }
-  // ---------------------------------------------------------------------------------------------- epilogue
-  else if (warp < 9) {
-    const int q = warp & 3;                          // TMEM lane quadrant this warp may read
+    const int q = warp;                              // epilogue: this warp owns tile rows 32q .. 32q + 31
     const int m = q * 32 + lane;                     // operand row owned by this thread
     const int rr = m / W, wcol = m % W;              // input row inside the tile, input column
     const bool has_right_q = (((q + 1) * 32) % W) != 0;   // the next quadrant continues the same image row
     const bool has_left_q = ((q * 32) % W) != 0;          // (k4 only) the previous quadrant does
     const int Do = 2 * p.D, Ho = 2 * p.H;
     const int Wo = 2 * Wp;
-    uint32_t itc = 0, exc = 0;
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x, ++itc) {
-      const ItemDc w = decode_dc<C>(p, it);
+    uint32_t unitc = 0, exc = 0;
+    uint32_t bph[KS] = {};                            // per-slice use counters (slices are loaded only for valid kh)
+    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+      const int cg = (it % C::NG) * C::G;            // output channel group of this item
+      const ItemDc w = decode_dc<C>(p, it / C::NG);
+      {
+        float acc[2][C::NGK / 2];
+        uint32_t accum = 0;
+        for (int kd = 0; kd < KS; ++kd) {
+          if (!kd_valid(w.od, kd, p.D)) continue;
+          for (int ch = 0; ch < nchunk; ++ch) {
+#pragma unroll
+            for (int kh = 0; kh < KS; ++kh) {
+              if (!kh_valid(w.ph, kh)) continue;        // warp-uniform
+              const uint32_t slot = unitc % C::STAGES, ph = (unitc / C::STAGES) & 1;
+              mbar_wait(&a_ready[slot], ph);
+              const uint32_t bslot = (bph[kh] & 1) * KS + kh;  // the buffers of tap kh alternate between its uses
+              mbar_wait(&b_full[bslot], (bph[kh] >> 1) & 1);
+              const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
+              const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
+              wg_fence();
+#pragma unroll
+              for (int ks = 0; ks < C::KSTEPS; ++ks)
+                wg_mma_split<C::NGK>(acc, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum);
+              wg_commit();
+              wg_wait_all();
+              accum = 1;
+              wg_release(&a_empty[slot], lane);
+              wg_release(&b_empty[bslot], lane);
+              ++bph[kh];
+              ++unitc;
+            }
+          }
+        }
+        named_bar_sync(2, 128);                      // every warp is done with the previous tile's staged rows
+        wg_stage<C::NGK>(stage, C::LD, acc, warp, lane);
+        named_bar_sync(2, 128);
+      }
       const int ntiles = min(TILES, (p.H - w.j0 + C::R - 1) / C::R);
       // tap pairs of this parity class: (1 or 2 kd) x (1 or 2 kh); each adds chunks x k-steps x 3 MMAs (tc_common.cuh: rz_kappa)
       const float corr = 1.f + p.kappa * (float)(w.nkd * (KS == 4 ? 2 : w.ph + 1) * nchunk * C::KSTEPS * 3);
@@ -322,13 +225,10 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
 #pragma unroll
           for (int k = 0; k < 2 * COUT; k += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(rp + k));
         }
-        mbar_wait_relaxed(&acc_full[t], itc & 1);
-        tc_fence_after();
         const size_t plane = (size_t)Do * Ho * Wo;                                   // NCDHW channel stride
         const size_t ncdhw0 = (size_t)w.b * p.cout_real * plane + ((size_t)w.od * Ho + oh) * Wo + 2 * col;
-        const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16) + t * C::N3;
-#pragma unroll 1
-        for (int cg = 0; cg < COUT; cg += 32) {
+        const float* srow = stage + m * C::LD;        // this voxel's staged accumulator columns
+        {
           float ev[32], od_[32];
           float* xb = xchg + (exc & 1) * (4 * 2 * 32);
           ++exc;
@@ -338,12 +238,7 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
 #pragma unroll
           for (int kw = 0; kw < 3; ++kw)
 #pragma unroll
-            for (int c0 = 0; c0 < 32; c0 += 16) tmem_ld16_nowait(trow + kw * COUT + cg + c0, &raw[kw][c0]);
-          tmem_ld_wait();
-          if (cg + 32 >= COUT) {                      // whole tile in registers: hand it back to the MMA warp
-            tc_fence_before();
-            mbar_arrive(&acc_empty[t]);
-          }
+            for (int c0 = 0; c0 < 32; c0 += 16) stage_ld16(srow + kw * C::G + c0, &raw[kw][c0]);
           if (lane == 0) {
 #pragma unroll
             for (int i = 0; i < 32; ++i) xb[(q * 2) * 32 + i] = __uint_as_float(raw[2][i]);
@@ -370,10 +265,9 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
           uint32_t ra[32], rb[32];
 #pragma unroll
           for (int c0 = 0; c0 < 32; c0 += 16) {
-            tmem_ld16_nowait(trow + 1 * COUT + cg + c0, &ra[c0]);       // P3
-            tmem_ld16_nowait(trow + 3 * COUT + cg + c0, &rb[c0]);       // P0
+            stage_ld16(srow + 1 * C::G + c0, &ra[c0]);       // P3
+            stage_ld16(srow + 3 * C::G + c0, &rb[c0]);       // P0
           }
-          tmem_ld_wait();
           if (lane == 31) {
 #pragma unroll
             for (int i = 0; i < 32; ++i) xb[(q * 2 + 1) * 32 + i] = __uint_as_float(ra[i]);   // P3 of this quadrant's last column
@@ -405,13 +299,8 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
           }
 #pragma unroll
           for (int c0 = 0; c0 < 32; c0 += 16) {
-            tmem_ld16_nowait(trow + 0 * COUT + cg + c0, &ra[c0]);       // P1
-            tmem_ld16_nowait(trow + 2 * COUT + cg + c0, &rb[c0]);       // P2
-          }
-          tmem_ld_wait();
-          if (cg + 32 >= COUT) {                      // whole tile in registers: hand it back to the MMA warp
-            tc_fence_before();
-            mbar_arrive(&acc_empty[t]);
+            stage_ld16(srow + 0 * C::G + c0, &ra[c0]);       // P1
+            stage_ld16(srow + 2 * C::G + c0, &rb[c0]);       // P2
           }
 #pragma unroll
           for (int i = 0; i < 32; ++i) {
@@ -425,8 +314,8 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
             // lane k owns output voxels (vox0 + 2k) and (vox0 + 2k + 1): two transposes with a 2-voxel lane stride
             float* y0 = p.y + (vox - 2 * lane) * YS + cg;
             const float* r0 = p.residual ? p.residual + (vox - 2 * lane) * YS + cg : nullptr;
-            store_ndhwc_chunk32(tpose + q * TP_WARP_FLOATS, lane, ev, y0, r0, 2 * YS, s_scale + cg, s_shift + cg, p.act, vmask);
-            store_ndhwc_chunk32(tpose + q * TP_WARP_FLOATS, lane, od_, y0 + YS, r0 ? r0 + YS : nullptr, 2 * YS, s_scale + cg,
+            store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, ev, y0, r0, 2 * YS, s_scale + cg, s_shift + cg, p.act, vmask);
+            store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, od_, y0 + YS, r0 ? r0 + YS : nullptr, 2 * YS, s_scale + cg,
                                 s_shift + cg, p.act, vmask);
           } else if (live && cvalid) {
 #pragma unroll
@@ -479,31 +368,96 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
           }
         }
       }
-      for (int t = ntiles; t < TILES; ++t) {            // unused tiles keep the barrier phases in step
-        mbar_wait_relaxed(&acc_full[t], itc & 1);
-        mbar_arrive(&acc_empty[t]);
-      }
     }
   }
+  // ---------------------------------------------------------------------------------------------- A-unit loaders
+  // One loader WARP per unit, units round-robin over the NLW loader warps (unit u -> warp u % NLW, ring slot u % STAGES), so NLW
+  // units' global loads are in flight per SM; a slot is refilled in unit order (the a_empty wait of use n cannot be overtaken: use
+  // n + 1 of that slot belongs to a warp that has not filled it yet, so no mbarrier phase is skipped); with all loader warps on one
+  // unit at a time they would sit on the load latency.  Each warp enumerates ONLY its own units (see the Cfg note): one runtime
+  // loop, one copy of the body (unrolled bodies bloat the kernel's code).
+  else if (warp < 8 || warp == 9) {
+    const int lw = warp < 8 ? warp - 4 : 4;
+    static_assert(KC == 16, "lane_voxel / unit-row mapping below is written for 64-byte operand rows");
+    constexpr int CPR = KC / 4;                      // fp32 16-byte chunks per voxel of the K chunk
+    constexpr int VPL = 32 / CPR;                    // voxels covered by one warp-wide LDG.128
+    constexpr int NLD = 128 / VPL;                   // loads per lane per unit
+    static_assert(W % VPL == 0, "a load instruction must not straddle image rows");
+    const int v0 = lane_voxel<KC>(lane), c = lane % CPR;   // permuted voxel order: conflict-free STS.64 (tc_common.cuh)
+    float amax = 0.f;
+    uint32_t ubase = 0;                              // global index of the current phase's first unit
+    int first = lw;                                  // this warp's first local unit index in the current phase: (ubase + first) % NLW == lw
+    auto fill = [&](const float* base, size_t rstride, size_t cstride, int h_first, int h_step, uint32_t u, int col0) {
+      // base: this lane's address for load 0; load j covers operand rows VPL*j .. VPL*j + VPL - 1 = columns (VPL*j) % W ..
+      // of tile row (VPL*j) / W, read from image row h_first + h_step * tile row (rstride / cstride floats per tile row / column).
+      // General widths: col0 = INPUT column of load 0 (columns >= Wp are zero: beyond the image).
+      float4 v[NLD];
+#pragma unroll
+      for (int j = 0; j < NLD; ++j) {
+        const int hin = h_first + h_step * ((VPL * j) / W);
+        const size_t off = (size_t)((VPL * j) / W) * rstride + (size_t)((VPL * j) % W) * cstride;
+        bool ok = hin >= 0 && hin < p.H;
+        if (GW) ok = ok && (unsigned)(col0 + VPL * j) < (unsigned)Wp;
+        v[j] = ok ? __ldg(reinterpret_cast<const float4*>(base + (ptrdiff_t)off)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      const uint32_t slot = u % C::STAGES, ph = (u / C::STAGES) & 1;   // u = global unit index
+      mbar_wait_relaxed(&a_empty[slot], ph ^ 1);
+      uint8_t* tile = a_buf + slot * C::UNIT_BYTES;
+#pragma unroll
+      for (int j = 0; j < NLD; ++j) stage_f16_split<KC>(tile, v0 + VPL * j, c, v[j], amax);
+      fence_proxy_async();
+      mbar_arrive(&a_ready[slot]);
+    };
+    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+      const ItemDc w = decode_dc<C>(p, it / C::NG);   // every channel group of a tile stages the same units
+      for (int kd = 0; kd < KS; ++kd) {
+        if (!kd_valid(w.od, kd, p.D)) continue;
+        const int id = (w.od + 1 - kd) >> 1;         // input plane feeding output plane od through tap kd
+        const float* plane = p.x + ((size_t)w.b * p.D + id) * p.H * (size_t)Wp * p.Cin;
+        const int col0 = w.ct * C::CSTEP + v0;       // INPUT column of this lane's first load (whole-row kernels: v0)
+        // valid kh taps of this row parity in issue order: k3: ph 0 -> {1}, ph 1 -> {0, 2};  k4: ph 0 -> {1, 3}, ph 1 -> {0, 2}
+        const int nkh = (KS == 4 || w.ph) ? 2 : 1, kh0 = w.ph ? 0 : 1;
+        const int upp = TILES * nkh;                 // units per (kd, chunk) phase, local index = t * nkh + tap index
+        for (int ch = 0; ch < nchunk; ++ch) {
+#pragma unroll 1
+          for (int j = first; j < upp; j += C::NLW) {
+            const int t = nkh == 2 ? (j >> 1) : j, kh = kh0 + 2 * (nkh == 2 ? (j & 1) : 0);
+            // operand row v = input voxel (row j0 + t*R + v / W + (ph + 1 - kh) / 2, column v % W): output row 2j + ph gathers
+            // tap kh from input row j + (ph + 1 - kh) / 2  (k3: +1 for kh = 0; k4: +1 for kh = 0, -1 for kh = 3)
+            const int h_first = w.j0 + t * C::R + ((w.ph + 1 - kh) >> 1);
+            const float* base = plane + ((ptrdiff_t)h_first * Wp + col0) * p.Cin + ch * KC + c * 4;
+            fill(base, (size_t)Wp * p.Cin, (size_t)p.Cin, h_first, 1, ubase + j, col0);
+          }
+          ubase += upp;
+          first = (first + C::NLW - upp % C::NLW) % C::NLW;
+        }
+      }
+    }
+    tc_report_overflow(p.overflow, amax);
+  }
   // ---------------------------------------------------------------------------------------------- weight-slice producer
-  // One elected lane streams the pre-swizzled (kd, chunk, kh) slices with 1-D TMA bulk copies into the two buffers of tap kh, up
-  // to a whole use ahead of the MMAs (tc_common.cuh: bulk_g2s).
-  else if (warp == 9) {
+  // One elected lane streams the item's channel group of the pre-swizzled (kd, chunk, kh) slices -- KS G-row kw blocks, 1-D bulk
+  // copies -- into the two buffers of tap kh, up to a whole use ahead of the MMAs (tc_common.cuh: bulk_g2s).
+  else if (warp == 8) {
     if (elect_one()) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w);
       uint32_t bph[KS] = {};
       for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
-        const ItemDc w = decode_dc<C>(p, it);
+        const int cg = (it % C::NG) * C::G;
+        const ItemDc w = decode_dc<C>(p, it / C::NG);
         for (int kd = 0; kd < KS; ++kd) {
-          if (!kd_valid(w.od, kd, p.D)) continue;         // same phase enumeration as the MMA warp and the A loaders
+          if (!kd_valid(w.od, kd, p.D)) continue;         // same phase enumeration as the consumer and the A loaders
           for (int ch = 0; ch < nchunk; ++ch) {
             for (int kh = 0; kh < KS; ++kh) {
               if (!kh_valid(w.ph, kh)) continue;
               const uint32_t slot = (bph[kh] & 1) * KS + kh;
               const size_t slice = ((size_t)kd * nchunk + ch) * KS + kh;
               mbar_wait_relaxed(&b_empty[slot], ((bph[kh] >> 1) & 1) ^ 1);
-              mbar_arrive_expect_tx(&b_full[slot], C::B_SLICE);
-              bulk_g2s(b_buf + slot * C::B_SLICE, wsrc + slice * C::B_SLICE, C::B_SLICE, &b_full[slot]);
+              mbar_arrive_expect_tx(&b_full[slot], C::B_SUB);
+#pragma unroll
+              for (int kw = 0; kw < KS; ++kw)
+                bulk_g2s(b_buf + slot * C::B_SUB + kw * C::G * C::ROWB, wsrc + slice * C::B_SLICE + (size_t)(kw * COUT + cg) * C::ROWB,
+                         C::G * C::ROWB, &b_full[slot]);
               ++bph[kh];
             }
           }
@@ -512,9 +466,6 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
     }
     __syncwarp();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 template <int COUT, int KC, int W, int TILES, bool GW = false, int KS = 3>
@@ -538,7 +489,7 @@ static int launch_tcdc(TcdcParams& p, cudaStream_t stream) {
   if (p.cout_real <= 0 || p.cout_real > COUT) p.cout_real = COUT;
   if (GW) p.ctiles = (p.Wr + C::CSTEP - 1) / C::CSTEP;
   else p.Wr = W, p.ctiles = 1;
-  const long long items = (long long)p.B * (2 * p.D) * 2 * p.hblocks * p.ctiles;
+  const long long items = (long long)p.B * (2 * p.D) * 2 * p.hblocks * p.ctiles * C::NG;
   OSB_REQUIRE(items < (1ll << 31), "conv3d_tcdc: too many work items");
   p.items = (int)items;
   const int sms = sm_count();
@@ -556,10 +507,6 @@ static int launch_tcdc(TcdcParams& p, cudaStream_t stream) {
   }
   return OSB_OK;
 }
-
-// conv3d_tcdq.cu: one work item per output-parity quad (conv6 shape); -1 = shape not instantiated there
-int launch_tcdq(const float* x, const void* w, const float* scale, const float* shift, const float* residual, float* y, int B,
-                int Cin, int Cout, int D, int H, int W, int act, cudaStream_t stream);
 
 }  // namespace osb
 
@@ -611,10 +558,10 @@ static int deconv3d_k4_tc_impl(const float* x_ndhwc, const void* w_split, const 
   p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
   OSB_REQUIRE(p.overflow, "tensor-core conv: cannot allocate the overflow flag");
   cudaStream_t s = (cudaStream_t)stream;
-  if (W == 16 && Cout == 64) return launch_tcdc<64, 16, 16, 2, false, 4>(p, s);   // StereoBase conv3_up: 6c -> 4c = 96 as slices 64 + 32
-  if (W == 16 && Cout == 32) return launch_tcdc<32, 16, 16, 4, false, 4>(p, s);
-  if (W == 32) return launch_tcdc<64, 16, 32, 2, false, 4>(p, s);
-  return launch_tcdc<32, 16, 64, 4, false, 4>(p, s);
+  if (W == 16 && Cout == 64) return launch_tcdc<64, 16, 16, 1, false, 4>(p, s);   // StereoBase conv3_up: 6c -> 4c = 96 as slices 64 + 32
+  if (W == 16 && Cout == 32) return launch_tcdc<32, 16, 16, 1, false, 4>(p, s);
+  if (W == 32) return launch_tcdc<64, 16, 32, 1, false, 4>(p, s);
+  return launch_tcdc<32, 16, 64, 1, false, 4>(p, s);
 }
 
 int osb_deconv3d_k3_tc_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
@@ -631,18 +578,10 @@ int osb_deconv3d_k3_tc_fwd(const float* x_ndhwc, const void* w_split, const floa
   p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
   OSB_REQUIRE(p.overflow, "tensor-core conv: cannot allocate the overflow flag");
   cudaStream_t s = (cudaStream_t)stream;
-  {
-    // conv6 (64 -> 32 at W' = 64), channels-last: the parity-quad kernel stages 4 units where this file's kernel stages 9
-    static const int quad = [] { const char* e = getenv("OSB_TCDQ"); return e ? atoi(e) : 1; }();
-    if (quad && W == 64 && Cout == 32 && out_ndhwc && (!residual || res_ndhwc)) {
-      const int rc = launch_tcdq(x_ndhwc, w_split, scale, shift, residual, y, B, Cin, Cout, D, H, W, act, s);
-      if (rc >= 0) return rc;
-    }
-  }
-  if (W == 32 && Cout == 64) return launch_tcdc<64, 16, 32, 2>(p, s);
-  if (W == 64 && Cout == 32) return launch_tcdc<32, 16, 64, 5>(p, s);
+  if (W == 32 && Cout == 64) return launch_tcdc<64, 16, 32, 1>(p, s);
+  if (W == 64 && Cout == 32) return launch_tcdc<32, 16, 64, 1>(p, s);
   p.Wr = W;
-  if (Cout == 64) return launch_tcdc<64, 16, 128, 2, true>(p, s);
-  return launch_tcdc<32, 16, 128, 5, true>(p, s);
+  if (Cout == 64) return launch_tcdc<64, 16, 128, 1, true>(p, s);
+  return launch_tcdc<32, 16, 128, 1, true>(p, s);
 }
 }

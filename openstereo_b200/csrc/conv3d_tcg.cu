@@ -1,14 +1,15 @@
-// Generic tensor-core (tcgen05) Conv3d 3x3x3 stride 1 for the hourglass-interior layers whose image width is below the
-// 128-row UMMA tile: an M tile is R = 128 / W consecutive image rows (W = 64 -> 2 rows, W = 32 -> 4 rows).
+// Generic tensor-core (Hopper wgmma) Conv3d 3x3x3 stride 1 for the hourglass-interior layers whose image width is below the
+// 128-row M tile: an M tile is R = 128 / W consecutive image rows (W = 64 -> 2 rows, W = 32 -> 4 rows).
 //   conv2 64->64 @ 1/8 res, conv4 128->128 (GwcNet) / 64->64 (PSMNet) @ 1/16 res:
 //   gwcnet/hourglass.py:25-32, psmnet/psmnet_cost_processor.py:86-98.
 // Same scheme as conv3d_tc.cu (3xFP16 split, kw taps stacked along N and un-shifted in the epilogue, LDG-staged swizzled
-// operands, warp-specialised persistent CTA), generalised:
-//   * an A "unit" is R consecutive input rows starting at block row s; tap kh of output tile t reads the unit with
-//     s = t*R + kh - 1, so units are shared between taps/tiles whenever those starts coincide;
-//   * K chunks are 16 channels (64-byte rows [16 hi | 16 lo] fp16, SWIZZLE_64B: one K = 16 MMA step each) so that the three
-//     kh weight slices of a phase fit in shared memory next to the ring for Cout = 64 / 128;
-//   * for Cout = 128 the kw-stacked N = 384 exceeds the UMMA maximum and is issued as three N = 128 MMAs;
+// operands, warp-specialised persistent CTA with a consumer warpgroup that issues the wgmmas and runs the epilogue), generalised:
+//   * an A "unit" is R consecutive input rows starting at block row s; tap kh of the output tile reads the unit with
+//     s = kh - 1 (the tile index machinery below is written for TILES tiles; the register-held accumulator limits it to one);
+//   * K chunks are 16 channels (64-byte rows [16 hi | 16 lo] fp16, SWIZZLE_64B: one K = 16 MMA step each);
+//   * a work item covers G = 32 output channels: the accumulator tile is 128 x 3G = 96 fp32 columns (96 registers per consumer
+//     thread), and the weight producer streams only the three G-row kw blocks of each slice (contiguous in shared memory, so one
+//     N = 96 wgmma covers them); wider layers are COUT / G items per tile;
 //   * the epilogue's +-1 column shift never crosses an image-row boundary (tile rows are whole image rows).
 // GENERAL WIDTHS (GW = true, W = 128 instantiations): an M tile is a 128-column SEGMENT of one image row of runtime width Wr,
 // starting at column ct * (128 - 2 DIL) - DIL: the first / last DIL tile columns are a halo (loaded like any other column, zero
@@ -32,7 +33,7 @@ struct TcgParams {
   float kappa;       // expected round-towards-zero loss per accumulating MMA (tc_common.cuh)
   unsigned int* overflow;  // sticky fp16-range flag (tc_common.cuh)
   int out_ndhwc, res_ndhwc;
-  int items, hblocks;
+  int items, hblocks;      // items = (b, d, row block, column tile) x output channel groups
   int Wr, ctiles;          // general-width instantiations: image width and column tiles per row (whole-row kernels: W, 1)
   int ystride;             // channels per voxel of the channels-last y / residual / gate tensors (0 = COUT); > COUT when this launch
                            // produces a channel SLICE of a wider tensor (pointers pre-offset to the slice's first channel)
@@ -50,16 +51,17 @@ struct TcgCfg {
   static constexpr int ROWB = KC * 4;                       // bytes per K-major operand row: [KC fp16 hi | KC fp16 lo]
   static constexpr int UNIT_BYTES = 128 * ROWB;
   static constexpr int N3 = 3 * COUT;
-  static constexpr int NMMA = (N3 <= 256) ? 1 : 3;          // MMAs per (A unit, weight slice, k step)
-  static constexpr int NPER = N3 / NMMA;
-  static constexpr int B_SLICE = N3 * ROWB;                 // one kh weight slice (hi and lo halves of every row)
-  // A-unit ring.  NLW loader warps (1-4 and 10) fill the units round-robin (unit u belongs to warp u mod NLW) into a ring as deep as
-  // shared memory allows (at most 10 units).  Each loader warp enumerates ONLY ITS OWN units: when every warp walked the whole
-  // (tile, tap) sequence and picked every NLW-th unit, that scalar control flow was the bound of these kernels -- a conv6 run with
-  // loads, conversions, MMAs and stores all disabled still took 0.37 of 0.69 ms, two thirds of the loader warps' stall samples on
-  // the loop lines (profiles/r2_conv6_barrier_skeleton_stalls.txt).
+  static constexpr int G = 32;                              // output channels per work item
+  static constexpr int NG = COUT / G;                       // channel groups
+  static constexpr int NG3 = 3 * G;                         // wgmma N: the three kw blocks of one channel group
+  static constexpr int B_SLICE = N3 * ROWB;                 // one kh weight slice in global memory (hi and lo halves of every row)
+  static constexpr int B_SUB = NG3 * ROWB;                  // the part of it one item reads
+  static constexpr int LD = NG3 + 4;                        // floats per row of the staged accumulator tile
+  // A-unit ring.  NLW loader warps (4-7 and 9) fill the units round-robin (unit u belongs to loader u mod NLW) into a ring as deep as
+  // shared memory allows (at most 10 units).  Each loader warp enumerates ONLY ITS OWN units: a walk over the whole (tile, tap)
+  // sequence by every warp, picking every NLW-th unit, makes that scalar control flow the bound of these kernels.
   static constexpr int NLW = 5;
-  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * 3 * B_SLICE + 1024 + 2 * 4 * 2 * DIL * 32 * 4 + 3 * COUT * 4 + TP_BYTES;
+  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * 3 * B_SUB + 128 * LD * 4 + 1024 + 2 * 4 * 2 * DIL * 32 * 4 + 3 * COUT * 4;
   static constexpr int STAGES = (232448 - FIXED_SMEM) / UNIT_BYTES < 10 ? (232448 - FIXED_SMEM) / UNIT_BYTES : 10;
   static_assert(STAGES >= NLW, "the ring must hold at least one unit per loader warp");
   static constexpr int S_FIRST = -DIL;                      // unit start rows run from S_FIRST to S_LAST (block-relative)
@@ -69,13 +71,14 @@ struct TcgCfg {
   static constexpr int LO = KC / 8;                         // descriptor offset (16-byte units) of the lo half of a row
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + STAGES * UNIT_BYTES;
-  static constexpr int BAR_OFF = B_OFF + TC_BSLOTS * 3 * B_SLICE;
-  static constexpr int THREADS = 32 + 128 + 128 + 64;       // MMA | A loaders | epilogue | weight loaders (11 warps)
-  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + 2 * 4 * 2 * DIL * 32 * 4 + 3 * COUT * 4 + TP_BYTES;
+  static constexpr int STAGE_OFF = B_OFF + TC_BSLOTS * 3 * B_SUB;   // [128][LD] fp32 accumulator tile
+  static constexpr int BAR_OFF = STAGE_OFF + 128 * LD * 4;
+  static constexpr int THREADS = 128 + 128 + 64;            // consumer warpgroup | A loaders | weight producer + 5th loader (10 warps)
+  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + 2 * 4 * 2 * DIL * 32 * 4 + 3 * COUT * 4;
   static_assert(SMEM <= 232448, "shared memory budget of one CTA exceeded");
-  static_assert(TILES * N3 <= 512, "accumulators exceed TMEM");
-  static_assert(B_SLICE % 1024 == 0 && UNIT_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
-  static_assert(NPER % 16 == 0 && NPER <= 256, "invalid UMMA N");
+  static_assert(TILES == 1, "the consumer warpgroup holds one accumulator tile");
+  static_assert(COUT % G == 0, "output channels come in groups of 32");
+  static_assert(B_SUB % 1024 == 0 && UNIT_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
   // tile fed by unit s through tap kh, or -1
   static constexpr int tile_of(int s, int kh) {
     const int num = s - (kh - 1) * DIL;
@@ -107,19 +110,16 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* a_buf = smem + C::A_OFF;
   uint8_t* b_buf = smem + C::B_OFF;
+  float* stage = reinterpret_cast<float*>(smem + C::STAGE_OFF);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
-  uint64_t* a_ready = bars;                         // [STAGES] loaders -> MMA        (32 arrivals: one warp)
-  uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] MMA -> loaders        (tcgen05.commit)
-  uint64_t* b_full = a_empty + C::STAGES;           // [2][3]   weight producer -> MMA (expect_tx + TMA bytes)
-  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   MMA -> weight producer (tcgen05.commit)
-  uint64_t* acc_full = b_empty + TC_BSLOTS * 3;                 // [TILES]
-  uint64_t* acc_empty = acc_full + TILES;           // [TILES]  (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + TILES);
+  uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumer   (32 arrivals: one warp)
+  uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] consumer -> loaders   (4 arrivals: one per consumer warp)
+  uint64_t* b_full = a_empty + C::STAGES;           // [2][3]   weight producer -> consumer (expect_tx + bulk-copy bytes)
+  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   consumer -> weight producer (4 arrivals)
   float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 1024);   // [2][4 quadrants][2 sides][DIL columns][32]
   float* s_scale = xchg + 2 * 4 * 2 * DIL * 32;
   float* s_shift = s_scale + COUT;
   float* zeros = s_shift + COUT;
-  float* tpose = zeros + COUT;                      // [4 warps][32][TP_STRIDE] transpose tiles of the epilogue
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nchunk = p.Cin / KC;
@@ -130,177 +130,77 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&a_ready[s], 32);                     // one loader warp fills a unit
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 4);
     }
     for (int k = 0; k < TC_BSLOTS * 3; ++k) {
       mbar_init(&b_full[k], 1);
-      mbar_init(&b_empty[k], 1);
-    }
-    for (int t = 0; t < TILES; ++t) {
-      mbar_init(&acc_full[t], 1);
-      mbar_init(&acc_empty[t], 128);
+      mbar_init(&b_empty[k], 4);
     }
     fence_mbar_init();
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   for (int c = threadIdx.x; c < COUT; c += blockDim.x) {
     s_scale[c] = p.scale ? p.scale[c] : 1.f;
     s_shift[c] = p.shift ? p.shift[c] : 0.f;
     zeros[c] = 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  // ---------------------------------------------------------------------------------------------- MMA issuer
-  if (warp == 0) {
-    const uint32_t idesc = idesc_f16(128, C::NPER);
+  // ---------------------------------------------------------------------------------------------- consumer warpgroup
+  // wgmma issue into one 128 x 96 register tile (output channels cg .. cg + 31 of all three kw taps), then the epilogue of that tile.
+  if (warp < 4) {
     const uint64_t dbase = (KC == 32) ? desc_sw128_base() : desc_sw64_base();
+    constexpr uint32_t A_HALF = 64 * C::ROWB / 16;  // descriptor offset of operand rows 64..127
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
-    uint32_t unitc = 0, phc = 0, itc = 0;
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x, ++itc) {
-      const int hb = (it / ctiles) % p.hblocks;
-      const int d = (it / (ctiles * p.hblocks)) % p.D;
-      const int ntiles = min(TILES, (p.H - hb * C::HBLK + C::R - 1) / C::R);
-      const int last_kd = (d + 1 < p.D) ? 2 : 1;
-      uint32_t started = 0;
-      for (int kd = 0; kd < 3; ++kd) {
-        const int din = d + kd - 1;
-        if (din < 0 || din >= p.D) continue;
-        for (int ch = 0; ch < nchunk; ++ch, ++phc) {
-          const bool last_phase = (kd == last_kd) && (ch == nchunk - 1);
-#pragma unroll
-          for (int s = C::S_FIRST; s <= C::S_LAST; ++s) {
-            if (!C::used(s)) continue;
-            const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
-            mbar_wait(&a_ready[slot], par);
-#pragma unroll
-            for (int kh = 0; kh < 3; ++kh)
-              if (C::tile_of(s, kh) == 0) mbar_wait(&b_full[(phc & 1) * 3 + kh], (phc >> 1) & 1);   // first needed by the unit feeding tile 0
-            tc_fence_after();
-            const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
-#pragma unroll
-            for (int kh = 0; kh < 3; ++kh) {
-              const int t = C::tile_of(s, kh);
-              if (t < 0) continue;
-              const uint32_t accum = (started >> t) & 1;
-              if (!accum) {                             // hand-shake taken for unused tiles too (parity must not alias)
-                mbar_wait(&acc_empty[t], (itc & 1) ^ 1);
-                tc_fence_after();
-                started |= 1u << t;
-              }
-              if (t < ntiles) {
-                if (elect_one()) {
-#pragma unroll
-                  for (int mm = 0; mm < C::NMMA; ++mm) {
-                    const uint32_t acc = tmem + t * C::N3 + mm * C::NPER;
-                    const uint64_t db0 = dbase | (uint64_t)(b16 + (((phc & 1) * 3 + kh) * C::B_SLICE + mm * C::NPER * C::ROWB) / 16);
-#pragma unroll
-                    for (int ks = 0; ks < C::KSTEPS; ++ks) {
-                      mma_f16(acc, da0 + C::LO + 2 * ks, db0 + 2 * ks, idesc, ks > 0 ? 1u : accum);   // small terms first
-                      mma_f16(acc, da0 + 2 * ks, db0 + C::LO + 2 * ks, idesc, 1);
-                      mma_f16(acc, da0 + 2 * ks, db0 + 2 * ks, idesc, 1);
-                    }
-                  }
-                }
-                __syncwarp();
-              }
-              if (t == TILES - 1 && elect_one()) mma_commit(&b_empty[(phc & 1) * 3 + kh]);   // last user of slice kh in this phase
-            }
-            if (elect_one()) {
-              mma_commit(&a_empty[slot]);
-              const int tdone = C::tile_of(s, 2);       // kh = 2 is the last tap a tile receives in a phase
-              if (last_phase && tdone >= 0) mma_commit(&acc_full[tdone]);
-            }
-            __syncwarp();
-            ++unitc;
-          }
-        }
-      }
-    }
-  }
-  // ---------------------------------------------------------------------------------------------- A-unit loaders
-  // One loader WARP per unit, units round-robin over the NLW loader warps (unit u -> warp u % NLW, ring slot u % STAGES), so NLW
-  // units' global loads are in flight per SM; a slot is refilled in unit order (the a_empty wait of use n cannot be overtaken: use
-  // n + 1 of that slot belongs to a warp that has not filled it yet, so no mbarrier phase is skipped).  ncu
-  // (profiles/r1_ncu_summary.md, r1_tcdc_conv6): with all four warps on one unit at a time the loaders sat on the load latency and
-  // the tensor pipe was 17 % busy.  Each warp enumerates ONLY its own units (see the Cfg note): one runtime loop, one copy of the
-  // body (unrolled bodies took the kernel to 254 KB of code).
-  else if (warp < 5 || warp == 10) {
-    const int lw = warp < 5 ? warp - 1 : 4;
-    static_assert(KC == 16, "lane_voxel / unit-row mapping below is written for 64-byte operand rows");
-    constexpr int CPR = KC / 4;                      // fp32 16-byte chunks per voxel of the K chunk
-    constexpr int VPL = 32 / CPR;                    // voxels covered by one warp-wide LDG.128
-    constexpr int NLD = 128 / VPL;                   // loads per lane per unit
-    static_assert(W % VPL == 0, "a load instruction must not straddle image rows");
-    const int v0 = lane_voxel<KC>(lane), c = lane % CPR;   // permuted voxel order: conflict-free STS.64 (tc_common.cuh)
-    float amax = 0.f;
-    uint32_t ubase = 0;                              // global index of the current phase's first unit
-    int first = lw;                                  // this warp's first local unit index in the current phase: (ubase + first) % NLW == lw
-    auto fill = [&](const float* base, size_t rstride, size_t cstride, int h_first, int h_step, uint32_t u, int col0) {
-      // base: this lane's address for load 0; load j covers operand rows VPL*j .. VPL*j + VPL - 1 = columns (VPL*j) % W ..
-      // of tile row (VPL*j) / W, read from image row h_first + h_step * tile row (rstride / cstride floats per tile row / column).
-      // General widths: col0 = image column of load 0 (may be -HALO .. or beyond Wr: those columns are zero padding).
-      float4 v[NLD];
-#pragma unroll
-      for (int j = 0; j < NLD; ++j) {
-        const int hin = h_first + h_step * ((VPL * j) / W);
-        const size_t off = (size_t)((VPL * j) / W) * rstride + (size_t)((VPL * j) % W) * cstride;
-        bool ok = hin >= 0 && hin < p.H;
-        if (GW) ok = ok && (unsigned)(col0 + VPL * j) < (unsigned)Wp;
-        v[j] = ok ? __ldg(reinterpret_cast<const float4*>(base + (ptrdiff_t)off)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      const uint32_t slot = u % C::STAGES, ph = (u / C::STAGES) & 1;   // u = global unit index
-      mbar_wait_relaxed(&a_empty[slot], ph ^ 1);
-      uint8_t* tile = a_buf + slot * C::UNIT_BYTES;
-#pragma unroll
-      for (int j = 0; j < NLD; ++j) stage_f16_split<KC>(tile, v0 + VPL * j, c, v[j], amax);
-      fence_proxy_async();
-      mbar_arrive(&a_ready[slot]);
-    };
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
-      const int ct = it % ctiles;
-      const int hb = (it / ctiles) % p.hblocks;
-      const int d = (it / (ctiles * p.hblocks)) % p.D;
-      const int b = it / (ctiles * p.hblocks * p.D);
-      const int h0 = hb * C::HBLK;
-      const int col0 = ct * C::CSTEP - C::HALO + v0;   // image column of this lane's first load (whole-row kernels: v0)
-      for (int kd = 0; kd < 3; ++kd) {
-        const int din = d + kd - 1;
-        if (din < 0 || din >= p.D) continue;
-        const float* plane = p.x + ((size_t)b * p.D + din) * p.H * (size_t)Wp * p.Cin;
-        for (int ch = 0; ch < nchunk; ++ch) {
-#pragma unroll 1
-          for (int j = first; j < C::NU; j += C::NLW) {
-            // unit = R consecutive image rows starting at h0 + s: operand row v is voxel (h0 + s) * W + v of the plane
-            const int s = C::unit_s(j);
-            const float* base = plane + ((ptrdiff_t)(h0 + s) * Wp + col0) * p.Cin + ch * KC + c * 4;
-            fill(base, (size_t)Wp * p.Cin, (size_t)p.Cin, h0 + s, 1, ubase + j, col0);
-          }
-          ubase += C::NU;
-          first = (first + C::NLW - C::NU % C::NLW) % C::NLW;
-        }
-      }
-    }
-    tc_report_overflow(p.overflow, amax);
-  }
-  // ---------------------------------------------------------------------------------------------- epilogue
-  else if (warp < 9) {
-    const int q = warp & 3;                          // TMEM lane quadrant this warp may read
+    const int q = warp;                              // epilogue: this warp owns tile rows 32q .. 32q + 31
     const int m = q * 32 + lane;                     // operand row owned by this thread
     const int rr = m / W, wcol = m % W;              // image row inside the tile, image column
     const bool has_left_q = ((q * 32) % W) != 0;     // the quadrant to the left continues the same image row
     const bool has_right_q = (((q + 1) * 32) % W) != 0;
-    uint32_t itc = 0, exc = 0;
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x, ++itc) {
-      const int ct = it % ctiles;
-      const int hb = (it / ctiles) % p.hblocks;
-      const int d = (it / (ctiles * p.hblocks)) % p.D;
-      const int b = it / (ctiles * p.hblocks * p.D);
+    uint32_t unitc = 0, phc = 0, exc = 0;
+    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+      const int cg = (it % C::NG) * C::G;            // output channel group of this item
+      const int it0 = it / C::NG;
+      const int ct = it0 % ctiles;
+      const int hb = (it0 / ctiles) % p.hblocks;
+      const int d = (it0 / (ctiles * p.hblocks)) % p.D;
+      const int b = it0 / (ctiles * p.hblocks * p.D);
+      {
+        float acc[2][C::NG3 / 2];
+        uint32_t accum = 0;
+        for (int kd = 0; kd < 3; ++kd) {
+          const int din = d + kd - 1;
+          if (din < 0 || din >= p.D) continue;
+          for (int ch = 0; ch < nchunk; ++ch, ++phc) {
+#pragma unroll
+            for (int s = C::S_FIRST; s <= C::S_LAST; ++s) {
+              if (!C::used(s)) continue;
+              const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
+              mbar_wait(&a_ready[slot], par);
+              const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
+#pragma unroll
+              for (int kh = 0; kh < 3; ++kh) {
+                if (C::tile_of(s, kh) != 0) continue;  // one tile: unit s meets the slices kh with s == (kh - 1) * DIL
+                const uint32_t bslot = (phc & 1) * 3 + kh;
+                mbar_wait(&b_full[bslot], (phc >> 1) & 1);
+                const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < C::KSTEPS; ++ks)
+                  wg_mma_split<C::NG3>(acc, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum);
+                wg_commit();
+                wg_wait_all();
+                accum = 1;
+                wg_release(&b_empty[bslot], lane);
+              }
+              wg_release(&a_empty[slot], lane);
+              ++unitc;
+            }
+          }
+        }
+        named_bar_sync(2, 128);                      // every warp is done with the previous tile's staged rows
+        wg_stage<C::NG3>(stage, C::LD, acc, warp, lane);
+        named_bar_sync(2, 128);
+      }
       const int h0 = hb * C::HBLK;
       const int ntiles = min(TILES, (p.H - h0 + C::R - 1) / C::R);
       // general widths: image column of this thread's tile column; halo columns and columns beyond the image are not stored
@@ -319,23 +219,14 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
 #pragma unroll
           for (int k = 0; k < COUT; k += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(rp + k));
         }
-        mbar_wait_relaxed(&acc_full[t], itc & 1);
-        tc_fence_after();
         const size_t plane = (size_t)p.D * p.H * Wp;                               // NCDHW channel stride
         const ptrdiff_t ncdhw0 = (ptrdiff_t)b * COUT * plane + ((ptrdiff_t)d * p.H + h) * Wp + col;
-        const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16) + t * C::N3;
-#pragma unroll 1
-        for (int cg = 0; cg < COUT; cg += 32) {
+        {
           uint32_t raw[3][32];
 #pragma unroll
           for (int kw = 0; kw < 3; ++kw)
 #pragma unroll
-            for (int c0 = 0; c0 < 32; c0 += 16) tmem_ld16_nowait(trow + kw * COUT + cg + c0, &raw[kw][c0]);
-          tmem_ld_wait();
-          if (cg + 32 >= COUT) {                      // whole tile in registers: hand it back to the MMA warp
-            tc_fence_before();
-            mbar_arrive(&acc_empty[t]);
-          }
+            for (int c0 = 0; c0 < 32; c0 += 16) stage_ld16(stage + m * C::LD + kw * C::G + c0, &raw[kw][c0]);
           float* xb = xchg + (exc & 1) * (4 * 2 * DIL * 32);
           ++exc;
           if (lane >= 32 - DIL) {                     // the next quadrant's first DIL columns need these P0 values
@@ -373,7 +264,7 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
           const uint32_t vm = (W < 32) ? __ballot_sync(0xffffffffu, live) : (live ? vmask : 0u);
           if (vm && p.out_ndhwc && (!p.residual || p.res_ndhwc)) {     // coalesced channels-last path (BN/residual/act inside)
             const ptrdiff_t gvox = GATE ? ((ptrdiff_t)b * p.H + h) * Wp + col - lane : 0;   // (B, H, W) index of lane 0's voxel
-            store_ndhwc_chunk32(tpose + q * TP_WARP_FLOATS, lane, out, p.y + (vox - lane) * YS + cg,
+            store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, out, p.y + (vox - lane) * YS + cg,
                                 p.residual ? p.residual + (vox - lane) * YS + cg : nullptr, YS, s_scale + cg, s_shift + cg, p.act,
                                 vm, (GATE && p.gate) ? p.gate + gvox * YS + cg : nullptr);
           } else if (live && cvalid) {
@@ -410,21 +301,84 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
           }
         }
       }
-      for (int t = ntiles; t < TILES; ++t) {            // unused tiles keep the barrier phases in step
-        mbar_wait_relaxed(&acc_full[t], itc & 1);
-        mbar_arrive(&acc_empty[t]);
-      }
     }
   }
+  // ---------------------------------------------------------------------------------------------- A-unit loaders
+  // One loader WARP per unit, units round-robin over the NLW loader warps (unit u -> warp u % NLW, ring slot u % STAGES), so NLW
+  // units' global loads are in flight per SM; a slot is refilled in unit order (the a_empty wait of use n cannot be overtaken: use
+  // n + 1 of that slot belongs to a warp that has not filled it yet, so no mbarrier phase is skipped); with all loader warps on one
+  // unit at a time they would sit on the load latency.  Each warp enumerates ONLY its own units (see the Cfg note): one runtime
+  // loop, one copy of the body (unrolled bodies bloat the kernel's code).
+  else if (warp < 8 || warp == 9) {
+    const int lw = warp < 8 ? warp - 4 : 4;
+    static_assert(KC == 16, "lane_voxel / unit-row mapping below is written for 64-byte operand rows");
+    constexpr int CPR = KC / 4;                      // fp32 16-byte chunks per voxel of the K chunk
+    constexpr int VPL = 32 / CPR;                    // voxels covered by one warp-wide LDG.128
+    constexpr int NLD = 128 / VPL;                   // loads per lane per unit
+    static_assert(W % VPL == 0, "a load instruction must not straddle image rows");
+    const int v0 = lane_voxel<KC>(lane), c = lane % CPR;   // permuted voxel order: conflict-free STS.64 (tc_common.cuh)
+    float amax = 0.f;
+    uint32_t ubase = 0;                              // global index of the current phase's first unit
+    int first = lw;                                  // this warp's first local unit index in the current phase: (ubase + first) % NLW == lw
+    auto fill = [&](const float* base, size_t rstride, size_t cstride, int h_first, int h_step, uint32_t u, int col0) {
+      // base: this lane's address for load 0; load j covers operand rows VPL*j .. VPL*j + VPL - 1 = columns (VPL*j) % W ..
+      // of tile row (VPL*j) / W, read from image row h_first + h_step * tile row (rstride / cstride floats per tile row / column).
+      // General widths: col0 = image column of load 0 (may be -HALO .. or beyond Wr: those columns are zero padding).
+      float4 v[NLD];
+#pragma unroll
+      for (int j = 0; j < NLD; ++j) {
+        const int hin = h_first + h_step * ((VPL * j) / W);
+        const size_t off = (size_t)((VPL * j) / W) * rstride + (size_t)((VPL * j) % W) * cstride;
+        bool ok = hin >= 0 && hin < p.H;
+        if (GW) ok = ok && (unsigned)(col0 + VPL * j) < (unsigned)Wp;
+        v[j] = ok ? __ldg(reinterpret_cast<const float4*>(base + (ptrdiff_t)off)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      const uint32_t slot = u % C::STAGES, ph = (u / C::STAGES) & 1;   // u = global unit index
+      mbar_wait_relaxed(&a_empty[slot], ph ^ 1);
+      uint8_t* tile = a_buf + slot * C::UNIT_BYTES;
+#pragma unroll
+      for (int j = 0; j < NLD; ++j) stage_f16_split<KC>(tile, v0 + VPL * j, c, v[j], amax);
+      fence_proxy_async();
+      mbar_arrive(&a_ready[slot]);
+    };
+    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+      const int it0 = it / C::NG;                    // every channel group of a tile stages the same units
+      const int ct = it0 % ctiles;
+      const int hb = (it0 / ctiles) % p.hblocks;
+      const int d = (it0 / (ctiles * p.hblocks)) % p.D;
+      const int b = it0 / (ctiles * p.hblocks * p.D);
+      const int h0 = hb * C::HBLK;
+      const int col0 = ct * C::CSTEP - C::HALO + v0;   // image column of this lane's first load (whole-row kernels: v0)
+      for (int kd = 0; kd < 3; ++kd) {
+        const int din = d + kd - 1;
+        if (din < 0 || din >= p.D) continue;
+        const float* plane = p.x + ((size_t)b * p.D + din) * p.H * (size_t)Wp * p.Cin;
+        for (int ch = 0; ch < nchunk; ++ch) {
+#pragma unroll 1
+          for (int j = first; j < C::NU; j += C::NLW) {
+            // unit = R consecutive image rows starting at h0 + s: operand row v is voxel (h0 + s) * W + v of the plane
+            const int s = C::unit_s(j);
+            const float* base = plane + ((ptrdiff_t)(h0 + s) * Wp + col0) * p.Cin + ch * KC + c * 4;
+            fill(base, (size_t)Wp * p.Cin, (size_t)p.Cin, h0 + s, 1, ubase + j, col0);
+          }
+          ubase += C::NU;
+          first = (first + C::NLW - C::NU % C::NLW) % C::NLW;
+        }
+      }
+    }
+    tc_report_overflow(p.overflow, amax);
+  }
   // ---------------------------------------------------------------------------------------------- weight-slice producer
-  // One elected lane streams the pre-swizzled (kd, chunk, kh) slices with 1-D TMA bulk copies into the two buffer sets, up to a
-  // whole phase ahead of the MMAs (tc_common.cuh: bulk_g2s).
-  else if (warp == 9) {
+  // One elected lane streams the item's channel group of the pre-swizzled (kd, chunk, kh) slices -- three G-row kw blocks, 1-D
+  // bulk copies -- into the two buffer sets, up to a whole phase ahead of the MMAs (tc_common.cuh: bulk_g2s).  The blocks keep
+  // their row index mod 8, so the swizzle applied by the packer stays valid.
+  else if (warp == 8) {
     if (elect_one()) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w);
       uint32_t phc = 0;
       for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
-        const int d = (it / (ctiles * p.hblocks)) % p.D;
+        const int cg = (it % C::NG) * C::G;
+        const int d = (it / C::NG / (ctiles * p.hblocks)) % p.D;
         for (int kd = 0; kd < 3; ++kd) {
           const int din = d + kd - 1;
           if (din < 0 || din >= p.D) continue;
@@ -433,8 +387,11 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
               const uint32_t slot = (phc & 1) * 3 + kh;
               const size_t slice = ((size_t)kd * nchunk + ch) * 3 + kh;
               mbar_wait_relaxed(&b_empty[slot], ((phc >> 1) & 1) ^ 1);
-              mbar_arrive_expect_tx(&b_full[slot], C::B_SLICE);
-              bulk_g2s(b_buf + slot * C::B_SLICE, wsrc + slice * C::B_SLICE, C::B_SLICE, &b_full[slot]);
+              mbar_arrive_expect_tx(&b_full[slot], C::B_SUB);
+#pragma unroll
+              for (int kw = 0; kw < 3; ++kw)
+                bulk_g2s(b_buf + slot * C::B_SUB + kw * C::G * C::ROWB, wsrc + slice * C::B_SLICE + (size_t)(kw * COUT + cg) * C::ROWB,
+                         C::G * C::ROWB, &b_full[slot]);
             }
           }
         }
@@ -442,9 +399,6 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
     }
     __syncwarp();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 template <int COUT, int KC, int W, int TILES, int DIL = 1, bool GW = false, bool GATE = false>
@@ -471,7 +425,7 @@ static int launch_tcg(TcgParams& p, cudaStream_t stream) {
   p.hblocks = (p.H + C::HBLK - 1) / C::HBLK;
   if (GW) p.ctiles = (p.Wr + C::CSTEP - 1) / C::CSTEP;
   else p.Wr = W, p.ctiles = 1;
-  const long long items = (long long)p.B * p.D * p.hblocks * p.ctiles;
+  const long long items = (long long)p.B * p.D * p.hblocks * p.ctiles * C::NG;
   OSB_REQUIRE(items < (1ll << 31), "conv3d_tcg: too many work items");
   p.items = (int)items;
   const int sms = sm_count();
@@ -501,20 +455,20 @@ int launch_tcg_dispatch(const float* x, const void* w, const float* scale, const
   p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
   if (!p.overflow) return OSB_ECUDA;
   if (Cin % 16 != 0 || Cin < 16) return -1;
-  if (W == 64 && Cout == 64 && gate) return launch_tcg<64, 16, 64, 2, 1, false, true>(p, stream);   // StereoBase 1/8 level (FeatureAtt gate)
+  if (W == 64 && Cout == 64 && gate) return launch_tcg<64, 16, 64, 1, 1, false, true>(p, stream);   // StereoBase 1/8 level (FeatureAtt gate)
   if (W == 32 && Cout == 96 && gate) return launch_tcg<96, 16, 32, 1, 1, false, true>(p, stream);   // ... 1/16 level
-  if (W == 64 && Cout == 64) return launch_tcg<64, 16, 64, 2>(p, stream);
-  if (W == 32 && Cout == 64) return launch_tcg<64, 16, 32, 2>(p, stream);
+  if (W == 64 && Cout == 64) return launch_tcg<64, 16, 64, 1>(p, stream);
+  if (W == 32 && Cout == 64) return launch_tcg<64, 16, 32, 1>(p, stream);
   if (W == 32 && Cout == 128) return launch_tcg<128, 16, 32, 1>(p, stream);
   if (W == 32 && Cout == 96) return launch_tcg<96, 16, 32, 1>(p, stream);         // StereoBase 1/16 level (4c = 96)
   if (W == 16 && Cout == 96) return launch_tcg<96, 16, 16, 1, 1, false, true>(p, stream);   // StereoBase 1/32 level: 6c = 144 -> 160 channels
-  if (W == 16 && Cout == 64) return launch_tcg<64, 16, 16, 2, 1, false, true>(p, stream);   // as two slices (96 + 64), 8 image rows per tile
-  if (W == 128 && Cout == 64) return launch_tcg<64, 16, 128, 2>(p, stream);      // 2D backbone stages as one-plane volumes
+  if (W == 16 && Cout == 64) return launch_tcg<64, 16, 16, 1, 1, false, true>(p, stream);   // as two slices (96 + 64), 8 image rows per tile
+  if (W == 128 && Cout == 64) return launch_tcg<64, 16, 128, 1>(p, stream);      // 2D backbone stages as one-plane volumes
   if (W == 128 && Cout == 128) return launch_tcg<128, 16, 128, 1>(p, stream);
   // every other width: 128-column tiles with a one-column halo (tc_general_width() is the single source of the W bound)
   p.Wr = W;
-  if (Cout == 32) return launch_tcg<32, 16, 128, 5, 1, true>(p, stream);
-  if (Cout == 64) return launch_tcg<64, 16, 128, 2, 1, true>(p, stream);
+  if (Cout == 32) return launch_tcg<32, 16, 128, 1, 1, true>(p, stream);
+  if (Cout == 64) return launch_tcg<64, 16, 128, 1, 1, true>(p, stream);
   if (Cout == 128) return launch_tcg<128, 16, 128, 1, 1, true>(p, stream);
   return -1;
 }

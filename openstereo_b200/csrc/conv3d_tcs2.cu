@@ -1,12 +1,13 @@
-// Tensor-core (tcgen05) Conv3d 3x3x3 STRIDE 2, pad 1: the down-sampling convs of the hourglasses
+// Tensor-core (Hopper wgmma) Conv3d 3x3x3 STRIDE 2, pad 1: the down-sampling convs of the hourglasses
 //   conv1 32->64 (1/4 -> 1/8 res) and conv3 64->128 / 64->64 (1/8 -> 1/16 res): gwcnet/hourglass.py:19-29,
 //   psmnet/psmnet_cost_processor.py:79-94.
-// Same machinery as conv3d_tcg.cu (3xFP16 split, LDG-staged swizzled operands, warp-specialised persistent CTA, taps
-// stacked along N and recombined in the epilogue); what changes is the gather:
+// Same machinery as conv3d_tcg.cu (3xFP16 split, LDG-staged swizzled operands, warp-specialised persistent CTA with a consumer
+// warpgroup, one accumulator tile of G = 32 output channels per work item, taps stacked along N and recombined in the epilogue);
+// what changes is the gather:
 //   out[ow] = in[2ow-1].W0 + in[2ow].W1 + in[2ow+1].W2.  With E[j] = in[2j] (even columns) and O[j] = in[2j+1] (odd columns)
 //   this is  out[ow] = E[ow].W1 + O[ow].W2 + O[ow-1].W0 ,  so per (output tile, kd, kh) the loaders stage TWO operand tiles
 //   -- the even and the odd columns of the RO = 128/Wo input rows 2*oh + kh - 1 -- and the issuer runs
-//   E x W1 (N = Cout) into accumulator columns [0,Cout) and O x [W0 | W2] (N = 2 Cout) into [Cout, 3 Cout); the epilogue
+//   E x W1 (N = G) into accumulator columns [0,G) and O x [W0 | W2] (N = 2G) into [G, 3G); the epilogue
 //   adds P1[ow] + P2[ow] + P0[ow-1] (a single left shift, zero at ow = 0 = the conv's left padding).
 // Weight slices are packed with the kw order (1, 0, 2) so both MMAs read contiguous rows.
 // GENERAL WIDTHS (GW = true, W = 128 instantiations; see conv3d_tcg.cu): an M tile is a 128-column segment of one OUTPUT row of
@@ -42,14 +43,16 @@ struct Tcs2Cfg {
   static constexpr int ROWB = KC * 4;                       // bytes per K-major operand row: [KC fp16 hi | KC fp16 lo]
   static constexpr int UNIT_BYTES = 128 * ROWB;
   static constexpr int N3 = 3 * COUT;
-  static constexpr int B_SLICE = N3 * ROWB;                 // one kh weight slice (hi and lo halves of every row)
-  // A-unit ring.  NLW loader warps (1-4 and 10) fill the units round-robin (unit u belongs to warp u mod NLW) into a ring as deep as
-  // shared memory allows (at most 10 units).  Each loader warp enumerates ONLY ITS OWN units: when every warp walked the whole
-  // (tile, tap) sequence and picked every NLW-th unit, that scalar control flow was the bound of these kernels -- a conv6 run with
-  // loads, conversions, MMAs and stores all disabled still took 0.37 of 0.69 ms, two thirds of the loader warps' stall samples on
-  // the loop lines (profiles/r2_conv6_barrier_skeleton_stalls.txt).
+  static constexpr int G = 32;                              // output channels per work item
+  static constexpr int NG = COUT / G;                       // channel groups
+  static constexpr int B_SLICE = N3 * ROWB;                 // one kh weight slice in global memory (hi and lo halves of every row)
+  static constexpr int B_SUB = 3 * G * ROWB;                // the part of it one item reads
+  static constexpr int LD = 3 * G + 4;                      // floats per row of the staged accumulator tile
+  // A-unit ring.  NLW loader warps (4-7 and 9) fill the units round-robin (unit u belongs to loader u mod NLW) into a ring as deep as
+  // shared memory allows (at most 10 units).  Each loader warp enumerates ONLY ITS OWN units: a walk over the whole (tile, tap)
+  // sequence by every warp, picking every NLW-th unit, makes that scalar control flow the bound of these kernels.
   static constexpr int NLW = 5;
-  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * 3 * B_SLICE + 1024 + 2 * 4 * 2 * 32 * 4 + 3 * COUT * 4 + TP_BYTES;
+  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * 3 * B_SUB + 128 * LD * 4 + 1024 + 2 * 4 * 2 * 32 * 4 + 3 * COUT * 4;
   static constexpr int STAGES = (232448 - FIXED_SMEM) / UNIT_BYTES < 10 ? (232448 - FIXED_SMEM) / UNIT_BYTES : 10;
   static_assert(STAGES >= NLW, "the ring must hold at least one unit per loader warp");
   static constexpr int NU = TILES * 3 * 2;                   // units of one (kd, chunk) phase: (tile, kh, column parity)
@@ -58,13 +61,14 @@ struct Tcs2Cfg {
   static constexpr int LO = KC / 8;                         // descriptor offset (16-byte units) of the lo half of a row
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + STAGES * UNIT_BYTES;
-  static constexpr int BAR_OFF = B_OFF + TC_BSLOTS * 3 * B_SLICE;
-  static constexpr int THREADS = 32 + 128 + 128 + 64;       // MMA | A loaders | epilogue | weight loaders (11 warps)
-  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + 2 * 4 * 2 * 32 * 4 + 3 * COUT * 4 + TP_BYTES;
+  static constexpr int STAGE_OFF = B_OFF + TC_BSLOTS * 3 * B_SUB;   // [128][LD] fp32 accumulator tile
+  static constexpr int BAR_OFF = STAGE_OFF + 128 * LD * 4;
+  static constexpr int THREADS = 128 + 128 + 64;            // consumer warpgroup | A loaders | weight producer + 5th loader (10 warps)
+  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + 2 * 4 * 2 * 32 * 4 + 3 * COUT * 4;
   static_assert(SMEM <= 232448, "shared memory budget of one CTA exceeded");
-  static_assert(TILES * N3 <= 512, "accumulators exceed TMEM");
-  static_assert(B_SLICE % 1024 == 0 && UNIT_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
-  static_assert(COUT % 16 == 0 && 2 * COUT <= 256, "invalid UMMA N");
+  static_assert(TILES == 1, "the consumer warpgroup holds one accumulator tile");
+  static_assert(COUT % G == 0, "output channels come in groups of 32");
+  static_assert(B_SUB % 1024 == 0 && UNIT_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
 };
 
 template <int COUT, int KC, int W, int TILES, bool GW = false>
@@ -74,19 +78,16 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* a_buf = smem + C::A_OFF;
   uint8_t* b_buf = smem + C::B_OFF;
+  float* stage = reinterpret_cast<float*>(smem + C::STAGE_OFF);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
-  uint64_t* a_ready = bars;                         // [STAGES] loaders -> MMA        (32 arrivals: one warp)
-  uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] MMA -> loaders        (tcgen05.commit)
-  uint64_t* b_full = a_empty + C::STAGES;           // [2][3]   weight producer -> MMA (expect_tx + TMA bytes)
-  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   MMA -> weight producer (tcgen05.commit)
-  uint64_t* acc_full = b_empty + TC_BSLOTS * 3;                 // [TILES]
-  uint64_t* acc_empty = acc_full + TILES;           // [TILES]  (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + TILES);
+  uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumer   (32 arrivals: one warp)
+  uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] consumer -> loaders   (4 arrivals: one per consumer warp)
+  uint64_t* b_full = a_empty + C::STAGES;           // [2][3]   weight producer -> consumer (expect_tx + bulk-copy bytes)
+  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   consumer -> weight producer (4 arrivals)
   float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 1024);   // [2][4 quadrants][2 sides][32]
   float* s_scale = xchg + 2 * 4 * 2 * 32;
   float* s_shift = s_scale + COUT;
   float* zeros = s_shift + COUT;
-  float* tpose = zeros + COUT;                      // [4 warps][32][TP_STRIDE] transpose tiles of the epilogue
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nchunk = p.Cin / KC;
@@ -97,176 +98,81 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&a_ready[s], 32);                     // one loader warp fills a unit
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 4);
     }
     for (int k = 0; k < TC_BSLOTS * 3; ++k) {
       mbar_init(&b_full[k], 1);
-      mbar_init(&b_empty[k], 1);
-    }
-    for (int t = 0; t < TILES; ++t) {
-      mbar_init(&acc_full[t], 1);
-      mbar_init(&acc_empty[t], 128);
+      mbar_init(&b_empty[k], 4);
     }
     fence_mbar_init();
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   for (int c = threadIdx.x; c < COUT; c += blockDim.x) {
     s_scale[c] = p.scale ? p.scale[c] : 1.f;
     s_shift[c] = p.shift ? p.shift[c] : 0.f;
     zeros[c] = 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  // ---------------------------------------------------------------------------------------------- MMA issuer
-  if (warp == 0) {
-    const uint32_t idesc_e = idesc_f16(128, COUT), idesc_o = idesc_f16(128, 2 * COUT);
+  // ---------------------------------------------------------------------------------------------- consumer warpgroup
+  // wgmma issue into one 128-row register tile of output channels cg .. cg + 31 -- E x W1 (N = G) and O x [W0 | W2] (N = 2G) --
+  // then the epilogue of that tile.
+  if (warp < 4) {
     const uint64_t dbase = (KC == 32) ? desc_sw128_base() : desc_sw64_base();
+    constexpr uint32_t A_HALF = 64 * C::ROWB / 16;  // descriptor offset of operand rows 64..127
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
     const int Do = p.D / 2, Ho = p.H / 2;
-    uint32_t unitc = 0, phc = 0, itc = 0;
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x, ++itc) {
-      const int hb = (it / ctiles) % p.hblocks;
-      const int od = (it / (ctiles * p.hblocks)) % Do;
-      const int ntiles = min(TILES, (Ho - hb * C::HBLK + C::R - 1) / C::R);
-      uint32_t started = 0;
-      for (int kd = 0; kd < 3; ++kd) {
-        const int din = 2 * od + kd - 1;
-        if (din < 0 || din >= p.D) continue;
-        for (int ch = 0; ch < nchunk; ++ch, ++phc) {
-          const bool last_phase = (kd == 2) && (ch == nchunk - 1);     // din = 2*od+1 always exists (even D)
-#pragma unroll
-          for (int t = 0; t < TILES; ++t) {
+    const int q = warp;                              // epilogue: this warp owns tile rows 32q .. 32q + 31
+    const int m = q * 32 + lane;                     // operand row owned by this thread
+    const int rr = m / W, wcol = m % W;              // image row inside the tile, image column
+    const bool has_left_q = ((q * 32) % W) != 0;     // the quadrant to the left continues the same image row
+    uint32_t unitc = 0, phc = 0, exc = 0;
+    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+      const int cg = (it % C::NG) * C::G;            // output channel group of this item
+      const int it0 = it / C::NG;
+      const int ct = it0 % ctiles;
+      const int hb = (it0 / ctiles) % p.hblocks;
+      const int d = (it0 / (ctiles * p.hblocks)) % Do;
+      const int b = it0 / (ctiles * p.hblocks * Do);
+      {
+        float acc_e[2][C::G / 2], acc_o[2][C::G];   // accumulator columns [P1 | P0 | P2]
+        uint32_t accum_e = 0, accum_o = 0;
+        for (int kd = 0; kd < 3; ++kd) {
+          const int din = 2 * d + kd - 1;
+          if (din < 0 || din >= p.D) continue;
+          for (int ch = 0; ch < nchunk; ++ch, ++phc) {
 #pragma unroll
             for (int kh = 0; kh < 3; ++kh) {
+              const uint32_t bslot = (phc & 1) * 3 + kh;
 #pragma unroll
               for (int par = 0; par < 2; ++par) {       // par 0: even input columns (kw = 1); par 1: odd columns (kw = 0, 2)
                 const uint32_t slot = unitc % C::STAGES, ph = (unitc / C::STAGES) & 1;
                 mbar_wait(&a_ready[slot], ph);
-                if (t == 0 && par == 0) mbar_wait(&b_full[(phc & 1) * 3 + kh], (phc >> 1) & 1);   // first use of slice kh in this phase
-                tc_fence_after();
-                const uint32_t accum = (started >> (2 * t + par)) & 1;
-                if (((started >> (2 * t)) & 3u) == 0u) {     // first touch of this tile in this item (unused tiles too)
-                  mbar_wait(&acc_empty[t], (itc & 1) ^ 1);
-                  tc_fence_after();
-                }
-                started |= 1u << (2 * t + par);
-                if (t < ntiles) {
-                  if (elect_one()) {
-                    const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
-                    // slice rows: [W1 (Cout) | W0 (Cout) | W2 (Cout)]; accumulator columns: [P1 | P0 | P2]
-                    const uint32_t acc = tmem + t * C::N3 + (par ? COUT : 0);
-                    const uint64_t db0 = dbase | (uint64_t)(b16 + (((phc & 1) * 3 + kh) * C::B_SLICE + (par ? COUT * C::ROWB : 0)) / 16);
-                    const uint32_t idesc = par ? idesc_o : idesc_e;
+                if (par == 0) mbar_wait(&b_full[bslot], (phc >> 1) & 1);   // first use of slice kh in this phase
+                const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
+                // sub-slice rows: [W1 (G) | W0 (G) | W2 (G)]
+                const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB + (par ? C::G * C::ROWB : 0)) / 16);
+                wg_fence();
 #pragma unroll
-                    for (int ks = 0; ks < C::KSTEPS; ++ks) {
-                      mma_f16(acc, da0 + C::LO + 2 * ks, db0 + 2 * ks, idesc, ks > 0 ? 1u : accum);   // small terms first
-                      mma_f16(acc, da0 + 2 * ks, db0 + C::LO + 2 * ks, idesc, 1);
-                      mma_f16(acc, da0 + 2 * ks, db0 + 2 * ks, idesc, 1);
-                    }
-                  }
-                  __syncwarp();
+                for (int ks = 0; ks < C::KSTEPS; ++ks) {
+                  if (par == 0) wg_mma_split<C::G>(acc_e, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum_e);
+                  else wg_mma_split<2 * C::G>(acc_o, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum_o);
                 }
-                if (elect_one()) {
-                  mma_commit(&a_empty[slot]);
-                  if (t == TILES - 1 && par == 1) mma_commit(&b_empty[(phc & 1) * 3 + kh]);   // last user of slice kh in this phase
-                  if (last_phase && kh == 2 && par == 1) mma_commit(&acc_full[t]); // tile t has received its last tap
-                }
-                __syncwarp();
+                wg_commit();
+                wg_wait_all();
+                if (par == 0) accum_e = 1;
+                else accum_o = 1;
+                wg_release(&a_empty[slot], lane);
+                if (par == 1) wg_release(&b_empty[bslot], lane);          // last user of slice kh in this phase
                 ++unitc;
               }
             }
           }
         }
+        named_bar_sync(2, 128);                      // every warp is done with the previous tile's staged rows
+        wg_stage<C::G>(stage, C::LD, acc_e, warp, lane);
+        wg_stage<2 * C::G>(stage + C::G, C::LD, acc_o, warp, lane);
+        named_bar_sync(2, 128);
       }
-    }
-  }
-  // ---------------------------------------------------------------------------------------------- A-unit loaders
-  // One loader WARP per unit, units round-robin over the NLW loader warps (unit u -> warp u % NLW, ring slot u % STAGES), so NLW
-  // units' global loads are in flight per SM; a slot is refilled in unit order (the a_empty wait of use n cannot be overtaken: use
-  // n + 1 of that slot belongs to a warp that has not filled it yet, so no mbarrier phase is skipped).  ncu
-  // (profiles/r1_ncu_summary.md, r1_tcdc_conv6): with all four warps on one unit at a time the loaders sat on the load latency and
-  // the tensor pipe was 17 % busy.  Each warp enumerates ONLY its own units (see the Cfg note): one runtime loop, one copy of the
-  // body (unrolled bodies took the kernel to 254 KB of code).
-  else if (warp < 5 || warp == 10) {
-    const int lw = warp < 5 ? warp - 1 : 4;
-    static_assert(KC == 16, "lane_voxel / unit-row mapping below is written for 64-byte operand rows");
-    constexpr int CPR = KC / 4;                      // fp32 16-byte chunks per voxel of the K chunk
-    constexpr int VPL = 32 / CPR;                    // voxels covered by one warp-wide LDG.128
-    constexpr int NLD = 128 / VPL;                   // loads per lane per unit
-    static_assert(W % VPL == 0, "a load instruction must not straddle image rows");
-    const int v0 = lane_voxel<KC>(lane), c = lane % CPR;   // permuted voxel order: conflict-free STS.64 (tc_common.cuh)
-    float amax = 0.f;
-    const int WI = 2 * Wp;                           // input width
-    const int Do = p.D / 2;
-    uint32_t ubase = 0;                              // global index of the current phase's first unit
-    int first = lw;                                  // this warp's first local unit index in the current phase: (ubase + first) % NLW == lw
-    auto fill = [&](const float* base, size_t rstride, size_t cstride, int h_first, int h_step, uint32_t u, int col0) {
-      // base: this lane's address for load 0; load j covers operand rows VPL*j .. VPL*j + VPL - 1 = columns (VPL*j) % W ..
-      // of tile row (VPL*j) / W, read from image row h_first + h_step * tile row (rstride / cstride floats per tile row / column).
-      // General widths: col0 = OUTPUT column of load 0 (-1 = the left halo; columns outside [0, Wp) are zero padding).
-      float4 v[NLD];
-#pragma unroll
-      for (int j = 0; j < NLD; ++j) {
-        const int hin = h_first + h_step * ((VPL * j) / W);
-        const size_t off = (size_t)((VPL * j) / W) * rstride + (size_t)((VPL * j) % W) * cstride;
-        bool ok = hin >= 0 && hin < p.H;
-        if (GW) ok = ok && (unsigned)(col0 + VPL * j) < (unsigned)Wp;
-        v[j] = ok ? __ldg(reinterpret_cast<const float4*>(base + (ptrdiff_t)off)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      const uint32_t slot = u % C::STAGES, ph = (u / C::STAGES) & 1;   // u = global unit index
-      mbar_wait_relaxed(&a_empty[slot], ph ^ 1);
-      uint8_t* tile = a_buf + slot * C::UNIT_BYTES;
-#pragma unroll
-      for (int j = 0; j < NLD; ++j) stage_f16_split<KC>(tile, v0 + VPL * j, c, v[j], amax);
-      fence_proxy_async();
-      mbar_arrive(&a_ready[slot]);
-    };
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
-      const int ct = it % ctiles;
-      const int hb = (it / ctiles) % p.hblocks;
-      const int od = (it / (ctiles * p.hblocks)) % Do;
-      const int b = it / (ctiles * p.hblocks * Do);
-      const int h0 = hb * C::HBLK;                   // first OUTPUT row of the block
-      const int col0 = ct * C::CSTEP - C::HALO + v0; // OUTPUT column of this lane's first load (whole-row kernels: v0)
-      for (int kd = 0; kd < 3; ++kd) {
-        const int din = 2 * od + kd - 1;
-        if (din < 0 || din >= p.D) continue;
-        const float* plane = p.x + ((size_t)b * p.D + din) * p.H * (size_t)WI * p.Cin;
-        for (int ch = 0; ch < nchunk; ++ch) {
-#pragma unroll 1
-          for (int j = first; j < C::NU; j += C::NLW) {       // local unit index = (t * 3 + kh) * 2 + par
-            const int t = j / 6, kh = (j >> 1) % 3, par = j & 1;
-            // operand row v = output voxel (row h0 + t*R + v / W, column v % W) reading input (2*row + kh - 1, 2*col + par)
-            const int h_first = 2 * (h0 + t * C::R) + kh - 1;
-            const float* base = plane + ((ptrdiff_t)h_first * WI + 2 * col0 + par) * p.Cin + ch * KC + c * 4;
-            fill(base, (size_t)2 * WI * p.Cin, (size_t)2 * p.Cin, h_first, 2, ubase + j, col0);
-          }
-          ubase += C::NU;
-          first = (first + C::NLW - C::NU % C::NLW) % C::NLW;
-        }
-      }
-    }
-    tc_report_overflow(p.overflow, amax);
-  }
-  // ---------------------------------------------------------------------------------------------- epilogue
-  else if (warp < 9) {
-    const int q = warp & 3;                          // TMEM lane quadrant this warp may read
-    const int m = q * 32 + lane;                     // operand row owned by this thread
-    const int rr = m / W, wcol = m % W;              // image row inside the tile, image column
-    const bool has_left_q = ((q * 32) % W) != 0;     // the quadrant to the left continues the same image row
-    const int Do = p.D / 2, Ho = p.H / 2;
-    uint32_t itc = 0, exc = 0;
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x, ++itc) {
-      const int ct = it % ctiles;
-      const int hb = (it / ctiles) % p.hblocks;
-      const int d = (it / (ctiles * p.hblocks)) % Do;
-      const int b = it / (ctiles * p.hblocks * Do);
       const int h0 = hb * C::HBLK;
       const int ntiles = min(TILES, (Ho - h0 + C::R - 1) / C::R);
       // general widths: output column of this thread's tile column; the halo column and columns beyond the image are not stored
@@ -276,26 +182,17 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
       // input planes 2d-1, 2d, 2d+1: the first is missing for d = 0 (tc_common.cuh: rz_kappa)
       const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (2 * d + 1 < p.D)) * nchunk * 3 * C::KSTEPS * 3);
       for (int t = 0; t < ntiles; ++t) {
-        mbar_wait_relaxed(&acc_full[t], itc & 1);
-        tc_fence_after();
         const int h = h0 + t * C::R + rr;
         const bool live = h < Ho;
         const ptrdiff_t vox = (((ptrdiff_t)b * Do + d) * Ho + h) * Wp + col;       // NDHWC voxel index (output)
         const size_t plane = (size_t)Do * Ho * Wp;                                 // NCDHW channel stride (output)
         const ptrdiff_t ncdhw0 = (ptrdiff_t)b * COUT * plane + ((ptrdiff_t)d * Ho + h) * Wp + col;
-        const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16) + t * C::N3;
-#pragma unroll 1
-        for (int cg = 0; cg < COUT; cg += 32) {
+        {
           uint32_t raw[3][32];
 #pragma unroll
           for (int kw = 0; kw < 3; ++kw)
 #pragma unroll
-            for (int c0 = 0; c0 < 32; c0 += 16) tmem_ld16_nowait(trow + kw * COUT + cg + c0, &raw[kw][c0]);
-          tmem_ld_wait();
-          if (cg + 32 >= COUT) {                      // whole tile in registers: hand it back to the MMA warp
-            tc_fence_before();
-            mbar_arrive(&acc_empty[t]);
-          }
+            for (int c0 = 0; c0 < 32; c0 += 16) stage_ld16(stage + m * C::LD + kw * C::G + c0, &raw[kw][c0]);
           float* xb = xchg + (exc & 1) * (4 * 2 * 32);
           ++exc;
           // accumulator column groups: raw[0] = P1 (kw=1, even columns), raw[1] = P0 (kw=0), raw[2] = P2 (kw=2)
@@ -321,7 +218,7 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
           }
           const uint32_t vm = (W < 32) ? __ballot_sync(0xffffffffu, live) : (live ? vmask : 0u);   // voxels of this warp that exist
           if (vm && p.out_ndhwc && (!p.residual || p.res_ndhwc)) {     // coalesced channels-last path (BN/residual/act inside)
-            store_ndhwc_chunk32(tpose + q * TP_WARP_FLOATS, lane, out, p.y + (vox - lane) * YS + cg,
+            store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, out, p.y + (vox - lane) * YS + cg,
                                 p.residual ? p.residual + (vox - lane) * YS + cg : nullptr, YS, s_scale + cg, s_shift + cg, p.act,
                                 vm);
           } else if (live && cvalid) {
@@ -358,31 +255,99 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
           }
         }
       }
-      for (int t = ntiles; t < TILES; ++t) {            // unused tiles keep the barrier phases in step
-        mbar_wait_relaxed(&acc_full[t], itc & 1);
-        mbar_arrive(&acc_empty[t]);
-      }
     }
   }
+  // ---------------------------------------------------------------------------------------------- A-unit loaders
+  // One loader WARP per unit, units round-robin over the NLW loader warps (unit u -> warp u % NLW, ring slot u % STAGES), so NLW
+  // units' global loads are in flight per SM; a slot is refilled in unit order (the a_empty wait of use n cannot be overtaken: use
+  // n + 1 of that slot belongs to a warp that has not filled it yet, so no mbarrier phase is skipped); with all loader warps on one
+  // unit at a time they would sit on the load latency.  Each warp enumerates ONLY its own units (see the Cfg note): one runtime
+  // loop, one copy of the body (unrolled bodies bloat the kernel's code).
+  else if (warp < 8 || warp == 9) {
+    const int lw = warp < 8 ? warp - 4 : 4;
+    static_assert(KC == 16, "lane_voxel / unit-row mapping below is written for 64-byte operand rows");
+    constexpr int CPR = KC / 4;                      // fp32 16-byte chunks per voxel of the K chunk
+    constexpr int VPL = 32 / CPR;                    // voxels covered by one warp-wide LDG.128
+    constexpr int NLD = 128 / VPL;                   // loads per lane per unit
+    static_assert(W % VPL == 0, "a load instruction must not straddle image rows");
+    const int v0 = lane_voxel<KC>(lane), c = lane % CPR;   // permuted voxel order: conflict-free STS.64 (tc_common.cuh)
+    float amax = 0.f;
+    const int WI = 2 * Wp;                           // input width
+    const int Do = p.D / 2;
+    uint32_t ubase = 0;                              // global index of the current phase's first unit
+    int first = lw;                                  // this warp's first local unit index in the current phase: (ubase + first) % NLW == lw
+    auto fill = [&](const float* base, size_t rstride, size_t cstride, int h_first, int h_step, uint32_t u, int col0) {
+      // base: this lane's address for load 0; load j covers operand rows VPL*j .. VPL*j + VPL - 1 = columns (VPL*j) % W ..
+      // of tile row (VPL*j) / W, read from image row h_first + h_step * tile row (rstride / cstride floats per tile row / column).
+      // General widths: col0 = OUTPUT column of load 0 (-1 = the left halo; columns outside [0, Wp) are zero padding).
+      float4 v[NLD];
+#pragma unroll
+      for (int j = 0; j < NLD; ++j) {
+        const int hin = h_first + h_step * ((VPL * j) / W);
+        const size_t off = (size_t)((VPL * j) / W) * rstride + (size_t)((VPL * j) % W) * cstride;
+        bool ok = hin >= 0 && hin < p.H;
+        if (GW) ok = ok && (unsigned)(col0 + VPL * j) < (unsigned)Wp;
+        v[j] = ok ? __ldg(reinterpret_cast<const float4*>(base + (ptrdiff_t)off)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      const uint32_t slot = u % C::STAGES, ph = (u / C::STAGES) & 1;   // u = global unit index
+      mbar_wait_relaxed(&a_empty[slot], ph ^ 1);
+      uint8_t* tile = a_buf + slot * C::UNIT_BYTES;
+#pragma unroll
+      for (int j = 0; j < NLD; ++j) stage_f16_split<KC>(tile, v0 + VPL * j, c, v[j], amax);
+      fence_proxy_async();
+      mbar_arrive(&a_ready[slot]);
+    };
+    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+      const int it0 = it / C::NG;                    // every channel group of a tile stages the same units
+      const int ct = it0 % ctiles;
+      const int hb = (it0 / ctiles) % p.hblocks;
+      const int od = (it0 / (ctiles * p.hblocks)) % Do;
+      const int b = it0 / (ctiles * p.hblocks * Do);
+      const int h0 = hb * C::HBLK;                   // first OUTPUT row of the block
+      const int col0 = ct * C::CSTEP - C::HALO + v0; // OUTPUT column of this lane's first load (whole-row kernels: v0)
+      for (int kd = 0; kd < 3; ++kd) {
+        const int din = 2 * od + kd - 1;
+        if (din < 0 || din >= p.D) continue;
+        const float* plane = p.x + ((size_t)b * p.D + din) * p.H * (size_t)WI * p.Cin;
+        for (int ch = 0; ch < nchunk; ++ch) {
+#pragma unroll 1
+          for (int j = first; j < C::NU; j += C::NLW) {       // local unit index = (t * 3 + kh) * 2 + par
+            const int t = j / 6, kh = (j >> 1) % 3, par = j & 1;
+            // operand row v = output voxel (row h0 + t*R + v / W, column v % W) reading input (2*row + kh - 1, 2*col + par)
+            const int h_first = 2 * (h0 + t * C::R) + kh - 1;
+            const float* base = plane + ((ptrdiff_t)h_first * WI + 2 * col0 + par) * p.Cin + ch * KC + c * 4;
+            fill(base, (size_t)2 * WI * p.Cin, (size_t)2 * p.Cin, h_first, 2, ubase + j, col0);
+          }
+          ubase += C::NU;
+          first = (first + C::NLW - C::NU % C::NLW) % C::NLW;
+        }
+      }
+    }
+    tc_report_overflow(p.overflow, amax);
+  }
   // ---------------------------------------------------------------------------------------------- weight-slice producer
-  // One elected lane streams the pre-swizzled (kd, chunk, kh) slices with 1-D TMA bulk copies into the two buffer sets, up to a
-  // whole phase ahead of the MMAs (tc_common.cuh: bulk_g2s).
-  else if (warp == 9) {
+  // One elected lane streams the item's channel group of the pre-swizzled (kd, chunk, kh) slices -- three G-row blocks [W1 | W0 | W2],
+  // 1-D bulk copies -- into the two buffer sets, up to a whole phase ahead of the MMAs (tc_common.cuh: bulk_g2s).
+  else if (warp == 8) {
     if (elect_one()) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w);
       uint32_t phc = 0;
       for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
-        const int od = (it / (ctiles * p.hblocks)) % (p.D / 2);
+        const int cg = (it % C::NG) * C::G;
+        const int od = (it / C::NG / (ctiles * p.hblocks)) % (p.D / 2);
         for (int kd = 0; kd < 3; ++kd) {
-          const int din = 2 * od + kd - 1;              // must enumerate the same phases as the MMA warp and the loaders
+          const int din = 2 * od + kd - 1;              // must enumerate the same phases as the consumer and the loaders
           if (din < 0 || din >= p.D) continue;
           for (int ch = 0; ch < nchunk; ++ch, ++phc) {
             for (int kh = 0; kh < 3; ++kh) {
               const uint32_t slot = (phc & 1) * 3 + kh;
               const size_t slice = ((size_t)kd * nchunk + ch) * 3 + kh;
               mbar_wait_relaxed(&b_empty[slot], ((phc >> 1) & 1) ^ 1);
-              mbar_arrive_expect_tx(&b_full[slot], C::B_SLICE);
-              bulk_g2s(b_buf + slot * C::B_SLICE, wsrc + slice * C::B_SLICE, C::B_SLICE, &b_full[slot]);
+              mbar_arrive_expect_tx(&b_full[slot], C::B_SUB);
+#pragma unroll
+              for (int kw = 0; kw < 3; ++kw)
+                bulk_g2s(b_buf + slot * C::B_SUB + kw * C::G * C::ROWB, wsrc + slice * C::B_SLICE + (size_t)(kw * COUT + cg) * C::ROWB,
+                         C::G * C::ROWB, &b_full[slot]);
             }
           }
         }
@@ -390,9 +355,6 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
     }
     __syncwarp();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 template <int COUT, int KC, int W, int TILES, bool GW = false>
@@ -415,7 +377,7 @@ static int launch_tcs2(Tcs2Params& p, cudaStream_t stream) {
   p.hblocks = (p.H / 2 + C::HBLK - 1) / C::HBLK;
   if (GW) p.ctiles = (p.Wr + C::CSTEP - 1) / C::CSTEP;
   else p.Wr = W, p.ctiles = 1;
-  const long long items = (long long)p.B * (p.D / 2) * p.hblocks * p.ctiles;
+  const long long items = (long long)p.B * (p.D / 2) * p.hblocks * p.ctiles * C::NG;
   OSB_REQUIRE(items < (1ll << 31), "conv3d_tcs2: too many work items");
   p.items = (int)items;
   const int sms = sm_count();
@@ -464,13 +426,13 @@ static int conv3d_k3_s2_tc_impl(const float* x_ndhwc, const void* w_split, const
   OSB_REQUIRE(p.overflow, "tensor-core conv: cannot allocate the overflow flag");
   cudaStream_t s = (cudaStream_t)stream;
   if (W == 32 && Cout == 96) return launch_tcs2<96, 16, 16, 1>(p, s);           // StereoBase conv3[0]: 4c -> 6c as two channel slices
-  if (W == 32 && Cout == 64) return launch_tcs2<64, 16, 16, 2>(p, s);
-  if (W == 128 && Cout == 64) return launch_tcs2<64, 16, 64, 2>(p, s);
-  if (W == 64 && Cout == 64) return launch_tcs2<64, 16, 32, 2>(p, s);
+  if (W == 32 && Cout == 64) return launch_tcs2<64, 16, 16, 1>(p, s);
+  if (W == 128 && Cout == 64) return launch_tcs2<64, 16, 64, 1>(p, s);
+  if (W == 64 && Cout == 64) return launch_tcs2<64, 16, 32, 1>(p, s);
   if (W == 64 && Cout == 128) return launch_tcs2<128, 16, 32, 1>(p, s);
   if (W == 64 && Cout == 96) return launch_tcs2<96, 16, 32, 1>(p, s);           // StereoBase conv2[0]: 2c -> 4c = 96
   p.Wr = W / 2;
-  if (Cout == 64) return launch_tcs2<64, 16, 128, 2, true>(p, s);
+  if (Cout == 64) return launch_tcs2<64, 16, 128, 1, true>(p, s);
   return launch_tcs2<128, 16, 128, 1, true>(p, s);
 }
 

@@ -107,7 +107,7 @@ int osb_regression_values_fwd(const float* prob, const float* values, float* out
 //     gate = sigmoid(Conv2d(Cf/2 -> Cv, 1, bias)(LeakyReLU(BN(Conv2d(Cf -> Cf/2, 1)(feat)))))
 // written CHANNELS-LAST and zero-padded, (B, H, W, Cpad), the operand the tensor-core conv epilogues multiply by
 // (tc_common.cuh: store_ndhwc_chunk32 gate0).  The unfused path was two 1x1-conv launches plus a layout conversion per gate --
-// 15 launches and 0.7 ms of latency-bound work per StereoBase forward at BASELINE config 3 (profiles/r2_c3_launches.csv).
+// 15 launches of latency-bound work per StereoBase forward.
 // CTA = 8 consecutive pixels of one image x 128 threads (16 channel groups x 8 pixels): the feature tile [Cf][8] is staged in shared
 // memory, a thread produces 4 channels of one pixel at a time (one LDG.128 of the (Cin, Cout)-packed weights per input channel,
 // shared by the 8 pixel lanes).  A first version with 32-pixel tiles left the 1/16-resolution gates on 64 CTAs: 244 us.

@@ -172,7 +172,7 @@ int osb_avgpool_pairs_fwd(const float* x, float* y, long long outer, int n, long
   OSB_REQUIRE(x && y, "avgpool_pairs: null pointer");
   OSB_REQUIRE(outer > 0 && n >= 2 && inner > 0, "avgpool_pairs: bad shape outer=%lld n=%d inner=%lld", outer, n, inner);
   const long long total = outer * (n / 2) * inner;
-  const unsigned blocks = (unsigned)std::min<long long>((total + 255) / 256, 148ll * 32);
+  const unsigned blocks = (unsigned)std::min<long long>((total + 255) / 256, (long long)osb::sm_count() * 32);
   avgpool_pairs_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, y, (size_t)outer, n, (size_t)inner);
   count_launch();
   return check_launch("avgpool_pairs_kernel");

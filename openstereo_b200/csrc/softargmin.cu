@@ -1,4 +1,4 @@
-// Soft-argmin tails for sm_100a: softmax over the disparity axis fused with the expectation, with or without the
+// Soft-argmin tails for sm_90a: softmax over the disparity axis fused with the expectation, with or without the
 // trilinear x4 up-sampling in front of it, and the per-image EPE partial sums.
 //
 //   disparity_regression(F.softmax(x, 1), D)   stereo/modeling/disp_pred/disp_regression.py:8-12

@@ -1,13 +1,13 @@
-// Shared device helpers of the tcgen05 convolution kernels (conv3d_tc.cu: W = 128 specialisation; conv3d_tcg.cu: generic
-// multi-row tiles).  See conv3d_tc.cu for the design notes.
+// Shared device helpers of the Hopper (wgmma) convolution kernels (conv3d_tc.cu: W = 128 specialisation; conv3d_tcg.cu: generic
+// multi-row tiles; conv3d_tcs2.cu, conv3d_tcdc.cu).  See conv3d_tc.cu for the design notes.
 #pragma once
 #include "common.cuh"
 
 namespace osb {
 
 // ------------------------------------------------------------------------------------------------ small PTX wrappers
-// Wait used by the helper roles (loaders, epilogue): they run AHEAD of the MMA warp and would otherwise burn issue
-// slots of the shared schedulers in a tight try_wait loop; back off between probes.
+// Wait used by the helper roles (loaders, weight producer): they run AHEAD of the consumer warpgroup and would otherwise burn
+// issue slots of the shared schedulers in a tight try_wait loop; back off between probes.
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity) {
   uint32_t done;
   for (;;) {
@@ -23,31 +23,125 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor: 8-row atoms of 1024 bytes (SBO), version 1, address 0.
+// K-major, SWIZZLE_128B wgmma shared-memory matrix descriptor: 8-row atoms of 1024 bytes (SBO), start address 0.
 __device__ __forceinline__ uint64_t desc_sw128_base() {
   uint64_t d = 0;
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// Instruction descriptor of a dense kind::f16 MMA: fp16 A and B (formats 0), fp32 accumulator, both operands K-major.
-__device__ __forceinline__ uint32_t idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// K-major SWIZZLE_64B descriptor base (64-byte rows, 512-byte 8-row atoms)
+__device__ __forceinline__ uint64_t desc_sw64_base() {
+  uint64_t d = 0;
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(512 >> 4) << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
 }
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+
+// ------------------------------------------------------------------------------------------------ wgmma
+// D (64 x N, fp32, registers of the issuing warpgroup) (+)= A (64 x 16 fp16, K-major, shared) * B (N x 16 fp16, K-major, shared)^T.
+// `accumulate` = 0 overwrites D.  Every thread of the warpgroup executes it (warpgroup-uniform control flow).
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate)
       : "memory");
 }
+
+template <>
+__device__ __forceinline__ void wgmma_f16<48>(float (&d)[24], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
+}
+
+template <>
+__device__ __forceinline__ void wgmma_f16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
+}
+
+template <>
+__device__ __forceinline__ void wgmma_f16<96>(float (&d)[48], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %50, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
+}
+
+template <>
+__device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
+}
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// One K = 16 step of the 3xFP16 product (below) into a 128-row accumulator tile held as two m64 halves: half h reads operand rows
+// 64h .. 64h + 63 (a_half = their descriptor offset in 16-byte units), `lo` = descriptor offset of the lo half of a row.
+template <int N>
+__device__ __forceinline__ void wg_mma_split(float (&acc)[2][N / 2], uint64_t da, uint32_t a_half, uint64_t db, uint32_t lo,
+                                             uint32_t accumulate) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    wgmma_f16<N>(acc[h], da + h * a_half + lo, db, accumulate);   // small terms first
+    wgmma_f16<N>(acc[h], da + h * a_half, db + lo, 1);
+    wgmma_f16<N>(acc[h], da + h * a_half, db, 1);
+  }
+}
+// Consumer-side release of a ring slot / weight buffer read by the wgmmas just waited for: one arrival per warp (barrier count 4).
+__device__ __forceinline__ void wg_release(uint64_t* bar, int lane) {
+  if (lane == 0) mbar_arrive(bar);
+}
+// Accumulator fragment of wgmma m64nN (f32): register 4j + r of lane l in warp w of the warpgroup holds row 16w + l/4 + 8(r/2),
+// column 8j + 2(l%4) + r%2.  The epilogues own one voxel (tile row) per thread, so a finished tile goes through shared memory:
+// `stage` is [128 rows][ld floats], ld = N + 4 (rows 16 B apart in bank space: the per-row LDS.128 of a warp are conflict-free).
+template <int N>
+__device__ __forceinline__ void wg_stage(float* stage, int ld, const float (&acc)[2][N / 2], int wq, int lane) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* r0 = stage + (64 * h + 16 * wq + (lane >> 2)) * ld + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+      *reinterpret_cast<float2*>(r0 + 8 * ld + 8 * j) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+    }
+  }
+}
+// 16 consecutive staged accumulator columns of one tile row
+__device__ __forceinline__ void stage_ld16(const float* row, uint32_t* r) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float4 v = reinterpret_cast<const float4*>(row)[i];
+    r[4 * i] = __float_as_uint(v.x), r[4 * i + 1] = __float_as_uint(v.y), r[4 * i + 2] = __float_as_uint(v.z), r[4 * i + 3] = __float_as_uint(v.w);
+  }
+}
+
 // 1-D bulk copy global -> shared through the TMA engine (SASS UBLKCP), completion counted in bytes on an mbarrier.  The weight
 // slices are stored PRE-SWIZZLED in global memory (ops.pack_tc_weight), so one elected thread can stream them with no register
-// staging, any number of slices in flight -- the LDG/STS weight loaders exposed one full L2 round trip per 12-24 KB slice
-// (12 slices per work item of the backbone layers: ~10 us of the 25 us an item took, profiles/r2_step_ncu_summary.md).
+// staging, any number of slices in flight, where LDG/STS weight loaders would expose one full L2 round trip per slice.
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
@@ -66,33 +160,10 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 constexpr int TC_BSLOTS = 2;       // weight-slice buffers per kh tap: the producer runs one (kd, chunk) phase ahead of the MMAs
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
-// One lane of a fully converged warp (the tcgen05 issue idiom: control flow stays warp-uniform so descriptors live in
-// uniform registers; only the MMA / commit instructions are predicated on the elected lane).
+// One lane of a fully converged warp (control flow stays warp-uniform; only the bulk-copy issue is predicated on the elected lane).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(pred));
@@ -100,11 +171,10 @@ __device__ __forceinline__ bool elect_one() {
 }
 // 3xFP16 operand split (fp32-accurate products on the 16-bit tensor-core rate).
 //   x * s  =  hi + lo + r,   hi = fp16_rn(x*s),  lo = fp16_rn(x*s - hi),   |r| <= max(2^-22 |x*s|, 2^-25)
-// and every product is issued as  a_lo*b_hi + a_hi*b_lo + a_hi*b_hi  on tcgen05.mma.kind::f16 with fp32 accumulation in TMEM
+// and every product is issued as  a_lo*b_hi + a_hi*b_lo + a_hi*b_hi  on wgmma (fp16 operands) with fp32 accumulation in registers
 // (the dropped lo*lo term is <= 2^-22 of the product; both roundings are to nearest, so the residual is zero-mean).  fp16
-// carries the same 11 significant bits as TF32, so the accuracy equals the 3xTF32 scheme this replaces (round 1 / early round 2)
-// while an MMA instruction covers K = 16 channels instead of 8: half the MMAs, half the operand bytes in shared memory --
-// the two resources that bounded the TF32 kernels (DESIGN.md section 4.3).  What fp16 lacks is exponent range, hence the
+// carries the same 11 significant bits as TF32, so the accuracy equals a 3xTF32 scheme while an MMA instruction covers K = 16
+// channels instead of 8: half the MMAs, half the operand bytes in shared memory.  What fp16 lacks is exponent range, hence the
 // power-of-two scales: activations are staged as x * TC_ACT_SCALE (|x| < 65504 / TC_ACT_SCALE = 4094 is representable; smaller
 // magnitudes keep 22 significant bits down to |x| ~ 2^-7 and an ABSOLUTE error of 2^-29 below that), weights are pre-scaled per
 // output channel on the host so that max |w| lands in [2^14, 2^15) (ops.pack_tc_weight), and the epilogue's folded-BN scale
@@ -138,25 +208,14 @@ __device__ __forceinline__ void tc_report_overflow(unsigned int* flag, float ama
   if (amax > TC_F16_MAX) atomicAdd(flag, 1u);
 }
 
-// The TMEM accumulator of tcgen05.mma rounds TOWARDS ZERO (tools/tc_probe.cu acc, profiles/r2_acc_probe.log: accumulating the same
-// positive product block n times loses n * 2^-24 of the sum, where round-to-nearest would lose ~sqrt(n) * 2^-25).  Each MMA
-// therefore shrinks the running sum by ~c * ulp, and because E[partial sum after i of n MMAs | final] = (i/n) * final, an
-// accumulator that received n MMAs comes out as final * (1 - kappa * n) plus zero-mean noise.  The shrink is coherent from
-// layer to layer (round 1: -4e-5 on the GwcNet logits, 2.3e-3 px EPE), the noise is not -- so the epilogue undoes the EXPECTED
-// loss: raw sum * (1 + kappa * n), n = MMAs issued into that accumulator for this work item.  kappa is measured
-// (tools/parity_bisect.py --layers: every kernel variant agrees within 10 %); osb_set_rz_kappa() overrides it for calibration.
+// The tensor core's fp32 accumulation truncates (rounds towards zero) rather than rounding to nearest.  Each MMA therefore
+// shrinks the running sum by ~c * ulp, and because E[partial sum after i of n MMAs | final] = (i/n) * final, an accumulator that
+// received n MMAs comes out as final * (1 - kappa * n) plus zero-mean noise.  The shrink is coherent from layer to layer, the
+// noise is not -- so the epilogue undoes the EXPECTED loss: raw sum * (1 + kappa * n), n = MMAs issued into that accumulator for
+// this work item.  kappa is a calibration constant (tools/parity_bisect.py --layers); osb_set_rz_kappa() overrides it.
 float rz_kappa();           // api.cu
 
 
-// K-major SWIZZLE_64B descriptor base (64-byte rows, 512-byte 8-row atoms)
-__device__ __forceinline__ uint64_t desc_sw64_base() {
-  uint64_t d = 0;
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(512 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;
-  return d;
-}
 // byte offset of 16-byte chunk `c` of K-major row `row` inside a swizzled operand tile
 template <int KC>
 __device__ __forceinline__ int swz_offset(int row, int c) {
@@ -193,13 +252,13 @@ struct TcK {
 // ------------------------------------------------------------------------------- coalesced channels-last epilogue output
 // An epilogue thread owns ONE voxel and all of its channels.  Storing those directly makes every STG.128 of a warp touch
 // 32 different 128-byte lines (16 B of each) -- 8x the L1 wavefronts of a coalesced store, on the data pipe the tensor
-// core's operand reads also use (ncu r1_conv3d_tc_v7: tc 49 % + lsu 43 % of that pipe).  Instead the warp transposes its
+// core's operand reads also use.  Instead the warp transposes its
 // 32 voxels x 32 channels through a private shared-memory tile so one instruction covers 4 voxels x 128 contiguous bytes;
 // folded BN, the channels-last residual and the activation are applied after the transpose, where a lane's four channels
 // are the same for every voxel (scale/shift sit in registers instead of one LDS per channel).
 constexpr int TP_STRIDE = 36;                       // floats per tile row: 144 B keeps STS.128 / LDS.128 conflict-free
-constexpr int TP_WARP_FLOATS = 32 * TP_STRIDE;      // 4608 B per epilogue warp
-constexpr int TP_BYTES = 4 * TP_WARP_FLOATS * 4;    // four epilogue warps
+constexpr int TP_WARP_FLOATS = 32 * TP_STRIDE;      // 4608 B per epilogue warp (the kernels reuse the warp's own rows of the staged
+                                                    // accumulator tile, which the warp has read into registers by then)
 
 // sum[32]: raw accumulator sums of this lane's voxel for channels [c, c+32).  y0 / res0 point at channel c of the voxel
 // owned by lane 0; lane k's voxel lies vstride floats further per lane.  sc / sh point at channel c of the folded BN.

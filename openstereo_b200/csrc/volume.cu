@@ -1,4 +1,4 @@
-// Fused cost-volume constructor for sm_100a.
+// Fused cost-volume constructor for sm_90a.
 //
 // Replaces the reference's Python loops of slice assignments
 //   build_gwc_volume     stereo/modeling/cost_volume/cost_volume.py:68-78

@@ -10,8 +10,8 @@ machine without easydict/timm (SURVEY.md section 8c); where it IS importable, us
 
 Division of labour: the 2D feature extractors are out of the kernel scope (SURVEY.md section 2.1
 row 12) and stay torch.nn/cuDNN -- except their 1/2-resolution front (eight 32->32 3x3 convs), which
-reuses the tcgen05 conv kernel when the input is 256 rows high (_front_tc); everything from the cost
-volume to the disparity map runs in the sm_100a kernels through the engines of aggregation.py.  The 3D modules below are PARAMETER
+reuses the wgmma conv kernel when the input is 256 rows high (_front_tc); everything from the cost
+volume to the disparity map runs in the sm_90a kernels through the engines of aggregation.py.  The 3D modules below are PARAMETER
 CONTAINERS: they are never called, only read by the engines.
 """
 import torch
@@ -23,7 +23,7 @@ from . import ops
 from .aggregation import GwcAggregation, PSMAggregation
 
 
-USE_TC_BACKBONE = True      # the 2D extractor's 3x3 residual blocks on the tcgen05 kernels (False: everything 2D stays cuDNN)
+USE_TC_BACKBONE = True      # the 2D extractor's 3x3 residual blocks on the wgmma kernels (False: everything 2D stays cuDNN)
 
 
 def _cfg_get(cfgs, key, default=None):
@@ -40,7 +40,7 @@ def _cb(cin, cout, k, stride, pad, dilation, bias=False):
 
 def _front_tc_ok(net, x):
     """The 1/2-resolution front of the backbone (firstconv[1:], layer1: eight 32->32 3x3 convs, where cuDNN's best fp32
-    kernel reaches ~8 TFLOP/s) can run on the tcgen05 conv kernel when the half-resolution HEIGHT is the 128-voxel UMMA tile:
+    kernel reaches ~8 TFLOP/s) can run on the wgmma conv kernel when the half-resolution HEIGHT is the 128-voxel M tile:
     a 2D conv commutes with transposing the image, so the kernel sees (rows = W/2, columns = H/2 = 128) and the 3x3 weights
     with kh/kw swapped, as a one-plane 3D conv (the kd != 1 phases are skipped for D = 1)."""
     return (getattr(net, "_osb_folded", False) and x.is_cuda and x.dim() == 4 and x.shape[2] == 2 * ops.TC_WIDTH and x.shape[3] % 2 == 0
@@ -62,7 +62,7 @@ def _front_tc(net, x):
 
 
 def _tc2d(net, conv, t, act, residual=None, last=False, transpose=False):
-    """One BN-folded 3x3 Conv2d (dilation 1 or 2) on the tcgen05 kernels: t (B, rows, 128, Cin) channels-last."""
+    """One BN-folded 3x3 Conv2d (dilation 1 or 2) on the wgmma kernels: t (B, rows, 128, Cin) channels-last."""
     cache = net.__dict__.setdefault("_osb_tc2d", {})
     dil = conv.dilation[0]
     if id(conv) not in cache:
@@ -95,7 +95,7 @@ def _block_tc_ok(blk, c):
 def _stage_tc(net, stage, x):
     """A residual stage (layer2 / layer3 / the dilated layer4 of the PSMNet-style extractor: gwcnet_backbone.py:38-60): a
     first block that changes stride / channels (+ 1x1 downsample) stays cuDNN; the identity-shortcut 3x3 blocks run on the
-    tcgen05 kernel when the feature map is 128 columns wide, channels-last in between, NCHW out of the last epilogue."""
+    wgmma kernel when the feature map is 128 columns wide, channels-last in between, NCHW out of the last epilogue."""
     blocks = list(stage.children())
     usable = getattr(net, "_osb_folded", False) and x.is_cuda and x.dtype == torch.float32 and _agg.USE_TENSOR_CORES and USE_TC_BACKBONE
     y, rest = x, blocks
@@ -115,7 +115,7 @@ def _stage_tc(net, stage, x):
 
 def _lastconv_tc_ok(net, x):
     """lastconv = conv3x3(320->128)+BN+ReLU, conv1x1(128->12) (gwcnet_backbone.py:62-67): cuDNN picks an FFT algorithm for the
-    320-channel 3x3 (2.1 ms); on the tcgen05 kernel it is the layer3 conv with 20 K chunks."""
+    320-channel 3x3 (2.1 ms); on the wgmma kernel it is the layer3 conv with 20 K chunks."""
     convs = [m for m in net.lastconv.modules() if isinstance(m, nn.Conv2d)]
     return (getattr(net, "_osb_folded", False) and x.is_cuda and x.dtype == torch.float32 and _agg.USE_TENSOR_CORES and USE_TC_BACKBONE
             and x.shape[3] == ops.TC_WIDTH and len(convs) == 2 and convs[0].kernel_size == (3, 3) and convs[0].stride == (1, 1)
@@ -131,7 +131,7 @@ def _lastconv_tc(net, x):
 
 def gwc_extract(net, x):
     """feature_extraction.forward of gwcnet_backbone.py:80-93 on any module with its attribute names (this file's mirror or a
-    BN-folded copy of the reference's own class): identical graph, the 3x3 residual blocks on the tcgen05 kernels where a
+    BN-folded copy of the reference's own class): identical graph, the 3x3 residual blocks on the wgmma kernels where a
     variant serves the shape, everything else through the module's own layers (cuDNN)."""
     x = _front_tc(net, x) if _front_tc_ok(net, x) else net.layer1(net.firstconv(x))
     l2 = _stage_tc(net, net.layer2, x)

@@ -1,5 +1,5 @@
 """Reference-facing operators: same names, argument meaning and error behaviour as the OpenStereo
-functions they replace, executed by the sm_100a kernels in libopenstereo_b200.so.
+functions they replace, executed by the sm_90a kernels in libopenstereo_b200.so.
 
 PyTorch is plumbing here: it owns device memory (tensor.data_ptr()) and the stream
 (torch.cuda.current_stream()).  All arithmetic happens in the hand-written kernels.  There is no
@@ -391,7 +391,7 @@ def conv3d_1x1(x0, w_packed, scale=None, shift=None, residual=None, gate=None, a
     return y.squeeze(2) if squeeze else y
 
 
-# --------------------------------------------------------------------------- tensor-core conv (tcgen05, 3xFP16 split)
+# --------------------------------------------------------------------------- tensor-core conv (wgmma, 3xFP16 split)
 def conv3d_tc_supported(cin, cout, w, stride=1):
     return bool(_lib.lib.osb_conv3d_tc_supported(int(cin), int(cout), int(w), int(stride)))
 
@@ -478,8 +478,8 @@ def f16_split(w):
 
 
 class TcWeight:
-    """A conv weight packed for the tcgen05 kernels: `data` fp16 [3 kd][Cin/kc][3 kh][3*Cout (kw-major)][kc hi | kc lo] of
-    w * 2^e_c with the 16-byte chunks of every row stored in UMMA swizzle order (pack_tc_weight), and `inv` = 2^-(e_c + TC_ACT_SCALE_LOG2) per output channel -- the exact factor the epilogue must apply.
+    """A conv weight packed for the wgmma kernels: `data` fp16 [3 kd][Cin/kc][3 kh][3*Cout (kw-major)][kc hi | kc lo] of
+    w * 2^e_c with the 16-byte chunks of every row stored in the wgmma swizzle order (pack_tc_weight), and `inv` = 2^-(e_c + TC_ACT_SCALE_LOG2) per output channel -- the exact factor the epilogue must apply.
     `cout` is the packed row count per kw slice (narrow heads are zero-padded to 16), `cout_real` the layer's channels."""
     __slots__ = ("data", "inv", "kc", "cout", "cout_real", "ksize", "_eff")
 
@@ -522,7 +522,7 @@ def pack_tc_weight(weight, kc=None, kw_order=(0, 1, 2), pad_cout_to=None):
     both = both.permute(4, 2, 5, 6, 1, 0, 3)                           # (kd, chunk, kh, kw, co, half, ci)
     data = both.reshape(k, cin // kc, k, k * cout, 2 * kc).contiguous()
     # Pre-swizzle: the kernels copy a (kd, chunk, kh) slice into shared memory with ONE 1-D TMA bulk copy, so global memory already
-    # holds the UMMA K-major swizzled layout: 16-byte chunk c of row n sits at chunk c ^ (n & 7) (128-byte rows, SWIZZLE_128B) or
+    # holds the wgmma K-major swizzled layout: 16-byte chunk c of row n sits at chunk c ^ (n & 7) (128-byte rows, SWIZZLE_128B) or
     # c ^ ((n >> 1) & 3) (64-byte rows, SWIZZLE_64B) -- an XOR within the row, i.e. a gather with an involutive index.
     cpr = (2 * kc) // 8                                                 # 16-byte chunks per row (8 halfs each)
     rows = torch.arange(k * cout, device=data.device)

@@ -1,5 +1,5 @@
 """patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo, built by the
-reference's own classes from an unchanged cfg YAML) run its cost-volume hot path on the sm_100a kernels.
+reference's own classes from an unchanged cfg YAML) run its cost-volume hot path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each
 needs its own rebinding:
@@ -61,7 +61,7 @@ def _refuse(what):
 def _patch_backbone(bb, net, extract, split):
     """2D feature extractor (gwcnet_backbone.py:96-107 / psmnet_backbone.py:118-126; not a SURVEY section-8 row, but inside the
     measured forward): CUDA inference calls run a BN-folded twin of `net` whose identity-shortcut 3x3 residual blocks use the
-    tcgen05 conv kernels where a variant serves the shape (host_models.gwc_extract / psm_extract; every other layer is the
+    wgmma conv kernels where a variant serves the shape (host_models.gwc_extract / psm_extract; every other layer is the
     module's own cuDNN conv), left and right images in ONE batched pass (the weights are shared).  Parameters stay in `net`;
     the twin is rebuilt when they change.  Any other call (CPU, training, autograd recording) runs the reference's forward."""
     from . import host_models
@@ -335,7 +335,7 @@ _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _pa
 
 def patch(model, strict=True, backbone=True):
     """Rebind the hot path of a reference model instance in place and return it.  backbone=True (default) also routes the
-    GwcNet / PSMNet 2D extractor's residual blocks to the tcgen05 conv kernels in CUDA inference calls (_patch_backbone);
+    GwcNet / PSMNet 2D extractor's residual blocks to the wgmma conv kernels in CUDA inference calls (_patch_backbone);
     backbone=False leaves the extractor entirely to the reference's cuDNN code."""
     if not isinstance(model, torch.nn.Module):
         raise TypeError("patch() expects an nn.Module")

@@ -1,7 +1,6 @@
 """GPU: the tensor-core convolutions at GENERAL image widths (VERDICT round 1, weak #8 / next #7).
 
-Round 1's tcgen05 kernels served W' in {128, 64, 32} only (a 512-pixel-wide input); every other width fell back to the fp32
-CUDA-core kernels.  The GW instantiations of conv3d_tcg.cu / conv3d_tcs2.cu / conv3d_tcdc.cu tile an image row into 128-column
+The whole-row tensor-core variants serve W' in {128, 64, 32} only (a 512-pixel-wide input).  The GW instantiations of conv3d_tcg.cu / conv3d_tcs2.cu / conv3d_tcdc.cu tile an image row into 128-column
 segments with a one-column halo, so the reference's own timing shape (544x960 -> W' = 240, tools/measure.py:32), KITTI
 (1248 -> 312) and IGEV's config-5 width (640 -> 160) take the tensor-core path.  Op level: against an fp64 convolution
 (<= 1e-5 of the output scale, the bar of the whole-row variants); engine level: against the CPU oracle of the reference modules

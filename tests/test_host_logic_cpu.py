@@ -25,7 +25,7 @@ def test_pack_tc_weight_split(kc, order):
     assert isinstance(p, ops.TcWeight) and p.kc == kc and p.cout == cout
     assert p.data.shape == (3, cin // kc, 3, 3 * cout, 2 * kc) and p.data.is_contiguous() and p.data.dtype == torch.float16
     assert torch.isfinite(p.data.float()).all()
-    # undo the UMMA pre-swizzle (16-byte chunk c of row n is stored at c ^ key(n): an involution), then
+    # undo the wgmma pre-swizzle (16-byte chunk c of row n is stored at c ^ key(n): an involution), then
     # un-permute: [kd][chunk][kh][kw*cout + co][half*kc + ci] -> (half, co, ci, kd, kh, kw) in the requested kw order
     cpr = 2 * kc // 8
     rows = torch.arange(3 * cout)
@@ -154,7 +154,7 @@ def test_pack_tc_weight_k4_transposed():
 
 
 def test_tensor_core_capability_queries():
-    """Which shapes the tcgen05 variants serve (answered by the C library without a GPU): whole-row widths, general widths through
+    """Which shapes the tensor-core variants serve (answered by the C library without a GPU): whole-row widths, general widths through
     column tiles (>= OSB_TC_MIN_WIDTH = 24), the StereoBase plan (Cout 96, k4 transposed conv, W' = 16 channel slices)."""
     assert ops.conv3d_tc_kc(32, 32, 128) == 32 and ops.conv3d_tc_kc(64, 64, 64) == 16 and ops.conv3d_tc_kc(128, 128, 32) == 16
     for w in (240, 312, 160, 120, 78, 60, 24):
@@ -171,7 +171,7 @@ def test_tensor_core_capability_queries():
 
 
 def test_stereobase_tc_route_gating_without_gpu():
-    """StereoBaseAggregation.tc_route_ok: shape / channel-plan gates of the tcgen05 route (pure host logic)."""
+    """StereoBaseAggregation.tc_route_ok: shape / channel-plan gates of the tensor-core route (pure host logic)."""
     from openstereo_b200 import aggregation as agg
     from oracle import aggregation as oagg
     m = oagg.StereoBaseHourglass(24, [96, 64, 192, 160]).eval()

@@ -203,7 +203,7 @@ def test_engine_repacks_after_weight_update(osb):
 
 
 def test_gwc_aggregation_full_width_tensor_cores(osb):
-    """W' = 128 (a 512-pixel-wide input): the stem and classifier convs run on the tcgen05 3xTF32 kernel.  Compared with
+    """W' = 128 (a 512-pixel-wide input): the stem and classifier convs run on the wgmma 3xFP16 kernel.  Compared with
     the CPU oracle on a short volume (D'=8, H'=10) and with the CUDA-core path of the same engine."""
     _, agg, _, _ = osb
     m = oagg.GwcDispProcessor(maxdisp=32, downsample=4, num_groups=40, use_concat_volume=True, concat_channels=12).eval()
@@ -232,7 +232,7 @@ def test_gwc_aggregation_full_width_tensor_cores(osb):
 
 
 def test_backbone_front_tensor_cores(osb):
-    """256-row inputs: firstconv[1:] + layer1 (eight 32->32 3x3 convs at 1/2 resolution) run on the tcgen05 conv kernel
+    """256-row inputs: firstconv[1:] + layer1 (eight 32->32 3x3 convs at 1/2 resolution) run on the wgmma conv kernel
     through the transposed-image mapping.  Compared with cuDNN on the same BN-folded weights and with the unfolded module
     on the CPU (fp32); 3xTF32 keeps fp32 accuracy, so the tolerance is the usual accumulation-order one."""
     _, agg, hm, _ = osb

@@ -434,7 +434,7 @@ def test_conv3d_s2_tc(ops, b, cin, cout, d, h, w):
     (2, 64, 64, 2, 5, 32),      # PSMNet conv5, ragged rows
     (1, 64, 32, 3, 10, 64),     # conv6: 1/8 -> 1/4 res (five 2-row tiles per item)
     (2, 16, 32, 1, 3, 64),      # ragged, single input plane
-    (1, 32, 32, 4, 9, 64),      # conv6 shape class on the parity-quad kernel (channels-last calls): odd row count, 4 planes
+    (1, 32, 32, 4, 9, 64),      # conv6 shape class (channels-last calls): odd row count, 4 planes
     (1, 64, 32, 2, 1, 64),      # one input row
 ])
 def test_deconv3d_tc(ops, b, cin, cout, d, h, w):

@@ -200,7 +200,7 @@ def _stereobase_case(osb, b, dq, hq, wq, seed):
 
 
 def test_stereobase_hourglass_tensor_cores(osb):
-    """Hourglass(24, [96, 64, 192, 160]) at W' = 128 (BASELINE config 3's width) on a short volume: tcgen05 route vs the CPU oracle
+    """Hourglass(24, [96, 64, 192, 160]) at W' = 128 (BASELINE config 3's width) on a short volume: tensor-core route vs the CPU oracle
     of the reference module and vs the fp32 CUDA-core route of the same engine."""
     agg, ops = osb
     m, vol, feats = _stereobase_case(osb, 1, 8, 16, 128, 460)
@@ -216,7 +216,7 @@ def test_stereobase_hourglass_tensor_cores(osb):
     got = eng(vol.cuda(), fg)
     launches = _lib.launch_count() - before
     err = ((got.cpu() - want_geo).abs().max() / want_geo.abs().max()).item()
-    print("StereoBase hourglass on tcgen05: rel err vs oracle %.2e, %d launches" % (err, launches))
+    print("StereoBase hourglass on the tensor cores: rel err vs oracle %.2e, %d launches" % (err, launches))
     assert err <= 5e-5
     agg.USE_TENSOR_CORES = False
     try:

@@ -1,9 +1,9 @@
 """GPU, last in collection order: end-to-end parity of the host mirrors at the BENCH configurations (256x512, D = 192), where
 every tensor-core route is live at once, against the CPU oracle with the same seeded weights.  Bar: the north star's 1e-3 px EPE.
 
-Round 1 failed here (2.27e-3 px): the TMEM accumulator of tcgen05.mma rounds towards zero, every conv came out ~1e-6 too small,
-and the shrink adds up coherently over the ~80 layers in front of a sharp 192-bin softmax (profiles/r2_parity_bisect.md).
-Fixed by the unbiased operand split + the expected-loss correction of the epilogues (csrc/tc_common.cuh)."""
+The tensor core's fp32 accumulation truncates, so every conv comes out slightly too small, and the shrink adds up coherently over
+the ~80 layers in front of a sharp 192-bin softmax.  The unbiased operand split + the expected-loss correction of the epilogues
+(csrc/tc_common.cuh) keep it inside the bar."""
 import pytest
 import torch
 
@@ -42,7 +42,7 @@ def _gwc_models(hm):
 
 @pytest.mark.parametrize("tc_backbone", [True, False])
 def test_gwcnet_bench_configuration_epe(osb, tc_backbone):
-    """BASELINE config 2, one pair.  tc_backbone=True: the 2D extractor's residual blocks on the tcgen05 kernels as well (86
+    """BASELINE config 2, one pair.  tc_backbone=True: the 2D extractor's residual blocks on the wgmma kernels as well (86
     launches); False: the extractor on cuDNN, the in-scope hot path (volume, aggregation, tail) on this library (33 launches)."""
     lib, hm = osb
     oracle, mine = _gwc_models(hm)
@@ -60,7 +60,7 @@ def test_gwcnet_bench_configuration_epe(osb, tc_backbone):
     assert got.shape == want.shape == (1, 256, 512)
     e = (got.cpu() - want).abs().mean().item()
     print("GwcNet 256x512 (backbone on %s) EPE vs oracle: %.3e px, %d launches of this library" % (
-        "tcgen05" if tc_backbone else "cuDNN", e, launches))
+        "wgmma" if tc_backbone else "cuDNN", e, launches))
     assert launches >= (80 if tc_backbone else 30)
     assert want.std() > 10 and e <= EPE_BAR
 
@@ -79,7 +79,7 @@ def test_gwcnet_bench_batch8_epe(osb):
 
 
 def test_psmnet_config1_epe(osb):
-    """BASELINE config 1: PSMNet, one pair at 256x512 (W' = 128: the tcgen05 stem / backbone routes that 256x256 never took)."""
+    """BASELINE config 1: PSMNet, one pair at 256x512 (W' = 128: the wgmma stem / backbone routes that 256x256 never took)."""
     lib, hm = osb
     oracle = omodels.PSMNet(192).eval()
     sd = si.seeded_state_dict(oracle.state_dict(), seed=1, scale=si.PSMNET_SCALE, keep=si.PSMNET_KEEP)

@@ -209,7 +209,7 @@ def c5(iters, B=8, gru_iters=16):
 def gw(iters):
     """GwcNet hot path (gwc+concat volume -> 3D aggregation -> fused tail) at widths the whole-row tensor-core kernels do not serve:
     the reference's own timing shape 1x3x544x960 (tools/measure.py:32, W' = 240) and a KITTI crop 384x1248 (W' = 312).  Three
-    columns: column-tile tcgen05 kernels, the fp32 CUDA-core kernels of the same engine (what round 1 ran at these widths) and the
+    columns: column-tile tensor-core kernels, the fp32 CUDA-core kernels of the same engine (what round 1 ran at these widths) and the
     oracle modules on cuDNN fp32."""
     for (h, w) in ((544, 960), (384, 1248)):
         gen = torch.Generator().manual_seed(17)
@@ -236,7 +236,7 @@ def gw(iters):
             finally:
                 agg.USE_TENSOR_CORES = True
             ms_ref, want = timeit(ref, max(2, iters // 3), warm=1)
-        emit(config="gw GwcNet hot path, 1 pair @%dx%d D=192 (W' = %d: column-tile tcgen05 kernels)" % (h, w, wq),
+        emit(config="gw GwcNet hot path, 1 pair @%dx%d D=192 (W' = %d: column-tile tensor-core kernels)" % (h, w, wq),
              ms_per_step=round(ms, 3), pairs_per_s=round(1e3 / ms, 2), cuda_core_kernels_ms=round(ms_cc, 2),
              reference_cudnn_fp32_ms=round(ms_ref, 2), speedup_vs_cuda_core=round(ms_cc / ms, 2),
              speedup_vs_reference_gpu=round(ms_ref / ms, 2),

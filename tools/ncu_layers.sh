@@ -1,5 +1,5 @@
 #!/bin/bash
-# Source-level `ncu --set full` of ONE launch per tcgen05 kernel variant at its bench shape (tools/layer_prof.py), GPU box:
+# Source-level `ncu --set full` of ONE launch per tensor-core kernel variant at its bench shape (tools/layer_prof.py), on the GPU:
 #     bash tools/ncu_layers.sh <tag> layer[:kernel-regex] ...      e.g.  r2 conv6:conv3d_tcdc conv1s2:conv3d_tcs2 bb64:conv3d_tcg
 # -> gpurun_out/<tag>_<layer>.ncu-rep (with -lineinfo source correlation; read here with `ncu -i ... --page source --csv`)
 set -u

@@ -1,4 +1,4 @@
-"""CPU emulation of the 3xTF32 operand split of the tcgen05 conv kernels, to measure what a split policy costs in
+"""CPU emulation of the 3xTF32 operand split of the tensor-core conv kernels, to measure what a split policy costs in
 end-to-end EPE WITHOUT a GPU (round-2 bisect of the 2.27e-3 px failure at 256x512).
 
 Every Conv3d / ConvTranspose3d (and optionally Conv2d) of the oracle GwcNet is replaced by
