@@ -56,10 +56,18 @@ int osb_tc_overflow_count(osb_stream_t stream, int reset, unsigned int* count);
 int osb_tc_overflow_poll(osb_stream_t stream, unsigned int* host_pinned);
 const unsigned int* osb_tc_overflow_flag(void);
 /* Expected round-towards-zero loss per accumulating tensor-core MMA, undone by the conv epilogues (csrc/tc_common.cuh: rz_kappa;
- * DESIGN.md section 4.3).  Process-wide; returns the previous value; 0 switches the correction off.  The default has not been
- * calibrated separately for H100; with it the full-size GwcNet / PSMNet tests stay within their 1e-3 px EPE bar there.  The
- * setter exists for calibration (tools/parity_bisect.py). */
+ * DESIGN.md section 2.1).  Process-wide; returns the previous value; 0 switches the correction off; values outside [0, 1e-6) are
+ * ignored.  The default 1.57e-8 is calibrated on the H100 (DESIGN.md section 2.1: it removes 87-100 % of the layer-level bias
+ * against fp64).  The setter exists for calibration and tests (tools/parity_bisect.py, tests/test_tc_contract_gpu.py). */
 float osb_set_rz_kappa(float kappa);
+/* Test hooks of the persistent kernels (the tensor-core convolutions and the volume constructors), process-wide.
+ * osb_set_persistent_grid_cap clamps their grid to `cap` CTAs (0 = no cap, the default: one CTA per resident slot) and returns the
+ * previous cap.  Every CTA walks the work items it = blockIdx.x, blockIdx.x + gridDim.x, ..., so cap = 1 makes one CTA compute every
+ * item in order; an item's result does not depend on the CTA that computes it, so outputs are bit-identical for any cap.
+ * osb_tc_last_variant returns the template arguments of the tensor-core instantiation this thread launched last, e.g.
+ * "tcg<64,16,64,1,1,0,1>" (COUT, KC, W, TILES, DIL, GW, GATE), "tc<32>", "tcs2<...>", "tcdc<...>"; "" before the first launch. */
+int osb_set_persistent_grid_cap(int cap);
+const char* osb_tc_last_variant(void);
 
 /* ---------------------------------------------------------------- cost-volume constructors --- */
 

@@ -85,6 +85,10 @@ def _load():
     lib.osb_tc_overflow_flag.restype = ctypes.c_void_p
     lib.osb_set_rz_kappa.argtypes = [ctypes.c_float]
     lib.osb_set_rz_kappa.restype = ctypes.c_float
+    lib.osb_set_persistent_grid_cap.argtypes = [ctypes.c_int]
+    lib.osb_set_persistent_grid_cap.restype = ctypes.c_int
+    lib.osb_tc_last_variant.argtypes = []
+    lib.osb_tc_last_variant.restype = ctypes.c_char_p
     for name, argtypes in SIGNATURES.items():
         try:
             fn = getattr(lib, name)

@@ -20,6 +20,23 @@ void set_error(const char* fmt, ...) {
 static std::atomic<float> g_rz_kappa{1.57e-8f};   // default of osb_set_rz_kappa (include/openstereo_b200.h)
 float rz_kappa() { return g_rz_kappa.load(std::memory_order_relaxed); }
 
+static std::atomic<int> g_grid_cap{0};            // osb_set_persistent_grid_cap; 0 = no cap
+long long cap_persistent_grid(long long grid) {
+  const int cap = g_grid_cap.load(std::memory_order_relaxed);
+  return (cap > 0 && grid > cap) ? cap : grid;
+}
+
+std::string tc_variant_name(const char* fmt, ...) {
+  char buf[64];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  return buf;
+}
+static thread_local const char* g_tc_variant = "";
+void set_tc_variant(const char* name) { g_tc_variant = name; }
+
 // Sticky fp16-range counter of the tensor-core convolutions (tc_common.cuh): one zero-initialised unsigned int per device,
 // allocated on first use, incremented by every loader thread that staged a value beyond +-65504 / TC_ACT_SCALE.
 static std::atomic<unsigned int*> g_overflow[64];
@@ -122,6 +139,8 @@ float osb_set_rz_kappa(float kappa) {
   if (kappa >= 0.f && kappa < 1e-6f) osb::g_rz_kappa.store(kappa, std::memory_order_relaxed);
   return old;
 }
+int osb_set_persistent_grid_cap(int cap) { return osb::g_grid_cap.exchange(cap > 0 ? cap : 0, std::memory_order_relaxed); }
+const char* osb_tc_last_variant(void) { return osb::g_tc_variant; }
 int osb_tc_overflow_count(osb_stream_t stream, int reset, unsigned int* count) {
   using namespace osb;
   OSB_REQUIRE(count, "tc_overflow_count: null pointer");

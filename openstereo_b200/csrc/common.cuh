@@ -5,6 +5,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <string>
+
 #include "../../include/openstereo_b200.h"
 
 namespace osb {
@@ -15,6 +17,13 @@ void count_launch(int n = 1);
 int check_launch(const char* what);  // cudaGetLastError -> OSB_OK / OSB_ECUDA (+message)
 int device_index();                   // current CUDA device (0 when the query fails)
 int sm_count();                       // multiprocessors of the CURRENT device (cached per device)
+// Grid of a persistent kernel (CTAs walk `for (it = blockIdx.x; it < items; it += gridDim.x)`): `grid` clamped to the cap set by
+// osb_set_persistent_grid_cap, so tests can make one CTA run many work items in a row.
+long long cap_persistent_grid(long long grid);
+// Template arguments of a tensor-core instantiation, spelled as osb_tc_last_variant returns them; each launcher formats its name
+// once (a function-local static) and records it on every launch with set_tc_variant (this thread only; `name` must outlive it).
+std::string tc_variant_name(const char* fmt, ...);
+void set_tc_variant(const char* name);
 // Per-device "already configured" flag: cudaFuncSetAttribute is per device, a process may drive several
 // (DataParallel, model.to('cuda:1')); a plain `static bool` would configure only the first one.
 struct PerDeviceFlag {

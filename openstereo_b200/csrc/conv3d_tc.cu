@@ -484,7 +484,9 @@ static int launch_tc(const TcParams& p, cudaStream_t stream) {
     configured.here() = true;
   }
   const int sms = sm_count();
-  const int grid = p.items < sms ? p.items : sms;   // persistent: one CTA per SM (its shared memory is taken)
+  const int grid = (int)cap_persistent_grid(p.items < sms ? p.items : sms);   // persistent: one CTA per SM (its shared memory is taken)
+  static const std::string variant = tc_variant_name("tc<%d>", COUT);
+  set_tc_variant(variant.c_str());
   kernel<<<grid, TC_THREADS, smem, stream>>>(p);
   count_launch();
   return check_launch("conv3d_tc_kernel");

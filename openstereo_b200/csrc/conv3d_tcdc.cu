@@ -493,7 +493,9 @@ static int launch_tcdc(TcdcParams& p, cudaStream_t stream) {
   OSB_REQUIRE(items < (1ll << 31), "conv3d_tcdc: too many work items");
   p.items = (int)items;
   const int sms = sm_count();
-  const int grid = p.items < sms ? p.items : sms;
+  const int grid = (int)cap_persistent_grid(p.items < sms ? p.items : sms);
+  static const std::string variant = tc_variant_name("tcdc<%d,%d,%d,%d,%d,%d>", COUT, KC, W, TILES, (int)GW, KS);
+  set_tc_variant(variant.c_str());
   kernel<<<grid, C::THREADS, C::SMEM, stream>>>(p);
   count_launch();
   cudaError_t le = cudaGetLastError();

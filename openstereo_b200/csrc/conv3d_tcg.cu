@@ -429,7 +429,9 @@ static int launch_tcg(TcgParams& p, cudaStream_t stream) {
   OSB_REQUIRE(items < (1ll << 31), "conv3d_tcg: too many work items");
   p.items = (int)items;
   const int sms = sm_count();
-  const int grid = p.items < sms ? p.items : sms;
+  const int grid = (int)cap_persistent_grid(p.items < sms ? p.items : sms);
+  static const std::string variant = tc_variant_name("tcg<%d,%d,%d,%d,%d,%d,%d>", COUT, KC, W, TILES, DIL, (int)GW, (int)GATE);
+  set_tc_variant(variant.c_str());
   kernel<<<grid, C::THREADS, C::SMEM, stream>>>(p);
   count_launch();
   cudaError_t le = cudaGetLastError();

@@ -344,6 +344,7 @@ static int launch_volume(const float* ref_g, const float* tgt_g, const float* re
   }
   long long grid = (long long)sm_count() * per_sm;                // persistent: every CTA resident, multiple of the SM count
   if (grid > total) grid = total;
+  grid = cap_persistent_grid(grid);
   kernel<<<(unsigned)grid, 32 * GU, smem, stream>>>(map, p, (int)total);
   count_launch();
   return check_launch("volume_kernel");

@@ -416,6 +416,17 @@ def set_rz_kappa(kappa):
     return float(_lib.lib.osb_set_rz_kappa(float(kappa)))
 
 
+def set_persistent_grid_cap(cap):
+    """Clamp the grid of the persistent kernels (tensor-core convs, volume constructors) to `cap` CTAs, 0 = no cap (include/
+    openstereo_b200.h: osb_set_persistent_grid_cap); returns the previous cap.  Tests only: cap = 1 runs every work item on one CTA."""
+    return int(_lib.lib.osb_set_persistent_grid_cap(int(cap)))
+
+
+def tc_last_variant():
+    """Template arguments of the tensor-core conv instantiation this thread launched last, e.g. "tcg<64,16,64,1,1,0,1>"."""
+    return (_lib.lib.osb_tc_last_variant() or b"").decode()
+
+
 def tc_overflow_count(device=None, reset=False):
     """Number of loader threads (since the last reset) that staged an activation outside the fp16 range of the tensor-core
     convolutions (|x| >= 4094).  Synchronises the current stream of `device`.  0 = every result is valid."""

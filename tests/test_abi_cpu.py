@@ -61,6 +61,20 @@ def test_version_and_error_channel(native):
         native.call("osb_gwc_volume_fwd", None, None, None, 1, 8, 4, 4, 4, 2, None)
 
 
+def test_persistent_grid_cap_and_variant_hooks(native):
+    """Test hooks of the persistent kernels: declared in the header, bound with their C types, host-only state (no device needed)."""
+    from openstereo_b200 import ops
+    names = declared_symbols()
+    assert "osb_set_persistent_grid_cap" in names and "osb_tc_last_variant" in names
+    assert native.lib.osb_set_persistent_grid_cap.argtypes == [ctypes.c_int]
+    assert native.lib.osb_set_persistent_grid_cap.restype is ctypes.c_int
+    assert native.lib.osb_tc_last_variant.restype is ctypes.c_char_p
+    assert ops.set_persistent_grid_cap(3) == 0
+    assert ops.set_persistent_grid_cap(-2) == 3                  # negative = no cap
+    assert ops.set_persistent_grid_cap(0) == 0
+    assert isinstance(ops.tc_last_variant(), str)
+
+
 def test_ops_refuse_cpu_tensors(native):
     from openstereo_b200 import ops
     x = torch.randn(1, 8, 4, 16)

@@ -102,6 +102,30 @@ def test_fused_volume_gwcnet_shape(ops):
     assert_close(out, ocv.gwc_concat_volume(lg, rg, lc, rc, 48, 40), 1e-6, "fused gwcnet")
 
 
+@pytest.mark.timeout(120)
+def test_volume_persistent_grid_cap(ops):
+    """The volume kernel's CTAs walk their items through a two-stage TMA ring (the next item's rows are prefetched while the
+    current one is computed).  With the grid capped to 1 and 3 CTAs every CTA runs many items in a row: gwc, concat and the
+    fused form must be bit-identical to the uncapped launch and within 1e-6 of the oracle."""
+    lg, rg, lc, rc = rnd(9, 2, 40, 3, 72), rnd(10, 2, 40, 3, 72), rnd(11, 2, 6, 3, 72), rnd(12, 2, 6, 3, 72)
+    cases = [
+        ("gwc", lambda: ops.build_gwc_volume(dev(lg), dev(rg), 20, 8), ocv.build_gwc_volume(lg, rg, 20, 8)),
+        ("concat", lambda: ops.build_concat_volume(dev(lc), dev(rc), 20), ocv.build_concat_volume(lc, rc, 20)),
+        ("fused", lambda: ops.gwc_concat_volume(dev(lg), dev(rg), dev(lc), dev(rc), 20, 8), ocv.gwc_concat_volume(lg, rg, lc, rc, 20, 8)),
+    ]
+    try:
+        for name, run, want in cases:
+            ops.set_persistent_grid_cap(0)
+            free = run().cpu()
+            for cap in (1, 3):
+                ops.set_persistent_grid_cap(cap)
+                got = run().cpu()
+                assert torch.equal(got, free), "%s volume at grid cap %d differs from the uncapped launch" % (name, cap)
+                assert_close(got, want, 1e-6, "%s volume at grid cap %d" % (name, cap))
+    finally:
+        ops.set_persistent_grid_cap(0)
+
+
 def test_volume_properties_full_size(ops):
     """Config-2 size (B=8, C=320, G=40, 64x128, D'=48): size-independent properties instead of a CPU oracle run.
     (1) linearity in the left feature; (2) the d=0 slice equals the plain group mean of l*r; (3) zero triangle;

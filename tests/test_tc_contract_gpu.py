@@ -1,0 +1,497 @@
+"""GPU: contract of every tensor-core convolution instantiation (csrc/conv3d_tc.cu, conv3d_tcg.cu, conv3d_tcs2.cu, conv3d_tcdc.cu).
+
+REGISTRY has one row per dispatcher branch (tests/test_host_logic_cpu.py checks that every launch_tc*<...> template list in csrc/
+has a row).  Each row names the C entry point, the channels, a small input shape with a partial row block (general-width rows: a
+last column tile holding a single valid column) and the instantiation the dispatcher must pick.  For every row:
+  routing      osb_tc_last_variant() names the row's instantiation;
+  item loop    the persistent CTAs walk their work items with state carried from item to item (ring and weight-buffer mbarrier
+               phases, the seam-exchange double buffer): outputs at grid caps 1 and 7, without a cap and again without a cap are
+               bit-identical -- an item's result does not depend on the CTA that computes it or on what that CTA ran before;
+  accuracy     weights scaled per output channel by 2^k (k over [-12, 12]) times a non-power-of-two factor, folded BN, residual,
+               activation and gate where the entry point has them, against an fp64 reference: error per output channel
+               <= 1e-5 x that channel's max |want| (so a fault in one small channel cannot hide behind a large one);
+  bounds       the output lives inside a buffer whose output region starts as NaN, guarded on each side by 4 KB of sentinels;
+               every output element is written and no sentinel changes (channel slices: nor do channels outside the slice);
+  range guard  activations within +-4090 spanning 1e-6 .. 1e3 across columns: no overflow report and per-column accuracy; one
+               +-5000 at an edge / column-tile seam in the last K chunk of the last plane: the overflow counter reports it and the
+               output stays finite;
+  kappa . n    with kappa = 9e-7 the ratio y(kappa) / y(0) - 1 recovers the MMA count n each epilogue applied; it must equal the n
+               counted here from the convolution geometry: (kd, kh) tap rows issued x Cin / 16 k-steps x 3 split products.
+"""
+import math
+import zlib
+from collections import namedtuple
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+pytestmark = pytest.mark.gpu
+
+ACT_NONE, ACT_RELU, ACT_LEAKY = 0, 1, 2
+GUARD = 1024                            # sentinel floats on each side of an output region (4 KB, keeps 16-byte alignment)
+SENTINEL = -1234.5
+KAPPA_TEST = 9e-7
+
+# kind: s1 = Conv3d k3 s1 p1 (s1n: same with an NCDHW input), 2d2 = Conv2d k3 dilation 2 (a one-plane volume), s2 = Conv3d k3 s2 p1,
+# dc3 / dc4 = ConvTranspose3d k3 s2 p1 op1 / k4 s2 p1.  cout = packed channels; shape = INPUT (B, D, H, W); ys / coff = channel
+# stride and first channel of a channel slice (0: the output is the whole tensor); creal < cout: zero-padded channel plan whose
+# NCDHW output holds only the real channels; gate: FeatureAtt gate operand.
+Row = namedtuple("Row", "id kind cin cout shape variant ys coff creal gate")
+
+
+def R(rid, kind, cin, cout, shape, variant, ys=0, coff=0, creal=None, gate=False):
+    return Row(rid, kind, cin, cout, shape, variant, ys, coff, cout if creal is None else creal, gate)
+
+
+REGISTRY = [
+    # conv3d_tc.cu, W = 128, 32-channel K chunks: one row per loader path of tc<32> (bulk-copied rows, register-staged rows, NCDHW)
+    R("tc32-bulk", "s1", 32, 32, (1, 3, 5, 128), "tc<32>"),
+    R("tc32-regs", "s1", 64, 32, (1, 3, 5, 128), "tc<32>"),
+    R("tc32-ncdhw-in", "s1n", 32, 32, (1, 3, 5, 128), "tc<32>"),
+    R("tc16-head", "s1", 32, 16, (2, 3, 4, 128), "tc<16>", creal=3),
+    # conv3d_tcg.cu whole-row tiles (R = 128 / W image rows per tile)
+    R("tcg64-w64-gate", "s1", 32, 64, (1, 3, 5, 64), "tcg<64,16,64,1,1,0,1>", gate=True),
+    R("tcg96-w32-gate", "s1", 32, 96, (1, 2, 7, 32), "tcg<96,16,32,1,1,0,1>", gate=True),
+    R("tcg64-w64", "s1", 32, 64, (1, 3, 5, 64), "tcg<64,16,64,1,1,0,0>"),
+    R("tcg64-w32", "s1", 48, 64, (1, 3, 7, 32), "tcg<64,16,32,1,1,0,0>"),
+    R("tcg128-w32", "s1", 32, 128, (1, 2, 7, 32), "tcg<128,16,32,1,1,0,0>"),
+    R("tcg96-w32", "s1", 32, 96, (1, 2, 7, 32), "tcg<96,16,32,1,1,0,0>"),
+    R("tcg96-w16-slice", "s1", 32, 96, (1, 2, 11, 16), "tcg<96,16,16,1,1,0,1>", ys=160, coff=0, gate=True),
+    R("tcg64-w16-slice", "s1", 32, 64, (1, 2, 11, 16), "tcg<64,16,16,1,1,0,1>", ys=160, coff=96),
+    R("tcg64-w128", "s1", 32, 64, (1, 2, 3, 128), "tcg<64,16,128,1,1,0,0>"),
+    R("tcg128-w128", "s1", 32, 128, (1, 2, 3, 128), "tcg<128,16,128,1,1,0,0>"),
+    R("tcg32-gw", "s1", 32, 32, (1, 2, 3, 127), "tcg<32,16,128,1,1,1,0>"),
+    R("tcg64-gw", "s1", 16, 64, (1, 2, 3, 127), "tcg<64,16,128,1,1,1,0>"),
+    R("tcg128-gw", "s1", 16, 128, (1, 2, 3, 127), "tcg<128,16,128,1,1,1,0>"),
+    R("tcg128-dil2", "2d2", 32, 128, (2, 1, 5, 128), "tcg<128,16,128,1,2,0,0>"),
+    # conv3d_tcs2.cu (output width W / 2)
+    R("tcs2-96-w16-slice", "s2", 32, 96, (1, 4, 10, 32), "tcs2<96,16,16,1,0>", ys=160, coff=64),
+    R("tcs2-64-w16-slice", "s2", 32, 64, (1, 4, 10, 32), "tcs2<64,16,16,1,0>", ys=160, coff=0),
+    R("tcs2-64-w64", "s2", 32, 64, (1, 4, 6, 128), "tcs2<64,16,64,1,0>"),
+    R("tcs2-64-w32", "s2", 32, 64, (1, 4, 10, 64), "tcs2<64,16,32,1,0>"),
+    R("tcs2-128-w32", "s2", 32, 128, (1, 4, 10, 64), "tcs2<128,16,32,1,0>"),
+    R("tcs2-96-w32", "s2", 32, 96, (1, 4, 10, 64), "tcs2<96,16,32,1,0>"),
+    R("tcs2-64-gw", "s2", 16, 64, (1, 4, 4, 256), "tcs2<64,16,128,1,1>"),
+    R("tcs2-128-gw", "s2", 16, 128, (1, 2, 4, 256), "tcs2<128,16,128,1,1>"),
+    # conv3d_tcdc.cu (output 2D x 2H x 2W)
+    R("tcdc4-64-w16-slice", "dc4", 32, 64, (1, 2, 11, 16), "tcdc<64,16,16,1,0,4>", ys=96, coff=32),
+    R("tcdc4-32-w16-slice", "dc4", 32, 32, (1, 2, 11, 16), "tcdc<32,16,16,1,0,4>", ys=96, coff=0),
+    R("tcdc4-64-w32", "dc4", 32, 64, (1, 2, 5, 32), "tcdc<64,16,32,1,0,4>"),
+    R("tcdc4-32-w64-narrow", "dc4", 32, 32, (1, 2, 3, 64), "tcdc<32,16,64,1,0,4>", creal=24),
+    R("tcdc3-64-w32", "dc3", 32, 64, (1, 2, 5, 32), "tcdc<64,16,32,1,0,3>"),
+    R("tcdc3-32-w64", "dc3", 32, 32, (1, 2, 3, 64), "tcdc<32,16,64,1,0,3>"),
+    R("tcdc3-64-gw", "dc3", 16, 64, (1, 2, 2, 128), "tcdc<64,16,128,1,1,3>"),
+    R("tcdc3-32-gw", "dc3", 16, 32, (1, 2, 2, 128), "tcdc<32,16,128,1,1,3>"),
+]
+
+
+@pytest.fixture(scope="module")
+def osb():
+    import __graft_entry__
+    __graft_entry__.build()
+    from openstereo_b200 import _lib, ops
+    return _lib, ops
+
+
+def gen(seed):
+    return torch.Generator().manual_seed(seed)
+
+
+def out_spatial(row):
+    _, d, h, w = row.shape
+    if row.kind == "s2":
+        return d // 2, h // 2, w // 2
+    if row.kind in ("dc3", "dc4"):
+        return 2 * d, 2 * h, 2 * w
+    return d, h, w
+
+
+def layouts(row):
+    """Output layouts the row's entry point accepts (1 = channels-last)."""
+    if row.ys or row.gate:
+        return (1,)
+    if row.creal < row.cout:
+        return (0,)
+    return (0, 1)
+
+
+def has_residual(row):
+    return not (row.ys and row.kind in ("s2", "dc4"))        # the stride-2 and k4 slice entry points take no residual
+
+
+def ksize(row):
+    return 4 if row.kind == "dc4" else 3
+
+
+def make_weight(row, g, chan_scale=None):
+    """fp32 weight in the layer's parameter layout (conv: (Cout, Cin, k, k, k); transposed: (Cin, Cout, k, k, k)); channels >= creal
+    zero (a zero-padded plan); 2d2: only the kd = 1 taps are non-zero."""
+    k = ksize(row)
+    fan = row.cin * (9 if row.kind == "2d2" else k ** 3)
+    scale = torch.ones(row.cout) if chan_scale is None else chan_scale
+    scale = scale.clone()
+    scale[row.creal:] = 0
+    if row.kind in ("dc3", "dc4"):
+        w = torch.randn(row.cin, row.cout, k, k, k, generator=g) * fan ** -0.5 * scale.view(1, -1, 1, 1, 1)
+    else:
+        w = torch.randn(row.cout, row.cin, k, k, k, generator=g) * fan ** -0.5 * scale.view(-1, 1, 1, 1, 1)
+    if row.kind == "2d2":
+        w[:, :, 0] = 0
+        w[:, :, 2] = 0
+    return w
+
+
+def pack(ops, row, w):
+    dw = w.cuda()
+    if row.kind in ("s1", "s1n"):
+        kc = ops.conv3d_tc_kc(row.cin, row.creal, row.shape[3])
+        if row.creal < row.cout:
+            return ops.pack_tc_weight(dw[:row.creal], kc, pad_cout_to=row.cout), kc
+        return ops.pack_tc_weight(dw, kc), kc
+    if row.kind == "2d2":
+        return ops.pack_tc_weight(dw, 16), 16
+    if row.kind == "s2":
+        return ops.pack_tc_weight(dw, 16, kw_order=(1, 0, 2)), 16
+    return ops.pack_tc_deconv_weight(dw), 16
+
+
+def reference(row, x, w):
+    """fp64 convolution of the row's operator: x (B, Cin, D, H, W) -> (B, Cout, Do, Ho, Wo)."""
+    x, w = x.double(), w.double()
+    if row.kind in ("s1", "s1n"):
+        return F.conv3d(x, w, padding=1)
+    if row.kind == "2d2":
+        return F.conv2d(x[:, :, 0], w[:, :, 1], padding=2, dilation=2).unsqueeze(2)
+    if row.kind == "s2":
+        return F.conv3d(x, w, stride=2, padding=1)
+    return F.conv_transpose3d(x, w, stride=2, padding=1, output_padding=1 if row.kind == "dc3" else 0)
+
+
+def epilogue(conv, sc, sh, res, gate, act):
+    """fp64 folded BN + residual + activation + gate on an NCDHW tensor; gate (B, Ho, Wo, C) channels-last."""
+    y = conv
+    if sc is not None:
+        y = y * sc.double().view(1, -1, 1, 1, 1)
+    if sh is not None:
+        y = y + sh.double().view(1, -1, 1, 1, 1)
+    if res is not None:
+        y = y + res.double()
+    if act == ACT_RELU:
+        y = F.relu(y)
+    elif act == ACT_LEAKY:
+        y = F.leaky_relu(y, 0.01)
+    if gate is not None:
+        y = y * gate.double().permute(0, 3, 1, 2).unsqueeze(2)
+    return y
+
+
+class Launch:
+    """The operands of one row in device memory and a direct call of its C entry point with a caller-chosen output address."""
+
+    def __init__(self, osb, row, x, w, sc=None, sh=None, res=None, gate=None, act=ACT_NONE, out_ndhwc=1):
+        self.lib, ops = osb
+        self.row, self.act, self.out_ndhwc = row, act, out_ndhwc
+        b, d, h, wd = row.shape
+        self.spatial = out_spatial(row)
+        self.ctot = row.ys or row.cout                           # channels per voxel of the channels-last tensors
+        wp, kc = pack(ops, row, w)
+        self.wp = wp
+        self.wptr, self.eff = ops._tc_args(wp, row.cin, kc, None if sc is None else sc.cuda())
+        self.sh = None if sh is None else sh.cuda()
+        xin = x if row.kind == "s1n" else x.permute(0, 2, 3, 4, 1)
+        self.x = xin.contiguous().cuda()
+        self.res = self.res_ptr = None
+        if res is not None:                                      # NCDHW (B, creal, ...) -> the output's layout
+            self.res = self._to_layout(res)
+            self.res_ptr = self.res.data_ptr() + 4 * (row.coff if out_ndhwc else 0)
+        self.gate = self.gate_ptr = None
+        if gate is not None:                                     # (B, Ho, Wo, cout) -> (B, Ho, Wo, ctot), slice channels at coff
+            full = torch.zeros(b, self.spatial[1], self.spatial[2], self.ctot)
+            full[..., row.coff:row.coff + row.cout] = gate
+            self.gate = full.cuda()
+            self.gate_ptr = self.gate.data_ptr() + 4 * row.coff
+
+    def _to_layout(self, t):
+        row = self.row
+        if not self.out_ndhwc:
+            return t[:, :row.creal].contiguous().cuda()
+        full = torch.zeros(t.shape[0], *self.spatial, self.ctot)
+        full[..., row.coff:row.coff + row.cout] = t.permute(0, 2, 3, 4, 1)
+        return full.cuda()
+
+    def numel(self):
+        b = self.row.shape[0]
+        n = b * math.prod(self.spatial)
+        return n * (self.ctot if self.out_ndhwc else self.row.creal)
+
+    def guarded(self):
+        """Fresh output buffer: sentinels | output region (NaN where this launch must write, sentinels elsewhere) | sentinels."""
+        buf = torch.full((GUARD + self.numel() + GUARD,), SENTINEL, device="cuda")
+        self.inner(buf).copy_(torch.where(self.written_mask(), torch.tensor(float("nan"), device="cuda"),
+                                          torch.tensor(SENTINEL, device="cuda")))
+        return buf
+
+    def inner(self, buf):
+        return buf[GUARD:GUARD + self.numel()]
+
+    def written_mask(self):
+        m = torch.ones(self.numel(), dtype=torch.bool, device="cuda")
+        if self.out_ndhwc and self.ctot != self.row.cout:
+            m = m.view(-1, self.ctot)
+            m[:, :self.row.coff] = False
+            m[:, self.row.coff + self.row.cout:] = False
+        return m.view(-1)
+
+    def run(self, buf):
+        row, s = self.row, torch.cuda.current_stream().cuda_stream
+        b, d, h, w = row.shape
+        yp = buf.data_ptr() + 4 * (GUARD + (row.coff if self.out_ndhwc else 0))
+        x, wp, sc, sh = self.x.data_ptr(), self.wptr, self.eff.data_ptr(), None if self.sh is None else self.sh.data_ptr()
+        o, act, call = self.out_ndhwc, self.act, self.lib.call
+        if row.ys and row.kind == "s1":
+            call("osb_conv3d_k3_tc_cs_fwd", x, wp, sc, sh, self.res_ptr, self.gate_ptr, yp, b, row.cin, row.cout, d, h, w, act, row.ys, s)
+        elif row.ys and row.kind == "s2":
+            call("osb_conv3d_k3_s2_tc_cs_fwd", x, wp, sc, sh, yp, b, row.cin, row.cout, d, h, w, act, row.ys, s)
+        elif row.ys:
+            call("osb_deconv3d_k4_tc_cs_fwd", x, wp, sc, sh, yp, b, row.cin, row.cout, d, h, w, act, row.ys, s)
+        elif row.gate:
+            call("osb_conv3d_k3_tc_gate_fwd", x, wp, sc, sh, self.res_ptr, self.gate_ptr, yp, b, row.cin, row.cout, d, h, w, act, s)
+        elif row.kind in ("s1", "s1n"):
+            call("osb_conv3d_k3_tc_ncdhw_fwd" if row.kind == "s1n" else "osb_conv3d_k3_tc_fwd", x, wp, sc, sh, self.res_ptr, yp, b,
+                 row.cin, row.creal, d, h, w, act, o, o, s)
+        elif row.kind == "2d2":
+            call("osb_conv2d_k3_tc_fwd", x, wp, sc, sh, self.res_ptr, yp, b, row.cin, row.cout, h, w, 2, act, o, o, s)
+        elif row.kind == "s2":
+            call("osb_conv3d_k3_s2_tc_fwd", x, wp, sc, sh, self.res_ptr, yp, b, row.cin, row.cout, d, h, w, act, o, o, s)
+        elif row.kind == "dc3":
+            call("osb_deconv3d_k3_tc_fwd", x, wp, sc, sh, self.res_ptr, yp, b, row.cin, row.cout, d, h, w, act, o, o, s)
+        else:
+            call("osb_deconv3d_k4_tc_fwd", x, wp, sc, sh, self.res_ptr, yp, b, row.cin, row.cout, row.creal, d, h, w, act, o, o, s)
+
+    def output(self, buf):
+        """-> the launch's result as NCDHW (B, creal, Do, Ho, Wo) on the CPU."""
+        row, b = self.row, self.row.shape[0]
+        y = self.inner(buf)
+        if self.out_ndhwc:
+            y = y.view(b, *self.spatial, self.ctot)[..., row.coff:row.coff + row.cout].permute(0, 4, 1, 2, 3)
+        else:
+            y = y.view(b, row.creal, *self.spatial)
+        return y.cpu()
+
+    def check_bounds(self, buf, what):
+        bits = buf.view(torch.int32)
+        sent = torch.tensor([SENTINEL]).view(torch.int32).item()
+        assert (bits[:GUARD] == sent).all() and (bits[-GUARD:] == sent).all(), "%s: a store left the output region" % what
+        inner, m = self.inner(buf), self.written_mask()
+        assert not torch.isnan(inner[m]).any(), "%s: %d output elements never written" % (what, int(torch.isnan(inner[m]).sum()))
+        assert (self.inner(bits)[~m] == sent).all(), "%s: a store touched a channel outside the slice" % what
+
+
+def per_channel_close(got, want, creal, tol, what):
+    got, want = got[:, :creal].double(), want[:, :creal]
+    err = (got - want).abs().amax(dim=(0, 2, 3, 4))
+    scale = want.abs().amax(dim=(0, 2, 3, 4))
+    bad = (err > tol * scale).nonzero().flatten().tolist()
+    assert not bad, "%s: channels %s exceed %g of their own max (err/max %s)" % (
+        what, bad[:8], tol, [float(err[c] / scale[c].clamp(min=1e-300)) for c in bad[:8]])
+
+
+def channel_scales(cout, g):
+    """2^k x a non-power-of-two factor per output channel, k spread over [-12, 12]."""
+    k = torch.linspace(-12, 12, cout).round()[torch.randperm(cout, generator=g)]
+    return torch.ldexp(torch.ones(cout), k.int()) * (1.0 + 0.9 * torch.rand(cout, generator=g)) * 0.77
+
+
+@pytest.fixture
+def grid_cap(osb):
+    _, ops = osb
+    yield ops.set_persistent_grid_cap
+    ops.set_persistent_grid_cap(0)
+
+
+@pytest.mark.timeout(120)
+@pytest.mark.parametrize("row", REGISTRY, ids=[r.id for r in REGISTRY])
+def test_routing_item_loop_accuracy_and_bounds(osb, grid_cap, row):
+    _, ops = osb
+    g = gen(zlib.crc32(row.id.encode()) % 10000)
+    b, d, h, w = row.shape
+    x = torch.randn(b, row.cin, d, h, w, generator=g)
+    cs = channel_scales(row.cout, g)
+    wt = make_weight(row, g, cs)
+    sc = torch.rand(row.cout, generator=g) + 0.5
+    sh = 0.1 * cs * torch.randn(row.cout, generator=g)
+    conv = reference(row, x, wt)
+    res = 0.3 * cs.view(1, -1, 1, 1, 1) * torch.randn(conv.shape, generator=g) if has_residual(row) else None
+    do, ho, wo = out_spatial(row)
+    gate = torch.sigmoid(torch.randn(b, ho, wo, row.cout, generator=g)) if row.gate else None
+    act = ACT_RELU if len(row.id) % 2 else ACT_LEAKY
+    want = epilogue(conv, sc, sh, res, gate, act)
+    for o in layouts(row):
+        what = "%s %s" % (row.id, "ndhwc" if o else "ncdhw")
+        L = Launch(osb, row, x, wt, sc, sh, res, gate, act, o)
+        outs = []
+        for cap in (1, 7, 0, 0):
+            grid_cap(cap)
+            buf = L.guarded()
+            L.run(buf)
+            torch.cuda.synchronize()
+            assert ops.tc_last_variant() == row.variant, "%s routed to %s" % (what, ops.tc_last_variant())
+            L.check_bounds(buf, "%s cap %d" % (what, cap))
+            outs.append(L.inner(buf).view(torch.int32).clone())
+            if cap == 1:
+                per_channel_close(L.output(buf), want, row.creal, 1e-5, what)
+        for cap, o_ in zip((7, 0, 0), outs[1:]):
+            assert torch.equal(outs[0], o_), "%s: output at grid cap %d differs from the one-CTA run" % (what, cap)
+
+
+@pytest.mark.timeout(120)
+@pytest.mark.parametrize("row", REGISTRY, ids=[r.id for r in REGISTRY])
+def test_fp16_range_guard(osb, row):
+    _, ops = osb
+    g = gen(7 + zlib.crc32(row.id.encode()) % 10000)
+    b, d, h, w = row.shape
+    x = torch.randn(b, row.cin, d, h, w, generator=g) * torch.logspace(-6, 3, w).view(1, 1, 1, 1, w)
+    x = x.clamp(-4090, 4090)
+    wt = make_weight(row, g)
+    want = reference(row, x, wt)
+    gate = torch.ones(b, *out_spatial(row)[1:], row.cout) if row.gate else None
+    o = layouts(row)[0]
+    ops.tc_overflow_count(reset=True)
+    L = Launch(osb, row, x, wt, gate=gate, out_ndhwc=o)
+    buf = L.guarded()
+    L.run(buf)
+    assert ops.tc_overflow_count() == 0, "%s: in-range activations reported as overflow" % row.id
+    got = L.output(buf).double()[:, :row.creal]
+    want = want[:, :row.creal]
+    # |x| below 2^-7 is staged with an ABSOLUTE error of 2^-29 (csrc/tc_common.cuh): at most 2^-29 * sum |w| per output
+    wsum = wt.abs().sum(dim=(1, 2, 3, 4) if row.kind not in ("dc3", "dc4") else (0, 2, 3, 4)).max().item()
+    err = (got - want).abs().amax(dim=(0, 1, 2, 3))
+    col_scale = want.abs().amax(dim=(0, 1, 2, 3))
+    bad = (err > 2e-5 * col_scale + 2.0 ** -27 * wsum).nonzero().flatten().tolist()
+    assert not bad, "%s: output columns %s off (err %s, scale %s)" % (row.id, bad[:8], err[bad[:8]].tolist(), col_scale[bad[:8]].tolist())
+    for value, col in ((5000.0, w - 1), (-5000.0, 0)):          # last K chunk, last plane; an image edge / column-tile seam
+        xo = x.clone()
+        xo[b - 1, row.cin - 1, d - 1, h // 2, col] = value
+        L = Launch(osb, row, xo, wt, gate=gate, out_ndhwc=o)
+        buf = L.guarded()
+        L.run(buf)
+        n = ops.tc_overflow_count(reset=True)
+        assert n >= 1, "%s: %g at column %d not reported" % (row.id, value, col)
+        assert torch.isfinite(L.inner(buf)[L.written_mask()]).all(), "%s: saturated operands must keep the output finite" % row.id
+    assert ops.tc_overflow_count() == 0
+
+
+def expected_mma_count(row):
+    """-> {(output plane, output row parity or None): MMAs each accumulator received}, from the convolution geometry alone:
+    (kd, kh) tap rows issued x Cin/16 k-steps x 3 split products.  Rows outside the image are issued as zero operands (they count);
+    planes outside the volume are skipped (they do not)."""
+    _, d, h, w = row.shape
+    steps = row.cin // 16 * 3
+    out = {}
+    if row.kind in ("s1", "s1n", "2d2", "s2"):
+        st = 2 if row.kind == "s2" else 1
+        for od in range(out_spatial(row)[0]):
+            planes = sum(1 for kd in range(3) if 0 <= st * od + kd - 1 < d)
+            out[(od, None)] = planes * 3 * steps
+        return out
+    k = ksize(row)
+    for od in range(2 * d):
+        planes = sum(1 for kd in range(k) if (od + 1 - kd) % 2 == 0 and 0 <= (od + 1 - kd) // 2 < d)
+        for ph in (0, 1):
+            rows = sum(1 for kh in range(k) if (ph + 1 - kh) % 2 == 0)
+            out[(od, ph)] = planes * rows * steps
+    return out
+
+
+@pytest.mark.timeout(120)
+@pytest.mark.parametrize("row", REGISTRY, ids=[r.id for r in REGISTRY])
+def test_kappa_mma_count(osb, row):
+    _, ops = osb
+    g = gen(11 + zlib.crc32(row.id.encode()) % 10000)
+    b, d, h, w = row.shape
+    x = torch.randn(b, row.cin, d, h, w, generator=g)
+    wt = make_weight(row, g)
+    gate = torch.ones(b, *out_spatial(row)[1:], row.cout) if row.gate else None
+    L = Launch(osb, row, x, wt, gate=gate, out_ndhwc=layouts(row)[0])
+    ys = []
+    old = ops.set_rz_kappa(0.0)
+    try:
+        for kappa in (0.0, KAPPA_TEST):
+            ops.set_rz_kappa(kappa)
+            buf = L.guarded()
+            L.run(buf)
+            ys.append(L.output(buf).double()[:, :row.creal])
+    finally:
+        ops.set_rz_kappa(old)
+    y0, y1 = ys
+    n_est = ((y1 / y0.where(y0 != 0, torch.ones_like(y0)) - 1) / KAPPA_TEST).round()
+    for (od, ph), n in expected_mma_count(row).items():
+        sel = (slice(None), slice(None), od) + ((slice(None),) if ph is None else (slice(ph, None, 2),))
+        a, e = y0[sel].abs().flatten(), n_est[sel].flatten()
+        big = a > a.median()
+        got = e[big].median().item()
+        assert got == n, "%s: output plane %d%s applied kappa * %d, the geometry gives %d MMAs" % (
+            row.id, od, "" if ph is None else " row parity %d" % ph, got, n)
+
+
+# ------------------------------------------------------------------------------------------------ rounding bias against fp64
+# The layer shapes of tools/parity_bisect.py --layers: post-ReLU (non-negative) inputs, fan-in scaled weights, >= 1e5 outputs each.
+# g = least-squares gain of the output against fp64 (y ~ (1 + g) * want).  Without the correction (kappa = 0) the truncating
+# accumulation leaves a coherent negative g; with the default kappa it must shrink to a quarter of that or below the floor, 2^-24
+# (half an fp32 ulp: a multiplicative correction rounded to fp32 cannot resolve less).  Measured on an H100 80GB HBM3 at 400 W
+# (DESIGN.md section 2.1): g(0) from -2.7e-7 to -3.2e-6, g(default) within +-1.2e-7 on interior rows.  Border rows (h = 0, H-1)
+# receive kh MMAs on zero operands, which cannot truncate, so the issued-MMA count over-corrects them by about kappa * n / 3; their
+# g is printed for the record, not asserted.
+BIAS_LAYERS = [
+    ("stem 64->32 W128", "s1", 64, 32, (1, 6, 20, 128)), ("stem 32->32 W128", "s1", 32, 32, (1, 6, 20, 128)),
+    ("conv2 64->64 W64", "s1", 64, 64, (1, 6, 16, 64)), ("conv4 128->128 W32", "s1", 128, 128, (1, 6, 16, 32)),
+    ("conv1 s2 32->64", "s2", 32, 64, (1, 8, 16, 128)), ("conv3 s2 64->128", "s2", 64, 128, (1, 8, 16, 64)),
+    ("conv5 dc 128->64", "dc3", 128, 64, (1, 4, 8, 32)), ("conv6 dc 64->32", "dc3", 64, 32, (1, 4, 10, 64)),
+    ("2d 64->64 W128", "s1", 64, 64, (1, 1, 64, 128)), ("2d 128->128 W128", "s1", 128, 128, (1, 1, 64, 128)),
+    ("2d dil2 128->128", "2d2", 128, 128, (1, 1, 64, 128)), ("2d 32->32 W128", "s1", 32, 32, (1, 1, 128, 128)),
+]
+BIAS_FLOOR = 2.0 ** -24
+
+
+def gain(got, want):
+    got, want = got.double().flatten(), want.double().flatten()
+    return ((got * want).sum() / (want * want).sum()).item() - 1.0
+
+
+@pytest.mark.timeout(180)
+def test_rounding_bias_vs_fp64(osb):
+    _, ops = osb
+    g = gen(5)
+    lines, fails = [], []
+    default = ops.set_rz_kappa(0.0)
+    ops.set_rz_kappa(default)
+    try:
+        for name, kind, cin, cout, shape in BIAS_LAYERS:
+            row = R(name, kind, cin, cout, shape, "")
+            b, d, h, w = shape
+            x = torch.randn(b, cin, d, h, w, generator=g).abs()
+            wt = make_weight(row, g)
+            want = reference(row, x.cuda(), wt.cuda()).cpu()
+            assert want.numel() >= 100000
+            L = Launch(osb, row, x, wt, out_ndhwc=0)
+            gains = []
+            for kappa in (0.0, default):
+                ops.set_rz_kappa(kappa)
+                buf = L.guarded()
+                L.run(buf)
+                y = L.output(buf)
+                ho = y.shape[3]
+                inner = slice(1, ho - 1)
+                border = [0, ho - 1]
+                gains.append((gain(y, want), gain(y[:, :, :, inner], want[:, :, :, inner]),
+                              gain(y[:, :, :, border], want[:, :, :, border])))
+            (g0, g0i, g0b), (gd, gdi, gdb) = gains
+            lines.append("%-20s g(0) %+.2e (interior %+.2e, border rows %+.2e)   g(%.3g) %+.2e (interior %+.2e, border rows %+.2e)" % (
+                name, g0, g0i, g0b, default, gd, gdi, gdb))
+            if abs(gd) > max(0.25 * abs(g0), BIAS_FLOOR):
+                fails.append(name)
+    finally:
+        ops.set_rz_kappa(default)
+    print("\n" + "\n".join(lines))
+    assert not fails, "rounding bias not corrected: %s\n%s" % (fails, "\n".join(lines))
