@@ -115,6 +115,13 @@ int osb_softargmin_fwd(const float* cost, float* out, int B, int D, int H, int W
 int osb_upsample_softargmin_fwd(const float* cost, float* out, int B, int Dl, int Hl, int Wl, int D,
                                 int H, int W, int align_corners, osb_stream_t stream);
 
+/* osb_upsample_softargmin_fwd with per-pixel hypothesis values: the expectation is sum_d p[b,d,h,w] * values[b,d,h,w]
+ * instead of sum_d p * d.  CasStereo's CostAggregation eval tail (casnet/cas_psm.py:268-274, cas_gwc.py:245-251):
+ * F.upsample(cost3, [D,H,W], 'trilinear', align_corners) -> softmax(dim=1) -> disparity_regression(p, values).
+ * cost: (B,1,Dl,Hl,Wl), values: (B,D,H,W) -> out: (B,H,W). */
+int osb_upsample_softargmin_values_fwd(const float* cost, const float* values, float* out, int B, int Dl, int Hl, int Wl,
+                                       int D, int H, int W, int align_corners, osb_stream_t stream);
+
 /* epe_metric partial sums   stereo/evaluation/metric_per_image.py:32-41 with the eval mask of
  * trainer_template.py:288 (0 < gt < maxdisp).  out: (B,2) = {sum |pred-gt| over valid, #valid}. */
 int osb_epe_partial_fwd(const float* pred, const float* gt, float* out, int B, int HW, float maxdisp,
@@ -253,6 +260,21 @@ int osb_gwc_volume_sum_fwd(const float* ref, const float* tgt, float* out, int B
 int osb_group_l2_normalize_fwd(const float* x, float* y, int B, int C, int H, int W, int G, float eps, osb_stream_t stream);
 int osb_sub_volume_fwd(const float* left, const float* right, float* out, int B, int C, int H, int W, int D, osb_stream_t stream);
 int osb_regression_values_fwd(const float* prob, const float* values, float* out, int B, int D, int H, int W, osb_stream_t stream);
+
+/* ---- CasStereo warped cost volumes (casnet/cas_psm.py:286-318, casnet/cas_gwc.py:263-329) --------------------------------
+ * The right features are sampled at fractional per-pixel hypotheses disp (B,D,H,W) exactly like
+ *   F.grid_sample(y, ((w - disp)/((W-1)/2) - 1, h/((H-1)/2) - 1), 'bilinear', padding_mode='zeros', align_corners=True)
+ * (coordinate round trip replayed in fp32); disp may be fractional, negative or beyond either edge.  H >= 2, W >= 2.
+ * osb_warped_concat_volume_fwd: CasPSMNet's GetCostVolume: x, y (B,C,H,W) -> out (B,2C,D,H,W) = [x repeated over D | warped y];
+ *   mask_left = 1 zeroes the left copy where w < disp (CasGwcNet's concatenation half).
+ * osb_warped_gwc_concat_volume_fwd: CasGwcNet's GetCostVolume: out (B, G + 2*Cc, D, H, W) =
+ *   [mean over each group's Cg/G channels of x_warped * y_warped | x_warped | y_warped], x_warped = 0 where w < disp;
+ *   Cg % G == 0, Cg/G <= 16.
+ * One launch each, every output element written once (no memset). */
+int osb_warped_concat_volume_fwd(const float* x, const float* y, const float* disp, float* out, int B, int C, int D, int H, int W,
+                                 int mask_left, osb_stream_t stream);
+int osb_warped_gwc_concat_volume_fwd(const float* xg, const float* yg, const float* xc, const float* yc, const float* disp,
+                                     float* out, int B, int Cg, int G, int Cc, int D, int H, int W, osb_stream_t stream);
 
 /* Backward (adjoint) kernels so the volume constructors and the soft-argmin stay differentiable under tools/train.py
  * (openstereo_b200/autograd.py wraps them in torch.autograd.Function).  grad_ref / grad_tgt may be NULL when not needed.

@@ -61,6 +61,9 @@ SIGNATURES = {
     "osb_softargmin_bwd": [_f32p] * 3 + [_i] * 4 + [_f, _f, _f, _i, _s],
     "osb_dwconv2d_fwd": [_f32p] * 6 + [_i] * 8 + [_s],
     "osb_deconv2d_k3s2_fwd": [_f32p] * 6 + [_i] * 6 + [_s],
+    "osb_upsample_softargmin_values_fwd": [_f32p] * 3 + [_i] * 8 + [_s],
+    "osb_warped_concat_volume_fwd": [_f32p] * 4 + [_i] * 6 + [_s],
+    "osb_warped_gwc_concat_volume_fwd": [_f32p] * 6 + [_i] * 7 + [_s],
 }
 
 

@@ -9,6 +9,7 @@ checkpoints and YAML configs keep working (SURVEY.md section 8b).
 
 Graphs restated (file:line of the reference forward each engine replaces):
   GwcAggregation        gwcnet/gwcnet_disp_processor.py:83-91,128-140 + gwcnet/hourglass.py:46-56
+  CascadeAggregation    casnet/cas_psm.py:233-279 (CostAggregation, eval) + cas_psm.py:33-43
   PSMAggregation        psmnet/psmnet_cost_processor.py:181-221,108-132 + psmnet_disp_processor.py:107-118
   StereoBaseAggregation stereobase/hourglass.py:79-104 + stereobase_gru.py:161-164
   LightStereoAggregation lightstereo/aggregation.py:42-60 (Aggregation.forward), :94-101 (MobileV2Residual), :119-134 (AttentionModule)
@@ -271,6 +272,20 @@ class GwcAggregation(_Engine):
     def __call__(self, volume, h, w):
         mon = self._watch(volume.device)
         out = ops.upsample_softargmin(self.logits(volume), self.module.maxdisp, h, w, align_corners=False)
+        if mon is not None:
+            mon.poll()
+        return out
+
+
+class CascadeAggregation(GwcAggregation):
+    """Eval branch of CasStereo's CostAggregation (casnet/cas_psm.py:233-279, the same class in cas_gwc.py:210-256): its
+    layers and module indices are GwcDispProcessor's, so GwcAggregation.logits runs it as is; the tail weights fine bin d by
+    the per-pixel hypothesis disp_range_samples[b, d, h, w] instead of d."""
+
+    def __call__(self, cost, fine_d, fine_h, fine_w, disp_range_samples):
+        mon = self._watch(cost.device)
+        assert tuple(disp_range_samples.shape[1:]) == (fine_d, fine_h, fine_w)
+        out = ops.upsample_softargmin_values(self.logits(cost), disp_range_samples, align_corners=False)
         if mon is not None:
             mon.poll()
         return out

@@ -83,9 +83,12 @@ __host__ inline Axis make_axis(int in, int out, int align) {
 // coarse interval (one extra exp per interval instead of one per sample).  The fine->coarse map depends on d only; it
 // is tabulated once per CTA in shared memory (lambda per fine sample, first fine sample per coarse interval).
 // Logits are pre-scaled by log2(e) so every exponential is a single MUFU.EX2.
+// VALUES: the value of fine bin d is values[b,d,h,w] (CasStereo's per-pixel hypotheses, casnet/cas_psm.py:268-274) instead
+// of d; `values` is unused otherwise.
+template <bool VALUES>
 __global__ void __launch_bounds__(128) upsample_softargmin_kernel(const float* __restrict__ cost, float* __restrict__ out,
                                                                   int Dl, int Hl, int Wl, int D, int H, int W, Axis ad,
-                                                                  Axis ah, Axis aw) {
+                                                                  Axis ah, Axis aw, const float* __restrict__ values) {
   extern __shared__ float s_tab[];
   float* s_lam = s_tab;                                  // [D]   weight of the upper neighbour
   int* s_first = reinterpret_cast<int*>(s_tab + D);      // [Dl+1] first fine sample of coarse interval c
@@ -124,6 +127,7 @@ __global__ void __launch_bounds__(128) upsample_softargmin_kernel(const float* _
   if (Dl > 1) {
     a0 = __ldg(p00 + slice), a1 = __ldg(p01 + slice), a2 = __ldg(p10 + slice), a3 = __ldg(p11 + slice);
   }
+  const float* vpix = VALUES ? values + (size_t)b * D * H * W + (size_t)y * W + x : nullptr;
   float m = -INFINITY, s = 0.f, t = 0.f;
   for (int c = 0; c < Dl; ++c) {
     const float t1 = (c + 1 < Dl) ? hy * (hx * a0 + lx * a1) + ly * (hx * a2 + lx * a3) : t0;
@@ -142,7 +146,7 @@ __global__ void __launch_bounds__(128) upsample_softargmin_kernel(const float* _
       for (int d = dbeg; d < dend; ++d) {
         const float e = exp2f(fmaf(s_lam[d], dt, tm));   // (1-l)*t0 + l*t1 - m
         s += e;
-        t = fmaf(e, fd, t);
+        t = fmaf(e, VALUES ? __ldg(vpix + (size_t)d * H * W) : fd, t);
         fd += 1.f;
       }
     }
@@ -204,11 +208,25 @@ int osb_upsample_softargmin_fwd(const float* cost, float* out, int B, int Dl, in
   OSB_REQUIRE(H <= 65535 && B <= 65535, "upsample_softargmin: grid too large");
   dim3 grid((W + 127) / 128, H, B);
   OSB_REQUIRE((size_t)(D + Dl + 1) * 4 <= 48 * 1024, "upsample_softargmin: D=%d too large for the shared tables", D);
-  osb::upsample_softargmin_kernel<<<grid, 128, (size_t)(D + Dl + 1) * 4, (cudaStream_t)stream>>>(
+  osb::upsample_softargmin_kernel<false><<<grid, 128, (size_t)(D + Dl + 1) * 4, (cudaStream_t)stream>>>(
       cost, out, Dl, Hl, Wl, D, H, W, osb::make_axis(Dl, D, align_corners), osb::make_axis(Hl, H, align_corners),
-      osb::make_axis(Wl, W, align_corners));
+      osb::make_axis(Wl, W, align_corners), nullptr);
   osb::count_launch();
   return osb::check_launch("upsample_softargmin_kernel");
+}
+
+int osb_upsample_softargmin_values_fwd(const float* cost, const float* values, float* out, int B, int Dl, int Hl, int Wl, int D,
+                                       int H, int W, int align_corners, osb_stream_t stream) {
+  OSB_REQUIRE(cost && values && out, "upsample_softargmin_values: null pointer");
+  OSB_REQUIRE(B > 0 && Dl > 0 && Hl > 0 && Wl > 0 && D > 0 && H > 0 && W > 0, "upsample_softargmin_values: empty shape");
+  OSB_REQUIRE(H <= 65535 && B <= 65535, "upsample_softargmin_values: grid too large");
+  dim3 grid((W + 127) / 128, H, B);
+  OSB_REQUIRE((size_t)(D + Dl + 1) * 4 <= 48 * 1024, "upsample_softargmin_values: D=%d too large for the shared tables", D);
+  osb::upsample_softargmin_kernel<true><<<grid, 128, (size_t)(D + Dl + 1) * 4, (cudaStream_t)stream>>>(
+      cost, out, Dl, Hl, Wl, D, H, W, osb::make_axis(Dl, D, align_corners), osb::make_axis(Hl, H, align_corners),
+      osb::make_axis(Wl, W, align_corners), values);
+  osb::count_launch();
+  return osb::check_launch("upsample_softargmin_kernel<values>");
 }
 
 int osb_epe_partial_fwd(const float* pred, const float* gt, float* out, int B, int HW, float maxdisp, osb_stream_t stream) {

@@ -233,6 +233,56 @@ def gwc_concat_volume(ref_gwc, tgt_gwc, ref_cat, tgt_cat, maxdisp, num_groups):
     return out.to(dt)
 
 
+def _no_autograd(name, *tensors):
+    if _recording(*tensors):
+        raise RuntimeError("openstereo_b200.ops.%s has no backward: call it under torch.no_grad() or on operands that do not "
+                           "require grad" % name)
+
+
+def warped_concat_volume(x, y, disp_samples, mask_left=False):
+    """CasPSMNet's GetCostVolume.forward (casnet/cas_psm.py:286-318) -> (B, 2C, D, H, W): channels [:C] are x repeated over D
+    (zeroed where w < disp when mask_left), channels [C:] are y sampled at column w - disp[b, d, h, w] like
+    F.grid_sample(bilinear, zeros, align_corners=True).  disp_samples: (B, D, H, W), any real values.  No backward."""
+    _no_autograd("warped_concat_volume", x, y, disp_samples)
+    xs, dt = _prep(x, "x")
+    ys, _ = _prep(y, "y")
+    ds, _ = _prep(disp_samples, "disp_samples")
+    assert xs.dim() == 4 and xs.shape == ys.shape and ds.dim() == 4
+    b, c, h, w = xs.shape
+    assert ds.shape[0] == b and ds.shape[2:] == (h, w)
+    _same_device(xs, ys, ds)
+    d = ds.shape[1]
+    out = torch.empty((b, 2 * c, d, h, w), dtype=torch.float32, device=xs.device)
+    if out.numel():
+        _call("osb_warped_concat_volume_fwd", xs.data_ptr(), ys.data_ptr(), ds.data_ptr(), out.data_ptr(), b, c, d, h, w,
+              1 if mask_left else 0, _stream(out))
+    return out.to(dt)
+
+
+def warped_gwc_concat_volume(x_gwc, y_gwc, x_cat, y_cat, disp_samples, num_groups):
+    """CasGwcNet's GetCostVolume.forward (casnet/cas_gwc.py:263-329) -> (B, G + 2*Cc, D, H, W): the group-wise correlation of
+    the masked left and warped right gwc features, then [masked left | warped right] concatenation features, in one launch.
+    No backward."""
+    _no_autograd("warped_gwc_concat_volume", x_gwc, y_gwc, x_cat, y_cat, disp_samples)
+    xg, dt = _prep(x_gwc, "x_gwc")
+    yg, _ = _prep(y_gwc, "y_gwc")
+    xc, _ = _prep(x_cat, "x_cat")
+    yc, _ = _prep(y_cat, "y_cat")
+    ds, _ = _prep(disp_samples, "disp_samples")
+    assert xg.dim() == 4 and xg.shape == yg.shape and xc.shape == yc.shape and ds.dim() == 4
+    b, cg, h, w = xg.shape
+    cc = xc.shape[1]
+    assert xc.shape[0] == b and xc.shape[2:] == (h, w) and ds.shape[0] == b and ds.shape[2:] == (h, w)
+    assert cg % num_groups == 0                                  # cas_gwc.py:312
+    _same_device(xg, yg, xc, yc, ds)
+    d = ds.shape[1]
+    out = torch.empty((b, num_groups + 2 * cc, d, h, w), dtype=torch.float32, device=xg.device)
+    if out.numel():
+        _call("osb_warped_gwc_concat_volume_fwd", xg.data_ptr(), yg.data_ptr(), xc.data_ptr(), yc.data_ptr(), ds.data_ptr(),
+              out.data_ptr(), b, cg, num_groups, cc, d, h, w, _stream(out))
+    return out.to(dt)
+
+
 # --------------------------------------------------------------------------- soft-argmin tails
 def softargmin(cost, maxdisp, keepdim=True, alpha=1.0, start=0.0, step=1.0, normalize=True):
     """disparity_regression(F.softmax(cost, 1), maxdisp) in one pass (stereobase_gru.py:163-164)."""
@@ -301,6 +351,24 @@ def upsample_softargmin(cost, maxdisp, out_h, out_w, align_corners=False):
     if out.numel():
         _call("osb_upsample_softargmin_fwd", c.data_ptr(), out.data_ptr(), b, dl, hl, wl, maxdisp, out_h, out_w,
                   1 if align_corners else 0, _stream(out))
+    return out.to(dt)
+
+
+def upsample_softargmin_values(cost, disp_values, align_corners=False):
+    """CasStereo's CostAggregation eval tail (casnet/cas_psm.py:268-274): F.upsample(cost, [D, H, W], 'trilinear') -> squeeze
+    -> softmax over D -> sum_d p * disp_values, fused.  cost: (B, 1, D', H', W'), disp_values: (B, D, H, W) -> (B, H, W).
+    No backward."""
+    _no_autograd("upsample_softargmin_values", cost, disp_values)
+    c, dt = _prep(cost, "cost")
+    v, _ = _prep(disp_values, "disp_values")
+    assert c.dim() == 5 and c.shape[1] == 1 and v.dim() == 4 and v.shape[0] == c.shape[0]
+    _same_device(c, v)
+    b, _, dl, hl, wl = c.shape
+    _, d, h, w = v.shape
+    out = torch.empty((b, h, w), dtype=torch.float32, device=c.device)
+    if out.numel():
+        _call("osb_upsample_softargmin_values_fwd", c.data_ptr(), v.data_ptr(), out.data_ptr(), b, dl, hl, wl, d, h, w,
+              1 if align_corners else 0, _stream(out))
     return out.to(dt)
 
 

@@ -1,5 +1,6 @@
-"""patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo, built by the
-reference's own classes from an unchanged cfg YAML) run its cost-volume hot path on the sm_90a kernels.
+"""patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo, and
+CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume hot
+path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each
 needs its own rebinding:
@@ -9,6 +10,7 @@ needs its own rebinding:
 * PSMNet      ``cat_fms`` captured by functools.partial at construction (psmnet_cost_processor.py:227-232),
               aggregator + FasterSoftArgmin modules                          -> ``CostProcessor.forward`` / ``FasterSoftArgmin.forward``
 * LightStereo / IGEVStereo  like StereoBase: names imported into lightstereo.py:4-6 / igev_stereo.py:1-3 (``from .submodule import *``)
+* CasStereo   ``get_cv`` (GetCostVolume) and ``cost_agg[i]`` (CostAggregation) modules  -> per-instance ``forward`` overrides
 * StereoBase  functions imported INTO the module namespace (stereobase_gru.py:5-6,10-11) and the ``cost_agg``
               Hourglass                                                      -> per-INSTANCE copies of the methods that use those names,
                                                                                 with a private globals dict (the module itself, and
@@ -28,7 +30,7 @@ import types
 import torch
 
 from . import ops
-from .aggregation import GwcAggregation, PSMAggregation, StereoBaseAggregation
+from .aggregation import CascadeAggregation, GwcAggregation, PSMAggregation, StereoBaseAggregation
 from .geo import CombinedGeoEncodingVolume
 
 
@@ -329,6 +331,55 @@ def _patch_igev(model, strict, backbone=True):
     return model
 
 
+def _patch_cascade(model, strict, backbone=True):
+    """CasStereo (casnet/cas_psm.py PSMNet = CasPSMNet, casnet/cas_gwc.py GwcNet = CasGwcNet): every stage's warped cost volume
+    (``get_cv.forward``) and every stage's aggregation + hypothesis-weighted soft-argmin (``cost_agg[i].forward``).  The FPN
+    feature extractor and get_disp_range_samples stay the reference's code inside model.forward; `backbone` has no effect."""
+    gcv = model.get_cv
+    gcv_orig = gcv.forward
+    if type(model).__module__.rsplit(".", 1)[-1] == "cas_gwc":
+        def cv_forward(self, features_left, features_right, disp_range_samples, ndisp, num_groups):
+            if not _accelerable(self, features_left, features_right, disp_range_samples):
+                if strict:
+                    _refuse("CasGwcNet GetCostVolume")
+                return gcv_orig(features_left, features_right, disp_range_samples, ndisp, num_groups)
+            assert disp_range_samples.shape[1] == ndisp
+            vol = ops.warped_gwc_concat_volume(features_left["gwc_feature"], features_right["gwc_feature"],
+                                               features_left["concat_feature"], features_right["concat_feature"],
+                                               disp_range_samples, num_groups)
+            return vol.to(features_left["gwc_feature"].dtype)
+    else:
+        def cv_forward(self, x, y, disp_range_samples, ndisp):
+            if not _accelerable(self, x, y, disp_range_samples):
+                if strict:
+                    _refuse("CasPSMNet GetCostVolume")
+                return gcv_orig(x, y, disp_range_samples, ndisp)
+            assert disp_range_samples.shape[1] == ndisp
+            return ops.warped_concat_volume(x, y, disp_range_samples, mask_left=False)
+    gcv.forward = types.MethodType(cv_forward, gcv)
+
+    for agg_mod in model.cost_agg:
+        _patch_cascade_agg(agg_mod, strict)
+    return model
+
+
+def _patch_cascade_agg(agg_mod, strict):
+    agg_orig = agg_mod.forward
+    engine = CascadeAggregation(agg_mod)
+
+    def agg_forward(self, cost, FineD, FineH, FineW, disp_range_samples):
+        if not _accelerable(self, cost, disp_range_samples):
+            if strict:
+                _refuse("CasStereo CostAggregation")
+            return agg_orig(cost, FineD, FineH, FineW, disp_range_samples)
+        return engine(cost, FineD, FineH, FineW, disp_range_samples).to(cost.dtype)
+
+    agg_mod.forward = types.MethodType(agg_forward, agg_mod)
+
+
+# CasStereo's classes are also named PSMNet / GwcNet: they are told apart by the module that defines them
+_CASCADE_MODULES = {("casnet", "cas_psm"): "PSMNet", ("casnet", "cas_gwc"): "GwcNet"}
+
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
              "IGEVStereo": _patch_igev}
 
@@ -336,14 +387,20 @@ _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _pa
 def patch(model, strict=True, backbone=True):
     """Rebind the hot path of a reference model instance in place and return it.  backbone=True (default) also routes the
     GwcNet / PSMNet 2D extractor's residual blocks to the wgmma conv kernels in CUDA inference calls (_patch_backbone);
-    backbone=False leaves the extractor entirely to the reference's cuDNN code."""
+    backbone=False leaves the extractor entirely to the reference's cuDNN code.  For the CasStereo models (casnet.cas_psm.PSMNet,
+    casnet.cas_gwc.GwcNet) `backbone` has no effect: their FPN extractor always runs the reference's code."""
     if not isinstance(model, torch.nn.Module):
         raise TypeError("patch() expects an nn.Module")
     name = type(model).__name__
-    if name not in _PATCHERS:
-        raise NotImplementedError("patch(): no hot-path drop-in for %s (supported: %s)" % (name, sorted(_PATCHERS)))
+    if _CASCADE_MODULES.get(tuple(type(model).__module__.split(".")[-2:])) == name:
+        patcher = _patch_cascade
+    elif name in _PATCHERS:
+        patcher = _PATCHERS[name]
+    else:
+        raise NotImplementedError("patch(): no hot-path drop-in for %s (supported: %s, and CasStereo's casnet.cas_psm.PSMNet / "
+                                  "casnet.cas_gwc.GwcNet)" % (name, sorted(_PATCHERS)))
     if getattr(model, "_osb_patched", False):
         return model
-    _PATCHERS[name](model, strict, backbone)
+    patcher(model, strict, backbone)
     model._osb_patched = True
     return model

@@ -11,6 +11,8 @@
       expanse 4, left attention) -> softmax/regression -> context_upsample (lightstereo.py:51-62)
   c5  IGEV cfgs/igev, batch 8 @480x640: gwc volume (C=96, G=8, D'=48) + 16 GRU-iteration lookups of the combined geometry
       encoding volume (igev_stereo.py:158,181-193; geometry.py:32-57) + 16 context up-samplings
+  c6  CasPSMNet cfgs/casnet (the reference's class + patch()), batch 10 @512x960: whole-model forward next to the unpatched model
+      on the same GPU, per-stage volume / aggregation / tail times  (python tools/bench_configs.py --only c6)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -31,6 +33,7 @@ __graft_entry__.build()
 from openstereo_b200 import aggregation as agg          # noqa: E402
 from openstereo_b200 import geo, host_models, ops       # noqa: E402
 from oracle import aggregation as oagg                  # noqa: E402
+from oracle import cascade as ocas                      # noqa: E402
 from oracle import cost_volume as ocv                   # noqa: E402
 from oracle import geo_lookup as ogeo                   # noqa: E402
 from oracle import lightstereo as olight                # noqa: E402
@@ -245,6 +248,72 @@ def gw(iters):
              overflow_count=ops.tc_overflow_count())
 
 
+def c6(iters, B=10, h=512, w=960):
+    """CasPSMNet (the reference's own class, cfgs/casnet/casnet_psm_sceneflow.yaml unchanged, seeded weights) at the cfg's eval
+    crop and evaluator batch: patch() next to the unpatched model on this GPU (cuDNN fp32, TF32 off).  Per stage: the warped
+    volume (GB/s on its algorithmic bytes), the aggregation (useful TFLOP/s on the 3D convolutions' MACs) and the fused tail."""
+    from oracle import _reference_shim as shim
+    from openstereo_b200.patch import patch
+    cfg = shim.load_cfg("cfgs/casnet/casnet_psm_sceneflow.yaml").MODEL
+    m = shim.load("stereo.modeling.models.casnet.cas_psm").PSMNet(cfg).eval()
+    m.load_state_dict(si.seeded_state_dict(m.state_dict(), seed=1, scale=ocas.CASNET_SCALE))
+    m.to(DEV)
+    gen = torch.Generator().manual_seed(19)
+    x = {"left": rnd(gen, B, 3, h, w), "right": rnd(gen, B, 3, h, w)}
+    with torch.no_grad():
+        ms_ref, want = timeit(lambda: m(dict(x))["disp_pred"], max(2, iters // 3), warm=1)
+        patch(m)
+        ms, got = timeit(lambda: m(dict(x))["disp_pred"], iters)
+        # per-stage split: CUDA events around each stage's volume / aggregation call, the tail's own entry point inside it
+        events = []
+
+        def timed(mod, tag):
+            inner = mod.forward
+
+            def fwd(*args, **kw):
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                out = inner(*args, **kw)
+                b.record()
+                events.append((tag, a, b))
+                return out
+            mod.forward = fwd
+        timed(m.get_cv, "volume")
+        for i, agg_mod in enumerate(m.cost_agg):
+            timed(agg_mod, "agg%d" % i)
+        ops.profile_start()
+        m(dict(x))
+        torch.cuda.synchronize()
+        prof = ops.profile_stop()
+    tails = [a.elapsed_time(b) for a, b in prof.get("osb_upsample_softargmin_values_fwd", [])]
+    vols = [a.elapsed_time(b) for tag, a, b in events if tag == "volume"]
+    aggs = [a.elapsed_time(b) for tag, a, b in events if tag.startswith("agg")]
+    stages = []
+    for i, (cin, hq, wq, gmac) in enumerate(((32, h // 4, w // 4, 109.0), (16, h // 2, w // 2, 395.0))):
+        vol_bytes = 4 * (2 * B * cin * hq * wq + B * 12 * hq * wq + B * 2 * cin * 12 * hq * wq)
+        agg_ms = aggs[i] - tails[i]
+        stages.append({"stage": i + 1, "volume_shape": [B, 2 * cin, 12, hq, wq], "volume_ms": round(vols[i], 3),
+                       "volume_GBps": round(vol_bytes / vols[i] / 1e6, 1), "volume_frac_of_3350GBps": round(vol_bytes / vols[i] / 1e6 / 3350, 3),
+                       "aggregation_ms": round(agg_ms, 3), "aggregation_useful_tflops": round(2 * gmac * B / agg_ms, 1),
+                       "tail_ms": round(tails[i], 3)})
+    emit(config="c6 CasPSMNet cfgs/casnet/casnet_psm_sceneflow.yaml, B=%d @%dx%d (reference class + patch())" % (B, h, w),
+         gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+         ms_per_step=round(ms, 3), pairs_per_s=round(B * 1e3 / ms, 2), reference_cudnn_fp32_ms=round(ms_ref, 2),
+         reference_pairs_per_s=round(B * 1e3 / ms_ref, 2), speedup_vs_reference_gpu=round(ms_ref / ms, 2),
+         epe_vs_reference_gpu_px=float("%.3e" % (got - want).abs().mean().item()), disparity_std_px=round(want.std().item(), 2),
+         stages=stages, overflow_count=ops.tc_overflow_count())
+
+
+def _power_limit_w():
+    try:
+        import subprocess
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(DEV.index or 0)],
+                             capture_output=True, text=True, timeout=30).stdout
+        return float(out.strip().splitlines()[0])
+    except Exception:
+        return float("nan")
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", default="c1,c3,c4,c5,gw")
@@ -252,7 +321,7 @@ if __name__ == "__main__":
     a = ap.parse_args()
     for name in a.only.split(","):
         try:
-            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw}[name](a.iters)
+            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:

@@ -23,6 +23,7 @@ sys.path.insert(0, ROOT)
 
 from oracle import _reference_shim as shim                      # noqa: E402
 from oracle import aggregation as oagg                          # noqa: E402
+from oracle import cascade as ocas                              # noqa: E402
 from oracle import cost_volume as ocv                           # noqa: E402
 from oracle import geo_lookup as ogeo                           # noqa: E402
 from oracle import lightstereo as olight                        # noqa: E402
@@ -304,15 +305,72 @@ def flavours():
     save("regression_flavours", prob=prob, maxdisp=48, interval=4, out_interval=ref, values=vals, out_values=ref2)
 
 
+def cascade_samples(seed, b, d, h, w):
+    """Per-pixel hypotheses covering every case of the warped volume: fractional, integer and negative samples, and columns
+    w - disp beyond both image edges (below -1, in (-1, 0), above W - 1)."""
+    g = torch.Generator().manual_seed(seed)
+    disp = torch.rand(b, d, h, w, generator=g) * (w + 8) - 6
+    disp[:, 0] = torch.randint(-3, w + 3, (b, h, w), generator=g).float()           # integer samples
+    disp[:, 1] = torch.arange(w).float() + 0.5                                      # column -0.5: between -1 and 0
+    disp[:, 2] = torch.arange(w).float() - (w - 1) - 0.25                           # column W - 0.75: beyond the right edge
+    return disp
+
+
+def cascade():
+    """CasStereo: both GetCostVolume variants at a height whose row coordinates partly come back off-integer, the
+    CostAggregation tail at x4 and x2, and a seeded CasPSMNet at 256x512 (a strided sample of its disparity map)."""
+    rpsm = shim.load("stereo.modeling.models.casnet.cas_psm")
+    rgwc = shim.load("stereo.modeling.models.casnet.cas_gwc")
+    b, d, h, w = 2, 5, 13, 21
+    assert any((hh / ((h - 1.0) / 2.0) - 1.0 + 1) * ((h - 1) / 2) != hh for hh in range(h))
+    disp = cascade_samples(90, b, d, h, w)
+    x, y = rnd(91, b, 6, h, w), rnd(92, b, 6, h, w)
+    ref = rpsm.GetCostVolume()(x, y, disp, d)
+    must_equal(ref, ocas.warped_concat_volume(x, y, disp, d), "CasPSMNet volume")
+    save("cas_volume_psm", x=x, y=y, disp=disp, out=ref)
+    fl = {"gwc_feature": rnd(93, b, 8, h, w), "concat_feature": rnd(94, b, 3, h, w)}
+    fr = {"gwc_feature": rnd(95, b, 8, h, w), "concat_feature": rnd(96, b, 3, h, w)}
+    ref = rgwc.GetCostVolume()(fl, fr, disp, d, 2)
+    must_equal(ref, ocas.warped_gwc_concat_volume(fl, fr, disp, d, 2), "CasGwcNet volume")
+    save("cas_volume_gwc", xg=fl["gwc_feature"], yg=fr["gwc_feature"], xc=fl["concat_feature"], yc=fr["concat_feature"],
+         disp=disp, groups=2, out=ref)
+    with torch.no_grad():
+        agg = rpsm.CostAggregation(8, 8).eval()
+        agg.load_state_dict(si.seeded_state_dict(agg.state_dict(), seed=97))
+        arrays = {}
+        for tag, (fd, hl, wl) in (("x4", (48, 5, 7)), ("x2", (24, 10, 14))):
+            logits = rnd(98, 1, 1, 12, hl, wl, scale=3.0)
+            vals = cascade_samples(99, 1, fd, 20, 28) * 4
+            want = ocas.upsample_softargmin_values(logits, fd, 20, 28, vals)
+            agg.classif3 = _Const(logits)                                           # feed the tail known logits
+            must_equal(agg(torch.zeros(1, 8, 4, 4, 4), fd, 20, 28, vals), want, "CasStereo tail " + tag)
+            arrays.update({"cost_" + tag: logits, "values_" + tag: vals, "out_" + tag: want})
+        save("cas_tail", **arrays)
+        cfg = shim.load_cfg("cfgs/casnet/casnet_psm_sceneflow.yaml").MODEL
+        m = rpsm.PSMNet(cfg).eval()
+        sd = si.seeded_state_dict(m.state_dict(), seed=1, scale=ocas.CASNET_SCALE)
+        m.load_state_dict(sd)
+        left, right = rnd(100, 1, 3, 256, 512), rnd(101, 1, 3, 256, 512)
+        out = m({"left": left, "right": right})["disp_pred"]
+        save("cas_psmnet_256x512", seed_left=100, seed_right=101, weight_seed=1, checksum=checksum(sd), disp_sample=out[:, ::8, ::8],
+             disp_mean=out.mean(), disp_std=out.std())
+
+
+class _Const(torch.nn.Module):
+    def __init__(self, t):
+        super().__init__()
+        self.t = t
+
+    def forward(self, _):
+        return self.t
+
+
+SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade"]
+
 if __name__ == "__main__":
     if not shim.available():
         raise SystemExit("reference tree not found; golden vectors can only be generated in the authoring container")
     torch.set_num_threads(os.cpu_count() or 1)
-    volumes()
-    regression()
-    modules()
-    models()
-    lookups()
-    flavours()
-    lightstereo()
+    for name in sys.argv[1:] or SECTIONS:                       # e.g. `python tools/make_golden.py cascade`
+        globals()[name]()
     print("all oracle restatements bit-equal to the reference; golden vectors written to", OUT)
