@@ -4,8 +4,10 @@
 //   gwcnet/hourglass.py:25-32, psmnet/psmnet_cost_processor.py:86-98.
 // Same scheme as conv3d_tc.cu (3xFP16 split, kw taps stacked along N and un-shifted in the epilogue, LDG-staged swizzled
 // operands, warp-specialised persistent CTA with a consumer warpgroup that issues the wgmmas and runs the epilogue), generalised:
-//   * an A "unit" is R consecutive input rows starting at block row s; tap kh of the output tile reads the unit with
-//     s = kh - 1 (the tile index machinery below is written for TILES tiles; the register-held accumulator limits it to one);
+//   * an A "unit" is R consecutive input rows starting at block row s; tap kh of output tile t reads the unit with
+//     s = t * R + kh - 1.  A work item is two such tiles, one per consumer warpgroup (TcgCfg::NT, tile_of): each unit and
+//     weight slice is staged once and read by both, so the units between the two tiles and the whole weight stream serve two
+//     output tiles;
 //   * K chunks are 16 channels (64-byte rows [16 hi | 16 lo] fp16, SWIZZLE_64B: one K = 16 MMA step each);
 //   * a work item covers G = 32 output channels: the accumulator tile is 128 x 3G = 96 fp32 columns (96 registers per consumer
 //     thread), and the weight producer streams only the three G-row kw blocks of each slice (contiguous in shared memory, so one
@@ -57,32 +59,41 @@ struct TcgCfg {
   static constexpr int B_SLICE = N3 * ROWB;                 // one kh weight slice in global memory (hi and lo halves of every row)
   static constexpr int B_SUB = NG3 * ROWB;                  // the part of it one item reads
   static constexpr int LD = NG3 + 4;                        // floats per row of the staged accumulator tile
-  // A-unit ring.  NLW loader warps (4-7 and 9) fill the units round-robin (unit u belongs to loader u mod NLW) into a ring as deep as
+  // Work item = NT output tiles, tile t (consumer warpgroup t) at image rows row0 + t * TS .. + R - 1.  DIL = 1: consecutive row
+  // blocks, so the units of rows between the tiles feed both.  DIL = 2: rows h and h + 2, whose taps share two of their three units
+  // (adjacent rows share none); row blocks then interleave, hb = 2k + j -> rows 4k + j and 4k + j + 2.
+  static constexpr int NT = TC_WGS * TILES;
+  static constexpr int TS = R * DIL;
+  static constexpr int HSPAN = NT * TS;                     // image rows covered by DIL interleaved row blocks
+  __host__ __device__ static constexpr int row0(int hb) { return (hb / DIL) * HSPAN + (hb % DIL) * R; }
+  __host__ static int hblocks(int H) { return DIL * ((H + HSPAN - 1) / HSPAN); }
+  // A-unit ring.  NLW loader warps (8-11) fill the units round-robin (unit u belongs to loader u mod NLW) into a ring as deep as
   // shared memory allows (at most 10 units).  Each loader warp enumerates ONLY ITS OWN units: a walk over the whole (tile, tap)
   // sequence by every warp, picking every NLW-th unit, makes that scalar control flow the bound of these kernels.
-  static constexpr int NLW = 5;
-  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * 3 * B_SUB + 128 * LD * 4 + 1024 + 2 * 4 * 2 * DIL * 32 * 4 + 3 * COUT * 4;
+  static constexpr int NLW = 4;
+  static constexpr int XCHG_FLOATS = 2 * 4 * 2 * DIL * 32;  // per consumer warpgroup: [2][4 quadrants][2 sides][DIL columns][32]
+  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * 3 * B_SUB + TC_WGS * 128 * LD * 4 + 1024 + TC_WGS * XCHG_FLOATS * 4 + 3 * COUT * 4;
   static constexpr int STAGES = (232448 - FIXED_SMEM) / UNIT_BYTES < 10 ? (232448 - FIXED_SMEM) / UNIT_BYTES : 10;
   static_assert(STAGES >= NLW, "the ring must hold at least one unit per loader warp");
   static constexpr int S_FIRST = -DIL;                      // unit start rows run from S_FIRST to S_LAST (block-relative)
-  static constexpr int S_LAST = (TILES - 1) * R + DIL;
-  static constexpr int HBLK = TILES * R;                    // output rows per work item
+  static constexpr int S_LAST = (NT - 1) * TS + DIL;
   static constexpr int KSTEPS = KC / 16;                    // K = 16 fp16 channels per MMA
   static constexpr int LO = KC / 8;                         // descriptor offset (16-byte units) of the lo half of a row
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + STAGES * UNIT_BYTES;
-  static constexpr int STAGE_OFF = B_OFF + TC_BSLOTS * 3 * B_SUB;   // [128][LD] fp32 accumulator tile
-  static constexpr int BAR_OFF = STAGE_OFF + 128 * LD * 4;
-  static constexpr int THREADS = 128 + 128 + 64;            // consumer warpgroup | A loaders | weight producer + 5th loader (10 warps)
-  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + 2 * 4 * 2 * DIL * 32 * 4 + 3 * COUT * 4;
+  static constexpr int STAGE_OFF = B_OFF + TC_BSLOTS * 3 * B_SUB;   // [TC_WGS][128][LD] fp32 accumulator tiles
+  static constexpr int BAR_OFF = STAGE_OFF + TC_WGS * 128 * LD * 4;
+  static constexpr int THREADS = TC_WG_THREADS;             // consumers 0-7 | A loaders 8-11 | weight producer 12, idle 13-15
+  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + TC_WGS * XCHG_FLOATS * 4 + 3 * COUT * 4;
   static_assert(SMEM <= 232448, "shared memory budget of one CTA exceeded");
-  static_assert(TILES == 1, "the consumer warpgroup holds one accumulator tile");
+  static_assert(TILES == 1, "a consumer warpgroup holds one accumulator tile");
+  static_assert(DIL == 1 || R == 1, "interleaved row blocks assume one image row per tile");
   static_assert(COUT % G == 0, "output channels come in groups of 32");
   static_assert(B_SUB % 1024 == 0 && UNIT_BYTES % 1024 == 0, "operand tiles must stay 1024-byte aligned");
   // tile fed by unit s through tap kh, or -1
   static constexpr int tile_of(int s, int kh) {
     const int num = s - (kh - 1) * DIL;
-    return (num >= 0 && num % R == 0 && num / R < TILES) ? num / R : -1;
+    return (num >= 0 && num % TS == 0 && num / TS < NT) ? num / TS : -1;
   }
   static constexpr bool used(int s) { return tile_of(s, 0) >= 0 || tile_of(s, 1) >= 0 || tile_of(s, 2) >= 0; }
   // units of one (kd, chunk) phase in issue order: their number and the start row of the j-th one
@@ -113,11 +124,11 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   float* stage = reinterpret_cast<float*>(smem + C::STAGE_OFF);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
   uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumer   (32 arrivals: one warp)
-  uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] consumer -> loaders   (4 arrivals: one per consumer warp)
-  uint64_t* b_full = a_empty + C::STAGES;           // [2][3]   weight producer -> consumer (expect_tx + bulk-copy bytes)
-  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   consumer -> weight producer (4 arrivals)
-  float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 1024);   // [2][4 quadrants][2 sides][DIL columns][32]
-  float* s_scale = xchg + 2 * 4 * 2 * DIL * 32;
+  uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] consumers -> loaders  (8 arrivals: one per consumer warp)
+  uint64_t* b_full = a_empty + C::STAGES;           // [2][3]   weight producer -> consumers (expect_tx + bulk-copy bytes)
+  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   consumers -> weight producer (8 arrivals)
+  float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 1024);   // [TC_WGS][XCHG_FLOATS]
+  float* s_scale = xchg + TC_WGS * C::XCHG_FLOATS;
   float* s_shift = s_scale + COUT;
   float* zeros = s_shift + COUT;
 
@@ -130,11 +141,11 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&a_ready[s], 32);                     // one loader warp fills a unit
-      mbar_init(&a_empty[s], 4);
+      mbar_init(&a_empty[s], 4 * TC_WGS);
     }
     for (int k = 0; k < TC_BSLOTS * 3; ++k) {
       mbar_init(&b_full[k], 1);
-      mbar_init(&b_empty[k], 4);
+      mbar_init(&b_empty[k], 4 * TC_WGS);
     }
     fence_mbar_init();
   }
@@ -145,13 +156,19 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   }
   __syncthreads();
 
-  // ---------------------------------------------------------------------------------------------- consumer warpgroup
-  // wgmma issue into one 128 x 96 register tile (output channels cg .. cg + 31 of all three kw taps), then the epilogue of that tile.
-  if (warp < 4) {
+  // ---------------------------------------------------------------------------------------------- consumer warpgroups
+  // Warpgroup wg issues the wgmmas of tile wg of the item into its 128 x 96 register tile (output channels cg .. cg + 31 of all
+  // three kw taps) from the units and weight slices both warpgroups read, then runs the epilogue of that tile.
+  if (warp < 4 * TC_WGS) {
+    setmaxnreg_inc<TC_CONSUMER_REGS>();
+    const int wg = warp >> 2;
+    stage += wg * 128 * C::LD;
+    xchg += wg * C::XCHG_FLOATS;
+    const int bar_stage = 1 + 2 * wg, bar_xchg = 2 + 2 * wg;   // this warpgroup's named barriers
     const uint64_t dbase = (KC == 32) ? desc_sw128_base() : desc_sw64_base();
     constexpr uint32_t A_HALF = 64 * C::ROWB / 16;  // descriptor offset of operand rows 64..127
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
-    const int q = warp;                              // epilogue: this warp owns tile rows 32q .. 32q + 31
+    const int q = warp & 3;                          // epilogue: this warp owns tile rows 32q .. 32q + 31
     const int m = q * 32 + lane;                     // operand row owned by this thread
     const int rr = m / W, wcol = m % W;              // image row inside the tile, image column
     const bool has_left_q = ((q * 32) % W) != 0;     // the quadrant to the left continues the same image row
@@ -179,7 +196,7 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
               const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
 #pragma unroll
               for (int kh = 0; kh < 3; ++kh) {
-                if (C::tile_of(s, kh) != 0) continue;  // one tile: unit s meets the slices kh with s == (kh - 1) * DIL
+                if (C::tile_of(s, kh) != wg) continue;   // unit s meets slice kh for tile wg when s == wg * TS + (kh - 1) * DIL
                 const uint32_t bslot = (phc & 1) * 3 + kh;
                 mbar_wait(&b_full[bslot], (phc >> 1) & 1);
                 const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
@@ -197,19 +214,19 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
             }
           }
         }
-        named_bar_sync(2, 128);                      // every warp is done with the previous tile's staged rows
-        wg_stage<C::NG3>(stage, C::LD, acc, warp, lane);
-        named_bar_sync(2, 128);
+        named_bar_sync(bar_stage, 128);              // every warp is done with the previous tile's staged rows
+        wg_stage<C::NG3>(stage, C::LD, acc, q, lane);
+        named_bar_sync(bar_stage, 128);
       }
-      const int h0 = hb * C::HBLK;
-      const int ntiles = min(TILES, (p.H - h0 + C::R - 1) / C::R);
       // general widths: image column of this thread's tile column; halo columns and columns beyond the image are not stored
       const int col = GW ? ct * C::CSTEP - C::HALO + m : wcol;
       const bool cvalid = !GW || (m >= C::HALO && m < 128 - C::HALO && col < Wp);
       const uint32_t vmask = GW ? __ballot_sync(0xffffffffu, cvalid) : 0xffffffffu;
       const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * C::KSTEPS * 3);   // tc_common.cuh: rz_kappa
-      for (int t = 0; t < ntiles; ++t) {
-        const int h = h0 + t * C::R + rr;
+      {
+        // a tile below the image (odd H, H not a multiple of the item's rows) received its MMAs and releases like any other:
+        // `live` masks every store of it
+        const int h = C::row0(hb) + wg * C::TS + rr;
         const bool live = h < p.H;
         const ptrdiff_t vox = (((ptrdiff_t)b * p.D + d) * p.H + h) * Wp + col;     // NDHWC voxel index
         if (live && cvalid && p.residual && p.res_ndhwc) {
@@ -222,22 +239,21 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
         const size_t plane = (size_t)p.D * p.H * Wp;                               // NCDHW channel stride
         const ptrdiff_t ncdhw0 = (ptrdiff_t)b * COUT * plane + ((ptrdiff_t)d * p.H + h) * Wp + col;
         {
-          uint32_t raw[3][32];
-#pragma unroll
-          for (int kw = 0; kw < 3; ++kw)
-#pragma unroll
-            for (int c0 = 0; c0 < 32; c0 += 16) stage_ld16(stage + m * C::LD + kw * C::G + c0, &raw[kw][c0]);
+          // this voxel's P_kw columns are read from the staged tile four channels at a time (holding all 96 would spill)
+          const float* srow = stage + m * C::LD;
           float* xb = xchg + (exc & 1) * (4 * 2 * DIL * 32);
           ++exc;
           if (lane >= 32 - DIL) {                     // the next quadrant's first DIL columns need these P0 values
 #pragma unroll
-            for (int i = 0; i < 32; ++i) xb[((q * 2) * DIL + lane - (32 - DIL)) * 32 + i] = __uint_as_float(raw[0][i]);
+            for (int i = 0; i < 32; i += 4)
+              *reinterpret_cast<float4*>(xb + ((q * 2) * DIL + lane - (32 - DIL)) * 32 + i) = *reinterpret_cast<const float4*>(srow + i);
           }
           if (lane < DIL) {                           // the previous quadrant's last DIL columns need these P2 values
 #pragma unroll
-            for (int i = 0; i < 32; ++i) xb[((q * 2 + 1) * DIL + lane) * 32 + i] = __uint_as_float(raw[2][i]);
+            for (int i = 0; i < 32; i += 4)
+              *reinterpret_cast<float4*>(xb + ((q * 2 + 1) * DIL + lane) * 32 + i) = *reinterpret_cast<const float4*>(srow + 2 * C::G + i);
           }
-          named_bar_sync(1, 128);
+          named_bar_sync(bar_xchg, 128);
           const float* xl = has_left_q ? xb + (((q - 1) * 2) * DIL + (lane < DIL ? lane : 0)) * 32 : zeros;
           const float* xr = has_right_q ? xb + (((q + 1) * 2 + 1) * DIL + (lane >= 32 - DIL ? lane - (32 - DIL) : 0)) * 32 : zeros;
           float out[32];
@@ -245,19 +261,23 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
           for (int i0 = 0; i0 < 32; i0 += 4) {        // neighbour values loaded unconditionally, merged with selects (no branches)
             const float4 l4 = *reinterpret_cast<const float4*>(xl + i0);
             const float4 r4 = *reinterpret_cast<const float4*>(xr + i0);
+            const float4 p04 = *reinterpret_cast<const float4*>(srow + i0);
+            const float4 p14 = *reinterpret_cast<const float4*>(srow + C::G + i0);
+            const float4 p24 = *reinterpret_cast<const float4*>(srow + 2 * C::G + i0);
             const float le[4] = {l4.x, l4.y, l4.z, l4.w}, re[4] = {r4.x, r4.y, r4.z, r4.w};
+            const float p0[4] = {p04.x, p04.y, p04.z, p04.w}, p1[4] = {p14.x, p14.y, p14.z, p14.w}, p2[4] = {p24.x, p24.y, p24.z, p24.w};
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
               const int i = i0 + k;
-              float left = __shfl_up_sync(0xffffffffu, __uint_as_float(raw[0][i]), DIL);
-              float right = __shfl_down_sync(0xffffffffu, __uint_as_float(raw[2][i]), DIL);
+              float left = __shfl_up_sync(0xffffffffu, p0[k], DIL);
+              float right = __shfl_down_sync(0xffffffffu, p2[k], DIL);
               left = (lane < DIL) ? le[k] : left;       // column w-DIL (zero at the image edge)
               right = (lane >= 32 - DIL) ? re[k] : right;   // column w+DIL
               if (W < 32) {                             // several image rows per warp: row seams inside the warp are image edges
                 left = (wcol < DIL) ? 0.f : left;
                 right = (wcol >= W - DIL) ? 0.f : right;
               }
-              out[i] = ((left + __uint_as_float(raw[1][i])) + right) * corr;
+              out[i] = ((left + p1[k]) + right) * corr;
             }
           }
           // voxels of this warp that exist (W < 32: the warp spans two image rows, the second may lie below the image)
@@ -309,8 +329,9 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   // n + 1 of that slot belongs to a warp that has not filled it yet, so no mbarrier phase is skipped); with all loader warps on one
   // unit at a time they would sit on the load latency.  Each warp enumerates ONLY its own units (see the Cfg note): one runtime
   // loop, one copy of the body (unrolled bodies bloat the kernel's code).
-  else if (warp < 8 || warp == 9) {
-    const int lw = warp < 8 ? warp - 4 : 4;
+  else if (warp < 4 * TC_WGS + C::NLW) {
+    setmaxnreg_dec<TC_LOADER_REGS>();
+    const int lw = warp - 4 * TC_WGS;
     static_assert(KC == 16, "lane_voxel / unit-row mapping below is written for 64-byte operand rows");
     constexpr int CPR = KC / 4;                      // fp32 16-byte chunks per voxel of the K chunk
     constexpr int VPL = 32 / CPR;                    // voxels covered by one warp-wide LDG.128
@@ -347,7 +368,7 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
       const int hb = (it0 / ctiles) % p.hblocks;
       const int d = (it0 / (ctiles * p.hblocks)) % p.D;
       const int b = it0 / (ctiles * p.hblocks * p.D);
-      const int h0 = hb * C::HBLK;
+      const int h0 = C::row0(hb);
       const int col0 = ct * C::CSTEP - C::HALO + v0;   // image column of this lane's first load (whole-row kernels: v0)
       for (int kd = 0; kd < 3; ++kd) {
         const int din = d + kd - 1;
@@ -371,9 +392,11 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   // ---------------------------------------------------------------------------------------------- weight-slice producer
   // One elected lane streams the item's channel group of the pre-swizzled (kd, chunk, kh) slices -- three G-row kw blocks, 1-D
   // bulk copies -- into the two buffer sets, up to a whole phase ahead of the MMAs (tc_common.cuh: bulk_g2s).  The blocks keep
-  // their row index mod 8, so the swizzle applied by the packer stays valid.
-  else if (warp == 8) {
-    if (elect_one()) {
+  // their row index mod 8, so the swizzle applied by the packer stays valid.  The other warps of this warpgroup are idle: they only
+  // hand their registers back.
+  else {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (warp == 4 * TC_WGS + C::NLW && elect_one()) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w);
       uint32_t phc = 0;
       for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
@@ -422,7 +445,7 @@ static int launch_tcg(TcgParams& p, cudaStream_t stream) {
     }
     configured.here() = true;
   }
-  p.hblocks = (p.H + C::HBLK - 1) / C::HBLK;
+  p.hblocks = C::hblocks(p.H);
   if (GW) p.ctiles = (p.Wr + C::CSTEP - 1) / C::CSTEP;
   else p.Wr = W, p.ctiles = 1;
   const long long items = (long long)p.B * p.D * p.hblocks * p.ctiles * C::NG;

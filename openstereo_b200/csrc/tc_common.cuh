@@ -111,7 +111,9 @@ __device__ __forceinline__ void wg_mma_split(float (&acc)[2][N / 2], uint64_t da
     wgmma_f16<N>(acc[h], da + h * a_half, db, 1);
   }
 }
-// Consumer-side release of a ring slot / weight buffer read by the wgmmas just waited for: one arrival per warp (barrier count 4).
+// Consumer-side release of a ring slot / weight buffer read by the wgmmas just waited for: one arrival per consumer warp (barrier
+// count 4 x consumer warpgroups).  With two consumer warpgroups, each releases every slot it is handed, including the ones its own
+// tile does not read, and only after waiting for that slot's fill, so neither can arrive on a later phase than the one being filled.
 __device__ __forceinline__ void wg_release(uint64_t* bar, int lane) {
   if (lane == 0) mbar_arrive(bar);
 }
@@ -162,6 +164,25 @@ __device__ __forceinline__ void cp_async_wait() {
 constexpr int TC_BSLOTS = 2;       // weight-slice buffers per kh tap: the producer runs one (kd, chunk) phase ahead of the MMAs
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// Warp roles of the stride-1 kernels (conv3d_tc.cu, conv3d_tcg.cu): 512 threads = two consumer warpgroups (one 128 x 3G
+// accumulator tile each) | one warpgroup of A loaders | one warpgroup of bulk-copy producers (single elected lanes) and idle warps.
+// The CTA starts at 128 registers per thread; setmaxnreg moves them to the consumers: 2 x 128 x 184 + 128 x 112 + 128 x 32 = 65536.
+constexpr int TC_WGS = 2;                 // consumer warpgroups per CTA: each owns one output tile of a work item
+constexpr int TC_CONSUMER_REGS = 184;
+constexpr int TC_LOADER_REGS = 112;
+constexpr int TC_PRODUCER_REGS = 32;
+constexpr int TC_WG_THREADS = 512;
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
 // One lane of a fully converged warp (control flow stays warp-uniform; only the bulk-copy issue is predicated on the elected lane).
 __device__ __forceinline__ bool elect_one() {
