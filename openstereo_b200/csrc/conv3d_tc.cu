@@ -19,20 +19,27 @@
 //   * an operand row is 128 bytes = [32 channels hi | 32 channels lo] fp16, SWIZZLE_128B; a K = 16 MMA step is 32 bytes, so
 //     the hi k-steps sit at descriptor offsets +0, +2 and the lo ones at +4, +6 (16-byte units) of the SAME tile.
 //   * kd taps and 32-channel Cin chunks are phases of one work item; the three kh weight slices of a phase are double-buffered.
-// Work item = (image b, output plane d, output row h): ONE accumulator tile of 128 x 3*Cout fp32, held in the registers of the
-// consumer warpgroup as two m64 halves (96 registers per thread for Cout = 32).  Register capacity is what sets one tile per
-// item: the tile of the next output row cannot be live at the same time, so an input row is staged for every output row it
-// feeds (3 stagings per output row).
+// Work item = (image b, output plane d, output rows 2p and 2p + 1): TWO accumulator tiles of 128 x 3*Cout fp32, one per consumer
+// warpgroup, each held in that warpgroup's registers as two m64 halves (96 registers per thread for Cout = 32).  A phase stages
+// input rows 2p - 1 .. 2p + 2 once and both warpgroups read them: warpgroup t meets phase row r with weight slice kh = r - t
+// (0 <= r - t <= 2), so an input row is staged twice per two output rows instead of three times per output row, and each weight
+// slice a phase streams serves both output rows.
 //
 // Operand staging.  The loader warps read coalesced float4 from global/L2 (or the raw rows a bulk-copy producer staged), convert
 // to the hi/lo fp16 pair, write both halves of the row with the 128-byte swizzle applied by hand (two conflict-free STS.64) and
 // publish the tile to the tensor core through fence.proxy.async + mbarrier.
 //
-// Warp roles (320 threads, 1 CTA/SM, persistent): warps 0-3 = consumer warpgroup (wgmma issue, then the epilogue of the finished
-// tile: registers -> shared staging -> one voxel per thread -> BN/residual/ReLU -> global), warps 4-7 = A-row loaders, warp 8 =
-// weight-slice producer (one elected lane issuing 1-D bulk copies of the pre-swizzled slices into two buffer sets), warp 9 =
-// raw-row producer (bulk copies of whole fp32 input rows ahead of the converters).
+// Warp roles (512 threads, 1 CTA/SM, persistent; setmaxnreg moves the registers, tc_common.cuh): warps 0-7 = two consumer
+// warpgroups (wgmma issue, then the epilogue of the finished tile: registers -> shared staging, 16 output channels per pass ->
+// one voxel per thread -> BN/residual/ReLU -> global), warps 8-11 = A-row loaders, warp 12 = weight-slice producer (one elected
+// lane issuing 1-D bulk copies of the pre-swizzled slices into two buffer sets), warp 13 = raw-row producer (bulk copies of
+// whole fp32 input rows ahead of the converters), warps 14-15 idle.
+//
+// Shared memory (Cout = 32): A ring 4 x 16 KB | weights 2 x 3 x 12 KB | raw rows 2 x 16 KB | per warpgroup a [128][52] fp32
+// staging tile (26 KB) and a seam-exchange buffer (0.75 KB) = 228,352 of the 232,448 bytes a CTA may have.  A full [128][100]
+// staging tile per warpgroup does not fit, so each warpgroup stages its finished tile in two passes of 16 output channels.
 #include <cstdlib>
+#include <type_traits>
 
 #include "tc_common.cuh"
 
@@ -40,12 +47,12 @@ namespace osb {
 
 constexpr int TC_W = 128;          // image width handled (M tile)
 constexpr int TC_KC = 32;          // input channels per phase: 128-byte K-major rows [32 hi | 32 lo] fp16, SWIZZLE_128B
-constexpr int TC_TILES = 1;        // output rows (accumulator tiles) per work item
+constexpr int TC_TILES = TC_WGS;   // output rows (accumulator tiles) per work item: one per consumer warpgroup
 constexpr int TC_ROWS = TC_TILES + 2;
 constexpr int TC_STAGES = 4;       // A-row ring depth (converted fp16 hi|lo tiles)
 constexpr int TC_RAW = 2;          // raw fp32 rows staged by 1-D TMA bulk copies ahead of the converters (Cin = 32 channels-last layers)
 constexpr int TC_ROW_BYTES = TC_W * TC_KC * 4;     // 16384: one staged input row (hi and lo halves of every voxel)
-constexpr int TC_THREADS = 320;
+constexpr int TC_PC = 16;          // output channels per epilogue pass (staged columns per kw block)
 
 struct TcParams {
   const float* x;          // (B, D, H, W, Cin) channels-last
@@ -69,40 +76,66 @@ template <int COUT>
 struct TcCfg {
   static constexpr int N3 = 3 * COUT;                      // kw-stacked MMA N
   static constexpr int B_SLICE = N3 * TC_KC * 4;           // one kh weight slice, rows [hi | lo] (12288 B for Cout = 32)
-  static constexpr int LD = N3 + 4;                        // floats per row of the staged accumulator tile
+  static constexpr int NPASS = COUT / TC_PC;               // epilogue passes: the staging tile holds TC_PC channels of each kw block
+  static constexpr int LD = 3 * TC_PC + 4;                 // floats per row of a staging tile
+  // per warpgroup: seam exchange [6 quadrant slots][2 sides][TC_PC]; slot q + 1 belongs to warp q, slots 0 and 5 stay zero (the
+  // image-edge neighbours), so that one register addresses everything a warp reads and writes there
+  static constexpr int XCHG_FLOATS = 6 * 2 * TC_PC;
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + TC_STAGES * TC_ROW_BYTES;      // [2][3 kh]
   static constexpr int RAW_OFF = B_OFF + TC_BSLOTS * 3 * B_SLICE;    // [TC_RAW] raw fp32 input rows
-  static constexpr int STAGE_OFF = RAW_OFF + TC_RAW * TC_ROW_BYTES;  // [128][LD] fp32 accumulator tile
-  static constexpr int BAR_OFF = STAGE_OFF + 128 * LD * 4;
-  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 256 + 2 * 4 * 2 * COUT * 4 + 3 * COUT * 4;
+  static constexpr int STAGE_OFF = RAW_OFF + TC_RAW * TC_ROW_BYTES;  // [TC_WGS][128][LD] fp32 staging tiles
+  static constexpr int BAR_OFF = STAGE_OFF + TC_WGS * 128 * LD * 4;
+  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 256 + TC_WGS * XCHG_FLOATS * 4 + 2 * COUT * 4;
+  static_assert(COUT % TC_PC == 0, "the epilogue stages whole passes of TC_PC channels");
   static_assert(B_SLICE % 1024 == 0, "weight slices must stay 1024-byte aligned");
-  static_assert(TC_TILES == 1, "the consumer warpgroup holds one accumulator tile");
+  static_assert(32 * LD >= TP_WARP_FLOATS, "store_ndhwc_chunk32 transposes through the warp's own rows of the staging tile");
   static_assert(SMEM <= 232448, "shared memory budget of one CTA exceeded");
 };
 
+// Columns [TC_PC * pass, TC_PC * (pass + 1)) of every kw block of a finished 128 x 3*COUT tile into a [128][LD] staging tile, kw block
+// kw at staged columns TC_PC * kw ..  Fragment layout as in wg_stage (tc_common.cuh): register 4j + r holds column 8j + 2(l%4) + r%2.
+// `pass` must be a compile-time constant after unrolling (it indexes the accumulator registers).
 template <int COUT>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams p) {
+__device__ __forceinline__ void tc_stage_pass(float* stage, const float (&acc)[2][3 * COUT / 2], int pass, int wq, int lane) {
+  constexpr int LD = TcCfg<COUT>::LD;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* r0 = stage + (64 * h + 16 * wq + (lane >> 2)) * LD + 2 * (lane & 3);
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw)
+#pragma unroll
+      for (int jj = 0; jj < TC_PC / 8; ++jj) {
+        const int j = (kw * COUT + pass * TC_PC) / 8 + jj;
+        *reinterpret_cast<float2*>(r0 + TC_PC * kw + 8 * jj) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+        *reinterpret_cast<float2*>(r0 + 8 * LD + TC_PC * kw + 8 * jj) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+      }
+  }
+}
+
+template <int COUT>
+__global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcParams p) {
   using C = TcCfg<COUT>;
   constexpr int N3 = C::N3;
   constexpr int B_SLICE = C::B_SLICE;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  // 1024-byte aligned (SWIZZLE_128B atoms).  Offsetting smem_raw itself, not a round-tripped integer address, keeps every derived
+  // pointer in the shared window: the compiler emits LDS/STS with 32-bit addresses instead of generic 64-bit ones.
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* a_buf = smem + C::A_OFF;
   uint8_t* b_buf = smem + C::B_OFF;
   uint8_t* raw_buf = smem + C::RAW_OFF;
   float* stage = reinterpret_cast<float*>(smem + C::STAGE_OFF);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
-  uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumer   (128 arrivals)
-  uint64_t* a_empty = a_ready + TC_STAGES;          // [STAGES] consumer -> loaders   (4 arrivals: one per consumer warp)
-  uint64_t* b_full = a_empty + TC_STAGES;           // [2][3]   weight producer -> consumer (expect_tx + bulk-copy bytes)
-  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   consumer -> weight producer (4 arrivals)
+  uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumers  (128 arrivals)
+  uint64_t* a_empty = a_ready + TC_STAGES;          // [STAGES] consumers -> loaders  (8 arrivals: one per consumer warp)
+  uint64_t* b_full = a_empty + TC_STAGES;           // [2][3]   weight producer -> consumers (expect_tx + bulk-copy bytes)
+  uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   consumers -> weight producer (8 arrivals)
   uint64_t* raw_full = b_empty + TC_BSLOTS * 3;     // [RAW]    row producer -> converters (expect_tx + bulk-copy bytes, or a plain arrive)
   uint64_t* raw_empty = raw_full + TC_RAW;          // [RAW]    converters -> row producer (128 arrivals)
-  float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 256);   // [2 tile parities][4 warps][2][COUT] boundary exchange
-  float* s_scale = xchg + 2 * 4 * 2 * COUT;                // [COUT]
+  float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 256);   // [TC_WGS][XCHG_FLOATS] boundary exchange
+  float* s_scale = xchg + TC_WGS * C::XCHG_FLOATS;         // [COUT]
   float* s_shift = s_scale + COUT;
-  float* zeros = s_shift + COUT;                           // [COUT] of 0.f (image-edge neighbours)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nchunk = p.Cin / TC_KC;
@@ -110,11 +143,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_STAGES; ++s) {
       mbar_init(&a_ready[s], 128);
-      mbar_init(&a_empty[s], 4);
+      mbar_init(&a_empty[s], 4 * TC_WGS);
     }
     for (int k = 0; k < TC_BSLOTS * 3; ++k) {
       mbar_init(&b_full[k], 1);
-      mbar_init(&b_empty[k], 4);
+      mbar_init(&b_empty[k], 4 * TC_WGS);
     }
     for (int k = 0; k < TC_RAW; ++k) {
       mbar_init(&raw_full[k], 1);
@@ -125,8 +158,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
   for (int c = threadIdx.x; c < COUT; c += blockDim.x) {
     s_scale[c] = p.scale ? p.scale[c] : 1.f;
     s_shift[c] = p.shift ? p.shift[c] : 0.f;
-    zeros[c] = 0.f;
   }
+  for (int i = threadIdx.x; i < TC_WGS * C::XCHG_FLOATS; i += blockDim.x) xchg[i] = 0.f;
   __syncthreads();
   // The rows a CTA stages form one flat sequence (item, kd, chunk, r).  `RowIter` walks it; loads run TWO rows ahead of
   // the stores (software pipeline in registers) so that a full L2/HBM round trip is always in flight.
@@ -152,33 +185,43 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
       s.kd = (d2 == 0) ? 1 : 0;                     // first input plane that exists
     }
   };
-  // ---------------------------------------------------------------------------------------------- consumer warpgroup
-  if (warp < 4) {
+  // ---------------------------------------------------------------------------------------------- consumer warpgroups
+  // Warpgroup wg accumulates output row 2p + wg of the item from the rows and weight slices both warpgroups read, then runs the
+  // epilogue of that row.
+  if (warp < 4 * TC_WGS) {
+    setmaxnreg_inc<TC_CONSUMER_REGS>();
+    const int wg = warp >> 2;
+    stage += wg * 128 * C::LD;
+    xchg += wg * C::XCHG_FLOATS;
+    const int bar_stage = 1 + 2 * wg, bar_xchg = 2 + 2 * wg;   // this warpgroup's named barriers
     constexpr uint32_t LO = TcK<TC_KC>::LO_OFF;     // descriptor offset of the lo half of an operand row
     constexpr uint32_t A_HALF = 64 * TC_KC * 4 / 16;  // descriptor offset of operand rows 64..127
     const uint64_t dbase = desc_sw128_base();
     // Descriptors differ only in their 14-bit start-address field (bits 0-13, units of 16 bytes).
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
-    const int q = warp;                              // epilogue: this warp owns tile rows 32q .. 32q + 31
+    const int q = warp & 3;                          // epilogue: this warp owns tile rows 32q .. 32q + 31
     const int m = q * 32 + lane;                     // voxel (image column) owned by this thread
-    uint32_t rowc = 0, phc = 0, tilec = 0;
+    uint32_t rowc = 0, phc = 0;
     for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
-      {
-        const int d = (it / p.hblocks) % p.D;
-        float acc[2][N3 / 2];
-        uint32_t accum = 0;
-        for (int kd = 0; kd < 3; ++kd) {
-          const int din = d + kd - 1;
-          if (din < 0 || din >= p.D) continue;
-          for (int ch = 0; ch < nchunk; ++ch, ++phc) {
-            const uint32_t bslot = (phc & 1) * 3;   // weight buffers alternate between phases
+      const int d = (it / p.hblocks) % p.D;
+      float acc[2][N3 / 2];
+      uint32_t accum = 0;
+      for (int kd = 0; kd < 3; ++kd) {
+        const int din = d + kd - 1;
+        if (din < 0 || din >= p.D) continue;
+        for (int ch = 0; ch < nchunk; ++ch, ++phc) {
+          const uint32_t bslot = (phc & 1) * 3;     // weight buffers alternate between phases
 #pragma unroll
-            for (int r = 0; r < TC_ROWS; ++r) {     // one output row: input row r of the phase meets weight slice kh = r
-              const uint32_t s = rowc % TC_STAGES, par = (rowc / TC_STAGES) & 1;
-              mbar_wait(&a_ready[s], par);
-              mbar_wait(&b_full[bslot + r], (phc >> 1) & 1);
+          for (int r = 0; r < TC_ROWS; ++r) {
+            // Every warpgroup waits for each row's fill and releases it, including the row its own tile does not read, so neither
+            // can arrive on a later phase of a slot than the one being filled.
+            const uint32_t s = rowc % TC_STAGES, par = (rowc / TC_STAGES) & 1;
+            mbar_wait(&a_ready[s], par);
+            const int kh = r - wg;                  // input row r of the phase meets weight slice kh for output row 2p + wg
+            if (kh >= 0 && kh < 3) {
+              mbar_wait(&b_full[bslot + kh], (phc >> 1) & 1);
               const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + s * TC_ROW_BYTES) & 0x3FFFF) >> 4);
-              const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot + r) * (B_SLICE / 16));
+              const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot + kh) * (B_SLICE / 16));
               wg_fence();
 #pragma unroll
               for (int ks = 0; ks < TcK<TC_KC>::KSTEPS; ++ks)
@@ -186,214 +229,230 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
               wg_commit();
               wg_wait_all();
               accum = 1;
-              wg_release(&a_empty[s], lane);        // ring slot and weight slice are free once these MMAs have read them
-              wg_release(&b_empty[bslot + r], lane);
-              ++rowc;
+              wg_release(&b_empty[bslot + kh], lane);   // the weight slice is free once these MMAs have read it
             }
+            wg_release(&a_empty[s], lane);
+            ++rowc;
           }
         }
-        named_bar_sync(2, 128);                      // every warp is done with the previous tile's staged rows
-        wg_stage<N3>(stage, C::LD, acc, warp, lane);
-        named_bar_sync(2, 128);
       }
-      const int hb = it % p.hblocks;
-      const int d = (it / p.hblocks) % p.D;
-      const int b = it / (p.hblocks * p.D);
-      const int h0 = hb * TC_TILES;
-      const int ntiles = min(TC_TILES, p.H - h0);
+      // A tile below the image (odd H) received its MMAs and releases like any other and stores nothing.  The branch is
+      // warpgroup-uniform and the epilogue's barriers are this warpgroup's own.
+      const int h = (it % p.hblocks) * TC_TILES + wg;
+      if (h >= p.H) continue;
       // MMAs each P_kw accumulator received: (existing kd planes) x chunks x 3 kh x k-steps x 3 split terms
       const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * TcK<TC_KC>::KSTEPS * 3);
-      // D[m] = P0[m-1] + P1[m] + P2[m+1], from the staged tile
-      for (int t = 0; t < ntiles; ++t) {           // ntiles == TC_TILES == 1
-        const int h = h0 + t;
-        const size_t vox = (((size_t)b * p.D + d) * p.H + h) * TC_W + m;           // NDHWC voxel index
-        const size_t plane = (size_t)p.D * p.H * TC_W;                             // NCDHW channel stride
-        const size_t ncdhw0 = (size_t)b * p.Cout * plane + ((size_t)d * p.H + h) * TC_W + m;   // p.Cout <= COUT real channels
-        // all 3*COUT accumulator columns of this voxel from the staged tile
-        uint32_t raw[3][COUT];
+      // D[m] = P0[m-1] + P1[m] + P2[m+1], from the staged tile, TC_PC channels per pass
+      float out[COUT];
 #pragma unroll
-        for (int kw = 0; kw < 3; ++kw)
-#pragma unroll
-          for (int c0 = 0; c0 < COUT; c0 += 16) stage_ld16(stage + m * C::LD + kw * COUT + c0, &raw[kw][c0]);
-        // lanes at the warp edges need the neighbour quadrant's values: exchange through shared memory (double-buffered
-        // by tile parity so one named barrier per tile suffices)
-        float* xb = xchg + (tilec & 1) * (4 * 2 * COUT);
-        ++tilec;                                      // running tile count: consecutive tiles never share a buffer
+      for (int pass = 0; pass < C::NPASS; ++pass) {
+        named_bar_sync(bar_stage, 128);              // every warp is done with the rows staged before (previous pass or tile)
+        tc_stage_pass<COUT>(stage, acc, pass, q, lane);
+        named_bar_sync(bar_stage, 128);
+        const float* srow = stage + m * C::LD;       // [P0 | P1 | P2] of this pass's channels
+        // lanes at the warp edges need the neighbour quadrant's values: exchange through shared memory.  One buffer suffices: its
+        // readers of the previous pass passed bar_stage above before any writer of this pass did.
+        float* xq = xchg + (q + 1) * 2 * TC_PC;      // this warp's slot: [P0 of its last column | P2 of its first column]
         if (lane == 31) {
 #pragma unroll
-          for (int i = 0; i < COUT; ++i) xb[(q * 2) * COUT + i] = __uint_as_float(raw[0][i]);
+          for (int i = 0; i < TC_PC; i += 4)
+            *reinterpret_cast<float4*>(xq + i) = *reinterpret_cast<const float4*>(srow + i);
         }
         if (lane == 0) {
 #pragma unroll
-          for (int i = 0; i < COUT; ++i) xb[(q * 2 + 1) * COUT + i] = __uint_as_float(raw[2][i]);
+          for (int i = 0; i < TC_PC; i += 4)
+            *reinterpret_cast<float4*>(xq + TC_PC + i) = *reinterpret_cast<const float4*>(srow + 2 * TC_PC + i);
         }
-        named_bar_sync(1, 128);
-        const float* xl = (q > 0) ? xb + ((q - 1) * 2) * COUT : zeros;
-        const float* xr = (q < 3) ? xb + ((q + 1) * 2 + 1) * COUT : zeros;
-        float out[COUT];
+        named_bar_sync(bar_xchg, 128);
+        const float* xl = xq - 2 * TC_PC;            // P0 of the previous quadrant's last column (zero slot at the image edge)
+        const float* xr = xq + 3 * TC_PC;            // P2 of the next quadrant's first column
         // The neighbour-quadrant values are loaded UNCONDITIONALLY (warp-uniform addresses: broadcast LDS.128) and merged with
         // selects: the `lane == 0 ? xl[i] : left` form compiles to a branch around a load per element.
 #pragma unroll
-        for (int i0 = 0; i0 < COUT; i0 += 4) {
+        for (int i0 = 0; i0 < TC_PC; i0 += 4) {
           const float4 l4 = *reinterpret_cast<const float4*>(xl + i0);
           const float4 r4 = *reinterpret_cast<const float4*>(xr + i0);
+          const float4 p04 = *reinterpret_cast<const float4*>(srow + i0);
+          const float4 p14 = *reinterpret_cast<const float4*>(srow + TC_PC + i0);
+          const float4 p24 = *reinterpret_cast<const float4*>(srow + 2 * TC_PC + i0);
           const float le[4] = {l4.x, l4.y, l4.z, l4.w}, re[4] = {r4.x, r4.y, r4.z, r4.w};
+          const float p0[4] = {p04.x, p04.y, p04.z, p04.w}, p1[4] = {p14.x, p14.y, p14.z, p14.w}, p2[4] = {p24.x, p24.y, p24.z, p24.w};
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
-            const int i = i0 + k;
-            float left = __shfl_up_sync(0xffffffffu, __uint_as_float(raw[0][i]), 1);
-            float right = __shfl_down_sync(0xffffffffu, __uint_as_float(raw[2][i]), 1);
+            float left = __shfl_up_sync(0xffffffffu, p0[k], 1);
+            float right = __shfl_down_sync(0xffffffffu, p2[k], 1);
             left = (lane == 0) ? le[k] : left;        // m-1 lives in the previous quadrant (zero at the image edge)
             right = (lane == 31) ? re[k] : right;     // m+1 lives in the next quadrant
-            out[i] = ((left + __uint_as_float(raw[1][i])) + right) * corr;
+            out[pass * TC_PC + i0 + k] = ((left + p1[k]) + right) * corr;
           }
         }
-        if constexpr (COUT == 32) {
-          if (p.out_ndhwc && (!p.residual || p.res_ndhwc)) {     // coalesced channels-last path (BN/residual/act inside)
-            store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, out, p.y + (vox - lane) * COUT,
-                                p.residual ? p.residual + (vox - lane) * COUT : nullptr, COUT, s_scale, s_shift, p.act);
-            continue;
+      }
+      const int b = it / (p.hblocks * p.D);
+      const size_t vox = (((size_t)b * p.D + d) * p.H + h) * TC_W + m;             // NDHWC voxel index
+      const size_t plane = (size_t)p.D * p.H * TC_W;                               // NCDHW channel stride
+      const size_t ncdhw0 = (size_t)b * p.Cout * plane + ((size_t)d * p.H + h) * TC_W + m;   // p.Cout <= COUT real channels
+      if constexpr (COUT == 32) {
+        if (p.out_ndhwc && (!p.residual || p.res_ndhwc)) {     // coalesced channels-last path (BN/residual/act inside)
+          store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, out, p.y + (vox - lane) * COUT,
+                              p.residual ? p.residual + (vox - lane) * COUT : nullptr, COUT, s_scale, s_shift, p.act);
+          continue;
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < COUT; ++i) out[i] = fmaf(out[i], s_scale[i], s_shift[i]);
+      if (p.residual) {
+        if (p.res_ndhwc) {
+          const float4* rp = reinterpret_cast<const float4*>(p.residual + vox * COUT);
+#pragma unroll
+          for (int i = 0; i < COUT / 4; ++i) {
+            const float4 rv = __ldg(rp + i);
+            out[4 * i] += rv.x, out[4 * i + 1] += rv.y, out[4 * i + 2] += rv.z, out[4 * i + 3] += rv.w;
           }
-        }
-#pragma unroll
-        for (int i = 0; i < COUT; ++i) out[i] = fmaf(out[i], s_scale[i], s_shift[i]);
-        if (p.residual) {
-          if (p.res_ndhwc) {
-            const float4* rp = reinterpret_cast<const float4*>(p.residual + vox * COUT);
-#pragma unroll
-            for (int i = 0; i < COUT / 4; ++i) {
-              const float4 rv = __ldg(rp + i);
-              out[4 * i] += rv.x, out[4 * i + 1] += rv.y, out[4 * i + 2] += rv.z, out[4 * i + 3] += rv.w;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < COUT; ++i)
-              if (i < p.Cout) out[i] += __ldg(p.residual + ncdhw0 + (size_t)i * plane);
-          }
-        }
-        if (p.act == OSB_ACT_RELU) {
-#pragma unroll
-          for (int i = 0; i < COUT; ++i) out[i] = fmaxf(out[i], 0.f);
-        } else if (p.act == OSB_ACT_LEAKY) {
-#pragma unroll
-          for (int i = 0; i < COUT; ++i) out[i] = out[i] > 0.f ? out[i] : 0.01f * out[i];
-        }
-        if (p.out_ndhwc) {
-          float4* yp = reinterpret_cast<float4*>(p.y + vox * COUT);
-#pragma unroll
-          for (int i = 0; i < COUT / 4; ++i) yp[i] = make_float4(out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
         } else {
 #pragma unroll
           for (int i = 0; i < COUT; ++i)
-            if (i < p.Cout) p.y[ncdhw0 + (size_t)i * plane] = out[i];                 // 128-byte rows per warp
+            if (i < p.Cout) out[i] += __ldg(p.residual + ncdhw0 + (size_t)i * plane);
         }
+      }
+      if (p.act == OSB_ACT_RELU) {
+#pragma unroll
+        for (int i = 0; i < COUT; ++i) out[i] = fmaxf(out[i], 0.f);
+      } else if (p.act == OSB_ACT_LEAKY) {
+#pragma unroll
+        for (int i = 0; i < COUT; ++i) out[i] = out[i] > 0.f ? out[i] : 0.01f * out[i];
+      }
+      if (p.out_ndhwc) {
+        float4* yp = reinterpret_cast<float4*>(p.y + vox * COUT);
+#pragma unroll
+        for (int i = 0; i < COUT / 4; ++i) yp[i] = make_float4(out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
+      } else {
+#pragma unroll
+        for (int i = 0; i < COUT; ++i)
+          if (i < p.Cout) p.y[ncdhw0 + (size_t)i * plane] = out[i];                 // 128-byte rows per warp
       }
     }
   }
   // ---------------------------------------------------------------------------------------------- A-row loaders
-  else if (warp < 8) {
-    const int lt = threadIdx.x - 128;                // 0..127
+  else if (warp < 4 * TC_WGS + 4) {
+    setmaxnreg_dec<TC_LOADER_REGS>();
+    const int lt = threadIdx.x - 4 * TC_WGS * 32;    // 0..127
     const int vsel = lt >> 3, c16 = lt & 7;          // this thread's voxel (mod 16) and fp32 16-byte chunk of the 32-channel slice
     // voxel order inside a half-warp alternates bit 2 of the column so that the STS.64 pairs of stage_f16_split hit disjoint banks
     const int vcol = ((vsel & 1) << 2) | ((vsel >> 1) & 3) | (vsel & 8);
     float amax = 0.f;
-    const size_t row_stride = (size_t)TC_W * p.Cin;  // floats per image row
-    auto load_row = [&](const RowIter& s, float4 (&v)[8]) {
-      const int hb = s.it % p.hblocks;
-      const int d = (s.it / p.hblocks) % p.D;
-      const int b = s.it / (p.hblocks * p.D);
-      const int hin = hb * TC_TILES - 1 + s.r, din = d + s.kd - 1;
-      if (hin >= 0 && hin < p.H && p.in_ncdhw) {
-        // NCDHW input: this thread stages voxel (column) lt for all eight channel quads; every LDG.32 of a warp is one
-        // contiguous 128-byte row segment of a channel plane.  v[j] holds channels 4*qj .. 4*qj+3, qj = j ^ ((lt >> 3) & 1)
-        // (the swap keeps the STS.64 of lanes 8 apart -- same swizzled chunk -- on different 8-byte halves).
-        const size_t plane = (size_t)p.D * p.H * TC_W;
-        const float* src = p.x + (((size_t)b * p.Cin + s.ch * TC_KC) * p.D + din) * p.H * TC_W + (size_t)hin * TC_W + lt;
+    // The two input layouts run separate copies of the loops below (NCDHW is a compile-time flag), so that each copy keeps only
+    // its own layout's swizzled store offsets live: both fit the loaders' register budget (TC_LOADER_REGS) without spilling.
+    auto run = [&](auto in_ncdhw) {
+      constexpr bool NCDHW = decltype(in_ncdhw)::value;
+      const size_t row_stride = (size_t)TC_W * p.Cin;  // floats per image row
+      auto load_row = [&](const RowIter& s, float4 (&v)[8]) {
+        const int hb = s.it % p.hblocks;
+        const int d = (s.it / p.hblocks) % p.D;
+        const int b = s.it / (p.hblocks * p.D);
+        const int hin = hb * TC_TILES - 1 + s.r, din = d + s.kd - 1;
+        if (hin >= 0 && hin < p.H && NCDHW) {
+          // NCDHW input: this thread stages voxel (column) lt for all eight channel quads; every LDG.32 of a warp is one
+          // contiguous 128-byte row segment of a channel plane.  v[j] holds channels 4*qj .. 4*qj+3, qj = j ^ ((lt >> 3) & 1)
+          // (the swap keeps the STS.64 of lanes 8 apart -- same swizzled chunk -- on different 8-byte halves).
+          const size_t plane = (size_t)p.D * p.H * TC_W;
+          const float* src = p.x + (((size_t)b * p.Cin + s.ch * TC_KC) * p.D + din) * p.H * TC_W + (size_t)hin * TC_W + lt;
+          // channels in plane order (one running address), then the quad swap as register selects
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float* q = src + (size_t)(4 * (j ^ ((lt >> 3) & 1))) * plane;
-          v[j] = make_float4(__ldg(q), __ldg(q + plane), __ldg(q + 2 * plane), __ldg(q + 3 * plane));
-        }
-      } else if (hin >= 0 && hin < p.H) {             // rows outside the image are the conv's zero padding
-        const float* src = p.x + (((size_t)b * p.D + din) * p.H + hin) * row_stride + s.ch * TC_KC + c16 * 4;
+          for (int j = 0; j < 8; ++j, src += 4 * plane)
+            v[j] = make_float4(__ldg(src), __ldg(src + plane), __ldg(src + 2 * plane), __ldg(src + 3 * plane));
+          const bool swap = (lt >> 3) & 1;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = __ldg(reinterpret_cast<const float4*>(src + (size_t)(vcol + 16 * j) * p.Cin));
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    };
-    uint32_t rowc = 0;
-    auto store_row = [&](const float4 (&v)[8]) {
-      const uint32_t s = rowc % TC_STAGES, par = (rowc / TC_STAGES) & 1;
-      mbar_wait_relaxed(&a_empty[s], par ^ 1);        // the MMAs that read this slot last time have completed
-      uint8_t* tile = a_buf + s * TC_ROW_BYTES;
-      if (p.in_ncdhw) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) stage_f16_split<TC_KC>(tile, lt, j ^ ((lt >> 3) & 1), v[j], amax);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) stage_f16_split<TC_KC>(tile, vcol + 16 * j, c16, v[j], amax);   // tile row = image column
-      }
-      fence_proxy_async();                            // generic-proxy writes -> visible to the tensor core (async proxy)
-      mbar_arrive(&a_ready[s]);
-      ++rowc;
-    };
-    RowIter ld{(int)blockIdx.x, 0, 0, -1};
-    if (ld.it < p.items) ld.kd = (((ld.it / p.hblocks) % p.D) == 0) ? 1 : 0;
-    if (p.bulk_rows) {
-      // The row producer (warp 9) keeps TC_RAW rows of raw fp32 in flight with 16 KB TMA bulk copies; these four warps only
-      // convert: LDS.128 (a warp reads 512 contiguous bytes) -> fp16 hi|lo -> swizzled STS.64.  No load latency on this path.
-      uint32_t rawc = 0;
-      while (advance(ld)) {
-        const int hb = ld.it % p.hblocks;
-        const int hin = hb * TC_TILES - 1 + ld.r;
-        const uint32_t slot = rawc % TC_RAW, par = (rawc / TC_RAW) & 1;
-        mbar_wait_relaxed(&raw_full[slot], par);
-        float4 v[8];
-        if (hin >= 0 && hin < p.H && p.in_ncdhw) {    // raw slot = [32 channels][128 columns]: this thread's column, 8 channel quads
-          const float* src = reinterpret_cast<const float*>(raw_buf + slot * TC_ROW_BYTES) + lt;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float* q = src + 4 * (j ^ ((lt >> 3) & 1)) * TC_W;
-            v[j] = make_float4(q[0], q[TC_W], q[2 * TC_W], q[3 * TC_W]);
+          for (int j = 0; j < 8; j += 2) {
+            const float4 e = v[j], o = v[j + 1];
+            v[j] = swap ? o : e;
+            v[j + 1] = swap ? e : o;
           }
-        } else if (hin >= 0 && hin < p.H) {
-          const float* src = reinterpret_cast<const float*>(raw_buf + slot * TC_ROW_BYTES) + c16 * 4;
+        } else if (hin >= 0 && hin < p.H) {             // rows outside the image are the conv's zero padding
+          const float* src = p.x + (((size_t)b * p.D + din) * p.H + hin) * row_stride + s.ch * TC_KC + c16 * 4 + vcol * p.Cin;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const float4*>(src + (vcol + 16 * j) * TC_KC);
+          for (int j = 0; j < 8; ++j) v[j] = __ldg(reinterpret_cast<const float4*>(src + 16 * j * p.Cin));
         } else {
 #pragma unroll
           for (int j = 0; j < 8; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        store_row(v);                                 // consumes v: the reads of the raw slot are complete behind it
-        mbar_arrive(&raw_empty[slot]);
-        ++rawc;
+      };
+      uint32_t rowc = 0;
+      auto store_row = [&](const float4 (&v)[8]) {
+        const uint32_t s = rowc % TC_STAGES, par = (rowc / TC_STAGES) & 1;
+        mbar_wait_relaxed(&a_empty[s], par ^ 1);        // the MMAs that read this slot last time have completed
+        uint8_t* tile = a_buf + s * TC_ROW_BYTES;
+        if (NCDHW) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) stage_f16_split<TC_KC>(tile, lt, j ^ ((lt >> 3) & 1), v[j], amax);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) stage_f16_split<TC_KC>(tile, vcol + 16 * j, c16, v[j], amax);   // tile row = image column
+        }
+        fence_proxy_async();                            // generic-proxy writes -> visible to the tensor core (async proxy)
+        mbar_arrive(&a_ready[s]);
+        ++rowc;
+      };
+      RowIter ld{(int)blockIdx.x, 0, 0, -1};
+      if (ld.it < p.items) ld.kd = (((ld.it / p.hblocks) % p.D) == 0) ? 1 : 0;
+      if (p.bulk_rows) {
+        // The row producer (warp 13) keeps TC_RAW rows of raw fp32 in flight with 16 KB TMA bulk copies; these four warps only
+        // convert: LDS.128 (a warp reads 512 contiguous bytes) -> fp16 hi|lo -> swizzled STS.64.  No load latency on this path.
+        uint32_t rawc = 0;
+        while (advance(ld)) {
+          const int hb = ld.it % p.hblocks;
+          const int hin = hb * TC_TILES - 1 + ld.r;
+          const uint32_t slot = rawc % TC_RAW, par = (rawc / TC_RAW) & 1;
+          mbar_wait_relaxed(&raw_full[slot], par);
+          float4 v[8];
+          if (hin >= 0 && hin < p.H && NCDHW) {    // raw slot = [32 channels][128 columns]: this thread's column, 8 channel quads
+            const float* src = reinterpret_cast<const float*>(raw_buf + slot * TC_ROW_BYTES) + lt;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const float* q = src + 4 * (j ^ ((lt >> 3) & 1)) * TC_W;
+              v[j] = make_float4(q[0], q[TC_W], q[2 * TC_W], q[3 * TC_W]);
+            }
+          } else if (hin >= 0 && hin < p.H) {
+            const float* src = reinterpret_cast<const float*>(raw_buf + slot * TC_ROW_BYTES) + c16 * 4;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const float4*>(src + (vcol + 16 * j) * TC_KC);
+          } else {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+          }
+          store_row(v);                                 // consumes v: the reads of the raw slot are complete behind it
+          mbar_arrive(&raw_empty[slot]);
+          ++rawc;
+        }
+        tc_report_overflow(p.overflow, amax);
+        amax = 0.f;
+      }
+      float4 va[8], vb[8];
+      bool has_a = !p.bulk_rows && advance(ld);
+      if (has_a) load_row(ld, va);
+      bool has_b = has_a && advance(ld);
+      if (has_b) load_row(ld, vb);
+      while (has_a) {
+        store_row(va);
+        has_a = has_b && advance(ld);
+        if (has_a) load_row(ld, va);
+        if (!has_b) break;
+        store_row(vb);
+        has_b = has_a && advance(ld);
+        if (has_b) load_row(ld, vb);
       }
       tc_report_overflow(p.overflow, amax);
-      amax = 0.f;
-    }
-    float4 va[8], vb[8];
-    bool has_a = !p.bulk_rows && advance(ld);
-    if (has_a) load_row(ld, va);
-    bool has_b = has_a && advance(ld);
-    if (has_b) load_row(ld, vb);
-    while (has_a) {
-      store_row(va);
-      has_a = has_b && advance(ld);
-      if (has_a) load_row(ld, va);
-      if (!has_b) break;
-      store_row(vb);
-      has_b = has_a && advance(ld);
-      if (has_b) load_row(ld, vb);
-    }
-    tc_report_overflow(p.overflow, amax);
+    };
+    if (p.in_ncdhw) run(std::true_type{});
+    else run(std::false_type{});
   }
-  // ---------------------------------------------------------------------------------------------- weight-slice producer
-  // One elected lane streams the pre-swizzled (kd, chunk, kh) slices with 1-D bulk copies into the two buffer sets; it runs up
-  // to a whole phase ahead of the MMAs.
-  else if (warp == 8) {
-    if (elect_one()) {
+  // ---------------------------------------------------------------------------------------------- producer warpgroup
+  // Warp 12 is the weight-slice producer, warp 13 the raw-row producer (bulk-copied input rows only); warps 14-15 are idle and
+  // only hand their registers back.
+  else {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    // weight-slice producer: one elected lane streams the pre-swizzled (kd, chunk, kh) slices with 1-D bulk copies into the two
+    // buffer sets; it runs up to a whole phase ahead of the MMAs.
+    if (warp == 4 * TC_WGS + 4 && elect_one()) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.w);
       uint32_t phc = 0;
       for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
@@ -413,11 +472,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv3d_tc_kernel(const TcParams
         }
       }
     }
-    __syncwarp();
-  }
-  // ---------------------------------------------------------------------------------------------- raw-row producer
-  else if (warp == 9 && p.bulk_rows) {
-    if (elect_one()) {
+    // raw-row producer: bulk copies of whole fp32 input rows, TC_RAW ahead of the converters
+    else if (warp == 4 * TC_WGS + 5 && p.bulk_rows && elect_one()) {
       RowIter ld{(int)blockIdx.x, 0, 0, -1};
       if (ld.it < p.items) ld.kd = (((ld.it / p.hblocks) % p.D) == 0) ? 1 : 0;
       uint32_t rawc = 0;
@@ -487,7 +543,7 @@ static int launch_tc(const TcParams& p, cudaStream_t stream) {
   const int grid = (int)cap_persistent_grid(p.items < sms ? p.items : sms);   // persistent: one CTA per SM (its shared memory is taken)
   static const std::string variant = tc_variant_name("tc<%d>", COUT);
   set_tc_variant(variant.c_str());
-  kernel<<<grid, TC_THREADS, smem, stream>>>(p);
+  kernel<<<grid, TC_WG_THREADS, smem, stream>>>(p);
   count_launch();
   return check_launch("conv3d_tc_kernel");
 }
