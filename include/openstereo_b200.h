@@ -276,6 +276,18 @@ int osb_warped_concat_volume_fwd(const float* x, const float* y, const float* di
 int osb_warped_gwc_concat_volume_fwd(const float* xg, const float* yg, const float* xc, const float* yc, const float* disp,
                                      float* out, int B, int Cg, int G, int Cc, int D, int H, int W, osb_stream_t stream);
 
+/* ---- CoEx (coex/coex_disp_processor.py:8-65, coex/coex_cost_processor.py:219-224) -------------------------------------------
+ * osb_coex_regression_fwd: Regression.forward (eval) + upfeat in one launch: cost (B,1,D,h,w) logits, spx (B,9,4h,4w) ->
+ *   out (B,4h,4w).  Per low-resolution pixel the top_k largest logits along D (2 <= top_k <= 8, top_k <= D; among equal values
+ *   the lower index first, like the reference's stable descending sort), their softmax and disp_4 = sum_j p_j * index_j; then
+ *   out[b,Y,X] = 4 * sum_{t<9} disp_4[b, Y/4 + t/3 - 1, X/4 + t%3 - 1] * p_t[b,Y,X] with zero outside the image.
+ *   spx_is_logits = 1: p = softmax of spx over its 9 channels; 0: spx already holds the probabilities.  spx and out 16-byte aligned.
+ * osb_nearest_resize3d_fwd: F.interpolate(x, size=(Do,Ho,Wo), mode='nearest') on N = B*C planes (Di,Hi,Wi) -> (Do,Ho,Wo), with
+ *   aten's source index per dimension (dst; dst >> 1 when out = 2*in; else min(floor(dst * ((float)in / out)), in - 1)). */
+int osb_coex_regression_fwd(const float* cost, const float* spx, float* out, int B, int D, int h, int w, int top_k, int spx_is_logits,
+                            osb_stream_t stream);
+int osb_nearest_resize3d_fwd(const float* x, float* y, int N, int Di, int Hi, int Wi, int Do, int Ho, int Wo, osb_stream_t stream);
+
 /* Backward (adjoint) kernels so the volume constructors and the soft-argmin stay differentiable under tools/train.py
  * (openstereo_b200/autograd.py wraps them in torch.autograd.Function).  grad_ref / grad_tgt may be NULL when not needed.
  *   osb_gwc_volume_bwd     adjoint of osb_gwc_volume_fwd (reduce_sum = 0) / osb_gwc_volume_sum_fwd (1): grad_vol (B,G,D,H,W)

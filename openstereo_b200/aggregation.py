@@ -13,6 +13,7 @@ Graphs restated (file:line of the reference forward each engine replaces):
   PSMAggregation        psmnet/psmnet_cost_processor.py:181-221,108-132 + psmnet_disp_processor.py:107-118
   StereoBaseAggregation stereobase/hourglass.py:79-104 + stereobase_gru.py:161-164
   LightStereoAggregation lightstereo/aggregation.py:42-60 (Aggregation.forward), :94-101 (MobileV2Residual), :119-134 (AttentionModule)
+  CoExAggregation       coex/coex_cost_processor.py:196-237 (Aggregation.forward), :68-80 (channelAtt)
 """
 import torch
 
@@ -638,6 +639,80 @@ class StereoBaseCostHead(_Engine):
         else:
             logits = _conv(lay, geo)                            # (B,1,D',H',W')
         return ops.softargmin(logits.squeeze(1), maxdisp_lowres, keepdim=True)
+
+
+# -------------------------------------------------------------------------------------------------------- CoEx
+def _basic_conv(m):
+    """CoEx's BasicConv (coex/submodule.py): conv, then its BN only when use_bn, then LeakyReLU only when relu -> (_Packed, act)."""
+    if m.relu and m.LeakyReLU.negative_slope != 0.01:
+        raise NotImplementedError("openstereo_b200: LeakyReLU slope %g (the kernels apply 0.01)" % m.LeakyReLU.negative_slope)
+    return _Packed(m.conv, m.bn if m.use_bn else None), ACT_LEAKY if m.relu else ACT_NONE
+
+
+class _ChannelAtt:
+    """channelAtt.im_att (coex_cost_processor.py:68-80): image features (B,Cim,H,W) -> sigmoid gate (B,Ccv,H,W), applied by
+    the epilogue of the conv the reference multiplies it into."""
+
+    def __init__(self, m):
+        self.a, self.act = _basic_conv(m.im_att[0])
+        self.b = _Packed(m.im_att[1])
+
+    def __call__(self, im):
+        hidden = ops.conv3d_1x1(im, self.a.w, self.a.scale, self.a.shift, act=self.act)
+        return ops.conv3d_1x1(hidden, self.b.w, self.b.scale, self.b.shift, sigmoid_out=True)
+
+
+class CoExAggregation(_Engine):
+    """Eval forward of CoEx's Aggregation (coex_cost_processor.py:196-237): cost (B, head, D, h, w) and the image features ->
+    logits (B, 1, D, h, w).  Every conv runs on the fp32 CUDA-core kernels; each channelAtt gate rides on the epilogue of the conv
+    it follows; each conv_skip is a 1x1 conv over (up, skip) without the concatenation; where a transposed conv's output is larger
+    than its skip level (an odd extent below it), nearest_resize3d brings it back like the reference's F.interpolate.
+    conv_skip[0], conv_agg[0] and channelAtt[0] are never used by the forward and are not read."""
+
+    def _pack(self):
+        m = self.module
+        self.gce = bool(m.gce)
+        self.down = [[_basic_conv(c) for c in seq] for seq in m.conv_down]
+        self.up = [_basic_conv(c) for c in m.conv_up]
+        self.stem = _basic_conv(m.conv_stem)
+        # indexed like the reference's up path: step i uses conv_skip[-i-1], conv_agg[-i-1], channelAtt[-i-1] for i = 0, 1
+        self.skip = [_basic_conv(m.conv_skip[-i - 1]) for i in range(2)]
+        self.agg = [[_basic_conv(c) for c in m.conv_agg[-i - 1]] for i in range(2)]
+        if self.gce:
+            self.att_stem = _ChannelAtt(m.channelAttStem)
+            self.att_down = [_ChannelAtt(a) for a in m.channelAttDown]
+            self.att = [_ChannelAtt(m.channelAtt[-i - 1]) for i in range(2)]
+
+    def _seq(self, layers, x, att, im):
+        """A chain of BasicConvs; the channelAtt gate (when gce) rides on the last one."""
+        for n, (layer, act) in enumerate(layers):
+            gate = att(im) if self.gce and n == len(layers) - 1 else None
+            x = _conv(layer, x, act, gate=gate)
+        return x
+
+    def __call__(self, img, cost):
+        cost = self._check(cost)
+        self._ensure(cost.device)
+        img = [self._check(f) for f in img]
+        b, _, h, w = img[0].shape
+        x = cost.reshape(b, -1, self.module.D, h, w)
+        x = self._seq([self.stem], x, getattr(self, "att_stem", None), img[0])
+        levels = [x]
+        for i in range(3):
+            x = self._seq(self.down[i], x, self.att_down[i] if self.gce else None, img[i + 1])
+            levels.append(x)
+        for i in range(3):
+            layer, act = self.up[-i - 1]
+            x = ops.deconv3d(x, layer.w, layer.scale, layer.shift, None, layer.kernel, act)
+            skip = levels[-i - 2]
+            if x.shape[2:] != skip.shape[2:]:
+                x = ops.nearest_resize3d(x, skip.shape[2:])
+            if i == 2:
+                break
+            sl, sa = self.skip[i]
+            x = ops.conv3d_1x1(x, sl.w, sl.scale, sl.shift, act=sa, x1=skip)
+            x = self._seq(self.agg[i], x, self.att[i] if self.gce else None, img[-i - 2])
+        return x
 
 
 # -------------------------------------------------------------------------------------------------- LightStereo

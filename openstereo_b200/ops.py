@@ -372,6 +372,62 @@ def upsample_softargmin_values(cost, disp_values, align_corners=False):
     return out.to(dt)
 
 
+def coex_attention_volume(x, y, maxdisp, head=1):
+    """CoEx's AttentionCostVolume after its convolutions (coex/coex_cost_processor.py:53-65 with the last plane dropped at :230):
+    x / ||x||_2 and y / ||y||_2 over ALL channels, then cost[b,g,d,h,w] = sum over group g's channels of x_n[.., w] * y_n[.., w-d]
+    for d < maxdisp, zero where w < d.  x, y (B,C,H,W) -> (B, head, maxdisp, H, W).  No backward."""
+    _no_autograd("coex_attention_volume", x, y)
+    xs, dt = _prep(x, "x")
+    ys, _ = _prep(y, "y")
+    assert xs.dim() == 4 and xs.shape == ys.shape
+    _same_device(xs, ys)
+    b, c, h, w = xs.shape
+    assert c % head == 0
+    out = torch.empty((b, head, maxdisp, h, w), dtype=torch.float32, device=xs.device)
+    if out.numel():
+        xn, yn = torch.empty_like(xs), torch.empty_like(ys)
+        _call("osb_group_l2_normalize_fwd", xs.data_ptr(), xn.data_ptr(), b, c, h, w, 1, 0.0, _stream(out))
+        _call("osb_group_l2_normalize_fwd", ys.data_ptr(), yn.data_ptr(), b, c, h, w, 1, 0.0, _stream(out))
+        _call("osb_gwc_volume_sum_fwd", xn.data_ptr(), yn.data_ptr(), out.data_ptr(), b, c, h, w, maxdisp, head, _stream(out))
+    return out.to(dt)
+
+
+def _aligned16(t):
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+def coex_regression(cost, spx, top_k, spx_is_logits=False):
+    """CoEx's Regression.forward (eval) with upfeat (coex/coex_disp_processor.py:8-65) in one launch: cost (B,1,D,h,w) logits,
+    spx (B,9,4h,4w) superpixel probabilities (or logits with spx_is_logits=True, fusing the softmax over the 9 channels) ->
+    disparity (B,4h,4w).  The top k logits along D (2 <= top_k <= 8) with ties to the lower index.  No backward."""
+    _no_autograd("coex_regression", cost, spx)
+    c, dt = _prep(cost, "cost")
+    s, _ = _prep(spx, "spx")
+    assert c.dim() == 5 and c.shape[1] == 1 and s.dim() == 4
+    b, _, d, h, w = c.shape
+    assert tuple(s.shape) == (b, 9, 4 * h, 4 * w), (tuple(s.shape), tuple(c.shape))
+    _same_device(c, s)
+    out = torch.empty((b, 4 * h, 4 * w), dtype=torch.float32, device=c.device)
+    if out.numel():
+        _call("osb_coex_regression_fwd", c.data_ptr(), _aligned16(s).data_ptr(), out.data_ptr(), b, d, h, w, int(top_k),
+              1 if spx_is_logits else 0, _stream(out))
+    return out.to(dt)
+
+
+def nearest_resize3d(x, size):
+    """F.interpolate(x, size=(D, H, W), mode='nearest') for a (B,C,D,H,W) volume, bit-equal (a gather with aten's source index).
+    No backward."""
+    _no_autograd("nearest_resize3d", x)
+    xs, dt = _prep(x, "x")
+    assert xs.dim() == 5 and len(size) == 3
+    b, c, di, hi, wi = xs.shape
+    do, ho, wo = (int(v) for v in size)
+    out = torch.empty((b, c, do, ho, wo), dtype=torch.float32, device=xs.device)
+    if out.numel():
+        _call("osb_nearest_resize3d_fwd", xs.data_ptr(), out.data_ptr(), b * c, di, hi, wi, do, ho, wo, _stream(out))
+    return out.to(dt)
+
+
 def epe_partial(disp_pred, disp_gt, maxdisp):
     """Per-image {sum |pred-gt| over 0<gt<maxdisp, #valid} -> (B, 2) fp32
     (metric_per_image.py:32-41 with the mask of trainer_template.py:288)."""

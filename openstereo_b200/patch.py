@@ -1,5 +1,5 @@
-"""patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo, and
-CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume hot
+"""patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / CoEx,
+and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume hot
 path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each
@@ -11,6 +11,7 @@ needs its own rebinding:
               aggregator + FasterSoftArgmin modules                          -> ``CostProcessor.forward`` / ``FasterSoftArgmin.forward``
 * LightStereo / IGEVStereo  like StereoBase: names imported into lightstereo.py:4-6 / igev_stereo.py:1-3 (``from .submodule import *``)
 * CasStereo   ``get_cv`` (GetCostVolume) and ``cost_agg[i]`` (CostAggregation) modules  -> per-instance ``forward`` overrides
+* CoEx        ``CostProcessor`` / ``DispProcessor`` / ``DispProcessor.regression`` modules -> per-instance ``forward`` overrides
 * StereoBase  functions imported INTO the module namespace (stereobase_gru.py:5-6,10-11) and the ``cost_agg``
               Hourglass                                                      -> per-INSTANCE copies of the methods that use those names,
                                                                                 with a private globals dict (the module itself, and
@@ -377,11 +378,70 @@ def _patch_cascade_agg(agg_mod, strict):
     agg_mod.forward = types.MethodType(agg_forward, agg_mod)
 
 
+def _trainable(module):
+    """True when autograd would record through the module's own parameters (a kernel call would cut them off)."""
+    return torch.is_grad_enabled() and any(p.requires_grad for p in module.parameters())
+
+
+def _patch_coex(model, strict, backbone=True):
+    """CoEx (coex/coex.py): the attention cost volume and the 3D aggregation (``CostProcessor.forward``), the top-k regression
+    with the superpixel up-sampling (``DispProcessor.forward``, and ``regression.forward`` for direct callers).  The MobileNet
+    encoder, FeatUp, the stems and the superpixel branch convs stay the reference's code; `backbone` has no effect."""
+    from .aggregation import CoExAggregation
+    cp, dp = model.CostProcessor, model.DispProcessor
+    reg = dp.regression
+    if not 2 <= reg.top_k <= 8:
+        raise NotImplementedError("patch(CoEx): REGRESSION_TOPK=%d is not supported (2..8; the reference's k = 1 branch gathers "
+                                  "index D, which is out of range)" % reg.top_k)
+    if cp.aggregation_disp_strides != 2:
+        raise NotImplementedError("patch(CoEx): AGGREGATION_DISP_STRIDES=%r is not supported (2: the isotropic stride-2 "
+                                  "convolutions of the kernels)" % (cp.aggregation_disp_strides,))
+    if cp.matching_weighted:
+        raise NotImplementedError("patch(CoEx): MATCHING_WEIGHTED=True is not supported")
+    cv = cp.cost_volume
+    engine = CoExAggregation(cp.cost_agg)
+    cp_orig, dp_orig, reg_orig = cp.forward, dp.forward, reg.forward
+
+    def cost_forward(self, inputs):
+        x, y = inputs["ref_feature"], inputs["tgt_feature"]
+        if _trainable(self) or not _accelerable(self, x, y):
+            return cp_orig(inputs) if not strict else _refuse("CoExCostProcessor")
+        xd, yd = cv.desc(cv.conv(x[0])), cv.desc(cv.conv(y[0]))       # the reference's own 2D convolutions
+        cost = ops.coex_attention_volume(xd, yd, cv.costVolume.maxdisp - 1, cv.head)
+        return {"cost_volume": engine(x, cost).to(x[0].dtype)}
+
+    def disp_forward(self, inputs):
+        cost = inputs["cost_volume"]
+        if _trainable(self) or not _accelerable(self, cost, inputs["ref_feature"], inputs["stem_2x"]):
+            return dp_orig(inputs) if not strict else _refuse("CoExDispProcessor")
+        xspx = self.spx_2(self.spx_4(inputs["ref_feature"][0]), inputs["stem_2x"])
+        # the raw superpixel logits go into the kernel, which applies the reference's softmax over the 9 channels itself
+        disp_pred = ops.coex_regression(cost, self.spx(xspx), self.regression.top_k, spx_is_logits=True).to(cost.dtype)
+        ref_img, tgt_img = inputs["left"], inputs["right"]
+        output = {"inference_disp": {"disp_est": disp_pred},
+                  "visual_summary": {"image/test/image_c": torch.cat([ref_img[0], tgt_img[0]], dim=1),
+                                     "image/test/disp_c": disp_pred[0]}}
+        if "disp_gt" in inputs:
+            output["visual_summary"] = {"image/val/image_c": torch.cat([ref_img[0], tgt_img[0]], dim=1),
+                                        "image/val/disp_c": torch.cat([inputs["disp_gt"][0], disp_pred[0]], dim=0)}
+        return output
+
+    def reg_forward(self, cost, spg):
+        if not _accelerable(self, cost, spg):
+            return reg_orig(cost, spg) if not strict else _refuse("CoEx Regression")
+        return [ops.coex_regression(cost, spg, self.top_k).to(cost.dtype)]
+
+    cp.forward = types.MethodType(cost_forward, cp)
+    dp.forward = types.MethodType(disp_forward, dp)
+    reg.forward = types.MethodType(reg_forward, reg)
+    return model
+
+
 # CasStereo's classes are also named PSMNet / GwcNet: they are told apart by the module that defines them
 _CASCADE_MODULES = {("casnet", "cas_psm"): "PSMNet", ("casnet", "cas_gwc"): "GwcNet"}
 
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
-             "IGEVStereo": _patch_igev}
+             "IGEVStereo": _patch_igev, "CoEx": _patch_coex}
 
 
 def patch(model, strict=True, backbone=True):

@@ -13,6 +13,9 @@
       encoding volume (igev_stereo.py:158,181-193; geometry.py:32-57) + 16 context up-samplings
   c6  CasPSMNet cfgs/casnet (the reference's class + patch()), batch 10 @512x960: whole-model forward next to the unpatched model
       on the same GPU, per-stage volume / aggregation / tail times  (python tools/bench_configs.py --only c6)
+  c7  CoEx cfgs/coex (the reference's class + patch()), batch 8 @256x512 and @540x960: whole-model forward next to the unpatched
+      model on the same GPU, per-stage volume / aggregation / regression times, the fused tail against the reference's tail
+      (python tools/bench_configs.py --only c7)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -304,6 +307,100 @@ def c6(iters, B=10, h=512, w=960):
          stages=stages, overflow_count=ops.tc_overflow_count())
 
 
+def c7(iters, B=8):
+    """CoEx (the reference's own class, cfgs/coex/coex_sceneflow_amp.yaml unchanged, seeded weights) at the cfg's eval size
+    540x960 and at 256x512, evaluator batch 8: patch() next to the unpatched model on this GPU (cuDNN fp32, TF32 off).  Per stage:
+    the attention volume, the 3D aggregation and the regression tail; the fused tail's GB/s on its algorithmic bytes and its time
+    next to the reference's tail (softmax over the 9 superpixel planes + Regression.forward) on the same inputs."""
+    from oracle import _reference_shim as shim
+    from openstereo_b200.patch import patch
+    shim.install_timm_stub()
+    cfg = shim.load_cfg("cfgs/coex/coex_sceneflow_amp.yaml").MODEL
+    cls = shim.load("stereo.modeling.models.coex.coex").CoEx
+    for (h, w) in ((256, 512), (540, 960)):
+        m = cls(cfg).eval()
+        m.load_state_dict(si.seeded_state_dict(m.state_dict(), seed=1))
+        m.to(DEV)
+        gen = torch.Generator().manual_seed(23)
+        x = {"left": rnd(gen, B, 3, h, w), "right": rnd(gen, B, 3, h, w)}
+        cp, dp = m.CostProcessor, m.DispProcessor
+        seen = {}
+
+        def grab(mod, args):
+            seen["cost"] = args[0]["cost_volume"]
+        hook = dp.register_forward_pre_hook(grab)
+        with torch.no_grad():
+            ms_ref, want = timeit(lambda: m(dict(x))["disp_pred"], max(2, iters // 3), warm=1)
+            ref_stages = _stage_times(lambda: m(dict(x)), {"volume": cp.cost_volume, "aggregation": cp.cost_agg,
+                                                         "regression": dp.regression})
+            # the reference's tail on the inputs it sees in this model: softmax over the 9 superpixel planes, then Regression
+            inputs = dict(x)
+            inputs.update(m.Backbone(inputs))
+            xspx = dp.spx_2(dp.spx_4(inputs["ref_feature"][0]), inputs["stem_2x"])
+            spx_logits = dp.spx(xspx)
+            cost = seen["cost"]
+            ms_ref_tail, _ = timeit(lambda: dp.regression(cost, F.softmax(spx_logits, 1)), iters)
+            patch(m)
+            ms, got = timeit(lambda: m(dict(x))["disp_pred"], iters)
+            ms_tail, _ = timeit(lambda: ops.coex_regression(cost, spx_logits, dp.regression.top_k, spx_is_logits=True), iters)
+            stages = _stage_times(lambda: m(dict(x)), {"aggregation": agg.CoExAggregation}, volume_fn="coex_attention_volume")
+            ops.profile_start()
+            m(dict(x))
+            torch.cuda.synchronize()
+            prof = ops.profile_stop()
+        hook.remove()
+        stages["regression"] = round(sum(a.elapsed_time(b) for a, b in prof["osb_coex_regression_fwd"]), 3)
+        hq, wq = cost.shape[-2:]
+        tail_bytes = 4 * (B * cost.shape[2] * hq * wq + 9 * B * 16 * hq * wq + B * 16 * hq * wq)
+        emit(config="c7 CoEx cfgs/coex/coex_sceneflow_amp.yaml, B=%d @%dx%d (reference class + patch())" % (B, h, w),
+             gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+             ms_per_step=round(ms, 3), pairs_per_s=round(B * 1e3 / ms, 2), reference_cudnn_fp32_ms=round(ms_ref, 2),
+             reference_pairs_per_s=round(B * 1e3 / ms_ref, 2), speedup_vs_reference_gpu=round(ms_ref / ms, 2),
+             stage_ms=stages, reference_stage_ms=ref_stages,
+             regression_tail_ms=round(ms_tail, 4), reference_tail_ms=round(ms_ref_tail, 4),
+             regression_tail_GBps=round(tail_bytes / ms_tail / 1e6, 1), regression_tail_frac_of_3350GBps=round(tail_bytes / ms_tail / 1e6 / 3350, 3),
+             epe_vs_reference_gpu_px=float("%.3e" % (got - want).abs().mean().item()), disparity_std_px=round(want.std().item(), 2))
+
+
+def _stage_times(run, targets, volume_fn=None):
+    """One run of `run` with CUDA events around the forward of each target (a module, or a class whose __call__ is wrapped) and,
+    with volume_fn, around ops.<volume_fn>: {stage: ms}."""
+    events, restore = [], []
+
+    def wrap(tag, inner):
+        def fwd(*args, **kw):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            out = inner(*args, **kw)
+            b.record()
+            events.append((tag, a, b))
+            return out
+        return fwd
+    for tag, t in targets.items():
+        if isinstance(t, type):
+            inner = t.__call__
+            t.__call__ = wrap(tag, inner)
+            restore.append(lambda t=t, inner=inner: setattr(t, "__call__", inner))
+        else:
+            inner = t.forward
+            t.forward = wrap(tag, inner)
+            restore.append(lambda t=t, inner=inner: setattr(t, "forward", inner))
+    if volume_fn:
+        inner = getattr(ops, volume_fn)
+        setattr(ops, volume_fn, wrap("volume", inner))
+        restore.append(lambda inner=inner: setattr(ops, volume_fn, inner))
+    try:
+        run()
+        torch.cuda.synchronize()
+    finally:
+        for r in restore:
+            r()
+    out = {}
+    for tag, a, b in events:
+        out[tag] = round(out.get(tag, 0.0) + a.elapsed_time(b), 3)
+    return out
+
+
 def _power_limit_w():
     try:
         import subprocess
@@ -321,7 +418,7 @@ if __name__ == "__main__":
     a = ap.parse_args()
     for name in a.only.split(","):
         try:
-            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6}[name](a.iters)
+            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:

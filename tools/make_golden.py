@@ -24,6 +24,7 @@ sys.path.insert(0, ROOT)
 from oracle import _reference_shim as shim                      # noqa: E402
 from oracle import aggregation as oagg                          # noqa: E402
 from oracle import cascade as ocas                              # noqa: E402
+from oracle import coex as ocx                                  # noqa: E402
 from oracle import cost_volume as ocv                           # noqa: E402
 from oracle import geo_lookup as ogeo                           # noqa: E402
 from oracle import lightstereo as olight                        # noqa: E402
@@ -356,6 +357,57 @@ def cascade():
              disp_mean=out.mean(), disp_std=out.std())
 
 
+def coex_tie_logits(seed, b, d, h, w):
+    """Small-integer logits: many exact ties along D, so the fixtures pin the order of equal values in the top-k selection."""
+    return torch.randint(-3, 3, (b, 1, d, h, w), generator=torch.Generator().manual_seed(seed)).float()
+
+
+def coex():
+    rcp = shim.load("stereo.modeling.models.coex.coex_cost_processor")
+    rdp = shim.load("stereo.modeling.models.coex.coex_disp_processor")
+    with torch.no_grad():
+        # attention volume: the reference module's own forward vs the oracle on the module's desc outputs
+        att = rcp.AttentionCostVolume(32, 20, 12, head=2).eval()
+        att.load_state_dict(si.seeded_state_dict(att.state_dict(), seed=110))
+        l, r = rnd(111, 2, 20, 6, 19), rnd(112, 2, 20, 6, 19)
+        ref = att(l, r)[:, :, :-1]
+        xd, yd = att.desc(att.conv(l)), att.desc(att.conv(r))
+        must_equal(ref, ocx.attention_volume(xd, yd, 8, 2), "CoEx attention volume")
+        save("coex_attention", x=xd, y=yd, maxdisp=8, head=2, out=ref)
+        # regression + upfeat, probabilities in; tie-heavy logits, k = 2 and 3
+        arrays = {}
+        cost = coex_tie_logits(113, 2, 10, 5, 7)
+        spx = torch.softmax(rnd(114, 2, 9, 20, 28, scale=2.0), 1)
+        for k in (2, 3):
+            reg = rdp.Regression(40, k).eval()
+            ref = reg(cost, spx)[0]
+            must_equal(ref, ocx.regression(cost, spx, k), "CoEx regression k=%d" % k)
+            arrays["out_k%d" % k] = ref
+            arrays["ind_k%d" % k] = ocx.topk_pool(cost, k)[1]
+        save("coex_regression", cost=cost, spx=spx, **arrays)
+        # nearest resampling along each dimension, including the 136 -> 135 of CoEx's 540 x 960 evaluation size
+        x = rnd(115, 1, 1, 7, 136, 12)
+        arrays = {"x": x}
+        for i, size in enumerate(((6, 135, 24), (14, 13, 12), (7, 136, 5))):
+            y = torch.nn.functional.interpolate(x, size=size, mode="nearest")
+            want = x[:, :, ocx.nearest_index(size[0], 7)][:, :, :, ocx.nearest_index(size[1], 136)][..., ocx.nearest_index(size[2], 12)]
+            must_equal(y, want, "nearest index %s" % (size,))
+            arrays["size%d" % i], arrays["out%d" % i] = torch.tensor(size), y
+        save("coex_nearest", **arrays)
+        # a small Aggregation (D = 16, 10 x 12 image: both upper levels mismatch their skip, 2 -> 3 rows and 3 -> 5)
+        ref_agg = rcp.Aggregation(max_disparity=64).eval()
+        mine = ocx.Aggregation(max_disparity=64).eval()
+        assert sorted(ref_agg.state_dict()) == sorted(mine.state_dict())
+        sd = si.seeded_state_dict(ref_agg.state_dict(), seed=116)
+        ref_agg.load_state_dict(sd), mine.load_state_dict(sd)
+        img = [rnd(117, 1, 96, 10, 12), rnd(118, 1, 64, 5, 6), rnd(119, 1, 192, 3, 3), rnd(120, 1, 160, 2, 2)]
+        cost = rnd(121, 1, 1, 16, 10, 12, scale=0.3)
+        ref = ref_agg(img, cost)
+        must_equal(ref, mine(img, cost), "CoEx Aggregation")
+        save("coex_aggregation", weight_seed=116, checksum=checksum(sd), img0=img[0], img1=img[1], img2=img[2], img3=img[3], cost=cost,
+             out=ref)
+
+
 class _Const(torch.nn.Module):
     def __init__(self, t):
         super().__init__()
@@ -365,7 +417,7 @@ class _Const(torch.nn.Module):
         return self.t
 
 
-SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade"]
+SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade", "coex"]
 
 if __name__ == "__main__":
     if not shim.available():
