@@ -30,14 +30,14 @@
 // publish the tile to the tensor core through fence.proxy.async + mbarrier.
 //
 // Warp roles (512 threads, 1 CTA/SM, persistent; setmaxnreg moves the registers, tc_common.cuh): warps 0-7 = two consumer
-// warpgroups (wgmma issue, then the epilogue of the finished tile: registers -> shared staging, 16 output channels per pass ->
-// one voxel per thread -> BN/residual/ReLU -> global), warps 8-11 = A-row loaders, warp 12 = weight-slice producer (one elected
+// warpgroups (wgmma issue, then the epilogue of the finished tile on the accumulator fragments: kw un-shift by shuffles, BN /
+// residual / activation, stores through a per-warp 16-row tile; tc_common.cuh: frag_unshift, frag_epilogue), warps 8-11 = A-row
+// loaders, warp 12 = weight-slice producer (one elected
 // lane issuing 1-D bulk copies of the pre-swizzled slices into two buffer sets), warp 13 = raw-row producer (bulk copies of
 // whole fp32 input rows ahead of the converters), warps 14-15 idle.
 //
-// Shared memory (Cout = 32): A ring 4 x 16 KB | weights 2 x 3 x 12 KB | raw rows 2 x 16 KB | per warpgroup a [128][52] fp32
-// staging tile (26 KB) and a seam-exchange buffer (0.75 KB) = 228,352 of the 232,448 bytes a CTA may have.  A full [128][100]
-// staging tile per warpgroup does not fit, so each warpgroup stages its finished tile in two passes of 16 output channels.
+// Shared memory (Cout = 32): A ring 4 x 16 KB | weights 2 x 3 x 12 KB | raw rows 2 x 16 KB | per warpgroup a double-buffered
+// seam-row buffer (4 KB) | per consumer warp a 16 x 40 fp32 output tile (2.5 KB) = 202,240 of the 232,448 bytes a CTA may have.
 #include <cstdlib>
 #include <type_traits>
 
@@ -52,7 +52,6 @@ constexpr int TC_ROWS = TC_TILES + 2;
 constexpr int TC_STAGES = 4;       // A-row ring depth (converted fp16 hi|lo tiles)
 constexpr int TC_RAW = 2;          // raw fp32 rows staged by 1-D TMA bulk copies ahead of the converters (Cin = 32 channels-last layers)
 constexpr int TC_ROW_BYTES = TC_W * TC_KC * 4;     // 16384: one staged input row (hi and lo halves of every voxel)
-constexpr int TC_PC = 16;          // output channels per epilogue pass (staged columns per kw block)
 
 struct TcParams {
   const float* x;          // (B, D, H, W, Cin) channels-last
@@ -76,42 +75,15 @@ template <int COUT>
 struct TcCfg {
   static constexpr int N3 = 3 * COUT;                      // kw-stacked MMA N
   static constexpr int B_SLICE = N3 * TC_KC * 4;           // one kh weight slice, rows [hi | lo] (12288 B for Cout = 32)
-  static constexpr int NPASS = COUT / TC_PC;               // epilogue passes: the staging tile holds TC_PC channels of each kw block
-  static constexpr int LD = 3 * TC_PC + 4;                 // floats per row of a staging tile
-  // per warpgroup: seam exchange [6 quadrant slots][2 sides][TC_PC]; slot q + 1 belongs to warp q, slots 0 and 5 stay zero (the
-  // image-edge neighbours), so that one register addresses everything a warp reads and writes there
-  static constexpr int XCHG_FLOATS = 6 * 2 * TC_PC;
+  static constexpr int XCHG_FLOATS = 2 * frag_xchg_floats<COUT, 1>();   // per consumer warpgroup: double-buffered seam rows
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + TC_STAGES * TC_ROW_BYTES;      // [2][3 kh]
   static constexpr int RAW_OFF = B_OFF + TC_BSLOTS * 3 * B_SLICE;    // [TC_RAW] raw fp32 input rows
-  static constexpr int STAGE_OFF = RAW_OFF + TC_RAW * TC_ROW_BYTES;  // [TC_WGS][128][LD] fp32 staging tiles
-  static constexpr int BAR_OFF = STAGE_OFF + TC_WGS * 128 * LD * 4;
-  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 256 + TC_WGS * XCHG_FLOATS * 4 + 2 * COUT * 4;
-  static_assert(COUT % TC_PC == 0, "the epilogue stages whole passes of TC_PC channels");
+  static constexpr int BAR_OFF = RAW_OFF + TC_RAW * TC_ROW_BYTES;
+  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 256 + TC_WGS * XCHG_FLOATS * 4 + 4 * TC_WGS * FRAG_TP_FLOATS * 4 + 2 * COUT * 4;
   static_assert(B_SLICE % 1024 == 0, "weight slices must stay 1024-byte aligned");
-  static_assert(32 * LD >= TP_WARP_FLOATS, "store_ndhwc_chunk32 transposes through the warp's own rows of the staging tile");
   static_assert(SMEM <= 232448, "shared memory budget of one CTA exceeded");
 };
-
-// Columns [TC_PC * pass, TC_PC * (pass + 1)) of every kw block of a finished 128 x 3*COUT tile into a [128][LD] staging tile, kw block
-// kw at staged columns TC_PC * kw ..  Fragment layout as in wg_stage (tc_common.cuh): register 4j + r holds column 8j + 2(l%4) + r%2.
-// `pass` must be a compile-time constant after unrolling (it indexes the accumulator registers).
-template <int COUT>
-__device__ __forceinline__ void tc_stage_pass(float* stage, const float (&acc)[2][3 * COUT / 2], int pass, int wq, int lane) {
-  constexpr int LD = TcCfg<COUT>::LD;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float* r0 = stage + (64 * h + 16 * wq + (lane >> 2)) * LD + 2 * (lane & 3);
-#pragma unroll
-    for (int kw = 0; kw < 3; ++kw)
-#pragma unroll
-      for (int jj = 0; jj < TC_PC / 8; ++jj) {
-        const int j = (kw * COUT + pass * TC_PC) / 8 + jj;
-        *reinterpret_cast<float2*>(r0 + TC_PC * kw + 8 * jj) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
-        *reinterpret_cast<float2*>(r0 + 8 * LD + TC_PC * kw + 8 * jj) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
-      }
-  }
-}
 
 template <int COUT>
 __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcParams p) {
@@ -125,7 +97,6 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
   uint8_t* a_buf = smem + C::A_OFF;
   uint8_t* b_buf = smem + C::B_OFF;
   uint8_t* raw_buf = smem + C::RAW_OFF;
-  float* stage = reinterpret_cast<float*>(smem + C::STAGE_OFF);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
   uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumers  (128 arrivals)
   uint64_t* a_empty = a_ready + TC_STAGES;          // [STAGES] consumers -> loaders  (8 arrivals: one per consumer warp)
@@ -134,7 +105,8 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
   uint64_t* raw_full = b_empty + TC_BSLOTS * 3;     // [RAW]    row producer -> converters (expect_tx + bulk-copy bytes, or a plain arrive)
   uint64_t* raw_empty = raw_full + TC_RAW;          // [RAW]    converters -> row producer (128 arrivals)
   float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 256);   // [TC_WGS][XCHG_FLOATS] boundary exchange
-  float* s_scale = xchg + TC_WGS * C::XCHG_FLOATS;         // [COUT]
+  float* tiles = xchg + TC_WGS * C::XCHG_FLOATS;           // [8 consumer warps][FRAG_TP_FLOATS] output tiles
+  float* s_scale = tiles + 4 * TC_WGS * FRAG_TP_FLOATS;     // [COUT]
   float* s_shift = s_scale + COUT;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -159,7 +131,6 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
     s_scale[c] = p.scale ? p.scale[c] : 1.f;
     s_shift[c] = p.shift ? p.shift[c] : 0.f;
   }
-  for (int i = threadIdx.x; i < TC_WGS * C::XCHG_FLOATS; i += blockDim.x) xchg[i] = 0.f;
   __syncthreads();
   // The rows a CTA stages form one flat sequence (item, kd, chunk, r).  `RowIter` walks it; loads run TWO rows ahead of
   // the stores (software pipeline in registers) so that a full L2/HBM round trip is always in flight.
@@ -187,23 +158,26 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
   };
   // ---------------------------------------------------------------------------------------------- consumer warpgroups
   // Warpgroup wg accumulates output row 2p + wg of the item from the rows and weight slices both warpgroups read, then runs the
-  // epilogue of that row.
+  // epilogue of that row on the accumulator fragments (tc_common.cuh: frag_unshift, frag_epilogue).
   if (warp < 4 * TC_WGS) {
     setmaxnreg_inc<TC_CONSUMER_REGS>();
     const int wg = warp >> 2;
-    stage += wg * 128 * C::LD;
     xchg += wg * C::XCHG_FLOATS;
-    const int bar_stage = 1 + 2 * wg, bar_xchg = 2 + 2 * wg;   // this warpgroup's named barriers
+    const int bar_xchg = 1 + wg;                     // this warpgroup's named barrier
     constexpr uint32_t LO = TcK<TC_KC>::LO_OFF;     // descriptor offset of the lo half of an operand row
     constexpr uint32_t A_HALF = 64 * TC_KC * 4 / 16;  // descriptor offset of operand rows 64..127
     const uint64_t dbase = desc_sw128_base();
     // Descriptors differ only in their 14-bit start-address field (bits 0-13, units of 16 bytes).
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
-    const int q = warp & 3;                          // epilogue: this warp owns tile rows 32q .. 32q + 31
-    const int m = q * 32 + lane;                     // voxel (image column) owned by this thread
-    uint32_t rowc = 0, phc = 0;
+    const int q = warp & 3;                          // warp of the warpgroup
+    uint32_t rowc = 0, phc = 0, exc = 0;
     for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
       const int d = (it / p.hblocks) % p.D;
+      const int b = it / (p.hblocks * p.D);
+      const int h = (it % p.hblocks) * TC_TILES + wg;
+      // the residual streams from HBM / L2: pull one voxel's channels per thread into L2 while the row is being accumulated
+      if (h < p.H && p.residual && p.res_ndhwc)
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + ((((size_t)b * p.D + d) * p.H + h) * TC_W + q * 32 + lane) * COUT));
       float acc[2][N3 / 2];
       uint32_t accum = 0;
       for (int kd = 0; kd < 3; ++kd) {
@@ -237,99 +211,23 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
         }
       }
       // A tile below the image (odd H) received its MMAs and releases like any other and stores nothing.  The branch is
-      // warpgroup-uniform and the epilogue's barriers are this warpgroup's own.
-      const int h = (it % p.hblocks) * TC_TILES + wg;
+      // warpgroup-uniform and the epilogue's barrier and seam buffer are this warpgroup's own.
       if (h >= p.H) continue;
       // MMAs each P_kw accumulator received: (existing kd planes) x chunks x 3 kh x k-steps x 3 split terms
       const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * TcK<TC_KC>::KSTEPS * 3);
-      // D[m] = P0[m-1] + P1[m] + P2[m+1], from the staged tile, TC_PC channels per pass
-      float out[COUT];
-#pragma unroll
-      for (int pass = 0; pass < C::NPASS; ++pass) {
-        named_bar_sync(bar_stage, 128);              // every warp is done with the rows staged before (previous pass or tile)
-        tc_stage_pass<COUT>(stage, acc, pass, q, lane);
-        named_bar_sync(bar_stage, 128);
-        const float* srow = stage + m * C::LD;       // [P0 | P1 | P2] of this pass's channels
-        // lanes at the warp edges need the neighbour quadrant's values: exchange through shared memory.  One buffer suffices: its
-        // readers of the previous pass passed bar_stage above before any writer of this pass did.
-        float* xq = xchg + (q + 1) * 2 * TC_PC;      // this warp's slot: [P0 of its last column | P2 of its first column]
-        if (lane == 31) {
-#pragma unroll
-          for (int i = 0; i < TC_PC; i += 4)
-            *reinterpret_cast<float4*>(xq + i) = *reinterpret_cast<const float4*>(srow + i);
-        }
-        if (lane == 0) {
-#pragma unroll
-          for (int i = 0; i < TC_PC; i += 4)
-            *reinterpret_cast<float4*>(xq + TC_PC + i) = *reinterpret_cast<const float4*>(srow + 2 * TC_PC + i);
-        }
-        named_bar_sync(bar_xchg, 128);
-        const float* xl = xq - 2 * TC_PC;            // P0 of the previous quadrant's last column (zero slot at the image edge)
-        const float* xr = xq + 3 * TC_PC;            // P2 of the next quadrant's first column
-        // The neighbour-quadrant values are loaded UNCONDITIONALLY (warp-uniform addresses: broadcast LDS.128) and merged with
-        // selects: the `lane == 0 ? xl[i] : left` form compiles to a branch around a load per element.
-#pragma unroll
-        for (int i0 = 0; i0 < TC_PC; i0 += 4) {
-          const float4 l4 = *reinterpret_cast<const float4*>(xl + i0);
-          const float4 r4 = *reinterpret_cast<const float4*>(xr + i0);
-          const float4 p04 = *reinterpret_cast<const float4*>(srow + i0);
-          const float4 p14 = *reinterpret_cast<const float4*>(srow + TC_PC + i0);
-          const float4 p24 = *reinterpret_cast<const float4*>(srow + 2 * TC_PC + i0);
-          const float le[4] = {l4.x, l4.y, l4.z, l4.w}, re[4] = {r4.x, r4.y, r4.z, r4.w};
-          const float p0[4] = {p04.x, p04.y, p04.z, p04.w}, p1[4] = {p14.x, p14.y, p14.z, p14.w}, p2[4] = {p24.x, p24.y, p24.z, p24.w};
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float left = __shfl_up_sync(0xffffffffu, p0[k], 1);
-            float right = __shfl_down_sync(0xffffffffu, p2[k], 1);
-            left = (lane == 0) ? le[k] : left;        // m-1 lives in the previous quadrant (zero at the image edge)
-            right = (lane == 31) ? re[k] : right;     // m+1 lives in the next quadrant
-            out[pass * TC_PC + i0 + k] = ((left + p1[k]) + right) * corr;
-          }
-        }
-      }
-      const int b = it / (p.hblocks * p.D);
-      const size_t vox = (((size_t)b * p.D + d) * p.H + h) * TC_W + m;             // NDHWC voxel index
+      frag_unshift<COUT, 1, TC_W>(acc, xchg + (exc & 1) * (C::XCHG_FLOATS / 2), q, lane, corr, bar_xchg);
+      ++exc;
+      const size_t row0 = (((size_t)b * p.D + d) * p.H + h) * TC_W;                // NDHWC voxel index of column 0
       const size_t plane = (size_t)p.D * p.H * TC_W;                               // NCDHW channel stride
-      const size_t ncdhw0 = (size_t)b * p.Cout * plane + ((size_t)d * p.H + h) * TC_W + m;   // p.Cout <= COUT real channels
-      if constexpr (COUT == 32) {
-        if (p.out_ndhwc && (!p.residual || p.res_ndhwc)) {     // coalesced channels-last path (BN/residual/act inside)
-          store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, out, p.y + (vox - lane) * COUT,
-                              p.residual ? p.residual + (vox - lane) * COUT : nullptr, COUT, s_scale, s_shift, p.act);
-          continue;
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < COUT; ++i) out[i] = fmaf(out[i], s_scale[i], s_shift[i]);
-      if (p.residual) {
-        if (p.res_ndhwc) {
-          const float4* rp = reinterpret_cast<const float4*>(p.residual + vox * COUT);
-#pragma unroll
-          for (int i = 0; i < COUT / 4; ++i) {
-            const float4 rv = __ldg(rp + i);
-            out[4 * i] += rv.x, out[4 * i + 1] += rv.y, out[4 * i + 2] += rv.z, out[4 * i + 3] += rv.w;
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < COUT; ++i)
-            if (i < p.Cout) out[i] += __ldg(p.residual + ncdhw0 + (size_t)i * plane);
-        }
-      }
-      if (p.act == OSB_ACT_RELU) {
-#pragma unroll
-        for (int i = 0; i < COUT; ++i) out[i] = fmaxf(out[i], 0.f);
-      } else if (p.act == OSB_ACT_LEAKY) {
-#pragma unroll
-        for (int i = 0; i < COUT; ++i) out[i] = out[i] > 0.f ? out[i] : 0.01f * out[i];
-      }
-      if (p.out_ndhwc) {
-        float4* yp = reinterpret_cast<float4*>(p.y + vox * COUT);
-#pragma unroll
-        for (int i = 0; i < COUT / 4; ++i) yp[i] = make_float4(out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < COUT; ++i)
-          if (i < p.Cout) p.y[ncdhw0 + (size_t)i * plane] = out[i];                 // 128-byte rows per warp
-      }
+      const size_t ncdhw0 = (size_t)b * p.Cout * plane + ((size_t)d * p.H + h) * TC_W;   // p.Cout <= COUT real channels
+      auto rows = [&](int m, ptrdiff_t& yo, ptrdiff_t& ro, ptrdiff_t& go) {      // m = image column
+        yo = p.out_ndhwc ? (ptrdiff_t)(row0 + m) * COUT : (ptrdiff_t)(ncdhw0 + m);
+        ro = p.res_ndhwc ? (ptrdiff_t)(row0 + m) * COUT : (ptrdiff_t)(ncdhw0 + m);
+        go = 0;
+        return true;
+      };
+      frag_epilogue<COUT>(acc, lane, q, tiles + warp * FRAG_TP_FLOATS, s_scale, s_shift, p.act, p.y, p.out_ndhwc ? 1 : plane, p.residual, p.res_ndhwc ? 1 : plane,
+                          nullptr, rows, COUT == 32 ? 32 : p.Cout);
     }
   }
   // ---------------------------------------------------------------------------------------------- A-row loaders

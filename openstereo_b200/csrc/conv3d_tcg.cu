@@ -58,7 +58,6 @@ struct TcgCfg {
   static constexpr int NG3 = 3 * G;                         // wgmma N: the three kw blocks of one channel group
   static constexpr int B_SLICE = N3 * ROWB;                 // one kh weight slice in global memory (hi and lo halves of every row)
   static constexpr int B_SUB = NG3 * ROWB;                  // the part of it one item reads
-  static constexpr int LD = NG3 + 4;                        // floats per row of the staged accumulator tile
   // Work item = NT output tiles, tile t (consumer warpgroup t) at image rows row0 + t * TS .. + R - 1.  DIL = 1: consecutive row
   // blocks, so the units of rows between the tiles feed both.  DIL = 2: rows h and h + 2, whose taps share two of their three units
   // (adjacent rows share none); row blocks then interleave, hb = 2k + j -> rows 4k + j and 4k + j + 2.
@@ -71,8 +70,9 @@ struct TcgCfg {
   // shared memory allows (at most 10 units).  Each loader warp enumerates ONLY ITS OWN units: a walk over the whole (tile, tap)
   // sequence by every warp, picking every NLW-th unit, makes that scalar control flow the bound of these kernels.
   static constexpr int NLW = 4;
-  static constexpr int XCHG_FLOATS = 2 * 4 * 2 * DIL * 32;  // per consumer warpgroup: [2][4 quadrants][2 sides][DIL columns][32]
-  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * 3 * B_SUB + TC_WGS * 128 * LD * 4 + 1024 + TC_WGS * XCHG_FLOATS * 4 + 3 * COUT * 4;
+  static constexpr int XCHG_FLOATS = 2 * frag_xchg_floats<G, DIL>();   // per consumer warpgroup: double-buffered seam rows
+  static constexpr int FIXED_SMEM = 1024 + TC_BSLOTS * 3 * B_SUB + 1024 + TC_WGS * XCHG_FLOATS * 4 + 4 * TC_WGS * FRAG_TP_FLOATS * 4 +
+                                    2 * COUT * 4;
   static constexpr int STAGES = (232448 - FIXED_SMEM) / UNIT_BYTES < 10 ? (232448 - FIXED_SMEM) / UNIT_BYTES : 10;
   static_assert(STAGES >= NLW, "the ring must hold at least one unit per loader warp");
   static constexpr int S_FIRST = -DIL;                      // unit start rows run from S_FIRST to S_LAST (block-relative)
@@ -81,10 +81,9 @@ struct TcgCfg {
   static constexpr int LO = KC / 8;                         // descriptor offset (16-byte units) of the lo half of a row
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + STAGES * UNIT_BYTES;
-  static constexpr int STAGE_OFF = B_OFF + TC_BSLOTS * 3 * B_SUB;   // [TC_WGS][128][LD] fp32 accumulator tiles
-  static constexpr int BAR_OFF = STAGE_OFF + TC_WGS * 128 * LD * 4;
+  static constexpr int BAR_OFF = B_OFF + TC_BSLOTS * 3 * B_SUB;
   static constexpr int THREADS = TC_WG_THREADS;             // consumers 0-7 | A loaders 8-11 | weight producer 12, idle 13-15
-  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + TC_WGS * XCHG_FLOATS * 4 + 3 * COUT * 4;
+  static constexpr size_t SMEM = 1024 + (size_t)BAR_OFF + 1024 + TC_WGS * XCHG_FLOATS * 4 + 4 * TC_WGS * FRAG_TP_FLOATS * 4 + 2 * COUT * 4;
   static_assert(SMEM <= 232448, "shared memory budget of one CTA exceeded");
   static_assert(TILES == 1, "a consumer warpgroup holds one accumulator tile");
   static_assert(DIL == 1 || R == 1, "interleaved row blocks assume one image row per tile");
@@ -121,16 +120,15 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* a_buf = smem + C::A_OFF;
   uint8_t* b_buf = smem + C::B_OFF;
-  float* stage = reinterpret_cast<float*>(smem + C::STAGE_OFF);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
   uint64_t* a_ready = bars;                         // [STAGES] loaders -> consumer   (32 arrivals: one warp)
   uint64_t* a_empty = a_ready + C::STAGES;          // [STAGES] consumers -> loaders  (8 arrivals: one per consumer warp)
   uint64_t* b_full = a_empty + C::STAGES;           // [2][3]   weight producer -> consumers (expect_tx + bulk-copy bytes)
   uint64_t* b_empty = b_full + TC_BSLOTS * 3;       // [2][3]   consumers -> weight producer (8 arrivals)
   float* xchg = reinterpret_cast<float*>(smem + C::BAR_OFF + 1024);   // [TC_WGS][XCHG_FLOATS]
-  float* s_scale = xchg + TC_WGS * C::XCHG_FLOATS;
+  float* tiles = xchg + TC_WGS * C::XCHG_FLOATS;       // [8 consumer warps][FRAG_TP_FLOATS] output tiles
+  float* s_scale = tiles + 4 * TC_WGS * FRAG_TP_FLOATS;
   float* s_shift = s_scale + COUT;
-  float* zeros = s_shift + COUT;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nchunk = p.Cin / KC;
@@ -152,27 +150,22 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   for (int c = threadIdx.x; c < COUT; c += blockDim.x) {
     s_scale[c] = p.scale ? p.scale[c] : 1.f;
     s_shift[c] = p.shift ? p.shift[c] : 0.f;
-    zeros[c] = 0.f;
   }
   __syncthreads();
 
   // ---------------------------------------------------------------------------------------------- consumer warpgroups
   // Warpgroup wg issues the wgmmas of tile wg of the item into its 128 x 96 register tile (output channels cg .. cg + 31 of all
-  // three kw taps) from the units and weight slices both warpgroups read, then runs the epilogue of that tile.
+  // three kw taps) from the units and weight slices both warpgroups read, then runs the epilogue of that tile on the accumulator
+  // fragments (tc_common.cuh: frag_unshift, frag_epilogue).
   if (warp < 4 * TC_WGS) {
     setmaxnreg_inc<TC_CONSUMER_REGS>();
     const int wg = warp >> 2;
-    stage += wg * 128 * C::LD;
     xchg += wg * C::XCHG_FLOATS;
-    const int bar_stage = 1 + 2 * wg, bar_xchg = 2 + 2 * wg;   // this warpgroup's named barriers
+    const int bar_xchg = 1 + wg;                     // this warpgroup's named barrier
     const uint64_t dbase = (KC == 32) ? desc_sw128_base() : desc_sw64_base();
     constexpr uint32_t A_HALF = 64 * C::ROWB / 16;  // descriptor offset of operand rows 64..127
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
-    const int q = warp & 3;                          // epilogue: this warp owns tile rows 32q .. 32q + 31
-    const int m = q * 32 + lane;                     // operand row owned by this thread
-    const int rr = m / W, wcol = m % W;              // image row inside the tile, image column
-    const bool has_left_q = ((q * 32) % W) != 0;     // the quadrant to the left continues the same image row
-    const bool has_right_q = (((q + 1) * 32) % W) != 0;
+    const int q = warp & 3;                          // warp of the warpgroup
     uint32_t unitc = 0, phc = 0, exc = 0;
     for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
       const int cg = (it % C::NG) * C::G;            // output channel group of this item
@@ -181,146 +174,73 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
       const int hb = (it0 / ctiles) % p.hblocks;
       const int d = (it0 / (ctiles * p.hblocks)) % p.D;
       const int b = it0 / (ctiles * p.hblocks * p.D);
+      // Tile row m -> image row h (a tile below the image, odd H or H not a multiple of the item's rows, received its MMAs and
+      // releases like any other and stores nothing) and column (general widths: halo columns and columns beyond the image are not
+      // stored).  Returns whether the row is stored.
+      auto tile_row = [&](int m, int& h, int& col) {
+        h = C::row0(hb) + wg * C::TS + m / W;
+        col = GW ? ct * C::CSTEP - C::HALO + m : m % W;
+        return h < p.H && (!GW || (m >= C::HALO && m < 128 - C::HALO && col < Wp));
+      };
       {
-        float acc[2][C::NG3 / 2];
-        uint32_t accum = 0;
-        for (int kd = 0; kd < 3; ++kd) {
-          const int din = d + kd - 1;
-          if (din < 0 || din >= p.D) continue;
-          for (int ch = 0; ch < nchunk; ++ch, ++phc) {
+        // the residual and the gate stream from HBM / L2: pull one voxel's channel group per thread into L2 while the tile is
+        // being accumulated
+        int h, col;
+        if (tile_row(q * 32 + lane, h, col)) {
+          const ptrdiff_t vox = (((ptrdiff_t)b * p.D + d) * p.H + h) * Wp + col;
+          if (p.residual && p.res_ndhwc) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + vox * YS + cg));
+          if (GATE && p.gate) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.gate + (((ptrdiff_t)b * p.H + h) * Wp + col) * YS + cg));
+        }
+      }
+      float acc[2][C::NG3 / 2];
+      uint32_t accum = 0;
+      for (int kd = 0; kd < 3; ++kd) {
+        const int din = d + kd - 1;
+        if (din < 0 || din >= p.D) continue;
+        for (int ch = 0; ch < nchunk; ++ch, ++phc) {
 #pragma unroll
-            for (int s = C::S_FIRST; s <= C::S_LAST; ++s) {
-              if (!C::used(s)) continue;
-              const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
-              mbar_wait(&a_ready[slot], par);
-              const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
+          for (int s = C::S_FIRST; s <= C::S_LAST; ++s) {
+            if (!C::used(s)) continue;
+            const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
+            mbar_wait(&a_ready[slot], par);
+            const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
 #pragma unroll
-              for (int kh = 0; kh < 3; ++kh) {
-                if (C::tile_of(s, kh) != wg) continue;   // unit s meets slice kh for tile wg when s == wg * TS + (kh - 1) * DIL
-                const uint32_t bslot = (phc & 1) * 3 + kh;
-                mbar_wait(&b_full[bslot], (phc >> 1) & 1);
-                const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
-                wg_fence();
+            for (int kh = 0; kh < 3; ++kh) {
+              if (C::tile_of(s, kh) != wg) continue;   // unit s meets slice kh for tile wg when s == wg * TS + (kh - 1) * DIL
+              const uint32_t bslot = (phc & 1) * 3 + kh;
+              mbar_wait(&b_full[bslot], (phc >> 1) & 1);
+              const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
+              wg_fence();
 #pragma unroll
-                for (int ks = 0; ks < C::KSTEPS; ++ks)
-                  wg_mma_split<C::NG3>(acc, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum);
-                wg_commit();
-                wg_wait_all();
-                accum = 1;
-                wg_release(&b_empty[bslot], lane);
-              }
-              wg_release(&a_empty[slot], lane);
-              ++unitc;
+              for (int ks = 0; ks < C::KSTEPS; ++ks)
+                wg_mma_split<C::NG3>(acc, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum);
+              wg_commit();
+              wg_wait_all();
+              accum = 1;
+              wg_release(&b_empty[bslot], lane);
             }
+            wg_release(&a_empty[slot], lane);
+            ++unitc;
           }
         }
-        named_bar_sync(bar_stage, 128);              // every warp is done with the previous tile's staged rows
-        wg_stage<C::NG3>(stage, C::LD, acc, q, lane);
-        named_bar_sync(bar_stage, 128);
       }
-      // general widths: image column of this thread's tile column; halo columns and columns beyond the image are not stored
-      const int col = GW ? ct * C::CSTEP - C::HALO + m : wcol;
-      const bool cvalid = !GW || (m >= C::HALO && m < 128 - C::HALO && col < Wp);
-      const uint32_t vmask = GW ? __ballot_sync(0xffffffffu, cvalid) : 0xffffffffu;
       const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * C::KSTEPS * 3);   // tc_common.cuh: rz_kappa
-      {
-        // a tile below the image (odd H, H not a multiple of the item's rows) received its MMAs and releases like any other:
-        // `live` masks every store of it
-        const int h = C::row0(hb) + wg * C::TS + rr;
-        const bool live = h < p.H;
+      frag_unshift<C::G, DIL, W>(acc, xchg + (exc & 1) * (C::XCHG_FLOATS / 2), q, lane, corr, bar_xchg);
+      ++exc;
+      const size_t plane = (size_t)p.D * p.H * Wp;                                 // NCDHW channel stride
+      auto rows = [&](int m, ptrdiff_t& yo, ptrdiff_t& ro, ptrdiff_t& go) {
+        int h, col;
+        const bool ok = tile_row(m, h, col);
         const ptrdiff_t vox = (((ptrdiff_t)b * p.D + d) * p.H + h) * Wp + col;     // NDHWC voxel index
-        if (live && cvalid && p.residual && p.res_ndhwc) {
-          // the residual streams from HBM / L2: start pulling this thread's voxel into L2 while the tile is still being accumulated
-          // (ncu source view of the backbone layers: 9 % of the samples waited on the residual loads after the transpose)
-          const float* rp = p.residual + vox * YS;
-#pragma unroll
-          for (int k = 0; k < COUT; k += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(rp + k));
-        }
-        const size_t plane = (size_t)p.D * p.H * Wp;                               // NCDHW channel stride
-        const ptrdiff_t ncdhw0 = (ptrdiff_t)b * COUT * plane + ((ptrdiff_t)d * p.H + h) * Wp + col;
-        {
-          // this voxel's P_kw columns are read from the staged tile four channels at a time (holding all 96 would spill)
-          const float* srow = stage + m * C::LD;
-          float* xb = xchg + (exc & 1) * (4 * 2 * DIL * 32);
-          ++exc;
-          if (lane >= 32 - DIL) {                     // the next quadrant's first DIL columns need these P0 values
-#pragma unroll
-            for (int i = 0; i < 32; i += 4)
-              *reinterpret_cast<float4*>(xb + ((q * 2) * DIL + lane - (32 - DIL)) * 32 + i) = *reinterpret_cast<const float4*>(srow + i);
-          }
-          if (lane < DIL) {                           // the previous quadrant's last DIL columns need these P2 values
-#pragma unroll
-            for (int i = 0; i < 32; i += 4)
-              *reinterpret_cast<float4*>(xb + ((q * 2 + 1) * DIL + lane) * 32 + i) = *reinterpret_cast<const float4*>(srow + 2 * C::G + i);
-          }
-          named_bar_sync(bar_xchg, 128);
-          const float* xl = has_left_q ? xb + (((q - 1) * 2) * DIL + (lane < DIL ? lane : 0)) * 32 : zeros;
-          const float* xr = has_right_q ? xb + (((q + 1) * 2 + 1) * DIL + (lane >= 32 - DIL ? lane - (32 - DIL) : 0)) * 32 : zeros;
-          float out[32];
-#pragma unroll
-          for (int i0 = 0; i0 < 32; i0 += 4) {        // neighbour values loaded unconditionally, merged with selects (no branches)
-            const float4 l4 = *reinterpret_cast<const float4*>(xl + i0);
-            const float4 r4 = *reinterpret_cast<const float4*>(xr + i0);
-            const float4 p04 = *reinterpret_cast<const float4*>(srow + i0);
-            const float4 p14 = *reinterpret_cast<const float4*>(srow + C::G + i0);
-            const float4 p24 = *reinterpret_cast<const float4*>(srow + 2 * C::G + i0);
-            const float le[4] = {l4.x, l4.y, l4.z, l4.w}, re[4] = {r4.x, r4.y, r4.z, r4.w};
-            const float p0[4] = {p04.x, p04.y, p04.z, p04.w}, p1[4] = {p14.x, p14.y, p14.z, p14.w}, p2[4] = {p24.x, p24.y, p24.z, p24.w};
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int i = i0 + k;
-              float left = __shfl_up_sync(0xffffffffu, p0[k], DIL);
-              float right = __shfl_down_sync(0xffffffffu, p2[k], DIL);
-              left = (lane < DIL) ? le[k] : left;       // column w-DIL (zero at the image edge)
-              right = (lane >= 32 - DIL) ? re[k] : right;   // column w+DIL
-              if (W < 32) {                             // several image rows per warp: row seams inside the warp are image edges
-                left = (wcol < DIL) ? 0.f : left;
-                right = (wcol >= W - DIL) ? 0.f : right;
-              }
-              out[i] = ((left + p1[k]) + right) * corr;
-            }
-          }
-          // voxels of this warp that exist (W < 32: the warp spans two image rows, the second may lie below the image)
-          const uint32_t vm = (W < 32) ? __ballot_sync(0xffffffffu, live) : (live ? vmask : 0u);
-          if (vm && p.out_ndhwc && (!p.residual || p.res_ndhwc)) {     // coalesced channels-last path (BN/residual/act inside)
-            const ptrdiff_t gvox = GATE ? ((ptrdiff_t)b * p.H + h) * Wp + col - lane : 0;   // (B, H, W) index of lane 0's voxel
-            store_ndhwc_chunk32(stage + q * 32 * C::LD, lane, out, p.y + (vox - lane) * YS + cg,
-                                p.residual ? p.residual + (vox - lane) * YS + cg : nullptr, YS, s_scale + cg, s_shift + cg, p.act,
-                                vm, (GATE && p.gate) ? p.gate + gvox * YS + cg : nullptr);
-          } else if (live && cvalid) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) out[i] = fmaf(out[i], s_scale[cg + i], s_shift[cg + i]);
-            if (p.residual) {
-              if (p.res_ndhwc) {
-                const float4* rp = reinterpret_cast<const float4*>(p.residual + vox * YS + cg);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const float4 rv = __ldg(rp + i);
-                  out[4 * i] += rv.x, out[4 * i + 1] += rv.y, out[4 * i + 2] += rv.z, out[4 * i + 3] += rv.w;
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) out[i] += __ldg(p.residual + ncdhw0 + (size_t)(cg + i) * plane);
-              }
-            }
-            if (p.act == OSB_ACT_RELU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) out[i] = fmaxf(out[i], 0.f);
-            } else if (p.act == OSB_ACT_LEAKY) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) out[i] = out[i] > 0.f ? out[i] : 0.01f * out[i];
-            }
-            if (p.out_ndhwc) {
-              float4* yp = reinterpret_cast<float4*>(p.y + vox * YS + cg);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) yp[i] = make_float4(out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) p.y[ncdhw0 + (size_t)(cg + i) * plane] = out[i];
-            }
-          }
-        }
-      }
+        const ptrdiff_t ncdhw = (ptrdiff_t)b * COUT * plane + ((ptrdiff_t)d * p.H + h) * Wp + col;
+        yo = p.out_ndhwc ? vox * YS : ncdhw;
+        ro = p.res_ndhwc ? vox * YS : ncdhw;
+        go = (((ptrdiff_t)b * p.H + h) * Wp + col) * YS;
+        return ok;
+      };
+      frag_epilogue<C::G>(acc, lane, q, tiles + warp * FRAG_TP_FLOATS, s_scale + cg, s_shift + cg, p.act, p.y + (p.out_ndhwc ? (size_t)cg : cg * plane),
+                          p.out_ndhwc ? 1 : plane, p.residual ? p.residual + (p.res_ndhwc ? (size_t)cg : cg * plane) : nullptr,
+                          p.res_ndhwc ? 1 : plane, (GATE && p.gate) ? p.gate + cg : nullptr, rows, C::G);
     }
   }
   // ---------------------------------------------------------------------------------------------- A-unit loaders

@@ -118,7 +118,8 @@ __device__ __forceinline__ void wg_release(uint64_t* bar, int lane) {
   if (lane == 0) mbar_arrive(bar);
 }
 // Accumulator fragment of wgmma m64nN (f32): register 4j + r of lane l in warp w of the warpgroup holds row 16w + l/4 + 8(r/2),
-// column 8j + 2(l%4) + r%2.  The epilogues own one voxel (tile row) per thread, so a finished tile goes through shared memory:
+// column 8j + 2(l%4) + r%2.  The epilogues of conv3d_tcs2.cu / conv3d_tcdc.cu own one voxel (tile row) per thread, so their finished
+// tiles go through shared memory:
 // `stage` is [128 rows][ld floats], ld = N + 4 (rows 16 B apart in bank space: the per-row LDS.128 of a warp are conflict-free).
 template <int N>
 __device__ __forceinline__ void wg_stage(float* stage, int ld, const float (&acc)[2][N / 2], int wq, int lane) {
@@ -269,6 +270,206 @@ struct TcK {
   static constexpr int KSTEPS = KC / 16;
   static constexpr int LO_OFF = KC / 8;           // descriptor start-address offset (16-byte units) of the lo half of a row
 };
+
+// ------------------------------------------------------------------------------- fragment-resident stride-1 epilogue
+// conv3d_tc.cu / conv3d_tcg.cu: a 128 x 3G accumulator tile holds the kw-stacked partial sums [P0 | P1 | P2] of G output channels,
+// and out[m] = P0[m - DIL] + P1[m] + P2[m + DIL].  In the fragment layout above, P0, P1 and P2 of one (row, channel) sit in
+// registers 4j + r, 4(j + G/8) + r and 4(j + G/4) + r of the same thread, and rows m -+ DIL sit DIL lane quads away in the same
+// warp, or DIL rows across the boundary of the warp's 16-row group.  So the un-shift runs on the registers: one shuffle per
+// neighbour value (the sending lane picks which of its two row registers the receiver needs), and only the DIL seam rows of each
+// 16-row group go through a small shared buffer.
+// Seam buffer of one warpgroup, per exchange: [8 row groups (group 4h + w = rows 64h + 16w ..)][2 sides][DIL rows][G channels]:
+// side 0 = P0 of the group's last DIL rows, side 1 = P2 of its first DIL rows.  Callers double-buffer it, so that a warp already
+// publishing the next item's seams cannot overwrite values another warp has still to read.
+template <int G, int DIL>
+constexpr int frag_xchg_floats() { return 8 * 2 * DIL * G; }
+// On return register 4(j + G/8) + r of acc[h] (the P1 registers) holds ((left + P1) + right) * corr for row 64h + 16wq + l/4 +
+// 8(r/2), channel 8j + 2(l%4) + r%2.  Neighbours outside the image row (tile rows with m % W < DIL or >= W - DIL, W = tile row
+// width) are +0, as the zero padding of the conv.  `bar`: this warpgroup's named barrier between the seam writes and reads.
+template <int G, int DIL, int W>
+__device__ __forceinline__ void frag_unshift(float (&acc)[2][3 * G / 2], float* xb, int wq, int lane, float corr, int bar) {
+  constexpr int SIDE = DIL * G;
+  const int l4 = lane >> 2, c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* grp = xb + (4 * h + wq) * 2 * SIDE;
+    if (l4 >= 8 - DIL) {
+#pragma unroll
+      for (int j = 0; j < G / 8; ++j)
+        *reinterpret_cast<float2*>(grp + (l4 - 8 + DIL) * G + 8 * j + c0) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+    }
+    if (l4 < DIL) {
+#pragma unroll
+      for (int j = 0; j < G / 8; ++j)
+        *reinterpret_cast<float2*>(grp + SIDE + l4 * G + 8 * j + c0) =
+            make_float2(acc[h][4 * (j + G / 4)], acc[h][4 * (j + G / 4) + 1]);
+    }
+  }
+  named_bar_sync(bar, 128);
+  const int src_l = (lane - 4 * DIL) & 31, src_r = (lane + 4 * DIL) & 31;
+  // a sender whose left-shuffle receiver wraps around to lanes 0 .. 4 DIL - 1 holds that receiver's hi-row neighbour in its lo row
+  // register; likewise for the right shuffle
+  const bool wrap_l = l4 >= 8 - DIL, wrap_r = l4 < DIL;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int g = 4 * h + wq;
+    // seam values, loaded unconditionally from clamped addresses and merged with selects
+    const float* xl = xb + (g > 0 ? g - 1 : 0) * 2 * SIDE + (l4 < DIL ? l4 : 0) * G + c0;
+    const float* xr = xb + (g < 7 ? g + 1 : 7) * 2 * SIDE + SIDE + (l4 >= 8 - DIL ? l4 - 8 + DIL : 0) * G + c0;
+    const int mlo = (64 * h + 16 * wq + l4) % W, mhi = (64 * h + 16 * wq + 8 + l4) % W;
+#pragma unroll
+    for (int j = 0; j < G / 8; ++j) {
+      const float2 sl = *reinterpret_cast<const float2*>(xl + 8 * j);
+      const float2 sr = *reinterpret_cast<const float2*>(xr + 8 * j);
+#pragma unroll
+      for (int c2 = 0; c2 < 2; ++c2) {
+        const float p0lo = acc[h][4 * j + c2], p0hi = acc[h][4 * j + 2 + c2];
+        const float p2lo = acc[h][4 * (j + G / 4) + c2], p2hi = acc[h][4 * (j + G / 4) + 2 + c2];
+        float llo = __shfl_sync(0xffffffffu, p0lo, src_l);
+        float lhi = __shfl_sync(0xffffffffu, wrap_l ? p0lo : p0hi, src_l);
+        float rlo = __shfl_sync(0xffffffffu, wrap_r ? p2hi : p2lo, src_r);
+        float rhi = __shfl_sync(0xffffffffu, p2hi, src_r);
+        llo = (l4 < DIL) ? (c2 ? sl.y : sl.x) : llo;
+        rhi = (l4 >= 8 - DIL) ? (c2 ? sr.y : sr.x) : rhi;
+        llo = (mlo < DIL) ? 0.f : llo;
+        lhi = (mhi < DIL) ? 0.f : lhi;
+        rlo = (mlo >= W - DIL) ? 0.f : rlo;
+        rhi = (mhi >= W - DIL) ? 0.f : rhi;
+        float& olo = acc[h][4 * (j + G / 8) + c2];
+        float& ohi = acc[h][4 * (j + G / 8) + 2 + c2];
+        olo = ((llo + olo) + rlo) * corr;
+        ohi = ((lhi + ohi) + rhi) * corr;
+      }
+    }
+  }
+}
+// Channels-last output tile of one consumer warp: 16 fragment rows x 32 channels.  40 floats per row: the STS.64 of a half-warp
+// (rows l/4, channel pairs 2(l%4)) hit distinct banks, and rows stay 16-byte aligned for the LDS.128 reads.
+constexpr int FRAG_TP_STRIDE = 40;
+constexpr int FRAG_TP_FLOATS = 16 * FRAG_TP_STRIDE;
+// Folded BN, residual, activation and gate on the un-shifted fragments (frag_unshift), in that order, then the stores.  Row (h, rh)
+// of this thread is tile row 64h + 16wq + l/4 + 8rh.  y / res / gate point at channel 0 of the tile's channel group;
+// rows(m, yo, ro, go) sets tile row m's offsets into them and returns whether the row is stored.  ycs / rcs are the channel
+// strides (1: channels-last, else NCDHW planes); nch: channels of the group that exist (channels-last callers pass G); sc / sh:
+// the group's folded BN in shared memory; gate: channels-last only.
+//   * channels-last output and residual (G = 32): the warp passes each m64 half's 16 rows through its own tile `tbuf`
+//     (FRAG_TP_FLOATS), so that every LDG.128 / STG.128 of the warp covers 4 whole 128-byte rows: a store straight from the
+//     fragments (32 bytes of each of 8 rows per instruction) needs 4x the L1 wavefronts on the data path the MMAs' operand reads
+//     also use.  BN, residual, activation and gate run on the transposed values, where a lane's 4 channels are fixed.
+//   * otherwise straight from the fragments: NCDHW planes take 8 consecutive voxels of 4 channels per warp instruction.
+template <int G, class Rows>
+__device__ __forceinline__ void frag_epilogue(const float (&acc)[2][3 * G / 2], int lane, int wq, float* tbuf, const float* sc,
+                                              const float* sh, int act, float* y, size_t ycs, const float* res, size_t rcs,
+                                              const float* gate, Rows rows, int nch) {
+  const int c0 = 2 * (lane & 3), l4 = lane >> 2;
+  if constexpr (G == 32) {
+    if (ycs == 1 && (!res || rcs == 1)) {
+      const int c4 = 4 * (lane & 7), sub = lane >> 3;
+      const float4 a = *reinterpret_cast<const float4*>(sc + c4);
+      const float4 b = *reinterpret_cast<const float4*>(sh + c4);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        __syncwarp();                                   // the previous half's readers are done with the tile
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh)
+            *reinterpret_cast<float2*>(tbuf + (8 * rh + l4) * FRAG_TP_STRIDE + 8 * j + c0) =
+                make_float2(acc[h][4 * (j + 4) + 2 * rh], acc[h][4 * (j + 4) + 2 * rh + 1]);
+        __syncwarp();
+        float4 o[4];
+        ptrdiff_t yo[4], ro[4], go[4];
+        bool ok[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {                   // tile row 4i + sub, channels c4 .. c4 + 3
+          ok[i] = rows(64 * h + 16 * wq + 4 * i + sub, yo[i], ro[i], go[i]);
+          o[i] = *reinterpret_cast<const float4*>(tbuf + (4 * i + sub) * FRAG_TP_STRIDE + c4);
+          o[i].x = fmaf(o[i].x, a.x, b.x), o[i].y = fmaf(o[i].y, a.y, b.y), o[i].z = fmaf(o[i].z, a.z, b.z), o[i].w = fmaf(o[i].w, a.w, b.w);
+        }
+        if (res) {
+          float4 r[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) r[i] = ok[i] ? __ldg(reinterpret_cast<const float4*>(res + ro[i] + c4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) o[i].x += r[i].x, o[i].y += r[i].y, o[i].z += r[i].z, o[i].w += r[i].w;
+        }
+        if (act == OSB_ACT_RELU) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) o[i].x = fmaxf(o[i].x, 0.f), o[i].y = fmaxf(o[i].y, 0.f), o[i].z = fmaxf(o[i].z, 0.f), o[i].w = fmaxf(o[i].w, 0.f);
+        } else if (act == OSB_ACT_LEAKY) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            o[i].x = o[i].x > 0.f ? o[i].x : 0.01f * o[i].x, o[i].y = o[i].y > 0.f ? o[i].y : 0.01f * o[i].y;
+            o[i].z = o[i].z > 0.f ? o[i].z : 0.01f * o[i].z, o[i].w = o[i].w > 0.f ? o[i].w : 0.01f * o[i].w;
+          }
+        }
+        if (gate) {
+          float4 g[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) g[i] = ok[i] ? __ldg(reinterpret_cast<const float4*>(gate + go[i] + c4)) : make_float4(1.f, 1.f, 1.f, 1.f);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) o[i].x *= g[i].x, o[i].y *= g[i].y, o[i].z *= g[i].z, o[i].w *= g[i].w;
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (ok[i]) *reinterpret_cast<float4*>(y + yo[i] + c4) = o[i];
+      }
+      return;
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    // one m64 half at a time, its residual and gate loads batched ahead of its stores (the compiler does not move a load across
+    // a store that may alias it, so per-element loads would expose one memory latency each)
+    float2 rv[G / 8][2], gv[G / 8][2];
+#pragma unroll
+    for (int j = 0; j < G / 8; ++j)
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        const int c = 8 * j + c0;
+        ptrdiff_t yo, ro, go;
+        const bool live = rows(64 * h + 16 * wq + l4 + 8 * rh, yo, ro, go);
+        rv[j][rh] = make_float2(0.f, 0.f);
+        gv[j][rh] = make_float2(1.f, 1.f);
+        if (res) {
+          if (rcs == 1) {
+            if (live) rv[j][rh] = __ldg(reinterpret_cast<const float2*>(res + ro + c));
+          } else {
+            if (live && c < nch) rv[j][rh].x = __ldg(res + ro + (size_t)c * rcs);
+            if (live && c + 1 < nch) rv[j][rh].y = __ldg(res + ro + (size_t)(c + 1) * rcs);
+          }
+        }
+        if (gate && live) gv[j][rh] = __ldg(reinterpret_cast<const float2*>(gate + go + c));
+      }
+#pragma unroll
+    for (int j = 0; j < G / 8; ++j) {
+      const int c = 8 * j + c0;
+      const float2 a = *reinterpret_cast<const float2*>(sc + c);
+      const float2 b = *reinterpret_cast<const float2*>(sh + c);
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        ptrdiff_t yo, ro, go;
+        const bool live = rows(64 * h + 16 * wq + l4 + 8 * rh, yo, ro, go);
+        float v0 = fmaf(acc[h][4 * (j + G / 8) + 2 * rh], a.x, b.x);
+        float v1 = fmaf(acc[h][4 * (j + G / 8) + 2 * rh + 1], a.y, b.y);
+        if (res) v0 += rv[j][rh].x, v1 += rv[j][rh].y;
+        if (act == OSB_ACT_RELU) {
+          v0 = fmaxf(v0, 0.f), v1 = fmaxf(v1, 0.f);
+        } else if (act == OSB_ACT_LEAKY) {
+          v0 = v0 > 0.f ? v0 : 0.01f * v0, v1 = v1 > 0.f ? v1 : 0.01f * v1;
+        }
+        if (gate) v0 *= gv[j][rh].x, v1 *= gv[j][rh].y;
+        if (!live) continue;
+        if (ycs == 1) {
+          *reinterpret_cast<float2*>(y + yo + c) = make_float2(v0, v1);
+        } else {
+          if (c < nch) y[yo + (size_t)c * ycs] = v0;
+          if (c + 1 < nch) y[yo + (size_t)(c + 1) * ycs] = v1;
+        }
+      }
+    }
+  }
+}
 
 // ------------------------------------------------------------------------------- coalesced channels-last epilogue output
 // An epilogue thread owns ONE voxel and all of its channels.  Storing those directly makes every STG.128 of a warp touch
