@@ -288,6 +288,22 @@ int osb_coex_regression_fwd(const float* cost, const float* spx, float* out, int
                             osb_stream_t stream);
 int osb_nearest_resize3d_fwd(const float* x, float* y, int N, int Di, int Hi, int Wi, int Do, int Ho, int Wo, osb_stream_t stream);
 
+/* ---- MSNet3D (msnet/submodule.py:136-173) ------------------------------------------------------------------------------------
+ * osb_mbv2_block3d_fwd: one whole MobileV2_Residual_3D block in one launch, IEEE fp32 on the CUDA cores:
+ *   y = scale3 * (w_proj . relu6(scale2 * dw3x3x3_stride(relu6(scale1 * (w_exp . x) + shift1)) + shift2)) + shift3 [+ residual]
+ *   (the three eval BatchNorms folded to per-channel scale/shift).  The expanded tensor never reaches global memory.
+ *   x (B,Cin,D,H,W) with in_layout = 0 or (B,D,H,W,Cin) with in_layout = 1; y and the optional residual (NULL = none) are
+ *   (B,Cout,Do,Ho,Wo) with out_layout = 0 or (B,Do,Ho,Wo,Cout) with out_layout = 1, where n_o = ceil(n / stride) (k3, padding 1).
+ *   w_exp (Cin, Chid), w_dw (27, Chid) with tap = (kd * 3 + kh) * 3 + kw, w_proj (Chid, Cout).  The depthwise conv zero-pads
+ *   the HIDDEN tensor: outside the volume the expanded value is 0, not relu6(shift1).  Any D, H, W >= 1.
+ *   Instantiated (Cin, Chid, Cout, stride): (40,120,32,1) (32,96,32,1) (32,64,32,1) (32,64,64,2) (64,128,64,1) (64,128,128,2)
+ *   (128,256,128,1); anything else is OSB_EINVAL.  Weights and BN vectors 16-byte aligned, and y / residual too when
+ *   out_layout = 1; y must not alias x. */
+int osb_mbv2_block3d_fwd(const float* x, const float* w_exp, const float* scale1, const float* shift1, const float* w_dw,
+                         const float* scale2, const float* shift2, const float* w_proj, const float* scale3, const float* shift3,
+                         const float* residual, float* y, int B, int Cin, int Chid, int Cout, int D, int H, int W, int stride,
+                         int in_layout, int out_layout, osb_stream_t stream);
+
 /* Backward (adjoint) kernels so the volume constructors and the soft-argmin stay differentiable under tools/train.py
  * (openstereo_b200/autograd.py wraps them in torch.autograd.Function).  grad_ref / grad_tgt may be NULL when not needed.
  *   osb_gwc_volume_bwd     adjoint of osb_gwc_volume_fwd (reduce_sum = 0) / osb_gwc_volume_sum_fwd (1): grad_vol (B,G,D,H,W)

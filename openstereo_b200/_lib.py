@@ -66,6 +66,7 @@ SIGNATURES = {
     "osb_warped_gwc_concat_volume_fwd": [_f32p] * 6 + [_i] * 7 + [_s],
     "osb_coex_regression_fwd": [_f32p] * 3 + [_i] * 6 + [_s],
     "osb_nearest_resize3d_fwd": [_f32p] * 2 + [_i] * 7 + [_s],
+    "osb_mbv2_block3d_fwd": [_f32p] * 12 + [_i] * 10 + [_s],
 }
 
 

@@ -14,6 +14,7 @@ Graphs restated (file:line of the reference forward each engine replaces):
   StereoBaseAggregation stereobase/hourglass.py:79-104 + stereobase_gru.py:161-164
   LightStereoAggregation lightstereo/aggregation.py:42-60 (Aggregation.forward), :94-101 (MobileV2Residual), :119-134 (AttentionModule)
   CoExAggregation       coex/coex_cost_processor.py:196-237 (Aggregation.forward), :68-80 (channelAtt)
+  MSNet3DAggregation    msnet/MSNet3D.py:118-161 (eval forward after the volume), :10-46 (hourglass3D), submodule.py:136-173
 """
 import torch
 
@@ -222,6 +223,22 @@ def _gwc_hourglass_channels_last(hg, x):
     return ops.deconv3d_k3_tc(c5, _dc_weight(hg.conv6), hg.conv6.scale, hg.conv6.shift, r1, ACT_RELU, out_ndhwc=True, res_ndhwc=True)
 
 
+def _classif3_channels_last(classif3, out):
+    """classif3 (conv+BN+ReLU, then the 32 -> 1 conv) on a channels-last volume -> (B,1,D,H,W) logits.  The first conv must have a
+    tensor-core variant for the width."""
+    head0, cls = classif3
+    width = out.shape[3]
+    if _tc_ok(cls, width):                                         # 32 -> 1 head on the narrow (Cout <= 16) tensor-core variant
+        return _conv_tc(cls, _conv_tc(head0, out, ACT_RELU), ACT_NONE, out_ndhwc=False, res_ndhwc=False)
+    if cls.cin == 32 and cls.cout == 1 and cls._w5 is not None and cls.stride == 1:
+        if "c1" not in cls._tc:
+            cls._tc["c1"] = ops.pack_c1_weight(cls._w5)
+        head = _conv_tc(head0, out, ACT_RELU)                      # stays channels-last for the 1-channel head
+        return ops.conv3d_k3_c1_ndhwc(head, cls._tc["c1"], cls.scale, cls.shift)
+    head = _conv_tc(head0, out, ACT_RELU, out_ndhwc=False)
+    return _conv(cls, head)
+
+
 class GwcAggregation(_Engine):
     """Eval branch of GwcDispProcessor: volume (B,64,D',H',W') -> disparity (B,H,W)."""
 
@@ -244,16 +261,7 @@ class GwcAggregation(_Engine):
             out = _conv_tc(self.dres1[1], _conv_tc(self.dres1[0], c, ACT_RELU), ACT_NONE, residual=c)
             for hg in self.hg:
                 out = _gwc_hourglass_channels_last(hg, out)
-            cls = self.classif3[1]
-            if _tc_ok(cls, width):                                         # 32 -> 1 head on the narrow (Cout <= 16) tensor-core variant
-                return _conv_tc(cls, _conv_tc(self.classif3[0], out, ACT_RELU), ACT_NONE, out_ndhwc=False, res_ndhwc=False)
-            if cls.cin == 32 and cls.cout == 1 and cls._w5 is not None and cls.stride == 1:
-                if "c1" not in cls._tc:
-                    cls._tc["c1"] = ops.pack_c1_weight(cls._w5)
-                head = _conv_tc(self.classif3[0], out, ACT_RELU)           # stays channels-last for the 1-channel head
-                return ops.conv3d_k3_c1_ndhwc(head, cls._tc["c1"], cls.scale, cls.shift)
-            head = _conv_tc(self.classif3[0], out, ACT_RELU, out_ndhwc=False)
-            return _conv(cls, head)
+            return _classif3_channels_last(self.classif3, out)
         if stem_tc:
             # full-resolution stem on the tensor cores: channels-last inside, NCDHW handed to the hourglasses
             c = _conv_tc(self.dres0[1], _stem_in(self.dres0[0], volume, ACT_RELU), ACT_RELU)
@@ -713,6 +721,160 @@ class CoExAggregation(_Engine):
             x = ops.conv3d_1x1(x, sl.w, sl.scale, sl.shift, act=sa, x1=skip)
             x = self._seq(self.agg[i], x, self.att[i] if self.gce else None, img[-i - 2])
         return x
+
+
+# ------------------------------------------------------------------------------------------------------ MSNet3D
+def _mbv2_check(m, name):
+    """Refuse a MobileV2_Residual_3D (msnet/submodule.py:136-173) that osb_mbv2_block3d_fwd does not implement, naming it."""
+    layers = list(m.conv)
+    if len(layers) != 8:
+        raise NotImplementedError("openstereo_b200: %s uses the expanse_ratio == 1 branch (no 1x1x1 expansion); only the expanding "
+                                  "MobileV2_Residual_3D has a kernel" % name)
+    pw, bn1, a1, dw, bn2, a2, pl, bn3 = layers
+    conv, bn = torch.nn.Conv3d, torch.nn.BatchNorm3d
+    ok = all(isinstance(l, conv) for l in (pw, dw, pl)) and all(isinstance(l, bn) for l in (bn1, bn2, bn3))
+    ok = ok and all(isinstance(l, torch.nn.ReLU6) for l in (a1, a2))
+    ok = ok and all(l.bias is None and tuple(l.dilation) == (1, 1, 1) and l.padding_mode == "zeros" for l in (pw, dw, pl))
+    ok = ok and all(tuple(l.kernel_size) == (1, 1, 1) and tuple(l.stride) == (1, 1, 1) and tuple(l.padding) == (0, 0, 0)
+                    and l.groups == 1 for l in (pw, pl))
+    hid = pw.out_channels if ok else 0
+    ok = ok and tuple(dw.kernel_size) == (3, 3, 3) and tuple(dw.padding) == (1, 1, 1) and dw.stride in ((1, 1, 1), (2, 2, 2))
+    ok = ok and dw.in_channels == dw.out_channels == dw.groups == hid and pl.in_channels == hid
+    if not ok:
+        raise NotImplementedError("openstereo_b200: %s is not the block osb_mbv2_block3d_fwd implements (1x1x1 expand + BN + ReLU6, "
+                                  "depthwise 3x3x3 stride 1/2 padding 1 with groups == hidden + BN + ReLU6, 1x1x1 project + BN, "
+                                  "no bias, no dilation)" % name)
+    key = (pw.in_channels, hid, pl.out_channels, dw.stride[0])
+    if key not in _MBV2_CONFIGS:
+        raise NotImplementedError("openstereo_b200: %s has (Cin, Chid, Cout, stride) = %s; osb_mbv2_block3d_fwd is instantiated for "
+                                  "%s" % (name, key, sorted(_MBV2_CONFIGS)))
+
+
+_MBV2_CONFIGS = {(40, 120, 32, 1), (32, 96, 32, 1), (32, 64, 32, 1), (32, 64, 64, 2), (64, 128, 64, 1), (64, 128, 128, 2),
+                 (128, 256, 128, 1)}
+
+
+class _MBV2Block3D:
+    """MobileV2_Residual_3D packed for osb_mbv2_block3d_fwd: the three BNs folded, w_exp (Cin, Chid), w_dw (27, Chid),
+    w_proj (Chid, Cout).  use_res_connect is honoured as the module computes it (False for every block MSNet3D builds: its int
+    stride never equals (1, 1, 1))."""
+
+    def __init__(self, m, name):
+        _mbv2_check(m, name)
+        pw, bn1, _, dw, bn2, _, pl, bn3 = list(m.conv)
+        self.cin, self.hid, self.cout, self.stride = pw.in_channels, pw.out_channels, pl.out_channels, dw.stride[0]
+        self.w_exp = pw.weight.detach().float().reshape(self.hid, self.cin).t().contiguous()
+        self.w_dw = dw.weight.detach().float().reshape(self.hid, 27).t().contiguous()
+        self.w_proj = pl.weight.detach().float().reshape(self.cout, self.hid).t().contiguous()
+        self.bn = [ops.fold_bn(b) for b in (bn1, bn2, bn3)]
+        if any(b.training for b in (bn1, bn2, bn3)):
+            raise RuntimeError("BatchNorm folding is only valid in eval mode (call model.eval())")
+        self.res = bool(m.use_res_connect)
+        self.name = name
+
+    def __call__(self, x, residual=None, in_ndhwc=False, out_ndhwc=False):
+        if self.res:
+            if residual is not None:
+                raise NotImplementedError("openstereo_b200: %s adds its identity and a second residual" % self.name)
+            assert out_ndhwc or not in_ndhwc
+            residual = x if in_ndhwc == out_ndhwc else ops.to_ndhwc(x)
+        (s1, b1), (s2, b2), (s3, b3) = self.bn
+        return ops.mbv2_block3d(x, self.w_exp, s1, b1, self.w_dw, s2, b2, self.w_proj, s3, b3, residual, self.stride, in_ndhwc,
+                                out_ndhwc)
+
+
+class _MSNetHourglass:
+    """hourglass3D (msnet/MSNet3D.py:10-46)."""
+
+    def __init__(self, m, name):
+        blk = lambda attr: _MBV2Block3D(getattr(m, attr), "%s.%s" % (name, attr))         # noqa: E731
+        self.conv1, self.conv2, self.conv3, self.conv4 = blk("conv1"), blk("conv2"), blk("conv3"), blk("conv4")
+        self.redir1, self.redir2 = blk("redir1"), blk("redir2")
+        self.conv5, self.conv6 = _Packed(m.conv5[0], m.conv5[1]), _Packed(m.conv6[0], m.conv6[1])
+
+    def __call__(self, x):
+        """NCDHW; relu(conv5(conv4) + redir2(conv2)) and relu(conv6(conv5) + redir1(x)) in the transposed convs' epilogues."""
+        c2 = self.conv2(self.conv1(x))
+        c4 = self.conv4(self.conv3(c2))
+        c5 = _deconv(self.conv5, c4, ACT_RELU, residual=self.redir2(c2))
+        return _deconv(self.conv6, c5, ACT_RELU, residual=self.redir1(x))
+
+    def channels_last(self, x):
+        c2 = self.conv2(self.conv1(x, in_ndhwc=True, out_ndhwc=True), in_ndhwc=True, out_ndhwc=True)
+        c4 = self.conv4(self.conv3(c2, in_ndhwc=True, out_ndhwc=True), in_ndhwc=True, out_ndhwc=True)
+        r2 = self.redir2(c2, in_ndhwc=True, out_ndhwc=True)
+        c5 = ops.deconv3d_k3_tc(c4, _dc_weight(self.conv5), self.conv5.scale, self.conv5.shift, r2, ACT_RELU, out_ndhwc=True,
+                                res_ndhwc=True)
+        r1 = self.redir1(x, in_ndhwc=True, out_ndhwc=True)
+        return ops.deconv3d_k3_tc(c5, _dc_weight(self.conv6), self.conv6.scale, self.conv6.shift, r1, ACT_RELU, out_ndhwc=True,
+                                  res_ndhwc=True)
+
+    def channels_last_ok(self, shape):
+        b, c, d, h, w = shape
+        return (USE_TENSOR_CORES and d % 4 == 0 and h % 4 == 0 and w % 4 == 0
+                and all(l._w5 is not None for l in (self.conv5, self.conv6))
+                and ops.deconv3d_tc_supported(self.conv5.cin, self.conv5.cout, w // 4)
+                and ops.deconv3d_tc_supported(self.conv6.cin, self.conv6.cout, w // 2))
+
+
+class MSNet3DAggregation(_Engine):
+    """Eval forward of MSNet3D after the cost volume (msnet/MSNet3D.py:118-161): dres0 -> dres1 (+ cost0) -> 3 x hourglass3D ->
+    classif3 -> trilinear x4 + softmax + regression.  ``module`` is the MSNet3D model; its parameters are read by the reference's
+    attribute names.  Every MobileV2_Residual_3D (22 per forward) is one osb_mbv2_block3d_fwd launch; dres1's `+ cost0` rides on
+    its last block's residual operand.  Constructing the engine checks every block, so an unsupported model is refused at once."""
+
+    def __init__(self, module):
+        super().__init__(module)
+        for name, m in self._blocks(module):
+            _mbv2_check(m, name)
+
+    @staticmethod
+    def _blocks(m):
+        for seq in ("dres0", "dres1"):
+            for i, blk in enumerate(getattr(m, seq)):
+                yield "%s.%d" % (seq, i), blk
+        for hg in ("encoder_decoder1", "encoder_decoder2", "encoder_decoder3"):
+            for attr in ("conv1", "conv2", "conv3", "conv4", "redir1", "redir2"):
+                yield "%s.%s" % (hg, attr), getattr(getattr(m, hg), attr)
+
+    def _pack(self):
+        m = self.module
+        self.dres0 = [_MBV2Block3D(b, "dres0.%d" % i) for i, b in enumerate(m.dres0)]
+        self.dres1 = [_MBV2Block3D(b, "dres1.%d" % i) for i, b in enumerate(m.dres1)]
+        self.hg = [_MSNetHourglass(getattr(m, n), n) for n in ("encoder_decoder1", "encoder_decoder2", "encoder_decoder3")]
+        self.classif3 = [_Packed(m.classif3[0][0], m.classif3[0][1]), _Packed(m.classif3[2])]
+
+    def logits(self, volume):
+        volume = self._check(volume)
+        self._ensure(volume.device)
+        shape = (volume.shape[0], self.dres0[-1].cout) + tuple(volume.shape[2:])
+        if all(hg.channels_last_ok(shape) for hg in self.hg) and _tc_ok(self.classif3[0], volume.shape[-1]):
+            # the first block reads the NCDHW volume, every later tensor is channels-last
+            c = self.dres0[0](volume, out_ndhwc=True)
+            for blk in self.dres0[1:]:
+                c = blk(c, in_ndhwc=True, out_ndhwc=True)
+            out = c
+            for i, blk in enumerate(self.dres1):
+                out = blk(out, residual=c if i == len(self.dres1) - 1 else None, in_ndhwc=True, out_ndhwc=True)
+            for hg in self.hg:
+                out = hg.channels_last(out)
+            return _classif3_channels_last(self.classif3, out)
+        c = volume
+        for blk in self.dres0:
+            c = blk(c)
+        out = c
+        for i, blk in enumerate(self.dres1):
+            out = blk(out, residual=c if i == len(self.dres1) - 1 else None)
+        for hg in self.hg:
+            out = hg(out)
+        return _conv_auto(self.classif3[1], _conv_auto(self.classif3[0], out, ACT_RELU))
+
+    def __call__(self, volume, h, w):
+        mon = self._watch(volume.device)
+        out = ops.upsample_softargmin(self.logits(volume), self.module.maxdisp, h, w, align_corners=False)
+        if mon is not None:
+            mon.poll()
+        return out
 
 
 # -------------------------------------------------------------------------------------------------- LightStereo

@@ -428,6 +428,37 @@ def nearest_resize3d(x, size):
     return out.to(dt)
 
 
+def mbv2_block3d(x, w_exp, scale1, shift1, w_dw, scale2, shift2, w_proj, scale3, shift3, residual=None, stride=1,
+                 in_ndhwc=False, out_ndhwc=False):
+    """MSNet3D's MobileV2_Residual_3D (msnet/submodule.py:136-173) in one launch: 1x1x1 expand + BN + ReLU6, depthwise 3x3x3
+    (stride 1 or 2, padding 1) + BN + ReLU6, 1x1x1 project + BN, + residual.  BNs folded to (scale, shift); w_exp (Cin, Chid),
+    w_dw (27, Chid) tap-major, w_proj (Chid, Cout).  x (B,Cin,D,H,W), or (B,D,H,W,Cin) with in_ndhwc; the result and the residual
+    are (B,Cout,Do,Ho,Wo), or (B,Do,Ho,Wo,Cout) with out_ndhwc, n_o = ceil(n / stride).  CUDA fp32 contiguous tensors.  No backward."""
+    _no_autograd("mbv2_block3d", x, w_exp, w_dw, w_proj, residual)
+    ts = [x, w_exp, scale1, shift1, w_dw, scale2, shift2, w_proj, scale3, shift3] + ([] if residual is None else [residual])
+    for t in ts:
+        if not t.is_cuda:
+            raise RuntimeError("mbv2_block3d: not implemented on the CPU (openstereo_b200 has no CPU fallback)")
+        assert t.dtype == torch.float32 and t.is_contiguous()
+    _same_device(*ts)
+    assert x.dim() == 5
+    if in_ndhwc:
+        b, d, h, w, cin = x.shape
+    else:
+        b, cin, d, h, w = x.shape
+    chid, cout = w_exp.shape[1], w_proj.shape[1]
+    assert tuple(w_exp.shape) == (cin, chid) and tuple(w_dw.shape) == (27, chid) and tuple(w_proj.shape) == (chid, cout)
+    do, ho, wo = (d - 1) // stride + 1, (h - 1) // stride + 1, (w - 1) // stride + 1
+    shape = (b, do, ho, wo, cout) if out_ndhwc else (b, cout, do, ho, wo)
+    y = torch.empty(shape, dtype=torch.float32, device=x.device)
+    if residual is not None:
+        assert tuple(residual.shape) == shape
+    _call("osb_mbv2_block3d_fwd", x.data_ptr(), w_exp.data_ptr(), scale1.data_ptr(), shift1.data_ptr(), w_dw.data_ptr(),
+          scale2.data_ptr(), shift2.data_ptr(), w_proj.data_ptr(), scale3.data_ptr(), shift3.data_ptr(), _ptr(residual), y.data_ptr(),
+          b, cin, chid, cout, d, h, w, int(stride), 1 if in_ndhwc else 0, 1 if out_ndhwc else 0, _stream(y))
+    return y
+
+
 def epe_partial(disp_pred, disp_gt, maxdisp):
     """Per-image {sum |pred-gt| over 0<gt<maxdisp, #valid} -> (B, 2) fp32
     (metric_per_image.py:32-41 with the mask of trainer_template.py:288)."""

@@ -1,6 +1,6 @@
-"""patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / CoEx,
-and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume hot
-path on the sm_90a kernels.
+"""patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / CoEx /
+MSNet3D, and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
+hot path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each
 needs its own rebinding:
@@ -12,6 +12,8 @@ needs its own rebinding:
 * LightStereo / IGEVStereo  like StereoBase: names imported into lightstereo.py:4-6 / igev_stereo.py:1-3 (``from .submodule import *``)
 * CasStereo   ``get_cv`` (GetCostVolume) and ``cost_agg[i]`` (CostAggregation) modules  -> per-instance ``forward`` overrides
 * CoEx        ``CostProcessor`` / ``DispProcessor`` / ``DispProcessor.regression`` modules -> per-instance ``forward`` overrides
+* MSNet3D     one monolithic ``forward`` (MSNet3D.py:110-161), no processor modules   -> per-instance ``model.forward`` override that
+                                                                                keeps the reference's ``feature_extraction``
 * StereoBase  functions imported INTO the module namespace (stereobase_gru.py:5-6,10-11) and the ``cost_agg``
               Hourglass                                                      -> per-INSTANCE copies of the methods that use those names,
                                                                                 with a private globals dict (the module itself, and
@@ -437,11 +439,32 @@ def _patch_coex(model, strict, backbone=True):
     return model
 
 
+def _patch_msnet3d(model, strict, backbone=True):
+    """MSNet3D (msnet/MSNet3D.py): everything after the 2D features in the eval forward -- the gwc volume, the MobileV2_Residual_3D
+    blocks (one fused launch each), the hourglass transposed convs, classif3 and the trilinear x4 + softmax + regression tail
+    (``model.forward``, per instance).  The MobileNet 2D feature extractor stays the reference's code; `backbone` has no effect.
+    A block the kernel does not implement is refused here, naming it."""
+    from .aggregation import MSNet3DAggregation
+    engine = MSNet3DAggregation(model)
+    orig = model.forward                                              # the reference's bound method
+
+    def forward(self, data):
+        left, right = data["left"], data["right"]
+        if _trainable(self) or not _accelerable(self, left, right):
+            return orig(data) if not strict else _refuse("MSNet3D")
+        fl, fr = self.feature_extraction(left), self.feature_extraction(right)
+        volume = ops.build_gwc_volume(fl, fr, self.maxdisp // 4, self.num_groups)
+        return {"disp_pred": engine(volume, left.shape[2], left.shape[3]).to(left.dtype)}
+
+    model.forward = types.MethodType(forward, model)
+    return model
+
+
 # CasStereo's classes are also named PSMNet / GwcNet: they are told apart by the module that defines them
 _CASCADE_MODULES = {("casnet", "cas_psm"): "PSMNet", ("casnet", "cas_gwc"): "GwcNet"}
 
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
-             "IGEVStereo": _patch_igev, "CoEx": _patch_coex}
+             "IGEVStereo": _patch_igev, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
 
 
 def patch(model, strict=True, backbone=True):

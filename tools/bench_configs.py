@@ -16,6 +16,9 @@
   c7  CoEx cfgs/coex (the reference's class + patch()), batch 8 @256x512 and @540x960: whole-model forward next to the unpatched
       model on the same GPU, per-stage volume / aggregation / regression times, the fused tail against the reference's tail
       (python tools/bench_configs.py --only c7)
+  c8  MSNet3D cfgs/msnet/msnet3d_sceneflow.yaml (the reference's class + patch()), batch 8 @256x512 and @512x960: whole-model
+      forward next to the unpatched model on the same GPU (timed alternately), per-stage volume / aggregation / tail times, and
+      per MobileV2_Residual_3D config the fused block's time, TFLOP/s and GB/s  (python tools/bench_configs.py --only c8)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -362,6 +365,100 @@ def c7(iters, B=8):
              epe_vs_reference_gpu_px=float("%.3e" % (got - want).abs().mean().item()), disparity_std_px=round(want.std().item(), 2))
 
 
+def _mbv2_rows(eng, prof, B, d, h, w):
+    """Per (Cin, Chid, Cout, stride) config of the fused MobileV2_Residual_3D block: launches, kernel ms, fp32 TFLOP/s on the
+    algorithmic MACs Vin*Cin*Chid + Vout*27*Chid + Vout*Chid*Cout, GB/s on the algorithmic bytes 4*(Vin*Cin + Vout*Cout [+ Vout*Cout
+    residual]), and which bound (67 TFLOP/s fp32, 3.35 TB/s HBM) is the larger."""
+    blocks = list(eng.dres0) + list(eng.dres1)
+    for hg in eng.hg:
+        blocks += [hg.conv1, hg.conv2, hg.conv3, hg.conv4, hg.redir2, hg.redir1]           # launch order
+    events = prof["osb_mbv2_block3d_fwd"]
+    assert len(events) == len(blocks) == 22
+    rows = {}
+    for blk, (a, b) in zip(blocks, events):
+        dims_in = _mbv2_dims(eng, blk, d, h, w)
+        vin = B * dims_in[0] * dims_in[1] * dims_in[2]
+        vout = B * ((dims_in[0] - 1) // blk.stride + 1) * ((dims_in[1] - 1) // blk.stride + 1) * ((dims_in[2] - 1) // blk.stride + 1)
+        res = blk is eng.dres1[-1]
+        macs = vin * blk.cin * blk.hid + vout * 27 * blk.hid + vout * blk.hid * blk.cout
+        byts = 4 * (vin * blk.cin + vout * blk.cout * (2 if res else 1))
+        key = "%d-%d-%d-s%d" % (blk.cin, blk.hid, blk.cout, blk.stride)
+        r = rows.setdefault(key, {"launches": 0, "ms": 0.0, "macs": 0, "bytes": 0})
+        r["launches"] += 1
+        r["ms"] += a.elapsed_time(b)
+        r["macs"] += macs
+        r["bytes"] += byts
+    for key, r in rows.items():
+        tflops = 2 * r["macs"] / r["ms"] / 1e9
+        gbps = r["bytes"] / r["ms"] / 1e6
+        r.update(ms=round(r["ms"], 3), TFLOPs=round(tflops, 2), GBps=round(gbps, 1),
+                 bound="fp32 FMA" if 2 * r["macs"] / 67e12 > r["bytes"] / 3.35e12 else "HBM",
+                 frac_of_bound=round(max(tflops / 67.0, gbps / 3350.0), 3))
+        del r["macs"], r["bytes"]
+    return rows
+
+
+def _mbv2_dims(eng, blk, d, h, w):
+    """Input extents of a block of MSNet3DAggregation for a (d, h, w) volume: full resolution except inside the hourglasses."""
+    for hg in eng.hg:
+        if blk in (hg.conv1, hg.redir1):
+            return (d, h, w)
+        if blk in (hg.conv2, hg.conv3, hg.redir2):
+            return (-(-d // 2), -(-h // 2), -(-w // 2))
+        if blk is hg.conv4:
+            return (-(-d // 4), -(-h // 4), -(-w // 4))
+    return (d, h, w)
+
+
+def c8(iters, B=8):
+    """MSNet3D (the reference's own class, cfgs/msnet/msnet3d_sceneflow.yaml unchanged, seeded and sharpened weights) at 256x512 and
+    at the cfg's eval crop 512x960, batch 8: patch() against the unpatched model on this GPU (cuDNN fp32, TF32 off), timed
+    alternately in the same process; per-stage times of the patched forward (volume, aggregation, tail) from CUDA events around
+    each launch; per block config the fused kernel's time and rates (_mbv2_rows)."""
+    from oracle import msnet as oms
+    from openstereo_b200.patch import patch
+    from oracle import _reference_shim as shim
+    shim_cfg = shim.load_cfg("cfgs/msnet/msnet3d_sceneflow.yaml").MODEL
+    cls = oms.load_reference("stereo.modeling.models.msnet.MSNet3D").MSNet3D
+    for (h, w) in ((256, 512), (512, 960)):
+        ref = cls(shim_cfg).eval()
+        ref.load_state_dict(si.seeded_state_dict(ref.state_dict(), seed=1, scale=oms.MSNET3D_SCALE))
+        ref.to(DEV)
+        pm = cls(shim_cfg).eval()
+        pm.load_state_dict(ref.state_dict())
+        patch(pm.to(DEV))
+        gen = torch.Generator().manual_seed(23)
+        x = {"left": rnd(gen, B, 3, h, w), "right": rnd(gen, B, 3, h, w)}
+        with torch.no_grad():
+            ms_ref, ms = [], []
+            for _ in range(3):                                          # alternate: the two share the GPU's state
+                t, want = timeit(lambda: ref(dict(x))["disp_pred"], max(1, iters // 5), warm=1)
+                ms_ref.append(t)
+                t, got = timeit(lambda: pm(dict(x))["disp_pred"], iters, warm=2)
+                ms.append(t)
+            ms_ref, ms = sorted(ms_ref)[1], sorted(ms)[1]
+            ops.profile_start()
+            pm(dict(x))
+            torch.cuda.synchronize()
+            prof = ops.profile_stop()
+        eng = agg.MSNet3DAggregation(pm)                                # the same blocks, in the patched forward's launch order
+        eng._ensure(DEV)
+        span = lambda name: round(sum(a.elapsed_time(b) for a, b in prof.get(name, [])), 3)         # noqa: E731
+        total = round(sum(a.elapsed_time(b) for evs in prof.values() for a, b in evs), 3)
+        stages = {"volume": span("osb_gwc_volume_fwd"), "tail": span("osb_upsample_softargmin_fwd")}
+        stages["aggregation"] = round(total - stages["volume"] - stages["tail"], 3)
+        stages["mbv2_blocks"] = span("osb_mbv2_block3d_fwd")
+        d4, h4, w4 = shim_cfg.MAX_DISP // 4, h // 4, w // 4
+        emit(config="c8 MSNet3D cfgs/msnet/msnet3d_sceneflow.yaml, B=%d @%dx%d (reference class + patch())" % (B, h, w),
+             gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+             ms_per_step=round(ms, 3), pairs_per_s=round(B * 1e3 / ms, 2), reference_cudnn_fp32_ms=round(ms_ref, 2),
+             reference_pairs_per_s=round(B * 1e3 / ms_ref, 2), speedup_vs_reference_gpu=round(ms_ref / ms, 2),
+             stage_ms=stages, block_configs=_mbv2_rows(eng, prof, B, d4, h4, w4),
+             epe_vs_reference_gpu_px=float("%.3e" % (got - want).abs().mean().item()), disparity_std_px=round(want.std().item(), 2))
+        del ref, pm, eng, prof
+        torch.cuda.empty_cache()
+
+
 def _stage_times(run, targets, volume_fn=None):
     """One run of `run` with CUDA events around the forward of each target (a module, or a class whose __call__ is wrapped) and,
     with volume_fn, around ops.<volume_fn>: {stage: ms}."""
@@ -418,7 +515,7 @@ if __name__ == "__main__":
     a = ap.parse_args()
     for name in a.only.split(","):
         try:
-            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7}[name](a.iters)
+            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:

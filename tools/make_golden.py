@@ -29,6 +29,7 @@ from oracle import cost_volume as ocv                           # noqa: E402
 from oracle import geo_lookup as ogeo                           # noqa: E402
 from oracle import lightstereo as olight                        # noqa: E402
 from oracle import models as omodels                            # noqa: E402
+from oracle import msnet as oms                                 # noqa: E402
 from oracle import regression as oreg                           # noqa: E402
 from oracle import seeded_init as si                            # noqa: E402
 
@@ -408,6 +409,50 @@ def coex():
              out=ref)
 
 
+def msnet():
+    rsub = oms.load_reference("stereo.modeling.models.msnet.submodule")
+    rm3 = oms.load_reference("stereo.modeling.models.msnet.MSNet3D")
+    with torch.no_grad():
+        # two MobileV2_Residual_3D blocks on odd extents: the first block of dres0 and a stride-2 hourglass block
+        arrays = {}
+        for i, (cin, chid, cout, stride) in enumerate(((40, 120, 32, 1), (32, 64, 64, 2))):
+            ref = rsub.MobileV2_Residual_3D(cin, cout, stride, chid / cin).eval()
+            mine = oms.MobileV2Residual3D(cin, cout, stride, chid / cin).eval()
+            assert not ref.use_res_connect and sorted(ref.state_dict()) == sorted(mine.state_dict())
+            seed = 130 + i
+            sd = si.seeded_state_dict(ref.state_dict(), seed=seed)
+            ref.load_state_dict(sd), mine.load_state_dict(sd)
+            x = rnd(132 + i, 1, cin, 5, 7, 9)
+            out = ref(x)
+            must_equal(out, mine(x), "MobileV2_Residual_3D %s" % ((cin, chid, cout, stride),))
+            arrays.update({"seed%d" % i: seed, "x%d" % i: x, "out%d" % i: out})
+        save("msnet_block", **arrays)
+        # the 3D part of the model (every block, the three hourglasses, classif3, the tail) on a small volume
+        cfg = shim.load_cfg("cfgs/msnet/msnet3d_sceneflow.yaml").MODEL
+        model = rm3.MSNet3D(cfg).eval()
+        agg = oms.Aggregation().eval()
+        sd = si.seeded_state_dict(agg.state_dict(), seed=134, scale=oms.MSNET3D_SCALE)
+        agg.load_state_dict(sd)
+        for name, mod in (("dres0", model.dres0), ("dres1", model.dres1), ("encoder_decoder1", model.encoder_decoder1),
+                          ("classif3", model.classif3)):
+            mod.load_state_dict({k[len(name) + 1:]: v for k, v in sd.items() if k.startswith(name + ".")})
+        vol = rnd(135, 1, 40, 8, 8, 8)
+        hg = model.encoder_decoder1(model.dres0(vol))
+        must_equal(hg, agg.encoder_decoder1(agg.dres0(vol)), "hourglass3D")
+        logits = agg.logits(vol)
+        disp = agg(vol, 32, 32)
+        save("msnet_aggregation", weight_seed=134, checksum=checksum(sd), volume=vol, logits=logits, disp=disp)
+        # the whole model from the unchanged YAML, seeded and sharpened: the reference's forward vs the restated eval forward
+        model.load_state_dict(si.seeded_state_dict(model.state_dict(), seed=1, scale=oms.MSNET3D_SCALE))
+        g = torch.Generator().manual_seed(136)
+        left, right = torch.randn(1, 3, 64, 128, generator=g), torch.randn(1, 3, 64, 128, generator=g)
+        disp = model({"left": left, "right": right})["disp_pred"]
+        must_equal(disp, oms.eval_forward(model.feature_extraction, oms.aggregation_of(model), left, right)["disp_pred"],
+                   "MSNet3D eval forward")
+        save("msnet3d_model", weight_seed=1, checksum=checksum(model.state_dict()), left=left, right=right, disp=disp,
+             disp_std=disp.std())
+
+
 class _Const(torch.nn.Module):
     def __init__(self, t):
         super().__init__()
@@ -417,7 +462,7 @@ class _Const(torch.nn.Module):
         return self.t
 
 
-SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade", "coex"]
+SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade", "coex", "msnet"]
 
 if __name__ == "__main__":
     if not shim.available():
