@@ -38,7 +38,6 @@
 //
 // Shared memory (Cout = 32): A ring 4 x 16 KB | weights 2 x 3 x 12 KB | raw rows 2 x 16 KB | per warpgroup a double-buffered
 // seam-row buffer (4 KB) | per consumer warp a 16 x 40 fp32 output tile (2.5 KB) = 202,240 of the 232,448 bytes a CTA may have.
-#include <cstdlib>
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -425,32 +424,16 @@ __global__ void __launch_bounds__(256) ncdhw_to_ndhwc_kernel(const float* __rest
 }
 
 template <int COUT>
-static int launch_tc(const TcParams& p, cudaStream_t stream) {
-  const size_t smem = TcCfg<COUT>::SMEM;
-  auto kernel = conv3d_tc_kernel<COUT>;
-  static PerDeviceFlag configured;
-  if (!configured.here()) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) {
-      set_error("conv3d_tc: cannot reserve %zu bytes of shared memory: %s", smem, cudaGetErrorString(e));
-      return OSB_ECUDA;
-    }
-    configured.here() = true;
-  }
-  const int sms = sm_count();
-  const int grid = (int)cap_persistent_grid(p.items < sms ? p.items : sms);   // persistent: one CTA per SM (its shared memory is taken)
+int launch_tc(const TcArgs& a, cudaStream_t stream) {
+  TcParams p{};
+  p.Cout = a.Cout, p.in_ncdhw = a.in_ncdhw;
+  p.bulk_rows = a.in_ncdhw || a.Cin == TC_KC;   // channels-last Cin = 64 rows are strided: register-staged
+  p.hblocks = (a.H + TC_TILES - 1) / TC_TILES;
   static const std::string variant = tc_variant_name("tc<%d>", COUT);
-  set_tc_variant(variant.c_str());
-  kernel<<<grid, TC_WG_THREADS, smem, stream>>>(p);
-  count_launch();
-  return check_launch("conv3d_tc_kernel");
+  return launch_persistent<conv3d_tc_kernel<COUT>>(a, p, (long long)a.B * a.D * p.hblocks, TcCfg<COUT>::SMEM, variant.c_str(), stream);
 }
-
-int launch_tcg_dispatch(const float* x, const void* w, const float* scale, const float* shift, const float* residual, float* y,
-                        int B, int Cin, int Cout, int D, int H, int W, int act, int out_ndhwc, int res_ndhwc, cudaStream_t stream,
-                        const float* gate = nullptr, int ystride = 0);
-int launch_tcg_dilated2(const float* x, const void* w, const float* scale, const float* shift, const float* residual, float* y,
-                        int B, int Cin, int Cout, int H, int W, int act, int out_ndhwc, int res_ndhwc, cudaStream_t stream);
+template int launch_tc<32>(const TcArgs&, cudaStream_t);
+template int launch_tc<16>(const TcArgs&, cudaStream_t);   // classifier heads (32 -> 1): NCDHW output only
 
 }  // namespace osb
 
@@ -462,16 +445,7 @@ int osb_tc_general_width(int W) { return W >= OSB_TC_MIN_WIDTH ? 1 : 0; }
 
 // K-chunk (input channels per operand tile) of the kernel variant that serves a shape; 0 = no tensor-core variant.
 int osb_conv3d_tc_kc(int Cin, int Cout, int W, int stride) {
-  if (stride != 1) return 0;
-  if (W == osb::TC_W && (Cout == 32 || (Cout >= 1 && Cout <= 16)) && Cin % 32 == 0 && Cin >= 32) return 32;   // conv3d_tc.cu (narrow
-                                                                                               // heads: weights zero-padded to 16 rows)
-  if (Cin % 16 == 0 && Cin >= 16 &&
-      ((W == 64 && Cout == 64) || (W == 32 && (Cout == 64 || Cout == 96 || Cout == 128)) || (W == 16 && (Cout == 64 || Cout == 96)) ||
-       (W == osb::TC_W && (Cout == 64 || Cout == 128))))
-    return 16;                                                                                  // conv3d_tcg.cu
-  if (Cin % 16 == 0 && Cin >= 16 && osb_tc_general_width(W) && (Cout == 32 || Cout == 64 || Cout == 128))
-    return 16;                                                                                  // conv3d_tcg.cu, column tiles
-  return 0;
+  return stride == 1 ? osb::select_conv3d_tc(Cin, Cout, W, 1, false, false).kc : 0;
 }
 
 int osb_conv3d_tc_supported(int Cin, int Cout, int W, int stride) { return osb_conv3d_tc_kc(Cin, Cout, W, stride) != 0; }
@@ -491,95 +465,53 @@ int osb_ncdhw_to_ndhwc(const float* x, float* y, int B, int C, int D, int H, int
   return osb_ncdhw_to_ndhwc_pad(x, y, B, C, C, D, H, W, stream);
 }
 
-static int conv3d_k3_tc_impl(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
-                             const float* residual, float* y, int B, int Cin, int Cout, int D, int H, int W, int act,
-                             int out_ndhwc, int res_ndhwc, int in_ncdhw, osb_stream_t stream, const float* gate = nullptr,
-                             int ystride = 0) {
+static int conv3d_k3_tc_impl(osb::TcArgs a, int dilation, osb_stream_t stream) {
   using namespace osb;
-  OSB_REQUIRE(x_ndhwc && w_split && y, "conv3d_k3_tc: null pointer");
-  OSB_REQUIRE(B > 0 && D > 0 && H > 0, "conv3d_k3_tc: empty shape");
-  OSB_REQUIRE(osb_conv3d_tc_supported(Cin, Cout, W, 1), "conv3d_k3_tc: unsupported shape Cin=%d Cout=%d W=%d", Cin, Cout, W);
-  OSB_REQUIRE(act >= 0 && act <= 2, "conv3d_k3_tc: unknown activation %d", act);
-  OSB_REQUIRE((reinterpret_cast<uintptr_t>(x_ndhwc) & 15) == 0 && (reinterpret_cast<uintptr_t>(w_split) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(y) & 15) == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0,
-              "conv3d_k3_tc: pointers must be 16-byte aligned");
-  OSB_REQUIRE(!in_ncdhw || osb_conv3d_tc_kc(Cin, Cout, W, 1) == 32, "conv3d_k3_tc: NCDHW input is served by the W = 128 kernel only");
-  OSB_REQUIRE(ystride == 0 || (ystride >= Cout && ystride % 4 == 0 && osb_conv3d_tc_kc(Cin, Cout, W, 1) == 16 && out_ndhwc &&
-                                (!residual || res_ndhwc)),
-              "conv3d_k3_tc: a channel slice (ystride %d) needs channels-last tensors on the 16-channel-chunk kernels", ystride);
-  OSB_REQUIRE(!gate || (osb_conv3d_tc_kc(Cin, Cout, W, 1) == 16 && out_ndhwc && (!residual || res_ndhwc) &&
-                        (reinterpret_cast<uintptr_t>(gate) & 15) == 0),
-              "conv3d_k3_tc: the gate operand needs a channels-last output (and residual) on the 16-channel-chunk kernels");
-  if (osb_conv3d_tc_kc(Cin, Cout, W, 1) == 16)
-    return launch_tcg_dispatch(x_ndhwc, w_split, scale, shift, residual, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc,
-                               (cudaStream_t)stream, gate, ystride);
-  TcParams p{};
-  p.x = x_ndhwc, p.w = w_split, p.scale = scale, p.shift = shift, p.residual = residual, p.y = y;
-  p.B = B, p.D = D, p.H = H, p.Cin = Cin, p.Cout = Cout, p.act = act;
-  p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
-  OSB_REQUIRE(p.overflow, "conv3d_k3_tc: cannot allocate the overflow flag");
-  p.out_ndhwc = out_ndhwc, p.res_ndhwc = res_ndhwc, p.in_ncdhw = in_ncdhw;
-  {
-    static const int bulk = [] { const char* e = getenv("OSB_TC_BULK"); return e ? atoi(e) : 1; }();   // 0: register-staged rows (A/B)
-    p.bulk_rows = (bulk && (in_ncdhw || Cin == TC_KC)) ? 1 : 0;   // channels-last Cin = 64 rows are strided: register path
-  }
-  p.hblocks = (H + TC_TILES - 1) / TC_TILES;
-  const long long items = (long long)B * D * p.hblocks;
-  OSB_REQUIRE(items < (1ll << 31), "conv3d_k3_tc: too many work items");
-  p.items = (int)items;
-  if (Cout <= 16) {                                  // classifier heads (32 -> 1): COUT = 16 instantiation, NCDHW output only
-    OSB_REQUIRE(!out_ndhwc && (!residual || !res_ndhwc), "conv3d_k3_tc: Cout <= 16 writes (and adds) NCDHW tensors only");
-    return launch_tc<16>(p, (cudaStream_t)stream);
-  }
-  return launch_tc<32>(p, (cudaStream_t)stream);
+  const int kc = select_conv3d_tc(a.Cin, a.Cout, a.W, dilation, false, false).kc;
+  OSB_REQUIRE(kc, "conv3d_k3_tc: unsupported shape Cin=%d Cout=%d W=%d dilation=%d", a.Cin, a.Cout, a.W, dilation);
+  OSB_REQUIRE(!a.in_ncdhw || kc == 32, "conv3d_k3_tc: NCDHW input is served by the W = 128 kernel only");
+  OSB_REQUIRE((!a.ystride && !a.gate) || kc == 16, "conv3d_k3_tc: a channel slice or gate needs the 16-channel-chunk kernels");
+  OSB_REQUIRE(a.Cout > 16 || (!a.out_ndhwc && (!a.residual || !a.res_ndhwc)), "conv3d_k3_tc: Cout <= 16 writes (and adds) NCDHW tensors only");
+  const TcLaunch launch = select_conv3d_tc(a.Cin, a.Cout, a.W, dilation, a.gate != nullptr, a.slice()).launch;
+  const int rc = check_tc_args("conv3d_k3_tc", a, launch);
+  return rc != OSB_OK ? rc : launch(a, (cudaStream_t)stream);
 }
 
 int osb_conv3d_k3_tc_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
                          const float* residual, float* y, int B, int Cin, int Cout, int D, int H, int W, int act,
                          int out_ndhwc, int res_ndhwc, osb_stream_t stream) {
-  return conv3d_k3_tc_impl(x_ndhwc, w_split, scale, shift, residual, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc, 0, stream);
+  return conv3d_k3_tc_impl({x_ndhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc, 0, 0,
+                            Cout}, 1, stream);
 }
 
 int osb_conv3d_k3_tc_gate_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
                               const float* residual, const float* gate_nhwc, float* y, int B, int Cin, int Cout, int D, int H, int W,
                               int act, osb_stream_t stream) {
   OSB_REQUIRE(gate_nhwc, "conv3d_k3_tc_gate: null gate");
-  return conv3d_k3_tc_impl(x_ndhwc, w_split, scale, shift, residual, y, B, Cin, Cout, D, H, W, act, 1, 1, 0, stream, gate_nhwc);
+  return conv3d_k3_tc_impl({x_ndhwc, w_split, scale, shift, residual, gate_nhwc, y, B, Cin, Cout, D, H, W, act, 1, 1, 0, 0, Cout}, 1,
+                           stream);
 }
 
 int osb_conv3d_k3_tc_cs_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
                             const float* gate_nhwc, float* y, int B, int Cin, int Cout, int D, int H, int W, int act, int ystride,
                             osb_stream_t stream) {
-  return conv3d_k3_tc_impl(x_ndhwc, w_split, scale, shift, residual, y, B, Cin, Cout, D, H, W, act, 1, 1, 0, stream, gate_nhwc, ystride);
+  return conv3d_k3_tc_impl({x_ndhwc, w_split, scale, shift, residual, gate_nhwc, y, B, Cin, Cout, D, H, W, act, 1, 1, 0, ystride, Cout},
+                           1, stream);
 }
 
 int osb_conv3d_k3_tc_ncdhw_fwd(const float* x_ncdhw, const void* w_split, const float* scale, const float* shift,
                                const float* residual, float* y, int B, int Cin, int Cout, int D, int H, int W, int act,
                                int out_ndhwc, int res_ndhwc, osb_stream_t stream) {
-  return conv3d_k3_tc_impl(x_ncdhw, w_split, scale, shift, residual, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc, 1, stream);
+  return conv3d_k3_tc_impl({x_ncdhw, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc, 1, 0,
+                            Cout}, 1, stream);
 }
 
-int osb_conv2d_tc_kc(int Cin, int Cout, int W, int dilation) {
-  if (dilation == 1) return osb_conv3d_tc_kc(Cin, Cout, W, 1);
-  if (dilation == 2 && W == osb::TC_W && Cout == 128 && Cin % 16 == 0 && Cin >= 16) return 16;
-  return 0;
-}
+int osb_conv2d_tc_kc(int Cin, int Cout, int W, int dilation) { return osb::select_conv3d_tc(Cin, Cout, W, dilation, false, false).kc; }
 
 int osb_conv2d_k3_tc_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
                          float* y, int B, int Cin, int Cout, int H, int W, int dilation, int act, int out_nhwc, int res_nhwc,
                          osb_stream_t stream) {
-  using namespace osb;
-  if (dilation == 1)
-    return osb_conv3d_k3_tc_fwd(x_nhwc, w_split, scale, shift, residual, y, B, Cin, Cout, 1, H, W, act, out_nhwc, res_nhwc, stream);
-  OSB_REQUIRE(x_nhwc && w_split && y, "conv2d_k3_tc: null pointer");
-  OSB_REQUIRE(B > 0 && H > 0, "conv2d_k3_tc: empty shape");
-  OSB_REQUIRE(osb_conv2d_tc_kc(Cin, Cout, W, dilation) != 0, "conv2d_k3_tc: unsupported shape Cin=%d Cout=%d W=%d dilation=%d", Cin, Cout,
-              W, dilation);
-  OSB_REQUIRE(act >= 0 && act <= 2, "conv2d_k3_tc: unknown activation %d", act);
-  OSB_REQUIRE((reinterpret_cast<uintptr_t>(x_nhwc) & 15) == 0 && (reinterpret_cast<uintptr_t>(w_split) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(y) & 15) == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0,
-              "conv2d_k3_tc: pointers must be 16-byte aligned");
-  return launch_tcg_dilated2(x_nhwc, w_split, scale, shift, residual, y, B, Cin, Cout, H, W, act, out_nhwc, res_nhwc,
-                             (cudaStream_t)stream);
+  return conv3d_k3_tc_impl({x_nhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, 1, H, W, act, out_nhwc, res_nhwc, 0, 0,
+                            Cout}, dilation, stream);
 }
 }

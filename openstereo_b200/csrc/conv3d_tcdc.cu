@@ -516,121 +516,72 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
 }
 
 template <int COUT, int KC, int W, int TILES, bool GW = false, int KS = 3>
-static int launch_tcdc(TcdcParams& p, cudaStream_t stream) {
+static int launch_tcdc(const TcArgs& a, cudaStream_t stream) {
   using C = TcdcCfg<COUT, KC, W, TILES, GW, KS>;
-  auto kernel = conv3d_tcdc_kernel<COUT, KC, W, TILES, GW, KS>;
-  static PerDeviceFlag configured;
-  if (!configured.here()) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
-    if (e != cudaSuccess) {
-      set_error("conv3d_tcg: cannot reserve %zu bytes of shared memory: %s", C::SMEM, cudaGetErrorString(e));
-      return OSB_ECUDA;
-    }
-    configured.here() = true;
-  }
-  if (W >= 32 && p.ystride && p.ystride != COUT) {
-    set_error("conv3d_tcdc: channel slices are instantiated for W = 16 only");
-    return OSB_EUNSUPPORTED;
-  }
-  p.hblocks = (p.H + C::HBLK - 1) / C::HBLK;
-  if (p.cout_real <= 0 || p.cout_real > COUT) p.cout_real = COUT;
-  if (GW) p.ctiles = (p.Wr + C::CSTEP - 1) / C::CSTEP;
-  else p.Wr = W, p.ctiles = 1;
-  const long long items = (long long)p.B * (2 * p.D) * p.hblocks * p.ctiles * C::NG;   // both row parities per item
-  OSB_REQUIRE(items < (1ll << 31), "conv3d_tcdc: too many work items");
-  p.items = (int)items;
-  const int sms = sm_count();
-  const int grid = (int)cap_persistent_grid(p.items < sms ? p.items : sms);
+  TcdcParams p{};
+  p.ystride = a.ystride, p.cout_real = a.cout_real;
+  p.hblocks = (a.H + C::HBLK - 1) / C::HBLK;
+  p.Wr = GW ? a.W : W;
+  p.ctiles = GW ? (a.W + C::CSTEP - 1) / C::CSTEP : 1;
   static const std::string variant = tc_variant_name("tcdc<%d,%d,%d,%d,%d,%d>", COUT, KC, W, TILES, (int)GW, KS);
-  set_tc_variant(variant.c_str());
-  kernel<<<grid, C::THREADS, C::SMEM, stream>>>(p);
-  count_launch();
-  cudaError_t le = cudaGetLastError();
-  if (le != cudaSuccess) {
-    cudaFuncAttributes fa{};
-    (void)cudaFuncGetAttributes(&fa, kernel);
-    set_error("conv3d_tcdc_kernel<%d,%d,%d,%d>: launch failed: %s (threads %d, kernel maxThreadsPerBlock %d, regs %d, static smem %zu, "
-              "dynamic smem %zu, max dynamic %d)", COUT, KC, W, TILES, cudaGetErrorString(le), C::THREADS, fa.maxThreadsPerBlock,
-              fa.numRegs, fa.sharedSizeBytes, C::SMEM, fa.maxDynamicSharedSizeBytes);
-    return OSB_ECUDA;
+  return launch_persistent<conv3d_tcdc_kernel<COUT, KC, W, TILES, GW, KS>>(   // both row parities per item
+      a, p, (long long)a.B * (2 * a.D) * p.hblocks * p.ctiles * C::NG, C::SMEM, variant.c_str(), stream);
+}
+
+// The instantiation that serves a transposed conv of kernel size `ks` (INPUT width W), writing a channel slice; null when there is
+// none.
+static TcLaunch select_deconv3d_tc(int ks, int Cin, int Cout, int W, bool slice) {
+  if (Cin % 16 != 0 || Cin < 16) return nullptr;
+  if (ks == 4) {
+    if (W == 16 && Cout == 64) return launch_tcdc<64, 16, 16, 1, false, 4>;   // StereoBase conv3_up: 6c -> 4c = 96 as slices 64 + 32
+    if (W == 16 && Cout == 32) return launch_tcdc<32, 16, 16, 1, false, 4>;
+    if (slice) return nullptr;                                              // channel slices are instantiated for W = 16 only
+    if (W == 32 && Cout == 64) return launch_tcdc<64, 16, 32, 1, false, 4>;
+    if (W == 64 && Cout == 32) return launch_tcdc<32, 16, 64, 1, false, 4>;
+    return nullptr;
   }
-  return OSB_OK;
+  if (ks != 3 || slice) return nullptr;
+  if (W == 32 && Cout == 64) return launch_tcdc<64, 16, 32, 1>;
+  if (W == 64 && Cout == 32) return launch_tcdc<32, 16, 64, 1>;
+  if (!osb_tc_general_width(W)) return nullptr;
+  if (Cout == 64) return launch_tcdc<64, 16, 128, 1, true>;                 // 128-column tiles of the INPUT row
+  if (Cout == 32) return launch_tcdc<32, 16, 128, 1, true>;
+  return nullptr;
+}
+
+static int deconv3d_tc_impl(int ks, TcArgs a, cudaStream_t stream) {
+  OSB_REQUIRE(select_deconv3d_tc(ks, a.Cin, a.Cout, a.W, false), "deconv3d_k%d_tc: unsupported shape Cin=%d Cout=%d W=%d", ks, a.Cin,
+              a.Cout, a.W);
+  const TcLaunch launch = select_deconv3d_tc(ks, a.Cin, a.Cout, a.W, a.slice());
+  const int rc = check_tc_args(ks == 4 ? "deconv3d_k4_tc" : "deconv3d_k3_tc", a, launch);
+  return rc != OSB_OK ? rc : launch(a, stream);
 }
 
 }  // namespace osb
 
 extern "C" {
 
-int osb_deconv3d_tc_supported(int Cin, int Cout, int W) {
-  if (Cin % 16 != 0 || Cin < 16) return 0;
-  if ((W == 32 && Cout == 64) || (W == 64 && Cout == 32)) return 1;                          // whole-row variants
-  return (osb_tc_general_width(W) && (Cout == 32 || Cout == 64)) ? 1 : 0;                   // 128-column tiles of the INPUT row
-}
+int osb_deconv3d_tc_supported(int Cin, int Cout, int W) { return osb::select_deconv3d_tc(3, Cin, Cout, W, false) ? 1 : 0; }
 
-int osb_deconv3d_k4_tc_supported(int Cin, int Cout, int W) {
-  if (Cin % 16 != 0 || Cin < 16) return 0;
-  return ((W == 32 && Cout == 64) || (W == 64 && Cout == 32) || (W == 16 && (Cout == 64 || Cout == 32))) ? 1 : 0;
-}
-
-static int deconv3d_k4_tc_impl(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
-                               const float* residual, float* y, int B, int Cin, int Cout, int cout_real, int D, int H, int W, int act,
-                               int out_ndhwc, int res_ndhwc, int ystride, osb_stream_t stream);
+int osb_deconv3d_k4_tc_supported(int Cin, int Cout, int W) { return osb::select_deconv3d_tc(4, Cin, Cout, W, false) ? 1 : 0; }
 
 int osb_deconv3d_k4_tc_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
                            const float* residual, float* y, int B, int Cin, int Cout, int cout_real, int D, int H, int W, int act,
                            int out_ndhwc, int res_ndhwc, osb_stream_t stream) {
-  return deconv3d_k4_tc_impl(x_ndhwc, w_split, scale, shift, residual, y, B, Cin, Cout, cout_real, D, H, W, act, out_ndhwc, res_ndhwc, 0,
-                             stream);
+  return osb::deconv3d_tc_impl(4, {x_ndhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc,
+                                   0, 0, cout_real}, (cudaStream_t)stream);
 }
 
 int osb_deconv3d_k4_tc_cs_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift, float* y, int B,
                               int Cin, int Cout, int D, int H, int W, int act, int ystride, osb_stream_t stream) {
-  return deconv3d_k4_tc_impl(x_ndhwc, w_split, scale, shift, nullptr, y, B, Cin, Cout, Cout, D, H, W, act, 1, 1, ystride, stream);
-}
-
-static int deconv3d_k4_tc_impl(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
-                               const float* residual, float* y, int B, int Cin, int Cout, int cout_real, int D, int H, int W, int act,
-                               int out_ndhwc, int res_ndhwc, int ystride, osb_stream_t stream) {
-  using namespace osb;
-  OSB_REQUIRE(x_ndhwc && w_split && y, "deconv3d_k4_tc: null pointer");
-  OSB_REQUIRE(ystride == 0 || (ystride >= Cout && ystride % 4 == 0 && out_ndhwc && (!residual || res_ndhwc)),
-              "deconv3d_k4_tc: a channel slice (ystride %d) needs channels-last tensors", ystride);
-  OSB_REQUIRE(B > 0 && D > 0 && H > 0, "deconv3d_k4_tc: empty shape");
-  OSB_REQUIRE(osb_deconv3d_k4_tc_supported(Cin, Cout, W), "deconv3d_k4_tc: unsupported shape Cin=%d Cout=%d W=%d", Cin, Cout, W);
-  OSB_REQUIRE(act >= 0 && act <= 2, "deconv3d_k4_tc: unknown activation %d", act);
-  OSB_REQUIRE(cout_real >= 1 && cout_real <= Cout && (out_ndhwc == 0 || cout_real == Cout) && (!residual || res_ndhwc == 0 || cout_real == Cout),
-              "deconv3d_k4_tc: only NCDHW tensors may hold fewer (%d) channels than the packed %d", cout_real, Cout);
-  TcdcParams p{};
-  p.cout_real = cout_real, p.ystride = ystride;
-  p.x = x_ndhwc, p.w = w_split, p.scale = scale, p.shift = shift, p.residual = residual, p.y = y;
-  p.B = B, p.D = D, p.H = H, p.Cin = Cin, p.act = act, p.out_ndhwc = out_ndhwc, p.res_ndhwc = res_ndhwc;
-  p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
-  OSB_REQUIRE(p.overflow, "tensor-core conv: cannot allocate the overflow flag");
-  cudaStream_t s = (cudaStream_t)stream;
-  if (W == 16 && Cout == 64) return launch_tcdc<64, 16, 16, 1, false, 4>(p, s);   // StereoBase conv3_up: 6c -> 4c = 96 as slices 64 + 32
-  if (W == 16 && Cout == 32) return launch_tcdc<32, 16, 16, 1, false, 4>(p, s);
-  if (W == 32) return launch_tcdc<64, 16, 32, 1, false, 4>(p, s);
-  return launch_tcdc<32, 16, 64, 1, false, 4>(p, s);
+  return osb::deconv3d_tc_impl(4, {x_ndhwc, w_split, scale, shift, nullptr, nullptr, y, B, Cin, Cout, D, H, W, act, 1, 1, 0, ystride,
+                                   Cout}, (cudaStream_t)stream);
 }
 
 int osb_deconv3d_k3_tc_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
                            const float* residual, float* y, int B, int Cin, int Cout, int D, int H, int W, int act,
                            int out_ndhwc, int res_ndhwc, osb_stream_t stream) {
-  using namespace osb;
-  OSB_REQUIRE(x_ndhwc && w_split && y, "deconv3d_k3_tc: null pointer");
-  OSB_REQUIRE(B > 0 && D > 0 && H > 0, "deconv3d_k3_tc: empty shape");
-  OSB_REQUIRE(osb_deconv3d_tc_supported(Cin, Cout, W), "deconv3d_k3_tc: unsupported shape Cin=%d Cout=%d W=%d", Cin, Cout, W);
-  OSB_REQUIRE(act >= 0 && act <= 2, "deconv3d_k3_tc: unknown activation %d", act);
-  TcdcParams p{};
-  p.x = x_ndhwc, p.w = w_split, p.scale = scale, p.shift = shift, p.residual = residual, p.y = y;
-  p.B = B, p.D = D, p.H = H, p.Cin = Cin, p.act = act, p.out_ndhwc = out_ndhwc, p.res_ndhwc = res_ndhwc;
-  p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
-  OSB_REQUIRE(p.overflow, "tensor-core conv: cannot allocate the overflow flag");
-  cudaStream_t s = (cudaStream_t)stream;
-  if (W == 32 && Cout == 64) return launch_tcdc<64, 16, 32, 1>(p, s);
-  if (W == 64 && Cout == 32) return launch_tcdc<32, 16, 64, 1>(p, s);
-  p.Wr = W;
-  if (Cout == 64) return launch_tcdc<64, 16, 128, 1, true>(p, s);
-  return launch_tcdc<32, 16, 128, 1, true>(p, s);
+  return osb::deconv3d_tc_impl(3, {x_ndhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc,
+                                   0, 0, Cout}, (cudaStream_t)stream);
 }
 }

@@ -345,90 +345,50 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
 }
 
 template <int COUT, int KC, int W, int TILES, int DIL = 1, bool GW = false, bool GATE = false>
-static int launch_tcg(TcgParams& p, cudaStream_t stream) {
+static int launch_tcg(const TcArgs& a, cudaStream_t stream) {
   using C = TcgCfg<COUT, KC, W, TILES, DIL, GW>;
-  auto kernel = conv3d_tcg_kernel<COUT, KC, W, TILES, DIL, GW, GATE>;
-  if (!GATE && p.gate) {
-    set_error("conv3d_tcg: no gated instantiation for Cout=%d W=%d", COUT, W);
-    return OSB_EUNSUPPORTED;
-  }
-  if (W >= 32 && p.ystride && p.ystride != COUT) {
-    set_error("conv3d_tcg: channel slices are instantiated for W = 16 only");
-    return OSB_EUNSUPPORTED;
-  }
-  static PerDeviceFlag configured;
-  if (!configured.here()) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
-    if (e != cudaSuccess) {
-      set_error("conv3d_tcg: cannot reserve %zu bytes of shared memory: %s", C::SMEM, cudaGetErrorString(e));
-      return OSB_ECUDA;
-    }
-    configured.here() = true;
-  }
-  p.hblocks = C::hblocks(p.H);
-  if (GW) p.ctiles = (p.Wr + C::CSTEP - 1) / C::CSTEP;
-  else p.Wr = W, p.ctiles = 1;
-  const long long items = (long long)p.B * p.D * p.hblocks * p.ctiles * C::NG;
-  OSB_REQUIRE(items < (1ll << 31), "conv3d_tcg: too many work items");
-  p.items = (int)items;
-  const int sms = sm_count();
-  const int grid = (int)cap_persistent_grid(p.items < sms ? p.items : sms);
+  TcgParams p{};
+  p.gate = a.gate, p.ystride = a.ystride;
+  p.hblocks = C::hblocks(a.H);
+  p.Wr = GW ? a.W : W;
+  p.ctiles = GW ? (a.W + C::CSTEP - 1) / C::CSTEP : 1;
   static const std::string variant = tc_variant_name("tcg<%d,%d,%d,%d,%d,%d,%d>", COUT, KC, W, TILES, DIL, (int)GW, (int)GATE);
-  set_tc_variant(variant.c_str());
-  kernel<<<grid, C::THREADS, C::SMEM, stream>>>(p);
-  count_launch();
-  cudaError_t le = cudaGetLastError();
-  if (le != cudaSuccess) {
-    cudaFuncAttributes fa{};
-    (void)cudaFuncGetAttributes(&fa, kernel);
-    set_error("conv3d_tcg_kernel<%d,%d,%d,%d>: launch failed: %s (threads %d, kernel maxThreadsPerBlock %d, regs %d, static smem %zu, "
-              "dynamic smem %zu, max dynamic %d)", COUT, KC, W, TILES, cudaGetErrorString(le), C::THREADS, fa.maxThreadsPerBlock,
-              fa.numRegs, fa.sharedSizeBytes, C::SMEM, fa.maxDynamicSharedSizeBytes);
-    return OSB_ECUDA;
+  return launch_persistent<conv3d_tcg_kernel<COUT, KC, W, TILES, DIL, GW, GATE>>(
+      a, p, (long long)a.B * a.D * p.hblocks * p.ctiles * C::NG, C::SMEM, variant.c_str(), stream);
+}
+
+TcRoute select_conv3d_tc(int Cin, int Cout, int W, int dilation, bool gate, bool slice) {
+  if (dilation == 1 && W == 128 && Cin % 32 == 0 && Cin >= 32 && !gate && !slice) {   // conv3d_tc.cu
+    if (Cout == 32) return {launch_tc<32>, 32};
+    if (Cout >= 1 && Cout <= 16) return {launch_tc<16>, 32};   // narrow heads: weights zero-padded to 16 rows
   }
-  return OSB_OK;
-}
-
-// dispatcher used by conv3d_tc.cu's C entry point; returns -1 when the shape has no generic instantiation
-int launch_tcg_dispatch(const float* x, const void* w, const float* scale, const float* shift, const float* residual, float* y,
-                        int B, int Cin, int Cout, int D, int H, int W, int act, int out_ndhwc, int res_ndhwc, cudaStream_t stream,
-                        const float* gate, int ystride) {
-  TcgParams p{};
-  p.x = x, p.w = w, p.scale = scale, p.shift = shift, p.residual = residual, p.y = y, p.gate = gate;
-  p.ystride = ystride;
-  p.B = B, p.D = D, p.H = H, p.Cin = Cin, p.act = act, p.out_ndhwc = out_ndhwc, p.res_ndhwc = res_ndhwc;
-  p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
-  if (!p.overflow) return OSB_ECUDA;
-  if (Cin % 16 != 0 || Cin < 16) return -1;
-  if (W == 64 && Cout == 64 && gate) return launch_tcg<64, 16, 64, 1, 1, false, true>(p, stream);   // StereoBase 1/8 level (FeatureAtt gate)
-  if (W == 32 && Cout == 96 && gate) return launch_tcg<96, 16, 32, 1, 1, false, true>(p, stream);   // ... 1/16 level
-  if (W == 64 && Cout == 64) return launch_tcg<64, 16, 64, 1>(p, stream);
-  if (W == 32 && Cout == 64) return launch_tcg<64, 16, 32, 1>(p, stream);
-  if (W == 32 && Cout == 128) return launch_tcg<128, 16, 32, 1>(p, stream);
-  if (W == 32 && Cout == 96) return launch_tcg<96, 16, 32, 1>(p, stream);         // StereoBase 1/16 level (4c = 96)
-  if (W == 16 && Cout == 96) return launch_tcg<96, 16, 16, 1, 1, false, true>(p, stream);   // StereoBase 1/32 level: 6c = 144 -> 160 channels
-  if (W == 16 && Cout == 64) return launch_tcg<64, 16, 16, 1, 1, false, true>(p, stream);   // as two slices (96 + 64), 8 image rows per tile
-  if (W == 128 && Cout == 64) return launch_tcg<64, 16, 128, 1>(p, stream);      // 2D backbone stages as one-plane volumes
-  if (W == 128 && Cout == 128) return launch_tcg<128, 16, 128, 1>(p, stream);
-  // every other width: 128-column tiles with a one-column halo (tc_general_width() is the single source of the W bound)
-  p.Wr = W;
-  if (Cout == 32) return launch_tcg<32, 16, 128, 1, 1, true>(p, stream);
-  if (Cout == 64) return launch_tcg<64, 16, 128, 1, 1, true>(p, stream);
-  if (Cout == 128) return launch_tcg<128, 16, 128, 1, 1, true>(p, stream);
-  return -1;
-}
-
-// dilated (2) one-plane variant for the 2D backbone: same parameters with D == 1
-int launch_tcg_dilated2(const float* x, const void* w, const float* scale, const float* shift, const float* residual, float* y,
-                        int B, int Cin, int Cout, int H, int W, int act, int out_ndhwc, int res_ndhwc, cudaStream_t stream) {
-  TcgParams p{};
-  p.x = x, p.w = w, p.scale = scale, p.shift = shift, p.residual = residual, p.y = y;
-  p.B = B, p.D = 1, p.H = H, p.Cin = Cin, p.act = act, p.out_ndhwc = out_ndhwc, p.res_ndhwc = res_ndhwc;
-  p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
-  if (!p.overflow) return OSB_ECUDA;
-  if (Cin % 16 != 0 || Cin < 16) return -1;
-  if (W == 128 && Cout == 128) return launch_tcg<128, 16, 128, 1, 2>(p, stream);
-  return -1;
+  if (Cin % 16 != 0 || Cin < 16) return {};
+  if (dilation == 2)                                            // 2D backbone stages as one-plane volumes
+    return (W == 128 && Cout == 128 && !gate && !slice) ? TcRoute{launch_tcg<128, 16, 128, 1, 2>, 16} : TcRoute{};
+  if (dilation != 1) return {};
+  if (W == 16) {                      // StereoBase 1/32 level: 6c = 144 -> 160 channels as two slices (96 + 64), 8 image rows per tile
+    if (Cout == 96) return {launch_tcg<96, 16, 16, 1, 1, false, true>, 16};
+    if (Cout == 64) return {launch_tcg<64, 16, 16, 1, 1, false, true>, 16};
+    return {};
+  }
+  if (slice) return {};                                         // channel slices are instantiated for W = 16 only
+  if (gate) {
+    if (W == 64 && Cout == 64) return {launch_tcg<64, 16, 64, 1, 1, false, true>, 16};   // StereoBase 1/8 level (FeatureAtt gate)
+    if (W == 32 && Cout == 96) return {launch_tcg<96, 16, 32, 1, 1, false, true>, 16};   // ... 1/16 level
+    return {};
+  }
+  if (W == 64 && Cout == 64) return {launch_tcg<64, 16, 64, 1>, 16};
+  if (W == 32 && Cout == 64) return {launch_tcg<64, 16, 32, 1>, 16};
+  if (W == 32 && Cout == 128) return {launch_tcg<128, 16, 32, 1>, 16};
+  if (W == 32 && Cout == 96) return {launch_tcg<96, 16, 32, 1>, 16};         // StereoBase 1/16 level (4c = 96)
+  if (W == 128 && Cout == 64) return {launch_tcg<64, 16, 128, 1>, 16};       // 2D backbone stages as one-plane volumes
+  if (W == 128 && Cout == 128) return {launch_tcg<128, 16, 128, 1>, 16};
+  if (!osb_tc_general_width(W)) return {};
+  // every other width: 128-column tiles with a one-column halo
+  if (Cout == 32) return {launch_tcg<32, 16, 128, 1, 1, true>, 16};
+  if (Cout == 64) return {launch_tcg<64, 16, 128, 1, 1, true>, 16};
+  if (Cout == 128) return {launch_tcg<128, 16, 128, 1, 1, true>, 16};
+  return {};
 }
 
 }  // namespace osb

@@ -403,44 +403,41 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
 }
 
 template <int COUT, int KC, int W, int TILES, bool GW = false>
-static int launch_tcs2(Tcs2Params& p, cudaStream_t stream) {
+static int launch_tcs2(const TcArgs& a, cudaStream_t stream) {
   using C = Tcs2Cfg<COUT, KC, W, TILES, GW>;
-  auto kernel = conv3d_tcs2_kernel<COUT, KC, W, TILES, GW>;
-  static PerDeviceFlag configured;
-  if (!configured.here()) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
-    if (e != cudaSuccess) {
-      set_error("conv3d_tcg: cannot reserve %zu bytes of shared memory: %s", C::SMEM, cudaGetErrorString(e));
-      return OSB_ECUDA;
-    }
-    configured.here() = true;
-  }
-  if (W >= 32 && p.ystride && p.ystride != COUT) {
-    set_error("conv3d_tcs2: channel slices are instantiated for W = 16 only");
-    return OSB_EUNSUPPORTED;
-  }
-  p.hblocks = (p.H / 2 + C::HBLK - 1) / C::HBLK;
-  if (GW) p.ctiles = (p.Wr + C::CSTEP - 1) / C::CSTEP;
-  else p.Wr = W, p.ctiles = 1;
-  const long long items = (long long)p.B * (p.D / 2) * p.hblocks * p.ctiles * C::NP;   // two channel groups per item
-  OSB_REQUIRE(items < (1ll << 31), "conv3d_tcs2: too many work items");
-  p.items = (int)items;
-  const int sms = sm_count();
-  const int grid = (int)cap_persistent_grid(p.items < sms ? p.items : sms);
+  Tcs2Params p{};
+  p.ystride = a.ystride;
+  p.hblocks = (a.H / 2 + C::HBLK - 1) / C::HBLK;
+  p.Wr = GW ? a.W / 2 : W;
+  p.ctiles = GW ? (p.Wr + C::CSTEP - 1) / C::CSTEP : 1;
   static const std::string variant = tc_variant_name("tcs2<%d,%d,%d,%d,%d>", COUT, KC, W, TILES, (int)GW);
-  set_tc_variant(variant.c_str());
-  kernel<<<grid, C::THREADS, C::SMEM, stream>>>(p);
-  count_launch();
-  cudaError_t le = cudaGetLastError();
-  if (le != cudaSuccess) {
-    cudaFuncAttributes fa{};
-    (void)cudaFuncGetAttributes(&fa, kernel);
-    set_error("conv3d_tcs2_kernel<%d,%d,%d,%d>: launch failed: %s (threads %d, kernel maxThreadsPerBlock %d, regs %d, static smem %zu, "
-              "dynamic smem %zu, max dynamic %d)", COUT, KC, W, TILES, cudaGetErrorString(le), C::THREADS, fa.maxThreadsPerBlock,
-              fa.numRegs, fa.sharedSizeBytes, C::SMEM, fa.maxDynamicSharedSizeBytes);
-    return OSB_ECUDA;
-  }
-  return OSB_OK;
+  return launch_persistent<conv3d_tcs2_kernel<COUT, KC, W, TILES, GW>>(   // two channel groups per item
+      a, p, (long long)a.B * (a.D / 2) * p.hblocks * p.ctiles * C::NP, C::SMEM, variant.c_str(), stream);
+}
+
+// The instantiation that serves a stride-2 shape (INPUT extents; template W = output width), writing a channel slice; null when
+// there is none.
+static TcLaunch select_conv3d_s2_tc(int Cin, int Cout, int D, int H, int W, bool slice) {
+  if (Cin % 16 != 0 || Cin < 16 || D % 2 || H % 2 || W % 2) return nullptr;
+  if (W == 32 && Cout == 96) return launch_tcs2<96, 16, 16, 1>;       // StereoBase conv3[0]: 4c -> 6c as two channel slices
+  if (W == 32 && Cout == 64) return launch_tcs2<64, 16, 16, 1>;
+  if (slice) return nullptr;                                           // channel slices are instantiated for W = 16 only
+  if (W == 128 && Cout == 64) return launch_tcs2<64, 16, 64, 1>;
+  if (W == 64 && Cout == 64) return launch_tcs2<64, 16, 32, 1>;
+  if (W == 64 && Cout == 128) return launch_tcs2<128, 16, 32, 1>;
+  if (W == 64 && Cout == 96) return launch_tcs2<96, 16, 32, 1>;       // StereoBase conv2[0]: 2c -> 4c = 96
+  if (!osb_tc_general_width(W / 2)) return nullptr;
+  if (Cout == 64) return launch_tcs2<64, 16, 128, 1, true>;           // 128-column tiles of the OUTPUT row
+  if (Cout == 128) return launch_tcs2<128, 16, 128, 1, true>;
+  return nullptr;
+}
+
+static int conv3d_k3_s2_tc_impl(TcArgs a, cudaStream_t stream) {
+  OSB_REQUIRE(select_conv3d_s2_tc(a.Cin, a.Cout, a.D, a.H, a.W, false), "conv3d_k3_s2_tc: unsupported shape Cin=%d Cout=%d D=%d H=%d W=%d",
+              a.Cin, a.Cout, a.D, a.H, a.W);
+  const TcLaunch launch = select_conv3d_s2_tc(a.Cin, a.Cout, a.D, a.H, a.W, a.slice());
+  const int rc = check_tc_args("conv3d_k3_s2_tc", a, launch);
+  return rc != OSB_OK ? rc : launch(a, stream);
 }
 
 }  // namespace osb
@@ -448,49 +445,19 @@ static int launch_tcs2(Tcs2Params& p, cudaStream_t stream) {
 extern "C" {
 
 int osb_conv3d_s2_tc_supported(int Cin, int Cout, int D, int H, int W) {
-  if (Cin % 16 != 0 || Cin < 16 || D % 2 || H % 2 || W % 2) return 0;
-  if ((W == 128 && Cout == 64) || (W == 64 && (Cout == 64 || Cout == 96 || Cout == 128)) || (W == 32 && (Cout == 64 || Cout == 96)))
-    return 1;                                                                               // whole-row variants
-  return (osb_tc_general_width(W / 2) && (Cout == 64 || Cout == 128)) ? 1 : 0;              // 128-column tiles of the OUTPUT row
-}
-
-static int conv3d_k3_s2_tc_impl(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
-                                const float* residual, float* y, int B, int Cin, int Cout, int D, int H, int W, int act,
-                                int out_ndhwc, int res_ndhwc, int ystride, osb_stream_t stream) {
-  using namespace osb;
-  OSB_REQUIRE(ystride == 0 || (ystride >= Cout && ystride % 4 == 0 && out_ndhwc && (!residual || res_ndhwc)),
-              "conv3d_k3_s2_tc: a channel slice (ystride %d) needs channels-last tensors", ystride);
-  OSB_REQUIRE(x_ndhwc && w_split && y, "conv3d_k3_s2_tc: null pointer");
-  OSB_REQUIRE(B > 0 && D > 0 && H > 0, "conv3d_k3_s2_tc: empty shape");
-  OSB_REQUIRE(osb_conv3d_s2_tc_supported(Cin, Cout, D, H, W), "conv3d_k3_s2_tc: unsupported shape Cin=%d Cout=%d D=%d H=%d W=%d", Cin,
-              Cout, D, H, W);
-  OSB_REQUIRE(act >= 0 && act <= 2, "conv3d_k3_s2_tc: unknown activation %d", act);
-  Tcs2Params p{};
-  p.x = x_ndhwc, p.w = w_split, p.scale = scale, p.shift = shift, p.residual = residual, p.y = y;
-  p.B = B, p.D = D, p.H = H, p.Cin = Cin, p.act = act, p.out_ndhwc = out_ndhwc, p.res_ndhwc = res_ndhwc;
-  p.kappa = rz_kappa(), p.overflow = tc_overflow_flag();
-  p.ystride = ystride;
-  OSB_REQUIRE(p.overflow, "tensor-core conv: cannot allocate the overflow flag");
-  cudaStream_t s = (cudaStream_t)stream;
-  if (W == 32 && Cout == 96) return launch_tcs2<96, 16, 16, 1>(p, s);           // StereoBase conv3[0]: 4c -> 6c as two channel slices
-  if (W == 32 && Cout == 64) return launch_tcs2<64, 16, 16, 1>(p, s);
-  if (W == 128 && Cout == 64) return launch_tcs2<64, 16, 64, 1>(p, s);
-  if (W == 64 && Cout == 64) return launch_tcs2<64, 16, 32, 1>(p, s);
-  if (W == 64 && Cout == 128) return launch_tcs2<128, 16, 32, 1>(p, s);
-  if (W == 64 && Cout == 96) return launch_tcs2<96, 16, 32, 1>(p, s);           // StereoBase conv2[0]: 2c -> 4c = 96
-  p.Wr = W / 2;
-  if (Cout == 64) return launch_tcs2<64, 16, 128, 1, true>(p, s);
-  return launch_tcs2<128, 16, 128, 1, true>(p, s);
+  return osb::select_conv3d_s2_tc(Cin, Cout, D, H, W, false) ? 1 : 0;
 }
 
 int osb_conv3d_k3_s2_tc_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,
                             const float* residual, float* y, int B, int Cin, int Cout, int D, int H, int W, int act,
                             int out_ndhwc, int res_ndhwc, osb_stream_t stream) {
-  return conv3d_k3_s2_tc_impl(x_ndhwc, w_split, scale, shift, residual, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc, 0, stream);
+  return osb::conv3d_k3_s2_tc_impl({x_ndhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc,
+                                    0, 0, Cout}, (cudaStream_t)stream);
 }
 
 int osb_conv3d_k3_s2_tc_cs_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift, float* y, int B,
                                int Cin, int Cout, int D, int H, int W, int act, int ystride, osb_stream_t stream) {
-  return conv3d_k3_s2_tc_impl(x_ndhwc, w_split, scale, shift, nullptr, y, B, Cin, Cout, D, H, W, act, 1, 1, ystride, stream);
+  return osb::conv3d_k3_s2_tc_impl({x_ndhwc, w_split, scale, shift, nullptr, nullptr, y, B, Cin, Cout, D, H, W, act, 1, 1, 0, ystride,
+                                    Cout}, (cudaStream_t)stream);
 }
 }

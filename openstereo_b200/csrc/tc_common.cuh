@@ -537,4 +537,98 @@ __device__ __forceinline__ void store_ndhwc_chunk32(float* tbuf, int lane, const
     if ((vmask >> (4 * j + sub)) & 1u) *reinterpret_cast<float4*>(y0 + (size_t)(4 * j + sub) * vstride + c4) = o[j];
 }
 
+// ------------------------------------------------------------------------------------------------ host: check and launch
+// Arguments of a tensor-core conv entry point (include/openstereo_b200.h).  Extents are those of the INPUT.
+struct TcArgs {
+  const float* x;
+  const void* w;
+  const float* scale;
+  const float* shift;
+  const float* residual;
+  const float* gate;       // stride 1: FeatureAtt gate (B, H, W, Cout) channels-last, or null
+  float* y;
+  int B, Cin, Cout, D, H, W;
+  int act, out_ndhwc, res_ndhwc;
+  int in_ncdhw;            // stride 1: the input is (B, Cin, D, H, W)
+  int ystride;             // channels per voxel of the channels-last y / residual / gate (0 = Cout)
+  int cout_real;           // channels an NCDHW output / residual holds (< Cout: a zero-padded channel plan)
+  float kappa;             // set by check_tc_args
+  unsigned int* overflow;  // set by check_tc_args
+  bool slice() const { return ystride != 0 && ystride != Cout; }
+};
+// Launcher of one instantiation: the result of a family's selector (null: no instantiation serves the arguments).
+using TcLaunch = int (*)(const TcArgs&, cudaStream_t);
+
+// The checks every tensor-core entry point runs after its family's shape rules and before any CUDA call: pointers (the kernels'
+// loaders and stores use 128-bit accesses and bulk copies), extents, activation, the layouts a channel slice, a gate or a
+// zero-padded channel plan need (OSB_EINVAL); a selector result for the requested gate / channel slice (OSB_EUNSUPPORTED); then
+// the overflow flag of the current device (OSB_ECUDA).
+inline int check_tc_args(const char* what, TcArgs& a, TcLaunch launch) {
+  auto aligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  OSB_REQUIRE(a.x && a.w && a.y, "%s: null pointer", what);
+  OSB_REQUIRE(a.B > 0 && a.D > 0 && a.H > 0, "%s: empty shape", what);
+  OSB_REQUIRE(a.act >= 0 && a.act <= 2, "%s: unknown activation %d", what, a.act);
+  OSB_REQUIRE(aligned(a.x) && aligned(a.w) && aligned(a.y) && aligned(a.residual) && aligned(a.gate),
+              "%s: pointers must be 16-byte aligned", what);
+  const bool channels_last = a.out_ndhwc && (!a.residual || a.res_ndhwc);
+  OSB_REQUIRE(a.ystride == 0 || (a.ystride >= a.Cout && a.ystride % 4 == 0 && channels_last),
+              "%s: a channel slice (ystride %d) needs channels-last tensors", what, a.ystride);
+  OSB_REQUIRE(!a.gate || channels_last, "%s: the gate operand needs a channels-last output (and residual)", what);
+  OSB_REQUIRE(a.cout_real == a.Cout || (a.cout_real >= 1 && a.cout_real < a.Cout && !a.out_ndhwc && (!a.residual || !a.res_ndhwc)),
+              "%s: only NCDHW tensors may hold fewer (%d) channels than the packed %d", what, a.cout_real, a.Cout);
+  if (!launch) {
+    set_error("%s: no instantiation serves Cout=%d W=%d with gate=%d ystride=%d", what, a.Cout, a.W, a.gate != nullptr, a.ystride);
+    return OSB_EUNSUPPORTED;
+  }
+  a.kappa = rz_kappa();
+  a.overflow = tc_overflow_flag();
+  return a.overflow ? OSB_OK : OSB_ECUDA;   // tc_overflow_flag has set the message
+}
+
+// Launch of a persistent tensor-core kernel over `items` work items (CTAs walk it = blockIdx.x, + gridDim.x, ...): one CTA per SM
+// at most (its shared memory is taken), the grid capped by osb_set_persistent_grid_cap.  Fills the fields every Params struct has
+// from `a`; the family launcher has set the rest.  `variant` is what osb_tc_last_variant reports.  A template on the kernel, so
+// that every instantiation has its own per-device "shared memory configured" flag.
+template <auto KERNEL, class P>
+int launch_persistent(const TcArgs& a, P p, long long items, size_t smem, const char* variant, cudaStream_t stream) {
+  OSB_REQUIRE(items < (1ll << 31), "%s: too many work items", variant);
+  static PerDeviceFlag configured;
+  if (!configured.here()) {
+    const cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) {
+      set_error("%s: cannot reserve %zu bytes of shared memory: %s", variant, smem, cudaGetErrorString(e));
+      return OSB_ECUDA;
+    }
+    configured.here() = true;
+  }
+  p.x = a.x, p.w = a.w, p.scale = a.scale, p.shift = a.shift, p.residual = a.residual, p.y = a.y;
+  p.B = a.B, p.D = a.D, p.H = a.H, p.Cin = a.Cin, p.act = a.act, p.out_ndhwc = a.out_ndhwc, p.res_ndhwc = a.res_ndhwc;
+  p.kappa = a.kappa, p.overflow = a.overflow;
+  p.items = (int)items;
+  const int sms = sm_count();
+  set_tc_variant(variant);
+  KERNEL<<<(int)cap_persistent_grid(p.items < sms ? p.items : sms), TC_WG_THREADS, smem, stream>>>(p);
+  count_launch();
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    cudaFuncAttributes fa{};
+    (void)cudaFuncGetAttributes(&fa, KERNEL);
+    set_error("%s: launch failed: %s (threads %d, kernel maxThreadsPerBlock %d, regs %d, static smem %zu, dynamic smem %zu, "
+              "max dynamic %d)", variant, cudaGetErrorString(e), TC_WG_THREADS, fa.maxThreadsPerBlock, fa.numRegs,
+              fa.sharedSizeBytes, smem, fa.maxDynamicSharedSizeBytes);
+    return OSB_ECUDA;
+  }
+  return OSB_OK;
+}
+
+// The stride-1 family's selector (conv3d_tcg.cu): the instantiation of conv3d_tc.cu or conv3d_tcg.cu that serves Conv3d k3 s1 p1
+// (dilation 2: the one-plane 2D conv), with a gate / writing a channel slice, and its K chunk; {nullptr, 0} when there is none.
+struct TcRoute {
+  TcLaunch launch;
+  int kc;
+};
+TcRoute select_conv3d_tc(int Cin, int Cout, int W, int dilation, bool gate, bool slice);
+template <int COUT>
+int launch_tc(const TcArgs& a, cudaStream_t stream);   // conv3d_tc.cu
+
 }  // namespace osb

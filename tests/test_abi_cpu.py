@@ -88,6 +88,33 @@ def test_ops_refuse_cpu_tensors(native):
         ops.cat_fms(x, x, max_disp=4, start_disp=-1)
 
 
+_A = 0x10000                                     # a 16-byte aligned address; no call below gets past the argument check
+TC_FWD_CALLS = {                                  # every tensor-core entry point on a shape it serves, x misaligned by 4 bytes
+    "conv3d": ("osb_conv3d_k3_tc_fwd", lambda x: (x, _A, _A, None, None, _A, 1, 32, 32, 2, 4, 128, 0, 1, 1, None)),
+    "conv3d-kc16": ("osb_conv3d_k3_tc_fwd", lambda x: (x, _A, _A, None, None, _A, 1, 32, 64, 2, 4, 64, 0, 1, 1, None)),
+    "conv3d-gate": ("osb_conv3d_k3_tc_gate_fwd", lambda x: (x, _A, _A, None, None, _A, _A, 1, 32, 64, 2, 4, 64, 0, None)),
+    "conv3d-slice": ("osb_conv3d_k3_tc_cs_fwd", lambda x: (x, _A, _A, None, None, None, _A, 1, 32, 96, 2, 4, 16, 0, 160, None)),
+    "conv3d-ncdhw": ("osb_conv3d_k3_tc_ncdhw_fwd", lambda x: (x, _A, _A, None, None, _A, 1, 32, 32, 2, 4, 128, 0, 1, 1, None)),
+    "conv2d": ("osb_conv2d_k3_tc_fwd", lambda x: (x, _A, _A, None, None, _A, 1, 32, 64, 4, 128, 1, 0, 1, 1, None)),
+    "conv2d-dil2": ("osb_conv2d_k3_tc_fwd", lambda x: (x, _A, _A, None, None, _A, 1, 32, 128, 4, 128, 2, 0, 1, 1, None)),
+    "conv3d-s2": ("osb_conv3d_k3_s2_tc_fwd", lambda x: (x, _A, _A, None, None, _A, 1, 32, 64, 2, 4, 128, 0, 1, 1, None)),
+    "conv3d-s2-slice": ("osb_conv3d_k3_s2_tc_cs_fwd", lambda x: (x, _A, _A, None, _A, 1, 32, 96, 2, 4, 32, 0, 160, None)),
+    "deconv3d-k3": ("osb_deconv3d_k3_tc_fwd", lambda x: (x, _A, _A, None, None, _A, 1, 64, 32, 2, 4, 64, 0, 1, 1, None)),
+    "deconv3d-k4": ("osb_deconv3d_k4_tc_fwd", lambda x: (x, _A, _A, None, None, _A, 1, 64, 32, 32, 2, 4, 64, 0, 1, 1, None)),
+    "deconv3d-k4-slice": ("osb_deconv3d_k4_tc_cs_fwd", lambda x: (x, _A, _A, None, _A, 1, 32, 64, 2, 4, 16, 0, 96, None)),
+}
+
+
+@pytest.mark.skipif(torch.cuda.is_available(), reason="a missing check would launch a kernel on a fake address")
+@pytest.mark.parametrize("case", sorted(TC_FWD_CALLS))
+def test_tc_entry_points_refuse_misaligned_pointers(native, case):
+    """The tensor-core kernels load and store 16 bytes at a time and bulk-copy rows: every entry point refuses a misaligned operand
+    as an argument error, before any CUDA call."""
+    name, args = TC_FWD_CALLS[case]
+    with pytest.raises(ValueError, match="16-byte aligned"):
+        native.call(name, *args(_A + 4))
+
+
 def test_product_does_not_import_oracle():
     pkg = os.path.join(ROOT, "openstereo_b200")
     for dirpath, _, files in os.walk(pkg):

@@ -189,8 +189,8 @@ def test_stereobase_tc_route_gating_without_gpu():
 
 
 def _launcher_variants():
-    """Every launch_tc / launch_tcg / launch_tcs2 / launch_tcdc template list the dispatchers in csrc/ instantiate, with the
-    launcher's default template arguments filled in, in the spelling of osb_tc_last_variant() ("tcg<64,16,64,1,1,0,1>")."""
+    """Every launch_tc / launch_tcg / launch_tcs2 / launch_tcdc template list the selectors in csrc/ name, with the launcher's
+    default template arguments filled in, in the spelling of osb_tc_last_variant() ("tcg<64,16,64,1,1,0,1>")."""
     import glob
     import os
     import re
@@ -198,11 +198,11 @@ def _launcher_variants():
     src = "".join(open(p).read() for p in sorted(glob.glob(os.path.join(root, "openstereo_b200", "csrc", "*.cu"))))
     lit = {"true": "1", "false": "0"}
     defaults = {}
-    for params, name in re.findall(r"template\s*<([^<>]*)>\s*static int (launch_tc\w*)\s*\(", src):
+    for params, name in re.findall(r"template\s*<([^<>]*)>\s*(?:static\s+)?int\s+(launch_tc\w*)\s*\(", src):
         defaults[name] = [p.split("=")[1].strip() if "=" in p else None for p in params.split(",")]
     assert set(defaults) == {"launch_tc", "launch_tcg", "launch_tcs2", "launch_tcdc"}, sorted(defaults)
     found = set()
-    for name, args in re.findall(r"\b(launch_tc\w*)<([^<>]*)>\s*\(", src):
+    for name, args in re.findall(r"\b(launch_tc\w*)<([^<>]*)>", src):
         vals = [a.strip() for a in args.split(",")]
         vals += defaults[name][len(vals):]
         assert None not in vals, (name, args)
@@ -210,7 +210,7 @@ def _launcher_variants():
     return found
 
 
-def test_tc_contract_registry_is_complete():
+def test_tc_contract_registry_matches_selectors():
     """A tensor-core instantiation cannot land without a row in the contract registry of tests/test_tc_contract_gpu.py (routing,
     grid-cap, per-channel accuracy, store-bounds, range-guard and kappa . n checks), and no row may name one that is gone."""
     from test_tc_contract_gpu import REGISTRY

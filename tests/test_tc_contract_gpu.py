@@ -1,8 +1,8 @@
 """GPU: contract of every tensor-core convolution instantiation (csrc/conv3d_tc.cu, conv3d_tcg.cu, conv3d_tcs2.cu, conv3d_tcdc.cu).
 
-REGISTRY has one row per dispatcher branch (tests/test_host_logic_cpu.py checks that every launch_tc*<...> template list in csrc/
+REGISTRY has one row per selector branch (tests/test_host_logic_cpu.py checks that every launch_tc*<...> template list in csrc/
 has a row).  Each row names the C entry point, the channels, a small input shape with a partial row block (general-width rows: a
-last column tile holding a single valid column) and the instantiation the dispatcher must pick.  For every row:
+last column tile holding a single valid column) and the instantiation the selector must pick.  For every row:
   routing      osb_tc_last_variant() names the row's instantiation;
   item loop    the persistent CTAs walk their work items with state carried from item to item (ring and weight-buffer mbarrier
                phases, the seam-exchange double buffer): outputs at grid caps 1 and 7, without a cap and again without a cap are
