@@ -60,7 +60,8 @@ const unsigned int* osb_tc_overflow_flag(void);
  * ignored.  The default 1.57e-8 is calibrated on the H100 (DESIGN.md section 2.1: it removes 87-100 % of the layer-level bias
  * against fp64).  The setter exists for calibration and tests (tools/parity_bisect.py, tests/test_tc_contract_gpu.py). */
 float osb_set_rz_kappa(float kappa);
-/* Test hooks of the persistent kernels (the tensor-core convolutions and the volume constructors), process-wide.
+/* Test hooks of the persistent kernels (the tensor-core convolutions, the volume constructors and the grid-stride channels-last
+ * 1x1 convolutions osb_conv1x1_ndhwc_fwd / osb_conv1x1_ndhwc_cat_fwd), process-wide.
  * osb_set_persistent_grid_cap clamps their grid to `cap` CTAs (0 = no cap, the default: one CTA per resident slot) and returns the
  * previous cap.  Every CTA walks the work items it = blockIdx.x, blockIdx.x + gridDim.x, ..., so cap = 1 makes one CTA compute every
  * item in order; an item's result does not depend on the CTA that computes it, so outputs are bit-identical for any cap.

@@ -761,7 +761,7 @@ static int launch_conv1x1_cat(const float* x0, const float* x1, int C0, const fl
   }
   const long long tiles = (voxels + 127) / 128;
   const int per_sm = smem <= 113 * 1024 ? 2 : 1;
-  const unsigned blocks = (unsigned)std::min<long long>(tiles, (long long)sm_count() * per_sm);
+  const unsigned blocks = (unsigned)cap_persistent_grid(std::min<long long>(tiles, (long long)sm_count() * per_sm));
   kernel<<<blocks, 128, smem, s>>>(x0, x1, C0, w, scale, shift, y, (size_t)voxels, act);
   count_launch();
   return check_launch("conv1x1_ndhwc_cat_kernel");
@@ -858,7 +858,7 @@ int osb_conv1x1_ndhwc_fwd(const float* x, const float* w_packed, const float* sc
   OSB_REQUIRE(act >= 0 && act <= 2, "conv1x1_ndhwc: unknown activation %d", act);
   OSB_REQUIRE(aligned16(x) && aligned16(y), "conv1x1_ndhwc: pointers must be 16-byte aligned");
   const long long groups = (voxels + 31) / 32;
-  const unsigned blocks = (unsigned)std::min<long long>((groups + 1) / 2, (long long)osb::sm_count() * 16);   // 2 warps per CTA, grid-stride over 32-voxel groups
+  const unsigned blocks = (unsigned)cap_persistent_grid(std::min<long long>((groups + 1) / 2, (long long)osb::sm_count() * 16));   // 2 warps per CTA, grid-stride over 32-voxel groups
   cudaStream_t s = (cudaStream_t)stream;
   if (Cin == 32 && Cout == 32) conv1x1_ndhwc_32_kernel<<<blocks, 64, 0, s>>>(x, w_packed, scale, shift, y, (size_t)voxels, act);
   else if (Cin == 64 && Cout == 64) conv1x1_ndhwc_kernel<64, 64><<<blocks, 64, 0, s>>>(x, w_packed, scale, shift, y, (size_t)voxels, act);

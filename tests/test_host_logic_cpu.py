@@ -218,3 +218,45 @@ def test_tc_contract_registry_matches_selectors():
     rows = {r.variant for r in REGISTRY}
     assert not found - rows, "instantiations without a contract row: %s" % sorted(found - rows)
     assert not rows - found, "contract rows naming no instantiation: %s" % sorted(rows - found)
+
+
+# flavours.cu kernels that are not convolutions: volume / regression gathers and reductions with their own oracle tests
+_NOT_CONVOLUTIONS = {"group_l2_normalize_kernel", "sub_volume_kernel", "regression_values_kernel"}
+# the local `auto kernel = ...<template parameters>` of each templated launcher, covered by the launcher's template lists
+_TEMPLATED_LAUNCHERS = {"conv3d_k3_kernel": "launch_conv_k3", "deconv3d_kernel": "launch_deconv",
+                        "conv1x1_ndhwc_cat_kernel": "launch_conv1x1_cat", "mbv2_block3d_kernel": "launch_mbv2"}
+
+
+def _cuda_core_variants():
+    """Every launch_conv_k3 / launch_deconv / launch_conv1x1_cat / launch_mbv2 template list and every kernel launched directly
+    with <<< in the CUDA-core convolution sources, in the registry spelling ("launch_deconv<3,8>", "conv1x1_ndhwc_kernel<64,64>")."""
+    import os
+    import re
+    csrc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "openstereo_b200", "csrc")
+    found = set()
+    for name in ("conv3d.cu", "lightstereo.cu", "msnet.cu", "flavours.cu"):
+        src = open(os.path.join(csrc, name)).read()
+        for launcher, args in re.findall(r"\b(launch_conv_k3|launch_deconv|launch_conv1x1_cat|launch_mbv2)\s*<([^<>]*)>", src):
+            found.add("%s<%s>" % (launcher, args.replace(" ", "")))
+        for m in re.finditer(r"\b(\w+)\s*(<[^<>]*>)?\s*<<<", src):
+            kernel, args = m.group(1), (m.group(2) or "").replace(" ", "")
+            if kernel == "kernel":                               # auto kernel = name<args>; ... kernel<<<...>>>
+                kernel, args = re.findall(r"auto\s+kernel\s*=\s*(\w+)\s*(<[^<>]*>)?\s*;", src[:m.start()])[-1]
+                args = args.replace(" ", "")
+                if not re.fullmatch(r"(<\d+(,\d+)*>)?", args):
+                    assert kernel in _TEMPLATED_LAUNCHERS, "%s: %s%s launched from an unknown templated launcher" % (name, kernel, args)
+                    continue
+            if kernel not in _NOT_CONVOLUTIONS:
+                found.add(kernel + args)
+    return found
+
+
+def test_cuda_core_contract_registry_matches_sources():
+    """A CUDA-core convolution instantiation or launch path cannot land without a row in the contract registry of
+    tests/test_cuda_core_contract_gpu.py (routing, per-channel accuracy, both store paths, store bounds, determinism, grid caps),
+    and no row may name one that is gone."""
+    from test_cuda_core_contract_gpu import REGISTRY
+    found = _cuda_core_variants()
+    rows = {r.variant for r in REGISTRY}
+    assert not found - rows, "instantiations without a contract row: %s" % sorted(found - rows)
+    assert not rows - found, "contract rows naming no instantiation: %s" % sorted(rows - found)
