@@ -69,6 +69,11 @@ float osb_set_rz_kappa(float kappa);
  * "tcg<64,16,64,1,1,0,1>" (COUT, KC, W, TILES, DIL, GW, GATE), "tc<32>", "tcs2<...>", "tcdc<...>"; "" before the first launch. */
 int osb_set_persistent_grid_cap(int cap);
 const char* osb_tc_last_variant(void);
+/* The cost-volume kernel this thread launched last, as "volume<VEC,K4,STAGE>": VEC = 1 for 16-byte loads and stores of the left
+ * features and the output (W % 4 == 0, ref and out 16-byte aligned), K4 = 1 when the channels per group are a multiple of 4
+ * (or the volume is concatenation only), STAGE = tma when the right features are staged by TMA tile loads (W % 4 == 0, tgt
+ * 16-byte aligned), ldg when by plain loads; "" before the first launch. */
+const char* osb_volume_last_variant(void);
 
 /* ---------------------------------------------------------------- cost-volume constructors --- */
 

@@ -95,6 +95,8 @@ def _load():
     lib.osb_set_persistent_grid_cap.restype = ctypes.c_int
     lib.osb_tc_last_variant.argtypes = []
     lib.osb_tc_last_variant.restype = ctypes.c_char_p
+    lib.osb_volume_last_variant.argtypes = []
+    lib.osb_volume_last_variant.restype = ctypes.c_char_p
     for name, argtypes in SIGNATURES.items():
         try:
             fn = getattr(lib, name)

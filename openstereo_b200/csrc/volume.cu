@@ -270,6 +270,8 @@ __global__ void __launch_bounds__(256, 2) volume_kernel(const __grid_constant__ 
   }
 }
 
+static thread_local const char* g_volume_variant = "";   // osb_volume_last_variant
+
 static int launch_volume(const float* ref_g, const float* tgt_g, const float* ref_c, const float* tgt_c, float* out,
                          int B, int Cg, int Cc, int H, int W, int D, int G, int mask_left, cudaStream_t stream, int reduce_sum = 0) {
   OSB_REQUIRE(B > 0 && H > 0 && W > 0 && D > 0, "volume: empty shape B=%d H=%d W=%d D=%d", B, H, W, D);
@@ -335,6 +337,9 @@ static int launch_volume(const float* ref_g, const float* tgt_g, const float* re
   }
   const long long total = (long long)(p.n_gwc_units + p.n_cat_units) * H * B * p.w_tiles * p.d_chunks;
   OSB_REQUIRE(total < (1ll << 31), "volume: too many work items (%lld)", total);
+  static const char* const names[8] = {"volume<0,0,ldg>", "volume<0,0,tma>", "volume<0,1,ldg>", "volume<0,1,tma>",
+                                       "volume<1,0,ldg>", "volume<1,0,tma>", "volume<1,1,ldg>", "volume<1,1,tma>"};
+  g_volume_variant = names[2 * variant + p.use_tma];
   int per_sm = 0;
   cudaError_t oe = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 32 * GU, smem);
   if (oe != cudaSuccess || per_sm < 1) {
@@ -353,6 +358,8 @@ static int launch_volume(const float* ref_g, const float* tgt_g, const float* re
 }  // namespace osb
 
 extern "C" {
+
+const char* osb_volume_last_variant(void) { return osb::g_volume_variant; }
 
 int osb_gwc_volume_fwd(const float* ref, const float* tgt, float* out, int B, int C, int H, int W, int D, int G,
                        osb_stream_t stream) {

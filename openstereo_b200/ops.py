@@ -582,6 +582,11 @@ def tc_last_variant():
     return (_lib.lib.osb_tc_last_variant() or b"").decode()
 
 
+def volume_last_variant():
+    """Cost-volume kernel this thread launched last, e.g. "volume<1,0,tma>" (VEC, K4, TMA or plain-load staging)."""
+    return (_lib.lib.osb_volume_last_variant() or b"").decode()
+
+
 def tc_overflow_count(device=None, reset=False):
     """Number of loader threads (since the last reset) that staged an activation outside the fp16 range of the tensor-core
     convolutions (|x| >= 4094).  Synchronises the current stream of `device`.  0 = every result is valid."""

@@ -65,14 +65,16 @@ def test_persistent_grid_cap_and_variant_hooks(native):
     """Test hooks of the persistent kernels: declared in the header, bound with their C types, host-only state (no device needed)."""
     from openstereo_b200 import ops
     names = declared_symbols()
-    assert "osb_set_persistent_grid_cap" in names and "osb_tc_last_variant" in names
+    assert "osb_set_persistent_grid_cap" in names and "osb_tc_last_variant" in names and "osb_volume_last_variant" in names
     assert native.lib.osb_set_persistent_grid_cap.argtypes == [ctypes.c_int]
     assert native.lib.osb_set_persistent_grid_cap.restype is ctypes.c_int
     assert native.lib.osb_tc_last_variant.restype is ctypes.c_char_p
+    assert native.lib.osb_volume_last_variant.restype is ctypes.c_char_p
     assert ops.set_persistent_grid_cap(3) == 0
     assert ops.set_persistent_grid_cap(-2) == 3                  # negative = no cap
     assert ops.set_persistent_grid_cap(0) == 0
     assert isinstance(ops.tc_last_variant(), str)
+    assert isinstance(ops.volume_last_variant(), str)
 
 
 def test_ops_refuse_cpu_tensors(native):

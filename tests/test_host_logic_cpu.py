@@ -260,3 +260,65 @@ def test_cuda_core_contract_registry_matches_sources():
     rows = {r.variant for r in REGISTRY}
     assert not found - rows, "instantiations without a contract row: %s" % sorted(found - rows)
     assert not rows - found, "contract rows naming no instantiation: %s" % sorted(rows - found)
+
+
+# Files of the non-convolution kernels.  Two __global__ functions there have rows in the convolution registries instead.
+_KERNEL_CONTRACT_FILES = ("volume.cu", "softargmin.cu", "backward.cu", "geo.cu", "cascade.cu", "coex.cu", "flavours.cu", "conv3d_tc.cu")
+_CONVOLUTIONS_THERE = {"feature_att_gate_kernel", "conv3d_tc_kernel"}
+_GLOBAL = r"__global__\s+void\s+(?:__launch_bounds__\s*\([^()]*\)\s*)?(\w+)\s*\("
+
+
+def _csrc(name):
+    import os
+    import re
+    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "openstereo_b200", "csrc", name)
+    return re.sub(r'//[^\n]*|/\*.*?\*/|"(?:\\.|[^"\\\n])*"', "", open(path).read(), flags=re.S)   # code only: no comments, no strings
+
+
+def _kernel_contract_variants():
+    """Every __global__ instantiation the non-convolution sources can launch, in the registry spelling ("volume_kernel<true,false>",
+    "coex_regression_kernel<5>", "softargmin_kernel").  A templated kernel contributes each spelling with literal template
+    arguments: the function-pointer table of launch_volume, the ternary of launch_warped, the switch of osb_coex_regression_fwd,
+    the if / else of osb_geo_lookup_fwd and direct <<< launches.  An untemplated kernel must be launched with <<<."""
+    import re
+    found = set()
+    for name in _KERNEL_CONTRACT_FILES:
+        src = _csrc(name)
+        for kernel in set(re.findall(_GLOBAL, src)) - _CONVOLUTIONS_THERE:
+            if re.search(r"template\s*<[^<>]*>\s*" + _GLOBAL.replace(r"(\w+)", kernel), src):
+                spellings = re.findall(r"\b%s\s*<([^<>;()]*)>" % kernel, src)
+                assert spellings, "%s: templated %s has no instantiation" % (name, kernel)
+                for args in spellings:
+                    args = args.replace(" ", "").replace("\n", "")
+                    assert re.fullmatch(r"(true|false|\d+)(,(true|false|\d+))*", args), "%s: %s<%s> is not literal" % (name, kernel, args)
+                    found.add("%s<%s>" % (kernel, args))
+            else:
+                assert re.search(r"\b%s\s*<<<" % kernel, src), "%s: %s is never launched with <<<" % (name, kernel)
+                found.add(kernel)
+    return found
+
+
+def test_kernel_contract_registry_matches_sources():
+    """A cost-volume, regression, lookup, backward or layout kernel cannot land without a row in the contract registry of
+    tests/test_kernel_contract_gpu.py (routing, accuracy against fp64, store bounds, store paths, determinism), and no row may
+    name one that is gone.  With the two convolution registries, every __global__ function defined under csrc/ has a row."""
+    import glob
+    import os
+    import re
+    from test_cuda_core_contract_gpu import REGISTRY as CUDA_CORE, kernel_of
+    from test_kernel_contract_gpu import REGISTRY
+    from test_tc_contract_gpu import REGISTRY as TENSOR_CORE
+    found = _kernel_contract_variants()
+    assert {"volume_kernel<false,false>", "volume_kernel<true,true>", "warped_volume_kernel<16>", "coex_regression_kernel<8>",
+            "geo_lookup_kernel<0>", "upsample_softargmin_kernel<true>", "ncdhw_to_ndhwc_kernel"} <= found
+    rows = {r.variant for r in REGISTRY}
+    assert not found - rows, "instantiations without a contract row: %s" % sorted(found - rows)
+    assert not rows - found, "contract rows naming no instantiation: %s" % sorted(rows - found)
+    covered = {v.split("<")[0] for v in rows}
+    covered |= {kernel_of(r.variant).split("<")[0] for r in CUDA_CORE}
+    covered |= {"conv3d_%s_kernel" % r.variant.split("<")[0] for r in TENSOR_CORE}
+    defined = set()
+    for path in glob.glob(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "openstereo_b200", "csrc", "*.cu*")):
+        defined |= set(re.findall(_GLOBAL, _csrc(os.path.basename(path))))
+    assert len(defined) >= 30
+    assert not defined - covered, "__global__ functions with no row in any contract registry: %s" % sorted(defined - covered)
