@@ -197,6 +197,21 @@ int osb_conv3d_k3_tc_gate_fwd(const float* x_ndhwc, const void* w_split, const f
 int osb_conv3d_k3_tc_ncdhw_fwd(const float* x_ncdhw, const void* w_split, const float* scale, const float* shift,
                                const float* residual, float* y, int B, int Cin, int Cout, int D, int H, int W, int act,
                                int out_ndhwc, int res_ndhwc, osb_stream_t stream);
+/* Split NDHWC activations: a channels-last (B,D,H,W,C) tensor stored as (B,D,H,W,2C) fp16 -- the bytes of the fp32 tensor, so
+ * the pointers below are typed float* --, per voxel granules of 16 channels [16 hi | 16 lo] with hi = fp16_rn(16x),
+ * lo = fp16_rn(16x - hi) (saturating; a value outside +-4094 raises the overflow count of osb_tc_overflow_count).  The W = 128
+ * wgmma layers read it with TMA tensor copies and write it from their epilogues, so that layers chained through it skip the
+ * conversion of their input; a split residual is read as (hi + lo) / 16.  Layout codes: */
+#define OSB_LAYOUT_NCDHW 0
+#define OSB_LAYOUT_NDHWC 1
+#define OSB_LAYOUT_SPLIT 2
+/* NCDHW fp32 (B,C,D,H,W) -> split NDHWC, C a multiple of 16. */
+int osb_ncdhw_to_split(const float* x, float* y_split, int B, int C, int D, int H, int W, osb_stream_t stream);
+/* osb_conv3d_k3_tc_fwd / _ncdhw_fwd with each of x, y and residual in any of the layouts above (W = 128; Cout = 32 for a split
+ * y or residual; a split y needs a channels-last residual). */
+int osb_conv3d_k3_tc_split_fwd(const float* x, const void* w_split, const float* scale, const float* shift, const float* residual,
+                               float* y, int B, int Cin, int Cout, int D, int H, int W, int act, int in_layout, int out_layout,
+                               int res_layout, osb_stream_t stream);
 /* Stride-2 variant (the down-sampling convs of the hourglasses): x (B,D,H,W,Cin) channels-last with even D,H,W ->
  * y (B,Cout,D/2,H/2,W/2) or channels-last.  w_split like above but with the kw slices stored in the order (1,0,2)
  * (ops.pack_tc_weight(..., kw_order=(1,0,2))), 16-channel K chunks.  Supported: W=128/Cout=64, W=64/Cout=64|128. */

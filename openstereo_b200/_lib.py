@@ -35,6 +35,8 @@ SIGNATURES = {
     "osb_conv3d_k3_s2_tc_fwd": [_f32p] * 6 + [_i] * 9 + [_s],
     "osb_conv3d_k3_tc_fwd": [_f32p] * 6 + [_i] * 9 + [_s],
     "osb_conv3d_k3_tc_ncdhw_fwd": [_f32p] * 6 + [_i] * 9 + [_s],
+    "osb_conv3d_k3_tc_split_fwd": [_f32p] * 6 + [_i] * 10 + [_s],
+    "osb_ncdhw_to_split": [_f32p, _f32p] + [_i] * 5 + [_s],
     "osb_conv3d_k3_tc_gate_fwd": [_f32p] * 7 + [_i] * 7 + [_s],
     "osb_deconv3d_k4_tc_supported": [_i, _i, _i],
     "osb_conv3d_k3_tc_cs_fwd": [_f32p] * 7 + [_i] * 8 + [_s],

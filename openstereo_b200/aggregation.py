@@ -99,15 +99,22 @@ def _tc_ok(layer, width):
     return _tc_weight(layer, width) is not None
 
 
-def _conv_tc(layer, x_ndhwc, act=ACT_NONE, residual=None, out_ndhwc=True, res_ndhwc=True, in_ncdhw=False):
+def _conv_tc(layer, x_ndhwc, act=ACT_NONE, residual=None, out_ndhwc=True, res_ndhwc=True, in_ncdhw=False, out_split=False):
     wt = _tc_weight(layer, x_ndhwc.shape[4] if in_ncdhw else x_ndhwc.shape[3])
-    return ops.conv3d_k3_tc(x_ndhwc, wt, layer.scale, layer.shift, residual, act, out_ndhwc, res_ndhwc, in_ncdhw)
+    return ops.conv3d_k3_tc(x_ndhwc, wt, layer.scale, layer.shift, residual, act, out_ndhwc, res_ndhwc, in_ncdhw,
+                            out_split=out_split)
 
 
-def _stem_in(layer, volume, act):
+def _split_chain_ok(width, *layers):
+    """True when every layer runs on the W = 128 kernel, which reads and writes split activations (ops.to_split): a chain of
+    them hands its intermediate tensors on in that form."""
+    return USE_TENSOR_CORES and all(ops.conv3d_tc_kc(l.cin, l.cout, width) == 32 for l in layers)
+
+
+def _stem_in(layer, volume, act, out_split=False):
     """First aggregation layer on an NCDHW cost volume: the W = 128 kernel reads NCDHW directly, other variants convert once."""
     if ops.conv3d_tc_kc(layer.cin, layer.cout, volume.shape[-1]) == 32:
-        return _conv_tc(layer, volume, act, in_ncdhw=True)
+        return _conv_tc(layer, volume, act, in_ncdhw=True, out_split=out_split)
     return _conv_tc(layer, ops.to_ndhwc(volume), act)
 
 
@@ -229,7 +236,8 @@ def _classif3_channels_last(classif3, out):
     head0, cls = classif3
     width = out.shape[3]
     if _tc_ok(cls, width):                                         # 32 -> 1 head on the narrow (Cout <= 16) tensor-core variant
-        return _conv_tc(cls, _conv_tc(head0, out, ACT_RELU), ACT_NONE, out_ndhwc=False, res_ndhwc=False)
+        mid = _conv_tc(head0, out, ACT_RELU, out_split=_split_chain_ok(width, head0, cls))
+        return _conv_tc(cls, mid, ACT_NONE, out_ndhwc=False, res_ndhwc=False)
     if cls.cin == 32 and cls.cout == 1 and cls._w5 is not None and cls.stride == 1:
         if "c1" not in cls._tc:
             cls._tc["c1"] = ops.pack_c1_weight(cls._w5)
@@ -256,9 +264,11 @@ class GwcAggregation(_Engine):
         stem_tc = all(_tc_ok(l, width) for l in (self.dres0[0], self.dres0[1], self.dres1[0], self.dres1[1]))
         b, _, dd, hh, ww = volume.shape
         if stem_tc and _tc_ok(self.classif3[0], width) and all(_hg_channels_last_ok(hg, (b, dd, hh, ww, 32)) for hg in self.hg):
-            # everything from the volume to the classifier runs channels-last on the tensor cores: ONE layout conversion
-            c = _conv_tc(self.dres0[1], _stem_in(self.dres0[0], volume, ACT_RELU), ACT_RELU)
-            out = _conv_tc(self.dres1[1], _conv_tc(self.dres1[0], c, ACT_RELU), ACT_NONE, residual=c)
+            # everything from the volume to the classifier runs channels-last on the tensor cores: ONE layout conversion; inside
+            # the W = 128 stem the activations stay split
+            split = _split_chain_ok(width, self.dres0[0], self.dres0[1], self.dres1[0], self.dres1[1])
+            c = _conv_tc(self.dres0[1], _stem_in(self.dres0[0], volume, ACT_RELU, out_split=split), ACT_RELU, out_split=split)
+            out = _conv_tc(self.dres1[1], _conv_tc(self.dres1[0], c, ACT_RELU, out_split=split), ACT_NONE, residual=c)
             for hg in self.hg:
                 out = _gwc_hourglass_channels_last(hg, out)
             return _classif3_channels_last(self.classif3, out)

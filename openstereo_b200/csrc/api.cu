@@ -128,6 +128,27 @@ bool make_tensor_map_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_
   return true;
 }
 
+bool make_tensor_map_split(CUtensorMap* out, const void* base, int C, int W, int H, int BD, int kc) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) {
+    set_error("cuTensorMapEncodeTiled not available from the driver");
+    return false;
+  }
+  const uint64_t vox = 2ull * C * sizeof(uint16_t);                  // bytes per voxel
+  const cuuint64_t dims[4] = {2ull * C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)BD};
+  const cuuint64_t strides[3] = {vox, vox * W, vox * W * H};
+  const cuuint32_t box[4] = {2u * kc, (cuuint32_t)W, 1, 1};
+  const cuuint32_t elem[4] = {1, 1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, elem,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, kc == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled (split activations) failed with CUresult %d", (int)r);
+    return false;
+  }
+  return true;
+}
+
 }  // namespace osb
 
 extern "C" {

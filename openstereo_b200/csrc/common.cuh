@@ -79,6 +79,14 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// 4-D TMA tile load (coordinates innermost-first; boxes partly or wholly outside the tensor are zero-filled)
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
@@ -92,5 +100,8 @@ __device__ __forceinline__ void st_cs_f4(float* p, float4 v) { __stcs(reinterpre
 // when the driver entry point is missing or the encode fails.
 bool make_tensor_map_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1_bytes,
                         uint64_t stride2_bytes, uint32_t box0, uint32_t box1, uint32_t box2);
+// Split NDHWC activations (tc_common.cuh) of a (B, D, H, W, C) tensor as a 4-D fp16 map (2C, W, H, B*D), box = `kc` channels'
+// granules x W voxels x 1 x 1, zero fill outside, the wgmma operand swizzle (kc = 32: 128 B, kc = 16: 64 B).
+bool make_tensor_map_split(CUtensorMap* out, const void* base, int C, int W, int H, int BD, int kc);
 
 }  // namespace osb

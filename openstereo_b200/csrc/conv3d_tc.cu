@@ -16,8 +16,9 @@
 //     implicit because a row tile spans the whole image width).
 //   * kh taps: output row h needs input rows h-1, h, h+1, staged through a shared-memory ring; row r of a phase meets weight
 //     slice kh = r.
-//   * an operand row is 128 bytes = [32 channels hi | 32 channels lo] fp16, SWIZZLE_128B; a K = 16 MMA step is 32 bytes, so
-//     the hi k-steps sit at descriptor offsets +0, +2 and the lo ones at +4, +6 (16-byte units) of the SAME tile.
+//   * an operand row is 128 bytes = two split granules [16 hi | 16 lo | 16 hi | 16 lo] fp16, SWIZZLE_128B; a K = 16 MMA step
+//     is 32 bytes, so the hi k-steps sit at descriptor offsets +0, +4 and the lo ones at +2, +6 (16-byte units) of the SAME tile
+//     (weight rows stay [32 hi | 32 lo]: hi +0, +2, lo +4, +6).
 //   * kd taps and 32-channel Cin chunks are phases of one work item; the three kh weight slices of a phase are double-buffered.
 // Work item = (image b, output plane d, output rows 2p and 2p + 1): TWO accumulator tiles of 128 x 3*Cout fp32, one per consumer
 // warpgroup, each held in that warpgroup's registers as two m64 halves (96 registers per thread for Cout = 32).  A phase stages
@@ -25,9 +26,11 @@
 // (0 <= r - t <= 2), so an input row is staged twice per two output rows instead of three times per output row, and each weight
 // slice a phase streams serves both output rows.
 //
-// Operand staging.  The loader warps read coalesced float4 from global/L2 (or the raw rows a bulk-copy producer staged), convert
-// to the hi/lo fp16 pair, write both halves of the row with the 128-byte swizzle applied by hand (two conflict-free STS.64) and
-// publish the tile to the tensor core through fence.proxy.async + mbarrier.
+// Operand staging.  A split NDHWC input (tc_common.cuh) is already in operand form: one elected lane of the loader warpgroup
+// copies each row with a TMA tensor copy (128-byte swizzle, zero fill for rows outside the image) straight into the ring.  fp32
+// inputs go through the converters: the loader warps read coalesced float4 from global/L2 (or the raw rows a bulk-copy producer
+// staged), convert to the hi/lo fp16 pair, write the row in the same granule order with the 128-byte swizzle applied by hand (two
+// conflict-free STS.64) and publish the tile to the tensor core through fence.proxy.async + mbarrier.
 //
 // Warp roles (512 threads, 1 CTA/SM, persistent; setmaxnreg moves the registers, tc_common.cuh): warps 0-7 = two consumer
 // warpgroups (wgmma issue, then the epilogue of the finished tile on the accumulator fragments: kw un-shift by shuffles, BN /
@@ -53,6 +56,7 @@ constexpr int TC_RAW = 2;          // raw fp32 rows staged by 1-D TMA bulk copie
 constexpr int TC_ROW_BYTES = TC_W * TC_KC * 4;     // 16384: one staged input row (hi and lo halves of every voxel)
 
 struct TcParams {
+  CUtensorMap xmap;        // in_split: the input as split NDHWC rows (make_tensor_map_split)
   const float* x;          // (B, D, H, W, Cin) channels-last
   const void* w;           // fp16 [3 kd][Cin/32][3 kh][3*Cout][32 hi | 32 lo]  (ops.pack_tc_weight)
   const float* scale;
@@ -67,6 +71,7 @@ struct TcParams {
   int bulk_rows;     // input rows staged by TMA bulk copies, TC_RAW deep: Cin == 32 channels-last (one 16 KB copy per row) or NCDHW
                      // (32 copies of 512 bytes, one per channel plane)
   int in_ncdhw;      // the INPUT is (B, Cin, D, H, W): the first aggregation layer reads the cost volume as the volume kernel wrote it
+  int in_split, out_split, res_split;   // x / y / residual are split NDHWC (tc_common.cuh)
   int items, hblocks;
 };
 
@@ -85,7 +90,7 @@ struct TcCfg {
 };
 
 template <int COUT>
-__global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcParams p) {
+__global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const __grid_constant__ TcParams p) {
   using C = TcCfg<COUT>;
   constexpr int N3 = C::N3;
   constexpr int B_SLICE = C::B_SLICE;
@@ -113,7 +118,7 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_STAGES; ++s) {
-      mbar_init(&a_ready[s], 128);
+      mbar_init(&a_ready[s], p.in_split ? 1 : 128);   // one expect_tx arrival of the TMA issuer, or every converter thread
       mbar_init(&a_empty[s], 4 * TC_WGS);
     }
     for (int k = 0; k < TC_BSLOTS * 3; ++k) {
@@ -163,7 +168,6 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
     const int wg = warp >> 2;
     xchg += wg * C::XCHG_FLOATS;
     const int bar_xchg = 1 + wg;                     // this warpgroup's named barrier
-    constexpr uint32_t LO = TcK<TC_KC>::LO_OFF;     // descriptor offset of the lo half of an operand row
     constexpr uint32_t A_HALF = 64 * TC_KC * 4 / 16;  // descriptor offset of operand rows 64..127
     const uint64_t dbase = desc_sw128_base();
     // Descriptors differ only in their 14-bit start-address field (bits 0-13, units of 16 bytes).
@@ -198,7 +202,8 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
               wg_fence();
 #pragma unroll
               for (int ks = 0; ks < TcK<TC_KC>::KSTEPS; ++ks)
-                wg_mma_split<N3>(acc, da0 + 2 * ks, A_HALF, db0 + 2 * ks, LO, ks > 0 ? 1u : accum);
+                wg_mma_split<N3>(acc, da0 + TcK<TC_KC>::A_KSTEP * ks, A_HALF, TcK<TC_KC>::A_LO, db0 + 2 * ks, TcK<TC_KC>::B_LO,
+                                 ks > 0 ? 1u : accum);
               wg_commit();
               wg_wait_all();
               accum = 1;
@@ -226,16 +231,38 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
         return true;
       };
       frag_epilogue<COUT>(acc, lane, q, tiles + warp * FRAG_TP_FLOATS, s_scale, s_shift, p.act, p.y, p.out_ndhwc ? 1 : plane, p.residual, p.res_ndhwc ? 1 : plane,
-                          nullptr, rows, COUT == 32 ? 32 : p.Cout);
+                          nullptr, rows, COUT == 32 ? 32 : p.Cout, p.out_split, p.res_split, p.overflow);
     }
   }
   // ---------------------------------------------------------------------------------------------- A-row loaders
   else if (warp < 4 * TC_WGS + 4) {
     setmaxnreg_dec<TC_LOADER_REGS>();
+    if (p.in_split) {
+      // split rows: one elected lane of warp 8 copies each row of the sequence with a TMA tensor copy of the chunk's two granules
+      // x 128 columns; rows above / below the image fall outside the map and arrive as zeros (the conv's padding)
+      if (warp == 4 * TC_WGS && elect_one()) {
+        RowIter ld{(int)blockIdx.x, 0, 0, -1};
+        if (ld.it < p.items) ld.kd = (((ld.it / p.hblocks) % p.D) == 0) ? 1 : 0;
+        uint32_t rowc = 0;
+        while (advance(ld)) {
+          const int hb = ld.it % p.hblocks;
+          const int d = (ld.it / p.hblocks) % p.D;
+          const int b = ld.it / (p.hblocks * p.D);
+          const uint32_t s = rowc % TC_STAGES, par = (rowc / TC_STAGES) & 1;
+          mbar_wait_relaxed(&a_empty[s], par ^ 1);
+          mbar_arrive_expect_tx(&a_ready[s], TC_ROW_BYTES);
+          tma_load_4d(a_buf + s * TC_ROW_BYTES, &p.xmap, &a_ready[s], 2 * TC_KC * ld.ch, 0, hb * TC_TILES - 1 + ld.r, b * p.D + d + ld.kd - 1);
+          ++rowc;
+        }
+      }
+      __syncwarp();
+      return;
+    }
     const int lt = threadIdx.x - 4 * TC_WGS * 32;    // 0..127
     const int vsel = lt >> 3, c16 = lt & 7;          // this thread's voxel (mod 16) and fp32 16-byte chunk of the 32-channel slice
-    // voxel order inside a half-warp alternates bit 2 of the column so that the STS.64 pairs of stage_f16_split hit disjoint banks
-    const int vcol = ((vsel & 1) << 2) | ((vsel >> 1) & 3) | (vsel & 8);
+    // voxel order inside a half-warp alternates bit 1 of the column: a granule-ordered row puts its hi halves in chunks {0,1,4,5}
+    // and its lo halves in {2,3,6,7}, and only rows differing in bit 1 swizzle those onto disjoint banks (conflict-free STS.64)
+    const int vcol = ((vsel & 1) << 1) | ((vsel >> 1) & 1) | (vsel & 12);
     float amax = 0.f;
     // The two input layouts run separate copies of the loops below (NCDHW is a compile-time flag), so that each copy keeps only
     // its own layout's swizzled store offsets live: both fit the loaders' register budget (TC_LOADER_REGS) without spilling.
@@ -402,14 +429,16 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const TcPar
 }
 
 // ---------------------------------------------------------------------------------------- layout conversion kernels
-// NCDHW -> NDHWC through a 32x32 shared-memory transpose (both sides coalesced).
+// NCDHW -> NDHWC through a 32x32 shared-memory transpose (both sides coalesced); with `ys`, to split NDHWC instead of y (each
+// value's hi and lo halves, out-of-range values reported on `overflow`).
 __global__ void __launch_bounds__(256) ncdhw_to_ndhwc_kernel(const float* __restrict__ x, float* __restrict__ y, int C, int Cp,
-                                                             size_t vol) {
+                                                             size_t vol, uint16_t* __restrict__ ys, unsigned int* overflow) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const size_t v0 = (size_t)blockIdx.x * 32;
   const int c0 = blockIdx.y * 32;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;       // 32 x 8
+  float amax = 0.f;
   for (int i = ty; i < 32; i += 8) {
     const int c = c0 + i;
     const size_t v = v0 + tx;
@@ -419,15 +448,28 @@ __global__ void __launch_bounds__(256) ncdhw_to_ndhwc_kernel(const float* __rest
   for (int i = ty; i < 32; i += 8) {
     const size_t v = v0 + i;
     const int c = c0 + tx;
-    if (c < Cp && v < vol) y[((size_t)b * vol + v) * Cp + c] = tile[tx][i];      // channels C .. Cp-1: zero padding
+    if (c >= Cp || v >= vol) continue;
+    if (!ys) {
+      y[((size_t)b * vol + v) * Cp + c] = tile[tx][i];      // channels C .. Cp-1: zero padding
+      continue;
+    }
+    const float s = tile[tx][i] * TC_ACT_SCALE;
+    const uint32_t hl = cvt_f16x2_sat(s, s - f16x2_to_float2(cvt_f16x2_sat(s, 0.f)).x);   // {hi, lo}
+    uint16_t* vox = ys + ((size_t)b * vol + v) * 2 * Cp;
+    vox[split_index(c)] = (uint16_t)(hl & 0xFFFFu);
+    vox[split_index(c) + SPLIT_GRANULE] = (uint16_t)(hl >> 16);
+    amax = fmaxf(amax, fabsf(s));
   }
+  if (ys) tc_report_overflow(overflow, amax);
 }
 
 template <int COUT>
 int launch_tc(const TcArgs& a, cudaStream_t stream) {
   TcParams p{};
   p.Cout = a.Cout, p.in_ncdhw = a.in_ncdhw;
-  p.bulk_rows = a.in_ncdhw || a.Cin == TC_KC;   // channels-last Cin = 64 rows are strided: register-staged
+  p.in_split = a.in_split, p.out_split = a.out_split, p.res_split = a.res_split;
+  p.bulk_rows = !a.in_split && (a.in_ncdhw || a.Cin == TC_KC);   // fp32 channels-last Cin = 64 rows are strided: register-staged
+  if (a.in_split && !make_tensor_map_split(&p.xmap, a.x, a.Cin, TC_W, a.H, a.B * a.D, TC_KC)) return OSB_ECUDA;
   p.hblocks = (a.H + TC_TILES - 1) / TC_TILES;
   static const std::string variant = tc_variant_name("tc<%d>", COUT);
   return launch_persistent<conv3d_tc_kernel<COUT>>(a, p, (long long)a.B * a.D * p.hblocks, TcCfg<COUT>::SMEM, variant.c_str(), stream);
@@ -456,7 +498,21 @@ int osb_ncdhw_to_ndhwc_pad(const float* x, float* y, int B, int C, int Cpad, int
   OSB_REQUIRE(B > 0 && C > 0 && Cpad >= C && D > 0 && H > 0 && W > 0 && B <= 65535, "ncdhw_to_ndhwc: bad shape");
   const size_t vol = (size_t)D * H * W;
   dim3 grid((unsigned)((vol + 31) / 32), (Cpad + 31) / 32, B);
-  ncdhw_to_ndhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, y, C, Cpad, vol);
+  ncdhw_to_ndhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, y, C, Cpad, vol, nullptr, nullptr);
+  count_launch();
+  return check_launch("ncdhw_to_ndhwc_kernel");
+}
+
+int osb_ncdhw_to_split(const float* x, float* y_split, int B, int C, int D, int H, int W, osb_stream_t stream) {
+  using namespace osb;
+  OSB_REQUIRE(x && y_split, "ncdhw_to_split: null pointer");
+  OSB_REQUIRE(B > 0 && C > 0 && C % SPLIT_GRANULE == 0 && D > 0 && H > 0 && W > 0 && B <= 65535,
+              "ncdhw_to_split: bad shape (C must be a multiple of %d)", SPLIT_GRANULE);
+  unsigned int* flag = tc_overflow_flag();
+  if (!flag) return OSB_ECUDA;
+  const size_t vol = (size_t)D * H * W;
+  dim3 grid((unsigned)((vol + 31) / 32), (C + 31) / 32, B);
+  ncdhw_to_ndhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, nullptr, C, C, vol, reinterpret_cast<uint16_t*>(y_split), flag);
   count_launch();
   return check_launch("ncdhw_to_ndhwc_kernel");
 }
@@ -472,6 +528,12 @@ static int conv3d_k3_tc_impl(osb::TcArgs a, int dilation, osb_stream_t stream) {
   OSB_REQUIRE(!a.in_ncdhw || kc == 32, "conv3d_k3_tc: NCDHW input is served by the W = 128 kernel only");
   OSB_REQUIRE((!a.ystride && !a.gate) || kc == 16, "conv3d_k3_tc: a channel slice or gate needs the 16-channel-chunk kernels");
   OSB_REQUIRE(a.Cout > 16 || (!a.out_ndhwc && (!a.residual || !a.res_ndhwc)), "conv3d_k3_tc: Cout <= 16 writes (and adds) NCDHW tensors only");
+  OSB_REQUIRE(!(a.in_split || a.out_split || a.res_split) || (kc == 32 && !a.ystride && !a.gate),
+              "conv3d_k3_tc: split activations are served by the W = 128 kernel only");
+  OSB_REQUIRE(!a.in_split || !a.in_ncdhw, "conv3d_k3_tc: an input is either NCDHW or split");
+  OSB_REQUIRE((!a.out_split || a.out_ndhwc) && (!a.res_split || a.res_ndhwc), "conv3d_k3_tc: split tensors are channels-last");
+  OSB_REQUIRE(!(a.out_split || a.res_split) || (a.out_ndhwc && (!a.residual || a.res_ndhwc)),
+              "conv3d_k3_tc: a split output or residual needs a channels-last output and residual");
   const TcLaunch launch = select_conv3d_tc(a.Cin, a.Cout, a.W, dilation, a.gate != nullptr, a.slice()).launch;
   const int rc = check_tc_args("conv3d_k3_tc", a, launch);
   return rc != OSB_OK ? rc : launch(a, (cudaStream_t)stream);
@@ -504,6 +566,17 @@ int osb_conv3d_k3_tc_ncdhw_fwd(const float* x_ncdhw, const void* w_split, const 
                                int out_ndhwc, int res_ndhwc, osb_stream_t stream) {
   return conv3d_k3_tc_impl({x_ncdhw, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, D, H, W, act, out_ndhwc, res_ndhwc, 1, 0,
                             Cout}, 1, stream);
+}
+
+int osb_conv3d_k3_tc_split_fwd(const float* x, const void* w_split, const float* scale, const float* shift, const float* residual,
+                               float* y, int B, int Cin, int Cout, int D, int H, int W, int act, int in_layout, int out_layout,
+                               int res_layout, osb_stream_t stream) {
+  auto known = [](int l) { return l == OSB_LAYOUT_NCDHW || l == OSB_LAYOUT_NDHWC || l == OSB_LAYOUT_SPLIT; };
+  OSB_REQUIRE(known(in_layout) && known(out_layout) && known(res_layout), "conv3d_k3_tc_split: unknown layout");
+  osb::TcArgs a{x, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, D, H, W, act, out_layout != OSB_LAYOUT_NCDHW, res_layout != OSB_LAYOUT_NCDHW,
+                in_layout == OSB_LAYOUT_NCDHW, 0, Cout};
+  a.in_split = in_layout == OSB_LAYOUT_SPLIT, a.out_split = out_layout == OSB_LAYOUT_SPLIT, a.res_split = res_layout == OSB_LAYOUT_SPLIT;
+  return conv3d_k3_tc_impl(a, 1, stream);
 }
 
 int osb_conv2d_tc_kc(int Cin, int Cout, int W, int dilation) { return osb::select_conv3d_tc(Cin, Cout, W, dilation, false, false).kc; }

@@ -76,7 +76,6 @@ struct TcdcCfg {
   static_assert(STAGES >= NLW, "the ring must hold at least one unit per loader warp");
   static constexpr int HBLK = TILES * R;                    // input rows per work item
   static constexpr int KSTEPS = KC / 16;                    // K = 16 fp16 channels per MMA
-  static constexpr int LO = KC / 8;                         // descriptor offset (16-byte units) of the lo half of a row
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + STAGES * UNIT_BYTES;
   static constexpr int STAGE_OFF = B_OFF + TC_BSLOTS * KS_ * B_SUB;   // [TC_WGS][128][LD] fp32 accumulator tiles
@@ -243,7 +242,7 @@ __global__ void __launch_bounds__(TcdcCfg<COUT, KC, W, TILES, GW, KS>::THREADS, 
               wg_fence();
 #pragma unroll
               for (int ks = 0; ks < C::KSTEPS; ++ks)
-                wg_mma_split<C::NGK>(acc, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum);
+                wg_mma_split<C::NGK>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, TcK<KC>::A_LO, db0 + 2 * ks, TcK<KC>::B_LO, ks > 0 ? 1u : accum);
               wg_commit();
               wg_wait_all();
               accum = 1;

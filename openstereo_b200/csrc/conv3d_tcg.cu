@@ -78,7 +78,6 @@ struct TcgCfg {
   static constexpr int S_FIRST = -DIL;                      // unit start rows run from S_FIRST to S_LAST (block-relative)
   static constexpr int S_LAST = (NT - 1) * TS + DIL;
   static constexpr int KSTEPS = KC / 16;                    // K = 16 fp16 channels per MMA
-  static constexpr int LO = KC / 8;                         // descriptor offset (16-byte units) of the lo half of a row
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + STAGES * UNIT_BYTES;
   static constexpr int BAR_OFF = B_OFF + TC_BSLOTS * 3 * B_SUB;
@@ -213,7 +212,7 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
               wg_fence();
 #pragma unroll
               for (int ks = 0; ks < C::KSTEPS; ++ks)
-                wg_mma_split<C::NG3>(acc, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum);
+                wg_mma_split<C::NG3>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, TcK<KC>::A_LO, db0 + 2 * ks, TcK<KC>::B_LO, ks > 0 ? 1u : accum);
               wg_commit();
               wg_wait_all();
               accum = 1;

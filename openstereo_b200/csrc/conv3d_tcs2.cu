@@ -72,7 +72,6 @@ struct Tcs2Cfg {
   static constexpr int NU = TILES * 3 * 2;                   // units of one (kd, chunk) phase: (tile, kh, column parity)
   static constexpr int HBLK = TILES * R;                    // output rows per work item
   static constexpr int KSTEPS = KC / 16;                    // K = 16 fp16 channels per MMA
-  static constexpr int LO = KC / 8;                         // descriptor offset (16-byte units) of the lo half of a row
   static constexpr int A_OFF = 0;
   static constexpr int B_OFF = A_OFF + STAGES * UNIT_BYTES;
   static constexpr int STAGE_OFF = B_OFF + TC_BSLOTS * 3 * B_SLOT;   // [TC_WGS][128][LD] fp32 accumulator tiles
@@ -196,8 +195,8 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
                 wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < C::KSTEPS; ++ks) {
-                  if (par == 0) wg_mma_split<C::G>(acc_e, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum_e);
-                  else wg_mma_split<2 * C::G>(acc_o, da0 + 2 * ks, A_HALF, db0 + 2 * ks, C::LO, ks > 0 ? 1u : accum_o);
+                  if (par == 0) wg_mma_split<C::G>(acc_e, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, TcK<KC>::A_LO, db0 + 2 * ks, TcK<KC>::B_LO, ks > 0 ? 1u : accum_e);
+                  else wg_mma_split<2 * C::G>(acc_o, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, TcK<KC>::A_LO, db0 + 2 * ks, TcK<KC>::B_LO, ks > 0 ? 1u : accum_o);
                 }
                 wg_commit();
                 wg_wait_all();

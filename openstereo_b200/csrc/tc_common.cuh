@@ -100,14 +100,15 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
 // One K = 16 step of the 3xFP16 product (below) into a 128-row accumulator tile held as two m64 halves: half h reads operand rows
-// 64h .. 64h + 63 (a_half = their descriptor offset in 16-byte units), `lo` = descriptor offset of the lo half of a row.
+// 64h .. 64h + 63 (a_half = their descriptor offset in 16-byte units), a_lo / b_lo = descriptor offset of the lo half of the k-step
+// in an A / B row (they differ for 32-channel rows: A rows are split granules, B rows [32 hi | 32 lo], see TcK).
 template <int N>
-__device__ __forceinline__ void wg_mma_split(float (&acc)[2][N / 2], uint64_t da, uint32_t a_half, uint64_t db, uint32_t lo,
-                                             uint32_t accumulate) {
+__device__ __forceinline__ void wg_mma_split(float (&acc)[2][N / 2], uint64_t da, uint32_t a_half, uint32_t a_lo, uint64_t db,
+                                             uint32_t b_lo, uint32_t accumulate) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    wgmma_f16<N>(acc[h], da + h * a_half + lo, db, accumulate);   // small terms first
-    wgmma_f16<N>(acc[h], da + h * a_half, db + lo, 1);
+    wgmma_f16<N>(acc[h], da + h * a_half + a_lo, db, accumulate);   // small terms first
+    wgmma_f16<N>(acc[h], da + h * a_half, db + b_lo, 1);
     wgmma_f16<N>(acc[h], da + h * a_half, db, 1);
   }
 }
@@ -246,29 +247,59 @@ __device__ __forceinline__ int swz_offset(int row, int c) {
 }
 
 
+// ------------------------------------------------------------------------------- split NDHWC activations
+// The format the wgmma layers hand each other channels-last activations in: per voxel, channel granules of 16, each
+// [16 fp16 hi | 16 fp16 lo] (64 bytes) of x * TC_ACT_SCALE split as f16_split4 does.  A (B, D, H, W, C) tensor is stored as
+// (B, D, H, W, 2C) fp16: the bytes of the fp32 tensor, so voxel and channel-group offsets counted in floats (a multiple of 16
+// channels) address the same bytes.  An operand row of KC channels is KC / 16 whole granules: a TMA tensor copy of it lands in
+// shared memory exactly as the converters stage it (stage_f16_split), and the MMAs read the same values either way.
+constexpr int SPLIT_GRANULE = 16;
+// fp16 index, inside its voxel, of the hi part of channel c (the lo part follows SPLIT_GRANULE halves later)
+__device__ __forceinline__ int split_index(int c) { return (c / SPLIT_GRANULE) * 2 * SPLIT_GRANULE + c % SPLIT_GRANULE; }
+// encode four channels c .. c + 3 (c % 4 == 0) of one voxel
+__device__ __forceinline__ void split_store4(uint16_t* vox, int c, const float4 v, float& amax) {
+  uint2 hi, lo;
+  f16_split4(v, hi, lo, amax);
+  *reinterpret_cast<uint2*>(vox + split_index(c)) = hi;
+  *reinterpret_cast<uint2*>(vox + split_index(c) + SPLIT_GRANULE) = lo;
+}
+// decode four channels: (hi + lo) * 2^-4, about 22 significant bits of the value that was encoded
+__device__ __forceinline__ float4 split_load4(const uint16_t* vox, int c) {
+  const uint2 hi = __ldg(reinterpret_cast<const uint2*>(vox + split_index(c)));
+  const uint2 lo = __ldg(reinterpret_cast<const uint2*>(vox + split_index(c) + SPLIT_GRANULE));
+  const float2 h01 = f16x2_to_float2(hi.x), h23 = f16x2_to_float2(hi.y), l01 = f16x2_to_float2(lo.x), l23 = f16x2_to_float2(lo.y);
+  constexpr float inv = 1.f / TC_ACT_SCALE;
+  return make_float4((h01.x + l01.x) * inv, (h01.y + l01.y) * inv, (h23.x + l23.x) * inv, (h23.y + l23.y) * inv);
+}
+
 // Stage four fp32 channels (fp32 16-byte chunk `q` of the KC-channel slice of operand row `row`) into a swizzled operand tile whose
-// K-major rows hold [KC fp16 hi | KC fp16 lo] = 4*KC bytes: hi part to 16-byte chunk q/2, lo part to chunk KC/8 + q/2, 8 bytes each.
+// K-major rows hold KC / 16 split granules = 4*KC bytes (the layout of a split NDHWC row): hi part to 16-byte chunk
+// 4(q/4) + (q%4)/2, lo part two chunks later, 8 bytes each.
 template <int KC>
 __device__ __forceinline__ void stage_f16_split(uint8_t* tile, int row, int q, const float4 v, float& amax) {
   uint2 hi, lo;
   f16_split4(v, hi, lo, amax);
-  const int sub = (q & 1) << 3;
-  *reinterpret_cast<uint2*>(tile + swz_offset<KC>(row, q >> 1) + sub) = hi;
-  *reinterpret_cast<uint2*>(tile + swz_offset<KC>(row, KC / 8 + (q >> 1)) + sub) = lo;
+  const int sub = (q & 1) << 3, chunk = 4 * (q >> 2) + ((q >> 1) & 1);
+  *reinterpret_cast<uint2*>(tile + swz_offset<KC>(row, chunk) + sub) = hi;
+  *reinterpret_cast<uint2*>(tile + swz_offset<KC>(row, chunk + 2) + sub) = lo;
 }
 // Lane -> operand row inside a warp-wide load of VPL = 128 / KC voxels (KC/4 lanes each), permuted so that the two STS.64 of
-// stage_f16_split are bank-conflict free per half-warp: SWIZZLE_128B rows (KC = 32) must differ in bit 2, SWIZZLE_64B rows
+// stage_f16_split are bank-conflict free per half-warp: SWIZZLE_128B rows (KC = 32, granule order) must differ in bit 1, SWIZZLE_64B rows
 // (KC = 16) must be {r, r+1, r+4, r+5}.  Global loads stay whole 16-byte chunks of whole voxels either way.
 template <int KC>
 __device__ __forceinline__ int lane_voxel(int lane) {
-  if constexpr (KC == 32) return (((lane >> 3) & 1) << 2) | (lane >> 4);                       // 4 voxels: 0,4 | 1,5 (caller adds the rest)
+  if constexpr (KC == 32) return (((lane >> 3) & 1) << 1) | (lane >> 4);                       // 4 voxels: 0,2 | 1,3 (caller adds the rest)
   else return ((lane >> 2) & 1) | (((lane >> 3) & 1) << 2) | ((lane >> 4) << 1);               // 8 voxels: 0,1,4,5 | 2,3,6,7
 }
-// MMAs issued per accumulator per staged (unit, weight slice): k-steps of 16 channels x 3 split terms
+// MMAs issued per accumulator per staged (unit, weight slice): k-steps of 16 channels x 3 split terms.  Descriptor start-address
+// offsets in 16-byte units: k-step ks of an A row (split granules) is hi at A_KSTEP * ks, lo A_LO further; of a B row
+// ([KC hi | KC lo], ops.pack_tc_weight) hi at 2 * ks, lo B_LO further.  For KC = 16 both layouts are the same.
 template <int KC>
 struct TcK {
   static constexpr int KSTEPS = KC / 16;
-  static constexpr int LO_OFF = KC / 8;           // descriptor start-address offset (16-byte units) of the lo half of a row
+  static constexpr int A_KSTEP = 4;
+  static constexpr int A_LO = 2;
+  static constexpr int B_LO = KC / 8;
 };
 
 // ------------------------------------------------------------------------------- fragment-resident stride-1 epilogue
@@ -357,16 +388,20 @@ constexpr int FRAG_TP_FLOATS = 16 * FRAG_TP_STRIDE;
 //     fragments (32 bytes of each of 8 rows per instruction) needs 4x the L1 wavefronts on the data path the MMAs' operand reads
 //     also use.  BN, residual, activation and gate run on the transposed values, where a lane's 4 channels are fixed.
 //   * otherwise straight from the fragments: NCDHW planes take 8 consecutive voxels of 4 channels per warp instruction.
+// y_split / res_split: the channels-last output / residual is split NDHWC (G = 32 only; offsets still count floats, which address
+// the same bytes); a split output reports values outside the fp16 range on `overflow`.
 template <int G, class Rows>
 __device__ __forceinline__ void frag_epilogue(const float (&acc)[2][3 * G / 2], int lane, int wq, float* tbuf, const float* sc,
                                               const float* sh, int act, float* y, size_t ycs, const float* res, size_t rcs,
-                                              const float* gate, Rows rows, int nch) {
+                                              const float* gate, Rows rows, int nch, bool y_split = false, bool res_split = false,
+                                              unsigned int* overflow = nullptr) {
   const int c0 = 2 * (lane & 3), l4 = lane >> 2;
   if constexpr (G == 32) {
     if (ycs == 1 && (!res || rcs == 1)) {
       const int c4 = 4 * (lane & 7), sub = lane >> 3;
       const float4 a = *reinterpret_cast<const float4*>(sc + c4);
       const float4 b = *reinterpret_cast<const float4*>(sh + c4);
+      float amax = 0.f;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         __syncwarp();                                   // the previous half's readers are done with the tile
@@ -389,7 +424,10 @@ __device__ __forceinline__ void frag_epilogue(const float (&acc)[2][3 * G / 2], 
         if (res) {
           float4 r[4];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) r[i] = ok[i] ? __ldg(reinterpret_cast<const float4*>(res + ro[i] + c4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          for (int i = 0; i < 4; ++i)
+            r[i] = !ok[i] ? make_float4(0.f, 0.f, 0.f, 0.f)
+                 : res_split ? split_load4(reinterpret_cast<const uint16_t*>(res + ro[i]), c4)
+                             : __ldg(reinterpret_cast<const float4*>(res + ro[i] + c4));
 #pragma unroll
           for (int i = 0; i < 4; ++i) o[i].x += r[i].x, o[i].y += r[i].y, o[i].z += r[i].z, o[i].w += r[i].w;
         }
@@ -411,9 +449,13 @@ __device__ __forceinline__ void frag_epilogue(const float (&acc)[2][3 * G / 2], 
           for (int i = 0; i < 4; ++i) o[i].x *= g[i].x, o[i].y *= g[i].y, o[i].z *= g[i].z, o[i].w *= g[i].w;
         }
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-          if (ok[i]) *reinterpret_cast<float4*>(y + yo[i] + c4) = o[i];
+        for (int i = 0; i < 4; ++i) {
+          if (!ok[i]) continue;
+          if (y_split) split_store4(reinterpret_cast<uint16_t*>(y + yo[i]), c4, o[i], amax);
+          else *reinterpret_cast<float4*>(y + yo[i] + c4) = o[i];
+        }
       }
+      if (y_split) tc_report_overflow(overflow, amax);
       return;
     }
   }
@@ -554,6 +596,7 @@ struct TcArgs {
   int cout_real;           // channels an NCDHW output / residual holds (< Cout: a zero-padded channel plan)
   float kappa;             // set by check_tc_args
   unsigned int* overflow;  // set by check_tc_args
+  int in_split = 0, out_split = 0, res_split = 0;   // stride 1, W = 128: the channels-last x / y / residual is split NDHWC
   bool slice() const { return ystride != 0 && ystride != Cout; }
 };
 // Launcher of one instantiation: the result of a family's selector (null: no instantiation serves the arguments).

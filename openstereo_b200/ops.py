@@ -49,22 +49,24 @@ def profile_stop():
     return out or {}
 
 
-def _call(name, *args):
+def _call(name, *args, profile_as=None):
+    """profile_as: the name the profile records the launch under (default: the entry point), so that an entry point serving
+    another layout of the same layers keeps the existing record of those layers."""
     dev = _LAUNCH_DEVICE[0]
     if dev is not None and dev != torch.cuda.current_device():
         with torch.cuda.device(dev):                     # device guard: kernels launch where their operands live
-            return _call_on_current(name, *args)
-    return _call_on_current(name, *args)
+            return _call_on_current(name, args, profile_as or name)
+    return _call_on_current(name, args, profile_as or name)
 
 
-def _call_on_current(name, *args):
+def _call_on_current(name, args, key):
     if _PROFILE is None:
         return _lib.call(name, *args)
     start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     start.record()
     _lib.call(name, *args)
     stop.record()
-    _PROFILE.setdefault(name, []).append((start, stop))
+    _PROFILE.setdefault(key, []).append((start, stop))
 
 
 def _prep(t, name):
@@ -729,26 +731,78 @@ def to_ndhwc(x, pad_to=None):
     return y
 
 
+# Split NDHWC activations (include/openstereo_b200.h, csrc/tc_common.cuh): a channels-last (B,D,H,W,C) fp32 tensor held as
+# (B,D,H,W,2C) fp16, per voxel granules of 16 channels [16 hi | 16 lo] of x * 2^4 -- the operand rows of the wgmma layers, so a
+# layer that reads one skips the conversion of its input.  Same bytes as the fp32 tensor; values keep about 22 significant bits.
+SPLIT_GRANULE = 16
+LAYOUT_NCDHW, LAYOUT_NDHWC, LAYOUT_SPLIT = 0, 1, 2
+
+
+def is_split(t):
+    """True for a split NDHWC activation (fp16, channels last, 2C entries per voxel)."""
+    return t.dtype == torch.float16 and t.dim() == 5
+
+
+def to_split(x):
+    """(B,C,D,H,W) fp32 -> split NDHWC (B,D,H,W,2C) fp16, C a multiple of 16.  Values outside +-4094 saturate and raise
+    tc_overflow_count."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 5
+    b, c, d, h, w = x.shape
+    assert c % SPLIT_GRANULE == 0, "split activations need a multiple of %d channels" % SPLIT_GRANULE
+    y = torch.empty((b, d, h, w, 2 * c), dtype=torch.float16, device=x.device)
+    _call("osb_ncdhw_to_split", x.data_ptr(), y.data_ptr(), b, c, d, h, w, _stream(y))
+    return y
+
+
+def from_split(x_split):
+    """split (B,D,H,W,2C) fp16 -> (B,D,H,W,C) fp32 channels-last, each value (hi + lo) / 16 as the kernels decode it.  For tests
+    and inspection: the layers read split tensors directly."""
+    assert is_split(x_split) and x_split.shape[4] % (2 * SPLIT_GRANULE) == 0
+    g = x_split.shape[4] // (2 * SPLIT_GRANULE)
+    v = x_split.view(*x_split.shape[:4], g, 2, SPLIT_GRANULE).float()
+    return ((v[..., 0, :] + v[..., 1, :]) * (1.0 / 16)).reshape(*x_split.shape[:4], g * SPLIT_GRANULE).contiguous()
+
+
 def conv3d_k3_tc(x_ndhwc, w_split, scale=None, shift=None, residual=None, act=ACT_NONE, out_ndhwc=True, res_ndhwc=True,
-                 in_ncdhw=False, gate=None):
+                 in_ncdhw=False, gate=None, out_split=False):
     """3x3x3 stride-1 conv + folded BN + residual + activation on the tensor cores.  x_ndhwc: (B,D,H,W,Cin), or the NCDHW
-    tensor (B,Cin,D,H,W) with in_ncdhw=True (W = 128 layers only: the cost volume goes in as the volume kernel wrote it)."""
-    assert x_ndhwc.is_cuda and x_ndhwc.dtype == torch.float32 and x_ndhwc.is_contiguous() and x_ndhwc.dim() == 5
+    tensor (B,Cin,D,H,W) with in_ncdhw=True (W = 128 layers only: the cost volume goes in as the volume kernel wrote it).
+    W = 128 layers also take x and a channels-last residual as split activations (to_split), and out_split=True returns y as one;
+    a split residual enters as (hi + lo) / 16."""
+    assert x_ndhwc.is_cuda and x_ndhwc.dtype in (torch.float32, torch.float16) and x_ndhwc.is_contiguous() and x_ndhwc.dim() == 5
+    in_split = is_split(x_ndhwc)
+    assert not (in_split and in_ncdhw)
     if in_ncdhw:
         b, cin, d, h, w = x_ndhwc.shape
     else:
         b, d, h, w, cin = x_ndhwc.shape
+        if in_split:
+            cin = w_split.data.shape[1] * w_split.kc
+            if x_ndhwc.shape[4] != 2 * cin:
+                raise ValueError("conv3d_k3_tc: an fp16 input is read as split activations (ops.to_split), 2 * Cin = %d entries per "
+                                 "voxel for this weight; got %d" % (2 * cin, x_ndhwc.shape[4]))
     cout = w_split.cout_real
     kc = conv3d_tc_kc(cin, cout, w)
     assert kc
     wptr, scale = _tc_args(w_split, cin, kc, scale)
     if shift is not None and shift.numel() < w_split.cout:               # zero-padded head
         shift = torch.cat((shift.float(), shift.new_zeros(w_split.cout - shift.numel()).float()))
+    res_split = residual is not None and is_split(residual)
+    if residual is not None:
+        want = (b, d, h, w, 2 * cout if res_split else cout) if res_ndhwc else (b, cout, d, h, w)
+        assert tuple(residual.shape) == want and residual.is_contiguous() and (res_split or residual.dtype == torch.float32)
+    if in_split or out_split or res_split:
+        assert gate is None and (out_ndhwc or not out_split)
+        shape = (b, d, h, w, 2 * cout if out_split else cout) if out_ndhwc else (b, cout, d, h, w)
+        y = torch.empty(shape, dtype=torch.float16 if out_split else torch.float32, device=x_ndhwc.device)
+        layout = lambda split, ndhwc: LAYOUT_SPLIT if split else (LAYOUT_NDHWC if ndhwc else LAYOUT_NCDHW)
+        # profiled as the fp32 entry point reading the same input layout would be: the same kernel and the same layers
+        _call("osb_conv3d_k3_tc_split_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), y.data_ptr(),
+              b, cin, cout, d, h, w, act, layout(in_split, not in_ncdhw), layout(out_split, out_ndhwc), layout(res_split, res_ndhwc),
+              _stream(y), profile_as="osb_conv3d_k3_tc_ncdhw_fwd" if in_ncdhw else "osb_conv3d_k3_tc_fwd")
+        return y
     shape = (b, d, h, w, cout) if out_ndhwc else (b, cout, d, h, w)
     y = torch.empty(shape, dtype=torch.float32, device=x_ndhwc.device)
-    if residual is not None:
-        want = (b, d, h, w, cout) if res_ndhwc else (b, cout, d, h, w)
-        assert tuple(residual.shape) == want and residual.is_contiguous()
     assert not in_ncdhw or kc == 32
     if gate is not None:                                                     # FeatureAtt: (B,H,W,Cout) multiplier after the activation
         assert kc == 16 and out_ndhwc and res_ndhwc and not in_ncdhw

@@ -1,6 +1,8 @@
 #!/usr/bin/env python
 """Run ONE aggregation layer at its bench shape (channels-last in/out) a few times: the target of ncu captures and of quick
-per-layer timings.  usage: layer_prof.py <stem|conv2|conv4|conv1s2|conv3s2|conv5|conv6> [batch] [iters]"""
+per-layer timings.  usage: layer_prof.py <stem|conv2|conv4|conv1s2|conv3s2|conv5|conv6> [batch] [iters]
+OSB_LP_SPLIT=1: the W = 128 stride-1 layers (stem, stem64, stem64n, head) read and write split activations (ops.to_split), as
+GwcNet's stem chain does; the input is converted once, outside the timed calls."""
 import json
 import os
 import sys
@@ -32,6 +34,7 @@ def main():
     x = torch.randn(B, d, h, w, cin, device=dev, generator=g)
     sc, sh = torch.rand(cout, device=dev, generator=g) + 0.5, torch.randn(cout, device=dev, generator=g) * 0.1
     flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=dev)
+    split = bool(os.environ.get("OSB_LP_SPLIT")) and kind in ("s1", "s1n", "s1h") and w == 128
     if kind == "2d":
         B = 2 * B
         x = torch.randn(B, h, w, cin, device=dev, generator=g)
@@ -56,20 +59,22 @@ def main():
         wgt = torch.randn(cout, cin, 3, 3, 3, device=dev, generator=g) * 0.05
         wp = ops.pack_tc_weight(wgt, ops.conv3d_tc_kc(cin, cout, w))
         xn = x.permute(0, 4, 1, 2, 3).contiguous()
-        fn = lambda: ops.conv3d_k3_tc(xn, wp, sc, sh, None, ops.ACT_RELU, out_ndhwc=True, in_ncdhw=True)  # noqa: E731
+        fn = lambda: ops.conv3d_k3_tc(xn, wp, sc, sh, None, ops.ACT_RELU, out_ndhwc=True, in_ncdhw=True, out_split=split)  # noqa: E731
         macs = B * d * h * w * 27 * cin * cout
     elif kind == "s1h":                                        # 32 -> 1 classifier head on the narrow variant
         wgt = torch.randn(cout, cin, 3, 3, 3, device=dev, generator=g) * 0.05
         wp = ops.pack_tc_weight(wgt, 32, pad_cout_to=16)
+        x = ops.to_split(x.permute(0, 4, 1, 2, 3).contiguous()) if split else x
         fn = lambda: ops.conv3d_k3_tc(x, wp, None, None, None, ops.ACT_NONE, out_ndhwc=False, res_ndhwc=False)  # noqa: E731
         macs = B * d * h * w * 27 * cin * cout
     else:
         wgt = torch.randn(cout, cin, 3, 3, 3, device=dev, generator=g) * 0.05
         wp = ops.pack_tc_weight(wgt, ops.conv3d_tc_kc(cin, cout, w))
-        fn = lambda: ops.conv3d_k3_tc(x, wp, sc, sh, None, ops.ACT_RELU, out_ndhwc=True)  # noqa: E731
+        x = ops.to_split(x.permute(0, 4, 1, 2, 3).contiguous()) if split else x
+        fn = lambda: ops.conv3d_k3_tc(x, wp, sc, sh, None, ops.ACT_RELU, out_ndhwc=True, out_split=split)  # noqa: E731
         macs = B * d * h * w * 27 * cin * cout
     ms, _ = timeit(fn, iters, flush)
-    print(json.dumps({"layer": name, "ms": round(ms, 4), "useful_TF": round(2 * macs / ms / 1e9, 1)}), flush=True)
+    print(json.dumps({"layer": name, "split": split, "ms": round(ms, 4), "useful_TF": round(2 * macs / ms / 1e9, 1)}), flush=True)
 
 
 if __name__ == "__main__":
