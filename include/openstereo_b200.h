@@ -365,6 +365,12 @@ int osb_avgpool_pairs_fwd(const float* x, float* y, long long outer, int n, long
 int osb_geo_lookup_fwd(const float* geo0, const float* geo1, const float* geo2, const float* geo3, const float* corr0,
                        const float* corr1, const float* corr2, const float* corr3, const float* disp, const float* coords,
                        float* out, int B, int C, int D, int H, int W, int W2, int num_levels, int radius, osb_stream_t stream);
+/* Geo_Encoding_Volume.__call__ (igev_rt/geometry.py:18-33, IGEV-RT): the same lookup of the geometry volume alone, no correlation
+ * row.  Per level i < num_levels, 2*radius+1 zero-padded bilinear taps of geo_i (B, C, D>>i, H, W) at d = dx + disp/2^i
+ *   -> channels [i*C*T + c*T + k],   T = 2*radius+1
+ * disp (B,1,H,W), out (B, num_levels*C*T, H, W).  Unused level pointers are NULL. */
+int osb_geo_volume_lookup_fwd(const float* geo0, const float* geo1, const float* geo2, const float* geo3, const float* disp,
+                              float* out, int B, int C, int D, int H, int W, int num_levels, int radius, osb_stream_t stream);
 /* context_upsample (stereobase/igev_blocks.py:51-63, igev/submodule.py:253-265): disp_low (B,1,h,w), up_weights
  * (B,9,scale*h,scale*w) -> out (B, scale*h, scale*w) = sum over the 3x3 low-resolution neighbourhood (zero padded). */
 int osb_context_upsample_fwd(const float* disp_low, const float* up_weights, float* out, int B, int h, int w, int scale,

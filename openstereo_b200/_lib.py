@@ -50,6 +50,7 @@ SIGNATURES = {
     "osb_conv3d_k3_c1_ndhwc_fwd": [_f32p] * 5 + [_i] * 5 + [_s],
     "osb_avgpool_pairs_fwd": [_f32p, _f32p, ctypes.c_longlong, _i, ctypes.c_longlong, _s],
     "osb_geo_lookup_fwd": [_f32p] * 11 + [_i] * 8 + [_s],
+    "osb_geo_volume_lookup_fwd": [_f32p] * 6 + [_i] * 7 + [_s],
     "osb_context_upsample_fwd": [_f32p] * 3 + [_i] * 4 + [_s],
     "osb_conv2d_tc_kc": [_i] * 4,
     "osb_conv2d_k3_tc_fwd": [_f32p] * 6 + [_i] * 9 + [_s],

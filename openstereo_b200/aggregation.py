@@ -11,7 +11,8 @@ Graphs restated (file:line of the reference forward each engine replaces):
   GwcAggregation        gwcnet/gwcnet_disp_processor.py:83-91,128-140 + gwcnet/hourglass.py:46-56
   CascadeAggregation    casnet/cas_psm.py:233-279 (CostAggregation, eval) + cas_psm.py:33-43
   PSMAggregation        psmnet/psmnet_cost_processor.py:181-221,108-132 + psmnet_disp_processor.py:107-118
-  StereoBaseAggregation stereobase/hourglass.py:79-104 + stereobase_gru.py:161-164
+  StereoBaseAggregation stereobase/hourglass.py:79-104 + stereobase_gru.py:161-164, and IGEV-RT's hourglass(8)
+                        igev_rt/igev_rt_stereo.py:21-87 (the same graph built from IGEV's BasicConv / FeatureAtt)
   LightStereoAggregation lightstereo/aggregation.py:42-60 (Aggregation.forward), :94-101 (MobileV2Residual), :119-134 (AttentionModule)
   CoExAggregation       coex/coex_cost_processor.py:196-237 (Aggregation.forward), :68-80 (channelAtt)
   MSNet3DAggregation    msnet/MSNet3D.py:118-161 (eval forward after the volume), :10-46 (hourglass3D), submodule.py:136-173
@@ -418,18 +419,35 @@ class PSMAggregation(_Engine):
 
 # -------------------------------------------------------------------------------------------------- StereoBase
 class _FeatureAtt:
+    """FeatureAtt: StereoBase's (feat_att[0] a BasicConv2d with `.block`) or IGEV's (feat_att[0] an IGEV BasicConv), then a biased
+    1x1 Conv2d."""
+
     def __init__(self, m):
-        blk = m.feat_att[0].block
-        self.a = _Packed(blk[0], blk[1])
+        first = m.feat_att[0]
+        if hasattr(first, "block"):
+            blk = first.block
+            self.a = _Packed(blk[0], blk[1])
+            self.act = ACT_LEAKY if any(isinstance(l, torch.nn.LeakyReLU) for l in blk) else ACT_NONE
+        else:
+            self.a, self.act = _igev_basic_conv(first)
         self.b = _Packed(m.feat_att[1])
-        self.act = ACT_LEAKY if any(isinstance(l, torch.nn.LeakyReLU) for l in blk) else ACT_NONE
 
     def __call__(self, feat):
-        hidden = ops.conv3d_1x1(feat, self.a.w, self.a.scale, self.a.shift, act=ACT_LEAKY)
+        hidden = ops.conv3d_1x1(feat, self.a.w, self.a.scale, self.a.shift, act=self.act)
         return ops.conv3d_1x1(hidden, self.b.w, self.b.scale, self.b.shift, sigmoid_out=True)   # (B, cv_chan, H, W)
 
 
+def _igev_basic_conv(m):
+    """IGEV's BasicConv (igev/submodule.py, igev_rt/submodule.py): `.conv`, then `.bn` only when `use_bn` (the module owns a `bn`
+    even with bn=False), then nn.LeakyReLU() -- slope 0.01, created inside forward -- only when `relu` -> (_Packed, act)."""
+    return _Packed(m.conv, m.bn if m.use_bn else None), ACT_LEAKY if m.relu else ACT_NONE
+
+
 def _block(m):
+    """(_Packed, act) of one hourglass layer: StereoBase's BasicConv3d / BasicDeconv3d (`.block` = conv, optional BN, optional
+    LeakyReLU) or IGEV's BasicConv."""
+    if not hasattr(m, "block"):
+        return _igev_basic_conv(m)
     layers = list(m.block)
     bn = layers[1] if len(layers) > 1 and isinstance(layers[1], torch.nn.BatchNorm3d) else None
     act = ACT_LEAKY if any(isinstance(l, torch.nn.LeakyReLU) for l in layers) else ACT_NONE
@@ -437,7 +455,8 @@ def _block(m):
 
 
 class StereoBaseAggregation(_Engine):
-    """Hourglass(volume_channel, backbone_channels) with FeatureAtt gates: (B,C,D',H',W') + 2D features -> same shape."""
+    """Hourglass(volume_channel, backbone_channels) with FeatureAtt gates: (B,C,D',H',W') + 2D features -> same shape.  Also runs
+    IGEV-RT's hourglass(8): its 8/16/32/48-channel plan fails tc_route_ok, so every layer takes the fp32 CUDA-core kernels."""
 
     def _pack(self):
         m = self.module
@@ -636,7 +655,8 @@ class StereoBaseCostHead(_Engine):
     def _pack(self):
         self.layer = _Packed(self.module)
 
-    def __call__(self, geo, maxdisp_lowres):
+    def logits(self, geo):
+        """classifier(geo) alone: (B,C,D',H',W') -> (B,1,D',H',W') fp32 logits (IGEV-RT's softmax and regression follow it)."""
         geo = self._check(geo)
         self._ensure(geo.device)
         lay = self.layer
@@ -656,7 +676,10 @@ class StereoBaseCostHead(_Engine):
                 mon.poll()
         else:
             logits = _conv(lay, geo)                            # (B,1,D',H',W')
-        return ops.softargmin(logits.squeeze(1), maxdisp_lowres, keepdim=True)
+        return logits
+
+    def __call__(self, geo, maxdisp_lowres):
+        return ops.softargmin(self.logits(geo).squeeze(1), maxdisp_lowres, keepdim=True)
 
 
 # -------------------------------------------------------------------------------------------------------- CoEx

@@ -3,6 +3,7 @@
 //   * geo_lookup_kernel     Combined_Geo_Encoding_Volume.__call__  stereo/modeling/models/igev/geometry.py:32-57 ==
 //                           CombinedGeoEncodingVolume.__call__     stereo/modeling/models/stereobase/gru_blocks.py:195-220
 //                           (bilinear_sampler = grid_sample(align_corners=True, zeros) igev/utils.py:61-79)
+//                           and, with no correlation rows, Geo_Encoding_Volume.__call__ stereo/modeling/models/igev_rt/geometry.py:18-33
 //   * avgpool_pairs_kernel  the F.avg_pool2d(.., [1,2], stride=[1,2]) pyramid of geometry.py:24-30
 //   * context_upsample_kernel  context_upsample  stereo/modeling/models/stereobase/igev_blocks.py:51-63
 // The reference materialises, per GRU iteration and level, a (B*H*W, C, 1, D) permuted copy of the volume (once), two grid
@@ -20,10 +21,10 @@ constexpr int GEO_MAX_LEVELS = 4;
 
 struct GeoParams {
   const float* geo[GEO_MAX_LEVELS];    // level i: (B, C, D >> i, H, W)
-  const float* corr[GEO_MAX_LEVELS];   // level i: (B, H, W, W2 >> i)
+  const float* corr[GEO_MAX_LEVELS];   // level i: (B, H, W, W2 >> i); all NULL = geometry-only lookup (no correlation row)
   const float* disp;                   // (B, 1, H, W)
-  const float* coords;                 // (B, H, W) left-image x coordinate of every pixel
-  float* out;                          // (B, L * (C + 1) * (2r + 1), H, W)
+  const float* coords;                 // (B, H, W) left-image x coordinate of every pixel (unused when geometry-only)
+  float* out;                          // (B, L * (C + 1) * (2r + 1), H, W), geometry-only (B, L * C * (2r + 1), H, W)
   int B, C, D, H, W, W2, levels, radius;
 };
 
@@ -49,12 +50,13 @@ __device__ __forceinline__ float lerp_row(const float* __restrict__ row, size_t 
 // One thread = one pixel x one "row" (a geometry channel of a level, or a level's correlation row): 2r+1 taps that, up to
 // coordinate rounding, slide over one window of 2r+2 consecutive samples.  The window is loaded once (zero padded) and each
 // tap picks its two samples from registers; a tap whose floor() does not land on window slot k (possible only when the
-// coordinate round trip moves it across an integer) falls back to a direct read.  RADIUS = 0 is the generic path.
+// coordinate round trip moves it across an integer) falls back to a direct read.  RADIUS = 0 is the generic path.  With
+// corr[0] == NULL (IGEV-RT's Geo_Encoding_Volume) a level has only its C geometry rows: a runtime mode, not an instantiation.
 template <int RADIUS>
 __global__ void __launch_bounds__(128) geo_lookup_kernel(const GeoParams p) {
   const int w = blockIdx.x * 128 + threadIdx.x;
   const int h = blockIdx.y;
-  const int rows = p.C + 1;
+  const int rows = p.corr[0] != nullptr ? p.C + 1 : p.C;
   const int b = blockIdx.z / (p.levels * rows), lr = blockIdx.z % (p.levels * rows);
   const int lvl = lr / rows, c = lr % rows;
   if (w >= p.W) return;
@@ -76,7 +78,7 @@ __global__ void __launch_bounds__(128) geo_lookup_kernel(const GeoParams p) {
     len = p.D >> lvl;
     row = geo + ((size_t)b * p.C + c) * len * hw + pix;
     stride = hw;
-    base = dq;
+    base = dq;                                         // geometry.py:22-26 adds dx + disp / 2^i: the same fp32 sum
   } else {
     len = p.W2 >> lvl;
     row = corr + ((size_t)b * hw + pix) * len;
@@ -200,6 +202,32 @@ int osb_geo_lookup_fwd(const float* geo0, const float* geo1, const float* geo2, 
   OSB_REQUIRE((long long)B * num_levels * (C + 1) <= 65535, "geo_lookup: B * levels * (C + 1) must fit a grid dimension");
   dim3 grid((W + 127) / 128, H, B * num_levels * (C + 1));
   if (radius == 4) geo_lookup_kernel<4><<<grid, 128, 0, (cudaStream_t)stream>>>(p);      // IGEV / StereoBase default (corr_radius 4)
+  else geo_lookup_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(p);
+  count_launch();
+  return check_launch("geo_lookup_kernel");
+}
+
+int osb_geo_volume_lookup_fwd(const float* geo0, const float* geo1, const float* geo2, const float* geo3, const float* disp,
+                              float* out, int B, int C, int D, int H, int W, int num_levels, int radius, osb_stream_t stream) {
+  using namespace osb;
+  OSB_REQUIRE(disp && out, "geo_volume_lookup: null pointer");
+  OSB_REQUIRE(B > 0 && C > 0 && D > 0 && H > 0 && W > 0, "geo_volume_lookup: empty shape");
+  OSB_REQUIRE(num_levels >= 1 && num_levels <= GEO_MAX_LEVELS, "geo_volume_lookup: num_levels %d outside 1..%d", num_levels,
+              GEO_MAX_LEVELS);
+  OSB_REQUIRE(radius >= 0 && radius <= 16, "geo_volume_lookup: radius %d outside 0..16", radius);
+  OSB_REQUIRE((D >> (num_levels - 1)) >= 2, "geo_volume_lookup: pyramid level shorter than 2 samples");
+  OSB_REQUIRE(H <= 65535 && B <= 65535, "geo_volume_lookup: H and B must fit a grid dimension");
+  GeoParams p{};                                       // p.corr stays NULL: the kernel's geometry-only mode
+  const float* g[GEO_MAX_LEVELS] = {geo0, geo1, geo2, geo3};
+  for (int i = 0; i < num_levels; ++i) {
+    OSB_REQUIRE(g[i], "geo_volume_lookup: pyramid level %d is null", i);
+    p.geo[i] = g[i];
+  }
+  p.disp = disp, p.coords = nullptr, p.out = out;
+  p.B = B, p.C = C, p.D = D, p.H = H, p.W = W, p.W2 = 0, p.levels = num_levels, p.radius = radius;
+  OSB_REQUIRE((long long)B * num_levels * C <= 65535, "geo_volume_lookup: B * levels * C must fit a grid dimension");
+  dim3 grid((W + 127) / 128, H, B * num_levels * C);
+  if (radius == 4) geo_lookup_kernel<4><<<grid, 128, 0, (cudaStream_t)stream>>>(p);      // IGEV-RT default (CORR_RADIUS 4)
   else geo_lookup_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(p);
   count_launch();
   return check_launch("geo_lookup_kernel");

@@ -1048,6 +1048,24 @@ def geo_lookup(geo_levels, corr_levels, disp, coords, radius):
     return out
 
 
+def geo_volume_lookup(geo_levels, disp, radius):
+    """One lookup of IGEV-RT's geometry-only encoding volume (igev_rt/geometry.py:18-33): geo_levels[i] (B,C,D>>i,H,W),
+    disp (B,1,H,W) -> (B, L*C*(2r+1), H, W), level-major, then channel, then tap."""
+    levels = len(geo_levels)
+    assert 1 <= levels <= 4
+    b, c, d, h, w = geo_levels[0].shape
+    for i in range(levels):
+        g = geo_levels[i]
+        assert g.is_cuda and g.dtype == torch.float32 and g.is_contiguous() and tuple(g.shape) == (b, c, d >> i, h, w)
+    disp = disp.contiguous().float()
+    assert tuple(disp.shape) == (b, 1, h, w)
+    _same_device(geo_levels[0], disp)
+    out = torch.empty((b, levels * c * (2 * radius + 1), h, w), dtype=torch.float32, device=disp.device)
+    gp = [geo_levels[i].data_ptr() if i < levels else None for i in range(4)]
+    _call("osb_geo_volume_lookup_fwd", *gp, disp.data_ptr(), out.data_ptr(), b, c, d, h, w, levels, radius, _stream(out))
+    return out
+
+
 def context_upsample(disp_low, up_weights, scale_factor=4):
     """stereobase/igev_blocks.py:51-63: disp_low (B,1,h,w), up_weights (B,9,s*h,s*w) -> (B, s*h, s*w)."""
     assert disp_low.is_cuda and disp_low.dim() == 4 and disp_low.shape[1] == 1

@@ -1,5 +1,5 @@
-"""patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / CoEx /
-MSNet3D, and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
+"""patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / IGEV-RT /
+CoEx / MSNet3D, and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
 hot path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each
@@ -10,6 +10,7 @@ needs its own rebinding:
 * PSMNet      ``cat_fms`` captured by functools.partial at construction (psmnet_cost_processor.py:227-232),
               aggregator + FasterSoftArgmin modules                          -> ``CostProcessor.forward`` / ``FasterSoftArgmin.forward``
 * LightStereo / IGEVStereo  like StereoBase: names imported into lightstereo.py:4-6 / igev_stereo.py:1-3 (``from .submodule import *``)
+* IGEV-RT     like IGEVStereo (igev_rt_stereo.py:1-6), plus per-instance ``cost_agg`` / ``classifier`` forward overrides
 * CasStereo   ``get_cv`` (GetCostVolume) and ``cost_agg[i]`` (CostAggregation) modules  -> per-instance ``forward`` overrides
 * CoEx        ``CostProcessor`` / ``DispProcessor`` / ``DispProcessor.regression`` modules -> per-instance ``forward`` overrides
 * MSNet3D     one monolithic ``forward`` (MSNet3D.py:110-161), no processor modules   -> per-instance ``model.forward`` override that
@@ -33,8 +34,8 @@ import types
 import torch
 
 from . import ops
-from .aggregation import CascadeAggregation, GwcAggregation, PSMAggregation, StereoBaseAggregation
-from .geo import CombinedGeoEncodingVolume
+from .aggregation import CascadeAggregation, GwcAggregation, PSMAggregation, StereoBaseAggregation, StereoBaseCostHead
+from .geo import CombinedGeoEncodingVolume, GeoEncodingVolume
 
 
 def _tensors(args):
@@ -334,6 +335,59 @@ def _patch_igev(model, strict, backbone=True):
     return model
 
 
+def _patch_igev_rt(model, strict, backbone=True):
+    """IGEV-RT (igev_rt/igev_rt_stereo.py:146-206, class IGEVRTtereo): the gwc volume, the hourglass(8) (``cost_agg.forward``), the
+    classifier Conv3d(8 -> 1) (``classifier.forward``, which returns logits: the reference's own softmax follows), the strided
+    regression of the initial disparity, the per-GRU-iteration lookup of the geometry-only encoding volume and the convex
+    up-sampling.  The feature nets, hnet / cnet and the ConvGRU update block stay the reference's code; `backbone` has no effect.
+    Under autocast (the AMP YAML) fp16 tensors arrive: every call computes in fp32 and returns the caller's dtype."""
+    g = type(model).forward.__globals__
+    orig = {n: g[n] for n in ("build_gwc_volume", "disparity_regression", "Geo_Encoding_Volume", "context_upsample")}
+
+    def gwc(ref, tgt, maxdisp, groups):
+        if _accelerable(model, ref, tgt):
+            return ops.build_gwc_volume(ref, tgt, maxdisp, groups)
+        return orig["build_gwc_volume"](ref, tgt, maxdisp, groups) if not strict else _refuse("build_gwc_volume")
+
+    def regression(prob, maxdisp, interval):
+        if _accelerable(model, prob):
+            return ops.disparity_regression_interval(prob, maxdisp, interval)
+        return orig["disparity_regression"](prob, maxdisp, interval) if not strict else _refuse("disparity_regression")
+
+    def geo_factory(geo_volume, num_levels=2, radius=4):
+        fast = _accelerable(model, geo_volume)
+        if not fast and strict:
+            _refuse("Geo_Encoding_Volume")
+        cls = GeoEncodingVolume if fast else orig["Geo_Encoding_Volume"]
+        return cls(geo_volume, num_levels=num_levels, radius=radius)
+
+    def upsample(disp_low, up_weights):                               # IGEV-RT's version keeps dim 1: (B, 1, 4h, 4w)
+        if _accelerable(model, disp_low, up_weights):
+            return ops.context_upsample(disp_low, up_weights, 4).unsqueeze(1).to(disp_low.dtype)
+        return orig["context_upsample"](disp_low, up_weights) if not strict else _refuse("context_upsample")
+
+    _rebind_methods(model, {"build_gwc_volume": gwc, "disparity_regression": regression, "Geo_Encoding_Volume": geo_factory,
+                            "context_upsample": upsample})
+
+    hg, cls_mod = model.cost_agg, model.classifier
+    hg_orig, cls_orig = hg.forward, cls_mod.forward
+    agg, head = StereoBaseAggregation(hg), StereoBaseCostHead(cls_mod)
+
+    def hg_forward(self, x, features):
+        if not _accelerable(self, x, features):
+            return hg_orig(x, features) if not strict else _refuse("IGEV-RT hourglass")
+        return agg(x, features).to(x.dtype)
+
+    def cls_forward(self, x):
+        if not _accelerable(self, x):
+            return cls_orig(x) if not strict else _refuse("IGEV-RT classifier")
+        return head.logits(x).to(x.dtype)
+
+    hg.forward = types.MethodType(hg_forward, hg)
+    cls_mod.forward = types.MethodType(cls_forward, cls_mod)
+    return model
+
+
 def _patch_cascade(model, strict, backbone=True):
     """CasStereo (casnet/cas_psm.py PSMNet = CasPSMNet, casnet/cas_gwc.py GwcNet = CasGwcNet): every stage's warped cost volume
     (``get_cv.forward``) and every stage's aggregation + hypothesis-weighted soft-argmin (``cost_agg[i].forward``).  The FPN
@@ -464,7 +518,7 @@ def _patch_msnet3d(model, strict, backbone=True):
 _CASCADE_MODULES = {("casnet", "cas_psm"): "PSMNet", ("casnet", "cas_gwc"): "GwcNet"}
 
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
-             "IGEVStereo": _patch_igev, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
+             "IGEVStereo": _patch_igev, "IGEVRTtereo": _patch_igev_rt, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
 
 
 def patch(model, strict=True, backbone=True):

@@ -19,6 +19,9 @@
   c8  MSNet3D cfgs/msnet/msnet3d_sceneflow.yaml (the reference's class + patch()), batch 8 @256x512 and @512x960: whole-model
       forward next to the unpatched model on the same GPU (timed alternately), per-stage volume / aggregation / tail times, and
       per MobileV2_Residual_3D config the fused block's time, TFLOP/s and GB/s  (python tools/bench_configs.py --only c8)
+  c9  IGEV-RT cfgs/igev_rt (the reference's class + patch()), batch 8 @256x512 and @544x960: the uniform YAML's model patched and
+      unpatched, timed alternately, the unpatched AMP YAML's model for context, per-stage times (volume, cost_agg, classifier, the 8
+      lookups, everything else) and the lookups' GB/s  (python tools/bench_configs.py --only c9)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -459,6 +462,55 @@ def c8(iters, B=8):
         torch.cuda.empty_cache()
 
 
+def c9(iters, B=8):
+    """IGEV-RT (the reference's own class, cfgs/igev_rt YAMLs unchanged, seeded weights with the classifier sharpened) at 256x512 and
+    at SceneFlow's 540x960 after DivisiblePad 32 (544x960), batch 8.  The uniform (fp32) YAML's model with and without patch() is
+    timed alternately in one process, with the unpatched AMP YAML's model (fp16 autocast) in the same rotation for context.  Stage
+    times of the patched forward come from CUDA events around ops.build_gwc_volume, cost_agg, classifier and the lookups; the rest
+    of the step (feature nets, hnet / cnet, the ConvGRU, regression, up-sampling) is "other".  Lookup GB/s counts the algorithmic
+    bytes: the output written, 2r+2 samples per (pixel, channel, level) read once and the disparity read once per channel row."""
+    from oracle import igev_rt as oigrt
+    from openstereo_b200.patch import patch
+    for (h, w) in ((256, 512), (544, 960)):
+        ref = oigrt.igev_rt(oigrt.UNIFORM_YAML).to(DEV)
+        amp = oigrt.igev_rt(oigrt.AMP_YAML).to(DEV)
+        pm = patch(oigrt.igev_rt(oigrt.UNIFORM_YAML).to(DEV))
+        cfg = pm.args
+        gen = torch.Generator().manual_seed(29)
+        x = {"left": rnd(gen, B, 3, h, w), "right": rnd(gen, B, 3, h, w)}
+        with torch.no_grad():
+            ms_ref, ms_amp, ms = [], [], []
+            for _ in range(3):                                          # alternate: the three share the GPU's state
+                t, want = timeit(lambda: ref(dict(x))["disp_pred"], max(1, iters // 2), warm=1)
+                ms_ref.append(t)
+                t, got_amp = timeit(lambda: amp(dict(x))["disp_pred"], max(1, iters // 2), warm=1)
+                ms_amp.append(t)
+                t, got = timeit(lambda: pm(dict(x))["disp_pred"], iters, warm=2)
+                ms.append(t)
+            ms_ref, ms_amp, ms = sorted(ms_ref)[1], sorted(ms_amp)[1], sorted(ms)[1]
+            stages = _stage_times(lambda: pm(dict(x)), {"cost_agg": pm.cost_agg, "classifier": pm.classifier,
+                                                        "lookups": geo.GeoEncodingVolume}, volume_fn="build_gwc_volume")
+        stages["other"] = round(ms - sum(stages.values()), 3)
+        c, d4, h4, w4 = 8, cfg.MAX_DISP // 4, h // 4, w // 4
+        levels, r = cfg.CORR_LEVELS, cfg.CORR_RADIUS
+        rows = B * levels * c * h4 * w4                                 # (pixel, channel, level) rows of one lookup
+        lookup_bytes = 4 * (rows * (2 * r + 1) + rows * (2 * r + 2) + rows)
+        n_lookups = cfg.VALID_ITERS
+        emit(config="c9 IGEV-RT cfgs/igev_rt, B=%d @%dx%d (reference class + patch())" % (B, h, w),
+             gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+             ms_per_step=round(ms, 3), pairs_per_s=round(B * 1e3 / ms, 2),
+             reference_uniform_fp32_ms=round(ms_ref, 2), reference_uniform_pairs_per_s=round(B * 1e3 / ms_ref, 2),
+             reference_amp_fp16_ms=round(ms_amp, 2), reference_amp_pairs_per_s=round(B * 1e3 / ms_amp, 2),
+             speedup_vs_reference_uniform=round(ms_ref / ms, 3), speedup_vs_reference_amp=round(ms_amp / ms, 3),
+             stage_ms=stages, lookups=n_lookups,
+             lookup_gb_per_s=round(n_lookups * lookup_bytes / (stages["lookups"] * 1e-3) / 1e9, 1) if stages.get("lookups") else None,
+             epe_vs_reference_uniform_px=float("%.3e" % (got - want).abs().mean().item()),
+             epe_amp_reference_vs_uniform_px=float("%.3e" % (got_amp - want).abs().mean().item()),
+             disparity_std_px=round(want.std().item(), 2))
+        del ref, amp, pm
+        torch.cuda.empty_cache()
+
+
 def _stage_times(run, targets, volume_fn=None):
     """One run of `run` with CUDA events around the forward of each target (a module, or a class whose __call__ is wrapped) and,
     with volume_fn, around ops.<volume_fn>: {stage: ms}."""
@@ -515,7 +567,7 @@ if __name__ == "__main__":
     a = ap.parse_args()
     for name in a.only.split(","):
         try:
-            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8}[name](a.iters)
+            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:

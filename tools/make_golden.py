@@ -27,6 +27,7 @@ from oracle import cascade as ocas                              # noqa: E402
 from oracle import coex as ocx                                  # noqa: E402
 from oracle import cost_volume as ocv                           # noqa: E402
 from oracle import geo_lookup as ogeo                           # noqa: E402
+from oracle import igev_rt as oigrt                             # noqa: E402
 from oracle import lightstereo as olight                        # noqa: E402
 from oracle import models as omodels                            # noqa: E402
 from oracle import msnet as oms                                 # noqa: E402
@@ -453,6 +454,27 @@ def msnet():
              disp_std=disp.std())
 
 
+# (B, C, D, H, W, levels, radius) of tests/golden/geo_volume_lookup.npz, case i stored under keys suffixed with i
+GEO_VOLUME_CASES = ((2, 8, 48, 3, 10, 2, 4), (1, 3, 17, 2, 21, 1, 4), (1, 5, 24, 2, 9, 3, 4), (2, 4, 20, 3, 7, 3, 2))
+
+
+def igev_rt():
+    """IGEV-RT's geometry-only encoding volume (igev_rt/geometry.py): the reference class against the oracle, bit for bit.  The
+    disparities run from below -r to past D + r, so taps leave the row at both ends on every level."""
+    rgeo = oigrt.load_reference("stereo.modeling.models.igev_rt.geometry")
+    arrays = {}
+    for i, (b, c, d, h, w, levels, radius) in enumerate(GEO_VOLUME_CASES):
+        vol = rnd(140 + i, b, c, d, h, w)
+        disp = torch.rand(b, 1, h, w, generator=torch.Generator().manual_seed(150 + i)) * (d + 2 * radius + 8) - radius - 4
+        disp[0, 0, 0, :5] = torch.tensor([0.0, d - 1.0, 2.5, -radius - 1.5, d + radius + 1.5])
+        ref = rgeo.Geo_Encoding_Volume(vol, num_levels=levels, radius=radius)
+        out = ref(disp)
+        must_equal(out, oigrt.GeoEncodingVolume(vol, num_levels=levels, radius=radius)(disp), "geo_volume_lookup case %d" % i)
+        assert out.shape == (b, levels * c * (2 * radius + 1), h, w)
+        arrays.update({"volume%d" % i: vol, "disp%d" % i: disp, "levels%d" % i: levels, "radius%d" % i: radius, "out%d" % i: out})
+    save("geo_volume_lookup", cases=len(GEO_VOLUME_CASES), **arrays)
+
+
 class _Const(torch.nn.Module):
     def __init__(self, t):
         super().__init__()
@@ -462,7 +484,7 @@ class _Const(torch.nn.Module):
         return self.t
 
 
-SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade", "coex", "msnet"]
+SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade", "coex", "msnet", "igev_rt"]
 
 if __name__ == "__main__":
     if not shim.available():
