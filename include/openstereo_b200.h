@@ -213,7 +213,8 @@ int osb_conv3d_k3_tc_split_fwd(const float* x, const void* w_split, const float*
                                float* y, int B, int Cin, int Cout, int D, int H, int W, int act, int in_layout, int out_layout,
                                int res_layout, osb_stream_t stream);
 /* Stride-2 variant (the down-sampling convs of the hourglasses): x (B,D,H,W,Cin) channels-last with even D,H,W ->
- * y (B,Cout,D/2,H/2,W/2) or channels-last.  w_split like above but with the kw slices stored in the order (1,0,2)
+ * y (B,Cout,D/2,H/2,W/2) or channels-last.  D = 1 is a stride-2 3x3 Conv2d (the backbone's stage entry): one output plane from
+ * the kd = 1 taps.  w_split like above but with the kw slices stored in the order (1,0,2)
  * (ops.pack_tc_weight(..., kw_order=(1,0,2))), 16-channel K chunks.  Supported: W=128/Cout=64, W=64/Cout=64|128. */
 int osb_conv3d_s2_tc_supported(int Cin, int Cout, int D, int H, int W);
 int osb_conv3d_k3_s2_tc_fwd(const float* x_ndhwc, const void* w_split, const float* scale, const float* shift,

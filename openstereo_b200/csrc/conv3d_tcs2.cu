@@ -31,7 +31,8 @@ struct Tcs2Params {
   const float* shift;
   const float* residual;
   float* y;
-  int B, D, H, Cin;        // INPUT extent D x H x (2*WO); output is D/2 x H/2 x WO
+  int B, D, H, Cin;        // INPUT extent D x H x (2*WO); output is Do x H/2 x WO
+  int Do;                  // D/2, or 1 for D = 1 (a one-plane 2D conv: only the kd = 1 taps meet the input)
   int act;
   float kappa;       // expected round-towards-zero loss per accumulating MMA (tc_common.cuh)
   unsigned int* overflow;  // sticky fp16-range flag (tc_common.cuh)
@@ -157,7 +158,7 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
     const uint64_t dbase = (KC == 32) ? desc_sw128_base() : desc_sw64_base();
     constexpr uint32_t A_HALF = 64 * C::ROWB / 16;  // descriptor offset of operand rows 64..127
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
-    const int Do = p.D / 2, Ho = p.H / 2;
+    const int Do = p.Do, Ho = p.H / 2;
     const int q = warp & 3;                          // epilogue: this warp owns tile rows 32q .. 32q + 31
     const int m = q * 32 + lane;                     // operand row owned by this thread
     const int rr = m / W, wcol = m % W;              // image row inside the tile, image column
@@ -312,7 +313,7 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
     const int v0 = lane_voxel<KC>(lane), c = lane % CPR;   // permuted voxel order: conflict-free STS.64 (tc_common.cuh)
     float amax = 0.f;
     const int WI = 2 * Wp;                           // input width
-    const int Do = p.D / 2;
+    const int Do = p.Do;
     uint32_t ubase = 0;                              // global index of the current phase's first unit
     int first = lw;                                  // this warp's first local unit index in the current phase: (ubase + first) % NLW == lw
     auto fill = [&](const float* base, size_t rstride, size_t cstride, int h_first, int h_step, uint32_t u, int col0) {
@@ -377,7 +378,7 @@ __global__ void __launch_bounds__(Tcs2Cfg<COUT, KC, W, TILES, GW>::THREADS, 1) c
       for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
         const int g0 = (it % C::NP) * TC_WGS;        // first channel group of the pair
         const int ngr = min(TC_WGS, C::NG - g0);     // groups in the pair
-        const int od = (it / C::NP / (ctiles * p.hblocks)) % (p.D / 2);
+        const int od = (it / C::NP / (ctiles * p.hblocks)) % p.Do;
         for (int kd = 0; kd < 3; ++kd) {
           const int din = 2 * od + kd - 1;              // must enumerate the same phases as the consumers and the loaders
           if (din < 0 || din >= p.D) continue;
@@ -406,18 +407,19 @@ static int launch_tcs2(const TcArgs& a, cudaStream_t stream) {
   using C = Tcs2Cfg<COUT, KC, W, TILES, GW>;
   Tcs2Params p{};
   p.ystride = a.ystride;
+  p.Do = a.D == 1 ? 1 : a.D / 2;
   p.hblocks = (a.H / 2 + C::HBLK - 1) / C::HBLK;
   p.Wr = GW ? a.W / 2 : W;
   p.ctiles = GW ? (p.Wr + C::CSTEP - 1) / C::CSTEP : 1;
   static const std::string variant = tc_variant_name("tcs2<%d,%d,%d,%d,%d>", COUT, KC, W, TILES, (int)GW);
   return launch_persistent<conv3d_tcs2_kernel<COUT, KC, W, TILES, GW>>(   // two channel groups per item
-      a, p, (long long)a.B * (a.D / 2) * p.hblocks * p.ctiles * C::NP, C::SMEM, variant.c_str(), stream);
+      a, p, (long long)a.B * p.Do * p.hblocks * p.ctiles * C::NP, C::SMEM, variant.c_str(), stream);
 }
 
 // The instantiation that serves a stride-2 shape (INPUT extents; template W = output width), writing a channel slice; null when
-// there is none.
+// there is none.  D = 1 is a one-plane 2D conv (the backbone's stride-2 stage entry): one output plane from the kd = 1 taps.
 static TcLaunch select_conv3d_s2_tc(int Cin, int Cout, int D, int H, int W, bool slice) {
-  if (Cin % 16 != 0 || Cin < 16 || D % 2 || H % 2 || W % 2) return nullptr;
+  if (Cin % 16 != 0 || Cin < 16 || (D % 2 && D != 1) || H % 2 || W % 2) return nullptr;
   if (W == 32 && Cout == 96) return launch_tcs2<96, 16, 16, 1>;       // StereoBase conv3[0]: 4c -> 6c as two channel slices
   if (W == 32 && Cout == 64) return launch_tcs2<64, 16, 16, 1>;
   if (slice) return nullptr;                                           // channel slices are instantiated for W = 16 only

@@ -10,7 +10,8 @@ machine without easydict/timm (SURVEY.md section 8c); where it IS importable, us
 
 Division of labour: the 2D feature extractors are out of the kernel scope (SURVEY.md section 2.1
 row 12) and stay torch.nn/cuDNN -- except their 1/2-resolution front (eight 32->32 3x3 convs), which
-reuses the wgmma conv kernel when the input is 256 rows high (_front_tc); everything from the cost
+reuses the wgmma conv kernel when the input is 256 rows high (_front_tc), and the residual stages, whose
+3x3 convs (the stride-2 stage entry included) run on it when the 1/4-resolution map is 128 wide (_stage_tc); everything from the cost
 volume to the disparity map runs in the sm_90a kernels through the engines of aggregation.py.  The 3D modules below are PARAMETER
 CONTAINERS: they are never called, only read by the engines.
 """
@@ -47,7 +48,9 @@ def _front_tc_ok(net, x):
             and _agg.USE_TENSOR_CORES and USE_TC_BACKBONE and x.dtype == torch.float32 and ops.conv3d_tc_kc(32, 32, ops.TC_WIDTH) == 32)
 
 
-def _front_tc(net, x):
+def _front_tc(net, x, nhwc=False):
+    """firstconv + layer1 -> (B, 32, H/2, W/2) NCHW, or with nhwc=True the (B, H/2, W/2, 32) channels-last view of the last
+    epilogue's (B, W/2, H/2 = 128, 32) output, which layer2 reads without a layout change (_stage_tc)."""
     convs = [m for m in net.firstconv.modules() if isinstance(m, nn.Conv2d)]
     blocks = list(net.layer1.children())
     y = F.relu(convs[0](x))                                                      # 3 -> 32, stride 2: stays cuDNN
@@ -56,24 +59,40 @@ def _front_tc(net, x):
     for i, blk in enumerate(blocks):                                             # conv-bn-relu, conv-bn, += identity
         c1, c2 = _block_convs(blk)
         assert blk.downsample is None
-        t = _tc2d(net, c2, _tc2d(net, c1, t, ops.ACT_RELU, transpose=True), ops.ACT_NONE, residual=t, last=(i == len(blocks) - 1),
-                  transpose=True)
-    return t.transpose(2, 3).contiguous()                                        # (B, 32, W/2, 128) -> (B, 32, 128, W/2)
+        t = _tc2d(net, c2, _tc2d(net, c1, t, ops.ACT_RELU, transpose=True), ops.ACT_NONE, residual=t,
+                  last=(i == len(blocks) - 1 and not nhwc), transpose=True)
+    return t.transpose(1, 2) if nhwc else t.transpose(2, 3).contiguous()          # (B, 32, W/2, 128) -> (B, 32, 128, W/2)
 
 
-def _tc2d(net, conv, t, act, residual=None, last=False, transpose=False):
-    """One BN-folded 3x3 Conv2d (dilation 1 or 2) on the wgmma kernels: t (B, rows, 128, Cin) channels-last."""
+def _front(net, x):
+    """firstconv + layer1 -> (NCHW output, possibly a view; its channels-last view when the tensor-core front ran, else None)."""
+    if not _front_tc_ok(net, x):
+        return net.layer1(net.firstconv(x)), None
+    t = _front_tc(net, x, nhwc=True)
+    return t.permute(0, 3, 1, 2), t
+
+
+def _tc2d(net, conv, t, act, residual=None, last=False, transpose=False, res_nhwc=True):
+    """One BN-folded 3x3 Conv2d (stride 1 with dilation 1 or 2, or stride 2) on the wgmma kernels: t (B, rows, cols, Cin)
+    channels-last with 128 OUTPUT columns; stride 2 runs as a one-plane stride-2 conv."""
     cache = net.__dict__.setdefault("_osb_tc2d", {})
-    dil = conv.dilation[0]
+    dil, s = conv.dilation[0], conv.stride[0]
     if id(conv) not in cache:
-        assert conv.kernel_size == (3, 3) and conv.stride == (1, 1) and conv.padding == (dil, dil) and conv.dilation == (dil, dil)
+        assert conv.kernel_size == (3, 3) and conv.padding == (dil, dil) and conv.dilation == (dil, dil) and conv.stride == (s, s)
+        assert s == 1 or (s == 2 and dil == 1 and not transpose)
         w5 = torch.zeros(conv.out_channels, conv.in_channels, 3, 3, 3, dtype=torch.float32, device=conv.weight.device)
         w2 = conv.weight.detach().float()
         w5[:, :, 1] = w2.transpose(2, 3) if transpose else w2                   # image transposed -> taps transposed
-        kc = ops.conv2d_tc_kc(conv.in_channels, conv.out_channels, ops.TC_WIDTH, dil)
-        cache[id(conv)] = (ops.pack_tc_weight(w5, kc), None if conv.bias is None else conv.bias.detach().float().contiguous())
+        if s == 2:
+            wp = ops.pack_tc_weight(w5, 16, kw_order=(1, 0, 2))
+        else:
+            wp = ops.pack_tc_weight(w5, ops.conv2d_tc_kc(conv.in_channels, conv.out_channels, ops.TC_WIDTH, dil))
+        cache[id(conv)] = (wp, None if conv.bias is None else conv.bias.detach().float().contiguous())
     wp, bias = cache[id(conv)]
-    return ops.conv2d_k3_tc(t, wp, None, bias, residual, act, dil, out_nhwc=not last, res_nhwc=True)
+    if s == 2:                                                                   # a stage entry's conv1: channels-last out
+        assert residual is None and not last
+        return ops.conv3d_k3_s2_tc(t.unsqueeze(1), wp, None, bias, None, act, out_ndhwc=True).squeeze(1)
+    return ops.conv2d_k3_tc(t, wp, None, bias, residual, act, dil, out_nhwc=not last, res_nhwc=res_nhwc)
 
 
 def _block_convs(blk):
@@ -92,25 +111,78 @@ def _block_tc_ok(blk, c):
                and cv.in_channels == c and cv.out_channels == c for cv in (c1, c2)) and ops.conv2d_tc_kc(c, c, ops.TC_WIDTH, dil) != 0
 
 
-def _stage_tc(net, stage, x):
-    """A residual stage (layer2 / layer3 / the dilated layer4 of the PSMNet-style extractor: gwcnet_backbone.py:38-60): a
-    first block that changes stride / channels (+ 1x1 downsample) stays cuDNN; the identity-shortcut 3x3 blocks run on the
-    wgmma kernel when the feature map is 128 columns wide, channels-last in between, NCHW out of the last epilogue."""
+def _downsample_conv(blk):
+    """The 1x1 conv that is a BN-folded block's whole downsample branch, None for any other branch."""
+    mods = [] if blk.downsample is None else [m for m in blk.downsample.modules() if not isinstance(m, nn.Sequential)]
+    return mods[0] if len(mods) == 1 and isinstance(mods[0], nn.Conv2d) else None
+
+
+def _entry_tc_ok(blk, c, h, w):
+    """A stage's first block that changes stride or channels (c -> cout, input h x w): 3x3 conv1 (stride 1 or 2, dilation 1), 3x3
+    conv2 (cout -> cout) and a 1x1 downsample of the same stride, where the output is 128 columns wide and both 3x3 convs have a
+    tensor-core kernel (stride 2: the one-plane stride-2 conv, which needs even h and w)."""
+    c1, c2 = _block_convs(blk)
+    ds = _downsample_conv(blk)
+    s, cout = c1.stride[0], c1.out_channels
+    if ds is None or s not in (1, 2) or w != s * ops.TC_WIDTH:
+        return False
+    if not (ds.kernel_size == (1, 1) and ds.stride == (s, s) and ds.padding == (0, 0) and ds.groups == 1
+            and ds.in_channels == c and ds.out_channels == cout):
+        return False
+    if not all(cv.kernel_size == (3, 3) and cv.dilation == (1, 1) and cv.padding == (1, 1) and cv.groups == 1 and cv.out_channels == cout
+               for cv in (c1, c2)) or c1.stride != (s, s) or c1.in_channels != c or c2.stride != (1, 1) or c2.in_channels != cout:
+        return False
+    conv1_ok = ops.conv3d_s2_tc_supported(c, cout, 1, h, w) if s == 2 else ops.conv2d_tc_kc(c, cout, ops.TC_WIDTH, 1) != 0
+    return conv1_ok and ops.conv2d_tc_kc(cout, cout, ops.TC_WIDTH, 1) != 0
+
+
+def _entry_tc(net, blk, x, t, last):
+    """An _entry_tc_ok block: conv1 + ReLU channels-last on the wgmma kernels from t (B, H, W, C); the downsample on the fp32 1x1
+    kernel from x, the same input as NCHW (a view is fine: only the rows and columns it reads are copied); conv2 adds it in its
+    epilogue."""
+    c1, c2 = _block_convs(blk)
+    ds = _downsample_conv(blk)
+    cache = net.__dict__.setdefault("_osb_tc2d", {})
+    if id(ds) not in cache:
+        cache[id(ds)] = (ops.pack_conv_weight(ds.weight.unsqueeze(2)), None if ds.bias is None else ds.bias.detach().float().contiguous())
+    wp, bias = cache[id(ds)]
+    r = ops.conv3d_1x1(x[:, :, ::2, ::2].contiguous() if ds.stride[0] == 2 else x.contiguous(), wp, None, bias)   # (B, Cout, H', 128)
+    return _tc2d(net, c2, _tc2d(net, c1, t, ops.ACT_RELU), ops.ACT_NONE, residual=r, last=last, res_nhwc=False)
+
+
+def _stage_tc(net, stage, x, t=None, nhwc_out=False):
+    """A residual stage (layer2 / layer3 / the dilated layer4 of the PSMNet-style extractor: gwcnet_backbone.py:38-60) on a
+    feature map 128 columns wide at its output.  x: the NCHW input (a view is fine); t: the same input channels-last (B, H, W, C)
+    when the layers before ran on the wgmma kernels, else None.  Returns (NCHW output, its channels-last copy or None).
+    The identity-shortcut 3x3 blocks run on the wgmma kernels, channels-last in between.  The first block runs there too when it
+    has an identity shortcut, or -- on a channels-last input -- as an _entry_tc block; a stage fed NCHW by cuDNN layers keeps
+    its entry block on cuDNN.  With nhwc_out a stage that got a channels-last input hands one on: the last epilogue writes it and
+    the NCHW output is its transpose; otherwise the last epilogue writes NCHW.  Any block without a kernel variant keeps the
+    stage on the module's own layers (cuDNN)."""
     blocks = list(stage.children())
     usable = getattr(net, "_osb_folded", False) and x.is_cuda and x.dtype == torch.float32 and _agg.USE_TENSOR_CORES and USE_TC_BACKBONE
-    y, rest = x, blocks
-    if not (usable and x.shape[3] == ops.TC_WIDTH and _block_tc_ok(blocks[0], x.shape[1])):
-        y, rest = blocks[0](x), blocks[1:]
-    c = y.shape[1]
-    if not (usable and rest and y.shape[3] == ops.TC_WIDTH and all(_block_tc_ok(b, c) for b in rest)):
-        for b in rest:
-            y = b(y)
-        return y
-    t = ops.to_ndhwc(y.unsqueeze(2).contiguous()).squeeze(1)                      # (B, H, 128, C)
-    for i, b in enumerate(rest):
-        c1, c2 = _block_convs(b)
-        t = _tc2d(net, c2, _tc2d(net, c1, t, ops.ACT_RELU), ops.ACT_NONE, residual=t, last=(i == len(rest) - 1))
-    return t                                                                      # (B, C, H, 128)
+    c, h, w = x.shape[1:]
+    entry = usable and t is not None and _entry_tc_ok(blocks[0], c, h, w)
+    if entry:
+        c = _block_convs(blocks[0])[1].out_channels
+    elif not (usable and w == ops.TC_WIDTH and _block_tc_ok(blocks[0], c)):
+        x, t = blocks[0](x.contiguous()), None
+        blocks, c, w = blocks[1:], x.shape[1], x.shape[3]
+    if not (usable and blocks and (entry or w == ops.TC_WIDTH) and all(_block_tc_ok(blk, c) for blk in blocks[entry:])):
+        y = x.contiguous()
+        for blk in blocks:
+            y = blk(y)
+        return y, None
+    keep = nhwc_out and t is not None
+    t = t.contiguous() if t is not None else ops.to_ndhwc(x.unsqueeze(2).contiguous()).squeeze(1)   # (B, H, W, C)
+    for i, blk in enumerate(blocks):
+        last = i == len(blocks) - 1 and not keep
+        if i == 0 and entry:
+            t = _entry_tc(net, blk, x, t, last)
+        else:
+            c1, c2 = _block_convs(blk)
+            t = _tc2d(net, c2, _tc2d(net, c1, t, ops.ACT_RELU), ops.ACT_NONE, residual=t, last=last)
+    return (t.permute(0, 3, 1, 2).contiguous(), t) if keep else (t, None)       # NCHW (B, C, H, 128)
 
 
 def _lastconv_tc_ok(net, x):
@@ -133,10 +205,9 @@ def gwc_extract(net, x):
     """feature_extraction.forward of gwcnet_backbone.py:80-93 on any module with its attribute names (this file's mirror or a
     BN-folded copy of the reference's own class): identical graph, the 3x3 residual blocks on the wgmma kernels where a
     variant serves the shape, everything else through the module's own layers (cuDNN)."""
-    x = _front_tc(net, x) if _front_tc_ok(net, x) else net.layer1(net.firstconv(x))
-    l2 = _stage_tc(net, net.layer2, x)
-    l3 = _stage_tc(net, net.layer3, l2)
-    l4 = _stage_tc(net, net.layer4, l3)
+    l2, t = _stage_tc(net, net.layer2, *_front(net, x), nhwc_out=True)
+    l3, t = _stage_tc(net, net.layer3, l2, t, nhwc_out=True)
+    l4, _ = _stage_tc(net, net.layer4, l3, t)
     gwc = torch.cat((l2, l3, l4), dim=1)
     out = {"gwc_feature": gwc}
     if net.concat_feature:
@@ -146,9 +217,8 @@ def gwc_extract(net, x):
 
 def psm_extract(net, x):
     """PSMNet._forward of psmnet_backbone.py:82-116 on any module with its attribute names (see gwc_extract)."""
-    o2 = _front_tc(net, x) if _front_tc_ok(net, x) else net.layer1(net.firstconv(x))
-    o4_0 = _stage_tc(net, net.layer2, o2)
-    o8 = _stage_tc(net, net.layer4, _stage_tc(net, net.layer3, o4_0))
+    o4_0, t = _stage_tc(net, net.layer2, *_front(net, x), nhwc_out=True)
+    o8, _ = _stage_tc(net, net.layer4, *_stage_tc(net, net.layer3, o4_0, t, nhwc_out=True))
     size = (o8.size()[2], o8.size()[3])
     up = [F.interpolate(getattr(net, "branch%d" % i)(o8), size, mode="bilinear", align_corners=True) for i in (1, 2, 3, 4)]
     cat = torch.cat((o4_0, o8, up[3], up[2], up[1], up[0]), 1)

@@ -820,13 +820,14 @@ def conv3d_s2_tc_supported(cin, cout, d, h, w):
 
 
 def conv3d_k3_s2_tc(x_ndhwc, w_split, scale=None, shift=None, residual=None, act=ACT_NONE, out_ndhwc=False, res_ndhwc=False):
-    """3x3x3 STRIDE-2 conv + folded BN + residual + activation on the tensor cores.  x_ndhwc: (B,D,H,W,Cin), even D,H,W;
+    """3x3x3 STRIDE-2 conv + folded BN + residual + activation on the tensor cores.  x_ndhwc: (B,D,H,W,Cin), even D,H,W, or D = 1:
+    a stride-2 3x3 Conv2d as one plane (its taps at kd = 1 of the weight, one output plane);
     w_split = pack_tc_weight(weight, 16, kw_order=(1, 0, 2))."""
     assert x_ndhwc.is_cuda and x_ndhwc.dtype == torch.float32 and x_ndhwc.is_contiguous() and x_ndhwc.dim() == 5
     b, d, h, w, cin = x_ndhwc.shape
     cout = w_split.cout
     wptr, scale = _tc_args(w_split, cin, 16, scale)
-    do, ho, wo = d // 2, h // 2, w // 2
+    do, ho, wo = max(1, d // 2), h // 2, w // 2
     shape = (b, do, ho, wo, cout) if out_ndhwc else (b, cout, do, ho, wo)
     y = torch.empty(shape, dtype=torch.float32, device=x_ndhwc.device)
     if residual is not None:

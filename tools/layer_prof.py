@@ -1,8 +1,10 @@
 #!/usr/bin/env python
 """Run ONE aggregation layer at its bench shape (channels-last in/out) a few times: the target of ncu captures and of quick
-per-layer timings.  usage: layer_prof.py <stem|conv2|conv4|conv1s2|conv3s2|conv5|conv6> [batch] [iters]
+per-layer timings.  usage: layer_prof.py <stem|conv2|conv4|conv1s2|conv3s2|conv5|conv6|bb64|bb2e|ds2|...> [batch] [iters]
 OSB_LP_SPLIT=1: the W = 128 stride-1 layers (stem, stem64, stem64n, head) read and write split activations (ops.to_split), as
-GwcNet's stem chain does; the input is converted once, outside the timed calls."""
+GwcNet's stem chain does; the input is converted once, outside the timed calls.
+OSB_LP_CUDNN=1: the 2D backbone layers (bb*, ds*) run as the module's own NCHW Conv2d on cuDNN instead (fp32, TF32 off, algorithm
+search on, as bench.py runs it)."""
 import json
 import os
 import sys
@@ -18,6 +20,10 @@ LAYERS = {  # name: (kind, cin, cout, D, H, W of the INPUT)
     "head": ("s1h", 32, 1, 48, 64, 128),
     # 2D backbone residual-block convs as one-plane volumes (B = 16 images = 8 pairs): layer2 64->64, layer3 128->128, front 32->32
     "bb64": ("2d", 64, 64, 1, 64, 128), "bb128": ("2d", 128, 128, 1, 64, 128), "bb32": ("2d", 32, 32, 1, 256, 128),
+    # stage entries: layer2[0].conv1 (stride 2, one-plane stride-2 conv), layer3[0].conv1 (64->128), their 1x1 downsamples (fp32
+    # pointwise kernel on the NCHW input; the stride-2 one includes the copy of the even rows and columns)
+    "bb2e": ("2ds2", 32, 64, 1, 128, 256), "bb3e": ("2d", 64, 128, 1, 64, 128),
+    "ds2": ("1x1s2", 32, 64, 1, 128, 256), "ds3": ("1x1", 64, 128, 1, 64, 128),
     "conv2": ("s1", 64, 64, 24, 32, 64), "conv4": ("s1", 128, 128, 12, 16, 32),
     "conv1s2": ("s2", 32, 64, 48, 64, 128), "conv3s2": ("s2", 64, 128, 24, 32, 64),
     "conv5": ("dc", 128, 64, 12, 16, 32), "conv6": ("dc", 64, 32, 24, 32, 64),
@@ -35,15 +41,31 @@ def main():
     sc, sh = torch.rand(cout, device=dev, generator=g) + 0.5, torch.randn(cout, device=dev, generator=g) * 0.1
     flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=dev)
     split = bool(os.environ.get("OSB_LP_SPLIT")) and kind in ("s1", "s1n", "s1h") and w == 128
-    if kind == "2d":
-        B = 2 * B
+    if kind in ("2d", "2ds2", "1x1", "1x1s2"):
+        B, s, k = 2 * B, 2 if kind.endswith("s2") else 1, 1 if kind.startswith("1x1") else 3
+        macs = B * (h // s) * (w // s) * k * k * cin * cout
+        wgt = torch.randn(cout, cin, k, k, device=dev, generator=g) * 0.05
+        xn = torch.randn(B, cin, h, w, device=dev, generator=g)
+    if os.environ.get("OSB_LP_CUDNN") and kind in ("2d", "2ds2", "1x1", "1x1s2"):
+        torch.backends.cudnn.allow_tf32 = False
+        torch.backends.cudnn.benchmark = True
+        fn = lambda: torch.nn.functional.conv2d(xn, wgt, sh, s, k // 2)  # noqa: E731
+    elif kind == "2ds2":
+        w5 = torch.zeros(cout, cin, 3, 3, 3, device=dev)
+        w5[:, :, 1] = wgt
+        wp = ops.pack_tc_weight(w5, 16, kw_order=(1, 0, 2))
+        x = torch.randn(B, 1, h, w, cin, device=dev, generator=g)
+        fn = lambda: ops.conv3d_k3_s2_tc(x, wp, None, sh, None, ops.ACT_RELU, out_ndhwc=True)  # noqa: E731
+    elif kind in ("1x1", "1x1s2"):
+        wp = ops.pack_conv_weight(wgt.unsqueeze(2))
+        fn = lambda: ops.conv3d_1x1(xn[:, :, ::s, ::s].contiguous(), wp, None, sh)  # noqa: E731
+    elif kind == "2d":
         x = torch.randn(B, h, w, cin, device=dev, generator=g)
         w5 = torch.zeros(cout, cin, 3, 3, 3, device=dev)
-        w5[:, :, 1] = torch.randn(cout, cin, 3, 3, device=dev, generator=g) * 0.05
+        w5[:, :, 1] = wgt
         wp = ops.pack_tc_weight(w5, ops.conv2d_tc_kc(cin, cout, w, 1))
         res = None if os.environ.get("OSB_LP_NORES") else torch.randn(B, h, w, cout, device=dev, generator=g)
         fn = lambda: ops.conv2d_k3_tc(x, wp, None, sh, res, ops.ACT_RELU)  # noqa: E731
-        macs = B * h * w * 9 * cin * cout
     elif kind == "dc":
         wgt = torch.randn(cin, cout, 3, 3, 3, device=dev, generator=g) * 0.05
         wp = ops.pack_tc_deconv_weight(wgt)
@@ -74,7 +96,7 @@ def main():
         fn = lambda: ops.conv3d_k3_tc(x, wp, sc, sh, None, ops.ACT_RELU, out_ndhwc=True, out_split=split)  # noqa: E731
         macs = B * d * h * w * 27 * cin * cout
     ms, _ = timeit(fn, iters, flush)
-    print(json.dumps({"layer": name, "split": split, "ms": round(ms, 4), "useful_TF": round(2 * macs / ms / 1e9, 1)}), flush=True)
+    print(json.dumps({"layer": name, "split": split, "cudnn": bool(os.environ.get("OSB_LP_CUDNN")), "ms": round(ms, 4), "useful_TF": round(2 * macs / ms / 1e9, 1)}), flush=True)
 
 
 if __name__ == "__main__":
