@@ -38,6 +38,8 @@ extern "C" {
 #define OSB_ACT_RELU 1
 #define OSB_ACT_LEAKY 2 /* LeakyReLU(0.01), nn.LeakyReLU default used by StereoBase */
 #define OSB_ACT_RELU6 3 /* nn.ReLU6 of LightStereo's MobileV2Residual; accepted by the CUDA-core 1x1, depthwise and 2D kernels */
+#define OSB_ACT_SIGMOID 4 /* the ConvGRU gates (torch.sigmoid / torch.tanh); accepted by osb_conv2d_k3_tc_gru_fwd */
+#define OSB_ACT_TANH 5
 
 typedef void* osb_stream_t;
 
@@ -270,6 +272,17 @@ int osb_conv2d_tc_kc(int Cin, int Cout, int W, int dilation);
 int osb_conv2d_k3_tc_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
                          float* y, int B, int Cin, int Cout, int H, int W, int dilation, int act, int out_nhwc, int res_nhwc,
                          osb_stream_t stream);
+/* osb_conv2d_k3_tc_fwd (dilation 1) with the epilogue of one ConvGRU step (igev/update.py:28-42, stereobase/gru_blocks.py:254-268),
+ * for Cout = 128 (the hidden size) and the widths the 16-channel-chunk kernels serve (osb_conv2d_tc_kc(Cin, 128, W, 1) == 16: W >= 24):
+ *     v = act(conv(x) * scale + shift + residual),  act also OSB_ACT_SIGMOID / OSB_ACT_TANH
+ *     v = v * mul                                    (mul_nhwc non-NULL: the GRU's r * h)
+ *     y = blend_h + blend_z * (v - blend_h)          (both non-NULL: h' = (1 - z) h + z q)
+ * mul_nhwc, blend_z_nhwc, blend_h_nhwc: (B,H,W,Cout) channels-last fp32.  res_bstride: floats between the batches of an NCHW
+ * residual (res_nhwc = 0), >= Cout*H*W -- a channel split() view of a wider (B, C', H, W) tensor -- or 0 for Cout*H*W.  With every
+ * new operand NULL and a standard activation the result is osb_conv2d_k3_tc_fwd's, bit for bit. */
+int osb_conv2d_k3_tc_gru_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
+                             const float* mul_nhwc, const float* blend_z_nhwc, const float* blend_h_nhwc, float* y, int B, int Cin,
+                             int Cout, int H, int W, int act, int out_nhwc, int res_nhwc, long long res_bstride, osb_stream_t stream);
 /* ---- SURVEY.md section 8(f) row 4: remaining volume / regression flavours of the model zoo -------------------------------------
  * osb_gwc_volume_sum_fwd: osb_gwc_volume_fwd with a plain SUM over the K channels of a group instead of the mean:
  *   - CoExCostVolume(maxdisp, group)(x, y) (cost_volume/cost_volume.py:9-29) = sum flavour with D = maxdisp + 1, G = group;
@@ -381,6 +394,9 @@ int osb_ncdhw_to_ndhwc(const float* x, float* y, int B, int C, int D, int H, int
 /* Same with the channel axis zero-padded to Cpad >= C: y (B,D,H,W,Cpad) -- channel plans that are not multiples of 16 (StereoBase's
  * 24 / 48) run on the tensor-core kernels as 32 / 64 with zero weights on the padding. */
 int osb_ncdhw_to_ndhwc_pad(const float* x, float* y, int B, int C, int Cpad, int D, int H, int W, osb_stream_t stream);
+/* Same into channels coff .. coff + C - 1 of y (B,D,H,W,ystride), ystride >= coff + C; the other channels are left as they are
+ * (the ConvGRU's torch.cat of its inputs, written channels-last without materialising the NCHW concatenation). */
+int osb_ncdhw_to_ndhwc_slice(const float* x, float* y, int B, int C, int D, int H, int W, int ystride, int coff, osb_stream_t stream);
 /* FeatureAtt gate in one launch (igev_blocks.py:35-48 as used by stereobase/hourglass.py:62-99):
  * gate_nhwc (B,H,W,Cpad) = sigmoid(conv1x1(act1(bn(conv1x1(feat_nchw (B,Cf,H,W)))))), channels Cv..Cpad-1 zero.
  * w1_packed (Cf,Ch), w2_packed (Ch,Cv); scale/shift = folded BN / bias (NULL = identity).  HW = H*W. */

@@ -54,6 +54,8 @@ SIGNATURES = {
     "osb_context_upsample_fwd": [_f32p] * 3 + [_i] * 4 + [_s],
     "osb_conv2d_tc_kc": [_i] * 4,
     "osb_conv2d_k3_tc_fwd": [_f32p] * 6 + [_i] * 9 + [_s],
+    "osb_conv2d_k3_tc_gru_fwd": [_f32p] * 9 + [_i] * 8 + [ctypes.c_longlong, _s],
+    "osb_ncdhw_to_ndhwc_slice": [_f32p, _f32p] + [_i] * 7 + [_s],
     "osb_ncdhw_to_ndhwc": [_f32p, _f32p, _i, _i, _i, _i, _i, _s],
     "osb_gwc_volume_sum_fwd": [_f32p, _f32p, _f32p, _i, _i, _i, _i, _i, _i, _s],
     "osb_group_l2_normalize_fwd": [_f32p, _f32p, _i, _i, _i, _i, _i, _f, _s],

@@ -430,9 +430,11 @@ __global__ void __launch_bounds__(TC_WG_THREADS, 1) conv3d_tc_kernel(const __gri
 
 // ---------------------------------------------------------------------------------------- layout conversion kernels
 // NCDHW -> NDHWC through a 32x32 shared-memory transpose (both sides coalesced); with `ys`, to split NDHWC instead of y (each
-// value's hi and lo halves, out-of-range values reported on `overflow`).
+// value's hi and lo halves, out-of-range values reported on `overflow`).  y voxels hold `ystride` >= Cp floats and the Cp channels
+// land at channel `coff` of each, so that several NCDHW tensors fill one channels-last concatenation.
 __global__ void __launch_bounds__(256) ncdhw_to_ndhwc_kernel(const float* __restrict__ x, float* __restrict__ y, int C, int Cp,
-                                                             size_t vol, uint16_t* __restrict__ ys, unsigned int* overflow) {
+                                                             size_t vol, uint16_t* __restrict__ ys, unsigned int* overflow,
+                                                             int ystride, int coff) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const size_t v0 = (size_t)blockIdx.x * 32;
@@ -450,7 +452,7 @@ __global__ void __launch_bounds__(256) ncdhw_to_ndhwc_kernel(const float* __rest
     const int c = c0 + tx;
     if (c >= Cp || v >= vol) continue;
     if (!ys) {
-      y[((size_t)b * vol + v) * Cp + c] = tile[tx][i];      // channels C .. Cp-1: zero padding
+      y[((size_t)b * vol + v) * ystride + coff + c] = tile[tx][i];      // channels C .. Cp-1: zero padding
       continue;
     }
     const float s = tile[tx][i] * TC_ACT_SCALE;
@@ -498,7 +500,7 @@ int osb_ncdhw_to_ndhwc_pad(const float* x, float* y, int B, int C, int Cpad, int
   OSB_REQUIRE(B > 0 && C > 0 && Cpad >= C && D > 0 && H > 0 && W > 0 && B <= 65535, "ncdhw_to_ndhwc: bad shape");
   const size_t vol = (size_t)D * H * W;
   dim3 grid((unsigned)((vol + 31) / 32), (Cpad + 31) / 32, B);
-  ncdhw_to_ndhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, y, C, Cpad, vol, nullptr, nullptr);
+  ncdhw_to_ndhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, y, C, Cpad, vol, nullptr, nullptr, Cpad, 0);
   count_launch();
   return check_launch("ncdhw_to_ndhwc_kernel");
 }
@@ -512,13 +514,26 @@ int osb_ncdhw_to_split(const float* x, float* y_split, int B, int C, int D, int 
   if (!flag) return OSB_ECUDA;
   const size_t vol = (size_t)D * H * W;
   dim3 grid((unsigned)((vol + 31) / 32), (C + 31) / 32, B);
-  ncdhw_to_ndhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, nullptr, C, C, vol, reinterpret_cast<uint16_t*>(y_split), flag);
+  ncdhw_to_ndhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, nullptr, C, C, vol, reinterpret_cast<uint16_t*>(y_split), flag, C, 0);
   count_launch();
   return check_launch("ncdhw_to_ndhwc_kernel");
 }
 
 int osb_ncdhw_to_ndhwc(const float* x, float* y, int B, int C, int D, int H, int W, osb_stream_t stream) {
   return osb_ncdhw_to_ndhwc_pad(x, y, B, C, C, D, H, W, stream);
+}
+
+int osb_ncdhw_to_ndhwc_slice(const float* x, float* y, int B, int C, int D, int H, int W, int ystride, int coff, osb_stream_t stream) {
+  using namespace osb;
+  OSB_REQUIRE(x && y, "ncdhw_to_ndhwc_slice: null pointer");
+  OSB_REQUIRE(B > 0 && C > 0 && D > 0 && H > 0 && W > 0 && B <= 65535, "ncdhw_to_ndhwc_slice: bad shape");
+  OSB_REQUIRE(coff >= 0 && ystride >= coff + C, "ncdhw_to_ndhwc_slice: channels %d .. %d do not fit a voxel of %d", coff, coff + C - 1,
+              ystride);
+  const size_t vol = (size_t)D * H * W;
+  dim3 grid((unsigned)((vol + 31) / 32), (C + 31) / 32, B);
+  ncdhw_to_ndhwc_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, y, C, C, vol, nullptr, nullptr, ystride, coff);
+  count_launch();
+  return check_launch("ncdhw_to_ndhwc_kernel");
 }
 
 static int conv3d_k3_tc_impl(osb::TcArgs a, int dilation, osb_stream_t stream) {
@@ -580,6 +595,17 @@ int osb_conv3d_k3_tc_split_fwd(const float* x, const void* w_split, const float*
 }
 
 int osb_conv2d_tc_kc(int Cin, int Cout, int W, int dilation) { return osb::select_conv3d_tc(Cin, Cout, W, dilation, false, false).kc; }
+
+int osb_conv2d_k3_tc_gru_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
+                             const float* mul_nhwc, const float* blend_z_nhwc, const float* blend_h_nhwc, float* y, int B, int Cin,
+                             int Cout, int H, int W, int act, int out_nhwc, int res_nhwc, long long res_bstride, osb_stream_t stream) {
+  // the ConvGRU epilogue is compiled into conv3d_tcg.cu's Cout = 128 instantiations (TcgCfg::GRU)
+  OSB_REQUIRE(Cout == 128 && osb::select_conv3d_tc(Cin, Cout, W, 1, false, false).kc == 16,
+              "conv2d_k3_tc_gru: no Cout = 128 kernel of conv3d_tcg.cu serves Cin=%d Cout=%d W=%d", Cin, Cout, W);
+  osb::TcArgs a{x_nhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, 1, H, W, act, out_nhwc, res_nhwc, 0, 0, Cout};
+  a.gru = 1, a.mul = mul_nhwc, a.blend_z = blend_z_nhwc, a.blend_h = blend_h_nhwc, a.res_bstride = res_bstride;
+  return conv3d_k3_tc_impl(a, 1, stream);
+}
 
 int osb_conv2d_k3_tc_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
                          float* y, int B, int Cin, int Cout, int H, int W, int dilation, int act, int out_nhwc, int res_nhwc,

@@ -28,7 +28,11 @@ struct TcgParams {
   const float* scale;
   const float* shift;
   const float* residual;
-  const float* gate;       // optional (B, H, W, Cout) channels-last multiplier applied after the activation (FeatureAtt), NDHWC output only
+  const float* gate;       // optional (B, H, W, Cout) channels-last multiplier applied after the activation: FeatureAtt's gate
+                           // (NDHWC output only), or the ConvGRU's h of r * h (TcArgs::mul)
+  const float* blend_z;    // optional ConvGRU blend operands (B, H, W, Cout) channels-last: y = blend_h + blend_z * (y - blend_h)
+  const float* blend_h;
+  long long res_bstride;   // floats between the batches of an NCDHW residual (0 = COUT * D * H * W)
   float* y;
   int B, D, H, Cin;
   int act;
@@ -44,6 +48,8 @@ struct TcgParams {
 template <int COUT, int KC, int W, int TILES, int DIL = 1, bool GW = false>
 struct TcgCfg {
   static_assert(!GW || W == 128, "general-width tiles are 128-column segments of one image row");
+  // Cout = 128, dilation 1 (hidden 128 at every width): the ConvGRU epilogue (tc_common.cuh: frag_epilogue, TcArgs::gru)
+  static constexpr bool GRU = COUT == 128 && DIL == 1;
   static constexpr int HALO = GW ? DIL : 0;                 // halo columns on each side of a column tile
   static constexpr int CSTEP = 128 - 2 * HALO;              // image columns a column tile produces
   // DIL = 2: dilated 2D convs of the backbone (layer4 of gwcnet_backbone.py:38-60, psmnet_backbone.py) as one-plane volumes:
@@ -227,19 +233,21 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
       frag_unshift<C::G, DIL, W>(acc, xchg + (exc & 1) * (C::XCHG_FLOATS / 2), q, lane, corr, bar_xchg);
       ++exc;
       const size_t plane = (size_t)p.D * p.H * Wp;                                 // NCDHW channel stride
+      const ptrdiff_t rbs = (C::GRU && p.res_bstride) ? (ptrdiff_t)p.res_bstride : (ptrdiff_t)(COUT * plane);   // NCDHW residual batch stride
       auto rows = [&](int m, ptrdiff_t& yo, ptrdiff_t& ro, ptrdiff_t& go) {
         int h, col;
         const bool ok = tile_row(m, h, col);
         const ptrdiff_t vox = (((ptrdiff_t)b * p.D + d) * p.H + h) * Wp + col;     // NDHWC voxel index
-        const ptrdiff_t ncdhw = (ptrdiff_t)b * COUT * plane + ((ptrdiff_t)d * p.H + h) * Wp + col;
-        yo = p.out_ndhwc ? vox * YS : ncdhw;
-        ro = p.res_ndhwc ? vox * YS : ncdhw;
+        const ptrdiff_t sp = ((ptrdiff_t)d * p.H + h) * Wp + col;                  // offset inside an NCDHW channel plane
+        yo = p.out_ndhwc ? vox * YS : (ptrdiff_t)b * COUT * plane + sp;
+        ro = p.res_ndhwc ? vox * YS : (ptrdiff_t)b * rbs + sp;
         go = (((ptrdiff_t)b * p.H + h) * Wp + col) * YS;
         return ok;
       };
-      frag_epilogue<C::G>(acc, lane, q, tiles + warp * FRAG_TP_FLOATS, s_scale + cg, s_shift + cg, p.act, p.y + (p.out_ndhwc ? (size_t)cg : cg * plane),
+      frag_epilogue<C::G, C::GRU>(acc, lane, q, tiles + warp * FRAG_TP_FLOATS, s_scale + cg, s_shift + cg, p.act, p.y + (p.out_ndhwc ? (size_t)cg : cg * plane),
                           p.out_ndhwc ? 1 : plane, p.residual ? p.residual + (p.res_ndhwc ? (size_t)cg : cg * plane) : nullptr,
-                          p.res_ndhwc ? 1 : plane, (GATE && p.gate) ? p.gate + cg : nullptr, rows, C::G);
+                          p.res_ndhwc ? 1 : plane, ((GATE || C::GRU) && p.gate) ? p.gate + cg : nullptr, rows, C::G, false, false, nullptr,
+                          p.blend_z ? p.blend_z + cg : nullptr, p.blend_h ? p.blend_h + cg : nullptr);
     }
   }
   // ---------------------------------------------------------------------------------------------- A-unit loaders
@@ -347,7 +355,8 @@ template <int COUT, int KC, int W, int TILES, int DIL = 1, bool GW = false, bool
 static int launch_tcg(const TcArgs& a, cudaStream_t stream) {
   using C = TcgCfg<COUT, KC, W, TILES, DIL, GW>;
   TcgParams p{};
-  p.gate = a.gate, p.ystride = a.ystride;
+  p.gate = a.gate ? a.gate : a.mul, p.ystride = a.ystride;
+  p.blend_z = a.blend_z, p.blend_h = a.blend_h, p.res_bstride = a.res_bstride;
   p.hblocks = C::hblocks(a.H);
   p.Wr = GW ? a.W : W;
   p.ctiles = GW ? (a.W + C::CSTEP - 1) / C::CSTEP : 1;

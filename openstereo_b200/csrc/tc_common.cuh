@@ -374,6 +374,8 @@ __device__ __forceinline__ void frag_unshift(float (&acc)[2][3 * G / 2], float* 
     }
   }
 }
+// The ConvGRU gate activations (OSB_ACT_SIGMOID, OSB_ACT_TANH) with IEEE expf / tanhf: torch.sigmoid / torch.tanh to a few ulp.
+static __device__ __noinline__ float gru_act(float v, int act) { return act == OSB_ACT_SIGMOID ? 1.f / (1.f + expf(-v)) : tanhf(v); }
 // Channels-last output tile of one consumer warp: 16 fragment rows x 32 channels.  40 floats per row: the STS.64 of a half-warp
 // (rows l/4, channel pairs 2(l%4)) hit distinct banks, and rows stay 16-byte aligned for the LDS.128 reads.
 constexpr int FRAG_TP_STRIDE = 40;
@@ -390,14 +392,18 @@ constexpr int FRAG_TP_FLOATS = 16 * FRAG_TP_STRIDE;
 //   * otherwise straight from the fragments: NCDHW planes take 8 consecutive voxels of 4 channels per warp instruction.
 // y_split / res_split: the channels-last output / residual is split NDHWC (G = 32 only; offsets still count floats, which address
 // the same bytes); a split output reports values outside the fp16 range on `overflow`.
-template <int G, class Rows>
+// GRU (conv3d_tcg.cu's Cout = 128 instantiations, the ConvGRU update): act may also be OSB_ACT_SIGMOID / OSB_ACT_TANH, and bz / bh
+// are channels-last operands at the gate's offsets; when set, the value after the gate becomes the blend bh + bz * (v - bh) =
+// (1 - z) h + z q.  With either, the values are stored straight from the fragments.  Compiled out of every other instantiation.
+template <int G, bool GRU = false, class Rows>
 __device__ __forceinline__ void frag_epilogue(const float (&acc)[2][3 * G / 2], int lane, int wq, float* tbuf, const float* sc,
                                               const float* sh, int act, float* y, size_t ycs, const float* res, size_t rcs,
                                               const float* gate, Rows rows, int nch, bool y_split = false, bool res_split = false,
-                                              unsigned int* overflow = nullptr) {
+                                              unsigned int* overflow = nullptr, const float* bz = nullptr, const float* bh = nullptr) {
   const int c0 = 2 * (lane & 3), l4 = lane >> 2;
   if constexpr (G == 32) {
-    if (ycs == 1 && (!res || rcs == 1)) {
+    // the GRU's multiplier and blend run on the path below: in this one they would make the Cout = 128 instantiations spill
+    if (ycs == 1 && (!res || rcs == 1) && !(GRU && (gate || bz))) {
       const int c4 = 4 * (lane & 7), sub = lane >> 3;
       const float4 a = *reinterpret_cast<const float4*>(sc + c4);
       const float4 b = *reinterpret_cast<const float4*>(sh + c4);
@@ -440,8 +446,12 @@ __device__ __forceinline__ void frag_epilogue(const float (&acc)[2][3 * G / 2], 
             o[i].x = o[i].x > 0.f ? o[i].x : 0.01f * o[i].x, o[i].y = o[i].y > 0.f ? o[i].y : 0.01f * o[i].y;
             o[i].z = o[i].z > 0.f ? o[i].z : 0.01f * o[i].z, o[i].w = o[i].w > 0.f ? o[i].w : 0.01f * o[i].w;
           }
+        } else if (GRU && (act == OSB_ACT_SIGMOID || act == OSB_ACT_TANH)) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            o[i].x = gru_act(o[i].x, act), o[i].y = gru_act(o[i].y, act), o[i].z = gru_act(o[i].z, act), o[i].w = gru_act(o[i].w, act);
         }
-        if (gate) {
+        if (!GRU && gate) {
           float4 g[4];
 #pragma unroll
           for (int i = 0; i < 4; ++i) g[i] = ok[i] ? __ldg(reinterpret_cast<const float4*>(gate + go[i] + c4)) : make_float4(1.f, 1.f, 1.f, 1.f);
@@ -481,7 +491,7 @@ __device__ __forceinline__ void frag_epilogue(const float (&acc)[2][3 * G / 2], 
             if (live && c + 1 < nch) rv[j][rh].y = __ldg(res + ro + (size_t)(c + 1) * rcs);
           }
         }
-        if (gate && live) gv[j][rh] = __ldg(reinterpret_cast<const float2*>(gate + go + c));
+        if (!GRU && gate && live) gv[j][rh] = __ldg(reinterpret_cast<const float2*>(gate + go + c));
       }
 #pragma unroll
     for (int j = 0; j < G / 8; ++j) {
@@ -499,9 +509,20 @@ __device__ __forceinline__ void frag_epilogue(const float (&acc)[2][3 * G / 2], 
           v0 = fmaxf(v0, 0.f), v1 = fmaxf(v1, 0.f);
         } else if (act == OSB_ACT_LEAKY) {
           v0 = v0 > 0.f ? v0 : 0.01f * v0, v1 = v1 > 0.f ? v1 : 0.01f * v1;
+        } else if (GRU && (act == OSB_ACT_SIGMOID || act == OSB_ACT_TANH)) {
+          v0 = gru_act(v0, act), v1 = gru_act(v1, act);
         }
-        if (gate) v0 *= gv[j][rh].x, v1 *= gv[j][rh].y;
+        if (!GRU && gate) v0 *= gv[j][rh].x, v1 *= gv[j][rh].y;
         if (!live) continue;
+        if (GRU && gate) {                              // loaded where it is used: batched like gv, the GRU operands would spill
+          const float2 m = __ldg(reinterpret_cast<const float2*>(gate + go + c));
+          v0 *= m.x, v1 *= m.y;
+        }
+        if (GRU && bz) {
+          const float2 z = __ldg(reinterpret_cast<const float2*>(bz + go + c));
+          const float2 hv = __ldg(reinterpret_cast<const float2*>(bh + go + c));
+          v0 = hv.x + z.x * (v0 - hv.x), v1 = hv.y + z.y * (v1 - hv.y);
+        }
         if (ycs == 1) {
           *reinterpret_cast<float2*>(y + yo + c) = make_float2(v0, v1);
         } else {
@@ -597,6 +618,14 @@ struct TcArgs {
   float kappa;             // set by check_tc_args
   unsigned int* overflow;  // set by check_tc_args
   int in_split = 0, out_split = 0, res_split = 0;   // stride 1, W = 128: the channels-last x / y / residual is split NDHWC
+  // ConvGRU epilogue (osb_conv2d_k3_tc_gru_fwd, conv3d_tcg.cu only): gru = 1 admits OSB_ACT_SIGMOID / OSB_ACT_TANH and the operands
+  // below, each (B,H,W,Cout) channels-last: y = act(...) * mul, then y = blend_h + blend_z * (y - blend_h).  res_bstride: floats
+  // between the batches of an NCDHW residual (0 = Cout*D*H*W), so that a channel split() view of a wider tensor needs no copy.
+  int gru = 0;
+  const float* mul = nullptr;
+  const float* blend_z = nullptr;
+  const float* blend_h = nullptr;
+  long long res_bstride = 0;
   bool slice() const { return ystride != 0 && ystride != Cout; }
 };
 // Launcher of one instantiation: the result of a family's selector (null: no instantiation serves the arguments).
@@ -610,9 +639,13 @@ inline int check_tc_args(const char* what, TcArgs& a, TcLaunch launch) {
   auto aligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   OSB_REQUIRE(a.x && a.w && a.y, "%s: null pointer", what);
   OSB_REQUIRE(a.B > 0 && a.D > 0 && a.H > 0, "%s: empty shape", what);
-  OSB_REQUIRE(a.act >= 0 && a.act <= 2, "%s: unknown activation %d", what, a.act);
-  OSB_REQUIRE(aligned(a.x) && aligned(a.w) && aligned(a.y) && aligned(a.residual) && aligned(a.gate),
-              "%s: pointers must be 16-byte aligned", what);
+  OSB_REQUIRE(a.act >= 0 && (a.act <= 2 || (a.gru && (a.act == OSB_ACT_SIGMOID || a.act == OSB_ACT_TANH))), "%s: unknown activation %d",
+              what, a.act);
+  OSB_REQUIRE(aligned(a.x) && aligned(a.w) && aligned(a.y) && aligned(a.residual) && aligned(a.gate) && aligned(a.mul) &&
+              aligned(a.blend_z) && aligned(a.blend_h), "%s: pointers must be 16-byte aligned", what);
+  OSB_REQUIRE(!a.blend_z == !a.blend_h, "%s: the blend needs both z and h", what);
+  OSB_REQUIRE(a.res_bstride == 0 || (a.residual && !a.res_ndhwc && a.res_bstride >= (long long)a.Cout * a.D * a.H * a.W),
+              "%s: a residual batch stride (%lld) needs an NCDHW residual and at least Cout*D*H*W floats", what, a.res_bstride);
   const bool channels_last = a.out_ndhwc && (!a.residual || a.res_ndhwc);
   OSB_REQUIRE(a.ystride == 0 || (a.ystride >= a.Cout && a.ystride % 4 == 0 && channels_last),
               "%s: a channel slice (ystride %d) needs channels-last tensors", what, a.ystride);

@@ -1098,3 +1098,47 @@ def conv2d_k3_tc(x_nhwc, w_split, scale=None, shift=None, residual=None, act=ACT
     _call("osb_conv2d_k3_tc_fwd", x_nhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), y.data_ptr(), b, cin,
           cout, h, w, dilation, act, int(out_nhwc), int(res_nhwc), _stream(y))
     return y
+
+
+# --------------------------------------------------------------------------- ConvGRU update (gru.py)
+ACT_SIGMOID, ACT_TANH = 4, 5     # include/openstereo_b200.h: OSB_ACT_SIGMOID / OSB_ACT_TANH, osb_conv2d_k3_tc_gru_fwd only
+
+
+def nchw_to_nhwc_cat(tensors):
+    """[(B,C_i,H,W) fp32 contiguous] -> (B,H,W,sum C_i) fp32: the channel concatenation, written channels-last one slice per tensor
+    (osb_ncdhw_to_ndhwc_slice) without materialising the NCHW torch.cat."""
+    b, _, h, w = tensors[0].shape
+    total = sum(t.shape[1] for t in tensors)
+    y = torch.empty((b, h, w, total), dtype=torch.float32, device=tensors[0].device)
+    coff = 0
+    for t in tensors:
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 4 and (t.shape[0], *t.shape[2:]) == (b, h, w)
+        _call("osb_ncdhw_to_ndhwc_slice", t.data_ptr(), y.data_ptr(), b, t.shape[1], 1, h, w, total, coff, _stream(y))
+        coff += t.shape[1]
+    return y
+
+
+def conv2d_k3_tc_gru(x_nhwc, w_split, shift=None, residual=None, act=ACT_NONE, mul=None, blend=None, out_nhwc=True, res_nhwc=True):
+    """3x3 Conv2d (stride 1, padding 1) with the ConvGRU epilogue on the tensor cores (osb_conv2d_k3_tc_gru_fwd), Cout = 128:
+        v = act(conv(x) + shift + residual);  v = v * mul;  y = h + z * (v - h) with (z, h) = blend.
+    x_nhwc (B,H,W,Cin); mul and the blend operands (B,H,W,128) channels-last; an NCHW residual (res_nhwc=False) may be a channel
+    split() view of a wider (B, C', H, W) tensor (its batch stride goes to the kernel, no copy)."""
+    assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float32 and x_nhwc.is_contiguous() and x_nhwc.dim() == 4
+    b, h, w, cin = x_nhwc.shape
+    cout = w_split.cout
+    wptr, scale = _tc_args(w_split, cin, 16, None)
+    y = torch.empty((b, h, w, cout) if out_nhwc else (b, cout, h, w), dtype=torch.float32, device=x_nhwc.device)
+    rbs = 0
+    if residual is not None:
+        assert residual.is_cuda and residual.dtype == torch.float32
+        if res_nhwc:
+            assert tuple(residual.shape) == (b, h, w, cout) and residual.is_contiguous()
+        else:
+            assert tuple(residual.shape) == (b, cout, h, w) and tuple(residual.stride()[1:]) == (h * w, w, 1)
+            rbs = 0 if residual.is_contiguous() else residual.stride(0)
+    z, hh = blend if blend is not None else (None, None)
+    for t in (mul, z, hh):
+        assert t is None or (tuple(t.shape) == (b, h, w, cout) and t.is_contiguous() and t.dtype == torch.float32 and t.is_cuda)
+    _call("osb_conv2d_k3_tc_gru_fwd", x_nhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), _ptr(mul), _ptr(z), _ptr(hh),
+          y.data_ptr(), b, cin, cout, h, w, act, int(out_nhwc), int(res_nhwc), rbs, _stream(y))
+    return y

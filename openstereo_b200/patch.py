@@ -19,6 +19,7 @@ needs its own rebinding:
               Hourglass                                                      -> per-INSTANCE copies of the methods that use those names,
                                                                                 with a private globals dict (the module itself, and
                                                                                 therefore every other StereoBase instance, is untouched)
+* StereoBase / IGEVStereo ConvGRUs ``update_block.gru04 / gru08 / gru16``   -> per-instance ``forward`` overrides (gru.py)
 
 Parameters stay where they are (the engines read them through the reference's attribute names), so
 ``state_dict()`` / ``load_state_dict()`` and checkpoints are untouched.
@@ -215,8 +216,30 @@ def _rebind_methods(model, overrides):
             setattr(model, name, types.MethodType(copy, model))
 
 
+def _patch_convgru(block, strict):
+    """Per-instance ``forward`` overrides of ``gru04 / gru08 / gru16`` of an IGEV / StereoBase BasicMultiUpdateBlock: CUDA inference
+    calls the wgmma kernels serve (gru.route_ok) run gru.ConvGRUEngine; the other shapes run the reference's own forward."""
+    from .gru import ConvGRUEngine
+    for name in ("gru04", "gru08", "gru16"):
+        mod = getattr(block, name)
+        _override_convgru(mod, ConvGRUEngine(mod), strict)
+
+
+def _override_convgru(mod, engine, strict):
+    orig = mod.forward
+
+    def forward(self, h, cz, cr, cq, *x_list):
+        if _trainable(self) or not _accelerable(self, h, cz, cr, cq, *x_list):
+            return orig(h, cz, cr, cq, *x_list) if not strict else _refuse("ConvGRU")
+        if not engine.serves(h, x_list):
+            return orig(h, cz, cr, cq, *x_list)                     # no kernel for this shape: today's reference computation
+        return engine(h, cz, cr, cq, *x_list)
+
+    mod.forward = types.MethodType(forward, mod)
+
+
 def _patch_stereobase(model, strict, backbone=True):
-    g = type(model).forward.__globals__                             # stereo.modeling.models.stereobase.stereobase_gru namespace
+    g = type(model).forward.__globals__                            # stereo.modeling.models.stereobase.stereobase_gru namespace
     hg = model.cost_agg
     hg_orig = hg.forward
     agg = StereoBaseAggregation(hg)
@@ -260,6 +283,7 @@ def _patch_stereobase(model, strict, backbone=True):
         return agg(x, features).to(x.dtype)
 
     hg.forward = types.MethodType(hg_forward, hg)
+    _patch_convgru(model.update_block, strict)
     return model
 
 
@@ -317,8 +341,10 @@ def _patch_lightstereo(model, strict, backbone=True):
 
 def _patch_igev(model, strict, backbone=True):
     """IGEV-Stereo (BASELINE config 5; igev/igev_stereo.py:136-213): the gwc volume, the soft-argmin regression of the initial
-    disparity, the per-GRU-iteration lookup of the combined geometry-encoding volume and the convex up-sampling.  The hourglass(8),
-    feature nets and ConvGRU update blocks stay the reference's cuDNN code."""
+    disparity, the per-GRU-iteration lookup of the combined geometry-encoding volume, the three ConvGRUs of the update block
+    (``update_block.gru04 / gru08 / gru16``, gru.py) and the convex up-sampling.  The hourglass(8), feature nets, motion encoder and
+    disp / mask heads stay the reference's cuDNN code.  Under autocast (the AMP YAML) the GRUs compute in fp32 and return the
+    reference's dtype."""
     g = type(model).forward.__globals__
     orig = {n: g[n] for n in ("build_gwc_volume", "disparity_regression", "context_upsample", "Combined_Geo_Encoding_Volume")}
     over = _volume_tail_overrides(model, strict, orig, with_corr=False)
@@ -332,6 +358,7 @@ def _patch_igev(model, strict, backbone=True):
 
     over["Combined_Geo_Encoding_Volume"] = geo_factory
     _rebind_methods(model, over)
+    _patch_convgru(model.update_block, strict)
     return model
 
 

@@ -22,6 +22,9 @@
   c9  IGEV-RT cfgs/igev_rt (the reference's class + patch()), batch 8 @256x512 and @544x960: the uniform YAML's model patched and
       unpatched, timed alternately, the unpatched AMP YAML's model for context, per-stage times (volume, cost_agg, classifier, the 8
       lookups, everything else) and the lookups' GB/s  (python tools/bench_configs.py --only c9)
+  c10 the ConvGRUs of IGEVStereo (cfgs/igev AMP YAML @480x640) and StereoBase (cfgs/stereobase @256x512), batch 8 (the reference's
+      classes + patch()): ms in the three ConvGRUs and per forward, patched / cuDNN fp32 / fp16 autocast in alternating rotation,
+      the GRU stage's TFLOP/s and the EPE against the unpatched model  (python tools/bench_configs.py --only c10)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -511,6 +514,94 @@ def c9(iters, B=8):
         torch.cuda.empty_cache()
 
 
+def _gru_stage(run, block):
+    """One run of `run` with CUDA events around every call of block.gru04 / gru08 / gru16: (ms in the three ConvGRUs, their MACs)."""
+    events, macs = [], [0]
+    mods = [getattr(block, n) for n in ("gru04", "gru08", "gru16")]
+    saved = [vars(m).get("forward") for m in mods]
+
+    def wrap(inner):
+        def fwd(h, *rest):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            cin = h.shape[1] + sum(t.shape[1] for t in rest[3:])
+            macs[0] += 3 * h.shape[0] * h.shape[2] * h.shape[3] * h.shape[1] * cin * 9
+            a.record()
+            out = inner(h, *rest)
+            b.record()
+            events.append((a, b))
+            return out
+        return fwd
+    for m in mods:
+        m.forward = wrap(m.forward)
+    try:
+        run()
+        torch.cuda.synchronize()
+    finally:
+        for m, s in zip(mods, saved):
+            if s is None:
+                del m.forward
+            else:
+                m.forward = s
+    return sum(a.elapsed_time(b) for a, b in events), macs[0]
+
+
+def c10(iters, B=8):
+    """The ConvGRUs of IGEV-Stereo (cfgs/igev AMP YAML, config 5's 480x640) and StereoBase (cfgs/stereobase, 256x512), batch 8, the
+    reference's classes with the timm stand-in the tests use.  Three variants timed in alternating rotation: patch() (the GRUs on the
+    wgmma kernels, fp32), unpatched cuDNN fp32 with TF32 off, and unpatched under fp16 autocast.  Per variant: whole-forward ms and
+    the ms spent in the three ConvGRUs (CUDA events around every gru04 / gru08 / gru16 call); the GRU stage's useful fp32-equivalent
+    TFLOP/s counts 2 x its MACs (three 3x3 convs of Cin = hidden + inputs per call); EPE of patched against unpatched fp32."""
+    from oracle import _reference_shim as shim
+    from openstereo_b200.patch import patch
+    shim.install_timm_stub()
+
+    def build(which):
+        if which == "igev":
+            cfg = shim.load_cfg("cfgs/igev/igev_sceneflow_amp.yaml").MODEL
+            m = shim.load("stereo.modeling.models.igev.igev_stereo").IGEVStereo(cfg).eval()
+            m.load_state_dict(si.seeded_state_dict(m.state_dict(), seed=12, scale={"classifier.weight": 8.0}))
+        else:
+            cfg = shim.load_cfg("cfgs/stereobase/stereobase_sceneflow.yaml").MODEL
+            m = shim.load("stereo.modeling.models.stereobase.stereobase_gru").StereoBase(cfg).eval()
+            m.load_state_dict(si.seeded_state_dict(m.state_dict(), seed=3, scale={"classifier.weight": 8.0}))
+        return m.to(DEV)
+
+    for which, name, (h, w) in (("igev", "IGEVStereo", (480, 640)), ("stereobase", "StereoBase", (256, 512))):
+        ref, pm = build(which), patch(build(which))
+        gen = torch.Generator().manual_seed(31)
+        x = {"left": (torch.rand(B, 3, h, w, generator=gen) * 255).to(DEV), "right": (torch.rand(B, 3, h, w, generator=gen) * 255).to(DEV)}
+        variants = {"patched": (pm, False), "cudnn_fp32": (ref, False), "amp_fp16": (ref, True)}
+
+        def fwd(m, amp):
+            with torch.autocast("cuda", dtype=torch.float16, enabled=amp):
+                return m(dict(x))["disp_pred"]
+        ms = {k: [] for k in variants}
+        gru_ms = {k: [] for k in variants}
+        outs, macs = {}, 0
+        with torch.no_grad():
+            for _ in range(3):                                          # alternate: the three share the GPU's state
+                for k, (m, amp) in variants.items():
+                    t, outs[k] = timeit(lambda: fwd(m, amp), max(1, iters // 5), warm=1)
+                    ms[k].append(t)
+                    g, macs = _gru_stage(lambda: fwd(m, amp), m.update_block)
+                    gru_ms[k].append(g)
+        med = lambda v: sorted(v)[1]
+        emit(config="c10 ConvGRUs of %s, B=%d @%dx%d (reference class + patch())" % (name, B, h, w),
+             gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+             gru_ms={k: round(med(v), 2) for k, v in gru_ms.items()},
+             forward_ms={k: round(med(v), 2) for k, v in ms.items()},
+             gru_share_of_forward={k: round(med(gru_ms[k]) / med(ms[k]), 3) for k in variants},
+             gru_gmac=round(macs / 1e9, 1),
+             gru_tflops_fp32_equivalent={k: round(2 * macs / (med(v) * 1e-3) / 1e12, 1) for k, v in gru_ms.items()},
+             gru_speedup_vs_cudnn_fp32=round(med(gru_ms["cudnn_fp32"]) / med(gru_ms["patched"]), 2),
+             gru_speedup_vs_amp_fp16=round(med(gru_ms["amp_fp16"]) / med(gru_ms["patched"]), 2),
+             epe_patched_vs_cudnn_fp32_px=float("%.3e" % (outs["patched"] - outs["cudnn_fp32"]).abs().mean().item()),
+             epe_amp_vs_cudnn_fp32_px=float("%.3e" % (outs["amp_fp16"].float() - outs["cudnn_fp32"]).abs().mean().item()),
+             disparity_std_px=round(outs["cudnn_fp32"].std().item(), 2))
+        del ref, pm
+        torch.cuda.empty_cache()
+
+
 def _stage_times(run, targets, volume_fn=None):
     """One run of `run` with CUDA events around the forward of each target (a module, or a class whose __call__ is wrapped) and,
     with volume_fn, around ops.<volume_fn>: {stage: ms}."""
@@ -567,7 +658,7 @@ if __name__ == "__main__":
     a = ap.parse_args()
     for name in a.only.split(","):
         try:
-            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9}[name](a.iters)
+            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:
