@@ -35,14 +35,8 @@ def pack_gru_conv(conv, hidden):
     """One of convz / convr / convq -> (h block, x block, bias): the (Cout, hidden + Cx, 3, 3) weight's two column blocks, each
     packed as a one-plane 3x3x3 weight (taps at kd = 1) for the 16-channel-chunk kernels."""
     w = conv.weight.detach().float()
-
-    def one(w2):
-        w5 = w2.new_zeros(w2.shape[0], w2.shape[1], 3, 3, 3)
-        w5[:, :, 1] = w2
-        return ops.pack_tc_weight(w5, 16)
-
     bias = None if conv.bias is None else conv.bias.detach().float().contiguous()
-    return one(w[:, :hidden]), one(w[:, hidden:]), bias
+    return ops.pack_tc_weight_2d(w[:, :hidden], 16), ops.pack_tc_weight_2d(w[:, hidden:], 16), bias
 
 
 class ConvGRUEngine(_Engine):

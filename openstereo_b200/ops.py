@@ -1083,6 +1083,14 @@ def conv2d_tc_kc(cin, cout, w, dilation=1):
     return int(_lib.lib.osb_conv2d_tc_kc(int(cin), int(cout), int(w), int(dilation)))
 
 
+def pack_tc_weight_2d(weight, kc):
+    """(Cout, Cin, 3, 3) Conv2d weight -> TcWeight of the one-plane 3x3x3 weight that holds its taps at kd = 1 (conv2d_k3_tc)."""
+    w2 = weight.detach().float()
+    w5 = w2.new_zeros(w2.shape[0], w2.shape[1], 3, 3, 3)
+    w5[:, :, 1] = w2
+    return pack_tc_weight(w5, kc)
+
+
 def conv2d_k3_tc(x_nhwc, w_split, scale=None, shift=None, residual=None, act=ACT_NONE, dilation=1, out_nhwc=True, res_nhwc=True):
     """3x3 Conv2d (stride 1, padding = dilation) + folded BN + residual + activation on the tensor cores.  x_nhwc (B,H,W,Cin);
     w_split = pack_tc_weight of the 3x3x3 weight that holds the 2D taps at kd = 1."""

@@ -20,6 +20,7 @@ needs its own rebinding:
                                                                                 with a private globals dict (the module itself, and
                                                                                 therefore every other StereoBase instance, is untouched)
 * StereoBase / IGEVStereo ConvGRUs ``update_block.gru04 / gru08 / gru16``   -> per-instance ``forward`` overrides (gru.py)
+* StereoBase / IGEVStereo ``update_block.encoder / disp_head / mask_feat_4``  -> per-instance ``forward`` overrides (update.py)
 
 Parameters stay where they are (the engines read them through the reference's attribute names), so
 ``state_dict()`` / ``load_state_dict()`` and checkpoints are untouched.
@@ -225,6 +226,29 @@ def _patch_convgru(block, strict):
         _override_convgru(mod, ConvGRUEngine(mod), strict)
 
 
+def _patch_update_heads(block, strict):
+    """Per-instance ``forward`` overrides of ``encoder / disp_head / mask_feat_4`` of an IGEV / StereoBase BasicMultiUpdateBlock:
+    CUDA inference calls the kernels serve (update.route_ok, the engines' serves()) run update.py's engines; the other shapes and
+    hyper-parameters run the reference's own forward."""
+    from .update import DispHeadEngine, MaskFeatEngine, MotionEncoderEngine
+    for name, cls in (("encoder", MotionEncoderEngine), ("disp_head", DispHeadEngine), ("mask_feat_4", MaskFeatEngine)):
+        mod = getattr(block, name)
+        _override_engine(mod, cls(mod), strict, name)
+
+
+def _override_engine(mod, engine, strict, what):
+    orig = mod.forward
+
+    def forward(self, *args):
+        if _trainable(self) or not _accelerable(self, *args):
+            return orig(*args) if not strict else _refuse(what)
+        if not engine.serves(*args):
+            return orig(*args)                                      # no kernel for this shape: the reference computation
+        return engine(*args)
+
+    mod.forward = types.MethodType(forward, mod)
+
+
 def _override_convgru(mod, engine, strict):
     orig = mod.forward
 
@@ -284,6 +308,7 @@ def _patch_stereobase(model, strict, backbone=True):
 
     hg.forward = types.MethodType(hg_forward, hg)
     _patch_convgru(model.update_block, strict)
+    _patch_update_heads(model.update_block, strict)
     return model
 
 
@@ -342,9 +367,9 @@ def _patch_lightstereo(model, strict, backbone=True):
 def _patch_igev(model, strict, backbone=True):
     """IGEV-Stereo (BASELINE config 5; igev/igev_stereo.py:136-213): the gwc volume, the soft-argmin regression of the initial
     disparity, the per-GRU-iteration lookup of the combined geometry-encoding volume, the three ConvGRUs of the update block
-    (``update_block.gru04 / gru08 / gru16``, gru.py) and the convex up-sampling.  The hourglass(8), feature nets, motion encoder and
-    disp / mask heads stay the reference's cuDNN code.  Under autocast (the AMP YAML) the GRUs compute in fp32 and return the
-    reference's dtype."""
+    (``update_block.gru04 / gru08 / gru16``, gru.py), its motion encoder and disp / mask heads (``update_block.encoder / disp_head /
+    mask_feat_4``, update.py) and the convex up-sampling.  The hourglass(8) and the feature nets stay the reference's cuDNN code.
+    Under autocast (the AMP YAML) the update block computes in fp32 and returns the reference's dtypes."""
     g = type(model).forward.__globals__
     orig = {n: g[n] for n in ("build_gwc_volume", "disparity_regression", "context_upsample", "Combined_Geo_Encoding_Volume")}
     over = _volume_tail_overrides(model, strict, orig, with_corr=False)
@@ -359,6 +384,7 @@ def _patch_igev(model, strict, backbone=True):
     over["Combined_Geo_Encoding_Volume"] = geo_factory
     _rebind_methods(model, over)
     _patch_convgru(model.update_block, strict)
+    _patch_update_heads(model.update_block, strict)
     return model
 
 

@@ -1,0 +1,151 @@
+"""The rest of the IGEV-Stereo / StereoBase update block on the library (DESIGN.md section 4.16): the motion encoder
+(igev/update.py:75-94 == stereobase/gru_blocks.py:233-251), the disparity head (igev/update.py:17-25 == gru_blocks.py:271-281) and
+mask_feat_4 (igev/update.py:123-125 == gru_blocks.py:304-306).  The 3x3 layers run on the wgmma convolutions (osb_conv2d_k3_tc_fwd,
+3xFP16 split) with channels-last fp32 intermediates, the three shapes they do not serve on the library's fp32 CUDA-core kernels:
+
+    MotionEncoderEngine  (disp (B,1,H,W), corr (B,Cc,H,W)) -> (B,128,H,W)
+        cor  = relu(convc2(relu(convc1(corr))))         osb_conv3d_1x1_bn_act_fwd on the lookup's NCHW output, pack, tc Cout 64
+        dsp  = relu(convd2(relu(convd1(disp))))         convd1 (7x7, 1 -> 64) as the depthwise osb_dwconv2d_fwd over disp
+                                                        broadcast to 64 planes, pack, tc Cout 64
+        part = conv(cor, W[:, :64]) + b                 conv's weight zero-padded from 127 to 128 output channels, K split in two
+        out  = relu(conv(dsp, W[:, 64:]) + part)        NCHW output with the channels-last residual: relu(conv(cat(cor, dsp)))
+        out[:, 127] = disp                              the reference's torch.cat([out, disp])
+    DispHeadEngine       net0 (B,128,H,W) -> (B,1,H,W)
+        one channels-last pack; conv1 + bias + relu as two Cout 128 launches (one per half of its 256 channels, NCHW);
+        conv2 + bias as two osb_conv3d_k3_bn_act_fwd launches (D = 1), the second adding the first as its residual
+    MaskFeatEngine       net0 -> (B,32,H,W): one pack, one Cout 32 launch with bias + relu and NCHW output
+
+patch.py installs them as per-instance forward overrides of update_block.encoder / disp_head / mask_feat_4 and runs the reference's
+own forward for every shape or hyper-parameter no kernel serves (route_ok, the engines' serves()).
+"""
+import torch
+
+from . import ops
+from .aggregation import _Engine
+
+
+def route_ok(w):
+    """True when the wgmma kernels serve every tensor-core layer of the three modules at image width w (the 64 -> 64, 64 -> 128 and
+    128 -> 128 layers on the 16-channel-chunk kernels, 128 -> 32 on any): W >= OSB_TC_MIN_WIDTH."""
+    return (all(ops.conv2d_tc_kc(cin, cout, w) == 16 for cin, cout in ((64, 64), (64, 128), (128, 128)))
+            and ops.conv2d_tc_kc(128, 32, w) != 0)
+
+
+def _is_conv(c, cin, cout, k):
+    return (isinstance(c, torch.nn.Conv2d) and c.in_channels == cin and c.out_channels == cout and c.kernel_size == (k, k)
+            and c.padding == (k // 2, k // 2) and c.stride == (1, 1) and c.dilation == (1, 1) and c.groups == 1
+            and c.padding_mode == "zeros")
+
+
+def _bias(conv, pad_to=None):
+    b = torch.zeros(conv.out_channels, device=conv.weight.device) if conv.bias is None else conv.bias.detach().float()
+    if pad_to is not None:
+        b = torch.cat((b, b.new_zeros(pad_to - b.numel())))
+    return b.contiguous()
+
+
+def _conv_dtype(*tensors):
+    """dtype of a reference Conv2d's output on these inputs: the autocast dtype where autocast is on, else the inputs' promotion."""
+    if torch.is_autocast_enabled("cuda"):
+        return torch.get_autocast_dtype("cuda")
+    dtype = tensors[0].dtype
+    for t in tensors[1:]:
+        dtype = torch.promote_types(dtype, t.dtype)
+    return dtype
+
+
+def _f32(t):
+    return t.detach().float().contiguous()
+
+
+class MotionEncoderEngine(_Engine):
+    """BasicMotionEncoder.forward(disp, corr) on the library (module docstring)."""
+
+    def _pack(self):
+        m = self.module
+        w = m.conv.weight.detach().float()
+        w = torch.cat((w, w.new_zeros((1,) + tuple(w.shape[1:]))), 0)           # 127 -> 128 output channels, row 127 zero
+        self.c1, self.bc1 = m.convc1.weight.detach().float()[:, :, 0, 0].t().contiguous(), _bias(m.convc1)     # (Cin, 64)
+        self.c2, self.bc2 = ops.pack_tc_weight_2d(m.convc2.weight, 16), _bias(m.convc2)
+        self.d1, self.bd1 = m.convd1.weight.detach().float()[:, 0].contiguous(), _bias(m.convd1)            # (64, 7, 7)
+        self.d2, self.bd2 = ops.pack_tc_weight_2d(m.convd2.weight, 16), _bias(m.convd2)
+        self.wc, self.wd, self.b = ops.pack_tc_weight_2d(w[:, :64], 16), ops.pack_tc_weight_2d(w[:, 64:], 16), _bias(m.conv, 128)
+
+    def serves(self, disp, corr):
+        m = self.module
+        return (disp.dim() == 4 and corr.dim() == 4 and disp.shape[1] == 1 and disp.shape[0] == corr.shape[0]
+                and disp.shape[2:] == corr.shape[2:] and _is_conv(m.convc1, corr.shape[1], 64, 1) and _is_conv(m.convc2, 64, 64, 3)
+                and _is_conv(m.convd1, 1, 64, 7) and _is_conv(m.convd2, 64, 64, 3) and _is_conv(m.conv, 128, 127, 3)
+                and route_ok(disp.shape[-1]))
+
+    def __call__(self, disp, corr):
+        self._ensure(disp.device)
+        mon = ops.TcOverflowMonitor.get(disp.device)
+        mon.check()
+        dtype = torch.promote_types(_conv_dtype(disp, corr), disp.dtype)        # the reference's torch.cat([out, disp])
+        d = _f32(disp)
+        cor = ops.conv3d_1x1(_f32(corr), self.c1, None, self.bc1, act=ops.ACT_RELU)
+        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), self.c2, None, self.bc2, act=ops.ACT_RELU)
+        dsp = ops.dwconv2d(d.expand(-1, 64, -1, -1).contiguous(), self.d1, None, self.bd1, act=ops.ACT_RELU)
+        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), self.d2, None, self.bd2, act=ops.ACT_RELU)
+        part = ops.conv2d_k3_tc(cor, self.wc, None, self.b)
+        out = ops.conv2d_k3_tc(dsp, self.wd, None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
+        out[:, 127:].copy_(d)
+        mon.poll()
+        return out.to(dtype)
+
+
+class DispHeadEngine(_Engine):
+    """DispHead.forward(x) = conv2(relu(conv1(x))) on the library (module docstring)."""
+
+    def _pack(self):
+        m = self.module
+        w, b = m.conv1.weight, _bias(m.conv1)
+        self.w1 = [ops.pack_tc_weight_2d(w[:128], 16), ops.pack_tc_weight_2d(w[128:], 16)]
+        self.b1 = [b[:128].contiguous(), b[128:].contiguous()]
+        w5 = m.conv2.weight.detach().float().new_zeros(1, 256, 3, 3, 3)
+        w5[:, :, 1] = m.conv2.weight.detach().float()                          # 2D taps at kd = 1 of a D = 1 volume
+        self.w2, self.b2 = [ops.pack_conv_weight(w5[:, :128]), ops.pack_conv_weight(w5[:, 128:])], _bias(m.conv2)
+
+    def serves(self, x):
+        m = self.module
+        return (x.dim() == 4 and _is_conv(m.conv1, x.shape[1], 256, 3) and x.shape[1] == 128 and _is_conv(m.conv2, 256, 1, 3)
+                and route_ok(x.shape[-1]))
+
+    def __call__(self, x):
+        self._ensure(x.device)
+        mon = ops.TcOverflowMonitor.get(x.device)
+        mon.check()
+        dtype = _conv_dtype(x)
+        xn = ops.nchw_to_nhwc_cat([_f32(x)])
+        h0 = ops.conv2d_k3_tc(xn, self.w1[0], None, self.b1[0], act=ops.ACT_RELU, out_nhwc=False)
+        h1 = ops.conv2d_k3_tc(xn, self.w1[1], None, self.b1[1], act=ops.ACT_RELU, out_nhwc=False)
+        y = ops.conv3d_k3(h0.unsqueeze(2), self.w2[0], None, self.b2)
+        y = ops.conv3d_k3(h1.unsqueeze(2), self.w2[1], None, None, y).squeeze(2)
+        mon.poll()
+        return y.to(dtype)
+
+
+class MaskFeatEngine(_Engine):
+    """mask_feat_4 = Sequential(Conv2d(128, 32, 3, padding=1), ReLU) on the library (module docstring)."""
+
+    def _pack(self):
+        self.w = {}                                                             # K chunk -> packed weight (W' = 128: 32, else 16)
+        self.b = _bias(self.module[0])
+
+    def serves(self, x):
+        m = self.module
+        return (len(m) == 2 and isinstance(m[1], torch.nn.ReLU) and x.dim() == 4 and x.shape[1] == 128 and _is_conv(m[0], 128, 32, 3)
+                and route_ok(x.shape[-1]))
+
+    def __call__(self, x):
+        self._ensure(x.device)
+        mon = ops.TcOverflowMonitor.get(x.device)
+        mon.check()
+        dtype = _conv_dtype(x)
+        kc = ops.conv2d_tc_kc(128, 32, x.shape[-1])
+        if kc not in self.w:
+            self.w[kc] = ops.pack_tc_weight_2d(self.module[0].weight, kc)
+        y = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([_f32(x)]), self.w[kc], None, self.b, act=ops.ACT_RELU, out_nhwc=False)
+        mon.poll()
+        return y.to(dtype)

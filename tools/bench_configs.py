@@ -25,6 +25,9 @@
   c10 the ConvGRUs of IGEVStereo (cfgs/igev AMP YAML @480x640) and StereoBase (cfgs/stereobase @256x512), batch 8 (the reference's
       classes + patch()): ms in the three ConvGRUs and per forward, patched / cuDNN fp32 / fp16 autocast in alternating rotation,
       the GRU stage's TFLOP/s and the EPE against the unpatched model  (python tools/bench_configs.py --only c10)
+  c11 the rest of the same update blocks (motion encoder, disp head, mask_feat_4), same models, shapes and rotation as c10: ms per
+      forward in each of the six update-block modules, the three new stages' TFLOP/s and the EPE against the unpatched model
+      (python tools/bench_configs.py --only c11)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -602,6 +605,108 @@ def c10(iters, B=8):
         torch.cuda.empty_cache()
 
 
+# MACs per 1/4-resolution pixel and call (igev/update.py:17-25,75-94,123-125): convc1 1x1 Cc -> 64, convc2 / convd2 3x3 64 -> 64,
+# convd1 7x7 1 -> 64, conv 3x3 128 -> 127; DispHead 3x3 128 -> 256 -> 1; mask_feat_4 3x3 128 -> 32
+_UPDATE_MACS = {"encoder": lambda cc: cc * 64 + 2 * 64 * 64 * 9 + 49 * 64 + 128 * 127 * 9,
+                "disp_head": lambda cc: 128 * 256 * 9 + 256 * 9, "mask_feat_4": lambda cc: 128 * 32 * 9}
+
+
+def _update_stages(run, block):
+    """One run of `run` with CUDA events around every call of the six update-block modules: {module: ms}, {module: MACs}."""
+    names = ("encoder", "disp_head", "mask_feat_4", "gru04", "gru08", "gru16")
+    events, macs = [], {n: 0 for n in _UPDATE_MACS}
+    mods = {n: getattr(block, n) for n in names}
+    saved = {n: vars(m).get("forward") for n, m in mods.items()}
+
+    def wrap(name, inner):
+        def fwd(*args):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            if name in _UPDATE_MACS:
+                x = args[-1]                                        # corr (encoder) or net0: (B, C, H, W)
+                macs[name] += _UPDATE_MACS[name](x.shape[1]) * x.shape[0] * x.shape[2] * x.shape[3]
+            a.record()
+            out = inner(*args)
+            b.record()
+            events.append((name, a, b))
+            return out
+        return fwd
+    for n, m in mods.items():
+        m.forward = wrap(n, m.forward)
+    try:
+        run()
+        torch.cuda.synchronize()
+    finally:
+        for n, m in mods.items():
+            if saved[n] is None:
+                del m.forward
+            else:
+                m.forward = saved[n]
+    ms = {n: 0.0 for n in names}
+    for n, a, b in events:
+        ms[n] += a.elapsed_time(b)
+    return ms, macs
+
+
+def c11(iters, B=8):
+    """The motion encoder, disp head and mask_feat_4 of IGEV-Stereo (cfgs/igev AMP YAML, 480x640) and StereoBase (cfgs/stereobase,
+    256x512), batch 8, the reference's classes: the variants of c10 (patch(), unpatched cuDNN fp32 with TF32 off, unpatched fp16
+    autocast) in alternating rotation, medians of three.  Per variant: whole-forward ms, ms in each update-block module (CUDA events
+    around every call), the three new stages' useful TFLOP/s (2 x the MACs of _UPDATE_MACS), EPE of each variant against fp32."""
+    from oracle import _reference_shim as shim
+    from openstereo_b200.patch import patch
+    shim.install_timm_stub()
+
+    def build(which):
+        if which == "igev":
+            cfg = shim.load_cfg("cfgs/igev/igev_sceneflow_amp.yaml").MODEL
+            m = shim.load("stereo.modeling.models.igev.igev_stereo").IGEVStereo(cfg).eval()
+            m.load_state_dict(si.seeded_state_dict(m.state_dict(), seed=12, scale={"classifier.weight": 8.0}))
+        else:
+            cfg = shim.load_cfg("cfgs/stereobase/stereobase_sceneflow.yaml").MODEL
+            m = shim.load("stereo.modeling.models.stereobase.stereobase_gru").StereoBase(cfg).eval()
+            m.load_state_dict(si.seeded_state_dict(m.state_dict(), seed=3, scale={"classifier.weight": 8.0}))
+        return m.to(DEV)
+
+    new = tuple(_UPDATE_MACS)
+    for which, name, (h, w) in (("igev", "IGEVStereo", (480, 640)), ("stereobase", "StereoBase", (256, 512))):
+        ref, pm = build(which), patch(build(which))
+        gen = torch.Generator().manual_seed(31)
+        x = {"left": (torch.rand(B, 3, h, w, generator=gen) * 255).to(DEV), "right": (torch.rand(B, 3, h, w, generator=gen) * 255).to(DEV)}
+        variants = {"patched": (pm, False), "cudnn_fp32": (ref, False), "amp_fp16": (ref, True)}
+
+        def fwd(m, amp):
+            with torch.autocast("cuda", dtype=torch.float16, enabled=amp):
+                return m(dict(x))["disp_pred"]
+        ms = {k: [] for k in variants}
+        stage = {k: [] for k in variants}
+        outs, macs = {}, {}
+        with torch.no_grad():
+            for _ in range(3):                                          # alternate: the three share the GPU's state
+                for k, (m, amp) in variants.items():
+                    t, outs[k] = timeit(lambda: fwd(m, amp), max(1, iters // 5), warm=1)
+                    ms[k].append(t)
+                    st, macs = _update_stages(lambda: fwd(m, amp), m.update_block)
+                    stage[k].append(st)
+        med = lambda v: sorted(v)[1]
+        stage_ms = {k: {n: round(med([s[n] for s in v]), 2) for n in v[0]} for k, v in stage.items()}
+        new_ms = {k: round(sum(v[n] for n in new), 2) for k, v in stage_ms.items()}
+        emit(config="c11 motion encoder + disp head + mask_feat_4 of %s, B=%d @%dx%d (reference class + patch())" % (name, B, h, w),
+             gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+             forward_ms={k: round(med(v), 2) for k, v in ms.items()},
+             stage_ms=stage_ms,
+             new_stages_ms=new_ms,
+             new_stages_gmac={n: round(v / 1e9, 1) for n, v in macs.items()},
+             new_stages_tflops_fp32_equivalent={k: {n: round(2 * macs[n] / (v[n] * 1e-3) / 1e12, 1) for n in new}
+                                                for k, v in stage_ms.items()},
+             new_stages_speedup_vs_cudnn_fp32=round(new_ms["cudnn_fp32"] / new_ms["patched"], 2),
+             new_stages_speedup_vs_amp_fp16=round(new_ms["amp_fp16"] / new_ms["patched"], 2),
+             epe_patched_vs_cudnn_fp32_px=float("%.3e" % (outs["patched"] - outs["cudnn_fp32"]).abs().mean().item()),
+             epe_amp_vs_cudnn_fp32_px=float("%.3e" % (outs["amp_fp16"].float() - outs["cudnn_fp32"]).abs().mean().item()),
+             disparity_std_px=round(outs["cudnn_fp32"].std().item(), 2))
+        del ref, pm
+        torch.cuda.empty_cache()
+
+
 def _stage_times(run, targets, volume_fn=None):
     """One run of `run` with CUDA events around the forward of each target (a module, or a class whose __call__ is wrapped) and,
     with volume_fn, around ops.<volume_fn>: {stage: ms}."""
@@ -658,7 +763,7 @@ if __name__ == "__main__":
     a = ap.parse_args()
     for name in a.only.split(","):
         try:
-            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10}[name](a.iters)
+            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:
