@@ -385,6 +385,18 @@ int osb_geo_lookup_fwd(const float* geo0, const float* geo1, const float* geo2, 
  * disp (B,1,H,W), out (B, num_levels*C*T, H, W).  Unused level pointers are NULL. */
 int osb_geo_volume_lookup_fwd(const float* geo0, const float* geo1, const float* geo2, const float* geo3, const float* disp,
                               float* out, int B, int C, int D, int H, int W, int num_levels, int radius, osb_stream_t stream);
+/* IGEV++'s multi-range Combined_Geo_Encoding_Volume.__call__ (igevpp/geometry.py:35-77) in one launch, T = 2*radius+1:
+ *   geo_i (B, C, D0>>i, H, W), i < num_levels, at d = dx + disp/2^i   -> out0     (B, num_levels*C*T, H, W), [i*C*T + c*T + k]
+ *   vol1  (B, C, D1, H, W)  at d = dx + disp/2                          -> out1     (B, C*T, H, W),            [c*T + k]
+ *   vol2  (B, C, D2, H, W)  at d = dx + disp/4                          -> out2     (B, C*T, H, W),            [c*T + k]
+ *   corr_i (B, H, W, W2>>i) at x = coords/2^i - disp/2^i + dx           -> out_corr (B, num_levels*T, H, W),   [i*T + k]
+ * geo_i is the pair-averaged pyramid of the first volume; D1 and D2 are independent of D0.  disp (B,1,H,W), coords (B,H,W).
+ * Unused level pointers are NULL. */
+int osb_geo_multirange_lookup_fwd(const float* geo0, const float* geo1, const float* geo2, const float* geo3, const float* vol1,
+                                  const float* vol2, const float* corr0, const float* corr1, const float* corr2, const float* corr3,
+                                  const float* disp, const float* coords, float* out0, float* out1, float* out2, float* out_corr,
+                                  int B, int C, int D0, int D1, int D2, int H, int W, int W2, int num_levels, int radius,
+                                  osb_stream_t stream);
 /* context_upsample (stereobase/igev_blocks.py:51-63, igev/submodule.py:253-265): disp_low (B,1,h,w), up_weights
  * (B,9,scale*h,scale*w) -> out (B, scale*h, scale*w) = sum over the 3x3 low-resolution neighbourhood (zero padded). */
 int osb_context_upsample_fwd(const float* disp_low, const float* up_weights, float* out, int B, int h, int w, int scale,

@@ -51,6 +51,7 @@ SIGNATURES = {
     "osb_avgpool_pairs_fwd": [_f32p, _f32p, ctypes.c_longlong, _i, ctypes.c_longlong, _s],
     "osb_geo_lookup_fwd": [_f32p] * 11 + [_i] * 8 + [_s],
     "osb_geo_volume_lookup_fwd": [_f32p] * 6 + [_i] * 7 + [_s],
+    "osb_geo_multirange_lookup_fwd": [_f32p] * 16 + [_i] * 10 + [_s],
     "osb_context_upsample_fwd": [_f32p] * 3 + [_i] * 4 + [_s],
     "osb_conv2d_tc_kc": [_i] * 4,
     "osb_conv2d_k3_tc_fwd": [_f32p] * 6 + [_i] * 9 + [_s],

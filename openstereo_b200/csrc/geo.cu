@@ -24,8 +24,16 @@ struct GeoParams {
   const float* corr[GEO_MAX_LEVELS];   // level i: (B, H, W, W2 >> i); all NULL = geometry-only lookup (no correlation row)
   const float* disp;                   // (B, 1, H, W)
   const float* coords;                 // (B, H, W) left-image x coordinate of every pixel (unused when geometry-only)
-  float* out;                          // (B, L * (C + 1) * (2r + 1), H, W), geometry-only (B, L * C * (2r + 1), H, W)
-  int B, C, D, H, W, W2, levels, radius;
+  float* out;                          // (B, L * (C + 1) * (2r + 1), H, W), geometry-only (B, L * C * (2r + 1), H, W),
+                                       // multi-range (B, L * C * (2r + 1), H, W): the geo_volume0 pyramid rows only
+  // multi-range mode (IGEV++'s Combined_Geo_Encoding_Volume), on when out_corr != NULL: two more single-level volumes, each
+  // with its own plane count, sampled at dx + disp / 2 and dx + disp / 4, and the correlation rows in a tensor of their own
+  const float* vol1;                   // (B, C, D1, H, W)
+  const float* vol2;                   // (B, C, D2, H, W)
+  float* out1;                         // (B, C * (2r + 1), H, W)
+  float* out2;                         // (B, C * (2r + 1), H, W)
+  float* out_corr;                     // (B, L * (2r + 1), H, W)
+  int B, C, D, H, W, W2, levels, radius, D1, D2;
 };
 
 // The reference turns a pixel coordinate into a normalised grid value and grid_sample turns it back
@@ -52,40 +60,65 @@ __device__ __forceinline__ float lerp_row(const float* __restrict__ row, size_t 
 // tap picks its two samples from registers; a tap whose floor() does not land on window slot k (possible only when the
 // coordinate round trip moves it across an integer) falls back to a direct read.  RADIUS = 0 is the generic path.  With
 // corr[0] == NULL (IGEV-RT's Geo_Encoding_Volume) a level has only its C geometry rows: a runtime mode, not an instantiation.
+// With out_corr != NULL (IGEV++'s multi-range Combined_Geo_Encoding_Volume) a batch item has L*C rows of the geo[] pyramid, C rows
+// of vol1, C rows of vol2 and L correlation rows, each written to its own output tensor: a third runtime mode.
 template <int RADIUS>
 __global__ void __launch_bounds__(128) geo_lookup_kernel(const GeoParams p) {
   const int w = blockIdx.x * 128 + threadIdx.x;
   const int h = blockIdx.y;
-  const int rows = p.corr[0] != nullptr ? p.C + 1 : p.C;
-  const int b = blockIdx.z / (p.levels * rows), lr = blockIdx.z % (p.levels * rows);
-  const int lvl = lr / rows, c = lr % rows;
   if (w >= p.W) return;
   const size_t hw = (size_t)p.H * p.W, pix = (size_t)h * p.W + w;
-  const float disp = __ldg(p.disp + (size_t)b * hw + pix);
   const int radius = RADIUS > 0 ? RADIUS : p.radius;
   const int taps = 2 * radius + 1;
-  const float scale = 1.f / (float)(1 << lvl);         // exact
-  const float dq = disp * scale;                       // disp / 2^lvl, exact
+  // this thread's row: batch item b, pyramid level lvl, sampled at disp / 2^shift; geometry channel c of a volume of len planes
+  // (vol1 / vol2 when src > 0), or the correlation row of level lvl
+  int b, lvl, c, shift, src = 0;
+  bool is_corr;
+  float* o;
+  if (p.out_corr == nullptr) {
+    const int rows = p.corr[0] != nullptr ? p.C + 1 : p.C;
+    b = blockIdx.z / (p.levels * rows);
+    const int lr = blockIdx.z % (p.levels * rows);
+    lvl = lr / rows, c = lr % rows, shift = lvl, is_corr = c == p.C;
+    o = p.out + (((size_t)b * p.levels + lvl) * rows * taps + (size_t)c * taps) * hw + pix;
+  } else {
+    const int rows = p.levels * p.C + 2 * p.C + p.levels;
+    b = blockIdx.z / rows;
+    int r = blockIdx.z % rows;
+    if (r < p.levels * p.C) {                          // geo_feat0: level, then channel, then tap
+      lvl = r / p.C, c = r % p.C, shift = lvl, is_corr = false;
+      o = p.out + (((size_t)b * p.levels + lvl) * p.C + c) * taps * hw + pix;
+    } else if ((r -= p.levels * p.C) < 2 * p.C) {      // geo_feat1 at disp / 2, geo_feat2 at disp / 4
+      lvl = 0, c = r % p.C, src = 1 + r / p.C, shift = src, is_corr = false;
+      o = (src == 1 ? p.out1 : p.out2) + ((size_t)b * p.C + c) * taps * hw + pix;
+    } else {                                           // init_corr
+      lvl = r - 2 * p.C, c = 0, shift = lvl, is_corr = true;
+      o = p.out_corr + ((size_t)b * p.levels + lvl) * taps * hw + pix;
+    }
+  }
+  const float disp = __ldg(p.disp + (size_t)b * hw + pix);
+  const float scale = 1.f / (float)(1 << shift);       // exact
+  const float dq = disp * scale;                       // disp / 2^shift, exact
   const float* row;
   size_t stride;
   int len;
   float base;                                          // tap k samples at base + (k - radius): the reference adds dx + base for
                                                        // the geometry rows and base + dx for the correlation (same fp32 sum)
   // constant indices only: a runtime index would make the compiler copy the pointer arrays to local memory
-  const float* geo = lvl == 0 ? p.geo[0] : lvl == 1 ? p.geo[1] : lvl == 2 ? p.geo[2] : p.geo[3];
-  const float* corr = lvl == 0 ? p.corr[0] : lvl == 1 ? p.corr[1] : lvl == 2 ? p.corr[2] : p.corr[3];
-  if (c < p.C) {
-    len = p.D >> lvl;
+  if (!is_corr) {
+    const float* geo = src == 1 ? p.vol1 : src == 2 ? p.vol2
+                     : lvl == 0 ? p.geo[0] : lvl == 1 ? p.geo[1] : lvl == 2 ? p.geo[2] : p.geo[3];
+    len = src == 1 ? p.D1 : src == 2 ? p.D2 : p.D >> lvl;
     row = geo + ((size_t)b * p.C + c) * len * hw + pix;
     stride = hw;
     base = dq;                                         // geometry.py:22-26 adds dx + disp / 2^i: the same fp32 sum
   } else {
+    const float* corr = lvl == 0 ? p.corr[0] : lvl == 1 ? p.corr[1] : lvl == 2 ? p.corr[2] : p.corr[3];
     len = p.W2 >> lvl;
     row = corr + ((size_t)b * hw + pix) * len;
     stride = 1;
     base = __fsub_rn(__ldg(p.coords + (size_t)b * hw + pix) * scale, dq);            // coords / 2^lvl - disp / 2^lvl
   }
-  float* o = p.out + (((size_t)b * p.levels + lvl) * rows * taps + (size_t)c * taps) * hw + pix;
   if (RADIUS > 0) {
     constexpr int T = 2 * RADIUS + 1;
     const float x0 = roundtrip(__fadd_rn((float)(-RADIUS), base), len);
@@ -228,6 +261,39 @@ int osb_geo_volume_lookup_fwd(const float* geo0, const float* geo1, const float*
   OSB_REQUIRE((long long)B * num_levels * C <= 65535, "geo_volume_lookup: B * levels * C must fit a grid dimension");
   dim3 grid((W + 127) / 128, H, B * num_levels * C);
   if (radius == 4) geo_lookup_kernel<4><<<grid, 128, 0, (cudaStream_t)stream>>>(p);      // IGEV-RT default (CORR_RADIUS 4)
+  else geo_lookup_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(p);
+  count_launch();
+  return check_launch("geo_lookup_kernel");
+}
+
+int osb_geo_multirange_lookup_fwd(const float* geo0, const float* geo1, const float* geo2, const float* geo3, const float* vol1,
+                                  const float* vol2, const float* corr0, const float* corr1, const float* corr2, const float* corr3,
+                                  const float* disp, const float* coords, float* out0, float* out1, float* out2, float* out_corr,
+                                  int B, int C, int D0, int D1, int D2, int H, int W, int W2, int num_levels, int radius,
+                                  osb_stream_t stream) {
+  using namespace osb;
+  OSB_REQUIRE(vol1 && vol2 && disp && coords && out0 && out1 && out2 && out_corr, "geo_multirange_lookup: null pointer");
+  OSB_REQUIRE(B > 0 && C > 0 && D0 > 0 && D1 > 0 && D2 > 0 && H > 0 && W > 0 && W2 > 0, "geo_multirange_lookup: empty shape");
+  OSB_REQUIRE(num_levels >= 1 && num_levels <= GEO_MAX_LEVELS, "geo_multirange_lookup: num_levels %d outside 1..%d", num_levels,
+              GEO_MAX_LEVELS);
+  OSB_REQUIRE(radius >= 0 && radius <= 16, "geo_multirange_lookup: radius %d outside 0..16", radius);
+  OSB_REQUIRE((D0 >> (num_levels - 1)) >= 2 && (W2 >> (num_levels - 1)) >= 2 && D1 >= 2 && D2 >= 2,
+              "geo_multirange_lookup: a volume or pyramid level shorter than 2 samples");
+  OSB_REQUIRE(H <= 65535 && B <= 65535, "geo_multirange_lookup: H and B must fit a grid dimension");
+  OSB_REQUIRE((long long)B * (num_levels * C + 2 * C + num_levels) <= 65535,
+              "geo_multirange_lookup: B * (levels * C + 2 * C + levels) must fit a grid dimension");
+  GeoParams p{};
+  const float* g[GEO_MAX_LEVELS] = {geo0, geo1, geo2, geo3};
+  const float* c[GEO_MAX_LEVELS] = {corr0, corr1, corr2, corr3};
+  for (int i = 0; i < num_levels; ++i) {
+    OSB_REQUIRE(g[i] && c[i], "geo_multirange_lookup: pyramid level %d is null", i);
+    p.geo[i] = g[i], p.corr[i] = c[i];
+  }
+  p.vol1 = vol1, p.vol2 = vol2, p.disp = disp, p.coords = coords;
+  p.out = out0, p.out1 = out1, p.out2 = out2, p.out_corr = out_corr;                    // out_corr != NULL: the multi-range mode
+  p.B = B, p.C = C, p.D = D0, p.D1 = D1, p.D2 = D2, p.H = H, p.W = W, p.W2 = W2, p.levels = num_levels, p.radius = radius;
+  dim3 grid((W + 127) / 128, H, B * (num_levels * C + 2 * C + num_levels));
+  if (radius == 4) geo_lookup_kernel<4><<<grid, 128, 0, (cudaStream_t)stream>>>(p);      // IGEV++ default (CORR_RADIUS 4)
   else geo_lookup_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(p);
   count_launch();
   return check_launch("geo_lookup_kernel");

@@ -1067,6 +1067,42 @@ def geo_volume_lookup(geo_levels, disp, radius):
     return out
 
 
+def geo_multirange_lookup(geo_levels, vol1, vol2, corr_levels, disp, coords, radius):
+    """One lookup of IGEV++'s multi-range encoding volume (igevpp/geometry.py:35-77), one launch: geo_levels[i] (B,C,D0>>i,H,W),
+    vol1 (B,C,D1,H,W), vol2 (B,C,D2,H,W), corr_levels[i] (B,H,W,W2>>i), disp (B,1,H,W), coords (B,H,W[,1]) ->
+    (geo_feat0 (B, L*C*T, H, W), geo_feat1 (B, C*T, H, W) at disp/2, geo_feat2 (B, C*T, H, W) at disp/4, init_corr (B, L*T, H, W)),
+    T = 2r+1, fp32 whatever the input dtype."""
+    levels = len(geo_levels)
+    if not (1 <= levels <= 4 and levels == len(corr_levels)):
+        raise ValueError("geo_multirange_lookup: 1..4 pyramid levels of both the volume and the correlation expected")
+    geo = [_prep(g, "geo_multirange_lookup")[0] for g in geo_levels]
+    corr = [_prep(cr, "geo_multirange_lookup")[0] for cr in corr_levels]
+    (v1, _), (v2, _) = _prep(vol1, "geo_multirange_lookup"), _prep(vol2, "geo_multirange_lookup")
+    disp, _ = _prep(disp, "geo_multirange_lookup")
+    b, c, d0, h, w = geo[0].shape
+    coords, _ = _prep(coords.reshape(b, h, w), "geo_multirange_lookup")
+    w2 = corr[0].shape[-1]
+    for i in range(levels):
+        if tuple(geo[i].shape) != (b, c, d0 >> i, h, w) or tuple(corr[i].shape) != (b, h, w, w2 >> i):
+            raise ValueError("geo_multirange_lookup: pyramid level %d has shape %s / %s" % (i, tuple(geo[i].shape), tuple(corr[i].shape)))
+    if v1.shape[:2] != (b, c) or v1.shape[3:] != (h, w) or v2.shape[:2] != (b, c) or v2.shape[3:] != (h, w):
+        raise ValueError("geo_multirange_lookup: range volumes %s / %s do not match %s" % (tuple(v1.shape), tuple(v2.shape), (b, c, h, w)))
+    if tuple(disp.shape) != (b, 1, h, w):
+        raise ValueError("geo_multirange_lookup: disp has shape %s, expected %s" % (tuple(disp.shape), (b, 1, h, w)))
+    _same_device(*geo, *corr, v1, v2, disp, coords)
+    t = 2 * radius + 1
+    out0 = torch.empty((b, levels * c * t, h, w), dtype=torch.float32, device=disp.device)
+    out1 = torch.empty((b, c * t, h, w), dtype=torch.float32, device=disp.device)
+    out2 = torch.empty((b, c * t, h, w), dtype=torch.float32, device=disp.device)
+    out_corr = torch.empty((b, levels * t, h, w), dtype=torch.float32, device=disp.device)
+    gp = [geo[i].data_ptr() if i < levels else None for i in range(4)]
+    cp = [corr[i].data_ptr() if i < levels else None for i in range(4)]
+    _call("osb_geo_multirange_lookup_fwd", *gp, v1.data_ptr(), v2.data_ptr(), *cp, disp.data_ptr(), coords.data_ptr(),
+          out0.data_ptr(), out1.data_ptr(), out2.data_ptr(), out_corr.data_ptr(), b, c, d0, v1.shape[2], v2.shape[2], h, w, w2, levels,
+          radius, _stream(out0))
+    return out0, out1, out2, out_corr
+
+
 def context_upsample(disp_low, up_weights, scale_factor=4):
     """stereobase/igev_blocks.py:51-63: disp_low (B,1,h,w), up_weights (B,9,s*h,s*w) -> (B, s*h, s*w)."""
     assert disp_low.is_cuda and disp_low.dim() == 4 and disp_low.shape[1] == 1

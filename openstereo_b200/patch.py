@@ -1,5 +1,5 @@
 """patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / IGEV-RT /
-CoEx / MSNet3D, and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
+IGEV++ / CoEx / MSNet3D, and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
 hot path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each
@@ -11,6 +11,8 @@ needs its own rebinding:
               aggregator + FasterSoftArgmin modules                          -> ``CostProcessor.forward`` / ``FasterSoftArgmin.forward``
 * LightStereo / IGEVStereo  like StereoBase: names imported into lightstereo.py:4-6 / igev_stereo.py:1-3 (``from .submodule import *``)
 * IGEV-RT     like IGEVStereo (igev_rt_stereo.py:1-6), plus per-instance ``cost_agg`` / ``classifier`` forward overrides
+* IGEV++      like IGEVStereo (igevpp_stereo.py:4-8), plus a per-instance ``classifier`` forward override and the update block's
+              ``gru04 / gru08 / gru16 / encoder / geo_encoder0..2 / disp_head / mask_feat_4`` forward overrides
 * CasStereo   ``get_cv`` (GetCostVolume) and ``cost_agg[i]`` (CostAggregation) modules  -> per-instance ``forward`` overrides
 * CoEx        ``CostProcessor`` / ``DispProcessor`` / ``DispProcessor.regression`` modules -> per-instance ``forward`` overrides
 * MSNet3D     one monolithic ``forward`` (MSNet3D.py:110-161), no processor modules   -> per-instance ``model.forward`` override that
@@ -37,7 +39,7 @@ import torch
 
 from . import ops
 from .aggregation import CascadeAggregation, GwcAggregation, PSMAggregation, StereoBaseAggregation, StereoBaseCostHead
-from .geo import CombinedGeoEncodingVolume, GeoEncodingVolume
+from .geo import CombinedGeoEncodingVolume, GeoEncodingVolume, MultiRangeGeoEncodingVolume
 
 
 def _tensors(args):
@@ -441,6 +443,62 @@ def _patch_igev_rt(model, strict, backbone=True):
     return model
 
 
+def _patch_igevpp(model, strict, backbone=True):
+    """IGEV++ (igevpp/igevpp_stereo.py:162-249, class IGEVPPStereo): the gwc volume, the classifier Conv3d(8 -> 1) of the three
+    disparity ranges (``classifier.forward``, which returns logits: the reference's own softmax follows), the strided regressions of
+    the three initial disparities, the per-GRU-iteration multi-range lookup (one launch), the update block's ConvGRUs, geometry
+    encoders, disparity encoder, disparity head and mask head, and the convex up-sampling.  The instance-normalised hourglasses,
+    patch0 / patch1, the feature nets, cnet, selective_conv, disp_conv and BasicMultiUpdateBlock.forward itself (the selective-weight
+    blend, cat, pool2x, interp) stay the reference's code; `backbone` has no effect.  Under autocast (the AMP YAML) every call
+    computes in fp32 and returns the reference's dtypes."""
+    g = type(model).forward.__globals__
+    orig = {n: g[n] for n in ("build_gwc_volume", "disparity_regression", "Combined_Geo_Encoding_Volume", "context_upsample")}
+
+    def gwc(ref, tgt, maxdisp, groups):
+        if _accelerable(model, ref, tgt):
+            return ops.build_gwc_volume(ref, tgt, maxdisp, groups)
+        return orig["build_gwc_volume"](ref, tgt, maxdisp, groups) if not strict else _refuse("build_gwc_volume")
+
+    def regression(prob, maxdisp, interval):
+        if _accelerable(model, prob):
+            return ops.disparity_regression_interval(prob, maxdisp, interval)
+        return orig["disparity_regression"](prob, maxdisp, interval) if not strict else _refuse("disparity_regression")
+
+    def geo_factory(geo_volume0, geo_volume1, geo_volume2, init_fmap1, init_fmap2, radius=4, num_levels=2):
+        fast = _accelerable(model, geo_volume0, geo_volume1, geo_volume2, init_fmap1, init_fmap2)
+        if not fast and strict:
+            _refuse("Combined_Geo_Encoding_Volume")
+        cls = MultiRangeGeoEncodingVolume if fast else orig["Combined_Geo_Encoding_Volume"]
+        return cls(geo_volume0, geo_volume1, geo_volume2, init_fmap1, init_fmap2, radius=radius, num_levels=num_levels)
+
+    def upsample(disp_low, up_weights):                               # IGEV++'s version keeps dim 1: (B, 1, 4h, 4w)
+        if _accelerable(model, disp_low, up_weights):
+            return ops.context_upsample(disp_low, up_weights, 4).unsqueeze(1).to(disp_low.dtype)
+        return orig["context_upsample"](disp_low, up_weights) if not strict else _refuse("context_upsample")
+
+    _rebind_methods(model, {"build_gwc_volume": gwc, "disparity_regression": regression, "Combined_Geo_Encoding_Volume": geo_factory,
+                            "context_upsample": upsample})
+
+    cls_mod = model.classifier
+    cls_orig, head = cls_mod.forward, StereoBaseCostHead(cls_mod)
+
+    def cls_forward(self, x):
+        if not _accelerable(self, x):
+            return cls_orig(x) if not strict else _refuse("IGEV++ classifier")
+        return head.logits(x).to(x.dtype)
+
+    cls_mod.forward = types.MethodType(cls_forward, cls_mod)
+
+    from .update import DispEncoderEngine, DispHeadEngine, GeoEncoderEngine, MaskFeatEngine
+    block = model.update_block
+    _patch_convgru(block, strict)
+    for name, cls in (("encoder", DispEncoderEngine), ("geo_encoder0", GeoEncoderEngine), ("geo_encoder1", GeoEncoderEngine),
+                      ("geo_encoder2", GeoEncoderEngine), ("disp_head", DispHeadEngine), ("mask_feat_4", MaskFeatEngine)):
+        mod = getattr(block, name)
+        _override_engine(mod, cls(mod), strict, name)
+    return model
+
+
 def _patch_cascade(model, strict, backbone=True):
     """CasStereo (casnet/cas_psm.py PSMNet = CasPSMNet, casnet/cas_gwc.py GwcNet = CasGwcNet): every stage's warped cost volume
     (``get_cv.forward``) and every stage's aggregation + hypothesis-weighted soft-argmin (``cost_agg[i].forward``).  The FPN
@@ -571,7 +629,8 @@ def _patch_msnet3d(model, strict, backbone=True):
 _CASCADE_MODULES = {("casnet", "cas_psm"): "PSMNet", ("casnet", "cas_gwc"): "GwcNet"}
 
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
-             "IGEVStereo": _patch_igev, "IGEVRTtereo": _patch_igev_rt, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
+             "IGEVStereo": _patch_igev, "IGEVRTtereo": _patch_igev_rt,
+             "IGEVPPStereo": _patch_igevpp, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
 
 
 def patch(model, strict=True, backbone=True):

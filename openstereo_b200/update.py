@@ -13,7 +13,11 @@ mask_feat_4 (igev/update.py:123-125 == gru_blocks.py:304-306).  The 3x3 layers r
     DispHeadEngine       net0 (B,128,H,W) -> (B,1,H,W)
         one channels-last pack; conv1 + bias + relu as two Cout 128 launches (one per half of its 256 channels, NCHW);
         conv2 + bias as two osb_conv3d_k3_bn_act_fwd launches (D = 1), the second adding the first as its residual
-    MaskFeatEngine       net0 -> (B,32,H,W): one pack, one Cout 32 launch with bias + relu and NCHW output
+    MaskFeatEngine       net0 -> (B,Cout,H,W): one pack, one Cout 32 (IGEV, StereoBase) or Cout 64 (IGEV++) launch with bias + relu
+                         and NCHW output
+
+IGEV++'s update block (igevpp/update.py) adds GeoEncoderEngine (geo_encoder0/1/2) and DispEncoderEngine (encoder); its ConvGRUs and
+disparity head are IGEV's modules and run on gru.ConvGRUEngine and DispHeadEngine as they are.
 
 patch.py installs them as per-instance forward overrides of update_block.encoder / disp_head / mask_feat_4 and runs the reference's
 own forward for every shape or hyper-parameter no kernel serves (route_ok, the engines' serves()).
@@ -127,25 +131,119 @@ class DispHeadEngine(_Engine):
 
 
 class MaskFeatEngine(_Engine):
-    """mask_feat_4 = Sequential(Conv2d(128, 32, 3, padding=1), ReLU) on the library (module docstring)."""
+    """mask_feat_4 = Sequential(Conv2d(128, Cout, 3, padding=1), ReLU) on the library (module docstring): Cout 32 (IGEV-Stereo,
+    StereoBase) or 64 (IGEV++)."""
 
     def _pack(self):
-        self.w = {}                                                             # K chunk -> packed weight (W' = 128: 32, else 16)
+        self.w = {}                                                             # K chunk -> packed weight (Cout 32 at W' = 128: 32, else 16)
         self.b = _bias(self.module[0])
 
     def serves(self, x):
         m = self.module
-        return (len(m) == 2 and isinstance(m[1], torch.nn.ReLU) and x.dim() == 4 and x.shape[1] == 128 and _is_conv(m[0], 128, 32, 3)
-                and route_ok(x.shape[-1]))
+        cout = getattr(m[0], "out_channels", 0) if len(m) else 0
+        return (len(m) == 2 and isinstance(m[1], torch.nn.ReLU) and x.dim() == 4 and x.shape[1] == 128 and cout in (32, 64)
+                and _is_conv(m[0], 128, cout, 3) and route_ok(x.shape[-1]) and ops.conv2d_tc_kc(128, cout, x.shape[-1]) != 0)
 
     def __call__(self, x):
         self._ensure(x.device)
         mon = ops.TcOverflowMonitor.get(x.device)
         mon.check()
         dtype = _conv_dtype(x)
-        kc = ops.conv2d_tc_kc(128, 32, x.shape[-1])
+        kc = ops.conv2d_tc_kc(128, self.module[0].out_channels, x.shape[-1])
         if kc not in self.w:
             self.w[kc] = ops.pack_tc_weight_2d(self.module[0].weight, kc)
         y = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([_f32(x)]), self.w[kc], None, self.b, act=ops.ACT_RELU, out_nhwc=False)
         mon.poll()
         return y.to(dtype)
+
+
+def _tc_serves(w, *shapes):
+    """True when a wgmma instantiation serves every (Cin, Cout) 3x3 layer at image width w.  For the shapes of the IGEV++ engines
+    (Cout 32 or 128) that is W >= OSB_TC_MIN_WIDTH."""
+    return all(ops.conv2d_tc_kc(cin, cout, w) != 0 for cin, cout in shapes)
+
+
+def _pad_rows(w, rows):
+    """(Cout, Cin, k, k) -> (rows, Cin, k, k): zero output channels appended (they compute exact zeros)."""
+    return torch.cat((w, w.new_zeros((rows - w.shape[0],) + tuple(w.shape[1:]))), 0)
+
+
+class GeoEncoderEngine(_Engine):
+    """IGEV++'s GeoEncoder.forward(geo) = convg2(relu(convg1(geo))) (igevpp/update.py:72-80) on the library:
+
+        x = relu(convg1(geo))       osb_conv3d_1x1_bn_act_fwd on the lookup's NCHW output, in place (geo_planes -> 128)
+        y = convg2(x)               one channels-last pack, one Cout-128 wgmma launch with NCHW output: the 128 -> 96 weight and bias
+                                    are zero-padded to 128 rows (there is no Cout-96 instantiation at W' = 128 or at general widths)
+        return y[:, :96]            a view; channels 96..127 are exact zeros
+    """
+
+    def _pack(self):
+        m = self.module
+        self.g1, self.bg1 = m.convg1.weight.detach().float()[:, :, 0, 0].t().contiguous(), _bias(m.convg1)     # (Cin, 128)
+        self.g2, self.bg2 = ops.pack_tc_weight_2d(_pad_rows(m.convg2.weight.detach().float(), 128), 16), _bias(m.convg2, 128)
+
+    def serves(self, geo):
+        m = self.module
+        return (geo.dim() == 4 and _is_conv(m.convg1, geo.shape[1], 128, 1) and _is_conv(m.convg2, 128, 96, 3)
+                and _tc_serves(geo.shape[-1], (128, 128)))
+
+    def __call__(self, geo):
+        self._ensure(geo.device)
+        mon = ops.TcOverflowMonitor.get(geo.device)
+        mon.check()
+        dtype = _conv_dtype(geo)
+        x = ops.conv3d_1x1(_f32(geo), self.g1, None, self.bg1, act=ops.ACT_RELU)
+        y = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([x]), self.g2, None, self.bg2, out_nhwc=False)
+        mon.poll()
+        return y[:, :96].to(dtype)
+
+
+class DispEncoderEngine(_Engine):
+    """IGEV++'s BasicDispEncoder.forward(disp, corr) (igevpp/update.py:82-100) on the library, MotionEncoderEngine's plan at IGEV++'s
+    widths:
+
+        cor  = relu(convc2(relu(convc1(corr))))     convc1 (Cc -> 128) on the CUDA-core 1x1 from the NCHW input, pack, convc2
+                                                    (128 -> 96) padded to 128 output channels (exact zeros), kept channels-last
+        dsp  = relu(convd2(relu(convd1(disp))))     convd1 (7x7, 1 -> 32) as the depthwise kernel over disp broadcast to 32 planes,
+                                                    pack, convd2 (32 -> 32) on the Cout-32 wgmma kernels
+        part = conv(cor, W[:, :96] | 0) + b         conv's weight padded from 127 to 128 output channels; the cor half gets zero
+                                                    columns for cor's 32 pad channels
+        out  = relu(conv(dsp, W[:, 96:]) + part)    NCHW output with the channels-last residual: relu(conv(cat(cor, dsp)))
+        out[:, 127] = disp                          the reference's torch.cat([out, disp])
+    """
+
+    def _pack(self):
+        m = self.module
+        self.c1, self.bc1 = m.convc1.weight.detach().float()[:, :, 0, 0].t().contiguous(), _bias(m.convc1)     # (Cin, 128)
+        self.c2, self.bc2 = ops.pack_tc_weight_2d(_pad_rows(m.convc2.weight.detach().float(), 128), 16), _bias(m.convc2, 128)
+        self.d1, self.bd1 = m.convd1.weight.detach().float()[:, 0].contiguous(), _bias(m.convd1)            # (32, 7, 7)
+        self.d2, self.bd2 = {}, _bias(m.convd2)                                 # K chunk -> packed convd2 (W' = 128: 32, else 16)
+        w = _pad_rows(m.conv.weight.detach().float(), 128)                      # 127 -> 128 output channels, row 127 zero
+        wc = torch.cat((w[:, :96], w.new_zeros(128, 32, 3, 3)), 1)              # cor's pad channels 96..127 meet zero columns
+        self.wc, self.wd, self.b = ops.pack_tc_weight_2d(wc, 16), ops.pack_tc_weight_2d(w[:, 96:], 16), _bias(m.conv, 128)
+
+    def serves(self, disp, corr):
+        m = self.module
+        return (disp.dim() == 4 and corr.dim() == 4 and disp.shape[1] == 1 and disp.shape[0] == corr.shape[0]
+                and disp.shape[2:] == corr.shape[2:] and _is_conv(m.convc1, corr.shape[1], 128, 1) and _is_conv(m.convc2, 128, 96, 3)
+                and _is_conv(m.convd1, 1, 32, 7) and _is_conv(m.convd2, 32, 32, 3) and _is_conv(m.conv, 128, 127, 3)
+                and _tc_serves(disp.shape[-1], (128, 128), (32, 32), (32, 128)))
+
+    def __call__(self, disp, corr):
+        self._ensure(disp.device)
+        mon = ops.TcOverflowMonitor.get(disp.device)
+        mon.check()
+        dtype = torch.promote_types(_conv_dtype(disp, corr), disp.dtype)        # the reference's torch.cat([out, disp])
+        d = _f32(disp)
+        kc = ops.conv2d_tc_kc(32, 32, d.shape[-1])
+        if kc not in self.d2:
+            self.d2[kc] = ops.pack_tc_weight_2d(self.module.convd2.weight, kc)
+        cor = ops.conv3d_1x1(_f32(corr), self.c1, None, self.bc1, act=ops.ACT_RELU)
+        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), self.c2, None, self.bc2, act=ops.ACT_RELU)
+        dsp = ops.dwconv2d(d.expand(-1, 32, -1, -1).contiguous(), self.d1, None, self.bd1, act=ops.ACT_RELU)
+        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), self.d2[kc], None, self.bd2, act=ops.ACT_RELU)
+        part = ops.conv2d_k3_tc(cor, self.wc, None, self.b)
+        out = ops.conv2d_k3_tc(dsp, self.wd, None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
+        out[:, 127:].copy_(d)
+        mon.poll()
+        return out.to(dtype)

@@ -28,6 +28,9 @@
   c11 the rest of the same update blocks (motion encoder, disp head, mask_feat_4), same models, shapes and rotation as c10: ms per
       forward in each of the six update-block modules, the three new stages' TFLOP/s and the EPE against the unpatched model
       (python tools/bench_configs.py --only c11)
+  c12 IGEV++ (reference class + patch()), B=8 @256x512, 32 iterations: patched / cuDNN fp32 / AMP YAML / patched AMP YAML in
+      alternating rotation, ms per forward in the lookups, ConvGRUs, geo + disp encoders, heads and the rest, and the EPE against
+      the unpatched fp32 model  (python tools/bench_configs.py --only c12)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -707,6 +710,53 @@ def c11(iters, B=8):
         torch.cuda.empty_cache()
 
 
+def c12(iters, B=8, h=256, w=512):
+    """IGEV++ (igevpp/igevpp_stereo.py, the reference's class with the timm stand-in), batch 8 at 256x512 (W' = 128), 32 GRU
+    iterations.  Variants in alternating rotation, medians of three: patch() of the uniform-YAML model (fp32), the unpatched
+    uniform-YAML model (cuDNN fp32, TF32 off), the unpatched AMP-YAML model (the reference's own fp16 autocast) and patch() of the
+    AMP-YAML model.  Per variant: whole-forward ms and ms per forward in the lookups (CUDA events around every lookup call), the
+    three ConvGRUs, the three geo encoders + the disparity encoder, the disparity + mask heads, and everything else; EPE of each
+    variant against the unpatched fp32 model."""
+    from oracle import igevpp as oigpp
+    from openstereo_b200 import geo
+    from openstereo_b200.patch import patch
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    ref_geo = oigpp.load_reference("stereo.modeling.models.igevpp.geometry").Combined_Geo_Encoding_Volume
+    variants = {"patched": patch(oigpp.igevpp().to(DEV)), "cudnn_fp32": oigpp.igevpp().to(DEV),
+                "amp_fp16": oigpp.igevpp(oigpp.AMP_YAML).to(DEV), "patched_amp_yaml": patch(oigpp.igevpp(oigpp.AMP_YAML).to(DEV))}
+    gen = torch.Generator().manual_seed(31)
+    x = {"left": (torch.rand(B, 3, h, w, generator=gen) * 2 - 1).to(DEV), "right": (torch.rand(B, 3, h, w, generator=gen) * 2 - 1).to(DEV)}
+    groups = {"lookups": ("lookup",), "convgrus": ("gru04", "gru08", "gru16"),
+              "geo_and_disp_encoders": ("geo_encoder0", "geo_encoder1", "geo_encoder2", "encoder"), "heads": ("disp_head", "mask_feat_4")}
+    ms = {k: [] for k in variants}
+    stage = {k: [] for k in variants}
+    outs = {}
+    with torch.no_grad():
+        for _ in range(3):                                              # alternate: the variants share the GPU's state
+            for k, m in variants.items():
+                t, outs[k] = timeit(lambda: m(dict(x))["disp_pred"], max(1, iters // 5), warm=1)
+                ms[k].append(t)
+                ub = m.update_block
+                targets = {n: getattr(ub, n) for g in list(groups.values())[1:] for n in g}
+                targets["lookup"] = geo.MultiRangeGeoEncodingVolume if k.startswith("patched") else ref_geo
+                st = _stage_times(lambda: m(dict(x)), targets)
+                stage[k].append({g: sum(st.get(n, 0.0) for n in names) for g, names in groups.items()})
+    med = lambda v: sorted(v)[1]
+    stage_ms = {k: {g: round(med([s[g] for s in v]), 2) for g in groups} for k, v in stage.items()}
+    for k in stage_ms:
+        stage_ms[k]["everything_else"] = round(med(ms[k]) - sum(stage_ms[k][g] for g in groups), 2)
+    fp32 = outs["cudnn_fp32"].float()
+    emit(config="c12 IGEV++ refinement loop, B=%d @%dx%d, 32 iterations (reference class + patch())" % (B, h, w),
+         gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+         forward_ms={k: round(med(v), 2) for k, v in ms.items()},
+         stage_ms_per_forward=stage_ms,
+         epe_vs_cudnn_fp32_px={k: float("%.3e" % (o.float() - fp32).abs().mean().item()) for k, o in outs.items() if k != "cudnn_fp32"},
+         disparity_std_px=round(fp32.std().item(), 2))
+    del variants
+    torch.cuda.empty_cache()
+
+
 def _stage_times(run, targets, volume_fn=None):
     """One run of `run` with CUDA events around the forward of each target (a module, or a class whose __call__ is wrapped) and,
     with volume_fn, around ops.<volume_fn>: {stage: ms}."""
@@ -763,7 +813,8 @@ if __name__ == "__main__":
     a = ap.parse_args()
     for name in a.only.split(","):
         try:
-            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11}[name](a.iters)
+            {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11,
+             "c12": c12}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:

@@ -28,6 +28,7 @@ from oracle import coex as ocx                                  # noqa: E402
 from oracle import cost_volume as ocv                           # noqa: E402
 from oracle import geo_lookup as ogeo                           # noqa: E402
 from oracle import igev_rt as oigrt                             # noqa: E402
+from oracle import igevpp as oigpp                              # noqa: E402
 from oracle import lightstereo as olight                        # noqa: E402
 from oracle import models as omodels                            # noqa: E402
 from oracle import msnet as oms                                 # noqa: E402
@@ -475,6 +476,37 @@ def igev_rt():
     save("geo_volume_lookup", cases=len(GEO_VOLUME_CASES), **arrays)
 
 
+# (B, C, D0, D1, D2, H, W, levels, radius) of tests/golden/igevpp_lookup.npz, case i stored under keys suffixed with i
+IGEVPP_CASES = ((1, 8, 48, 48, 48, 2, 10, 2, 4), (1, 3, 20, 13, 30, 2, 21, 1, 4), (1, 5, 24, 17, 9, 2, 9, 2, 2),
+                (2, 4, 16, 24, 6, 3, 7, 2, 4))
+
+
+def igevpp():
+    """IGEV++'s multi-range encoding volume (igevpp/geometry.py): the reference class against the oracle, bit for bit.  The
+    disparities run from below -r to past 4 * max(D) + r, so taps leave every row at both ends; D1 and D2 differ from D0 >> i."""
+    rgeo = oigpp.load_reference("stereo.modeling.models.igevpp.geometry")
+    arrays = {}
+    for i, (b, c, d0, d1, d2, h, w, levels, radius) in enumerate(IGEVPP_CASES):
+        v0, v1, v2 = rnd(170 + i, b, c, d0, h, w), rnd(180 + i, b, c, d1, h, w), rnd(190 + i, b, c, d2, h, w)
+        f1, f2 = rnd(200 + i, b, 6, h, w), rnd(210 + i, b, 6, h, w)
+        top = 4 * max(d0, d1, d2) + 2 * radius + 8
+        disp = torch.rand(b, 1, h, w, generator=torch.Generator().manual_seed(220 + i)) * top - radius - 4
+        disp[0, 0, 0, :5] = torch.tensor([0.0, d0 - 1.0, 2.5, -radius - 1.5, 4 * d2 + radius + 1.5])
+        coords = torch.arange(w).float().reshape(1, 1, w, 1).repeat(b, h, 1, 1)
+        ref = rgeo.Combined_Geo_Encoding_Volume(v0, v1, v2, f1, f2, radius=radius, num_levels=levels)
+        outs = ref(disp, coords)
+        mine = oigpp.MultiRangeGeoEncodingVolume(v0, v1, v2, f1, f2, radius=radius, num_levels=levels)(disp, coords)
+        t = 2 * radius + 1
+        for name, a, m, shape in zip(("feat0", "feat1", "feat2", "corr"), outs, mine,
+                                     ((b, levels * c * t, h, w), (b, c * t, h, w), (b, c * t, h, w), (b, levels * t, h, w))):
+            must_equal(a, m, "igevpp_lookup case %d %s" % (i, name))
+            assert a.shape == shape, (name, a.shape, shape)
+            arrays["%s%d" % (name, i)] = a
+        arrays.update({"vol0_%d" % i: v0, "vol1_%d" % i: v1, "vol2_%d" % i: v2, "fmap1_%d" % i: f1, "fmap2_%d" % i: f2,
+                       "disp%d" % i: disp, "levels%d" % i: levels, "radius%d" % i: radius})
+    save("igevpp_lookup", cases=len(IGEVPP_CASES), **arrays)
+
+
 class _Const(torch.nn.Module):
     def __init__(self, t):
         super().__init__()
@@ -484,7 +516,7 @@ class _Const(torch.nn.Module):
         return self.t
 
 
-SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade", "coex", "msnet", "igev_rt"]
+SECTIONS = ["volumes", "regression", "modules", "models", "lookups", "flavours", "lightstereo", "cascade", "coex", "msnet", "igev_rt", "igevpp"]
 
 if __name__ == "__main__":
     if not shim.available():
