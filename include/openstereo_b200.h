@@ -310,6 +310,10 @@ int osb_warped_concat_volume_fwd(const float* x, const float* y, const float* di
                                  int mask_left, osb_stream_t stream);
 int osb_warped_gwc_concat_volume_fwd(const float* xg, const float* yg, const float* xc, const float* yc, const float* disp,
                                      float* out, int B, int Cg, int G, int Cc, int D, int H, int W, osb_stream_t stream);
+/* osb_disp_warp_fwd: MonSter's disp_warp(img, disp)[0] (monster/warp.py): img (B,C,H,W), disp (B,1,H,W) -> out (B,C,H,W), img
+ *   sampled at column w - disp like F.grid_sample(bilinear, padding_mode='border', align_corners=False) of MonSter's
+ *   normalize_coords grid, bit for bit with the reference on the CPU.  The same kernel as the two above, one launch; H >= 2, W >= 2. */
+int osb_disp_warp_fwd(const float* img, const float* disp, float* out, int B, int C, int H, int W, osb_stream_t stream);
 
 /* ---- CoEx (coex/coex_disp_processor.py:8-65, coex/coex_cost_processor.py:219-224) -------------------------------------------
  * osb_coex_regression_fwd: Regression.forward (eval) + upfeat in one launch: cost (B,1,D,h,w) logits, spx (B,9,4h,4w) ->

@@ -23,6 +23,13 @@
 // ne = s*w, sw = n*e, se = n*w, then v_nw*nw, fused multiply-adds of the ne, sw and se taps in that order.  The warped
 // right features therefore match the reference bit for bit; the group mean sums the K products in order and divides by K.
 //
+// Disparity-warp mode (border = 1, MonSter's disp_warp, monster/warp.py): a concatenation unit with D = 1 that writes only the
+// warped right features to an NCHW (B, C, H, W) output.  The grid is MonSter's normalize_coords, g = 2 * (v / (size - 1)) - 1
+// with v = w - disp for x and v = h for y, sampled with align_corners=False and padding_mode='border'.  aten's vectorised CPU
+// sampler unnormalises that as (g + 1) * (size / 2) - 0.5, which its build contracts into one fused multiply-add, then clamps
+// to [0, size - 1] before the floor; the kernel does the same, so the warped features match the reference's CPU disp_warp bit
+// for bit.  The row coordinate is not an integer here (about h * H / (H - 1) - 0.5), so rows y0 and y0 + 1 are both real taps.
+//
 // Roofline: HBM-bound.  Algorithmic bytes = 4*(2*B*C*H*W + B*D*H*W + B*Cout*D*H*W)  (both feature maps of each pair,
 // the hypotheses, the volume).
 #include "common.cuh"
@@ -43,13 +50,23 @@ struct WarpParams {
   int Ctot, oc_cat;    // output channels; first concatenation channel (= G)
   int n_gwc_units, n_cat_units;
   int mask_left;       // zero the left copy where w < disp (CasGwcNet) or not (CasPSMNet)
+  int border;          // disparity-warp mode: MonSter's coordinates, border padding, warped right features only
   float half_w, half_h;  // (W - 1) / 2, (H - 1) / 2
+  float wm1, hm1;        // W - 1, H - 1
 };
 
 // grid value and grid_sample's unnormalisation of it (align_corners=True), IEEE fp32 without contraction
 __device__ __forceinline__ float cas_roundtrip(float v, float half) {
   const float g = __fsub_rn(__fdiv_rn(v, half), 1.f);
   return __fmul_rn(__fadd_rn(g, 1.f), half);
+}
+
+// MonSter's normalize_coords, then grid_sample's align_corners=False unnormalisation as aten's vectorised CPU sampler computes
+// it, fmaf(g + 1, size / 2, -0.5), and the border clamp to [0, size - 1]; IEEE fp32 otherwise without contraction
+__device__ __forceinline__ float border_roundtrip(float v, float sizem1) {
+  const float g = __fsub_rn(__fmul_rn(2.f, __fdiv_rn(v, sizem1)), 1.f);
+  const float u = fmaf(__fadd_rn(g, 1.f), __fmul_rn(__fadd_rn(sizem1, 1.f), 0.5f), -0.5f);
+  return fminf(fmaxf(u, 0.f), sizem1);
 }
 
 // KMAX: compile-time bound of the channels a unit stages (gwc: K; concatenation: kCasCatChunk)
@@ -68,7 +85,7 @@ __global__ void __launch_bounds__(kCasThreads) warped_volume_kernel(const WarpPa
   const size_t HW = (size_t)p.H * p.W;
 
   // row coordinate: the same for every sample of this CTA
-  const float iy = cas_roundtrip((float)h, p.half_h);
+  const float iy = p.border ? border_roundtrip((float)h, p.hm1) : cas_roundtrip((float)h, p.half_h);
   const float fy = floorf(iy);
   const int y0 = (int)fy;
   const float n = __fsub_rn(iy, fy), s = __fsub_rn(1.f, n);
@@ -81,6 +98,34 @@ __global__ void __launch_bounds__(kCasThreads) warped_volume_kernel(const WarpPa
     s_rows[((size_t)c * 2 + r) * p.W + w] = (row >= 0 && row < p.H) ? __ldg(ysrc + c * HW + (size_t)row * p.W + w) : 0.f;
   }
   __syncthreads();
+
+  if (p.border) {      // disparity warp: D = 1, the warped right features only, (B, C, H, W); its own loop keeps the volume path's code
+    const float* dsrc = p.disp + (size_t)b * HW + (size_t)h * p.W;
+    float* dst = p.out + ((size_t)b * p.Cc + c0) * HW + (size_t)h * p.W;
+    for (int w = threadIdx.x; w < p.W; w += kCasThreads) {
+      const float ix = border_roundtrip(__fsub_rn((float)w, __ldg(dsrc + w)), p.wm1);   // in [0, W - 1]: x0 is a real column
+      const float fx = floorf(ix);
+      const int x0 = (int)fx;
+      const float wx = __fsub_rn(ix, fx), e = __fsub_rn(1.f, wx);
+      const float nw = __fmul_rn(s, e), ne = __fmul_rn(s, wx), sw = __fmul_rn(n, e), se = __fmul_rn(n, wx);
+      const bool in1 = x0 + 1 < p.W;
+#pragma unroll
+      for (int c = 0; c < KMAX; ++c) {
+        if (c < nch) {
+          const float* r0 = s_rows + (size_t)c * 2 * p.W;
+          float acc = __fmul_rn(r0[x0], nw);
+          acc = fmaf(in1 ? r0[x0 + 1] : 0.f, ne, acc);
+          if (two) {
+            const float* r1 = r0 + p.W;
+            acc = fmaf(r1[x0], sw, acc);
+            acc = fmaf(in1 ? r1[x0 + 1] : 0.f, se, acc);
+          }
+          __stcs(dst + c * HW + w, acc);
+        }
+      }
+    }
+    return;
+  }
 
   const float* dsrc = p.disp + (size_t)b * p.D * HW + (size_t)h * p.W;
   const float kf = (float)p.K;
@@ -154,12 +199,14 @@ static int launch_warped(const WarpParams& p0, cudaStream_t stream) {
   } else {
     p.G = 0;
   }
-  p.Ctot = p.G + 2 * p.Cc;
+  p.Ctot = p.border ? p.Cc : p.G + 2 * p.Cc;
   p.oc_cat = p.G;
   p.n_gwc_units = p.G;
   p.n_cat_units = (p.Cc + kCasCatChunk - 1) / kCasCatChunk;
   p.half_w = (float)((p.W - 1.0) / 2.0);
   p.half_h = (float)((p.H - 1.0) / 2.0);
+  p.wm1 = (float)(p.W - 1);
+  p.hm1 = (float)(p.H - 1);
   const int kmax = p.K > 8 ? 16 : 8;
   const size_t smem = (size_t)kmax * 2 * p.W * sizeof(float);
   OSB_REQUIRE(smem <= 227 * 1024, "warped_volume: W=%d needs %zu bytes of shared memory for %d staged channel rows (227 KB max)",
@@ -203,6 +250,14 @@ int osb_warped_gwc_concat_volume_fwd(const float* xg, const float* yg, const flo
   osb::WarpParams p{};
   p.xg = xg, p.yg = yg, p.xc = xc, p.yc = yc, p.disp = disp, p.out = out;
   p.B = B, p.Cg = Cg, p.G = G, p.Cc = Cc, p.D = D, p.H = H, p.W = W, p.mask_left = 1;
+  return osb::launch_warped(p, (cudaStream_t)stream);
+}
+
+int osb_disp_warp_fwd(const float* img, const float* disp, float* out, int B, int C, int H, int W, osb_stream_t stream) {
+  OSB_REQUIRE(img && disp && out, "disp_warp: null pointer");
+  osb::WarpParams p{};
+  p.yc = img, p.disp = disp, p.out = out;
+  p.B = B, p.Cg = 0, p.G = 0, p.Cc = C, p.D = 1, p.H = H, p.W = W, p.border = 1;
   return osb::launch_warped(p, (cudaStream_t)stream);
 }
 }

@@ -27,7 +27,9 @@ class CombinedGeoEncodingVolume:
             raise RuntimeError("CombinedGeoEncodingVolume: CUDA tensors required (the reference class serves CPU tensors)")
         self.num_levels, self.radius = int(num_levels), int(radius)
         self.geo_volume_pyramid = _volume_pyramid(geo_volume, self.num_levels)
-        self.init_corr_pyramid = self.corr_pyramid(init_fmap1, init_fmap2, self.num_levels)
+        # MonSter builds the volume inside its AMP YAML's bf16 autocast, where einsum would return bf16: the lookup reads fp32
+        with torch.autocast("cuda", enabled=False):
+            self.init_corr_pyramid = self.corr_pyramid(init_fmap1, init_fmap2, self.num_levels)
 
     def __call__(self, disp, coords):
         return ops.geo_lookup(self.geo_volume_pyramid, self.init_corr_pyramid, disp, coords, self.radius)

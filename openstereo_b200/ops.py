@@ -285,6 +285,23 @@ def warped_gwc_concat_volume(x_gwc, y_gwc, x_cat, y_cat, disp_samples, num_group
     return out.to(dt)
 
 
+def disp_warp(img, disp):
+    """MonSter's disp_warp(img, disp)[0] (monster/warp.py) -> (B, C, H, W) in img's dtype: img (B, C, H, W) sampled at column
+    w - disp[b, 0, h, w] like its F.grid_sample(bilinear, padding_mode='border', align_corners=False), computed in fp32 (the
+    reference's interp runs with autocast off).  disp: (B, 1, H, W), any real values.  One launch; no backward."""
+    _no_autograd("disp_warp", img, disp)
+    x, dt = _prep(img, "img")
+    d, _ = _prep(disp, "disp")
+    if x.dim() != 4 or tuple(d.shape) != (x.shape[0], 1) + tuple(x.shape[2:]):
+        raise ValueError("disp_warp: img %s and disp %s do not match (B, C, H, W) / (B, 1, H, W)" % (tuple(x.shape), tuple(d.shape)))
+    _same_device(x, d)
+    b, c, h, w = x.shape
+    out = torch.empty_like(x)
+    if out.numel():
+        _call("osb_disp_warp_fwd", x.data_ptr(), d.data_ptr(), out.data_ptr(), b, c, h, w, _stream(out))
+    return out.to(dt)
+
+
 # --------------------------------------------------------------------------- soft-argmin tails
 def softargmin(cost, maxdisp, keepdim=True, alpha=1.0, start=0.0, step=1.0, normalize=True):
     """disparity_regression(F.softmax(cost, 1), maxdisp) in one pass (stereobase_gru.py:163-164)."""

@@ -1,5 +1,5 @@
 """patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / IGEV-RT /
-IGEV++ / CoEx / MSNet3D, and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
+IGEV++ / MonSter / CoEx / MSNet3D, and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
 hot path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each
@@ -11,6 +11,8 @@ needs its own rebinding:
               aggregator + FasterSoftArgmin modules                          -> ``CostProcessor.forward`` / ``FasterSoftArgmin.forward``
 * LightStereo / IGEVStereo  like StereoBase: names imported into lightstereo.py:4-6 / igev_stereo.py:1-3 (``from .submodule import *``)
 * IGEV-RT     like IGEVStereo (igev_rt_stereo.py:1-6), plus per-instance ``cost_agg`` / ``classifier`` forward overrides
+* MonSter     like IGEVStereo (monster.py:1-8, plus ``disp_warp``), and the ConvGRU / encoder / head overrides on all three update
+              blocks (the two mix2 blocks' encoders on MixMotionEncoderEngine)
 * IGEV++      like IGEVStereo (igevpp_stereo.py:4-8), plus a per-instance ``classifier`` forward override and the update block's
               ``gru04 / gru08 / gru16 / encoder / geo_encoder0..2 / disp_head / mask_feat_4`` forward overrides
 * CasStereo   ``get_cv`` (GetCostVolume) and ``cost_agg[i]`` (CostAggregation) modules  -> per-instance ``forward`` overrides
@@ -228,12 +230,12 @@ def _patch_convgru(block, strict):
         _override_convgru(mod, ConvGRUEngine(mod), strict)
 
 
-def _patch_update_heads(block, strict):
-    """Per-instance ``forward`` overrides of ``encoder / disp_head / mask_feat_4`` of an IGEV / StereoBase BasicMultiUpdateBlock:
+def _patch_update_heads(block, strict, encoder=None):
+    """Per-instance ``forward`` overrides of ``encoder / disp_head / mask_feat_4`` of an IGEV / StereoBase / MonSter update block:
     CUDA inference calls the kernels serve (update.route_ok, the engines' serves()) run update.py's engines; the other shapes and
-    hyper-parameters run the reference's own forward."""
+    hyper-parameters run the reference's own forward.  `encoder`: the engine class of ``encoder`` (default MotionEncoderEngine)."""
     from .update import DispHeadEngine, MaskFeatEngine, MotionEncoderEngine
-    for name, cls in (("encoder", MotionEncoderEngine), ("disp_head", DispHeadEngine), ("mask_feat_4", MaskFeatEngine)):
+    for name, cls in (("encoder", encoder or MotionEncoderEngine), ("disp_head", DispHeadEngine), ("mask_feat_4", MaskFeatEngine)):
         mod = getattr(block, name)
         _override_engine(mod, cls(mod), strict, name)
 
@@ -375,18 +377,56 @@ def _patch_igev(model, strict, backbone=True):
     g = type(model).forward.__globals__
     orig = {n: g[n] for n in ("build_gwc_volume", "disparity_regression", "context_upsample", "Combined_Geo_Encoding_Volume")}
     over = _volume_tail_overrides(model, strict, orig, with_corr=False)
+    over["Combined_Geo_Encoding_Volume"] = _igev_geo_factory(model, strict, orig["Combined_Geo_Encoding_Volume"])
+    _rebind_methods(model, over)
+    _patch_convgru(model.update_block, strict)
+    _patch_update_heads(model.update_block, strict)
+    return model
 
+
+def _igev_geo_factory(model, strict, orig_cls):
+    """Guarded replacement of IGEV's Combined_Geo_Encoding_Volume (igev/geometry.py, and MonSter's copy of it)."""
     def geo_factory(fmap1, fmap2, volume, num_levels=2, radius=4):
         fast = _accelerable(model, fmap1, fmap2, volume)
         if not fast and strict:
             _refuse("Combined_Geo_Encoding_Volume")
-        cls = CombinedGeoEncodingVolume if fast else orig["Combined_Geo_Encoding_Volume"]
+        cls = CombinedGeoEncodingVolume if fast else orig_cls
         return cls(fmap1, fmap2, volume, num_levels=num_levels, radius=radius)
+    return geo_factory
 
-    over["Combined_Geo_Encoding_Volume"] = geo_factory
+
+def _patch_monster(model, strict, backbone=True):
+    """MonSter (monster/monster.py, class MonSter): the stereo branch's IGEV-shaped hot path -- the gwc volume, the soft-argmin
+    regression of the initial disparity, every lookup of the combined geometry-encoding volume (at disp, and at disp_mono_4x in
+    the last 7 iterations), the disparity warps of features_right[0] (``disp_warp``), the ConvGRUs, motion encoders and disp /
+    mask heads of ``update_block``, ``update_block_mix_stereo`` and ``update_block_mix_mono`` (the mix2 blocks' encoders on
+    update.MixMotionEncoderEngine) and the convex up-sampling.  The Depth Anything encoder and decoders, feat_transfer*, the stems,
+    corr_stem / corr_feature_att / cost_agg, the classifier, compute_scale_shift, REMP and the update blocks' own forward stay the
+    reference's code; `backbone` has no effect.  Under autocast (the AMP YAML, bf16) every patched call computes in fp32 and
+    returns the reference's dtypes."""
+    from .update import MixMotionEncoderEngine
+    g = type(model).forward.__globals__
+    orig = {n: g[n] for n in ("build_gwc_volume", "disparity_regression", "context_upsample", "Combined_Geo_Encoding_Volume",
+                              "disp_warp")}
+    over = _volume_tail_overrides(model, strict, orig, with_corr=False)
+    over["Combined_Geo_Encoding_Volume"] = _igev_geo_factory(model, strict, orig["Combined_Geo_Encoding_Volume"])
+
+    def warp(img, disp, padding_mode="border"):
+        """disp_warp(img, disp) -> (warped, None) on the library.  The valid mask (disp_warp(...)[1]) is not computed: the only
+        method the patch rebinds that calls disp_warp, _forward_pair, takes [0]."""
+        if not _accelerable(model, img, disp):
+            return orig["disp_warp"](img, disp, padding_mode) if not strict else _refuse("disp_warp")
+        if padding_mode != "border":
+            return orig["disp_warp"](img, disp, padding_mode)           # the kernel replays the border padding only
+        return ops.disp_warp(img, disp), None
+
+    over["disp_warp"] = warp
     _rebind_methods(model, over)
     _patch_convgru(model.update_block, strict)
     _patch_update_heads(model.update_block, strict)
+    for block in (model.update_block_mix_stereo, model.update_block_mix_mono):
+        _patch_convgru(block, strict)
+        _patch_update_heads(block, strict, encoder=MixMotionEncoderEngine)
     return model
 
 
@@ -630,7 +670,7 @@ _CASCADE_MODULES = {("casnet", "cas_psm"): "PSMNet", ("casnet", "cas_gwc"): "Gwc
 
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
              "IGEVStereo": _patch_igev, "IGEVRTtereo": _patch_igev_rt,
-             "IGEVPPStereo": _patch_igevpp, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
+             "IGEVPPStereo": _patch_igevpp, "MonSter": _patch_monster, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
 
 
 def patch(model, strict=True, backbone=True):

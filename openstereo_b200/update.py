@@ -16,7 +16,8 @@ mask_feat_4 (igev/update.py:123-125 == gru_blocks.py:304-306).  The 3x3 layers r
     MaskFeatEngine       net0 -> (B,Cout,H,W): one pack, one Cout 32 (IGEV, StereoBase) or Cout 64 (IGEV++) launch with bias + relu
                          and NCHW output
 
-IGEV++'s update block (igevpp/update.py) adds GeoEncoderEngine (geo_encoder0/1/2) and DispEncoderEngine (encoder); its ConvGRUs and
+MonSter's mix2 update blocks (monster/update.py) add MixMotionEncoderEngine (BasicMotionEncoder_mix2); their ConvGRUs, disparity and
+mask heads are IGEV's modules.  IGEV++'s update block (igevpp/update.py) adds GeoEncoderEngine (geo_encoder0/1/2) and DispEncoderEngine (encoder); its ConvGRUs and
 disparity head are IGEV's modules and run on gru.ConvGRUEngine and DispHeadEngine as they are.
 
 patch.py installs them as per-instance forward overrides of update_block.encoder / disp_head / mask_feat_4 and runs the reference's
@@ -245,5 +246,70 @@ class DispEncoderEngine(_Engine):
         part = ops.conv2d_k3_tc(cor, self.wc, None, self.b)
         out = ops.conv2d_k3_tc(dsp, self.wd, None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
         out[:, 127:].copy_(d)
+        mon.poll()
+        return out.to(dtype)
+
+
+class MixMotionEncoderEngine(_Engine):
+    """MonSter's BasicMotionEncoder_mix2.forward(disp, corr, flaw_stereo, disp_mono, corr_mono, flaw_mono) (monster/update.py:523-561)
+    on the library, MotionEncoderEngine's plan once per branch (stereo: convc1 / convc2 / convd1 / convd2 / conv; mono: the *_mono
+    layers):
+
+        cor  = relu(convc2(relu(convc1(cat(corr, flaw)))))   convc1 (162 + 96 -> 64) on the CUDA-core 1x1 over its two NCHW inputs
+                                                            (the concatenation is never built), pack, tc Cout 64
+        dsp  = relu(convd2(relu(convd1(disp))))             convd1 (7x7, 1 -> 64) as the depthwise kernel over disp broadcast to
+                                                            64 planes, pack, tc Cout 64
+        part = conv(cor, W[:, :64]) + b                     conv's weight zero-padded from 63 to 64 output channels, K split in two
+        out  = relu(conv(dsp, W[:, 64:]) + part)            NCHW output with the channels-last residual: relu(conv(cat(cor, dsp)))
+        out[:, 63] = disp                                   the reference's cat: channel 63 <- disp, channel 127 <- disp_mono
+
+    The two 64-channel NCHW halves are joined by one torch.cat into the module's (B, 128, H, W) output.
+    """
+
+    _BRANCHES = ("", "_mono")
+
+    def _pack(self):
+        m = self.module
+        self.w = []
+        for sfx in self._BRANCHES:
+            c1, c2, d1, d2, conv = (getattr(m, n + sfx) for n in ("convc1", "convc2", "convd1", "convd2", "conv"))
+            w = _pad_rows(conv.weight.detach().float(), 64)                      # 63 -> 64 output channels, row 63 zero
+            self.w.append(dict(c1=c1.weight.detach().float()[:, :, 0, 0].t().contiguous(), bc1=_bias(c1),    # (Cin, 64)
+                               c2=ops.pack_tc_weight_2d(c2.weight, 16), bc2=_bias(c2),
+                               d1=d1.weight.detach().float()[:, 0].contiguous(), bd1=_bias(d1),               # (64, 7, 7)
+                               d2=ops.pack_tc_weight_2d(d2.weight, 16), bd2=_bias(d2),
+                               wc=ops.pack_tc_weight_2d(w[:, :64], 16), wd=ops.pack_tc_weight_2d(w[:, 64:], 16), b=_bias(conv, 64)))
+
+    def serves(self, disp, corr, flaw, disp_mono, corr_mono, flaw_mono):
+        m = self.module
+        ts = (disp, corr, flaw, disp_mono, corr_mono, flaw_mono)
+        if not all(t.dim() == 4 and t.shape[0] == disp.shape[0] and t.shape[2:] == disp.shape[2:] for t in ts):
+            return False
+        if disp.shape[1] != 1 or disp_mono.shape[1] != 1 or corr.shape[1] != corr_mono.shape[1] or flaw.shape[1] != flaw_mono.shape[1]:
+            return False
+        cin = corr.shape[1] + flaw.shape[1]
+        return (all(_is_conv(getattr(m, "convc1" + s), cin, 64, 1) and _is_conv(getattr(m, "convc2" + s), 64, 64, 3)
+                    and _is_conv(getattr(m, "convd1" + s), 1, 64, 7) and _is_conv(getattr(m, "convd2" + s), 64, 64, 3)
+                    and _is_conv(getattr(m, "conv" + s), 128, 63, 3) for s in self._BRANCHES)
+                and route_ok(disp.shape[-1]))
+
+    def _branch(self, p, d, corr, flaw):
+        cor = ops.conv3d_1x1(_f32(corr), p["c1"], None, p["bc1"], act=ops.ACT_RELU, x1=_f32(flaw))
+        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), p["c2"], None, p["bc2"], act=ops.ACT_RELU)
+        dsp = ops.dwconv2d(d.expand(-1, 64, -1, -1).contiguous(), p["d1"], None, p["bd1"], act=ops.ACT_RELU)
+        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), p["d2"], None, p["bd2"], act=ops.ACT_RELU)
+        part = ops.conv2d_k3_tc(cor, p["wc"], None, p["b"])
+        out = ops.conv2d_k3_tc(dsp, p["wd"], None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
+        out[:, 63:].copy_(d)
+        return out
+
+    def __call__(self, disp, corr, flaw, disp_mono, corr_mono, flaw_mono):
+        self._ensure(disp.device)
+        mon = ops.TcOverflowMonitor.get(disp.device)
+        mon.check()
+        # the reference's torch.cat([out, disp, out_mono, disp_mono]) promotes the convolutions' dtype with both disparities'
+        dtype = torch.promote_types(torch.promote_types(_conv_dtype(disp, corr, flaw, disp_mono, corr_mono, flaw_mono), disp.dtype),
+                                    disp_mono.dtype)
+        out = torch.cat((self._branch(self.w[0], _f32(disp), corr, flaw), self._branch(self.w[1], _f32(disp_mono), corr_mono, flaw_mono)), 1)
         mon.poll()
         return out.to(dtype)

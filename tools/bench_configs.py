@@ -31,6 +31,10 @@
   c12 IGEV++ (reference class + patch()), B=8 @256x512, 32 iterations: patched / cuDNN fp32 / AMP YAML / patched AMP YAML in
       alternating rotation, ms per forward in the lookups, ConvGRUs, geo + disp encoders, heads and the rest, and the EPE against
       the unpatched fp32 model  (python tools/bench_configs.py --only c12)
+  c13 MonSter (reference class + patch(), ViT-L Depth Anything encoder), B=8 @256x512, 32 iterations: patched uniform YAML / cuDNN
+      fp32 / the AMP YAML's bf16 autocast / patched AMP YAML in alternating rotation, ms per forward in the lookups, ConvGRUs,
+      motion encoders, heads, warps and the rest, and the EPE against the unpatched fp32 model
+      (python tools/bench_configs.py --only c13 > results/h100_c13_monster.jsonl)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -757,6 +761,87 @@ def c12(iters, B=8, h=256, w=512):
     torch.cuda.empty_cache()
 
 
+def c13(iters, B=8, h=256, w=512):
+    """MonSter (monster/monster.py, the reference's class; oracle/monster.py supplies seeded weights for its Depth Anything V2
+    ViT-L), batch 8 at 256x512 (W' = 128), 32 GRU iterations.  Variants in alternating rotation, medians of three: patch() of the
+    uniform-YAML model (fp32), the unpatched uniform-YAML model (cuDNN fp32, TF32 off), the unpatched AMP-YAML model under the bf16
+    autocast its trainer uses and patch() of the AMP-YAML model under the same autocast.  Per variant: whole-forward ms and ms per
+    forward in the 39 lookups, the ConvGRUs, the motion encoders and the disp + mask heads of the three update blocks, the 14
+    disparity warps, and everything else; EPE of each variant against the unpatched fp32 model."""
+    import contextlib
+    from oracle import monster as omon
+    from openstereo_b200 import geo
+    from openstereo_b200.patch import patch
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    ref_mod = omon.load_reference("stereo.modeling.models.monster.monster")
+    ref_geo = omon.load_reference("stereo.modeling.models.monster.geometry").Combined_Geo_Encoding_Volume
+    amp = omon.amp_dtype(omon.AMP_YAML)
+    variants = {"patched": (patch(omon.monster(encoder="vitl").to(DEV)), None),
+                "cudnn_fp32": (omon.monster(encoder="vitl").to(DEV), None),
+                "amp_bf16": (omon.monster(omon.AMP_YAML, encoder="vitl").to(DEV), amp),
+                "patched_amp_yaml": (patch(omon.monster(omon.AMP_YAML, encoder="vitl").to(DEV)), amp)}
+    gen = torch.Generator().manual_seed(37)
+    x = {"left": (torch.rand(B, 3, h, w, generator=gen) * 2 - 1).to(DEV), "right": (torch.rand(B, 3, h, w, generator=gen) * 2 - 1).to(DEV)}
+    blocks = ("update_block", "update_block_mix_stereo", "update_block_mix_mono")
+    groups = {"lookups": ("lookup",), "convgrus": ("gru04", "gru08", "gru16"), "encoders": ("encoder",),
+              "heads": ("disp_head", "mask_feat_4"), "warps": ("warp",)}
+    ms = {k: [] for k in variants}
+    stage = {k: [] for k in variants}
+    outs = {}
+
+    def forward(m, dtype):
+        with torch.autocast("cuda", dtype=dtype) if dtype else contextlib.nullcontext():
+            return m(dict(x))["disp_pred"]
+
+    def stage_times(k, m, dtype):
+        targets = {"%s.%s" % (b, n): getattr(getattr(m, b), n) for b in blocks for names in list(groups.values())[1:4] for n in names}
+        targets["lookup"] = geo.CombinedGeoEncodingVolume if k.startswith("patched") else ref_geo
+        if k.startswith("patched"):
+            return _stage_times(lambda: forward(m, dtype), targets, volume_fn="disp_warp")
+        inner = ref_mod.disp_warp                                     # the unpatched _forward_pair reads the module global
+        ref_mod.disp_warp = lambda *a, **kw: _timed_call(events, inner, *a, **kw)
+        events = []
+        try:
+            st = _stage_times(lambda: forward(m, dtype), targets)
+        finally:
+            ref_mod.disp_warp = inner
+        st["volume"] = round(sum(a.elapsed_time(b) for a, b in events), 3)
+        return st
+
+    with torch.no_grad():
+        for _ in range(3):                                              # alternate: the variants share the GPU's state
+            for k, (m, dtype) in variants.items():
+                t, outs[k] = timeit(lambda: forward(m, dtype), max(1, iters // 5), warm=1)
+                ms[k].append(t)
+                st = stage_times(k, m, dtype)
+                st["warp"] = st.pop("volume", 0.0)
+                stage[k].append({g: sum(v for n, v in st.items() if n.rsplit(".", 1)[-1] in names) for g, names in groups.items()})
+    med = lambda v: sorted(v)[1]
+    stage_ms = {k: {g: round(med([s[g] for s in v]), 2) for g in groups} for k, v in stage.items()}
+    for k in stage_ms:
+        stage_ms[k]["everything_else"] = round(med(ms[k]) - sum(stage_ms[k][g] for g in groups), 2)
+    fp32 = outs["cudnn_fp32"].float()
+    emit(config="c13 MonSter refinement loop, B=%d @%dx%d, 32 iterations, vitl (reference class + patch())" % (B, h, w),
+         gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+         forward_ms={k: round(med(v), 2) for k, v in ms.items()},
+         stage_ms_per_forward=stage_ms,
+         epe_vs_cudnn_fp32_px={k: float("%.3e" % (o.float() - fp32).abs().mean().item()) for k, o in outs.items() if k != "cudnn_fp32"},
+         output_dtype={k: str(o.dtype) for k, o in outs.items()},
+         disparity_std_px=round(fp32.std().item(), 2))
+    del variants
+    torch.cuda.empty_cache()
+
+
+def _timed_call(events, fn, *args, **kw):
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    out = fn(*args, **kw)
+    b.record()
+    events.append((a, b))
+    return out
+
+
 def _stage_times(run, targets, volume_fn=None):
     """One run of `run` with CUDA events around the forward of each target (a module, or a class whose __call__ is wrapped) and,
     with volume_fn, around ops.<volume_fn>: {stage: ms}."""
@@ -814,7 +899,7 @@ if __name__ == "__main__":
     for name in a.only.split(","):
         try:
             {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11,
-             "c12": c12}[name](a.iters)
+             "c12": c12, "c13": c13}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:
