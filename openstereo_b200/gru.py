@@ -19,7 +19,7 @@ forward for every other shape.
 import torch
 
 from . import ops
-from .aggregation import _Engine
+from .update import _BlockEngine
 
 HIDDEN = 128
 
@@ -39,7 +39,7 @@ def pack_gru_conv(conv, hidden):
     return ops.pack_tc_weight_2d(w[:, :hidden], 16), ops.pack_tc_weight_2d(w[:, hidden:], 16), bias
 
 
-class ConvGRUEngine(_Engine):
+class ConvGRUEngine(_BlockEngine):
     """Packs convz / convr / convq of a reference ConvGRU module (re-packed when a parameter changes) and runs its forward."""
 
     def _pack(self):
@@ -53,12 +53,10 @@ class ConvGRUEngine(_Engine):
         return (c.kernel_size == (3, 3) and c.padding == (1, 1) and c.stride == (1, 1) and c.dilation == (1, 1) and c.in_channels == cin
                 and route_ok(self.module.convz.out_channels, cin, h.shape[-1]))
 
-    def __call__(self, h, cz, cr, cq, *x_list):
-        self._ensure(h.device)
-        mon = ops.TcOverflowMonitor.get(h.device)
-        mon.check()
-        dtype = torch.promote_types(torch.promote_types(h.dtype, cz.dtype), cq.dtype)   # the reference's result dtype
+    def _dtype(self, h, cz, cr, cq, *x_list):
+        return torch.promote_types(torch.promote_types(h.dtype, cz.dtype), cq.dtype)   # the reference's result dtype
 
+    def _run(self, h, cz, cr, cq, *x_list):
         def f32(t):
             return t.detach().float().contiguous()
 
@@ -74,6 +72,4 @@ class ConvGRUEngine(_Engine):
         qx = ops.conv2d_k3_tc_gru(xn, qxw, qb, ctx(cq), res_nhwc=False)
         z = ops.conv2d_k3_tc_gru(hn, zh, None, zx, ops.ACT_SIGMOID)
         rh = ops.conv2d_k3_tc_gru(hn, rhw, None, rx, ops.ACT_SIGMOID, mul=hn)
-        out = ops.conv2d_k3_tc_gru(rh, qh, None, qx, ops.ACT_TANH, blend=(z, hn), out_nhwc=False)
-        mon.poll()
-        return out.to(dtype)
+        return ops.conv2d_k3_tc_gru(rh, qh, None, qx, ops.ACT_TANH, blend=(z, hn), out_nhwc=False)

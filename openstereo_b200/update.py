@@ -3,25 +3,30 @@
 mask_feat_4 (igev/update.py:123-125 == gru_blocks.py:304-306).  The 3x3 layers run on the wgmma convolutions (osb_conv2d_k3_tc_fwd,
 3xFP16 split) with channels-last fp32 intermediates, the three shapes they do not serve on the library's fp32 CUDA-core kernels:
 
-    MotionEncoderEngine  (disp (B,1,H,W), corr (B,Cc,H,W)) -> (B,128,H,W)
-        cor  = relu(convc2(relu(convc1(corr))))         osb_conv3d_1x1_bn_act_fwd on the lookup's NCHW output, pack, tc Cout 64
-        dsp  = relu(convd2(relu(convd1(disp))))         convd1 (7x7, 1 -> 64) as the depthwise osb_dwconv2d_fwd over disp
-                                                        broadcast to 64 planes, pack, tc Cout 64
-        part = conv(cor, W[:, :64]) + b                 conv's weight zero-padded from 127 to 128 output channels, K split in two
-        out  = relu(conv(dsp, W[:, 64:]) + part)        NCHW output with the channels-last residual: relu(conv(cat(cor, dsp)))
-        out[:, 127] = disp                              the reference's torch.cat([out, disp])
+    MotionEncoderEngine  one branch (disp (B,1,H,W), corr (B,Cc,H,W)) -> (B,C,H,W), at the widths of _ENCODER_PLANS:
+        cor  = relu(convc2(relu(convc1(corr))))         osb_conv3d_1x1_bn_act_fwd on the lookup's NCHW output, pack, tc convc2
+                                                        (zero-padded to `rows` output channels where it is narrower)
+        dsp  = relu(convd2(relu(convd1(disp))))         convd1 (7x7, 1 -> Cd) as the depthwise osb_dwconv2d_fwd over disp
+                                                        broadcast to Cd planes, pack, tc convd2
+        part = conv(cor, W[:, :Cc2] | 0) + b            conv's weight zero-padded from C - 1 to C output channels, K split in two;
+                                                        the cor half has zero columns for cor's pad channels
+        out  = relu(conv(dsp, W[:, Cc2:]) + part)       NCHW output with the channels-last residual: relu(conv(cat(cor, dsp)))
+        out[:, C - 1] = disp                            the reference's torch.cat([out, disp])
+      BasicMotionEncoder (IGEV, StereoBase) and IGEV++'s BasicDispEncoder run one branch; MonSter's BasicMotionEncoder_mix2 runs
+      one per layer suffix "" / "_mono" (its convc1 reads corr and flaw as two NCHW blocks, the concatenation is never built) and
+      joins the two 64-channel halves by one torch.cat into the module's (B, 128, H, W) output.
     DispHeadEngine       net0 (B,128,H,W) -> (B,1,H,W)
         one channels-last pack; conv1 + bias + relu as two Cout 128 launches (one per half of its 256 channels, NCHW);
         conv2 + bias as two osb_conv3d_k3_bn_act_fwd launches (D = 1), the second adding the first as its residual
     MaskFeatEngine       net0 -> (B,Cout,H,W): one pack, one Cout 32 (IGEV, StereoBase) or Cout 64 (IGEV++) launch with bias + relu
                          and NCHW output
+    GeoEncoderEngine     IGEV++'s geo_encoder0/1/2 (igevpp/update.py:72-80)
 
-MonSter's mix2 update blocks (monster/update.py) add MixMotionEncoderEngine (BasicMotionEncoder_mix2); their ConvGRUs, disparity and
-mask heads are IGEV's modules.  IGEV++'s update block (igevpp/update.py) adds GeoEncoderEngine (geo_encoder0/1/2) and DispEncoderEngine (encoder); its ConvGRUs and
-disparity head are IGEV's modules and run on gru.ConvGRUEngine and DispHeadEngine as they are.
+MonSter's mix2 update blocks (monster/update.py) use IGEV's ConvGRUs, disparity and mask heads; IGEV++'s update block
+(igevpp/update.py) uses IGEV's ConvGRUs and disparity head.  All run on gru.ConvGRUEngine and the engines here as they are.
 
-patch.py installs them as per-instance forward overrides of update_block.encoder / disp_head / mask_feat_4 and runs the reference's
-own forward for every shape or hyper-parameter no kernel serves (route_ok, the engines' serves()).
+patch.py installs them as per-instance forward overrides of the update blocks' modules and runs the reference's own forward for
+every shape or hyper-parameter no kernel serves (route_ok, the engines' serves()).
 """
 import torch
 
@@ -36,6 +41,12 @@ def route_ok(w):
             and ops.conv2d_tc_kc(128, 32, w) != 0)
 
 
+def _tc_serves(w, *shapes):
+    """True when a wgmma instantiation serves every (Cin, Cout) 3x3 layer at image width w.  For the shapes of the IGEV++ engines
+    (Cout 32 or 128) that is W >= OSB_TC_MIN_WIDTH."""
+    return all(ops.conv2d_tc_kc(cin, cout, w) != 0 for cin, cout in shapes)
+
+
 def _is_conv(c, cin, cout, k):
     return (isinstance(c, torch.nn.Conv2d) and c.in_channels == cin and c.out_channels == cout and c.kernel_size == (k, k)
             and c.padding == (k // 2, k // 2) and c.stride == (1, 1) and c.dilation == (1, 1) and c.groups == 1
@@ -47,6 +58,11 @@ def _bias(conv, pad_to=None):
     if pad_to is not None:
         b = torch.cat((b, b.new_zeros(pad_to - b.numel())))
     return b.contiguous()
+
+
+def _pad_rows(w, rows):
+    """(Cout, Cin, k, k) -> (rows, Cin, k, k): zero output channels appended (they compute exact zeros)."""
+    return torch.cat((w, w.new_zeros((rows - w.shape[0],) + tuple(w.shape[1:]))), 0)
 
 
 def _conv_dtype(*tensors):
@@ -63,44 +79,117 @@ def _f32(t):
     return t.detach().float().contiguous()
 
 
-class MotionEncoderEngine(_Engine):
-    """BasicMotionEncoder.forward(disp, corr) on the library (module docstring)."""
+class _BlockEngine(_Engine):
+    """An update-block module's forward on the library: re-pack if needed, report a past fp16 overflow of the tensor-core
+    convolutions, run _run, schedule the next overflow read, return in _dtype(*args), the dtype the reference's forward returns."""
+
+    def __call__(self, *args):
+        device = args[0].device
+        self._ensure(device)
+        mon = ops.TcOverflowMonitor.get(device)
+        mon.check()
+        out = self._run(*args)
+        mon.poll()
+        return out.to(self._dtype(*args))
+
+    def _dtype(self, *args):
+        return _conv_dtype(*args)
+
+
+# The layer plans MotionEncoderEngine serves, keyed by the output channels of convc1, convc2, convd1 and conv and by whether the
+# module has the mix2 "_mono" branch -> (rows convc2 is packed with, the image widths the wgmma kernels serve at).  conv is packed
+# with one more output row, a zero one: the kernel's output channel that disp is copied into.
+_ENCODER_PLANS = {
+    (64, 64, 64, 127, False): (64, route_ok),                                                      # BasicMotionEncoder
+    (128, 96, 32, 127, False): (128, lambda w: _tc_serves(w, (128, 128), (32, 32), (32, 128))),    # BasicDispEncoder (no Cout 96)
+    (64, 64, 64, 63, True): (64, route_ok),                                                        # BasicMotionEncoder_mix2
+}
+
+
+class MotionEncoderEngine(_BlockEngine):
+    """BasicMotionEncoder.forward(disp, corr), BasicDispEncoder.forward(disp, corr) and BasicMotionEncoder_mix2.forward(disp, corr,
+    flaw_stereo, disp_mono, corr_mono, flaw_mono) (monster/update.py:523-561) on the library (module docstring).  self.w holds one
+    dict of packed weights per branch, named after the layers: c1 / bc1 (convc1), c2 / bc2, d1 / bd1, d2 / bd2, wc / wd / b
+    (conv).  A one-branch module's dict is also the engine's attributes (engine.wc, ...)."""
+
+    def _layout(self):
+        """(convc1, convc2, convd1, conv output channels), the branch suffixes, the plan (None: not one of _ENCODER_PLANS)."""
+        m = self.module
+        widths = tuple(getattr(getattr(m, n, None), "out_channels", None) for n in ("convc1", "convc2", "convd1", "conv"))
+        mix = hasattr(m, "conv_mono")
+        return widths, ("", "_mono") if mix else ("",), _ENCODER_PLANS.get(widths + (mix,))
+
+    @staticmethod
+    def _branches(args, suffixes):
+        """The forward's arguments as one (disp, corr[, flaw]) tuple per branch."""
+        return [tuple(args)] if len(suffixes) == 1 else [tuple(args[:3]), tuple(args[3:])]
 
     def _pack(self):
         m = self.module
-        w = m.conv.weight.detach().float()
-        w = torch.cat((w, w.new_zeros((1,) + tuple(w.shape[1:]))), 0)           # 127 -> 128 output channels, row 127 zero
-        self.c1, self.bc1 = m.convc1.weight.detach().float()[:, :, 0, 0].t().contiguous(), _bias(m.convc1)     # (Cin, 64)
-        self.c2, self.bc2 = ops.pack_tc_weight_2d(m.convc2.weight, 16), _bias(m.convc2)
-        self.d1, self.bd1 = m.convd1.weight.detach().float()[:, 0].contiguous(), _bias(m.convd1)            # (64, 7, 7)
-        self.d2, self.bd2 = ops.pack_tc_weight_2d(m.convd2.weight, 16), _bias(m.convd2)
-        self.wc, self.wd, self.b = ops.pack_tc_weight_2d(w[:, :64], 16), ops.pack_tc_weight_2d(w[:, 64:], 16), _bias(m.conv, 128)
+        (_, c2, _, out), suffixes, (rows, _) = self._layout()
+        self.w = []
+        for s in suffixes:
+            convc1, convc2, convd1, convd2, conv = (getattr(m, n + s) for n in ("convc1", "convc2", "convd1", "convd2", "conv"))
+            w = _pad_rows(conv.weight.detach().float(), out + 1)
+            wc = torch.cat((w[:, :c2], w.new_zeros(out + 1, rows - c2, 3, 3)), 1)                   # cor's pad channels: zero
+            self.w.append(dict(c1=convc1.weight.detach().float()[:, :, 0, 0].t().contiguous(), bc1=_bias(convc1),   # (Cin, Cc1)
+                               c2=ops.pack_tc_weight_2d(_pad_rows(convc2.weight.detach().float(), rows), 16),
+                               bc2=_bias(convc2, rows), d1=convd1.weight.detach().float()[:, 0].contiguous(),   # (Cd, 7, 7)
+                               bd1=_bias(convd1), d2=ops.pack_tc_weight_2d(convd2.weight, 16), bd2=_bias(convd2),
+                               wc=ops.pack_tc_weight_2d(wc, 16), wd=ops.pack_tc_weight_2d(w[:, c2:], 16), b=_bias(conv, out + 1),
+                               convd2=convd2, d2_kc={}))
+        if len(self.w) == 1:
+            vars(self).update(self.w[0])
 
-    def serves(self, disp, corr):
+    @staticmethod
+    def _convd2(p, w):
+        """Branch p's convd2 packed for the K chunk of image width w: the 16-channel chunk, or one packed on first use (Cd 32 at
+        W' = 128: 32)."""
+        kc = ops.conv2d_tc_kc(p["d2"].cout, p["d2"].cout, w)
+        if kc == p["d2"].kc:
+            return p["d2"]
+        if kc not in p["d2_kc"]:
+            p["d2_kc"][kc] = ops.pack_tc_weight_2d(p["convd2"].weight, kc)
+        return p["d2_kc"][kc]
+
+    def serves(self, *args):
         m = self.module
-        return (disp.dim() == 4 and corr.dim() == 4 and disp.shape[1] == 1 and disp.shape[0] == corr.shape[0]
-                and disp.shape[2:] == corr.shape[2:] and _is_conv(m.convc1, corr.shape[1], 64, 1) and _is_conv(m.convc2, 64, 64, 3)
-                and _is_conv(m.convd1, 1, 64, 7) and _is_conv(m.convd2, 64, 64, 3) and _is_conv(m.conv, 128, 127, 3)
-                and route_ok(disp.shape[-1]))
+        (c1, c2, cd, out), suffixes, plan = self._layout()
+        disp = args[0]
+        if plan is None or not all(t.dim() == 4 and t.shape[0] == disp.shape[0] and t.shape[2:] == disp.shape[2:] for t in args):
+            return False
+        branches = self._branches(args, suffixes)
+        planes = [t.shape[1] for t in branches[0][1:]]                 # corr[, flaw]: the same in every branch
+        if any(b[0].shape[1] != 1 or [t.shape[1] for t in b[1:]] != planes for b in branches):
+            return False
+        return (all(_is_conv(getattr(m, "convc1" + s), sum(planes), c1, 1) and _is_conv(getattr(m, "convc2" + s), c1, c2, 3)
+                    and _is_conv(getattr(m, "convd1" + s), 1, cd, 7) and _is_conv(getattr(m, "convd2" + s), cd, cd, 3)
+                    and _is_conv(getattr(m, "conv" + s), c2 + cd, out, 3) for s in suffixes)
+                and plan[1](disp.shape[-1]))
 
-    def __call__(self, disp, corr):
-        self._ensure(disp.device)
-        mon = ops.TcOverflowMonitor.get(disp.device)
-        mon.check()
-        dtype = torch.promote_types(_conv_dtype(disp, corr), disp.dtype)        # the reference's torch.cat([out, disp])
-        d = _f32(disp)
-        cor = ops.conv3d_1x1(_f32(corr), self.c1, None, self.bc1, act=ops.ACT_RELU)
-        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), self.c2, None, self.bc2, act=ops.ACT_RELU)
-        dsp = ops.dwconv2d(d.expand(-1, 64, -1, -1).contiguous(), self.d1, None, self.bd1, act=ops.ACT_RELU)
-        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), self.d2, None, self.bd2, act=ops.ACT_RELU)
-        part = ops.conv2d_k3_tc(cor, self.wc, None, self.b)
-        out = ops.conv2d_k3_tc(dsp, self.wd, None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
-        out[:, 127:].copy_(d)
-        mon.poll()
-        return out.to(dtype)
+    def _branch(self, p, d, corr, flaw=None):
+        """One branch on the packed weights p: d is disp in fp32, channels-last intermediates, NCHW output."""
+        cor = ops.conv3d_1x1(_f32(corr), p["c1"], None, p["bc1"], act=ops.ACT_RELU, x1=None if flaw is None else _f32(flaw))
+        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), p["c2"], None, p["bc2"], act=ops.ACT_RELU)
+        dsp = ops.dwconv2d(d.expand(-1, p["d1"].shape[0], -1, -1).contiguous(), p["d1"], None, p["bd1"], act=ops.ACT_RELU)
+        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), self._convd2(p, d.shape[-1]), None, p["bd2"], act=ops.ACT_RELU)
+        part = ops.conv2d_k3_tc(cor, p["wc"], None, p["b"])
+        out = ops.conv2d_k3_tc(dsp, p["wd"], None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
+        out[:, -1:].copy_(d)
+        return out
+
+    def _run(self, *args):
+        outs = [self._branch(p, _f32(b[0]), *b[1:]) for p, b in zip(self.w, self._branches(args, self._layout()[1]))]
+        return outs[0] if len(outs) == 1 else torch.cat(outs, 1)
+
+    def _dtype(self, *args):
+        dtype = _conv_dtype(*args)                                     # promoted with every disp: the reference's torch.cat
+        for b in self._branches(args, self._layout()[1]):
+            dtype = torch.promote_types(dtype, b[0].dtype)
+        return dtype
 
 
-class DispHeadEngine(_Engine):
+class DispHeadEngine(_BlockEngine):
     """DispHead.forward(x) = conv2(relu(conv1(x))) on the library (module docstring)."""
 
     def _pack(self):
@@ -117,21 +206,15 @@ class DispHeadEngine(_Engine):
         return (x.dim() == 4 and _is_conv(m.conv1, x.shape[1], 256, 3) and x.shape[1] == 128 and _is_conv(m.conv2, 256, 1, 3)
                 and route_ok(x.shape[-1]))
 
-    def __call__(self, x):
-        self._ensure(x.device)
-        mon = ops.TcOverflowMonitor.get(x.device)
-        mon.check()
-        dtype = _conv_dtype(x)
+    def _run(self, x):
         xn = ops.nchw_to_nhwc_cat([_f32(x)])
         h0 = ops.conv2d_k3_tc(xn, self.w1[0], None, self.b1[0], act=ops.ACT_RELU, out_nhwc=False)
         h1 = ops.conv2d_k3_tc(xn, self.w1[1], None, self.b1[1], act=ops.ACT_RELU, out_nhwc=False)
         y = ops.conv3d_k3(h0.unsqueeze(2), self.w2[0], None, self.b2)
-        y = ops.conv3d_k3(h1.unsqueeze(2), self.w2[1], None, None, y).squeeze(2)
-        mon.poll()
-        return y.to(dtype)
+        return ops.conv3d_k3(h1.unsqueeze(2), self.w2[1], None, None, y).squeeze(2)
 
 
-class MaskFeatEngine(_Engine):
+class MaskFeatEngine(_BlockEngine):
     """mask_feat_4 = Sequential(Conv2d(128, Cout, 3, padding=1), ReLU) on the library (module docstring): Cout 32 (IGEV-Stereo,
     StereoBase) or 64 (IGEV++)."""
 
@@ -145,31 +228,14 @@ class MaskFeatEngine(_Engine):
         return (len(m) == 2 and isinstance(m[1], torch.nn.ReLU) and x.dim() == 4 and x.shape[1] == 128 and cout in (32, 64)
                 and _is_conv(m[0], 128, cout, 3) and route_ok(x.shape[-1]) and ops.conv2d_tc_kc(128, cout, x.shape[-1]) != 0)
 
-    def __call__(self, x):
-        self._ensure(x.device)
-        mon = ops.TcOverflowMonitor.get(x.device)
-        mon.check()
-        dtype = _conv_dtype(x)
+    def _run(self, x):
         kc = ops.conv2d_tc_kc(128, self.module[0].out_channels, x.shape[-1])
         if kc not in self.w:
             self.w[kc] = ops.pack_tc_weight_2d(self.module[0].weight, kc)
-        y = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([_f32(x)]), self.w[kc], None, self.b, act=ops.ACT_RELU, out_nhwc=False)
-        mon.poll()
-        return y.to(dtype)
+        return ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([_f32(x)]), self.w[kc], None, self.b, act=ops.ACT_RELU, out_nhwc=False)
 
 
-def _tc_serves(w, *shapes):
-    """True when a wgmma instantiation serves every (Cin, Cout) 3x3 layer at image width w.  For the shapes of the IGEV++ engines
-    (Cout 32 or 128) that is W >= OSB_TC_MIN_WIDTH."""
-    return all(ops.conv2d_tc_kc(cin, cout, w) != 0 for cin, cout in shapes)
-
-
-def _pad_rows(w, rows):
-    """(Cout, Cin, k, k) -> (rows, Cin, k, k): zero output channels appended (they compute exact zeros)."""
-    return torch.cat((w, w.new_zeros((rows - w.shape[0],) + tuple(w.shape[1:]))), 0)
-
-
-class GeoEncoderEngine(_Engine):
+class GeoEncoderEngine(_BlockEngine):
     """IGEV++'s GeoEncoder.forward(geo) = convg2(relu(convg1(geo))) (igevpp/update.py:72-80) on the library:
 
         x = relu(convg1(geo))       osb_conv3d_1x1_bn_act_fwd on the lookup's NCHW output, in place (geo_planes -> 128)
@@ -188,128 +254,10 @@ class GeoEncoderEngine(_Engine):
         return (geo.dim() == 4 and _is_conv(m.convg1, geo.shape[1], 128, 1) and _is_conv(m.convg2, 128, 96, 3)
                 and _tc_serves(geo.shape[-1], (128, 128)))
 
-    def __call__(self, geo):
-        self._ensure(geo.device)
-        mon = ops.TcOverflowMonitor.get(geo.device)
-        mon.check()
-        dtype = _conv_dtype(geo)
+    def _run(self, geo):
         x = ops.conv3d_1x1(_f32(geo), self.g1, None, self.bg1, act=ops.ACT_RELU)
-        y = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([x]), self.g2, None, self.bg2, out_nhwc=False)
-        mon.poll()
-        return y[:, :96].to(dtype)
+        return ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([x]), self.g2, None, self.bg2, out_nhwc=False)[:, :96]
 
 
-class DispEncoderEngine(_Engine):
-    """IGEV++'s BasicDispEncoder.forward(disp, corr) (igevpp/update.py:82-100) on the library, MotionEncoderEngine's plan at IGEV++'s
-    widths:
-
-        cor  = relu(convc2(relu(convc1(corr))))     convc1 (Cc -> 128) on the CUDA-core 1x1 from the NCHW input, pack, convc2
-                                                    (128 -> 96) padded to 128 output channels (exact zeros), kept channels-last
-        dsp  = relu(convd2(relu(convd1(disp))))     convd1 (7x7, 1 -> 32) as the depthwise kernel over disp broadcast to 32 planes,
-                                                    pack, convd2 (32 -> 32) on the Cout-32 wgmma kernels
-        part = conv(cor, W[:, :96] | 0) + b         conv's weight padded from 127 to 128 output channels; the cor half gets zero
-                                                    columns for cor's 32 pad channels
-        out  = relu(conv(dsp, W[:, 96:]) + part)    NCHW output with the channels-last residual: relu(conv(cat(cor, dsp)))
-        out[:, 127] = disp                          the reference's torch.cat([out, disp])
-    """
-
-    def _pack(self):
-        m = self.module
-        self.c1, self.bc1 = m.convc1.weight.detach().float()[:, :, 0, 0].t().contiguous(), _bias(m.convc1)     # (Cin, 128)
-        self.c2, self.bc2 = ops.pack_tc_weight_2d(_pad_rows(m.convc2.weight.detach().float(), 128), 16), _bias(m.convc2, 128)
-        self.d1, self.bd1 = m.convd1.weight.detach().float()[:, 0].contiguous(), _bias(m.convd1)            # (32, 7, 7)
-        self.d2, self.bd2 = {}, _bias(m.convd2)                                 # K chunk -> packed convd2 (W' = 128: 32, else 16)
-        w = _pad_rows(m.conv.weight.detach().float(), 128)                      # 127 -> 128 output channels, row 127 zero
-        wc = torch.cat((w[:, :96], w.new_zeros(128, 32, 3, 3)), 1)              # cor's pad channels 96..127 meet zero columns
-        self.wc, self.wd, self.b = ops.pack_tc_weight_2d(wc, 16), ops.pack_tc_weight_2d(w[:, 96:], 16), _bias(m.conv, 128)
-
-    def serves(self, disp, corr):
-        m = self.module
-        return (disp.dim() == 4 and corr.dim() == 4 and disp.shape[1] == 1 and disp.shape[0] == corr.shape[0]
-                and disp.shape[2:] == corr.shape[2:] and _is_conv(m.convc1, corr.shape[1], 128, 1) and _is_conv(m.convc2, 128, 96, 3)
-                and _is_conv(m.convd1, 1, 32, 7) and _is_conv(m.convd2, 32, 32, 3) and _is_conv(m.conv, 128, 127, 3)
-                and _tc_serves(disp.shape[-1], (128, 128), (32, 32), (32, 128)))
-
-    def __call__(self, disp, corr):
-        self._ensure(disp.device)
-        mon = ops.TcOverflowMonitor.get(disp.device)
-        mon.check()
-        dtype = torch.promote_types(_conv_dtype(disp, corr), disp.dtype)        # the reference's torch.cat([out, disp])
-        d = _f32(disp)
-        kc = ops.conv2d_tc_kc(32, 32, d.shape[-1])
-        if kc not in self.d2:
-            self.d2[kc] = ops.pack_tc_weight_2d(self.module.convd2.weight, kc)
-        cor = ops.conv3d_1x1(_f32(corr), self.c1, None, self.bc1, act=ops.ACT_RELU)
-        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), self.c2, None, self.bc2, act=ops.ACT_RELU)
-        dsp = ops.dwconv2d(d.expand(-1, 32, -1, -1).contiguous(), self.d1, None, self.bd1, act=ops.ACT_RELU)
-        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), self.d2[kc], None, self.bd2, act=ops.ACT_RELU)
-        part = ops.conv2d_k3_tc(cor, self.wc, None, self.b)
-        out = ops.conv2d_k3_tc(dsp, self.wd, None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
-        out[:, 127:].copy_(d)
-        mon.poll()
-        return out.to(dtype)
-
-
-class MixMotionEncoderEngine(_Engine):
-    """MonSter's BasicMotionEncoder_mix2.forward(disp, corr, flaw_stereo, disp_mono, corr_mono, flaw_mono) (monster/update.py:523-561)
-    on the library, MotionEncoderEngine's plan once per branch (stereo: convc1 / convc2 / convd1 / convd2 / conv; mono: the *_mono
-    layers):
-
-        cor  = relu(convc2(relu(convc1(cat(corr, flaw)))))   convc1 (162 + 96 -> 64) on the CUDA-core 1x1 over its two NCHW inputs
-                                                            (the concatenation is never built), pack, tc Cout 64
-        dsp  = relu(convd2(relu(convd1(disp))))             convd1 (7x7, 1 -> 64) as the depthwise kernel over disp broadcast to
-                                                            64 planes, pack, tc Cout 64
-        part = conv(cor, W[:, :64]) + b                     conv's weight zero-padded from 63 to 64 output channels, K split in two
-        out  = relu(conv(dsp, W[:, 64:]) + part)            NCHW output with the channels-last residual: relu(conv(cat(cor, dsp)))
-        out[:, 63] = disp                                   the reference's cat: channel 63 <- disp, channel 127 <- disp_mono
-
-    The two 64-channel NCHW halves are joined by one torch.cat into the module's (B, 128, H, W) output.
-    """
-
-    _BRANCHES = ("", "_mono")
-
-    def _pack(self):
-        m = self.module
-        self.w = []
-        for sfx in self._BRANCHES:
-            c1, c2, d1, d2, conv = (getattr(m, n + sfx) for n in ("convc1", "convc2", "convd1", "convd2", "conv"))
-            w = _pad_rows(conv.weight.detach().float(), 64)                      # 63 -> 64 output channels, row 63 zero
-            self.w.append(dict(c1=c1.weight.detach().float()[:, :, 0, 0].t().contiguous(), bc1=_bias(c1),    # (Cin, 64)
-                               c2=ops.pack_tc_weight_2d(c2.weight, 16), bc2=_bias(c2),
-                               d1=d1.weight.detach().float()[:, 0].contiguous(), bd1=_bias(d1),               # (64, 7, 7)
-                               d2=ops.pack_tc_weight_2d(d2.weight, 16), bd2=_bias(d2),
-                               wc=ops.pack_tc_weight_2d(w[:, :64], 16), wd=ops.pack_tc_weight_2d(w[:, 64:], 16), b=_bias(conv, 64)))
-
-    def serves(self, disp, corr, flaw, disp_mono, corr_mono, flaw_mono):
-        m = self.module
-        ts = (disp, corr, flaw, disp_mono, corr_mono, flaw_mono)
-        if not all(t.dim() == 4 and t.shape[0] == disp.shape[0] and t.shape[2:] == disp.shape[2:] for t in ts):
-            return False
-        if disp.shape[1] != 1 or disp_mono.shape[1] != 1 or corr.shape[1] != corr_mono.shape[1] or flaw.shape[1] != flaw_mono.shape[1]:
-            return False
-        cin = corr.shape[1] + flaw.shape[1]
-        return (all(_is_conv(getattr(m, "convc1" + s), cin, 64, 1) and _is_conv(getattr(m, "convc2" + s), 64, 64, 3)
-                    and _is_conv(getattr(m, "convd1" + s), 1, 64, 7) and _is_conv(getattr(m, "convd2" + s), 64, 64, 3)
-                    and _is_conv(getattr(m, "conv" + s), 128, 63, 3) for s in self._BRANCHES)
-                and route_ok(disp.shape[-1]))
-
-    def _branch(self, p, d, corr, flaw):
-        cor = ops.conv3d_1x1(_f32(corr), p["c1"], None, p["bc1"], act=ops.ACT_RELU, x1=_f32(flaw))
-        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), p["c2"], None, p["bc2"], act=ops.ACT_RELU)
-        dsp = ops.dwconv2d(d.expand(-1, 64, -1, -1).contiguous(), p["d1"], None, p["bd1"], act=ops.ACT_RELU)
-        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), p["d2"], None, p["bd2"], act=ops.ACT_RELU)
-        part = ops.conv2d_k3_tc(cor, p["wc"], None, p["b"])
-        out = ops.conv2d_k3_tc(dsp, p["wd"], None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
-        out[:, 63:].copy_(d)
-        return out
-
-    def __call__(self, disp, corr, flaw, disp_mono, corr_mono, flaw_mono):
-        self._ensure(disp.device)
-        mon = ops.TcOverflowMonitor.get(disp.device)
-        mon.check()
-        # the reference's torch.cat([out, disp, out_mono, disp_mono]) promotes the convolutions' dtype with both disparities'
-        dtype = torch.promote_types(torch.promote_types(_conv_dtype(disp, corr, flaw, disp_mono, corr_mono, flaw_mono), disp.dtype),
-                                    disp_mono.dtype)
-        out = torch.cat((self._branch(self.w[0], _f32(disp), corr, flaw), self._branch(self.w[1], _f32(disp_mono), corr_mono, flaw_mono)), 1)
-        mon.poll()
-        return out.to(dtype)
+# BasicDispEncoder's and BasicMotionEncoder_mix2's engine, by the module class's name
+DispEncoderEngine = MixMotionEncoderEngine = MotionEncoderEngine

@@ -50,11 +50,11 @@ def load(dotted):
     for sub in ("fast_foundationstereo", "foundationstereo", "igevpp", "casnet"):
         _namespace("stereo.modeling.models." + sub, os.path.join(root, "modeling", "models", sub))
         _namespace("stereo.modeling.models.%s.core" % sub, os.path.join(root, "modeling", "models", sub, "core"))
-    if "timm" not in sys.modules:       # only dereferenced inside backbone constructors we never build
+    if "timm" not in sys.modules:       # a module imported now binds whichever timm this leaves in sys.modules
         try:
             importlib.import_module("timm")
         except Exception:
-            sys.modules["timm"] = types.ModuleType("timm")
+            install_timm_stub()
     if "Utils" not in sys.modules:      # fast_foundationstereo/core/submodule.py:7-8 (`from Utils import AMP_DTYPE`)
         import torch
         stub = types.ModuleType("Utils")
@@ -72,8 +72,8 @@ def install_timm_stub():
     encoder's outputs on is the reference's unmodified code."""
     import torch.nn as nn
     timm = sys.modules.get("timm")
-    if timm is not None and hasattr(timm, "create_model") and not getattr(timm, "_osb_stub", False):
-        return timm                                     # a real timm is installed: use it
+    if timm is not None and hasattr(timm, "create_model"):
+        return timm                                     # a real timm, or the stand-in already installed: modules hold it
 
     def cbr(cin, cout, stride):
         return nn.Sequential(nn.Conv2d(cin, cout, 3, stride, 1, bias=False), nn.BatchNorm2d(cout), nn.ReLU6(inplace=True))
