@@ -169,6 +169,34 @@ int osb_conv3d_1x1_bn_act_fwd(const float* x0, const float* x1, int Cin0, const 
                               const float* gate, float* y, int B, int Cin, int Cout, int D, int H,
                               int W, int act, int sigmoid_out, osb_stream_t stream);
 
+/* Instance-normalised variants of the three convolutions above (IGEV++'s BasicConv: conv -> InstanceNorm -> LeakyReLU(0.01),
+ * igevpp/submodule.py:8-34), same kernels and instantiations.  Two modes, each on when its pointers are given:
+ *   normalised input: every in-bounds input element of channel c is staged as
+ *       leaky((x - in_stats[b,c,0]) * in_stats[b,c,1]) * in_gate[b,c,h,w]        (in_gate NULL: no gate; broadcast over D)
+ *     and out-of-bounds taps stay 0 (the reference pads the normalised, gated tensor).  The 1x1 takes one pair per slab.
+ *   moments out: y is stored raw (scale, shift, act and sigmoid_out must be 0 / NULL) and stats_out[b,co] = (mean, 1/sqrt(var +
+ *     1e-5)) of y over D*H*W, biased variance as F.instance_norm, computed in the same launch: per-CTA partials (count, sum, M2)
+ *     in their own workspace slots, merged in slot order (Chan et al.) by the last CTA of each (b, channel block).
+ * in_stats / stats_out: (B, C, 2) fp32, 8-byte aligned.  workspace: workspace_floats >= osb_conv3d_in_workspace_floats(...)
+ * floats, 16-byte aligned, zero-filled before its first use (its counters return to 0 after every launch).  Where the counters
+ * sit depends on the op and the shapes, so a workspace may only be reused by launches of the same op and shapes, and never by
+ * launches that may run concurrently.  D*H*W of the output <= 2^24. */
+int osb_conv3d_k3_in_fwd(const float* x, const float* w_packed, const float* scale, const float* shift,
+                         const float* in_stats, const float* in_gate, float* y, float* stats_out, float* workspace,
+                         long long workspace_floats, int B, int Cin, int Cout, int D, int H, int W, int stride, int act,
+                         osb_stream_t stream);
+int osb_deconv3d_in_fwd(const float* x, const float* w_packed, const float* scale, const float* shift,
+                        const float* in_stats, const float* in_gate, float* y, float* stats_out, float* workspace,
+                        long long workspace_floats, int B, int Cin, int Cout, int D, int H, int W, int kernel, int act,
+                        osb_stream_t stream);
+int osb_conv3d_1x1_in_fwd(const float* x0, const float* x1, int Cin0, const float* w_packed, const float* scale,
+                          const float* shift, const float* in_stats0, const float* in_gate0, const float* in_stats1,
+                          const float* in_gate1, float* y, float* stats_out, float* workspace, long long workspace_floats,
+                          int B, int Cin, int Cout, int D, int H, int W, int act, int sigmoid_out, osb_stream_t stream);
+/* Workspace (floats) the moments-out launch of op 0 = osb_conv3d_k3_in_fwd (param = stride), 1 = osb_deconv3d_in_fwd (param =
+ * kernel) or 2 = osb_conv3d_1x1_in_fwd (param ignored) needs for INPUT extents D, H, W; -1 for invalid arguments. */
+int osb_conv3d_in_workspace_floats(int op, int B, int Cout, int D, int H, int W, int param);
+
 /* ------------------------------------------------------- tensor-core (wgmma) variant of the 3x3x3 conv ----- */
 
 /* Same operator as osb_conv3d_k3_bn_act_fwd (stride 1) for the full-resolution layers, computed on the Hopper (wgmma) tensor

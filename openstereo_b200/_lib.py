@@ -26,6 +26,10 @@ SIGNATURES = {
     "osb_conv3d_k3_bn_act_fwd": [_f32p] * 7 + [_i] * 8 + [_s],
     "osb_deconv3d_bn_act_fwd": [_f32p] * 6 + [_i] * 8 + [_s],
     "osb_conv3d_1x1_bn_act_fwd": [_f32p, _f32p, _i] + [_f32p] * 6 + [_i] * 8 + [_s],
+    "osb_conv3d_k3_in_fwd": [_f32p] * 9 + [ctypes.c_longlong] + [_i] * 8 + [_s],
+    "osb_deconv3d_in_fwd": [_f32p] * 9 + [ctypes.c_longlong] + [_i] * 8 + [_s],
+    "osb_conv3d_1x1_in_fwd": [_f32p, _f32p, _i] + [_f32p] * 10 + [ctypes.c_longlong] + [_i] * 8 + [_s],
+    "osb_conv3d_in_workspace_floats": [_i] * 7,
     "osb_conv3d_tc_supported": [_i, _i, _i, _i],
     "osb_conv3d_tc_kc": [_i, _i, _i, _i],
     "osb_tc_general_width": [_i],

@@ -16,6 +16,7 @@ Graphs restated (file:line of the reference forward each engine replaces):
   LightStereoAggregation lightstereo/aggregation.py:42-60 (Aggregation.forward), :94-101 (MobileV2Residual), :119-134 (AttentionModule)
   CoExAggregation       coex/coex_cost_processor.py:196-237 (Aggregation.forward), :68-80 (channelAtt)
   MSNet3DAggregation    msnet/MSNet3D.py:118-161 (eval forward after the volume), :10-46 (hourglass3D), submodule.py:136-173
+  IGEVPPAggregation     igevpp/igevpp_stereo.py:69-94 (hourglass.forward), submodule.py:8-34 (BasicConv), :162-175 (FeatureAtt)
 """
 import torch
 
@@ -1008,3 +1009,139 @@ class LightStereoAggregation(_Engine):
         up = ops.deconv2d_k3s2(quarter, w5, s5, b5, residual=self.redir2(half), act=ACT_RELU)
         w6, s6, b6 = self.up[1]
         return [ops.deconv2d_k3s2(up, w6, s6, b6, residual=self.redir1(x), act=ACT_RELU)]
+
+
+# ------------------------------------------------------------------------------------------------------ IGEV++
+def _in_refusal(m, norm, relu):
+    """Why IGEV++'s BasicConv `m` (igevpp/submodule.py:8-34: conv, InstanceNorm when use_in, LeakyReLU() made in forward when relu)
+    is not the layer the instance-norm kernels run with flags (norm, relu), or None."""
+    if bool(m.use_in) != norm or bool(m.relu) != relu:
+        return "%r: IN=%s, relu=%s (the graph runs IN=%s, relu=%s)" % (m.conv, m.use_in, m.relu, norm, relu)
+    inorm = m.IN
+    if norm and (inorm.affine or inorm.track_running_stats or inorm.eps != 1e-5):
+        return "%r: affine / tracked statistics / eps %g (eval normalises by each image's statistics with eps 1e-5)" % (inorm, inorm.eps)
+    if norm and m.conv.bias is not None:
+        return "%r: bias in front of the instance norm" % (m.conv,)
+    slopes = [l.negative_slope for l in m.modules() if isinstance(l, torch.nn.LeakyReLU)]
+    if any(s != 0.01 for s in slopes):
+        return "LeakyReLU slope %s (the kernels apply 0.01)" % slopes
+    try:
+        _Packed(m.conv)
+    except NotImplementedError as exc:
+        return str(exc)
+    return None
+
+
+class _InstanceFeatureAtt:
+    """IGEV++'s FeatureAtt (igevpp/submodule.py:162-175): feature map -> sigmoid(conv(leaky(instance_norm2d(conv(feat))))), two 1x1
+    launches: the hidden layer with moments out, then the biased 1x1 on its normalised output with sigmoid_out."""
+
+    def __init__(self, m):
+        self.a, self.b = _Packed(m.feat_att[0].conv), _Packed(m.feat_att[1])
+
+    def __call__(self, feat):
+        hidden, stats = ops.conv3d_1x1_in(feat, self.a.w, moments=True)
+        return ops.conv3d_1x1_in(hidden, self.b.w, in_stats0=stats, shift=self.b.shift, sigmoid_out=True)
+
+
+_IGEVPP_CONVS = ("conv0", "conv1.0", "conv1.1", "conv2.0", "conv2.1", "conv3.0", "conv3.1", "conv3_up", "agg_0.0", "agg_0.1", "agg_0.2",
+                 "conv2_up", "agg_1.0", "agg_1.1", "agg_1.2", "conv1_up")
+_IGEVPP_GATES = ("4", "8", "16", "32", "up_16", "up_8")
+
+
+class IGEVPPAggregation(_Engine):
+    """IGEV++'s instance-normalised hourglass(8) (igevpp/igevpp_stereo.py:22-94): cost volume (B, C, D, H, W) + the four left
+    feature maps -> (B, C, 2 * ceil(D / 2), ...), on the fp32 CUDA-core kernels.  Each BasicConv is conv -> InstanceNorm3d ->
+    LeakyReLU(0.01): its convolution stores the raw output with the per-(b, channel) statistics (moments out) and every consumer
+    normalises, activates and gates the tensor as it stages it (normalised input), so an instance-norm layer costs no pass over HBM
+    of its own.  16 convolutions and 6 two-launch FeatureAtt gates: 28 launches.  conv1_up (IN=False, relu=False) writes the plain
+    output."""
+
+    def __init__(self, module):
+        super().__init__(module)
+        self._why = self._refusal()
+
+    def _blocks(self):
+        m = self.module
+        for name in _IGEVPP_CONVS:
+            mod = m
+            for part in name.split("."):
+                mod = mod[int(part)] if part.isdigit() else getattr(mod, part)
+            yield name, mod
+
+    def _refusal(self):
+        m = self.module
+        for name, blk in self._blocks():
+            last = name == "conv1_up"
+            why = _in_refusal(blk, not last, not last)
+            if why:
+                return "%s: %s" % (name, why)
+        for g in _IGEVPP_GATES:
+            fa = getattr(m, "feature_att_" + g).feat_att
+            why = _in_refusal(fa[0], True, True)
+            if why:
+                return "feature_att_%s: %s" % (g, why)
+            try:
+                _Packed(fa[1])
+            except NotImplementedError as exc:
+                return "feature_att_%s: %s" % (g, exc)
+        return None
+
+    def serves(self, x, features):
+        """True when the kernels run this call: every layer is the one they implement (no affine or tracked instance norm, slope
+        0.01, the reference's kernel sizes, strides and flags) and the volume and the features have the shapes the graph
+        concatenates and gates (the reference's own torch.cat and broadcast would refuse any other)."""
+        if self._why is not None or x.dim() != 5 or len(features) < 4:
+            return False
+        if any(p.device != x.device for p in self.module.parameters()):
+            return False
+        b, c, d, h, w = x.shape
+        l = dict(self._blocks())
+        if c != l["conv0"].conv.in_channels or d * h * w > (1 << 24):        # moments count voxels exactly in fp32
+            return False
+        ext = [(d, h, w)]                                                      # extents of the four levels
+        for _ in range(3):
+            ext.append(tuple((e - 1) // 2 + 1 for e in ext[-1]))
+        if any(tuple(2 * e for e in ext[k + 1]) != ext[k] for k in (1, 2)):   # the deconvs land on the skip levels of agg_0 / agg_1
+            return False
+        att = [self.module.feature_att_4, self.module.feature_att_8, self.module.feature_att_16, self.module.feature_att_32]
+        return all(f.dim() == 4 and tuple(f.shape) == (b, a.feat_att[0].conv.in_channels) + e[1:]
+                   for f, a, e in zip(features, att, ext))
+
+    def _pack(self):
+        self.l = {name: _Packed(blk.conv) for name, blk in self._blocks()}
+        self.att = {g: _InstanceFeatureAtt(getattr(self.module, "feature_att_" + g)) for g in _IGEVPP_GATES}
+
+    def __call__(self, x, features):
+        if self._why is not None:
+            raise NotImplementedError("openstereo_b200: IGEV++ hourglass: %s" % self._why)
+        x = self._check(x)
+        if any(p.device != x.device for p in self.module.parameters()):
+            raise RuntimeError("openstereo_b200: IGEV++ hourglass: the module's parameters are not on %s" % x.device)
+        self._ensure(x.device)
+        f = [self._check(t) for t in features[:4]]
+        l, att = self.l, self.att
+        k3, dc, pw = ops.conv3d_k3_in, ops.deconv3d_in, ops.conv3d_1x1_in
+        c0, s0 = k3(x, l["conv0"].w, moments=True)
+        g4 = att["4"](f[0])
+        y, s = k3(c0, l["conv1.0"].w, 2, s0, g4, moments=True)
+        c1, s1 = k3(y, l["conv1.1"].w, 1, s, moments=True)
+        g8 = att["8"](f[1])
+        y, s = k3(c1, l["conv2.0"].w, 2, s1, g8, moments=True)
+        c2, s2 = k3(y, l["conv2.1"].w, 1, s, moments=True)
+        g16 = att["16"](f[2])
+        y, s = k3(c2, l["conv3.0"].w, 2, s2, g16, moments=True)
+        c3, s3 = k3(y, l["conv3.1"].w, 1, s, moments=True)
+        g32 = att["32"](f[3])
+        y, s = dc(c3, l["conv3_up"].w, 4, s3, g32, moments=True)
+        # torch.cat((conv3_up, conv2), 1) -> agg_0 without the concat: the up slab has no gate, the skip slab feature_att_16's
+        y, s = pw(y, l["agg_0.0"].w, s, None, c2, s2, g16, moments=True)
+        y, s = k3(y, l["agg_0.1"].w, 1, s, moments=True)
+        c2, s2 = k3(y, l["agg_0.2"].w, 1, s, moments=True)
+        gu16 = att["up_16"](f[2])
+        y, s = dc(c2, l["conv2_up"].w, 4, s2, gu16, moments=True)
+        y, s = pw(y, l["agg_1.0"].w, s, None, c1, s1, g8, moments=True)
+        y, s = k3(y, l["agg_1.1"].w, 1, s, moments=True)
+        c1, s1 = k3(y, l["agg_1.2"].w, 1, s, moments=True)
+        gu8 = att["up_8"](f[1])
+        return dc(c1, l["conv1_up"].w, 4, s1, gu8)

@@ -15,6 +15,12 @@
 // (~22 FMA per shared-memory load instruction), so the kernel is bound by the fp32 FMA pipe, not by LDS or HBM.
 // BatchNorm (eval) is folded into a per-channel scale/shift epilogue together with the residual add, the activation
 // and StereoBase's sigmoid channel gate, so no elementwise pass ever touches HBM.
+//
+// Instance normalisation (IGEV++'s BasicConv: conv -> InstanceNorm -> LeakyReLU(0.01), igevpp/submodule.py:8-34) cannot be
+// folded that way: its scale and shift come from each image's statistics over the whole output.  Two runtime modes carry it
+// without an extra pass over HBM.  Moments out: the producer stores its raw output and, in the same launch, the per-(b, channel)
+// mean and 1/sqrt(var + 1e-5).  Normalised input: the consumer applies leaky((v - mean) * rstd) * gate to every in-bounds
+// input element it stages, so the padding stays 0 after normalisation as in the reference.
 #include <algorithm>
 
 #include "common.cuh"
@@ -35,6 +41,16 @@ struct ConvParams {
   int Do, Ho, Wo;        // output extent
   int tiles_w, tiles_h, tiles_d;
   int act, sigmoid_out, vec_ok;
+  // instance norm (all null in the _bn_act_ entry points)
+  const float* in_stats;  // normalised input: (B, Cin0) x {mean, rstd} of x
+  const float* in_gate;   // (B, Cin0, H, W) multiplied after the activation, broadcast over D; or null
+  const float* in_stats1; // the same for the second channel slab x1 (1x1 only)
+  const float* in_gate1;
+  float* stats;           // moments out: (B, Cout) x {mean, rstd} of y
+  float* part;            // workspace: (B, Cout, CTAs along grid x) x {count, sum, M2}, then the counters
+  unsigned* counter;      // one per (b, channel block): 0 before and after every launch
+  long long ws_floats;    // workspace capacity
+  long long* ws_need;     // non-null: report the workspace the launch needs and launch nothing
 };
 
 __device__ __forceinline__ float activate(float v, int act) {
@@ -42,6 +58,120 @@ __device__ __forceinline__ float activate(float v, int act) {
   if (act == OSB_ACT_LEAKY) return v > 0.f ? v : 0.01f * v;
   if (act == OSB_ACT_RELU6) return fminf(fmaxf(v, 0.f), 6.f);
   return v;
+}
+
+// Normalised input: leaky((v - mean) * rstd) * gate of one staged element of channel bc = b * C + c at plane offset hw.
+__device__ __forceinline__ float normalise(const float* stats, const float* gate, float v, int bc, size_t hw, size_t plane) {
+  const float2 s = __ldg(reinterpret_cast<const float2*>(stats) + bc);
+  v = (v - s.x) * s.y;
+  v = v > 0.f ? v : 0.01f * v;
+  return gate ? v * __ldg(gate + (size_t)bc * plane + hw) : v;
+}
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// (n, mean, M2) <- (n, mean, M2) merged with (nb, meanb, M2b): Chan, Golub and LeVeque's parallel update
+__device__ __forceinline__ void chan_merge(float& n, float& mean, float& m2, float nb, float meanb, float m2b) {
+  if (nb == 0.f) return;
+  if (n == 0.f) {
+    n = nb, mean = meanb, m2 = m2b;
+    return;
+  }
+  const float t = n + nb, d = meanb - mean, f = nb / t;
+  mean = fmaf(d, f, mean);
+  m2 = m2 + m2b + d * d * n * f;
+  n = t;
+}
+
+// Moments out.  Every thread of the CTA calls this after the epilogue with the nvalid (0..8) leading columns of its row that it
+// stored.  The CTA reduces its stored outputs per channel to (count, sum, M2 about its own mean) in a fixed order (warp trees, then
+// the warps of a channel group in index order) and writes them to its own slot of p.part: no float is accumulated atomically.  The
+// CTA that arrives last for its (b, channel block) merges the slots in slot order with chan_merge into (mean, rstd), the biased
+// variance of F.instance_norm, and re-arms the counter.  Warps never straddle channel groups (threads per group: 32, 64 or 128).
+// red: shared scratch of nwarps * (TCO + 1) + 2 * COB + 1 floats, free once the CTA's last compute step is behind a barrier.
+template <int TCO>
+__device__ __forceinline__ void moments_out(const ConvParams& p, const float (&acc)[TCO][8], int b, int co0, int cg, int cob, int nvalid,
+                                         float* red) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+  const int wpc = nwarps / (cob / TCO);
+  const float (&v)[TCO][8] = acc;                      // what the epilogue stored: no scale, shift or activation in this mode
+  float* wred = red;                                   // [nwarps][TCO + 1]
+  float* cmean = red + nwarps * (TCO + 1);             // [COB]
+  float* ccount = cmean + cob;                         // [COB]
+  float* last = ccount + cob;
+  __syncthreads();                                     // every thread is past its compute: the staging buffers are free
+#pragma unroll
+  for (int c = 0; c < TCO; ++c) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s += i < nvalid ? v[c][i] : 0.f;
+    s = warp_sum(s);
+    if (lane == 0) wred[warp * (TCO + 1) + c] = s;
+  }
+  const float n = warp_sum((float)nvalid);
+  if (lane == 0) wred[warp * (TCO + 1) + TCO] = n;
+  __syncthreads();
+  if (tid < cob) {
+    const int g = tid / TCO, c = tid % TCO;
+    float sum = 0.f, cnt = 0.f;
+    for (int w = g * wpc; w < (g + 1) * wpc; ++w) sum += wred[w * (TCO + 1) + c], cnt += wred[w * (TCO + 1) + TCO];
+    cmean[tid] = cnt > 0.f ? sum / cnt : 0.f;
+    ccount[tid] = cnt;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int c = 0; c < TCO; ++c) {
+    const float m = cmean[cg * TCO + c];
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float d = v[c][i] - m;
+      s = i < nvalid ? fmaf(d, d, s) : s;
+    }
+    s = warp_sum(s);
+    if (lane == 0) wred[warp * (TCO + 1) + c] = s;
+  }
+  __syncthreads();
+  const size_t slots = gridDim.x;
+  if (tid < cob && co0 + tid < p.Cout) {
+    const int g = tid / TCO, c = tid % TCO;
+    float m2 = 0.f;
+    for (int w = g * wpc; w < (g + 1) * wpc; ++w) m2 += wred[w * (TCO + 1) + c];
+    float* slot = p.part + ((size_t)(b * p.Cout + co0 + tid) * slots + blockIdx.x) * 3;
+    slot[0] = ccount[tid], slot[1] = cmean[tid] * ccount[tid], slot[2] = m2;
+  }
+  __threadfence();                                     // the slots are visible device-wide before this CTA is counted
+  __syncthreads();
+  unsigned* counter = p.counter + b * gridDim.y + blockIdx.y;
+  if (tid == 0) *last = atomicAdd(counter, 1u) == gridDim.x - 1 ? 1.f : 0.f;
+  __syncthreads();
+  if (*last == 0.f) return;
+  __threadfence();
+  for (int j = warp; j < cob; j += nwarps) {
+    const int co = co0 + j;
+    if (co >= p.Cout) break;
+    const float* base = p.part + (size_t)(b * p.Cout + co) * slots * 3;
+    float cnt = 0.f, mean = 0.f, m2 = 0.f;
+    for (size_t s = lane; s < slots; s += 32) {
+      const float nb = __ldcg(base + 3 * s);
+      chan_merge(cnt, mean, m2, nb, nb > 0.f ? __ldcg(base + 3 * s + 1) / nb : 0.f, __ldcg(base + 3 * s + 2));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float nb = __shfl_down_sync(0xffffffffu, cnt, o), mb = __shfl_down_sync(0xffffffffu, mean, o);
+      const float qb = __shfl_down_sync(0xffffffffu, m2, o);
+      chan_merge(cnt, mean, m2, nb, mb, qb);
+    }
+    if (lane == 0) {
+      p.stats[2 * (b * p.Cout + co)] = mean;
+      p.stats[2 * (b * p.Cout + co) + 1] = 1.f / sqrtf(m2 / cnt + 1e-5f);
+    }
+  }
+  if (tid == 0) *counter = 0u;
 }
 
 // Shared epilogue: acc[c][v] -> y for TCO channels x 8 consecutive output columns.
@@ -149,8 +279,10 @@ __global__ void __launch_bounds__(NCG* TD* TH * 4) conv3d_k3_kernel(const ConvPa
       const int ci = r / C::ID;
       const int gd = id0 + dz, gh = ih0 + hy, gw = iw0 + wx, gc = c0 + ci;
       float v = 0.f;
-      if (wx < C::IW && gc < p.Cin && gd >= 0 && gd < p.D && gh >= 0 && gh < p.H && gw >= 0 && gw < p.W)
+      if (wx < C::IW && gc < p.Cin && gd >= 0 && gd < p.D && gh >= 0 && gh < p.H && gw >= 0 && gw < p.W) {
         v = __ldg(p.x + (size_t)(b * p.Cin + gc) * in_vol + (size_t)gd * in_plane + (size_t)gh * p.W + gw);
+        if (p.in_stats) v = normalise(p.in_stats, p.in_gate, v, b * p.Cin + gc, (size_t)gh * p.W + gw, in_plane);
+      }
       xs[idx] = v;
     }
     // ---- stage the weight slab (CI, 27, COB) ----
@@ -202,6 +334,10 @@ __global__ void __launch_bounds__(NCG* TD* TH * 4) conv3d_k3_kernel(const ConvPa
     }
   }
   epilogue<TCO>(p, acc, b, co0 + cg * TCO, od0 + td, oh0 + th, ow0 + wg * 8);
+  if (p.stats) {
+    const bool row = od0 + td < p.Do && oh0 + th < p.Ho;
+    moments_out<TCO>(p, acc, b, co0, cg, C::COB, row ? max(0, min(8, p.Wo - ow0 - wg * 8)) : 0, smem);
+  }
 }
 
 // ------------------------------------------------------------------------------------- transposed conv, stride 2
@@ -259,8 +395,10 @@ __global__ void __launch_bounds__(256) deconv3d_kernel(const ConvParams p) {
       const int ci = r / C::ID;
       const int gd = id0 + dz, gh = ih0 + hy, gw = iw0 + wx, gc = c0 + ci;
       float v = 0.f;
-      if (wx < C::IW && gc < p.Cin && gd >= 0 && gd < p.D && gh >= 0 && gh < p.H && gw >= 0 && gw < p.W)
+      if (wx < C::IW && gc < p.Cin && gd >= 0 && gd < p.D && gh >= 0 && gh < p.H && gw >= 0 && gw < p.W) {
         v = __ldg(p.x + (size_t)(b * p.Cin + gc) * in_vol + (size_t)gd * in_plane + (size_t)gh * p.W + gw);
+        if (p.in_stats) v = normalise(p.in_stats, p.in_gate, v, b * p.Cin + gc, (size_t)gh * p.W + gw, in_plane);
+      }
       xs[idx] = v;
     }
     for (int idx = tid; idx < C::WS; idx += C::THREADS) {
@@ -313,6 +451,10 @@ __global__ void __launch_bounds__(256) deconv3d_kernel(const ConvParams p) {
     }
   }
   epilogue<8>(p, acc, b, co0 + cg * 8, od0 + 2 * dd + pd, oh0 + 2 * hh + ph, ow0 + wg * 8);
+  if (p.stats) {
+    const bool row = od0 + 2 * dd + pd < p.Do && oh0 + 2 * hh + ph < p.Ho;
+    moments_out<8>(p, acc, b, co0, cg, C::COB, row ? max(0, min(8, p.Wo - ow0 - wg * 8)) : 0, smem);
+  }
 }
 
 // --------------------------------------------------------------------------------------------------- 1x1x1 conv
@@ -365,6 +507,14 @@ __global__ void __launch_bounds__(256) conv3d_1x1_kernel(const ConvParams p) {
 #pragma unroll
           for (int v = 0; v < 8; ++v) xv[v] = (ow + v < p.W) ? __ldg(src + off + v) : 0.f;
         }
+        const bool slab0 = gc < p.Cin0;
+        if (const float* st = slab0 ? p.in_stats : p.in_stats1) {
+          const int bc = slab0 ? b * p.Cin0 + gc : b * (p.Cin - p.Cin0) + gc - p.Cin0;
+          const size_t hw = (row % p.H) * p.W + ow;
+#pragma unroll
+          for (int v = 0; v < 8; ++v)
+            if (ow + v < p.W) xv[v] = normalise(st, slab0 ? p.in_gate : p.in_gate1, xv[v], bc, hw + v, (size_t)p.H * p.W);
+        }
         const float4 wa = *reinterpret_cast<const float4*>(ws + ci * 32 + cg * 8);
         const float4 wb = *reinterpret_cast<const float4*>(ws + ci * 32 + cg * 8 + 4);
         const float wv[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
@@ -379,6 +529,7 @@ __global__ void __launch_bounds__(256) conv3d_1x1_kernel(const ConvParams p) {
     const int od = (int)(row / p.H), oh = (int)(row % p.H);
     epilogue<8>(p, acc, b, co0 + cg * 8, od, oh, ow);
   }
+  if (p.stats) moments_out<8>(p, acc, b, co0, cg, 32, live ? min(8, p.W - ow) : 0, ws);
 }
 
 // --------------------------------------------------------------------------------- channels-last 1x1x1 conv
@@ -610,20 +761,36 @@ static int set_smem(K kernel, size_t bytes, const char* what) {
   return OSB_OK;
 }
 
+// Moments out needs 3 floats per (b, channel, CTA along grid x) and one counter per (b, channel block).  With p.ws_need set the
+// launchers only report that size (osb_conv3d_in_workspace_floats); otherwise a moments launch checks the caller's workspace.
+static int moments_workspace(ConvParams& p, dim3 grid, const char* what) {
+  const long long part = 3ll * p.B * p.Cout * grid.x, need = part + (long long)p.B * grid.y;
+  if (p.ws_need) {
+    *p.ws_need = need;
+    return OSB_OK;
+  }
+  if (!p.stats) return OSB_OK;
+  OSB_REQUIRE(p.part && p.ws_floats >= need, "%s: workspace of %lld floats, %lld needed", what, p.ws_floats, need);
+  p.counter = reinterpret_cast<unsigned*>(p.part + part);
+  return OSB_OK;
+}
+
 template <int S, int TCO, int NCG, int TD, int TH, int CI>
 static int launch_conv_k3(ConvParams& p, cudaStream_t stream) {
   using C = ConvCfg<S, TCO, NCG, TD, TH, CI>;
   auto kernel = conv3d_k3_kernel<S, TCO, NCG, TD, TH, CI>;
-  static PerDeviceFlag configured;
-  if (!configured.here()) {
-    if (int rc = set_smem(kernel, C::SMEM, "conv3d_k3")) return rc;
-    configured.here() = true;
-  }
   p.tiles_w = (p.Wo + C::TW - 1) / C::TW;
   p.tiles_h = (p.Ho + TH - 1) / TH;
   p.tiles_d = (p.Do + TD - 1) / TD;
   dim3 grid(p.tiles_w * p.tiles_h * p.tiles_d, (p.Cout + C::COB - 1) / C::COB, p.B);
   OSB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "conv3d_k3: grid too large");
+  if (int rc = moments_workspace(p, grid, "conv3d_k3")) return rc;
+  if (p.ws_need) return OSB_OK;
+  static PerDeviceFlag configured;
+  if (!configured.here()) {
+    if (int rc = set_smem(kernel, C::SMEM, "conv3d_k3")) return rc;
+    configured.here() = true;
+  }
   kernel<<<grid, C::THREADS, C::SMEM, stream>>>(p);
   count_launch();
   return check_launch("conv3d_k3_kernel");
@@ -633,22 +800,64 @@ template <int KS, int CI>
 static int launch_deconv(ConvParams& p, cudaStream_t stream) {
   using C = DeconvCfg<KS, CI>;
   auto kernel = deconv3d_kernel<KS, CI>;
-  static PerDeviceFlag configured;
-  if (!configured.here()) {
-    if (int rc = set_smem(kernel, C::SMEM, "deconv3d")) return rc;
-    configured.here() = true;
-  }
   p.tiles_w = (p.Wo + C::TW - 1) / C::TW;
   p.tiles_h = (p.Ho + C::TH - 1) / C::TH;
   p.tiles_d = (p.Do + C::TD - 1) / C::TD;
   dim3 grid(p.tiles_w * p.tiles_h * p.tiles_d, (p.Cout + C::COB - 1) / C::COB, p.B);
   OSB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "deconv3d: grid too large");
+  if (int rc = moments_workspace(p, grid, "deconv3d")) return rc;
+  if (p.ws_need) return OSB_OK;
+  static PerDeviceFlag configured;
+  if (!configured.here()) {
+    if (int rc = set_smem(kernel, C::SMEM, "deconv3d")) return rc;
+    configured.here() = true;
+  }
   kernel<<<grid, C::THREADS, C::SMEM, stream>>>(p);
   count_launch();
   return check_launch("deconv3d_kernel");
 }
 
+static int launch_conv_1x1(ConvParams& p, cudaStream_t stream) {
+  const size_t octs = (size_t)p.D * p.H * ((p.W + 7) / 8);
+  dim3 grid((unsigned)((octs + 63) / 64), (p.Cout + 31) / 32, p.B);
+  OSB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "conv3d_1x1: grid too large");
+  if (int rc = moments_workspace(p, grid, "conv3d_1x1")) return rc;
+  if (p.ws_need) return OSB_OK;
+  conv3d_1x1_kernel<<<grid, 256, 0, stream>>>(p);
+  count_launch();
+  return check_launch("conv3d_1x1_kernel");
+}
+
+// The instantiation for (Cout, stride): one channel per thread for the classifier heads (32 -> 1), 24-channel groups for
+// StereoBase's widths 24/48/96/144, 32-channel groups otherwise.
+static int dispatch_conv_k3(ConvParams& p, int stride, cudaStream_t s) {
+  if (p.Cout < 8) return stride == 1 ? launch_conv_k3<1, 1, 1, 4, 4, 8>(p, s) : launch_conv_k3<2, 1, 1, 2, 4, 4>(p, s);
+  if (p.Cout % 32 != 0 && p.Cout % 24 == 0) {
+    return stride == 1 ? launch_conv_k3<1, 8, 3, 4, 4, 8>(p, s) : launch_conv_k3<2, 8, 3, 2, 4, 4>(p, s);
+  }
+  return stride == 1 ? launch_conv_k3<1, 8, 4, 4, 4, 8>(p, s) : launch_conv_k3<2, 8, 4, 2, 4, 4>(p, s);
+}
+
 static bool aligned16(const void* q) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
+static bool aligned8(const void* q) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & 7) == 0; }
+
+// Common checks and fields of the three _in_fwd entry points.  Moments out (stats_out given) stores the raw output: no scale,
+// shift, activation or sigmoid may follow it (a bias in front of an instance norm cancels anyway).
+static int in_params(ConvParams& p, const char* what, const float* in_stats, const float* in_gate, const float* in_stats1,
+                     const float* in_gate1, float* stats_out, float* workspace, long long workspace_floats) {
+  OSB_REQUIRE(!stats_out || workspace, "%s: null pointer (moments out needs a workspace)", what);
+  OSB_REQUIRE(!in_gate || in_stats, "%s: an input gate needs the input's statistics", what);
+  OSB_REQUIRE(!in_gate1 || in_stats1, "%s: an input gate needs the input's statistics", what);
+  OSB_REQUIRE(!stats_out || (p.act == OSB_ACT_NONE && !p.sigmoid_out && !p.scale && !p.shift),
+              "%s: moments out stores the raw output (no scale, shift, activation or sigmoid)", what);
+  OSB_REQUIRE(aligned8(in_stats) && aligned8(in_stats1) && aligned8(stats_out) && aligned16(workspace),
+              "%s: statistics must be 8-byte and the workspace 16-byte aligned", what);
+  OSB_REQUIRE((long long)p.Do * p.Ho * p.Wo <= (1ll << 24), "%s: %lld voxels per channel exceed the exact fp32 count", what,
+              (long long)p.Do * p.Ho * p.Wo);
+  p.in_stats = in_stats, p.in_gate = in_gate, p.in_stats1 = in_stats1, p.in_gate1 = in_gate1;
+  p.stats = stats_out, p.part = workspace, p.ws_floats = workspace_floats;
+  return OSB_OK;
+}
 
 
 // ------------------------------------------------------------------------------- channels-last 1x1 conv over two channel slabs
@@ -785,14 +994,7 @@ int osb_conv3d_k3_bn_act_fwd(const float* x, const float* w_packed, const float*
   p.Do = (D - 1) / stride + 1, p.Ho = (H - 1) / stride + 1, p.Wo = (W - 1) / stride + 1;
   p.act = act, p.sigmoid_out = 0;
   p.vec_ok = (p.Wo % 4 == 0) && aligned16(y) && aligned16(residual) && aligned16(gate);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (Cout < 8) {  // classifier heads (32 -> 1): one channel per thread
-    return stride == 1 ? launch_conv_k3<1, 1, 1, 4, 4, 8>(p, s) : launch_conv_k3<2, 1, 1, 2, 4, 4>(p, s);
-  }
-  if (Cout % 32 != 0 && Cout % 24 == 0) {  // StereoBase widths 24/48/96/144
-    return stride == 1 ? launch_conv_k3<1, 8, 3, 4, 4, 8>(p, s) : launch_conv_k3<2, 8, 3, 2, 4, 4>(p, s);
-  }
-  return stride == 1 ? launch_conv_k3<1, 8, 4, 4, 4, 8>(p, s) : launch_conv_k3<2, 8, 4, 2, 4, 4>(p, s);
+  return dispatch_conv_k3(p, stride, (cudaStream_t)stream);
 }
 
 int osb_deconv3d_bn_act_fwd(const float* x, const float* w_packed, const float* scale, const float* shift,
@@ -827,12 +1029,88 @@ int osb_conv3d_1x1_bn_act_fwd(const float* x0, const float* x1, int Cin0, const 
   p.Do = D, p.Ho = H, p.Wo = W;
   p.act = act, p.sigmoid_out = sigmoid_out;
   p.vec_ok = (W % 4 == 0) && aligned16(y) && aligned16(residual) && aligned16(gate) && aligned16(x0) && aligned16(x1);
-  const size_t octs = (size_t)D * H * ((W + 7) / 8);
-  dim3 grid((unsigned)((octs + 63) / 64), (Cout + 31) / 32, B);
-  OSB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "conv3d_1x1: grid too large");
-  conv3d_1x1_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
-  count_launch();
-  return check_launch("conv3d_1x1_kernel");
+  return launch_conv_1x1(p, (cudaStream_t)stream);
+}
+
+
+int osb_conv3d_k3_in_fwd(const float* x, const float* w_packed, const float* scale, const float* shift, const float* in_stats,
+                         const float* in_gate, float* y, float* stats_out, float* workspace, long long workspace_floats, int B,
+                         int Cin, int Cout, int D, int H, int W, int stride, int act, osb_stream_t stream) {
+  using namespace osb;
+  OSB_REQUIRE(x && w_packed && y, "conv3d_k3_in: null pointer");
+  OSB_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && D > 0 && H > 0 && W > 0, "conv3d_k3_in: empty shape");
+  OSB_REQUIRE(stride == 1 || stride == 2, "conv3d_k3_in: stride %d not supported (1 or 2)", stride);
+  OSB_REQUIRE(act >= 0 && act <= 2, "conv3d_k3_in: unknown activation %d", act);
+  ConvParams p{};
+  p.x = x, p.w = w_packed, p.scale = scale, p.shift = shift, p.y = y;
+  p.B = B, p.Cin = Cin, p.Cin0 = Cin, p.Cout = Cout, p.D = D, p.H = H, p.W = W;
+  p.Do = (D - 1) / stride + 1, p.Ho = (H - 1) / stride + 1, p.Wo = (W - 1) / stride + 1;
+  p.act = act;
+  p.vec_ok = (p.Wo % 4 == 0) && aligned16(y);
+  if (int rc = in_params(p, "conv3d_k3_in", in_stats, in_gate, nullptr, nullptr, stats_out, workspace, workspace_floats)) return rc;
+  return dispatch_conv_k3(p, stride, (cudaStream_t)stream);
+}
+
+int osb_deconv3d_in_fwd(const float* x, const float* w_packed, const float* scale, const float* shift, const float* in_stats,
+                        const float* in_gate, float* y, float* stats_out, float* workspace, long long workspace_floats, int B,
+                        int Cin, int Cout, int D, int H, int W, int kernel, int act, osb_stream_t stream) {
+  using namespace osb;
+  OSB_REQUIRE(x && w_packed && y, "deconv3d_in: null pointer");
+  OSB_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && D > 0 && H > 0 && W > 0, "deconv3d_in: empty shape");
+  OSB_REQUIRE(kernel == 3 || kernel == 4, "deconv3d_in: kernel %d not supported (3 or 4)", kernel);
+  OSB_REQUIRE(act >= 0 && act <= 2, "deconv3d_in: unknown activation %d", act);
+  ConvParams p{};
+  p.x = x, p.w = w_packed, p.scale = scale, p.shift = shift, p.y = y;
+  p.B = B, p.Cin = Cin, p.Cin0 = Cin, p.Cout = Cout, p.D = D, p.H = H, p.W = W;
+  p.Do = 2 * D, p.Ho = 2 * H, p.Wo = 2 * W;
+  p.act = act;
+  p.vec_ok = (p.Wo % 4 == 0) && aligned16(y);
+  if (int rc = in_params(p, "deconv3d_in", in_stats, in_gate, nullptr, nullptr, stats_out, workspace, workspace_floats)) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  return kernel == 3 ? launch_deconv<3, 8>(p, s) : launch_deconv<4, 8>(p, s);
+}
+
+int osb_conv3d_1x1_in_fwd(const float* x0, const float* x1, int Cin0, const float* w_packed, const float* scale, const float* shift,
+                          const float* in_stats0, const float* in_gate0, const float* in_stats1, const float* in_gate1, float* y,
+                          float* stats_out, float* workspace, long long workspace_floats, int B, int Cin, int Cout, int D, int H,
+                          int W, int act, int sigmoid_out, osb_stream_t stream) {
+  using namespace osb;
+  OSB_REQUIRE(x0 && w_packed && y, "conv3d_1x1_in: null pointer");
+  OSB_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && D > 0 && H > 0 && W > 0, "conv3d_1x1_in: empty shape");
+  OSB_REQUIRE(Cin0 > 0 && Cin0 <= Cin && (Cin0 == Cin || x1 != nullptr), "conv3d_1x1_in: bad channel split %d of %d", Cin0, Cin);
+  OSB_REQUIRE(Cin0 < Cin || (!in_stats1 && !in_gate1), "conv3d_1x1_in: statistics for a second slab that is not there");
+  OSB_REQUIRE(act >= 0 && act <= 3, "conv3d_1x1_in: unknown activation %d", act);
+  ConvParams p{};
+  p.x = x0, p.x1 = x1, p.w = w_packed, p.scale = scale, p.shift = shift, p.y = y;
+  p.B = B, p.Cin = Cin, p.Cin0 = Cin0, p.Cout = Cout, p.D = D, p.H = H, p.W = W;
+  p.Do = D, p.Ho = H, p.Wo = W;
+  p.act = act, p.sigmoid_out = sigmoid_out;
+  p.vec_ok = (W % 4 == 0) && aligned16(y) && aligned16(x0) && aligned16(x1);
+  if (int rc = in_params(p, "conv3d_1x1_in", in_stats0, in_gate0, in_stats1, in_gate1, stats_out, workspace, workspace_floats)) {
+    return rc;
+  }
+  return launch_conv_1x1(p, (cudaStream_t)stream);
+}
+
+int osb_conv3d_in_workspace_floats(int op, int B, int Cout, int D, int H, int W, int param) {
+  using namespace osb;
+  if (B <= 0 || Cout <= 0 || D <= 0 || H <= 0 || W <= 0 || op < 0 || op > 2) return -1;
+  if ((op == 0 && param != 1 && param != 2) || (op == 1 && param != 3 && param != 4)) return -1;
+  long long need = -1;
+  ConvParams p{};
+  p.B = B, p.Cout = Cout, p.D = D, p.H = H, p.W = W, p.ws_need = &need;
+  int rc;
+  if (op == 0) {
+    p.Do = (D - 1) / param + 1, p.Ho = (H - 1) / param + 1, p.Wo = (W - 1) / param + 1;
+    rc = dispatch_conv_k3(p, param, nullptr);
+  } else if (op == 1) {
+    p.Do = 2 * D, p.Ho = 2 * H, p.Wo = 2 * W;
+    rc = param == 3 ? launch_deconv<3, 8>(p, nullptr) : launch_deconv<4, 8>(p, nullptr);
+  } else {
+    p.Do = D, p.Ho = H, p.Wo = W;
+    rc = launch_conv_1x1(p, nullptr);
+  }
+  return rc != OSB_OK || need > 0x7fffffffll ? -1 : (int)need;
 }
 
 int osb_conv1x1_ndhwc_cat_fwd(const float* x0, const float* x1, int C0, int C1, const float* w_packed, const float* scale,

@@ -565,6 +565,101 @@ def conv3d_1x1(x0, w_packed, scale=None, shift=None, residual=None, gate=None, a
     return y.squeeze(2) if squeeze else y
 
 
+# --------------------------------------------------------------------------- instance-normalised convolutions
+# IGEV++'s BasicConv (conv -> InstanceNorm -> LeakyReLU(0.01)) on the kernels above: the producer stores its raw output with the
+# per-(b, channel) (mean, rstd) of it ("moments out"), the consumer normalises, activates and gates each element as it stages it
+# ("normalised input").  Statistics are (B, C, 2) fp32.
+_IN_OPS = {"k3": 0, "deconv": 1, "1x1": 2}
+_IN_WORKSPACE = {}
+
+
+def _in_workspace(op, b, cout, d, h, w, param, device, stream):
+    """The moments workspace of one launch configuration on (device, stream), zero-filled once.  Its counters return to 0 after
+    every launch and launches on one stream never overlap; one buffer per configuration, because the counters of another layout
+    would sit where this one writes its partials."""
+    key = (device, stream, op, b, cout, d, h, w, param)
+    ws = _IN_WORKSPACE.get(key)
+    if ws is None:
+        need = int(_lib.lib.osb_conv3d_in_workspace_floats(_IN_OPS[op], b, cout, d, h, w, param))
+        if need < 0:
+            raise ValueError("openstereo_b200: no moments workspace for %s (B=%d, Cout=%d, %dx%dx%d)" % (op, b, cout, d, h, w))
+        ws = _IN_WORKSPACE[key] = torch.zeros(need, dtype=torch.float32, device=device)
+    return ws
+
+
+def _in_launch(name, op, y, moments, b, cout, d, h, w, param, head, tail):
+    """head + (y, stats, workspace, capacity) + shape + tail -> y, or (y, stats) with moments."""
+    stream = _stream(y)
+    stats, ws = None, None
+    if moments:
+        stats = torch.empty((b, cout, 2), dtype=torch.float32, device=y.device)
+        ws = _in_workspace(op, b, cout, d, h, w, param, y.device, stream)
+    _call(name, *head, y.data_ptr(), _ptr(stats), _ptr(ws), 0 if ws is None else ws.numel(), *tail, stream)
+    return (y, stats) if moments else y
+
+
+def _in_operands(x, in_stats, in_gate, c, h, w):
+    if in_stats is not None:
+        assert in_stats.shape == (x.shape[0], c, 2) and in_stats.dtype == torch.float32 and in_stats.is_contiguous()
+    if in_gate is not None:
+        assert in_stats is not None and in_gate.shape == (x.shape[0], c, h, w) and in_gate.is_contiguous()
+
+
+def conv3d_k3_in(x, w_packed, stride=1, in_stats=None, in_gate=None, moments=False):
+    """3x3x3 conv (padding 1) of leaky(instance_norm(x)) * in_gate (in_stats given) or of x; moments=True -> (y, stats of y)."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 5
+    b, cin, d, h, w = x.shape
+    assert w_packed.shape[0] == cin and w_packed.shape[1] == 27
+    _in_operands(x, in_stats, in_gate, cin, h, w)
+    cout = w_packed.shape[2]
+    y = torch.empty((b, cout, (d - 1) // stride + 1, (h - 1) // stride + 1, (w - 1) // stride + 1), dtype=torch.float32,
+                    device=x.device)
+    return _in_launch("osb_conv3d_k3_in_fwd", "k3", y, moments, b, cout, d, h, w, stride,
+                      (x.data_ptr(), w_packed.data_ptr(), None, None, _ptr(in_stats), _ptr(in_gate)),
+                      (b, cin, cout, d, h, w, stride, ACT_NONE))
+
+
+def deconv3d_in(x, w_packed, kernel=4, in_stats=None, in_gate=None, moments=False):
+    """Transposed conv (stride 2) of leaky(instance_norm(x)) * in_gate (in_stats given) or of x; moments=True -> (y, stats)."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 5
+    b, cin, d, h, w = x.shape
+    assert w_packed.shape[0] == cin and w_packed.shape[1] == kernel ** 3
+    _in_operands(x, in_stats, in_gate, cin, h, w)
+    cout = w_packed.shape[2]
+    y = torch.empty((b, cout, 2 * d, 2 * h, 2 * w), dtype=torch.float32, device=x.device)
+    return _in_launch("osb_deconv3d_in_fwd", "deconv", y, moments, b, cout, d, h, w, kernel,
+                      (x.data_ptr(), w_packed.data_ptr(), None, None, _ptr(in_stats), _ptr(in_gate)),
+                      (b, cin, cout, d, h, w, kernel, ACT_NONE))
+
+
+def conv3d_1x1_in(x0, w_packed, in_stats0=None, in_gate0=None, x1=None, in_stats1=None, in_gate1=None, moments=False, shift=None,
+                  sigmoid_out=False):
+    """1x1x1 conv over the channel concat of x0 (and x1), each slab normalised by its own statistics and gate when given; 4-D
+    inputs are D = 1 volumes.  shift (a bias) and sigmoid_out apply to the output; moments=True -> (y, stats of y)."""
+    squeeze = x0.dim() == 4
+    if squeeze:
+        x0 = x0.unsqueeze(2)
+        x1 = None if x1 is None else x1.unsqueeze(2)
+    assert x0.is_cuda and x0.dtype == torch.float32 and x0.is_contiguous()
+    b, c0, d, h, w = x0.shape
+    _in_operands(x0, in_stats0, in_gate0, c0, h, w)
+    cin = c0
+    if x1 is not None:
+        assert x1.is_contiguous() and x1.dtype == torch.float32 and x1.shape[0] == b and x1.shape[2:] == x0.shape[2:]
+        _in_operands(x1, in_stats1, in_gate1, x1.shape[1], h, w)
+        cin += x1.shape[1]
+    assert w_packed.shape[0] == cin
+    cout = w_packed.shape[-1]
+    y = torch.empty((b, cout, d, h, w), dtype=torch.float32, device=x0.device)
+    out = _in_launch("osb_conv3d_1x1_in_fwd", "1x1", y, moments, b, cout, d, h, w, 0,
+                     (x0.data_ptr(), _ptr(x1), c0, w_packed.data_ptr(), None, _ptr(shift), _ptr(in_stats0), _ptr(in_gate0),
+                      _ptr(in_stats1), _ptr(in_gate1)),
+                     (b, cin, cout, d, h, w, ACT_NONE, 1 if sigmoid_out else 0))
+    if not squeeze:
+        return out
+    return (out[0].squeeze(2), out[1]) if moments else out.squeeze(2)
+
+
 # --------------------------------------------------------------------------- tensor-core conv (wgmma, 3xFP16 split)
 def conv3d_tc_supported(cin, cout, w, stride=1):
     return bool(_lib.lib.osb_conv3d_tc_supported(int(cin), int(cout), int(w), int(stride)))

@@ -20,7 +20,8 @@ rebinding.  What each model rebinds:
 * IGEV-RT     globals (igev_rt_stereo.py:1-6): build_gwc_volume, disparity_regression (strided), Geo_Encoding_Volume,
               context_upsample ((B, 1, 4h, 4w)); ``cost_agg`` and ``classifier`` forward
 * IGEV++      globals (igevpp_stereo.py:4-8): build_gwc_volume, disparity_regression (strided), Combined_Geo_Encoding_Volume
-              (multi-range), context_upsample ((B, 1, 4h, 4w)); ``classifier`` forward; the update block with ``geo_encoder0..2``
+              (multi-range), context_upsample ((B, 1, 4h, 4w)); ``classifier`` forward; the update block with ``geo_encoder0..2``;
+              with aggregation=True also ``cost_agg0 / cost_agg1 / cost_agg2`` forward
 * CasStereo   ``get_cv`` (GetCostVolume) and every ``cost_agg[i]`` (CostAggregation) forward
 * CoEx        ``CostProcessor`` / ``DispProcessor`` / ``DispProcessor.regression`` forward
 * MSNet3D     one monolithic ``forward`` (MSNet3D.py:110-161), no processor modules: ``model.forward``, which keeps the
@@ -41,12 +42,14 @@ either.  The kernels have no backward, so any other call must NOT reach them sil
 A CUDA inference call that no kernel serves (a shape or hyper-parameter outside the kernels' envelope) runs the reference's own
 code in both modes.  Every other call runs the library.
 """
+import functools
 import types
 
 import torch
 
 from . import ops
-from .aggregation import CascadeAggregation, GwcAggregation, PSMAggregation, StereoBaseAggregation, StereoBaseCostHead
+from .aggregation import (CascadeAggregation, GwcAggregation, IGEVPPAggregation, PSMAggregation, StereoBaseAggregation,
+                          StereoBaseCostHead)
 from .geo import CombinedGeoEncodingVolume, GeoEncodingVolume, MultiRangeGeoEncodingVolume
 from .gru import ConvGRUEngine
 from .update import DispHeadEngine, GeoEncoderEngine, MaskFeatEngine, MotionEncoderEngine
@@ -372,13 +375,15 @@ def _patch_igev_rt(model, strict, backbone=True):
     return model
 
 
-def _patch_igevpp(model, strict, backbone=True):
+def _patch_igevpp(model, strict, backbone=True, aggregation=False):
     """IGEV++ (igevpp/igevpp_stereo.py:162-249, class IGEVPPStereo): the gwc volume, the classifier Conv3d(8 -> 1) of the three
     disparity ranges (``classifier.forward``, which returns logits: the reference's own softmax follows), the strided regressions of
     the three initial disparities, the per-GRU-iteration multi-range lookup (one launch), the update block's ConvGRUs, geometry
-    encoders, disparity encoder, disparity head and mask head, and the convex up-sampling.  The instance-normalised hourglasses,
-    patch0 / patch1, the feature nets, cnet, selective_conv, disp_conv and BasicMultiUpdateBlock.forward itself (the selective-weight
-    blend, cat, pool2x, interp) stay the reference's code; `backbone` has no effect.  Under autocast (the AMP YAML) every call
+    encoders, disparity encoder, disparity head and mask head, and the convex up-sampling.  With aggregation=True also the three
+    instance-normalised hourglasses (``cost_agg0 / cost_agg1 / cost_agg2.forward``, aggregation.IGEVPPAggregation); calls whose
+    layers or shapes the kernels do not implement run the module's own forward.  patch0 / patch1, the feature nets, cnet,
+    selective_conv, disp_conv and BasicMultiUpdateBlock.forward itself (the selective-weight blend, cat, pool2x, interp) stay the
+    reference's code, and so do the hourglasses by default; `backbone` has no effect.  Under autocast (the AMP YAML) every call
     computes in fp32 and returns the reference's dtypes."""
     _rebind_globals(model, strict, {"build_gwc_volume": _GWC, "disparity_regression": _REGRESSION_INTERVAL,
                                     "Combined_Geo_Encoding_Volume": (MultiRangeGeoEncodingVolume, None),
@@ -386,6 +391,11 @@ def _patch_igevpp(model, strict, backbone=True):
     head = StereoBaseCostHead(model.classifier)
     _override(model.classifier, "IGEV++ classifier", strict, lambda x: head.logits(x).to(x.dtype))
     _patch_update_block(model.update_block, strict, _IGEV_UPDATE + ("geo_encoder0", "geo_encoder1", "geo_encoder2"))
+    if aggregation:
+        for name in ("cost_agg0", "cost_agg1", "cost_agg2"):
+            eng = IGEVPPAggregation(getattr(model, name))
+            _override(getattr(model, name), "IGEV++ " + name, strict, lambda x, features, eng=eng: eng(x, features).to(x.dtype),
+                      serves=eng.serves)
     return model
 
 
@@ -491,11 +501,12 @@ _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _pa
              "IGEVPPStereo": _patch_igevpp, "MonSter": _patch_monster, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
 
 
-def patch(model, strict=True, backbone=True):
+def patch(model, strict=True, backbone=True, aggregation=False):
     """Rebind the hot path of a reference model instance in place and return it.  backbone=True (default) also routes the
     GwcNet / PSMNet 2D extractor's residual blocks to the wgmma conv kernels in CUDA inference calls (_patch_backbone);
     backbone=False leaves the extractor entirely to the reference's cuDNN code.  For the CasStereo models (casnet.cas_psm.PSMNet,
-    casnet.cas_gwc.GwcNet) `backbone` has no effect: their FPN extractor always runs the reference's code."""
+    casnet.cas_gwc.GwcNet) `backbone` has no effect: their FPN extractor always runs the reference's code.  aggregation=True
+    (IGEV++ only) also runs the three instance-normalised hourglasses on the library; off by default."""
     if not isinstance(model, torch.nn.Module):
         raise TypeError("patch() expects an nn.Module")
     name = type(model).__name__
@@ -506,6 +517,10 @@ def patch(model, strict=True, backbone=True):
     else:
         raise NotImplementedError("patch(): no hot-path drop-in for %s (supported: %s, and CasStereo's casnet.cas_psm.PSMNet / "
                                   "casnet.cas_gwc.GwcNet)" % (name, sorted(_PATCHERS)))
+    if aggregation:
+        if patcher is not _patch_igevpp:
+            raise NotImplementedError("patch(%s, aggregation=True): only IGEVPPStereo has an aggregation option" % name)
+        patcher = functools.partial(_patch_igevpp, aggregation=True)
     if getattr(model, "_osb_patched", False):
         return model
     patcher(model, strict, backbone)

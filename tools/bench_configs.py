@@ -35,6 +35,10 @@
       fp32 / the AMP YAML's bf16 autocast / patched AMP YAML in alternating rotation, ms per forward in the lookups, ConvGRUs,
       motion encoders, heads, warps and the rest, and the EPE against the unpatched fp32 model
       (python tools/bench_configs.py --only c13 > results/h100_c13_monster.jsonl)
+  c14 IGEV++'s three instance-normalised hourglasses (reference class + patch()), B=8 @256x512, 32 iterations: patch(m,
+      aggregation=True) / patch(m) / cuDNN fp32 / AMP YAML in alternating rotation, ms per forward in cost_agg0..2 (CUDA events) and
+      for the whole forward, and the EPE against the unpatched fp32 model
+      (python tools/bench_configs.py --only c14 > results/h100_c14_igevpp_aggregation.jsonl)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -833,6 +837,46 @@ def c13(iters, B=8, h=256, w=512):
     torch.cuda.empty_cache()
 
 
+def c14(iters, B=8, h=256, w=512):
+    """IGEV++'s hourglasses (igevpp/igevpp_stereo.py:22-94, the reference's class with the timm stand-in), batch 8 at 256x512 (D' =
+    48 at 1/4), 32 GRU iterations.  Variants in alternating rotation, medians of three: patch(m, aggregation=True) and patch(m) of the
+    uniform-YAML model (fp32), the unpatched uniform-YAML model (cuDNN fp32, TF32 off) and the unpatched AMP-YAML model (the
+    reference's fp16 autocast).  Per variant: ms per forward in the three hourglasses (CUDA events around cost_agg0..2) and for the
+    whole forward; EPE of each variant against the unpatched fp32 model."""
+    from oracle import igevpp as oigpp
+    from openstereo_b200.patch import patch
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    variants = {"patched_aggregation": patch(oigpp.igevpp().to(DEV), aggregation=True), "patched": patch(oigpp.igevpp().to(DEV)),
+                "cudnn_fp32": oigpp.igevpp().to(DEV), "amp_fp16": oigpp.igevpp(oigpp.AMP_YAML).to(DEV)}
+    gen = torch.Generator().manual_seed(41)
+    x = {"left": (torch.rand(B, 3, h, w, generator=gen) * 2 - 1).to(DEV), "right": (torch.rand(B, 3, h, w, generator=gen) * 2 - 1).to(DEV)}
+    names = ("cost_agg0", "cost_agg1", "cost_agg2")
+    ms = {k: [] for k in variants}
+    hg = {k: [] for k in variants}
+    outs = {}
+    with torch.no_grad():
+        for _ in range(3):                                              # alternate: the variants share the GPU's state
+            for k, m in variants.items():
+                t, outs[k] = timeit(lambda: m(dict(x))["disp_pred"], max(1, iters // 5), warm=1)
+                ms[k].append(t)
+                st = _stage_times(lambda: m(dict(x)), {n: getattr(m, n) for n in names})
+                hg[k].append(sum(st.get(n, 0.0) for n in names))
+    med = lambda v: sorted(v)[1]
+    fp32 = outs["cudnn_fp32"].float()
+    hg_ms = {k: round(med(v), 2) for k, v in hg.items()}
+    emit(config="c14 IGEV++ instance-normalised hourglasses, B=%d @%dx%d, 32 iterations (reference class + patch())" % (B, h, w),
+         gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+         forward_ms={k: round(med(v), 2) for k, v in ms.items()},
+         hourglasses_ms_per_forward=hg_ms,
+         hourglasses_speedup_vs_cudnn_fp32=round(hg_ms["cudnn_fp32"] / hg_ms["patched_aggregation"], 2),
+         hourglasses_speedup_vs_amp_fp16=round(hg_ms["amp_fp16"] / hg_ms["patched_aggregation"], 2),
+         epe_vs_cudnn_fp32_px={k: float("%.3e" % (o.float() - fp32).abs().mean().item()) for k, o in outs.items() if k != "cudnn_fp32"},
+         disparity_std_px=round(fp32.std().item(), 2))
+    del variants
+    torch.cuda.empty_cache()
+
+
 def _timed_call(events, fn, *args, **kw):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
@@ -899,7 +943,7 @@ if __name__ == "__main__":
     for name in a.only.split(","):
         try:
             {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11,
-             "c12": c12, "c13": c13}[name](a.iters)
+             "c12": c12, "c13": c13, "c14": c14}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:
