@@ -41,6 +41,10 @@ extern "C" {
 #define OSB_ACT_SIGMOID 4 /* the ConvGRU gates (torch.sigmoid / torch.tanh); accepted by osb_conv2d_k3_tc_gru_fwd */
 #define OSB_ACT_TANH 5
 
+/* Precision of the tensor-core products (osb_conv2d_k3_tc_prec_fwd, osb_conv2d_k3_tc_gru_prec_fwd) */
+#define OSB_PREC_FP32 0 /* fp32-accurate 3xFP16 split products (the default of every other entry point) */
+#define OSB_PREC_F16 1  /* one fp16 MMA per product, a_hi * b_hi: autocast precision (DESIGN.md section 4.20) */
+
 typedef void* osb_stream_t;
 
 int osb_abi_version(void);
@@ -311,6 +315,19 @@ int osb_conv2d_k3_tc_fwd(const float* x_nhwc, const void* w_split, const float* 
 int osb_conv2d_k3_tc_gru_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
                              const float* mul_nhwc, const float* blend_z_nhwc, const float* blend_h_nhwc, float* y, int B, int Cin,
                              int Cout, int H, int W, int act, int out_nhwc, int res_nhwc, long long res_bstride, osb_stream_t stream);
+/* osb_conv2d_k3_tc_fwd and osb_conv2d_k3_tc_gru_fwd with the precision of the products, `precision` = OSB_PREC_FP32 (the result is
+ * the entry point without it, bit for bit) or OSB_PREC_F16: the single-term mode of the 16-channel-chunk kernels (csrc/conv3d_tcg.cu),
+ * activations staged as fp16(x * 16) alone -- the same range guard (|x| < 4094, the overflow counter) -- and one fp16 MMA per product
+ * with fp32 accumulation, the accuracy of the reference's fp16 / bf16 autocast.  Scale, shift, residual, activation, gate and blend
+ * stay fp32.  A shape the selector routes to csrc/conv3d_tc.cu (Cout <= 32 at W = 128: osb_conv2d_tc_kc(...) == 32) keeps the
+ * 3-term product under either value.  Any other value of `precision` returns OSB_EINVAL before any launch. */
+int osb_conv2d_k3_tc_prec_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
+                              float* y, int B, int Cin, int Cout, int H, int W, int dilation, int act, int out_nhwc, int res_nhwc,
+                              int precision, osb_stream_t stream);
+int osb_conv2d_k3_tc_gru_prec_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift,
+                                  const float* residual, const float* mul_nhwc, const float* blend_z_nhwc, const float* blend_h_nhwc,
+                                  float* y, int B, int Cin, int Cout, int H, int W, int act, int out_nhwc, int res_nhwc,
+                                  long long res_bstride, int precision, osb_stream_t stream);
 /* ---- SURVEY.md section 8(f) row 4: remaining volume / regression flavours of the model zoo -------------------------------------
  * osb_gwc_volume_sum_fwd: osb_gwc_volume_fwd with a plain SUM over the K channels of a group instead of the mean:
  *   - CoExCostVolume(maxdisp, group)(x, y) (cost_volume/cost_volume.py:9-29) = sum flavour with D = maxdisp + 1, G = group;

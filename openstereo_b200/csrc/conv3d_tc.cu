@@ -596,21 +596,43 @@ int osb_conv3d_k3_tc_split_fwd(const float* x, const void* w_split, const float*
 
 int osb_conv2d_tc_kc(int Cin, int Cout, int W, int dilation) { return osb::select_conv3d_tc(Cin, Cout, W, dilation, false, false).kc; }
 
-int osb_conv2d_k3_tc_gru_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
-                             const float* mul_nhwc, const float* blend_z_nhwc, const float* blend_h_nhwc, float* y, int B, int Cin,
-                             int Cout, int H, int W, int act, int out_nhwc, int res_nhwc, long long res_bstride, osb_stream_t stream) {
+// Split terms per product of a precision (OSB_PREC_*), or 0 for an unknown value
+static int prec_terms(int precision) { return precision == OSB_PREC_FP32 ? 3 : precision == OSB_PREC_F16 ? 1 : 0; }
+
+int osb_conv2d_k3_tc_gru_prec_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift,
+                                  const float* residual, const float* mul_nhwc, const float* blend_z_nhwc, const float* blend_h_nhwc,
+                                  float* y, int B, int Cin, int Cout, int H, int W, int act, int out_nhwc, int res_nhwc,
+                                  long long res_bstride, int precision, osb_stream_t stream) {
+  OSB_REQUIRE(prec_terms(precision), "conv2d_k3_tc_gru: unknown precision %d", precision);
   // the ConvGRU epilogue is compiled into conv3d_tcg.cu's Cout = 128 instantiations (TcgCfg::GRU)
   OSB_REQUIRE(Cout == 128 && osb::select_conv3d_tc(Cin, Cout, W, 1, false, false).kc == 16,
               "conv2d_k3_tc_gru: no Cout = 128 kernel of conv3d_tcg.cu serves Cin=%d Cout=%d W=%d", Cin, Cout, W);
   osb::TcArgs a{x_nhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, 1, H, W, act, out_nhwc, res_nhwc, 0, 0, Cout};
   a.gru = 1, a.mul = mul_nhwc, a.blend_z = blend_z_nhwc, a.blend_h = blend_h_nhwc, a.res_bstride = res_bstride;
+  a.terms = prec_terms(precision);
   return conv3d_k3_tc_impl(a, 1, stream);
+}
+
+int osb_conv2d_k3_tc_gru_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
+                             const float* mul_nhwc, const float* blend_z_nhwc, const float* blend_h_nhwc, float* y, int B, int Cin,
+                             int Cout, int H, int W, int act, int out_nhwc, int res_nhwc, long long res_bstride, osb_stream_t stream) {
+  return osb_conv2d_k3_tc_gru_prec_fwd(x_nhwc, w_split, scale, shift, residual, mul_nhwc, blend_z_nhwc, blend_h_nhwc, y, B, Cin, Cout,
+                                       H, W, act, out_nhwc, res_nhwc, res_bstride, OSB_PREC_FP32, stream);
+}
+
+int osb_conv2d_k3_tc_prec_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
+                              float* y, int B, int Cin, int Cout, int H, int W, int dilation, int act, int out_nhwc, int res_nhwc,
+                              int precision, osb_stream_t stream) {
+  OSB_REQUIRE(prec_terms(precision), "conv2d_k3_tc: unknown precision %d", precision);
+  osb::TcArgs a{x_nhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, 1, H, W, act, out_nhwc, res_nhwc, 0, 0, Cout};
+  a.terms = prec_terms(precision);   // conv3d_tc.cu's instantiations (Cout <= 32 at W = 128) keep the 3-term product
+  return conv3d_k3_tc_impl(a, dilation, stream);
 }
 
 int osb_conv2d_k3_tc_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
                          float* y, int B, int Cin, int Cout, int H, int W, int dilation, int act, int out_nhwc, int res_nhwc,
                          osb_stream_t stream) {
-  return conv3d_k3_tc_impl({x_nhwc, w_split, scale, shift, residual, nullptr, y, B, Cin, Cout, 1, H, W, act, out_nhwc, res_nhwc, 0, 0,
-                            Cout}, dilation, stream);
+  return osb_conv2d_k3_tc_prec_fwd(x_nhwc, w_split, scale, shift, residual, y, B, Cin, Cout, H, W, dilation, act, out_nhwc, res_nhwc,
+                                   OSB_PREC_FP32, stream);
 }
 }

@@ -18,6 +18,11 @@
 // outside the image -- the conv's padding), the kw-stacked partial sums are un-shifted across the whole tile exactly as before and
 // only the 128 - 2 DIL interior columns that exist in the image are stored.  Work items gain a column-tile index (fastest), so
 // widths such as 240 (the reference's 544x960 timing shape), 312 (KITTI) or 160 take the tensor-core path with 1.6 % halo overhead.
+// SINGLE-TERM MODE (runtime, TcArgs::terms == 1; DESIGN.md section 4.20): the loaders stage only the hi part of each operand row
+// (same scale, saturation and overflow flag), the consumers issue one a_hi * b_hi MMA per half and K step instead of three, and the
+// kappa * n correction counts those MMAs.  The weight pack is the same; its lo half is not read.  Epilogues are unchanged (fp32).
+#include <type_traits>
+
 #include "tc_common.cuh"
 
 namespace osb {
@@ -43,6 +48,7 @@ struct TcgParams {
   int Wr, ctiles;          // general-width instantiations: image width and column tiles per row (whole-row kernels: W, 1)
   int ystride;             // channels per voxel of the channels-last y / residual / gate tensors (0 = COUT); > COUT when this launch
                            // produces a channel SLICE of a wider tensor (pointers pre-offset to the slice's first channel)
+  int terms;               // split terms per product (TcArgs::terms): 3, or 1 = hi parts only (staged and multiplied)
 };
 
 template <int COUT, int KC, int W, int TILES, int DIL = 1, bool GW = false>
@@ -198,38 +204,49 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
         }
       }
       float acc[2][C::NG3 / 2];
-      uint32_t accum = 0;
-      for (int kd = 0; kd < 3; ++kd) {
-        const int din = d + kd - 1;
-        if (din < 0 || din >= p.D) continue;
-        for (int ch = 0; ch < nchunk; ++ch, ++phc) {
+      // The MMA loop of one item, written once for both modes and entered per item on the (CTA-uniform) mode: each copy issues one
+      // fixed wgmma sequence, so no code path inside the loop has to reconcile two (a per-unit branch costs a synchronising dummy wgmma
+      // at every merge).  HI: single-term mode, a_hi * b_hi only.
+      auto mma_item = [&](auto hi_c) {
+        constexpr bool HI = decltype(hi_c)::value;
+        uint32_t accum = 0;
+        for (int kd = 0; kd < 3; ++kd) {
+          const int din = d + kd - 1;
+          if (din < 0 || din >= p.D) continue;
+          for (int ch = 0; ch < nchunk; ++ch, ++phc) {
 #pragma unroll
-          for (int s = C::S_FIRST; s <= C::S_LAST; ++s) {
-            if (!C::used(s)) continue;
-            const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
-            mbar_wait(&a_ready[slot], par);
-            const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
+            for (int s = C::S_FIRST; s <= C::S_LAST; ++s) {
+              if (!C::used(s)) continue;
+              const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
+              mbar_wait(&a_ready[slot], par);
+              const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
 #pragma unroll
-            for (int kh = 0; kh < 3; ++kh) {
-              if (C::tile_of(s, kh) != wg) continue;   // unit s meets slice kh for tile wg when s == wg * TS + (kh - 1) * DIL
-              const uint32_t bslot = (phc & 1) * 3 + kh;
-              mbar_wait(&b_full[bslot], (phc >> 1) & 1);
-              const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
-              wg_fence();
+              for (int kh = 0; kh < 3; ++kh) {
+                if (C::tile_of(s, kh) != wg) continue;   // unit s meets slice kh for tile wg when s == wg * TS + (kh - 1) * DIL
+                const uint32_t bslot = (phc & 1) * 3 + kh;
+                mbar_wait(&b_full[bslot], (phc >> 1) & 1);
+                const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
+                wg_fence();
 #pragma unroll
-              for (int ks = 0; ks < C::KSTEPS; ++ks)
-                wg_mma_split<C::NG3>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, TcK<KC>::A_LO, db0 + 2 * ks, TcK<KC>::B_LO, ks > 0 ? 1u : accum);
-              wg_commit();
-              wg_wait_all();
-              accum = 1;
-              wg_release(&b_empty[bslot], lane);
+                for (int ks = 0; ks < C::KSTEPS; ++ks) {
+                  if constexpr (HI) wg_mma_hi<C::NG3>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, db0 + 2 * ks, ks > 0 ? 1u : accum);
+                  else wg_mma_split<C::NG3>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, TcK<KC>::A_LO, db0 + 2 * ks, TcK<KC>::B_LO, ks > 0 ? 1u : accum);
+                }
+                wg_commit();
+                wg_wait_all();
+                accum = 1;
+                wg_release(&b_empty[bslot], lane);
+              }
+              wg_release(&a_empty[slot], lane);
+              ++unitc;
             }
-            wg_release(&a_empty[slot], lane);
-            ++unitc;
           }
         }
-      }
-      const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * C::KSTEPS * 3);   // tc_common.cuh: rz_kappa
+      };
+      if (p.terms == 1) mma_item(std::true_type{});
+      else mma_item(std::false_type{});
+      // n = MMAs issued into each accumulator: kd planes x chunks x 3 kh taps x k-steps x split terms (tc_common.cuh: rz_kappa)
+      const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * C::KSTEPS * p.terms);
       frag_unshift<C::G, DIL, W>(acc, xchg + (exc & 1) * (C::XCHG_FLOATS / 2), q, lane, corr, bar_xchg);
       ++exc;
       const size_t plane = (size_t)p.D * p.H * Wp;                                 // NCDHW channel stride
@@ -284,8 +301,13 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
       const uint32_t slot = u % C::STAGES, ph = (u / C::STAGES) & 1;   // u = global unit index
       mbar_wait_relaxed(&a_empty[slot], ph ^ 1);
       uint8_t* tile = a_buf + slot * C::UNIT_BYTES;
+      if (p.terms == 1) {                            // the hi part alone: the single-term MMAs read nothing else
 #pragma unroll
-      for (int j = 0; j < NLD; ++j) stage_f16_split<KC>(tile, v0 + VPL * j, c, v[j], amax);
+        for (int j = 0; j < NLD; ++j) stage_f16_hi<KC>(tile, v0 + VPL * j, c, v[j], amax);
+      } else {
+#pragma unroll
+        for (int j = 0; j < NLD; ++j) stage_f16_split<KC>(tile, v0 + VPL * j, c, v[j], amax);
+      }
       fence_proxy_async();
       mbar_arrive(&a_ready[slot]);
     };
@@ -355,7 +377,7 @@ template <int COUT, int KC, int W, int TILES, int DIL = 1, bool GW = false, bool
 static int launch_tcg(const TcArgs& a, cudaStream_t stream) {
   using C = TcgCfg<COUT, KC, W, TILES, DIL, GW>;
   TcgParams p{};
-  p.gate = a.gate ? a.gate : a.mul, p.ystride = a.ystride;
+  p.gate = a.gate ? a.gate : a.mul, p.ystride = a.ystride, p.terms = a.terms;
   p.blend_z = a.blend_z, p.blend_h = a.blend_h, p.res_bstride = a.res_bstride;
   p.hblocks = C::hblocks(a.H);
   p.Wr = GW ? a.W : W;

@@ -112,6 +112,12 @@ __device__ __forceinline__ void wg_mma_split(float (&acc)[2][N / 2], uint64_t da
     wgmma_f16<N>(acc[h], da + h * a_half, db, 1);
   }
 }
+// The same K = 16 step as one 16-bit product per half: a_hi * b_hi only (TcArgs::terms == 1, the autocast-precision mode).
+template <int N>
+__device__ __forceinline__ void wg_mma_hi(float (&acc)[2][N / 2], uint64_t da, uint32_t a_half, uint64_t db, uint32_t accumulate) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) wgmma_f16<N>(acc[h], da + h * a_half, db, accumulate);
+}
 // Consumer-side release of a ring slot / weight buffer read by the wgmmas just waited for: one arrival per consumer warp (barrier
 // count 4 x consumer warpgroups).  With two consumer warpgroups, each releases every slot it is handed, including the ones its own
 // tile does not read, and only after waiting for that slot's fill, so neither can arrive on a later phase than the one being filled.
@@ -282,6 +288,15 @@ __device__ __forceinline__ void stage_f16_split(uint8_t* tile, int row, int q, c
   const int sub = (q & 1) << 3, chunk = 4 * (q >> 2) + ((q >> 1) & 1);
   *reinterpret_cast<uint2*>(tile + swz_offset<KC>(row, chunk) + sub) = hi;
   *reinterpret_cast<uint2*>(tile + swz_offset<KC>(row, chunk + 2) + sub) = lo;
+}
+// stage_f16_split's hi part alone (TcArgs::terms == 1): the same scale, saturating conversion and amax; the lo chunk is neither
+// computed nor written (the single-term MMAs do not read it)
+template <int KC>
+__device__ __forceinline__ void stage_f16_hi(uint8_t* tile, int row, int q, const float4 v, float& amax) {
+  const float x0 = v.x * TC_ACT_SCALE, x1 = v.y * TC_ACT_SCALE, x2 = v.z * TC_ACT_SCALE, x3 = v.w * TC_ACT_SCALE;
+  amax = fmaxf(amax, fmaxf(fmaxf(fabsf(x0), fabsf(x1)), fmaxf(fabsf(x2), fabsf(x3))));
+  const int sub = (q & 1) << 3, chunk = 4 * (q >> 2) + ((q >> 1) & 1);
+  *reinterpret_cast<uint2*>(tile + swz_offset<KC>(row, chunk) + sub) = make_uint2(cvt_f16x2_sat(x0, x1), cvt_f16x2_sat(x2, x3));
 }
 // Lane -> operand row inside a warp-wide load of VPL = 128 / KC voxels (KC/4 lanes each), permuted so that the two STS.64 of
 // stage_f16_split are bank-conflict free per half-warp: SWIZZLE_128B rows (KC = 32, granule order) must differ in bit 1, SWIZZLE_64B rows
@@ -626,6 +641,10 @@ struct TcArgs {
   const float* blend_z = nullptr;
   const float* blend_h = nullptr;
   long long res_bstride = 0;
+  // Split terms per product (conv3d_tcg.cu only): 3 = the fp32-accurate 3xFP16 product; 1 = a_hi * b_hi alone, one fp16 MMA per
+  // product at autocast precision (OSB_PREC_F16 of osb_conv2d_k3_tc_prec_fwd / osb_conv2d_k3_tc_gru_prec_fwd).  conv3d_tc.cu's
+  // instantiations ignore it: the layers the selector routes there keep the 3-term product.
+  int terms = 3;
   bool slice() const { return ystride != 0 && ystride != Cout; }
 };
 // Launcher of one instantiation: the result of a family's selector (null: no instantiation serves the arguments).

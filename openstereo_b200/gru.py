@@ -67,9 +67,10 @@ class ConvGRUEngine(_BlockEngine):
         hn = ops.nchw_to_nhwc_cat([f32(h)])
         xn = ops.nchw_to_nhwc_cat([f32(t) for t in x_list])
         (zh, zxw, zb), (rhw, rxw, rb), (qh, qxw, qb) = self.w["z"], self.w["r"], self.w["q"]
-        zx = ops.conv2d_k3_tc_gru(xn, zxw, zb, ctx(cz), res_nhwc=False)
-        rx = ops.conv2d_k3_tc_gru(xn, rxw, rb, ctx(cr), res_nhwc=False)
-        qx = ops.conv2d_k3_tc_gru(xn, qxw, qb, ctx(cq), res_nhwc=False)
-        z = ops.conv2d_k3_tc_gru(hn, zh, None, zx, ops.ACT_SIGMOID)
-        rh = ops.conv2d_k3_tc_gru(hn, rhw, None, rx, ops.ACT_SIGMOID, mul=hn)
-        return ops.conv2d_k3_tc_gru(rh, qh, None, qx, ops.ACT_TANH, blend=(z, hn), out_nhwc=False)
+        p = self._precision()                            # "f16" under autocast with amp=True (update._BlockEngine)
+        zx = ops.conv2d_k3_tc_gru(xn, zxw, zb, ctx(cz), res_nhwc=False, precision=p)
+        rx = ops.conv2d_k3_tc_gru(xn, rxw, rb, ctx(cr), res_nhwc=False, precision=p)
+        qx = ops.conv2d_k3_tc_gru(xn, qxw, qb, ctx(cq), res_nhwc=False, precision=p)
+        z = ops.conv2d_k3_tc_gru(hn, zh, None, zx, ops.ACT_SIGMOID, precision=p)
+        rh = ops.conv2d_k3_tc_gru(hn, rhw, None, rx, ops.ACT_SIGMOID, mul=hn, precision=p)
+        return ops.conv2d_k3_tc_gru(rh, qh, None, qx, ops.ACT_TANH, blend=(z, hn), out_nhwc=False, precision=p)

@@ -1239,9 +1239,23 @@ def pack_tc_weight_2d(weight, kc):
     return pack_tc_weight(w5, kc)
 
 
-def conv2d_k3_tc(x_nhwc, w_split, scale=None, shift=None, residual=None, act=ACT_NONE, dilation=1, out_nhwc=True, res_nhwc=True):
+# precision= of the tensor-core 2D convolutions -> include/openstereo_b200.h OSB_PREC_*
+PRECISIONS = {"fp32": 0, "f16": 1}
+
+
+def _precision(precision):
+    if precision not in PRECISIONS:
+        raise ValueError("precision must be one of %s, not %r" % (sorted(PRECISIONS), precision))
+    return PRECISIONS[precision]
+
+
+def conv2d_k3_tc(x_nhwc, w_split, scale=None, shift=None, residual=None, act=ACT_NONE, dilation=1, out_nhwc=True, res_nhwc=True,
+                 precision="fp32"):
     """3x3 Conv2d (stride 1, padding = dilation) + folded BN + residual + activation on the tensor cores.  x_nhwc (B,H,W,Cin);
-    w_split = pack_tc_weight of the 3x3x3 weight that holds the 2D taps at kd = 1."""
+    w_split = pack_tc_weight of the 3x3x3 weight that holds the 2D taps at kd = 1.  precision="fp32": fp32-accurate 3xFP16
+    products; "f16": one fp16 MMA per product (autocast accuracy, osb_conv2d_k3_tc_prec_fwd) where a 16-channel-chunk kernel
+    serves the shape -- a 32-channel-chunk shape (conv2d_tc_kc(...) == 32) keeps the fp32-accurate product.  fp32 in and out."""
+    prec = _precision(precision)
     assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float32 and x_nhwc.is_contiguous() and x_nhwc.dim() == 4
     b, h, w, cin = x_nhwc.shape
     cout = w_split.cout
@@ -1251,8 +1265,12 @@ def conv2d_k3_tc(x_nhwc, w_split, scale=None, shift=None, residual=None, act=ACT
     y = torch.empty((b, h, w, cout) if out_nhwc else (b, cout, h, w), dtype=torch.float32, device=x_nhwc.device)
     if residual is not None:
         assert residual.is_contiguous() and residual.numel() == y.numel()
-    _call("osb_conv2d_k3_tc_fwd", x_nhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), y.data_ptr(), b, cin,
-          cout, h, w, dilation, act, int(out_nhwc), int(res_nhwc), _stream(y))
+    args = (x_nhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), y.data_ptr(), b, cin, cout, h, w, dilation, act,
+            int(out_nhwc), int(res_nhwc))
+    if prec:
+        _call("osb_conv2d_k3_tc_prec_fwd", *args, prec, _stream(y))
+    else:
+        _call("osb_conv2d_k3_tc_fwd", *args, _stream(y))
     return y
 
 
@@ -1274,11 +1292,14 @@ def nchw_to_nhwc_cat(tensors):
     return y
 
 
-def conv2d_k3_tc_gru(x_nhwc, w_split, shift=None, residual=None, act=ACT_NONE, mul=None, blend=None, out_nhwc=True, res_nhwc=True):
+def conv2d_k3_tc_gru(x_nhwc, w_split, shift=None, residual=None, act=ACT_NONE, mul=None, blend=None, out_nhwc=True, res_nhwc=True,
+                     precision="fp32"):
     """3x3 Conv2d (stride 1, padding 1) with the ConvGRU epilogue on the tensor cores (osb_conv2d_k3_tc_gru_fwd), Cout = 128:
         v = act(conv(x) + shift + residual);  v = v * mul;  y = h + z * (v - h) with (z, h) = blend.
     x_nhwc (B,H,W,Cin); mul and the blend operands (B,H,W,128) channels-last; an NCHW residual (res_nhwc=False) may be a channel
-    split() view of a wider (B, C', H, W) tensor (its batch stride goes to the kernel, no copy)."""
+    split() view of a wider (B, C', H, W) tensor (its batch stride goes to the kernel, no copy).  precision: as conv2d_k3_tc
+    (osb_conv2d_k3_tc_gru_prec_fwd); the epilogue is fp32 either way."""
+    prec = _precision(precision)
     assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float32 and x_nhwc.is_contiguous() and x_nhwc.dim() == 4
     b, h, w, cin = x_nhwc.shape
     cout = w_split.cout
@@ -1295,6 +1316,10 @@ def conv2d_k3_tc_gru(x_nhwc, w_split, shift=None, residual=None, act=ACT_NONE, m
     z, hh = blend if blend is not None else (None, None)
     for t in (mul, z, hh):
         assert t is None or (tuple(t.shape) == (b, h, w, cout) and t.is_contiguous() and t.dtype == torch.float32 and t.is_cuda)
-    _call("osb_conv2d_k3_tc_gru_fwd", x_nhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), _ptr(mul), _ptr(z), _ptr(hh),
-          y.data_ptr(), b, cin, cout, h, w, act, int(out_nhwc), int(res_nhwc), rbs, _stream(y))
+    args = (x_nhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), _ptr(mul), _ptr(z), _ptr(hh), y.data_ptr(), b, cin,
+            cout, h, w, act, int(out_nhwc), int(res_nhwc), rbs)
+    if prec:
+        _call("osb_conv2d_k3_tc_gru_prec_fwd", *args, prec, _stream(y))
+    else:
+        _call("osb_conv2d_k3_tc_gru_fwd", *args, _stream(y))
     return y

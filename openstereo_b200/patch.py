@@ -41,6 +41,13 @@ either.  The kernels have no backward, so any other call must NOT reach them sil
   strict=False           it runs the reference's own original code, gradients intact (tools/train.py).
 A CUDA inference call that no kernel serves (a shape or hyper-parameter outside the kernels' envelope) runs the reference's own
 code in both modes.  Every other call runs the library.
+
+Precision.  By default every patched layer computes fp32-accurate results, under autocast too, and returns the reference's dtypes.
+``patch(model, amp=True)`` (IGEVStereo, StereoBase, IGEV++, MonSter) lets the update block's tensor-core 3x3 convolutions run at
+the accuracy the reference's AMP YAMLs ask for: inside ``torch.autocast("cuda", ...)`` (fp16 or bf16) they issue one fp16 MMA per
+product instead of the three of the fp32-accurate split (gru.py, update.py: _BlockEngine; DESIGN.md section 4.20).  Outside
+autocast ``amp=True`` computes exactly what ``amp=False`` does.  The overrides installed, the shapes served and the dtypes returned
+are the same either way.
 """
 import functools
 import types
@@ -183,16 +190,17 @@ _UPDATE_ENGINES = {"encoder": MotionEncoderEngine, "geo_encoder0": GeoEncoderEng
 _IGEV_UPDATE = ("gru04", "gru08", "gru16", "encoder", "disp_head", "mask_feat_4")
 
 
-def _patch_update_block(block, strict, names=_IGEV_UPDATE):
+def _patch_update_block(block, strict, names=_IGEV_UPDATE, amp=False):
     """Per-instance ``forward`` overrides of the update block's modules `names`: the ConvGRUs ``gru04 / gru08 / gru16`` on
-    gru.ConvGRUEngine, the others on their update.py engine.  CUDA inference calls the kernels serve (the engines' serves()) run
-    the engine, the other shapes and hyper-parameters the reference's own forward."""
+    gru.ConvGRUEngine, the others on their update.py engine, each built with `amp` (autocast-precision tensor-core layers).  CUDA
+    inference calls the kernels serve (the engines' serves()) run the engine, the other shapes and hyper-parameters the reference's
+    own forward."""
     for name in names:
         mod = getattr(block, name)
         if name.startswith("gru"):
-            _override_convgru(mod, ConvGRUEngine(mod), strict)
+            _override_convgru(mod, ConvGRUEngine(mod, amp), strict)
         else:
-            _override_engine(mod, _UPDATE_ENGINES[name](mod), strict, name)
+            _override_engine(mod, _UPDATE_ENGINES[name](mod, amp), strict, name)
 
 
 def _patch_backbone(bb, net, extract, split):
@@ -310,14 +318,14 @@ def _patch_psmnet(model, strict, backbone=True):
     return model
 
 
-def _patch_stereobase(model, strict, backbone=True):
+def _patch_stereobase(model, strict, backbone=True, amp=False):
     # SURVEY.md section 8(f) rows 1 and 3: the per-GRU-iteration lookup and the convex up-sampling (stereobase_gru.py:172-209)
     _rebind_globals(model, strict, {"build_gwc_volume": _GWC, "build_concat_volume": _CONCAT, "disparity_regression": _REGRESSION,
                                     "CombinedGeoEncodingVolume": _COMBINED_GEO, "context_upsample": _UPSAMPLE})
     agg = StereoBaseAggregation(model.cost_agg)
     _override(model.cost_agg, "StereoBase Hourglass", strict, lambda x, features, return_multi=False: agg(x, features).to(x.dtype),
               serves=lambda x, features, return_multi=False: not return_multi)
-    _patch_update_block(model.update_block, strict)
+    _patch_update_block(model.update_block, strict, amp=amp)
     return model
 
 
@@ -334,18 +342,19 @@ def _patch_lightstereo(model, strict, backbone=True):
     return model
 
 
-def _patch_igev(model, strict, backbone=True):
+def _patch_igev(model, strict, backbone=True, amp=False):
     """IGEV-Stereo (BASELINE config 5; igev/igev_stereo.py:136-213): the gwc volume, the soft-argmin regression of the initial
     disparity, the per-GRU-iteration lookup of the combined geometry-encoding volume, the three ConvGRUs of the update block
     (``update_block.gru04 / gru08 / gru16``, gru.py), its motion encoder and disp / mask heads (``update_block.encoder / disp_head /
     mask_feat_4``, update.py) and the convex up-sampling.  The hourglass(8) and the feature nets stay the reference's cuDNN code.
-    Under autocast (the AMP YAML) the update block computes in fp32 and returns the reference's dtypes."""
+    Under autocast (the AMP YAML) the update block computes in fp32 and returns the reference's dtypes; with amp=True its
+    tensor-core layers compute at autocast accuracy instead (module docstring)."""
     _rebind_globals(model, strict, _IGEV_GLOBALS)
-    _patch_update_block(model.update_block, strict)
+    _patch_update_block(model.update_block, strict, amp=amp)
     return model
 
 
-def _patch_monster(model, strict, backbone=True):
+def _patch_monster(model, strict, backbone=True, amp=False):
     """MonSter (monster/monster.py, class MonSter): the stereo branch's IGEV-shaped hot path -- the gwc volume, the soft-argmin
     regression of the initial disparity, every lookup of the combined geometry-encoding volume (at disp, and at disp_mono_4x in
     the last 7 iterations), the disparity warps of features_right[0] (``disp_warp``; the kernel replays the border padding only),
@@ -353,11 +362,11 @@ def _patch_monster(model, strict, backbone=True):
     ``update_block_mix_mono`` and the convex up-sampling.  The Depth Anything encoder and decoders, feat_transfer*, the stems,
     corr_stem / corr_feature_att / cost_agg, the classifier, compute_scale_shift, REMP and the update blocks' own forward stay the
     reference's code; `backbone` has no effect.  Under autocast (the AMP YAML, bf16) every patched call computes in fp32 and
-    returns the reference's dtypes."""
+    returns the reference's dtypes; with amp=True the update blocks' tensor-core layers compute at autocast accuracy instead."""
     warp = (_disp_warp, lambda img, disp, padding_mode="border": padding_mode == "border")
     _rebind_globals(model, strict, dict(_IGEV_GLOBALS, disp_warp=warp))
     for block in (model.update_block, model.update_block_mix_stereo, model.update_block_mix_mono):
-        _patch_update_block(block, strict)
+        _patch_update_block(block, strict, amp=amp)
     return model
 
 
@@ -375,7 +384,7 @@ def _patch_igev_rt(model, strict, backbone=True):
     return model
 
 
-def _patch_igevpp(model, strict, backbone=True, aggregation=False):
+def _patch_igevpp(model, strict, backbone=True, aggregation=False, amp=False):
     """IGEV++ (igevpp/igevpp_stereo.py:162-249, class IGEVPPStereo): the gwc volume, the classifier Conv3d(8 -> 1) of the three
     disparity ranges (``classifier.forward``, which returns logits: the reference's own softmax follows), the strided regressions of
     the three initial disparities, the per-GRU-iteration multi-range lookup (one launch), the update block's ConvGRUs, geometry
@@ -384,13 +393,14 @@ def _patch_igevpp(model, strict, backbone=True, aggregation=False):
     layers or shapes the kernels do not implement run the module's own forward.  patch0 / patch1, the feature nets, cnet,
     selective_conv, disp_conv and BasicMultiUpdateBlock.forward itself (the selective-weight blend, cat, pool2x, interp) stay the
     reference's code, and so do the hourglasses by default; `backbone` has no effect.  Under autocast (the AMP YAML) every call
-    computes in fp32 and returns the reference's dtypes."""
+    computes in fp32 and returns the reference's dtypes; with amp=True the update block's tensor-core layers compute at autocast
+    accuracy instead (the hourglasses stay fp32-accurate)."""
     _rebind_globals(model, strict, {"build_gwc_volume": _GWC, "disparity_regression": _REGRESSION_INTERVAL,
                                     "Combined_Geo_Encoding_Volume": (MultiRangeGeoEncodingVolume, None),
                                     "context_upsample": _UPSAMPLE_KEEPDIM})
     head = StereoBaseCostHead(model.classifier)
     _override(model.classifier, "IGEV++ classifier", strict, lambda x: head.logits(x).to(x.dtype))
-    _patch_update_block(model.update_block, strict, _IGEV_UPDATE + ("geo_encoder0", "geo_encoder1", "geo_encoder2"))
+    _patch_update_block(model.update_block, strict, _IGEV_UPDATE + ("geo_encoder0", "geo_encoder1", "geo_encoder2"), amp=amp)
     if aggregation:
         for name in ("cost_agg0", "cost_agg1", "cost_agg2"):
             eng = IGEVPPAggregation(getattr(model, name))
@@ -499,14 +509,19 @@ _CASCADE_MODULES = {("casnet", "cas_psm"): "PSMNet", ("casnet", "cas_gwc"): "Gwc
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
              "IGEVStereo": _patch_igev, "IGEVRTtereo": _patch_igev_rt,
              "IGEVPPStereo": _patch_igevpp, "MonSter": _patch_monster, "CoEx": _patch_coex, "MSNet3D": _patch_msnet3d}
+# the patchers whose update blocks take amp=True
+_AMP_PATCHERS = (_patch_stereobase, _patch_igev, _patch_igevpp, _patch_monster)
 
 
-def patch(model, strict=True, backbone=True, aggregation=False):
+def patch(model, strict=True, backbone=True, aggregation=False, amp=False):
     """Rebind the hot path of a reference model instance in place and return it.  backbone=True (default) also routes the
     GwcNet / PSMNet 2D extractor's residual blocks to the wgmma conv kernels in CUDA inference calls (_patch_backbone);
     backbone=False leaves the extractor entirely to the reference's cuDNN code.  For the CasStereo models (casnet.cas_psm.PSMNet,
     casnet.cas_gwc.GwcNet) `backbone` has no effect: their FPN extractor always runs the reference's code.  aggregation=True
-    (IGEV++ only) also runs the three instance-normalised hourglasses on the library; off by default."""
+    (IGEV++ only) also runs the three instance-normalised hourglasses on the library; off by default.  amp=True (IGEVStereo,
+    StereoBase, IGEVPPStereo, MonSter) runs the update blocks' tensor-core convolutions at autocast accuracy -- one fp16 MMA per
+    product -- inside torch.autocast("cuda"), for users of the AMP YAMLs; outside autocast it changes nothing.  Off by default:
+    every patched layer is then fp32-accurate under autocast too."""
     if not isinstance(model, torch.nn.Module):
         raise TypeError("patch() expects an nn.Module")
     name = type(model).__name__
@@ -521,6 +536,11 @@ def patch(model, strict=True, backbone=True, aggregation=False):
         if patcher is not _patch_igevpp:
             raise NotImplementedError("patch(%s, aggregation=True): only IGEVPPStereo has an aggregation option" % name)
         patcher = functools.partial(_patch_igevpp, aggregation=True)
+    if amp:
+        if patcher not in _AMP_PATCHERS and getattr(patcher, "func", None) not in _AMP_PATCHERS:
+            raise NotImplementedError("patch(%s, amp=True): only the update blocks of %s have an autocast-precision mode"
+                                      % (name, ", ".join(sorted(k for k, v in _PATCHERS.items() if v in _AMP_PATCHERS))))
+        patcher = functools.partial(patcher, amp=True)
     if getattr(model, "_osb_patched", False):
         return model
     patcher(model, strict, backbone)

@@ -81,7 +81,21 @@ def _f32(t):
 
 class _BlockEngine(_Engine):
     """An update-block module's forward on the library: re-pack if needed, report a past fp16 overflow of the tensor-core
-    convolutions, run _run, schedule the next overflow read, return in _dtype(*args), the dtype the reference's forward returns."""
+    convolutions, run _run, schedule the next overflow read, return in _dtype(*args), the dtype the reference's forward returns.
+
+    amp=True (patch(model, amp=True)): under CUDA autocast, fp16 or bf16, the engine's tensor-core 3x3 layers run at autocast
+    accuracy -- one fp16 MMA per product (ops.conv2d_k3_tc precision="f16", DESIGN.md section 4.20) -- as the reference's autocast
+    convolutions do.  fp16 operands serve bf16 autocast too: finer mantissa, and the same range guard as the fp32 mode.  Outside
+    autocast, and with amp=False, every layer keeps the fp32-accurate product.  The CUDA-core layers, the dtypes returned and the
+    overflow monitor are the same either way."""
+
+    def __init__(self, module, amp=False):
+        super().__init__(module)
+        self.amp = bool(amp)
+
+    def _precision(self):
+        """precision= of this call's tensor-core launches."""
+        return "f16" if self.amp and torch.is_autocast_enabled("cuda") else "fp32"
 
     def __call__(self, *args):
         device = args[0].device
@@ -167,19 +181,21 @@ class MotionEncoderEngine(_BlockEngine):
                     and _is_conv(getattr(m, "conv" + s), c2 + cd, out, 3) for s in suffixes)
                 and plan[1](disp.shape[-1]))
 
-    def _branch(self, p, d, corr, flaw=None):
+    def _branch(self, p, d, corr, flaw=None, prec="fp32"):
         """One branch on the packed weights p: d is disp in fp32, channels-last intermediates, NCHW output."""
         cor = ops.conv3d_1x1(_f32(corr), p["c1"], None, p["bc1"], act=ops.ACT_RELU, x1=None if flaw is None else _f32(flaw))
-        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), p["c2"], None, p["bc2"], act=ops.ACT_RELU)
+        cor = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([cor]), p["c2"], None, p["bc2"], act=ops.ACT_RELU, precision=prec)
         dsp = ops.dwconv2d(d.expand(-1, p["d1"].shape[0], -1, -1).contiguous(), p["d1"], None, p["bd1"], act=ops.ACT_RELU)
-        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), self._convd2(p, d.shape[-1]), None, p["bd2"], act=ops.ACT_RELU)
-        part = ops.conv2d_k3_tc(cor, p["wc"], None, p["b"])
-        out = ops.conv2d_k3_tc(dsp, p["wd"], None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True)
+        dsp = ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([dsp]), self._convd2(p, d.shape[-1]), None, p["bd2"], act=ops.ACT_RELU,
+                               precision=prec)
+        part = ops.conv2d_k3_tc(cor, p["wc"], None, p["b"], precision=prec)
+        out = ops.conv2d_k3_tc(dsp, p["wd"], None, None, part, ops.ACT_RELU, out_nhwc=False, res_nhwc=True, precision=prec)
         out[:, -1:].copy_(d)
         return out
 
     def _run(self, *args):
-        outs = [self._branch(p, _f32(b[0]), *b[1:]) for p, b in zip(self.w, self._branches(args, self._layout()[1]))]
+        prec = self._precision()
+        outs = [self._branch(p, _f32(b[0]), *b[1:], prec=prec) for p, b in zip(self.w, self._branches(args, self._layout()[1]))]
         return outs[0] if len(outs) == 1 else torch.cat(outs, 1)
 
     def _dtype(self, *args):
@@ -207,9 +223,9 @@ class DispHeadEngine(_BlockEngine):
                 and route_ok(x.shape[-1]))
 
     def _run(self, x):
-        xn = ops.nchw_to_nhwc_cat([_f32(x)])
-        h0 = ops.conv2d_k3_tc(xn, self.w1[0], None, self.b1[0], act=ops.ACT_RELU, out_nhwc=False)
-        h1 = ops.conv2d_k3_tc(xn, self.w1[1], None, self.b1[1], act=ops.ACT_RELU, out_nhwc=False)
+        xn, prec = ops.nchw_to_nhwc_cat([_f32(x)]), self._precision()
+        h0 = ops.conv2d_k3_tc(xn, self.w1[0], None, self.b1[0], act=ops.ACT_RELU, out_nhwc=False, precision=prec)
+        h1 = ops.conv2d_k3_tc(xn, self.w1[1], None, self.b1[1], act=ops.ACT_RELU, out_nhwc=False, precision=prec)
         y = ops.conv3d_k3(h0.unsqueeze(2), self.w2[0], None, self.b2)
         return ops.conv3d_k3(h1.unsqueeze(2), self.w2[1], None, None, y).squeeze(2)
 
@@ -232,7 +248,8 @@ class MaskFeatEngine(_BlockEngine):
         kc = ops.conv2d_tc_kc(128, self.module[0].out_channels, x.shape[-1])
         if kc not in self.w:
             self.w[kc] = ops.pack_tc_weight_2d(self.module[0].weight, kc)
-        return ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([_f32(x)]), self.w[kc], None, self.b, act=ops.ACT_RELU, out_nhwc=False)
+        return ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([_f32(x)]), self.w[kc], None, self.b, act=ops.ACT_RELU, out_nhwc=False,
+                                precision=self._precision())                # kc = 32 (conv3d_tc.cu) keeps the 3-term product
 
 
 class GeoEncoderEngine(_BlockEngine):
@@ -256,7 +273,7 @@ class GeoEncoderEngine(_BlockEngine):
 
     def _run(self, geo):
         x = ops.conv3d_1x1(_f32(geo), self.g1, None, self.bg1, act=ops.ACT_RELU)
-        return ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([x]), self.g2, None, self.bg2, out_nhwc=False)[:, :96]
+        return ops.conv2d_k3_tc(ops.nchw_to_nhwc_cat([x]), self.g2, None, self.bg2, out_nhwc=False, precision=self._precision())[:, :96]
 
 
 # BasicDispEncoder's and BasicMotionEncoder_mix2's engine, by the module class's name

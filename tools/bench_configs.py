@@ -39,6 +39,11 @@
       aggregation=True) / patch(m) / cuDNN fp32 / AMP YAML in alternating rotation, ms per forward in cost_agg0..2 (CUDA events) and
       for the whole forward, and the EPE against the unpatched fp32 model
       (python tools/bench_configs.py --only c14 > results/h100_c14_igevpp_aggregation.jsonl)
+  c15 the update blocks under the AMP YAMLs: IGEVStereo @480x640, StereoBase, IGEV++ and MonSter (ViT-L) @256x512, batch 8 (the
+      reference's classes): patch(amp=True) / patch() under the AMP YAML's autocast / the unpatched AMP YAML / the unpatched fp32
+      model in alternating rotation, ms per forward in the ConvGRUs, in the encoders + heads (CUDA events around the module calls)
+      and for the whole forward, and the EPE against the unpatched fp32 model
+      (python tools/bench_configs.py --only c15 > results/h100_c15_amp.jsonl)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -877,6 +882,83 @@ def c14(iters, B=8, h=256, w=512):
     torch.cuda.empty_cache()
 
 
+def c15(iters, B=8):
+    """patch(model, amp=True) under the AMP YAMLs (DESIGN.md section 4.20): IGEV-Stereo (cfgs/igev AMP YAML, fp16 autocast) at 480x640,
+    StereoBase (cfgs/stereobase, AMP: fp16 autocast), IGEV++ (its AMP YAML, which autocasts itself) and MonSter (its AMP YAML's bf16
+    autocast, ViT-L as c13) at 256x512, batch 8.  Per model four variants in alternating rotation, medians of three: patch(amp=True)
+    and patch() of the AMP-YAML model under its autocast, the unpatched AMP-YAML model under it, and the unpatched fp32 model
+    (uniform YAML where the model has one; cuDNN fp32, TF32 off).  Per variant: ms per forward in the three ConvGRUs and in the
+    encoders + heads (encoder, disp_head, mask_feat_4 and IGEV++'s geo_encoder0..2) of every update block, CUDA events around the
+    module calls, the whole forward, and the EPE against the unpatched fp32 model."""
+    import contextlib
+    from oracle import _reference_shim as shim
+    from oracle import igevpp as oigpp
+    from oracle import monster as omon
+    from openstereo_b200.patch import patch
+    shim.install_timm_stub()
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+
+    def igev():
+        m = shim.load("stereo.modeling.models.igev.igev_stereo").IGEVStereo(shim.load_cfg("cfgs/igev/igev_sceneflow_amp.yaml").MODEL)
+        m.load_state_dict(si.seeded_state_dict(m.state_dict(), seed=12, scale={"classifier.weight": 8.0}))
+        return m.eval()
+
+    def stereobase():
+        cfg = shim.load_cfg("cfgs/stereobase/stereobase_sceneflow.yaml").MODEL
+        m = shim.load("stereo.modeling.models.stereobase.stereobase_gru").StereoBase(cfg)
+        m.load_state_dict(si.seeded_state_dict(m.state_dict(), seed=3, scale={"classifier.weight": 8.0}))
+        return m.eval()
+
+    # name, (h, w), build(AMP YAML?), autocast dtype of the AMP YAML (None: the model autocasts itself), input range, update blocks
+    models = [("IGEVStereo", (480, 640), lambda amp: igev(), torch.float16, 255.0, ("update_block",)),
+              ("StereoBase", (256, 512), lambda amp: stereobase(), torch.float16, 255.0, ("update_block",)),
+              ("IGEVPPStereo", (256, 512), lambda amp: oigpp.igevpp(oigpp.AMP_YAML if amp else oigpp.UNIFORM_YAML), None, 1.0,
+               ("update_block",)),
+              ("MonSter", (256, 512), lambda amp: omon.monster(omon.AMP_YAML if amp else omon.UNIFORM_YAML, encoder="vitl"),
+               omon.amp_dtype(omon.AMP_YAML), 1.0, ("update_block", "update_block_mix_stereo", "update_block_mix_mono"))]
+    groups = {"convgrus": ("gru04", "gru08", "gru16"),
+              "encoders_and_heads": ("encoder", "disp_head", "mask_feat_4", "geo_encoder0", "geo_encoder1", "geo_encoder2")}
+    for name, (h, w), build, dtype, scale, blocks in models:
+        variants = {"patched_amp": (patch(build(True).to(DEV), amp=True), dtype), "patched": (patch(build(True).to(DEV)), dtype),
+                    "amp_yaml": (build(True).to(DEV), dtype), "fp32": (build(False).to(DEV), None)}
+        gen = torch.Generator().manual_seed(31)
+        lo = 0.0 if scale == 255.0 else -1.0
+        x = {k: (torch.rand(B, 3, h, w, generator=gen) * (scale - lo) + lo).to(DEV) for k in ("left", "right")}
+
+        def forward(m, dt):
+            with torch.autocast("cuda", dtype=dt) if dt else contextlib.nullcontext():
+                return m(dict(x))["disp_pred"]
+        ms = {k: [] for k in variants}
+        stage = {k: [] for k in variants}
+        outs = {}
+        with torch.no_grad():
+            for _ in range(3):                                          # alternate: the variants share the GPU's state
+                for k, (m, dt) in variants.items():
+                    t, outs[k] = timeit(lambda: forward(m, dt), max(1, iters // 5), warm=1)
+                    ms[k].append(t)
+                    targets = {"%s.%s" % (b, n): getattr(getattr(m, b), n) for b in blocks for names in groups.values() for n in names
+                               if hasattr(getattr(m, b), n)}
+                    st = _stage_times(lambda: forward(m, dt), targets)
+                    stage[k].append({g: sum(v for n, v in st.items() if n.rsplit(".", 1)[-1] in names) for g, names in groups.items()})
+        med = lambda v: sorted(v)[1]
+        stage_ms = {k: {g: round(med([s[g] for s in v]), 2) for g in groups} for k, v in stage.items()}
+        fp32 = outs["fp32"].float()
+        emit(config="c15 update blocks under the AMP YAML of %s, B=%d @%dx%d (reference class + patch(amp=True))" % (name, B, h, w),
+             gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+             autocast=str(dtype) if dtype else "the model's own (fp16)",
+             forward_ms={k: round(med(v), 2) for k, v in ms.items()},
+             stage_ms_per_forward=stage_ms,
+             convgru_speedup_amp_vs_patched=round(stage_ms["patched"]["convgrus"] / stage_ms["patched_amp"]["convgrus"], 2),
+             encoders_heads_speedup_amp_vs_patched=round(stage_ms["patched"]["encoders_and_heads"]
+                                                         / stage_ms["patched_amp"]["encoders_and_heads"], 2),
+             epe_vs_fp32_px={k: float("%.3e" % (o.float() - fp32).abs().mean().item()) for k, o in outs.items() if k != "fp32"},
+             output_dtype={k: str(o.dtype) for k, o in outs.items()},
+             disparity_std_px=round(fp32.std().item(), 2))
+        del variants
+        torch.cuda.empty_cache()
+
+
 def _timed_call(events, fn, *args, **kw):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
@@ -943,7 +1025,7 @@ if __name__ == "__main__":
     for name in a.only.split(","):
         try:
             {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11,
-             "c12": c12, "c13": c13, "c14": c14}[name](a.iters)
+             "c12": c12, "c13": c13, "c14": c14, "c15": c15}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:
