@@ -328,6 +328,28 @@ int osb_conv2d_k3_tc_gru_prec_fwd(const float* x_nhwc, const void* w_split, cons
                                   const float* residual, const float* mul_nhwc, const float* blend_z_nhwc, const float* blend_h_nhwc,
                                   float* y, int B, int Cin, int Cout, int H, int W, int act, int out_nhwc, int res_nhwc,
                                   long long res_bstride, int precision, osb_stream_t stream);
+/* Modulated deformable 3x3 convolution (DCNv2, groups = 1) + folded BN + activation on the tensor cores: the forward of the
+ * reference's ModulatedDeformConvFunction (libs/AANet/deform_conv/deform_conv.py:113-150) as a gather mode of the general-width
+ * csrc/conv3d_tcg.cu instantiations (DESIGN.md section 4.21):
+ *     y[b,o,ho,wo] = act(scale[o] * sum_{c,tap} w[o,c,tap] * m * bilinear(x[b,:,:,c], ho*stride - padding + kh*dilation + dy,
+ *                                                                           wo*stride - padding + kw*dilation + dx) + shift[o])
+ * tap = 3 kh + kw; deformable group g = c / (Cin / deformable_groups); dy / dx = offset[b, 18 g + 2 tap + {0, 1}, ho, wo];
+ * m = mask[b, 9 g + tap, ho, wo], or 2 * sigmoid(that) with mask_mode = OSB_MASK_DOUBLE_SIGMOID (AANet's DeformConv2d with
+ * double_mask, applied to the raw offset_conv logits).  A sample outside (-1, H) x (-1, W) is 0, and each bilinear corner outside
+ * the image is 0 (dmcn_im2col_bilinear).  x (B,H,W,Cin) channels-last; offset and mask NCHW over the output extents (Ho, Wo) =
+ * ((H + 2 padding - 2 dilation - 1) / stride + 1, ...), offset_bstride / mask_bstride floats between their batches (>= dg*18*Ho*Wo
+ * / dg*9*Ho*Wo, so both may be channel slices of one (B, dg*27, Ho, Wo) tensor); w_split = the 2D packing at kd = 1 (Cout rows:
+ * 32, 64 or 128; a 16-channel layer is packed zero-padded to 32 rows and its caller keeps the first 16 output channels);
+ * y (B,Ho,Wo,Cout) or (B,Cout,Ho,Wo).  Products are 3xFP16 (fp32-accurate); the staged operand m * bilinear(x) must stay below 4094 in magnitude
+ * (the overflow counter; with m <= 2, |x| < 2047).  Cin % 16 == 0, Cin % deformable_groups == 0 with a multiple of 4 channels per
+ * group, stride 1 or 2, padding >= 0, dilation >= 1, act OSB_ACT_NONE / RELU / LEAKY; anything else returns OSB_EINVAL before any
+ * launch.  osb_tc_last_variant names the instantiation ("tcg<64,16,128,1,1,1,0>"). */
+#define OSB_MASK_PROB 0           /* the mask is used as given */
+#define OSB_MASK_DOUBLE_SIGMOID 1 /* the mask holds logits: m = 2 * sigmoid(mask) */
+int osb_mdconv2d_k3_tc_fwd(const float* x_nhwc, const float* offset, long long offset_bstride, const float* mask,
+                           long long mask_bstride, int mask_mode, const void* w_split, const float* scale, const float* shift, float* y,
+                           int B, int Cin, int Cout, int H, int W, int stride, int padding, int dilation,
+                           int deformable_groups, int act, int out_nhwc, osb_stream_t stream);
 /* ---- SURVEY.md section 8(f) row 4: remaining volume / regression flavours of the model zoo -------------------------------------
  * osb_gwc_volume_sum_fwd: osb_gwc_volume_fwd with a plain SUM over the K channels of a group instead of the mean:
  *   - CoExCostVolume(maxdisp, group)(x, y) (cost_volume/cost_volume.py:9-29) = sum flavour with D = maxdisp + 1, G = group;

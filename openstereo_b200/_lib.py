@@ -62,6 +62,7 @@ SIGNATURES = {
     "osb_conv2d_k3_tc_gru_fwd": [_f32p] * 9 + [_i] * 8 + [ctypes.c_longlong, _s],
     "osb_conv2d_k3_tc_prec_fwd": [_f32p] * 6 + [_i] * 10 + [_s],
     "osb_conv2d_k3_tc_gru_prec_fwd": [_f32p] * 9 + [_i] * 8 + [ctypes.c_longlong, _i, _s],
+    "osb_mdconv2d_k3_tc_fwd": [_f32p, _f32p, ctypes.c_longlong, _f32p, ctypes.c_longlong, _i] + [_f32p] * 4 + [_i] * 11 + [_s],
     "osb_ncdhw_to_ndhwc_slice": [_f32p, _f32p] + [_i] * 7 + [_s],
     "osb_ncdhw_to_ndhwc": [_f32p, _f32p, _i, _i, _i, _i, _i, _s],
     "osb_gwc_volume_sum_fwd": [_f32p, _f32p, _f32p, _i, _i, _i, _i, _i, _i, _s],

@@ -629,6 +629,37 @@ int osb_conv2d_k3_tc_prec_fwd(const float* x_nhwc, const void* w_split, const fl
   return conv3d_k3_tc_impl(a, dilation, stream);
 }
 
+int osb_mdconv2d_k3_tc_fwd(const float* x_nhwc, const float* offset, long long offset_bstride, const float* mask,
+                           long long mask_bstride, int mask_mode, const void* w_split, const float* scale, const float* shift, float* y,
+                           int B, int Cin, int Cout, int H, int W, int stride, int padding, int dilation,
+                           int deformable_groups, int act, int out_nhwc, osb_stream_t stream) {
+  OSB_REQUIRE(offset && mask, "mdconv2d_k3_tc: null offset or mask");
+  OSB_REQUIRE(B > 0 && H > 0 && W > 0 && Cin >= 16 && Cin % 16 == 0, "mdconv2d_k3_tc: bad shape B=%d Cin=%d H=%d W=%d", B, Cin, H, W);
+  OSB_REQUIRE(osb::select_mdconv_tc(Cout), "mdconv2d_k3_tc: no instantiation serves Cout=%d (32, 64 or 128 packed rows)", Cout);
+  OSB_REQUIRE(stride == 1 || stride == 2, "mdconv2d_k3_tc: stride %d (1 or 2)", stride);
+  OSB_REQUIRE(padding >= 0 && dilation >= 1 && padding <= 4096 && dilation <= 4096, "mdconv2d_k3_tc: padding %d dilation %d", padding,
+              dilation);
+  OSB_REQUIRE(deformable_groups >= 1 && Cin % deformable_groups == 0 && (Cin / deformable_groups) % 4 == 0,
+              "mdconv2d_k3_tc: %d deformable groups of %d channels (a multiple of 4 channels per group)", deformable_groups, Cin);
+  OSB_REQUIRE(mask_mode == OSB_MASK_PROB || mask_mode == OSB_MASK_DOUBLE_SIGMOID, "mdconv2d_k3_tc: unknown mask mode %d", mask_mode);
+  OSB_REQUIRE(act == OSB_ACT_NONE || act == OSB_ACT_RELU || act == OSB_ACT_LEAKY, "mdconv2d_k3_tc: unknown activation %d", act);
+  const int Ho = (H + 2 * padding - 2 * dilation - 1) / stride + 1, Wo = (W + 2 * padding - 2 * dilation - 1) / stride + 1;
+  OSB_REQUIRE(H + 2 * padding >= 2 * dilation + 1 && W + 2 * padding >= 2 * dilation + 1 && Ho > 0 && Wo > 0,
+              "mdconv2d_k3_tc: the input is too small for the 3x3 window");
+  const long long plane = (long long)Ho * Wo;
+  OSB_REQUIRE(offset_bstride >= 18ll * deformable_groups * plane && mask_bstride >= 9ll * deformable_groups * plane,
+              "mdconv2d_k3_tc: offset / mask batch strides %lld / %lld below dg*18*Ho*Wo / dg*9*Ho*Wo", offset_bstride, mask_bstride);
+  OSB_REQUIRE((long long)B * H * W * Cin < (1ll << 40) && (long long)B * offset_bstride < (1ll << 40) && plane < (1ll << 30),
+              "mdconv2d_k3_tc: tensors too large");
+  osb::TcArgs a{x_nhwc, w_split, scale, shift, nullptr, nullptr, y, B, Cin, Cout, 1, Ho, Wo, act, out_nhwc, 0, 0, 0, Cout};
+  a.dcn = 1, a.dcn_offset = offset, a.dcn_mask = mask, a.dcn_off_bstride = offset_bstride, a.dcn_mask_bstride = mask_bstride;
+  a.dcn_h = H, a.dcn_w = W, a.dcn_stride = stride, a.dcn_pad = padding, a.dcn_dil = dilation, a.dcn_dg = deformable_groups;
+  a.dcn_mask_mode = mask_mode;
+  const osb::TcLaunch launch = osb::select_mdconv_tc(Cout);
+  const int rc = osb::check_tc_args("mdconv2d_k3_tc", a, launch);
+  return rc != OSB_OK ? rc : launch(a, (cudaStream_t)stream);
+}
+
 int osb_conv2d_k3_tc_fwd(const float* x_nhwc, const void* w_split, const float* scale, const float* shift, const float* residual,
                          float* y, int B, int Cin, int Cout, int H, int W, int dilation, int act, int out_nhwc, int res_nhwc,
                          osb_stream_t stream) {

@@ -21,6 +21,13 @@
 // SINGLE-TERM MODE (runtime, TcArgs::terms == 1; DESIGN.md section 4.20): the loaders stage only the hi part of each operand row
 // (same scale, saturation and overflow flag), the consumers issue one a_hi * b_hi MMA per half and K step instead of three, and the
 // kappa * n correction counts those MMAs.  The weight pack is the same; its lo half is not read.  Epilogues are unchanged (fp32).
+// MODULATED DEFORMABLE GATHER (runtime, TcgParams::dcn, general-width instantiations only; DESIGN.md section 4.21): the 3x3 DCNv2
+// convolution of deform_conv_cuda_kernel.cu:571 (modulated_deformable_im2col + GEMM) as one launch.  Tiles are those of the 2D
+// convolution (128 output columns of one row; the halo columns are gathered and not stored).  The loader warps stage, per
+// (16-channel chunk, tap, tile), one unit of mask * bilinear(x) at the tap's offset position for the tile's 128 pixels, split hi / lo
+// as any operand row; the consumer issues one N = G MMA chain per unit with the tap's kw block of the unchanged weight slice into
+// the P0 accumulators, which move to P1 for the epilogue (no kw un-shift).  The weight stream, ring, epilogue and stores are those
+// of the one-plane 2D convolution.
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -49,6 +56,12 @@ struct TcgParams {
   int ystride;             // channels per voxel of the channels-last y / residual / gate tensors (0 = COUT); > COUT when this launch
                            // produces a channel SLICE of a wider tensor (pointers pre-offset to the slice's first channel)
   int terms;               // split terms per product (TcArgs::terms): 3, or 1 = hi parts only (staged and multiplied)
+  // modulated deformable gather (TcArgs::dcn; general-width instantiations): x is the (B, Hin, Win, Cin) input, H / Wr the output
+  int dcn;
+  const float* offset;
+  const float* mask;
+  long long off_bstride, mask_bstride;
+  int Hin, Win, stride, pad, dil, cpg, mask_mode;   // cpg: input channels per deformable group
 };
 
 template <int COUT, int KC, int W, int TILES, int DIL = 1, bool GW = false>
@@ -146,6 +159,7 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
   const int Wp = GW ? p.Wr : W;                     // image width = row pitch in voxels
   const int YS = (W < 32 && p.ystride) ? p.ystride : COUT;   // (compile-time COUT in the wide instantiations: slices exist at W' = 16 only)      // channel stride of the channels-last output / residual / gate
   const int ctiles = GW ? p.ctiles : 1;             // work item = (b, d, row block, column tile), column tile fastest
+  const bool dcn = GW && p.dcn;                     // modulated deformable gather (same tiles, halo columns gathered and not stored)
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
@@ -177,95 +191,153 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
     constexpr uint32_t A_HALF = 64 * C::ROWB / 16;  // descriptor offset of operand rows 64..127
     const uint32_t b16 = (smem_u32(b_buf) & 0x3FFFF) >> 4;
     const int q = warp & 3;                          // warp of the warpgroup
-    uint32_t unitc = 0, phc = 0, exc = 0;
-    for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
-      const int cg = (it % C::NG) * C::G;            // output channel group of this item
-      const int it0 = it / C::NG;
-      const int ct = it0 % ctiles;
-      const int hb = (it0 / ctiles) % p.hblocks;
-      const int d = (it0 / (ctiles * p.hblocks)) % p.D;
-      const int b = it0 / (ctiles * p.hblocks * p.D);
-      // Tile row m -> image row h (a tile below the image, odd H or H not a multiple of the item's rows, received its MMAs and
-      // releases like any other and stores nothing) and column (general widths: halo columns and columns beyond the image are not
-      // stored).  Returns whether the row is stored.
-      auto tile_row = [&](int m, int& h, int& col) {
-        h = C::row0(hb) + wg * C::TS + m / W;
-        col = GW ? ct * C::CSTEP - C::HALO + m : m % W;
-        return h < p.H && (!GW || (m >= C::HALO && m < 128 - C::HALO && col < Wp));
-      };
-      {
-        // the residual and the gate stream from HBM / L2: pull one voxel's channel group per thread into L2 while the tile is
-        // being accumulated
-        int h, col;
-        if (tile_row(q * 32 + lane, h, col)) {
-          const ptrdiff_t vox = (((ptrdiff_t)b * p.D + d) * p.H + h) * Wp + col;
-          if (p.residual && p.res_ndhwc) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + vox * YS + cg));
-          if (GATE && p.gate) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.gate + (((ptrdiff_t)b * p.H + h) * Wp + col) * YS + cg));
-        }
-      }
-      float acc[2][C::NG3 / 2];
-      // The MMA loop of one item, written once for both modes and entered per item on the (CTA-uniform) mode: each copy issues one
-      // fixed wgmma sequence, so no code path inside the loop has to reconcile two (a per-unit branch costs a synchronising dummy wgmma
-      // at every merge).  HI: single-term mode, a_hi * b_hi only.
-      auto mma_item = [&](auto hi_c) {
-        constexpr bool HI = decltype(hi_c)::value;
-        uint32_t accum = 0;
-        for (int kd = 0; kd < 3; ++kd) {
-          const int din = d + kd - 1;
-          if (din < 0 || din >= p.D) continue;
-          for (int ch = 0; ch < nchunk; ++ch, ++phc) {
-#pragma unroll
-            for (int s = C::S_FIRST; s <= C::S_LAST; ++s) {
-              if (!C::used(s)) continue;
-              const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
-              mbar_wait(&a_ready[slot], par);
-              const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
-#pragma unroll
-              for (int kh = 0; kh < 3; ++kh) {
-                if (C::tile_of(s, kh) != wg) continue;   // unit s meets slice kh for tile wg when s == wg * TS + (kh - 1) * DIL
-                const uint32_t bslot = (phc & 1) * 3 + kh;
-                mbar_wait(&b_full[bslot], (phc >> 1) & 1);
-                const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
-                wg_fence();
-#pragma unroll
-                for (int ks = 0; ks < C::KSTEPS; ++ks) {
-                  if constexpr (HI) wg_mma_hi<C::NG3>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, db0 + 2 * ks, ks > 0 ? 1u : accum);
-                  else wg_mma_split<C::NG3>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, TcK<KC>::A_LO, db0 + 2 * ks, TcK<KC>::B_LO, ks > 0 ? 1u : accum);
-                }
-                wg_commit();
-                wg_wait_all();
-                accum = 1;
-                wg_release(&b_empty[bslot], lane);
-              }
-              wg_release(&a_empty[slot], lane);
-              ++unitc;
-            }
+    // The item loop, written once and entered on the (launch-uniform) mode: the gather's copy has its own MMA loop and epilogue, so
+    // that its registers do not weigh on the convolution's copy, which is the code of the instantiations without the mode.
+    auto items = [&](auto gather_c) {
+      constexpr bool GATHER = decltype(gather_c)::value;
+      uint32_t unitc = 0, phc = 0, exc = 0;
+      for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+        const int cg = (it % C::NG) * C::G;            // output channel group of this item
+        const int it0 = it / C::NG;
+        const int ct = it0 % ctiles;
+        const int hb = (it0 / ctiles) % p.hblocks;
+        const int d = (it0 / (ctiles * p.hblocks)) % p.D;
+        const int b = it0 / (ctiles * p.hblocks * p.D);
+        // Tile row m -> image row h (a tile below the image, odd H or H not a multiple of the item's rows, received its MMAs and
+        // releases like any other and stores nothing) and column (general widths: halo columns and columns beyond the image are not
+        // stored).  Returns whether the row is stored.
+        auto tile_row = [&](int m, int& h, int& col) {
+          h = C::row0(hb) + wg * C::TS + m / W;
+          col = GW ? ct * C::CSTEP - C::HALO + m : m % W;
+          return h < p.H && (!GW || (m >= C::HALO && m < 128 - C::HALO && col < Wp));
+        };
+        {
+          // the residual and the gate stream from HBM / L2: pull one voxel's channel group per thread into L2 while the tile is
+          // being accumulated
+          int h, col;
+          if (tile_row(q * 32 + lane, h, col)) {
+            const ptrdiff_t vox = (((ptrdiff_t)b * p.D + d) * p.H + h) * Wp + col;
+            if (p.residual && p.res_ndhwc) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + vox * YS + cg));
+            if (GATE && p.gate) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.gate + (((ptrdiff_t)b * p.H + h) * Wp + col) * YS + cg));
           }
         }
-      };
-      if (p.terms == 1) mma_item(std::true_type{});
-      else mma_item(std::false_type{});
-      // n = MMAs issued into each accumulator: kd planes x chunks x 3 kh taps x k-steps x split terms (tc_common.cuh: rz_kappa)
-      const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * C::KSTEPS * p.terms);
-      frag_unshift<C::G, DIL, W>(acc, xchg + (exc & 1) * (C::XCHG_FLOATS / 2), q, lane, corr, bar_xchg);
-      ++exc;
-      const size_t plane = (size_t)p.D * p.H * Wp;                                 // NCDHW channel stride
-      const ptrdiff_t rbs = (C::GRU && p.res_bstride) ? (ptrdiff_t)p.res_bstride : (ptrdiff_t)(COUT * plane);   // NCDHW residual batch stride
-      auto rows = [&](int m, ptrdiff_t& yo, ptrdiff_t& ro, ptrdiff_t& go) {
-        int h, col;
-        const bool ok = tile_row(m, h, col);
-        const ptrdiff_t vox = (((ptrdiff_t)b * p.D + d) * p.H + h) * Wp + col;     // NDHWC voxel index
-        const ptrdiff_t sp = ((ptrdiff_t)d * p.H + h) * Wp + col;                  // offset inside an NCDHW channel plane
-        yo = p.out_ndhwc ? vox * YS : (ptrdiff_t)b * COUT * plane + sp;
-        ro = p.res_ndhwc ? vox * YS : (ptrdiff_t)b * rbs + sp;
-        go = (((ptrdiff_t)b * p.H + h) * Wp + col) * YS;
-        return ok;
-      };
-      frag_epilogue<C::G, C::GRU>(acc, lane, q, tiles + warp * FRAG_TP_FLOATS, s_scale + cg, s_shift + cg, p.act, p.y + (p.out_ndhwc ? (size_t)cg : cg * plane),
-                          p.out_ndhwc ? 1 : plane, p.residual ? p.residual + (p.res_ndhwc ? (size_t)cg : cg * plane) : nullptr,
-                          p.res_ndhwc ? 1 : plane, ((GATE || C::GRU) && p.gate) ? p.gate + cg : nullptr, rows, C::G, false, false, nullptr,
+        float acc[2][C::NG3 / 2];
+        // The MMA loop of one item, written once for both modes and entered per item on the (CTA-uniform) mode: each copy issues one
+        // fixed wgmma sequence, so no code path inside the loop has to reconcile two (a per-unit branch costs a synchronising dummy wgmma
+        // at every merge).  HI: single-term mode, a_hi * b_hi only.
+        auto mma_item = [&](auto hi_c) {
+          constexpr bool HI = decltype(hi_c)::value;
+          uint32_t accum = 0;
+          for (int kd = 0; kd < 3; ++kd) {
+            const int din = d + kd - 1;
+            if (din < 0 || din >= p.D) continue;
+            for (int ch = 0; ch < nchunk; ++ch, ++phc) {
+  #pragma unroll
+              for (int s = C::S_FIRST; s <= C::S_LAST; ++s) {
+                if (!C::used(s)) continue;
+                const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
+                mbar_wait(&a_ready[slot], par);
+                const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
+  #pragma unroll
+                for (int kh = 0; kh < 3; ++kh) {
+                  if (C::tile_of(s, kh) != wg) continue;   // unit s meets slice kh for tile wg when s == wg * TS + (kh - 1) * DIL
+                  const uint32_t bslot = (phc & 1) * 3 + kh;
+                  mbar_wait(&b_full[bslot], (phc >> 1) & 1);
+                  const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB) / 16);
+                  wg_fence();
+  #pragma unroll
+                  for (int ks = 0; ks < C::KSTEPS; ++ks) {
+                    if constexpr (HI) wg_mma_hi<C::NG3>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, db0 + 2 * ks, ks > 0 ? 1u : accum);
+                    else wg_mma_split<C::NG3>(acc, da0 + TcK<KC>::A_KSTEP * ks, A_HALF, TcK<KC>::A_LO, db0 + 2 * ks, TcK<KC>::B_LO, ks > 0 ? 1u : accum);
+                  }
+                  wg_commit();
+                  wg_wait_all();
+                  accum = 1;
+                  wg_release(&b_empty[bslot], lane);
+                }
+                wg_release(&a_empty[slot], lane);
+                ++unitc;
+              }
+            }
+          }
+        };
+        // The gather's MMA loop: per chunk, units (tap, tile) in that order, tap-major; this warpgroup multiplies its own tile's units
+        // with the tap's kw block of slice kh and releases every unit.  All nine taps accumulate into the P0 registers (columns
+        // 0 .. G - 1 of the 3G-wide tile: a 16-register block at the start of each half, which keeps the consumers' register
+        // allocation -- an N = G chain into the P1 block spilled); they move to P1, which the epilogue reads.
+        auto mma_gather = [&]() {
+          uint32_t accum = 0;
+          for (int ch = 0; ch < nchunk; ++ch, ++phc) {
+  #pragma unroll
+            for (int tap = 0; tap < 9; ++tap) {
+              const int kh = tap / 3, kw = tap % 3;
+  #pragma unroll
+              for (int t = 0; t < C::NT; ++t) {
+                const uint32_t slot = unitc % C::STAGES, par = (unitc / C::STAGES) & 1;
+                mbar_wait(&a_ready[slot], par);
+                if (t == wg) {
+                  const uint32_t bslot = (phc & 1) * 3 + kh;
+                  mbar_wait(&b_full[bslot], (phc >> 1) & 1);
+                  const uint64_t da0 = dbase | (uint64_t)((smem_u32(a_buf + slot * C::UNIT_BYTES) & 0x3FFFF) >> 4);
+                  const uint64_t db0 = dbase | (uint64_t)(b16 + (bslot * C::B_SUB + kw * C::G * C::ROWB) / 16);
+                  wg_fence();
+  #pragma unroll
+                  for (int ks = 0; ks < C::KSTEPS; ++ks)
+  #pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                      float(&p1)[C::G / 2] = *reinterpret_cast<float(*)[C::G / 2]>(&acc[h][0]);
+                      const uint64_t da = da0 + TcK<KC>::A_KSTEP * ks + h * A_HALF, db = db0 + 2 * ks;
+                      wgmma_f16<C::G>(p1, da + TcK<KC>::A_LO, db, ks > 0 ? 1u : accum);   // small terms first, as wg_mma_split
+                      wgmma_f16<C::G>(p1, da, db + TcK<KC>::B_LO, 1);
+                      wgmma_f16<C::G>(p1, da, db, 1);
+                    }
+                  wg_commit();
+                  wg_wait_all();
+                  accum = 1;
+                  if (kw == 2) wg_release(&b_empty[bslot], lane);
+                }
+                wg_release(&a_empty[slot], lane);
+                ++unitc;
+              }
+            }
+          }
+        };
+        if constexpr (GATHER) {
+          mma_gather();
+          // n = MMAs issued into the P1 accumulators: chunks x 9 taps x k-steps x 3 split terms (tc_common.cuh: rz_kappa)
+          const float corr = 1.f + p.kappa * (float)(nchunk * 9 * C::KSTEPS * 3);
+  #pragma unroll
+          for (int h = 0; h < 2; ++h)
+  #pragma unroll
+            for (int i = 0; i < C::G / 2; ++i) acc[h][C::G / 2 + i] = acc[h][i] * corr;
+        } else {
+          if (p.terms == 1) mma_item(std::true_type{});
+          else mma_item(std::false_type{});
+          // n = MMAs issued into each accumulator: kd planes x chunks x 3 kh taps x k-steps x split terms (tc_common.cuh: rz_kappa)
+          const float corr = 1.f + p.kappa * (float)(((d > 0) + 1 + (d + 1 < p.D)) * nchunk * 3 * C::KSTEPS * p.terms);
+          frag_unshift<C::G, DIL, W>(acc, xchg + (exc & 1) * (C::XCHG_FLOATS / 2), q, lane, corr, bar_xchg);
+          ++exc;
+        }
+        const size_t plane = (size_t)p.D * p.H * Wp;                                 // NCDHW channel stride
+        const ptrdiff_t rbs = (C::GRU && p.res_bstride) ? (ptrdiff_t)p.res_bstride : (ptrdiff_t)(COUT * plane);   // NCDHW residual batch stride
+        auto rows = [&](int m, ptrdiff_t& yo, ptrdiff_t& ro, ptrdiff_t& go) {
+          int h, col;
+          const bool ok = tile_row(m, h, col);
+          const ptrdiff_t vox = (((ptrdiff_t)b * p.D + d) * p.H + h) * Wp + col;     // NDHWC voxel index
+          const ptrdiff_t sp = ((ptrdiff_t)d * p.H + h) * Wp + col;                  // offset inside an NCDHW channel plane
+          yo = p.out_ndhwc ? vox * YS : (ptrdiff_t)b * COUT * plane + sp;
+          ro = p.res_ndhwc ? vox * YS : (ptrdiff_t)b * rbs + sp;
+          go = (((ptrdiff_t)b * p.H + h) * Wp + col) * YS;
+          return ok;
+        };
+        frag_epilogue<C::G, C::GRU>(acc, lane, q, tiles + warp * FRAG_TP_FLOATS, s_scale + cg, s_shift + cg, p.act, p.y + (p.out_ndhwc ? (size_t)cg : cg * plane),
+                            p.out_ndhwc ? 1 : plane, p.residual ? p.residual + (p.res_ndhwc ? (size_t)cg : cg * plane) : nullptr,
+                            p.res_ndhwc ? 1 : plane, ((GATE || C::GRU) && p.gate) ? p.gate + cg : nullptr, rows, C::G, false, false, nullptr,
                           p.blend_z ? p.blend_z + cg : nullptr, p.blend_h ? p.blend_h + cg : nullptr);
-    }
+      }
+    };
+    if (dcn) items(std::true_type{});
+    else items(std::false_type{});
   }
   // ---------------------------------------------------------------------------------------------- A-unit loaders
   // One loader WARP per unit, units round-robin over the NLW loader warps (unit u -> warp u % NLW, ring slot u % STAGES), so NLW
@@ -311,6 +383,68 @@ __global__ void __launch_bounds__(TcgCfg<COUT, KC, W, TILES, DIL, GW>::THREADS, 
       fence_proxy_async();
       mbar_arrive(&a_ready[slot]);
     };
+    // The gather's unit (chunk ch, tap, tile t): operand row v = output pixel (row h, column col) of tile t, its 4-channel quad c of
+    // chunk ch = mask * bilinear sample of x at the tap's offset position, as modulated_deformable_im2col_gpu_kernel and
+    // dmcn_im2col_bilinear compute it (deform_conv_cuda_kernel.cu:468-497, 571-633): zero outside (-1, Hin) x (-1, Win), each corner
+    // checked on its own.  A quad never spans two deformable groups (cpg % 4 == 0, checked by the entry point).
+    auto fill_gather = [&](int b, int h, int col_first, int ch, int tap, uint32_t u) {
+      const int kh = tap / 3, kw = tap % 3;
+      const int cin = ch * KC + c * 4, g = cin / p.cpg;
+      const size_t plane = (size_t)p.H * Wp;
+      const float* off = p.offset + b * p.off_bstride + (size_t)(g * 18 + 2 * tap) * plane + (size_t)h * Wp;
+      const float* msk = p.mask + b * p.mask_bstride + (size_t)(g * 9 + tap) * plane + (size_t)h * Wp;
+      const float* img = p.x + (size_t)b * p.Hin * p.Win * p.Cin + cin;
+      const int hb0 = h * p.stride - p.pad + kh * p.dil;
+      const uint32_t slot = u % C::STAGES, ph = (u / C::STAGES) & 1;
+      mbar_wait_relaxed(&a_empty[slot], ph ^ 1);
+      uint8_t* tile = a_buf + slot * C::UNIT_BYTES;
+#pragma unroll 4
+      for (int j = 0; j < NLD; ++j) {
+        const int col = col_first + VPL * j;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (h < p.H && (unsigned)col < (unsigned)Wp) {
+          const float dy = __ldg(off + col), dx = __ldg(off + plane + col), ml = __ldg(msk + col);
+          const float m = p.mask_mode ? 2.f * (1.f / (1.f + expf(-ml))) : ml;
+          const float hi = (float)hb0 + dy, wi = (float)(col * p.stride - p.pad + kw * p.dil) + dx;
+          if (hi > -1.f && wi > -1.f && hi < (float)p.Hin && wi < (float)p.Win) {
+            const int hl = (int)floorf(hi), wl = (int)floorf(wi), hh = hl + 1, wh = wl + 1;
+            const float lh = hi - hl, lw = wi - wl, uh = 1.f - lh, uw = 1.f - lw;
+            const float w1 = uh * uw, w2 = uh * lw, w3 = lh * uw, w4 = lh * lw;
+            const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+            auto at = [&](int y, int x) { return __ldg(reinterpret_cast<const float4*>(img + ((size_t)y * p.Win + x) * p.Cin)); };
+            const float4 v1 = (hl >= 0 && wl >= 0) ? at(hl, wl) : z;
+            const float4 v2 = (hl >= 0 && wh <= p.Win - 1) ? at(hl, wh) : z;
+            const float4 v3 = (hh <= p.Hin - 1 && wl >= 0) ? at(hh, wl) : z;
+            const float4 v4 = (hh <= p.Hin - 1 && wh <= p.Win - 1) ? at(hh, wh) : z;
+            v.x = (w1 * v1.x + w2 * v2.x + w3 * v3.x + w4 * v4.x) * m;
+            v.y = (w1 * v1.y + w2 * v2.y + w3 * v3.y + w4 * v4.y) * m;
+            v.z = (w1 * v1.z + w2 * v2.z + w3 * v3.z + w4 * v4.z) * m;
+            v.w = (w1 * v1.w + w2 * v2.w + w3 * v3.w + w4 * v4.w) * m;
+          }
+        }
+        stage_f16_split<KC>(tile, v0 + VPL * j, c, v, amax);   // amax sees the modulated operand: |m| <= 2 doubles the input's range
+      }
+      fence_proxy_async();
+      mbar_arrive(&a_ready[slot]);
+    };
+    if (dcn) {
+      constexpr int NUG = 9 * C::NT;                 // units per chunk: (tap, tile), tap-major as the consumers take them
+#pragma unroll 1
+      for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+        const int it0 = it / C::NG;
+        const int ct = it0 % ctiles;
+        const int hb = (it0 / ctiles) % p.hblocks;
+        const int b = it0 / (ctiles * p.hblocks);
+#pragma unroll 1
+        for (int ch = 0; ch < nchunk; ++ch) {
+#pragma unroll 1
+          for (int j = first; j < NUG; j += C::NLW)
+            fill_gather(b, C::row0(hb) + (j % C::NT) * C::TS, ct * C::CSTEP - C::HALO + v0, ch, j / C::NT, ubase + j);
+          ubase += NUG;
+          first = (first + C::NLW - NUG % C::NLW) % C::NLW;
+        }
+      }
+    } else
     for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
       const int it0 = it / C::NG;                    // every channel group of a tile stages the same units
       const int ct = it0 % ctiles;
@@ -382,9 +516,20 @@ static int launch_tcg(const TcArgs& a, cudaStream_t stream) {
   p.hblocks = C::hblocks(a.H);
   p.Wr = GW ? a.W : W;
   p.ctiles = GW ? (a.W + C::CSTEP - 1) / C::CSTEP : 1;
+  p.dcn = a.dcn, p.offset = a.dcn_offset, p.mask = a.dcn_mask, p.off_bstride = a.dcn_off_bstride, p.mask_bstride = a.dcn_mask_bstride;
+  p.Hin = a.dcn_h, p.Win = a.dcn_w, p.stride = a.dcn_stride, p.pad = a.dcn_pad, p.dil = a.dcn_dil, p.mask_mode = a.dcn_mask_mode;
+  p.cpg = a.Cin / a.dcn_dg;
   static const std::string variant = tc_variant_name("tcg<%d,%d,%d,%d,%d,%d,%d>", COUT, KC, W, TILES, DIL, (int)GW, (int)GATE);
   return launch_persistent<conv3d_tcg_kernel<COUT, KC, W, TILES, DIL, GW, GATE>>(
       a, p, (long long)a.B * a.D * p.hblocks * p.ctiles * C::NG, C::SMEM, variant.c_str(), stream);
+}
+
+TcLaunch select_mdconv_tc(int Cout) {
+  // the general-width instantiations of select_conv3d_tc below
+  if (Cout == 32) return launch_tcg<32, 16, 128, 1, 1, true>;
+  if (Cout == 64) return launch_tcg<64, 16, 128, 1, 1, true>;
+  if (Cout == 128) return launch_tcg<128, 16, 128, 1, 1, true>;
+  return nullptr;
 }
 
 TcRoute select_conv3d_tc(int Cin, int Cout, int W, int dilation, bool gate, bool slice) {

@@ -645,6 +645,15 @@ struct TcArgs {
   // product at autocast precision (OSB_PREC_F16 of osb_conv2d_k3_tc_prec_fwd / osb_conv2d_k3_tc_gru_prec_fwd).  conv3d_tc.cu's
   // instantiations ignore it: the layers the selector routes there keep the 3-term product.
   int terms = 3;
+  // Modulated deformable gather (osb_mdconv2d_k3_tc_fwd, conv3d_tcg.cu's general-width instantiations only): dcn = 1 stages, per
+  // 3x3 tap, mask * bilinear(x) at the offset positions instead of input rows.  H / W are then the OUTPUT extents and dcn_h /
+  // dcn_w the channels-last input's; offsets (B, dg*18, H, W) and mask (B, dg*9, H, W) are NCHW planes with their own batch strides
+  // (both may be slices of one offset_conv output); dcn_mask_mode 1 applies 2 * sigmoid(.) to the mask as it is read.
+  int dcn = 0;
+  const float* dcn_offset = nullptr;
+  const float* dcn_mask = nullptr;
+  long long dcn_off_bstride = 0, dcn_mask_bstride = 0;
+  int dcn_h = 0, dcn_w = 0, dcn_stride = 1, dcn_pad = 0, dcn_dil = 1, dcn_dg = 1, dcn_mask_mode = 0;
   bool slice() const { return ystride != 0 && ystride != Cout; }
 };
 // Launcher of one instantiation: the result of a family's selector (null: no instantiation serves the arguments).
@@ -723,6 +732,9 @@ struct TcRoute {
   int kc;
 };
 TcRoute select_conv3d_tc(int Cin, int Cout, int W, int dilation, bool gate, bool slice);
+// The general-width conv3d_tcg.cu instantiation that runs the modulated deformable gather (TcArgs::dcn) at packed width Cout
+// (32, 64 or 128), or null.
+TcLaunch select_mdconv_tc(int Cout);
 template <int COUT>
 int launch_tc(const TcArgs& a, cudaStream_t stream);   // conv3d_tc.cu
 

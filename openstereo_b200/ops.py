@@ -1231,12 +1231,13 @@ def conv2d_tc_kc(cin, cout, w, dilation=1):
     return int(_lib.lib.osb_conv2d_tc_kc(int(cin), int(cout), int(w), int(dilation)))
 
 
-def pack_tc_weight_2d(weight, kc):
-    """(Cout, Cin, 3, 3) Conv2d weight -> TcWeight of the one-plane 3x3x3 weight that holds its taps at kd = 1 (conv2d_k3_tc)."""
+def pack_tc_weight_2d(weight, kc, pad_cout_to=None):
+    """(Cout, Cin, 3, 3) Conv2d weight -> TcWeight of the one-plane 3x3x3 weight that holds its taps at kd = 1 (conv2d_k3_tc,
+    mdconv2d_k3_tc); pad_cout_to as pack_tc_weight."""
     w2 = weight.detach().float()
     w5 = w2.new_zeros(w2.shape[0], w2.shape[1], 3, 3, 3)
     w5[:, :, 1] = w2
-    return pack_tc_weight(w5, kc)
+    return pack_tc_weight(w5, kc, pad_cout_to=pad_cout_to)
 
 
 # precision= of the tensor-core 2D convolutions -> include/openstereo_b200.h OSB_PREC_*
@@ -1323,3 +1324,70 @@ def conv2d_k3_tc_gru(x_nhwc, w_split, shift=None, residual=None, act=ACT_NONE, m
     else:
         _call("osb_conv2d_k3_tc_gru_fwd", *args, _stream(y))
     return y
+
+
+# --------------------------------------------------------------------------- modulated deformable convolution (aanet.py)
+MASK_PROB, MASK_DOUBLE_SIGMOID = 0, 1      # include/openstereo_b200.h: OSB_MASK_PROB / OSB_MASK_DOUBLE_SIGMOID
+
+
+def mdconv_packed_rows(cout):
+    """Rows of the tensor-core packing that serves a modulated deformable conv with `cout` output channels (16 rides the
+    32-row instantiation zero-padded), or None when no instantiation does."""
+    return 32 if cout == 16 else cout if cout in (32, 64, 128) else None
+
+
+def mdconv2d_k3_tc(x_nhwc, offset, mask, w_split, scale=None, shift=None, stride=1, padding=1, dilation=1, deformable_groups=1,
+                   act=ACT_NONE, mask_mode=MASK_PROB, out_nhwc=False):
+    """Modulated deformable 3x3 Conv2d + folded BN + activation on the tensor cores (osb_mdconv2d_k3_tc_fwd).  x_nhwc (B,H,W,Cin)
+    fp32 contiguous; offset (B, dg*18, Ho, Wo) and mask (B, dg*9, Ho, Wo) fp32 with unit strides inside each batch (channel slices
+    of one offset_conv output are fine: only the batch strides go to the kernel); mask_mode=MASK_DOUBLE_SIGMOID reads mask as
+    logits, m = 2 * sigmoid(mask); w_split = pack_tc_weight_2d(weight, 16, pad_cout_to=32 for 16 channels); scale / shift:
+    per output channel (w_split.cout_real of them).  -> (B, cout_real, Ho, Wo), or (B, Ho, Wo, cout) when out_nhwc (no zero-padded
+    plan).  No backward."""
+    assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float32 and x_nhwc.is_contiguous() and x_nhwc.dim() == 4
+    b, h, w, cin = x_nhwc.shape
+    ho = (h + 2 * padding - 2 * dilation - 1) // stride + 1
+    wo = (w + 2 * padding - 2 * dilation - 1) // stride + 1
+    for t, n in ((offset, 18), (mask, 9)):
+        assert t.is_cuda and t.dtype == torch.float32 and tuple(t.shape) == (b, deformable_groups * n, ho, wo), (tuple(t.shape), n)
+        assert tuple(t.stride()[1:]) == (ho * wo, wo, 1), "offset / mask need unit strides inside each batch"
+    cout, real = w_split.cout, w_split.cout_real
+    assert not (out_nhwc and real != cout), "a zero-padded channel plan writes NCHW"
+    wptr, eff = _tc_args(w_split, cin, 16, scale)
+    if shift is not None and shift.numel() < cout:
+        shift = torch.cat((shift.float(), shift.new_zeros(cout - shift.numel()).float()))
+    shift = None if shift is None else shift.float().contiguous()
+    y = torch.empty((b, ho, wo, cout) if out_nhwc else (b, cout, ho, wo), dtype=torch.float32, device=x_nhwc.device)
+    _call("osb_mdconv2d_k3_tc_fwd", x_nhwc.data_ptr(), offset.data_ptr(), offset.stride(0), mask.data_ptr(), mask.stride(0),
+          int(mask_mode), wptr, _ptr(eff), _ptr(shift), y.data_ptr(), b, cin, cout, h, w, stride, padding, dilation,
+          deformable_groups, act, int(out_nhwc), _stream(y))
+    return y if real == cout else y[:, :real].contiguous()
+
+
+def modulated_deform_conv(input, offset, mask, weight, bias=None, stride=1, padding=0, dilation=1, groups=1, deformable_groups=1):
+    """The forward of the reference's modulated_deform_conv (libs/AANet/deform_conv/deform_conv.py:113-150, 187: DCNv2) on the
+    tensor cores: input (B, Cin, H, W), offset (B, dg*18, Ho, Wo), mask (B, dg*9, Ho, Wo) in [0, 1] or any real, weight
+    (Cout, Cin, 3, 3), optional bias (Cout,) -> (B, Cout, Ho, Wo) fp32, fp32-accurate products.  Served: fp32 CUDA tensors,
+    groups = 1, a 3x3 kernel, Cin a multiple of 16, Cout in {16, 32, 64, 128}, stride 1 or 2, Cin / dg a multiple of 4.  The
+    weight is packed on every call.  No backward: a call under autograd recording raises."""
+    _no_autograd("modulated_deform_conv", input, offset, mask, weight, bias)
+    for t, n in ((input, "input"), (offset, "offset"), (mask, "mask"), (weight, "weight")) + (((bias, "bias"),) if bias is not None else ()):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError("modulated_deform_conv: %s must be a tensor" % n)
+        if not t.is_cuda:
+            raise RuntimeError("modulated_deform_conv: %s is not on a CUDA device (openstereo_b200 has no CPU fallback)" % n)
+        if t.dtype != torch.float32:
+            raise TypeError("modulated_deform_conv: %s is %s; only fp32 is served" % (n, t.dtype))
+    _same_device(input, offset, mask, weight, bias)
+    stride, padding, dilation = (int(v[0]) if isinstance(v, (tuple, list)) else int(v) for v in (stride, padding, dilation))
+    cout, cin = weight.shape[:2]
+    if groups != 1 or tuple(weight.shape[2:]) != (3, 3) or input.dim() != 4 or input.shape[1] != cin:
+        raise ValueError("modulated_deform_conv: groups=1 with a (Cout, Cin, 3, 3) weight and a (B, Cin, H, W) input is served, "
+                         "not groups=%d, weight %s, input %s" % (groups, tuple(weight.shape), tuple(input.shape)))
+    rows = mdconv_packed_rows(cout)
+    if rows is None or cin % 16 or stride not in (1, 2) or cin % deformable_groups or (cin // deformable_groups) % 4:
+        raise ValueError("modulated_deform_conv: Cin=%d Cout=%d stride=%d deformable_groups=%d is not served" %
+                         (cin, cout, stride, deformable_groups))
+    x = input.permute(0, 2, 3, 1).contiguous()
+    wp = pack_tc_weight_2d(weight, 16, pad_cout_to=rows)
+    return mdconv2d_k3_tc(x, offset.contiguous(), mask.contiguous(), wp, None, bias, stride, padding, dilation, deformable_groups)

@@ -1,5 +1,5 @@
 """patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / IGEV-RT /
-IGEV++ / MonSter / CoEx / MSNet3D, and CasStereo's CasPSMNet / CasGwcNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
+IGEV++ / MonSter / CoEx / MSNet3D, CasStereo's CasPSMNet / CasGwcNet, and AANet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
 hot path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each needs its own
@@ -24,6 +24,8 @@ rebinding.  What each model rebinds:
               with aggregation=True also ``cost_agg0 / cost_agg1 / cost_agg2`` forward
 * CasStereo   ``get_cv`` (GetCostVolume) and every ``cost_agg[i]`` (CostAggregation) forward
 * CoEx        ``CostProcessor`` / ``DispProcessor`` / ``DispProcessor.regression`` forward
+* AANet       ``cost_volume`` and ``disparity_estimation`` forward; the ``disp_warp`` global of every ``refinement[i]``
+              (aanet/submodule.py:748, 801-824)
 * MSNet3D     one monolithic ``forward`` (MSNet3D.py:110-161), no processor modules: ``model.forward``, which keeps the
               reference's ``feature_extraction``
 
@@ -485,6 +487,37 @@ def _patch_coex(model, strict, backbone=True):
     return model
 
 
+def _aanet_disp_warp(img, disp, padding_mode="border"):
+    """(warped, None) with the reference's precondition (aanet/submodule.py:811); StereoDRNetRefinement.forward takes [0]."""
+    assert disp.min() >= 0
+    return ops.disp_warp(img, disp), None
+
+
+def _patch_aanet(model, strict, backbone=True):
+    """AANet (aanet/aanet.py, class aanet): the correlation pyramid (``cost_volume.forward``: one correlation volume per scale at
+    max_disp // 2^s), the soft-argmin of every scale (``disparity_estimation.forward``; match_similarity=False runs the reference's
+    code) and the disparity warp of each StereoDRNet refinement (its ``disp_warp`` global).  The deformable bottlenecks keep the
+    reference's DCNv2 extension, which the model cannot be built without and which is faster than the tensor-core gather mode
+    (aanet.DeformBottleneckEngine, DESIGN.md section 4.21): that engine is not installed here.  The FPN, the bottlenecks, the
+    cross-scale fusion layers and the refinements' convolutions stay the reference's code; `backbone` has no effect."""
+    cv = model.cost_volume
+
+    def cost_volume(left_feature_pyramid, right_feature_pyramid):
+        return [ops.correlation_volume(l, r, cv.max_disp // (2 ** s))
+                for s, (l, r) in enumerate(zip(left_feature_pyramid, right_feature_pyramid))]
+
+    _override(cv, "AANet CostVolumePyramid", strict, cost_volume,
+              serves=lambda left, right: cv.feature_similarity == "correlation")
+    de = model.disparity_estimation
+    _override(de, "AANet DisparityEstimation", strict, lambda cost: ops.softargmin(cost, cost.shape[1], keepdim=False),
+              serves=lambda cost: de.match_similarity and cost.dim() == 4)
+    for ref in model.refinement:
+        orig = type(ref).forward.__globals__["disp_warp"]
+        _rebind_methods(ref, {"disp_warp": _guard("disp_warp", strict, _aanet_disp_warp, orig, ref,
+                                                  lambda img, disp, padding_mode="border": padding_mode == "border")})
+    return model
+
+
 def _patch_msnet3d(model, strict, backbone=True):
     """MSNet3D (msnet/MSNet3D.py): everything after the 2D features in the eval forward -- the gwc volume, the MobileV2_Residual_3D
     blocks (one fused launch each), the hourglass transposed convs, classif3 and the trilinear x4 + softmax + regression tail
@@ -503,8 +536,10 @@ def _patch_msnet3d(model, strict, backbone=True):
     return model
 
 
-# CasStereo's classes are also named PSMNet / GwcNet: they are told apart by the module that defines them
-_CASCADE_MODULES = {("casnet", "cas_psm"): "PSMNet", ("casnet", "cas_gwc"): "GwcNet"}
+# Models routed by (package, module, class) of their defining module: CasStereo's classes are also named PSMNet / GwcNet, and
+# AANet's class is the bare lowercase `aanet`
+_MODULE_PATCHERS = {("casnet", "cas_psm", "PSMNet"): _patch_cascade, ("casnet", "cas_gwc", "GwcNet"): _patch_cascade,
+                    ("aanet", "aanet", "aanet"): _patch_aanet}
 
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
              "IGEVStereo": _patch_igev, "IGEVRTtereo": _patch_igev_rt,
@@ -517,7 +552,7 @@ def patch(model, strict=True, backbone=True, aggregation=False, amp=False):
     """Rebind the hot path of a reference model instance in place and return it.  backbone=True (default) also routes the
     GwcNet / PSMNet 2D extractor's residual blocks to the wgmma conv kernels in CUDA inference calls (_patch_backbone);
     backbone=False leaves the extractor entirely to the reference's cuDNN code.  For the CasStereo models (casnet.cas_psm.PSMNet,
-    casnet.cas_gwc.GwcNet) `backbone` has no effect: their FPN extractor always runs the reference's code.  aggregation=True
+    casnet.cas_gwc.GwcNet) and AANet (aanet.aanet.aanet) `backbone` has no effect: their FPN extractor always runs the reference's code.  aggregation=True
     (IGEV++ only) also runs the three instance-normalised hourglasses on the library; off by default.  amp=True (IGEVStereo,
     StereoBase, IGEVPPStereo, MonSter) runs the update blocks' tensor-core convolutions at autocast accuracy -- one fp16 MMA per
     product -- inside torch.autocast("cuda"), for users of the AMP YAMLs; outside autocast it changes nothing.  Off by default:
@@ -525,13 +560,14 @@ def patch(model, strict=True, backbone=True, aggregation=False, amp=False):
     if not isinstance(model, torch.nn.Module):
         raise TypeError("patch() expects an nn.Module")
     name = type(model).__name__
-    if _CASCADE_MODULES.get(tuple(type(model).__module__.split(".")[-2:])) == name:
-        patcher = _patch_cascade
+    key = tuple(type(model).__module__.split(".")[-2:]) + (name,)
+    if key in _MODULE_PATCHERS:
+        patcher = _MODULE_PATCHERS[key]
     elif name in _PATCHERS:
         patcher = _PATCHERS[name]
     else:
-        raise NotImplementedError("patch(): no hot-path drop-in for %s (supported: %s, and CasStereo's casnet.cas_psm.PSMNet / "
-                                  "casnet.cas_gwc.GwcNet)" % (name, sorted(_PATCHERS)))
+        raise NotImplementedError("patch(): no hot-path drop-in for %s (supported: %s, CasStereo's casnet.cas_psm.PSMNet / "
+                                  "casnet.cas_gwc.GwcNet and aanet.aanet.aanet)" % (name, sorted(_PATCHERS)))
     if aggregation:
         if patcher is not _patch_igevpp:
             raise NotImplementedError("patch(%s, aggregation=True): only IGEVPPStereo has an aggregation option" % name)

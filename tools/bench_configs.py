@@ -44,6 +44,10 @@
       model in alternating rotation, ms per forward in the ConvGRUs, in the encoders + heads (CUDA events around the module calls)
       and for the whole forward, and the EPE against the unpatched fp32 model
       (python tools/bench_configs.py --only c15 > results/h100_c15_amp.jsonl)
+  c16 AANet (the reference's class and its own DCNv2 extension), B=2 @576x960 fp32: patch() / patch() with the deformable
+      bottlenecks on the gather mode / unpatched in alternating rotation, ms per forward (median and range over the rounds) and in
+      the deformable convolutions (CUDA events around every call), and the EPE against the unpatched model
+      (python tools/bench_configs.py --only c16 > results/h100_c16_aanet.jsonl)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -959,6 +963,57 @@ def c15(iters, B=8):
         torch.cuda.empty_cache()
 
 
+def c16(iters, B=2, h=576, w=960, rounds=5):
+    """AANet (aanet/aanet.py, the reference's class with its own DCNv2 extension), batch 2 at the eval YAML's 576x960
+    (RightTopPad), fp32, TF32 off, seeded weights with offset_conv x30 (offsets of several pixels; the default init zeroes them).
+    Three variants in alternating rotation, `rounds` rounds of `iters` timed forwards each (after 2 warm-ups): patch(m) (the
+    correlation pyramid, soft-argmin and warps; the deformable bottlenecks keep the reference's extension), patch(m) with every
+    deformable bottleneck on aanet.DeformBottleneckEngine (the tensor-core gather mode), and the unpatched model.  Per variant: ms
+    per forward (median, min, max over the rounds) and ms per forward in the 15 deformable convolutions (CUDA events around every
+    ModulatedDeformConv call, or every ops.mdconv2d_k3_tc call, which also applies bn2 and the ReLU); EPE against the unpatched
+    model."""
+    from oracle import aanet as oa
+    from openstereo_b200.aanet import DeformBottleneckEngine
+    from openstereo_b200.patch import _override, patch
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    engines = patch(oa.aanet(offset_scale=30.0).to(DEV))
+    for mod in engines.modules():
+        if type(mod).__name__ in ("DeformBottleneck", "DeformSimpleBottleneck"):
+            eng = DeformBottleneckEngine(mod)
+            _override(mod, "AANet " + type(mod).__name__, True, eng, eng.serves)
+    variants = {"patched": patch(oa.aanet(offset_scale=30.0).to(DEV)), "patched_gather_engines": engines,
+                "reference": oa.aanet(offset_scale=30.0).to(DEV)}
+    gen = torch.Generator().manual_seed(16)
+    x = {"left": (torch.rand(B, 3, h, w, generator=gen) * 2 - 1).to(DEV), "right": (torch.rand(B, 3, h, w, generator=gen) * 2 - 1).to(DEV)}
+    ms = {k: [] for k in variants}
+    dms = {k: [] for k in variants}
+    outs = {}
+    with torch.no_grad():
+        for _ in range(rounds):
+            for k, m in variants.items():
+                t, outs[k] = timeit(lambda: m(dict(x))["disp_pred"], iters, warm=2)
+                ms[k].append(t)
+                dcn = [mod for mod in m.modules() if type(mod).__name__ == "ModulatedDeformConv"]
+                if k == "patched_gather_engines":
+                    st = _stage_times(lambda: m(dict(x)), {}, volume_fn="mdconv2d_k3_tc")
+                else:
+                    st = _stage_times(lambda: m(dict(x)), {"dcn%d" % i: mod for i, mod in enumerate(dcn)})
+                dms[k].append(sum(st.values()))
+    med = lambda v: sorted(v)[len(v) // 2]
+    spread = lambda v: {"median": round(med(v), 2), "min": round(min(v), 2), "max": round(max(v), 2)}
+    ref = outs["reference"]
+    emit(config="c16 AANet, B=%d @%dx%d, %d rounds x %d forwards (reference class + patch(); unpatched: the reference's "
+         "deform_conv_cuda, cuDNN fp32, TF32 off)" % (B, h, w, rounds, iters),
+         gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+         forward_ms={k: spread(v) for k, v in ms.items()},
+         deformable_ms_per_forward={k: spread(v) for k, v in dms.items()},
+         epe_vs_reference_px={k: float("%.3e" % (o - ref).abs().mean().item()) for k, o in outs.items() if k != "reference"},
+         disparity_std_px=round(ref.std().item(), 2))
+    del variants, engines
+    torch.cuda.empty_cache()
+
+
 def _timed_call(events, fn, *args, **kw):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
@@ -1025,7 +1080,7 @@ if __name__ == "__main__":
     for name in a.only.split(","):
         try:
             {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11,
-             "c12": c12, "c13": c13, "c14": c14, "c15": c15}[name](a.iters)
+             "c12": c12, "c13": c13, "c14": c14, "c15": c15, "c16": c16}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:
