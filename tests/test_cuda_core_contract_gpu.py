@@ -17,6 +17,17 @@ the instantiation it must reach, in the template spelling of the source.  For ev
   determinism  two launches of the same row are bit-identical (no kernel here uses atomics: a difference is a race);
   item loop    the grid-stride channels-last 1x1 launchers run at persistent-grid caps 1, 7 and uncapped, so one CTA walks many
                tiles with its staged weights and pipelined loads carried over: outputs are bit-identical across caps.
+Instance-norm rows (fam in-k3 / in-dc / in-pw: osb_conv3d_k3_in_fwd, osb_deconv3d_in_fwd, osb_conv3d_1x1_in_fwd) cover every
+instantiation the three entry points dispatch to, with partial tiles, rows of more than 64 CTAs along grid x (the slot-merge loop of
+moments_out takes several passes) and rows whose channels carry a mean offset of about 30 standard deviations (opt `offset`):
+  normalised input  leaky((x - mean) * rstd) * gate as the operand, ungated, gated, and gated with the scale / shift / activation
+               (and output sigmoid) the entry point accepts: run through the checks above (both store paths, bounds, determinism);
+  moments out  test_instance_norm_moments_out: raw output and per-(b, channel) (mean, rstd) of the stored output in sentinel-guarded
+               buffers, aligned and with y 4 bytes off (scalar epilogue) and aligned again: outputs AND statistics bit-identical, the
+               workspace's counters back to 0 after every launch; output per channel within 1e-5 of fp64, mean within 1e-5 of
+               |mean| + std and rstd within 1e-5 of fp64 statistics of the stored output.
+CONV_PARAMS_FIELDS classifies every field of struct ConvParams as an operand / geometry field or as the instance-norm mode
+(tests/test_host_logic_cpu.py).
 test_refusals: every input an entry point refuses returns its error code and launches nothing.
 """
 import re
@@ -103,9 +114,56 @@ REGISTRY = [
     # flavours.cu FeatureAtt gate, 8-pixel tiles (HW = 35 / 27): a padded channel plan, and hidden / output loops of several passes
     R("fa-pad", "fa", "feature_att_gate_kernel", 48, 24, (2, 5, 7), ch=24, cpad=32, ep="sc1 sh1 sh2", act=ACT_LEAKY),
     R("fa-wide", "fa", "feature_att_gate_kernel", 160, 144, (2, 3, 9), ch=80, cpad=160, ep="sh1 sc2 sh2", act=ACT_RELU),
+    # ---- instance-norm modes (conv3d.cu, in_params): dispatch_conv_k3's six instantiations, both transposed kernels, the 1x1 over
+    # one slab, two slabs and in 2D.  slots: k3 72 (4 x 6 x 3 tiles of 32 x 4 x 4), dc 70 (2 x 7 x 5 of 64 x 4 x 4), pw 65 (4160 voxel
+    # octets / 64).  offset: mean offset of the input channels, in standard deviations (cancellation in the statistics)
+    R("in-k3-co3-s1", "in-k3", "launch_conv_k3<1,1,1,4,4,8>", 13, 3, (2, 5, 6, 36), stride=1, act=ACT_RELU),
+    R("in-k3-co5-s2", "in-k3", "launch_conv_k3<2,1,1,2,4,4>", 11, 5, (2, 5, 9, 71), stride=2, act=ACT_LEAKY),
+    R("in-k3-co24-s1", "in-k3", "launch_conv_k3<1,8,3,4,4,8>", 13, 24, (2, 5, 6, 36), stride=1, act=ACT_LEAKY),
+    R("in-k3-co48-s2", "in-k3", "launch_conv_k3<2,8,3,2,4,4>", 11, 48, (2, 5, 9, 71), stride=2, act=ACT_RELU),
+    R("in-k3-co8-s1", "in-k3", "launch_conv_k3<1,8,4,4,4,8>", 13, 8, (2, 5, 6, 36), stride=1, act=ACT_LEAKY),
+    R("in-k3-co40-s1", "in-k3", "launch_conv_k3<1,8,4,4,4,8>", 16, 40, (2, 5, 6, 36), stride=1, act=ACT_RELU),
+    R("in-k3-co64-w70", "in-k3", "launch_conv_k3<1,8,4,4,4,8>", 8, 64, (1, 7, 10, 70), stride=1, act=ACT_LEAKY),
+    R("in-k3-slots", "in-k3", "launch_conv_k3<1,8,4,4,4,8>", 4, 16, (1, 9, 22, 100), stride=1, act=ACT_LEAKY),
+    R("in-k3-cancel", "in-k3", "launch_conv_k3<1,8,4,4,4,8>", 13, 32, (2, 5, 6, 36), stride=1, act=ACT_RELU, offset=30.0),
+    R("in-k3-co16-s2", "in-k3", "launch_conv_k3<2,8,4,2,4,4>", 11, 16, (2, 5, 9, 71), stride=2, act=ACT_LEAKY),
+    R("in-k3-co64-s2", "in-k3", "launch_conv_k3<2,8,4,2,4,4>", 32, 64, (2, 3, 5, 17), stride=2, act=ACT_RELU),
+    R("in-dc3", "in-dc", "launch_deconv<3,8>", 13, 20, (2, 3, 3, 34), k=3, act=ACT_RELU),
+    R("in-dc3-slots", "in-dc", "launch_deconv<3,8>", 4, 8, (1, 9, 13, 40), k=3, act=ACT_LEAKY),
+    R("in-dc4", "in-dc", "launch_deconv<4,8>", 12, 8, (2, 3, 5, 34), k=4, act=ACT_LEAKY),
+    R("in-dc4-w9", "in-dc", "launch_deconv<4,8>", 64, 32, (1, 2, 3, 9), k=4, act=ACT_RELU),
+    R("in-dc4-cancel", "in-dc", "launch_deconv<4,8>", 8, 16, (1, 3, 4, 32), k=4, act=ACT_LEAKY, offset=30.0),
+    R("in-pw-one", "in-pw", "conv3d_1x1_kernel", 40, 24, (2, 3, 5, 20), act=ACT_RELU6),
+    R("in-pw-two", "in-pw", "conv3d_1x1_kernel", 64, 32, (2, 3, 5, 20), c0=32, act=ACT_LEAKY, sigmoid=1),
+    R("in-pw-two-w30", "in-pw", "conv3d_1x1_kernel", 32, 16, (2, 6, 9, 30), c0=16, act=ACT_RELU),
+    R("in-pw-2d", "in-pw", "conv3d_1x1_kernel", 96, 48, (2, 1, 7, 44), act=ACT_LEAKY),
+    R("in-pw-2d-wide", "in-pw", "conv3d_1x1_kernel", 48, 96, (2, 1, 7, 44), act=ACT_RELU6, sigmoid=1),
+    R("in-pw-slots", "in-pw", "conv3d_1x1_kernel", 16, 40, (1, 8, 40, 100), c0=8, act=ACT_LEAKY),
+    R("in-pw-cancel", "in-pw", "conv3d_1x1_kernel", 24, 32, (2, 3, 6, 24), c0=16, act=ACT_RELU, offset=30.0),
 ]
 
-VEC_RULE = ("k3", "dc", "pw")           # entry points whose vec_ok rule picks the vector or the scalar epilogue
+VEC_RULE = ("k3", "dc", "pw", "in-k3", "in-dc", "in-pw")   # entry points whose vec_ok rule picks the vector or the scalar epilogue
+IN_FAMS = ("in-k3", "in-dc", "in-pw")
+
+# Every field of struct ConvParams (csrc/conv3d.cu): "" = an operand, geometry or launch field of every row, "in" = the instance-norm
+# modes, exercised by the in-* rows.  A field that is in neither fails tests/test_host_logic_cpu.py.
+CONV_PARAMS_FIELDS = {
+    **{f: "" for f in ("x x1 w scale shift residual gate y B Cin Cin0 Cout D H W Do Ho Wo tiles_w tiles_h tiles_d act sigmoid_out "
+                       "vec_ok").split()},
+    **{f: "in" for f in "in_stats in_gate in_stats1 in_gate1 stats part counter ws_floats ws_need".split()},
+}
+
+
+def in_grid(row):
+    """(CTAs along grid x = moments slots, channel blocks along grid y) of an instance-norm row's launch."""
+    b, d, h, w = row.shape
+    if row.fam == "in-k3":
+        s, tco, ncg, td, th = (int(v) for v in row.variant[len("launch_conv_k3<"):-1].split(",")[:5])
+        do, ho, wo = (d - 1) // s + 1, (h - 1) // s + 1, (w - 1) // s + 1
+        return -(-wo // 32) * -(-ho // th) * -(-do // td), -(-row.cout // (tco * ncg))
+    if row.fam == "in-dc":
+        return -(-2 * w // 64) * -(-2 * h // 4) * -(-2 * d // 4), -(-row.cout // 16)
+    return -(-d * h * -(-w // 8) // 64), -(-row.cout // 32)
 CAPPED = ("nd", "cat")                  # launchers whose grid follows osb_set_persistent_grid_cap
 
 
@@ -286,6 +344,9 @@ def cases(osb, row, g):
                                        row.cin, row.cout, d, h, w, k, act, s())
         return [Case(row.id, want, 1, fn, res, gate)]
 
+    if row.fam in IN_FAMS:
+        return in_cases(osb, row, g)
+
     if row.fam == "pw":
         b, d, h, w = row.shape
         c0 = o.get("c0", row.cin)
@@ -421,6 +482,110 @@ def cases(osb, row, g):
     return [Case(row.id, want, 3, fn, mag=mag)]
 
 
+def in_input(row, g, mean=1.0, spread=2.0):
+    """Input of an instance-norm row: spread * N(0, 1) + mean, plus opt `offset` standard deviations on every other channel."""
+    b, d, h, w = row.shape
+    x = torch.randn(b, row.cin, d, h, w, generator=g) * spread + mean
+    off = row.opts.get("offset", 0.0)
+    if off:
+        x[:, 0::2] += off * spread * torch.sign(torch.randn(1, (row.cin + 1) // 2, 1, 1, 1, generator=g))
+    return x
+
+
+def in_weight(row, g, cs):
+    """-> (fp32 weight in the reference's layout, packed weight on the device)."""
+    from openstereo_b200 import ops
+    if row.fam == "in-k3":
+        wt = torch.randn(row.cout, row.cin, 3, 3, 3, generator=g) * (27 * row.cin) ** -0.5 * cs.view(-1, 1, 1, 1, 1)
+        return wt, ops.pack_conv_weight(wt).cuda()
+    if row.fam == "in-dc":
+        k = row.opts["k"]
+        wt = torch.randn(row.cin, row.cout, k, k, k, generator=g) * (row.cin * k ** 3 / 8) ** -0.5 * cs.view(1, -1, 1, 1, 1)
+        return wt, ops.pack_deconv_weight(wt).cuda()
+    wt = torch.randn(row.cout, row.cin, 1, 1, 1, generator=g) * row.cin ** -0.5 * cs.view(-1, 1, 1, 1, 1)
+    return wt, wt.reshape(row.cout, row.cin).t().contiguous().cuda()
+
+
+def in_conv64(row, x, wt):
+    """fp64 convolution of an instance-norm row (the zero padding applies to the normalised, gated tensor)."""
+    x, wt = x.double(), wt.double()
+    if row.fam == "in-k3":
+        return F.conv3d(x, wt, stride=row.opts["stride"], padding=1)
+    if row.fam == "in-dc":
+        return F.conv_transpose3d(x, wt, stride=2, padding=1, output_padding=1 if row.opts["k"] == 3 else 0)
+    return F.conv3d(x, wt)
+
+
+def in_stats32(x):
+    """(B, C, 2) fp32 (mean, rstd) of x computed in fp64: the normalised-input cases feed exact statistics."""
+    y = x.double().flatten(2)
+    return torch.stack([y.mean(2), 1 / torch.sqrt(y.var(2, unbiased=False) + 1e-5)], -1).float().contiguous()
+
+
+def in_normalised64(x, st, gate):
+    """leaky((x - mean) * rstd) * gate in fp64 with the fp32 statistics the kernel reads; gate (B, C, H, W) broadcast over D."""
+    mean, rstd = st[..., 0].double().view(*st.shape[:2], 1, 1, 1), st[..., 1].double().view(*st.shape[:2], 1, 1, 1)
+    y = F.leaky_relu((x.double() - mean) * rstd, 0.01)
+    return y if gate is None else y * gate.double().unsqueeze(2)
+
+
+def in_call(osb, row, xs, wp, stats_in, gates, y, stats_out=None, ws=None, sc=None, sh=None, act=ACT_NONE, sigmoid=0):
+    """One launch of an instance-norm row.  xs / stats_in / gates: one entry per slab (the 1x1 takes two); pointers are addresses."""
+    lib, _ = osb
+    b, d, h, w = row.shape
+    s = torch.cuda.current_stream().cuda_stream
+    wsn = 0 if ws is None else ws[1]
+    ws = None if ws is None else ws[0]
+    if row.fam == "in-k3":
+        lib.call("osb_conv3d_k3_in_fwd", xs[0], wp, sc, sh, stats_in[0], gates[0], y, stats_out, ws, wsn, b, row.cin, row.cout, d, h, w,
+                 row.opts["stride"], act, s)
+    elif row.fam == "in-dc":
+        lib.call("osb_deconv3d_in_fwd", xs[0], wp, sc, sh, stats_in[0], gates[0], y, stats_out, ws, wsn, b, row.cin, row.cout, d, h, w,
+                 row.opts["k"], act, s)
+    else:
+        c0 = row.opts.get("c0", row.cin)
+        two = c0 < row.cin
+        lib.call("osb_conv3d_1x1_in_fwd", xs[0], xs[1] if two else None, c0, wp, sc, sh, stats_in[0], gates[0],
+                 stats_in[1] if two else None, gates[1] if two else None, y, stats_out, ws, wsn, b, row.cin, row.cout, d, h, w, act,
+                 sigmoid, s)
+
+
+def in_slabs(row, x):
+    c0 = row.opts.get("c0", row.cin)
+    return [x[:, :c0]] + ([x[:, c0:]] if c0 < row.cin else [])
+
+
+def in_cases(osb, row, g):
+    """Normalised-input cases of an instance-norm row: ungated, gated, gated + scale / shift / activation (+ output sigmoid)."""
+    o = row.opts
+    b, d, h, w = row.shape
+    cs = channel_scales(row.cout, g)
+    x = in_input(row, g)
+    wt, wp = in_weight(row, g, cs)
+    slabs = in_slabs(row, x)
+    stats = [in_stats32(t) for t in slabs]
+    gates = [torch.sigmoid(torch.randn(b, t.shape[1], h, w, generator=g)) for t in slabs]
+    dev = lambda t: None if t is None else t.float().contiguous().cuda()      # noqa: E731
+    xd, std = [dev(t) for t in slabs], [dev(t) for t in stats]
+    out = []
+    for name, gated, ep in (("ungated", False, False), ("gated", True, False), ("gated+epilogue", True, True)):
+        gs = gates if gated else [None] * len(slabs)
+        xn = torch.cat([in_normalised64(t, st, gt) for t, st, gt in zip(slabs, stats, gs)], 1)
+        conv = in_conv64(row, xn, wt)
+        sc = torch.rand(row.cout, generator=g) + 0.5 if ep else None
+        sh = 0.1 * cs * torch.randn(row.cout, generator=g) if ep else None
+        act, sig = (o.get("act", ACT_NONE), o.get("sigmoid", 0)) if ep else (ACT_NONE, 0)
+        want = ref_epilogue(conv, 1, sc, sh, None, act, None, sig)
+        mag = saturated_magnitude(in_conv64(row, xn.abs(), wt.abs()), 1, sc, sh, None, act, sig)
+        gd, scd, shd = [dev(t) for t in gs], dev(sc), dev(sh)
+
+        def fn(y, r, gt, gd=gd, scd=scd, shd=shd, act=act, sig=sig):
+            in_call(osb, row, [t.data_ptr() for t in xd], wp.data_ptr(), [t.data_ptr() for t in std], [ptr(t) for t in gd], y,
+                    sc=ptr(scd), sh=ptr(shd), act=act, sigmoid=sig)
+        out.append(Case("%s %s" % (row.id, name), want, 1, fn, mag=mag))
+    return out
+
+
 def seed(row, salt=0):
     return torch.Generator().manual_seed(salt + zlib.crc32(row.id.encode()) % 10000)
 
@@ -432,7 +597,8 @@ def test_accuracy_store_paths_bounds_determinism(osb, grid_cap, row):
     for case in cases(osb, row, seed(row)):
         runs = [("aligned", {}, 0), ("aligned again", {}, 0)]
         if row.fam in VEC_RULE:
-            assert case.want.shape[-1] % 4 == 0, "%s: Wo %% 4 != 0 would send the aligned run to the scalar path" % case.name
+            assert case.want.shape[-1] % 4 == 0 or row.fam in IN_FAMS, "%s: Wo %% 4 != 0 would send the aligned run to the scalar path" % (
+                case.name)
             runs.append(("y+4", {"y_off": 1}, 0))
             if case.res is not None:
                 runs.append(("residual+4", {"res_off": 1}, 0))
@@ -475,13 +641,81 @@ def test_routing(osb, row):
     from torch.profiler import ProfilerActivity, profile
     case = cases(osb, row, seed(row, 3))[0]
     buf = case.guarded()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        case.fn(buf.data_ptr() + 4 * GUARD, ptr(case.res), ptr(case.gate))
+    for _ in range(2):                  # a profiling window that delivered no kernel record at all is taken once more
         torch.cuda.synchronize()
-    names = sorted({e.name.replace(" ", "") for e in prof.events() if "osb::" in e.name})
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            case.fn(buf.data_ptr() + 4 * GUARD, ptr(case.res), ptr(case.gate))
+            torch.cuda.synchronize()
+        names = sorted({e.name.replace(" ", "") for e in prof.events() if "osb::" in e.name})
+        if names:
+            break
     want = re.compile(r"osb::%s\(" % re.escape(kernel_of(row.variant)))
     assert len(names) == 1 and want.search(names[0]), "%s: launched %s, expected %s" % (row.id, names, kernel_of(row.variant))
+
+
+IN_ROWS = [r for r in REGISTRY if r.fam in IN_FAMS]
+STATS_TOL = 1e-5            # |mean - mean64| / (|mean64| + std64) and |rstd / rstd64 - 1|
+
+
+@pytest.mark.timeout(120)
+@pytest.mark.parametrize("row", IN_ROWS, ids=[r.id for r in IN_ROWS])
+def test_instance_norm_moments_out(osb, row):
+    lib, _ = osb
+    g = seed(row, 5)
+    b, d, h, w = row.shape
+    x = in_input(row, g, mean=0.5, spread=1.0)
+    wt, wp = in_weight(row, g, channel_scales(row.cout, g))
+    want = in_conv64(row, x, wt)
+    op, param = {"in-k3": (0, row.opts.get("stride")), "in-dc": (1, row.opts.get("k")), "in-pw": (2, 0)}[row.fam]
+    need = lib.lib.osb_conv3d_in_workspace_floats(op, b, row.cout, d, h, w, param)
+    slots, blocks = in_grid(row)
+    assert need == 3 * b * row.cout * slots + b * blocks, "%s: workspace %d for %d slots" % (row.id, need, slots)
+    n_y, n_s = want.numel(), 2 * b * row.cout
+    # one buffer of sentinels: | y region (+1 float for the shifted run) | statistics | workspace |, GUARD sentinels around each
+    o_y = GUARD
+    o_s = o_y + (n_y + 1 + 3) // 4 * 4 + GUARD
+    o_w = o_s + (n_s + 3) // 4 * 4 + GUARD
+    buf = torch.full((o_w + (need + 3) // 4 * 4 + GUARD,), SENTINEL, device="cuda")
+    buf[o_w:o_w + need] = 0.0                                     # zero-filled before its first use, reused by every launch
+    xs = [t.contiguous().cuda() for t in in_slabs(row, x)]
+    sent = torch.tensor([SENTINEL]).view(torch.int32).item()
+    runs = []
+    for what, y_off in (("aligned", 0), ("y+4", 1), ("aligned again", 0)):
+        lead = o_y + y_off
+        buf[o_y:o_y + n_y + 1] = SENTINEL
+        buf[lead:lead + n_y] = float("nan")
+        buf[o_s:o_s + n_s] = float("nan")
+        in_call(osb, row, [t.data_ptr() for t in xs], wp.data_ptr(), [None, None], [None, None], buf.data_ptr() + 4 * lead,
+                stats_out=buf.data_ptr() + 4 * o_s, ws=(buf.data_ptr() + 4 * o_w, need))
+        torch.cuda.synchronize()
+        outside = torch.ones(buf.numel(), dtype=torch.bool, device="cuda")
+        outside[lead:lead + n_y] = False
+        outside[o_s:o_s + n_s] = False
+        outside[o_w:o_w + need] = False
+        assert (buf.view(torch.int32)[outside] == sent).all(), "%s %s: a store left the output, statistics or workspace" % (row.id, what)
+        y, st = buf[lead:lead + n_y], buf[o_s:o_s + n_s]
+        assert not torch.isnan(y).any() and not torch.isnan(st).any(), "%s %s: outputs or statistics never written" % (row.id, what)
+        assert (buf[o_w + need - b * blocks:o_w + need].view(torch.int32) == 0).all(), "%s %s: counters not re-armed" % (row.id, what)
+        runs.append((y.view(torch.int32).clone(), st.view(torch.int32).clone()))
+    for what, (y_bits, s_bits) in zip(("y+4 (scalar epilogue)", "aligned again"), runs[1:]):
+        assert torch.equal(runs[0][0], y_bits), "%s: output of the %s run differs bit-wise" % (row.id, what)
+        assert torch.equal(runs[0][1], s_bits), "%s: statistics of the %s run differ bit-wise" % (row.id, what)
+    y = runs[0][0].view(torch.float32).cpu().double().view(want.shape)
+    err = (y - want).abs().amax(dim=(0, 2, 3, 4))
+    scale = want.abs().amax(dim=(0, 2, 3, 4))
+    bad = (err > TOL * scale).nonzero().flatten().tolist()
+    assert not bad, "%s: raw output channels %s exceed %g of their own max" % (row.id, bad[:8], TOL)
+    yf = y.flatten(2)
+    mean64, var64 = yf.mean(2), yf.var(2, unbiased=False)          # statistics OF THE STORED OUTPUT
+    std64 = var64.sqrt()
+    st = runs[0][1].view(torch.float32).cpu().double().view(b, row.cout, 2)
+    err_m = ((st[..., 0] - mean64).abs() / (mean64.abs() + std64)).max().item()
+    err_r = (st[..., 1] * torch.sqrt(var64 + 1e-5) - 1).abs().max().item()
+    ratio = (mean64.abs() / std64).max().item()
+    print("\n%-16s slots %d  max |mean| / std %.1f  mean err %.2e  rstd err %.2e" % (row.id, slots, ratio, err_m, err_r))
+    if row.opts.get("offset") and row.fam == "in-pw":                # (k3 / dc: the zero padding spreads the means over the border)
+        assert ratio >= 15, "%s: the cancellation row's channels have |mean| / std of at most %.1f" % (row.id, ratio)
+    assert err_m <= STATS_TOL and err_r <= STATS_TOL, "%s: mean err %.2e, rstd err %.2e" % (row.id, err_m, err_r)
 
 
 def refusals(P, s):

@@ -322,3 +322,64 @@ def test_kernel_contract_registry_matches_sources():
         defined |= set(re.findall(_GLOBAL, _csrc(os.path.basename(path))))
     assert len(defined) >= 30
     assert not defined - covered, "__global__ functions with no row in any contract registry: %s" % sorted(defined - covered)
+
+
+def _struct_fields(name, struct):
+    """Field names of `struct <struct> { ... };` in csrc/<name> (member functions skipped)."""
+    import re
+    body = re.search(r"struct\s+%s\s*\{(.*?)\n\};" % struct, _csrc(name), re.S).group(1)
+    body = re.sub(r"[\w:<>]+\s+\w+\s*\([^()]*\)\s*(?:const\s*)?\{[^{}]*\}", "", body)      # bool slice() const { ... }
+    fields = []
+    for stmt in body.split(";"):
+        stmt = re.sub(r"=[^,]*", "", stmt).strip()
+        if stmt:
+            fields += [re.findall(r"\w+", part)[-1] for part in stmt.split(",")]
+    return fields
+
+
+def test_tc_runtime_modes_have_contract_rows():
+    """Every field of struct TcArgs is classified in TC_ARGS_FIELDS (tests/test_tc_contract_gpu.py) as an operand / geometry field or
+    as a runtime mode; every mode has its rows: one per instantiation MODE_VARIANTS lists for it (test_mode_sweep checks that list on
+    the GPU), and the split rows cover every accepted (input, output, residual) layout combination."""
+    from test_tc_contract_gpu import MODE_VARIANTS, REGISTRY, SPLIT_COMBOS, TC_ARGS_FIELDS
+    fields = _struct_fields("tc_common.cuh", "TcArgs")
+    assert len(fields) == len(set(fields)) and {"x", "terms", "dcn_mask_mode", "res_bstride"} <= set(fields)
+    assert set(fields) == set(TC_ARGS_FIELDS), "TcArgs fields not classified: %s; classified fields that are gone: %s" % (
+        sorted(set(fields) - set(TC_ARGS_FIELDS)), sorted(set(TC_ARGS_FIELDS) - set(fields)))
+    modes = {r.mode for r in REGISTRY} - {""}
+    assert {m for m in TC_ARGS_FIELDS.values() if m} <= modes and modes == set(MODE_VARIANTS)
+    for mode, variants in MODE_VARIANTS.items():
+        rows = [r for r in REGISTRY if r.mode == mode]
+        assert {r.variant for r in rows} == variants, "mode %s: instantiations without a row: %s" % (
+            mode, sorted(variants - {r.variant for r in rows}))
+        if mode != "split":
+            assert len({r.variant for r in rows}) == len(rows), "mode %s: two rows for one instantiation" % mode
+    assert {r.opt for r in REGISTRY if r.mode == "split"} == SPLIT_COMBOS
+    dcn = [r for r in REGISTRY if r.kind == "dcn"]
+    assert {r.opt[0] for r in dcn} == {1, 2} and {r.opt[1] for r in dcn} == {1, 2, 3}
+    assert {r.cin // r.opt[2] for r in dcn} >= {4, 8, 16}
+
+
+def test_instance_norm_modes_have_contract_rows():
+    """Every field of struct ConvParams is classified in CONV_PARAMS_FIELDS (tests/test_cuda_core_contract_gpu.py); the instance-norm
+    rows reach every instantiation of the three _in_ entry points (dispatch_conv_k3's six, both transposed kernels, the 1x1 over one
+    slab, two slabs and in 2D), each family has a row of more than 64 CTAs along grid x (not a multiple of 32) and a row with a large
+    mean offset."""
+    import re
+    from test_cuda_core_contract_gpu import CONV_PARAMS_FIELDS, IN_FAMS, REGISTRY, in_grid
+    fields = _struct_fields("conv3d.cu", "ConvParams")
+    assert len(fields) == len(set(fields)) and {"in_stats", "ws_need", "vec_ok"} <= set(fields)
+    assert set(fields) == set(CONV_PARAMS_FIELDS), "ConvParams fields not classified: %s; classified fields that are gone: %s" % (
+        sorted(set(fields) - set(CONV_PARAMS_FIELDS)), sorted(set(CONV_PARAMS_FIELDS) - set(fields)))
+    rows = [r for r in REGISTRY if r.fam in IN_FAMS]
+    src = _csrc("conv3d.cu")
+    dispatch = re.search(r"static int dispatch_conv_k3\(.*?\n\}", src, re.S).group(0)
+    k3 = {"launch_conv_k3<%s>" % a.replace(" ", "") for a in re.findall(r"launch_conv_k3\s*<([^<>]*)>", dispatch)}
+    assert len(k3) == 6 and {r.variant for r in rows if r.fam == "in-k3"} == k3
+    assert {r.variant for r in rows if r.fam == "in-dc"} == {"launch_deconv<3,8>", "launch_deconv<4,8>"}
+    pw = [r for r in rows if r.fam == "in-pw"]
+    assert any(r.opts.get("c0", r.cin) < r.cin for r in pw) and any(r.opts.get("c0", r.cin) == r.cin and r.shape[1] > 1 for r in pw)
+    assert any(r.shape[1] == 1 for r in pw)
+    for fam in IN_FAMS:
+        assert any(in_grid(r)[0] > 64 and in_grid(r)[0] % 32 for r in rows if r.fam == fam), "%s: no many-slot row" % fam
+        assert any(r.opts.get("offset", 0) >= 20 for r in rows if r.fam == fam), "%s: no cancellation row" % fam

@@ -17,6 +17,18 @@ last column tile holding a single valid column) and the instantiation the select
                output stays finite;
   kappa . n    with kappa = 9e-7 the ratio y(kappa) / y(0) - 1 recovers the MMA count n each epilogue applied; it must equal the n
                counted here from the convolution geometry: (kd, kh) tap rows issued x Cin / 16 k-steps x 3 split products.
+Runtime modes of existing instantiations are rows too (Row.mode; MODE_VARIANTS lists the instantiations each mode reaches, which
+test_mode_sweep checks on the GPU and tests/test_host_logic_cpu.py checks against the rows; TC_ARGS_FIELDS classifies every field of
+struct TcArgs as an operand / geometry field of every row or as the mode whose rows exercise it):
+  f16          osb_conv2d_k3_tc_prec_fwd at OSB_PREC_F16: accuracy against fp64 of the operands exactly as staged (fp16_rn(16 x) / 16
+               and the weights' hi halves), kappa . n with one split term; tc<32> / tc<16> return the OSB_PREC_FP32 bits;
+  gru-*        osb_conv2d_k3_tc_gru_prec_fwd (suffix -f16: single-term products): sigmoid . mul / tanh + blend, an NCHW residual that
+               is a channel view of a wider tensor (res_bstride), NHWC and NCHW outputs;
+  dcn, dcn-2sig  osb_mdconv2d_k3_tc_fwd with mask mode 0 / 1: offsets at and beyond every edge, integer offsets, negative masks,
+               strides 1 and 2, dilations 1..3, 4 / 8 / 16 channels per deformable group, one row of 120 work items; kappa . n =
+               Cin / 16 x 9 taps x 3 at every output pixel; the range guard sees the modulated operand (m <= 2);
+  split        osb_conv3d_k3_tc_split_fwd, one row per (input, output, residual) layout combination of tc<32>: accuracy against fp64
+               of the decoded split operands, a split output checked between 16-bit sentinels and decoded.
 """
 import math
 import zlib
@@ -25,23 +37,30 @@ from collections import namedtuple
 import pytest
 import torch
 import torch.nn.functional as F
+from torchvision.ops import deform_conv2d
 
 pytestmark = pytest.mark.gpu
 
-ACT_NONE, ACT_RELU, ACT_LEAKY = 0, 1, 2
+ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_SIGMOID, ACT_TANH = 0, 1, 2, 4, 5
+PREC_FP32, PREC_F16 = 0, 1              # include/openstereo_b200.h: OSB_PREC_*
+NCDHW, NDHWC, SPLIT = 0, 1, 2           # include/openstereo_b200.h: OSB_LAYOUT_*
+SENTINEL16 = -0x2b2e                    # 16-bit sentinel of a split (fp16) output buffer (0xd4d2: fp16 -77.1)
+RES_CTOT, RES_COFF = 144, 16            # GRU rows: the NCHW residual is channels 16 .. 16 + Cout of a (B, 144, H, W) tensor
 GUARD = 1024                            # sentinel floats on each side of an output region (4 KB, keeps 16-byte alignment)
 SENTINEL = -1234.5
 KAPPA_TEST = 9e-7
 
-# kind: s1 = Conv3d k3 s1 p1 (s1n: same with an NCDHW input), 2d2 = Conv2d k3 dilation 2 (a one-plane volume), s2 = Conv3d k3 s2 p1,
-# dc3 / dc4 = ConvTranspose3d k3 s2 p1 op1 / k4 s2 p1.  cout = packed channels; shape = INPUT (B, D, H, W); ys / coff = channel
-# stride and first channel of a channel slice (0: the output is the whole tensor); creal < cout: zero-padded channel plan whose
-# NCDHW output holds only the real channels; gate: FeatureAtt gate operand.
-Row = namedtuple("Row", "id kind cin cout shape variant ys coff creal gate")
+# kind: s1 = Conv3d k3 s1 p1 (s1n: same with an NCDHW input), 2d1 / 2d2 = Conv2d k3 dilation 1 / 2 (a one-plane volume), s2 = Conv3d
+# k3 s2 p1, dc3 / dc4 = ConvTranspose3d k3 s2 p1 op1 / k4 s2 p1, dcn = modulated deformable Conv2d k3, padding = dilation.  cout =
+# packed channels; shape = INPUT (B, D, H, W); ys / coff = channel stride and first channel of a channel slice (0: the output is the
+# whole tensor); creal < cout: zero-padded channel plan whose NCDHW output holds only the real channels; gate: FeatureAtt gate
+# operand; mode: "" (the entry point of the kind) or a runtime mode (module docstring); opt: dcn (stride, dilation, deformable
+# groups), split (input, output, residual layout; residual None = no residual).
+Row = namedtuple("Row", "id kind cin cout shape variant ys coff creal gate mode opt")
 
 
-def R(rid, kind, cin, cout, shape, variant, ys=0, coff=0, creal=None, gate=False):
-    return Row(rid, kind, cin, cout, shape, variant, ys, coff, cout if creal is None else creal, gate)
+def R(rid, kind, cin, cout, shape, variant, ys=0, coff=0, creal=None, gate=False, mode="", opt=None):
+    return Row(rid, kind, cin, cout, shape, variant, ys, coff, cout if creal is None else creal, gate, mode, opt)
 
 
 REGISTRY = [
@@ -83,7 +102,64 @@ REGISTRY = [
     R("tcdc3-32-w64", "dc3", 32, 32, (1, 2, 3, 64), "tcdc<32,16,64,1,0,3>"),
     R("tcdc3-64-gw", "dc3", 16, 64, (1, 2, 2, 128), "tcdc<64,16,128,1,1,3>"),
     R("tcdc3-32-gw", "dc3", 16, 32, (1, 2, 2, 128), "tcdc<32,16,128,1,1,3>"),
+    # ---- runtime modes
+    # single-term fp16 (osb_conv2d_k3_tc_prec_fwd, OSB_PREC_F16): every instantiation the 2D entry point reaches (test_mode_sweep)
+    R("f16-tc32", "2d1", 32, 32, (1, 1, 5, 128), "tc<32>", mode="f16"),
+    R("f16-tc16-head", "2d1", 64, 16, (2, 1, 4, 128), "tc<16>", creal=3, mode="f16"),
+    R("f16-tcg96-w16", "2d1", 32, 96, (1, 1, 11, 16), "tcg<96,16,16,1,1,0,1>", mode="f16"),
+    R("f16-tcg64-w16", "2d1", 32, 64, (1, 1, 11, 16), "tcg<64,16,16,1,1,0,1>", mode="f16"),
+    R("f16-tcg64-w64", "2d1", 32, 64, (1, 1, 5, 64), "tcg<64,16,64,1,1,0,0>", mode="f16"),
+    R("f16-tcg64-w32", "2d1", 48, 64, (1, 1, 7, 32), "tcg<64,16,32,1,1,0,0>", mode="f16"),
+    R("f16-tcg128-w32", "2d1", 32, 128, (1, 1, 7, 32), "tcg<128,16,32,1,1,0,0>", mode="f16"),
+    R("f16-tcg96-w32", "2d1", 32, 96, (1, 1, 7, 32), "tcg<96,16,32,1,1,0,0>", mode="f16"),
+    R("f16-tcg64-w128", "2d1", 32, 64, (1, 1, 3, 128), "tcg<64,16,128,1,1,0,0>", mode="f16"),
+    R("f16-tcg128-w128", "2d1", 32, 128, (1, 1, 3, 128), "tcg<128,16,128,1,1,0,0>", mode="f16"),
+    R("f16-tcg32-gw", "2d1", 32, 32, (1, 1, 3, 127), "tcg<32,16,128,1,1,1,0>", mode="f16"),
+    R("f16-tcg64-gw", "2d1", 16, 64, (1, 1, 3, 127), "tcg<64,16,128,1,1,1,0>", mode="f16"),
+    R("f16-tcg128-gw", "2d1", 16, 128, (1, 1, 3, 127), "tcg<128,16,128,1,1,1,0>", mode="f16"),
+    R("f16-tcg128-dil2", "2d2", 32, 128, (2, 1, 5, 128), "tcg<128,16,128,1,2,0,0>", mode="f16"),
+    # ConvGRU epilogue (osb_conv2d_k3_tc_gru_prec_fwd): every Cout = 128 instantiation, both gate activations, both precisions
+    *[R("%s-%s" % (m, v), "2d1", cin, 128, shape, var, mode=m)
+      for m in ("gru-sig", "gru-tanh", "gru-sig-f16", "gru-tanh-f16")
+      for v, cin, shape, var in (("w32", 32, (1, 1, 7, 32), "tcg<128,16,32,1,1,0,0>"), ("w128", 32, (1, 1, 3, 128), "tcg<128,16,128,1,1,0,0>"),
+                                 ("gw", 16, (1, 1, 3, 160), "tcg<128,16,128,1,1,1,0>"))],
+    # modulated deformable gather (osb_mdconv2d_k3_tc_fwd), opt = (stride, dilation, deformable groups); channels per group 4, 8, 16
+    R("dcn32-s1", "dcn", 32, 32, (2, 1, 7, 130), "tcg<32,16,128,1,1,1,0>", mode="dcn", opt=(1, 1, 8)),
+    R("dcn32-s2-dil3", "dcn", 16, 32, (2, 1, 11, 45), "tcg<32,16,128,1,1,1,0>", mode="dcn-2sig", opt=(2, 3, 1)),
+    R("dcn64-s1", "dcn", 32, 64, (1, 1, 5, 60), "tcg<64,16,128,1,1,1,0>", mode="dcn", opt=(1, 2, 4)),
+    R("dcn64-s2", "dcn", 64, 64, (2, 1, 6, 127), "tcg<64,16,128,1,1,1,0>", mode="dcn-2sig", opt=(2, 2, 8)),
+    R("dcn128-items", "dcn", 32, 128, (2, 1, 9, 300), "tcg<128,16,128,1,1,1,0>", mode="dcn", opt=(1, 3, 2)),   # 2 x 5 x 3 x 4 items
+    R("dcn128-s2", "dcn", 16, 128, (1, 1, 8, 100), "tcg<128,16,128,1,1,1,0>", mode="dcn-2sig", opt=(2, 1, 4)),
+    # split NDHWC activations (osb_conv3d_k3_tc_split_fwd), opt = (input, output, residual) layouts
+    R("split-in", "s1", 32, 32, (1, 3, 5, 128), "tc<32>", mode="split", opt=(SPLIT, NDHWC, None)),
+    R("split-out-res", "s1", 64, 32, (1, 3, 5, 128), "tc<32>", mode="split", opt=(NDHWC, SPLIT, NDHWC)),
+    R("split-all", "s1", 32, 32, (2, 2, 3, 128), "tc<32>", mode="split", opt=(SPLIT, SPLIT, SPLIT)),
+    R("split-ncdhw-in", "s1n", 32, 32, (1, 3, 5, 128), "tc<32>", mode="split", opt=(NCDHW, SPLIT, None)),
 ]
+
+# The instantiations each runtime mode reaches through its entry point (test_mode_sweep enumerates them on the GPU); every one has a
+# row of that mode, and the split rows cover every accepted layout combination of tc<32> (tests/test_host_logic_cpu.py).
+_F16 = {"tc<32>", "tc<16>", "tcg<96,16,16,1,1,0,1>", "tcg<64,16,16,1,1,0,1>", "tcg<64,16,64,1,1,0,0>", "tcg<64,16,32,1,1,0,0>",
+        "tcg<128,16,32,1,1,0,0>", "tcg<96,16,32,1,1,0,0>", "tcg<64,16,128,1,1,0,0>", "tcg<128,16,128,1,1,0,0>", "tcg<32,16,128,1,1,1,0>",
+        "tcg<64,16,128,1,1,1,0>", "tcg<128,16,128,1,1,1,0>", "tcg<128,16,128,1,2,0,0>"}
+_GRU = {"tcg<128,16,32,1,1,0,0>", "tcg<128,16,128,1,1,0,0>", "tcg<128,16,128,1,1,1,0>"}
+_DCN = {"tcg<32,16,128,1,1,1,0>", "tcg<64,16,128,1,1,1,0>", "tcg<128,16,128,1,1,1,0>"}
+MODE_VARIANTS = {"f16": _F16, "gru-sig": _GRU, "gru-tanh": _GRU, "gru-sig-f16": _GRU, "gru-tanh-f16": _GRU, "dcn": _DCN,
+                 "dcn-2sig": _DCN, "split": {"tc<32>"}}
+SPLIT_COMBOS = {(SPLIT, NDHWC, None), (NDHWC, SPLIT, NDHWC), (SPLIT, SPLIT, SPLIT), (NCDHW, SPLIT, None)}
+
+# Every field of struct TcArgs (csrc/tc_common.cuh): "" = an operand or geometry field the plain rows exercise, otherwise the mode
+# whose rows exercise it.  A field that is in neither fails tests/test_host_logic_cpu.py.
+TC_ARGS_FIELDS = {
+    **{f: "" for f in ("x w scale shift residual gate y B Cin Cout D H W act out_ndhwc res_ndhwc in_ncdhw ystride cout_real kappa "
+                       "overflow").split()},
+    "in_split": "split", "out_split": "split", "res_split": "split",
+    "gru": "gru-sig", "mul": "gru-sig", "blend_z": "gru-tanh", "blend_h": "gru-tanh", "res_bstride": "gru-tanh",
+    "terms": "f16",
+    **{f: "dcn" for f in ("dcn dcn_offset dcn_mask dcn_off_bstride dcn_mask_bstride dcn_h dcn_w dcn_stride dcn_pad dcn_dil "
+                          "dcn_dg").split()},
+    "dcn_mask_mode": "dcn-2sig",
+}
 
 
 @pytest.fixture(scope="module")
@@ -104,11 +180,25 @@ def out_spatial(row):
         return d // 2, h // 2, w // 2
     if row.kind in ("dc3", "dc4"):
         return 2 * d, 2 * h, 2 * w
+    if row.kind == "dcn":
+        st, dil, _ = row.opt
+        return 1, (h - 1) // st + 1, (w - 1) // st + 1            # padding = dilation
     return d, h, w
+
+
+def precision(row):
+    return PREC_F16 if row.mode == "f16" or row.mode.endswith("-f16") else PREC_FP32
+
+
+def terms(row):
+    """Split terms per product the row's kernel issues: conv3d_tc.cu's instantiations keep three under OSB_PREC_F16."""
+    return 1 if precision(row) == PREC_F16 and not row.variant.startswith("tc<") else 3
 
 
 def layouts(row):
     """Output layouts the row's entry point accepts (1 = channels-last)."""
+    if row.mode == "split":
+        return (1,)
     if row.ys or row.gate:
         return (1,)
     if row.creal < row.cout:
@@ -117,6 +207,8 @@ def layouts(row):
 
 
 def has_residual(row):
+    if row.kind == "dcn" or (row.mode == "split" and row.opt[2] is None):
+        return False
     return not (row.ys and row.kind in ("s2", "dc4"))        # the stride-2 and k4 slice entry points take no residual
 
 
@@ -126,9 +218,10 @@ def ksize(row):
 
 def make_weight(row, g, chan_scale=None):
     """fp32 weight in the layer's parameter layout (conv: (Cout, Cin, k, k, k); transposed: (Cin, Cout, k, k, k)); channels >= creal
-    zero (a zero-padded plan); 2d2: only the kd = 1 taps are non-zero."""
+    zero (a zero-padded plan); 2D kinds: only the kd = 1 taps are non-zero."""
     k = ksize(row)
-    fan = row.cin * (9 if row.kind == "2d2" else k ** 3)
+    two_d = row.kind in ("2d1", "2d2", "dcn")
+    fan = row.cin * (9 if two_d else k ** 3)
     scale = torch.ones(row.cout) if chan_scale is None else chan_scale
     scale = scale.clone()
     scale[row.creal:] = 0
@@ -136,7 +229,7 @@ def make_weight(row, g, chan_scale=None):
         w = torch.randn(row.cin, row.cout, k, k, k, generator=g) * fan ** -0.5 * scale.view(1, -1, 1, 1, 1)
     else:
         w = torch.randn(row.cout, row.cin, k, k, k, generator=g) * fan ** -0.5 * scale.view(-1, 1, 1, 1, 1)
-    if row.kind == "2d2":
+    if two_d:
         w[:, :, 0] = 0
         w[:, :, 2] = 0
     return w
@@ -144,8 +237,8 @@ def make_weight(row, g, chan_scale=None):
 
 def pack(ops, row, w):
     dw = w.cuda()
-    if row.kind in ("s1", "s1n"):
-        kc = ops.conv3d_tc_kc(row.cin, row.creal, row.shape[3])
+    if row.kind in ("s1", "s1n", "2d1", "dcn"):
+        kc = 16 if row.kind == "dcn" else ops.conv3d_tc_kc(row.cin, row.creal, row.shape[3])
         if row.creal < row.cout:
             return ops.pack_tc_weight(dw[:row.creal], kc, pad_cout_to=row.cout), kc
         return ops.pack_tc_weight(dw, kc), kc
@@ -156,20 +249,96 @@ def pack(ops, row, w):
     return ops.pack_tc_deconv_weight(dw), 16
 
 
-def reference(row, x, w):
-    """fp64 convolution of the row's operator: x (B, Cin, D, H, W) -> (B, Cout, Do, Ho, Wo)."""
+def staged_f16(x):
+    """fp16_rn(16 x) saturating to +-65504: the hi part of a staged activation (csrc/tc_common.cuh, TC_ACT_SCALE)."""
+    s = x.float() * 16.0
+    h = s.half()
+    return torch.where(torch.isinf(h), torch.sign(s).half() * 65504.0, h)
+
+
+def host_split(x):
+    """(B,D,H,W,C) fp32 -> (B,D,H,W,2C) fp16 split NDHWC: per 16-channel granule [16 hi | 16 lo] of x * 16, round to nearest,
+    saturating (include/openstereo_b200.h, OSB_LAYOUT_SPLIT)."""
+    hi = staged_f16(x)
+    lo = staged_f16((x.float() - hi.float() / 16.0))            # fp16_rn(16 x - hi): the scale is a power of two
+    g = x.shape[-1] // 16
+    both = torch.stack((hi.view(*x.shape[:4], g, 16), lo.view(*x.shape[:4], g, 16)), dim=5)   # (..., g, 2, 16)
+    return both.reshape(*x.shape[:4], 2 * x.shape[-1]).contiguous()
+
+
+def split_decode(s):
+    """split NDHWC (B,D,H,W,2C) fp16 -> (B,D,H,W,C) fp64 (hi + lo) / 16."""
+    t = s.double().view(*s.shape[:4], s.shape[-1] // 32, 2, 16)
+    return ((t[..., 0, :] + t[..., 1, :]) / 16.0).reshape(*s.shape[:4], s.shape[-1] // 2)
+
+
+def tc_weight_hi(wp):
+    """fp64 (Cout, Cin, 3, 3, 3) weights the single-term MMAs multiply: the hi halves of a TcWeight read back from its packing (the
+    wgmma pre-swizzle undone as tests/test_host_logic_cpu.py::test_pack_tc_weight_split does), the per-channel 2^e_c removed."""
+    from openstereo_b200 import ops
+    kc, cout = wp.kc, wp.cout
+    data = wp.data.cpu()
+    nch = data.shape[1]
+    cpr = 2 * kc // 8
+    rows = torch.arange(3 * cout)
+    key = (rows & 7) if kc == 32 else ((rows >> 1) & 3)
+    src = (torch.arange(cpr).view(1, cpr) ^ key.view(-1, 1)).view(1, 1, 1, 3 * cout, cpr, 1).expand(3, nch, 3, 3 * cout, cpr, 8)
+    lin = torch.gather(data.view(3, nch, 3, 3 * cout, cpr, 8), 4, src).reshape(3, nch, 3, 3 * cout, 2 * kc)
+    t = lin.double().view(3, nch, 3, 3, cout, 2, kc).permute(5, 4, 1, 6, 0, 2, 3).reshape(2, cout, nch * kc, 3, 3, 3)
+    scale = 2.0 ** -ops.TC_ACT_SCALE_LOG2 / wp.inv.double().cpu()
+    return t[0] / scale.view(-1, 1, 1, 1, 1)
+
+
+def dcn_operands(row, g, spread=4.0):
+    """(offset (B, dg*18, Ho, Wo), mask (B, dg*9, Ho, Wo)) of a dcn row: offsets several pixels wide, every 7th offset channel an
+    integer, some beyond every edge of the image; mode 0 masks of both signs, mode 1 logits."""
+    b = row.shape[0]
+    _, ho, wo = out_spatial(row)
+    dg = row.opt[2]
+    off = torch.randn(b, dg * 18, ho, wo, generator=g) * spread
+    off[:, 0::7] = torch.randint(-3, 4, off[:, 0::7].shape, generator=g).float()
+    off[0, :2, 0, :3] = torch.tensor([[-1e3, 0.0, 2.5e3], [3.0, -1e3, 0.5]])
+    off[-1, -2:, -1, -3:] = torch.tensor([[1e3, -0.5, -2.5e3], [-3.0, 1e3, 0.25]])
+    mask = torch.randn(b, dg * 9, ho, wo, generator=g) * (2.0 if row.mode == "dcn-2sig" else 1.0)
+    return off, mask
+
+
+def dcn_positions(off, stride, pad, dil):
+    """The offsets as the kernel applies them: each sample position is the fp32 sum of the integer tap position and the offset, so
+    a float64 reference fed these offsets samples the same points."""
+    b, c, ho, wo = off.shape
+    ys = torch.arange(ho, dtype=torch.float64).view(1, 1, ho, 1) * stride - pad
+    xs = torch.arange(wo, dtype=torch.float64).view(1, 1, 1, wo) * stride - pad
+    out = off.double().clone()
+    for tap in range(9):
+        kh, kw = divmod(tap, 3)
+        for base, k in ((ys + kh * dil, 0), (xs + kw * dil, 1)):
+            out[:, k + 2 * tap::18] = (base.float() + off[:, k + 2 * tap::18].float()).double() - base
+    return out
+
+
+def reference(row, x, w, dcn=None):
+    """fp64 convolution of the row's operator: x (B, Cin, D, H, W) -> (B, Cout, Do, Ho, Wo); dcn = (offset, mask, mask mode)."""
     x, w = x.double(), w.double()
     if row.kind in ("s1", "s1n"):
         return F.conv3d(x, w, padding=1)
-    if row.kind == "2d2":
-        return F.conv2d(x[:, :, 0], w[:, :, 1], padding=2, dilation=2).unsqueeze(2)
+    if row.kind in ("2d1", "2d2"):
+        dil = 2 if row.kind == "2d2" else 1
+        return F.conv2d(x[:, :, 0], w[:, :, 1], padding=dil, dilation=dil).unsqueeze(2)
+    if row.kind == "dcn":
+        st, dil, _ = row.opt
+        off, mask, mode = dcn
+        m = 2 * torch.sigmoid(mask.double()) if mode else mask.double()
+        return deform_conv2d(x[:, :, 0], dcn_positions(off, st, dil, dil), w[:, :, 1], stride=st, padding=dil, dilation=dil,
+                             mask=m).unsqueeze(2)
     if row.kind == "s2":
         return F.conv3d(x, w, stride=2, padding=1)
     return F.conv_transpose3d(x, w, stride=2, padding=1, output_padding=1 if row.kind == "dc3" else 0)
 
 
-def epilogue(conv, sc, sh, res, gate, act):
-    """fp64 folded BN + residual + activation + gate on an NCDHW tensor; gate (B, Ho, Wo, C) channels-last."""
+def epilogue(conv, sc, sh, res, gate, act, mul=None, blend=None):
+    """fp64 folded BN + residual + activation + gate on an NCDHW tensor; gate, mul and blend (z, h): (B, Ho, Wo, C) channels-last."""
+    cl = lambda t: t.double().permute(0, 3, 1, 2).unsqueeze(2)        # noqa: E731
     y = conv
     if sc is not None:
         y = y * sc.double().view(1, -1, 1, 1, 1)
@@ -181,36 +350,72 @@ def epilogue(conv, sc, sh, res, gate, act):
         y = F.relu(y)
     elif act == ACT_LEAKY:
         y = F.leaky_relu(y, 0.01)
+    elif act == ACT_SIGMOID:
+        y = torch.sigmoid(y)
+    elif act == ACT_TANH:
+        y = torch.tanh(y)
     if gate is not None:
-        y = y * gate.double().permute(0, 3, 1, 2).unsqueeze(2)
+        y = y * cl(gate)
+    if mul is not None:
+        y = y * cl(mul)
+    if blend is not None:
+        z, h = cl(blend[0]), cl(blend[1])
+        y = h + z * (y - h)
     return y
 
 
 class Launch:
-    """The operands of one row in device memory and a direct call of its C entry point with a caller-chosen output address."""
+    """The operands of one row in device memory and a direct call of its C entry point with a caller-chosen output address.
+    mul / blend (z, h): ConvGRU epilogue operands (B, Ho, Wo, Cout); dcn: (offset, mask, mask mode); prec: OSB_PREC_* of the
+    f16 / gru rows (default: the row's)."""
 
-    def __init__(self, osb, row, x, w, sc=None, sh=None, res=None, gate=None, act=ACT_NONE, out_ndhwc=1):
+    def __init__(self, osb, row, x, w, sc=None, sh=None, res=None, gate=None, act=ACT_NONE, out_ndhwc=1, mul=None, blend=None, dcn=None,
+                 prec=None):
         self.lib, ops = osb
         self.row, self.act, self.out_ndhwc = row, act, out_ndhwc
+        self.prec = precision(row) if prec is None else prec
         b, d, h, wd = row.shape
         self.spatial = out_spatial(row)
         self.ctot = row.ys or row.cout                           # channels per voxel of the channels-last tensors
+        self.split_out = row.mode == "split" and row.opt[1] == SPLIT
         wp, kc = pack(ops, row, w)
         self.wp = wp
         self.wptr, self.eff = ops._tc_args(wp, row.cin, kc, None if sc is None else sc.cuda())
         self.sh = None if sh is None else sh.cuda()
-        xin = x if row.kind == "s1n" else x.permute(0, 2, 3, 4, 1)
+        x_cl = x.permute(0, 2, 3, 4, 1)
+        if row.mode == "split":
+            xin = {NCDHW: x, NDHWC: x_cl, SPLIT: host_split(x_cl.contiguous())}[row.opt[0]]
+        else:
+            xin = x if row.kind == "s1n" else x_cl
         self.x = xin.contiguous().cuda()
         self.res = self.res_ptr = None
-        if res is not None:                                      # NCDHW (B, creal, ...) -> the output's layout
-            self.res = self._to_layout(res)
-            self.res_ptr = self.res.data_ptr() + 4 * (row.coff if out_ndhwc else 0)
+        self.res_bstride = 0
+        if res is not None:
+            if row.mode.startswith("gru"):                       # an NCHW channel view of a wider tensor: batch stride 144 H W
+                full = torch.zeros(b, RES_CTOT, *self.spatial[1:])
+                full[:, RES_COFF:RES_COFF + row.cout] = res[:, :, 0]
+                self.res = full.cuda()
+                self.res_ptr = self.res.data_ptr() + 4 * RES_COFF * self.spatial[1] * self.spatial[2]
+                self.res_bstride = RES_CTOT * self.spatial[1] * self.spatial[2]
+            elif row.mode == "split" and row.opt[2] == SPLIT:
+                self.res = host_split(res.permute(0, 2, 3, 4, 1).contiguous()).cuda()
+                self.res_ptr = self.res.data_ptr()
+            else:                                                # NCDHW (B, creal, ...) -> the output's layout
+                self.res = self._to_layout(res)
+                self.res_ptr = self.res.data_ptr() + 4 * (row.coff if out_ndhwc else 0)
         self.gate = self.gate_ptr = None
         if gate is not None:                                     # (B, Ho, Wo, cout) -> (B, Ho, Wo, ctot), slice channels at coff
             full = torch.zeros(b, self.spatial[1], self.spatial[2], self.ctot)
             full[..., row.coff:row.coff + row.cout] = gate
             self.gate = full.cuda()
             self.gate_ptr = self.gate.data_ptr() + 4 * row.coff
+        self.mul = None if mul is None else mul.contiguous().cuda()
+        self.blend = None if blend is None else [t.contiguous().cuda() for t in blend]
+        self.dcn = None
+        if dcn is not None:                                      # offsets and mask as channel slices of one tensor
+            off, mask, self.mask_mode = dcn
+            self.dcn = torch.cat((off, mask), 1).contiguous().cuda()
+            self.n_off = off.shape[1]
 
     def _to_layout(self, t):
         row = self.row
@@ -220,13 +425,32 @@ class Launch:
         full[..., row.coff:row.coff + row.cout] = t.permute(0, 2, 3, 4, 1)
         return full.cuda()
 
+    def operands(self, x, w):
+        """fp64 (x, w) the row's MMAs multiply: the staged hi parts in single-term mode, the decoded split input of a split row."""
+        if terms(self.row) == 1:
+            return staged_f16(x).double() / 16.0, tc_weight_hi(self.wp)
+        if self.row.mode == "split" and self.row.opt[0] == SPLIT:
+            return split_decode(self.x.cpu()).permute(0, 4, 1, 2, 3), w
+        return x, w
+
+    def residual64(self, res):
+        """fp64 residual the epilogue adds (a split residual: decoded)."""
+        if res is not None and self.row.mode == "split" and self.row.opt[2] == SPLIT:
+            return split_decode(self.res.cpu()).permute(0, 4, 1, 2, 3)
+        return res
+
     def numel(self):
         b = self.row.shape[0]
         n = b * math.prod(self.spatial)
         return n * (self.ctot if self.out_ndhwc else self.row.creal)
 
     def guarded(self):
-        """Fresh output buffer: sentinels | output region (NaN where this launch must write, sentinels elsewhere) | sentinels."""
+        """Fresh output buffer: sentinels | output region (NaN where this launch must write, sentinels elsewhere) | sentinels.  A split
+        output (fp16, the bytes of the fp32 tensor) is guarded by 16-bit sentinels and starts as fp16 NaN."""
+        if self.split_out:
+            buf = torch.full((2 * (GUARD + self.numel() + GUARD),), SENTINEL16, dtype=torch.int16, device="cuda")
+            buf.view(torch.float16)[2 * GUARD:2 * (GUARD + self.numel())] = float("nan")
+            return buf.view(torch.float32)
         buf = torch.full((GUARD + self.numel() + GUARD,), SENTINEL, device="cuda")
         self.inner(buf).copy_(torch.where(self.written_mask(), torch.tensor(float("nan"), device="cuda"),
                                           torch.tensor(SENTINEL, device="cuda")))
@@ -249,7 +473,25 @@ class Launch:
         yp = buf.data_ptr() + 4 * (GUARD + (row.coff if self.out_ndhwc else 0))
         x, wp, sc, sh = self.x.data_ptr(), self.wptr, self.eff.data_ptr(), None if self.sh is None else self.sh.data_ptr()
         o, act, call = self.out_ndhwc, self.act, self.lib.call
-        if row.ys and row.kind == "s1":
+        if row.mode == "split":
+            i_l, o_l, r_l = row.opt
+            call("osb_conv3d_k3_tc_split_fwd", x, wp, sc, sh, self.res_ptr, yp, b, row.cin, row.cout, d, h, w, act, i_l, o_l,
+                 NDHWC if r_l is None else r_l, s)
+        elif row.mode.startswith("gru"):
+            p = lambda t: None if t is None else t.data_ptr()     # noqa: E731
+            bz, bh = self.blend if self.blend is not None else (None, None)
+            call("osb_conv2d_k3_tc_gru_prec_fwd", x, wp, sc, sh, self.res_ptr, p(self.mul), p(bz), p(bh), yp, b, row.cin, row.cout, h, w,
+                 act, o, 0, self.res_bstride, self.prec, s)
+        elif row.kind == "dcn":
+            st, dil, dg = row.opt
+            ho, wo = self.spatial[1:]
+            om, bs = self.dcn.data_ptr(), self.dcn.stride(0)
+            call("osb_mdconv2d_k3_tc_fwd", x, om, bs, om + 4 * self.n_off * ho * wo, bs, self.mask_mode, wp, sc, sh, yp, b, row.cin,
+                 row.cout, h, w, st, dil, dil, dg, act, o, s)
+        elif row.mode == "f16":
+            call("osb_conv2d_k3_tc_prec_fwd", x, wp, sc, sh, self.res_ptr, yp, b, row.cin, row.creal, h, w, 2 if row.kind == "2d2" else 1,
+                 act, o, o, self.prec, s)
+        elif row.ys and row.kind == "s1":
             call("osb_conv3d_k3_tc_cs_fwd", x, wp, sc, sh, self.res_ptr, self.gate_ptr, yp, b, row.cin, row.cout, d, h, w, act, row.ys, s)
         elif row.ys and row.kind == "s2":
             call("osb_conv3d_k3_s2_tc_cs_fwd", x, wp, sc, sh, yp, b, row.cin, row.cout, d, h, w, act, row.ys, s)
@@ -270,9 +512,11 @@ class Launch:
             call("osb_deconv3d_k4_tc_fwd", x, wp, sc, sh, self.res_ptr, yp, b, row.cin, row.cout, row.creal, d, h, w, act, o, o, s)
 
     def output(self, buf):
-        """-> the launch's result as NCDHW (B, creal, Do, Ho, Wo) on the CPU."""
+        """-> the launch's result as NCDHW (B, creal, Do, Ho, Wo) on the CPU (a split output decoded, in fp64)."""
         row, b = self.row, self.row.shape[0]
         y = self.inner(buf)
+        if self.split_out:
+            return split_decode(y.view(torch.float16).view(b, *self.spatial, 2 * row.cout).cpu()).permute(0, 4, 1, 2, 3)
         if self.out_ndhwc:
             y = y.view(b, *self.spatial, self.ctot)[..., row.coff:row.coff + row.cout].permute(0, 4, 1, 2, 3)
         else:
@@ -280,6 +524,13 @@ class Launch:
         return y.cpu()
 
     def check_bounds(self, buf, what):
+        if self.split_out:
+            h16 = buf.view(torch.int16)
+            g, n = 2 * GUARD, 2 * self.numel()
+            assert (h16[:g] == SENTINEL16).all() and (h16[g + n:] == SENTINEL16).all(), "%s: a store left the split output" % what
+            inner = buf.view(torch.float16)[g:g + n]
+            assert not torch.isnan(inner).any(), "%s: %d fp16 output halves never written" % (what, int(torch.isnan(inner).sum()))
+            return
         bits = buf.view(torch.int32)
         sent = torch.tensor([SENTINEL]).view(torch.int32).item()
         assert (bits[:GUARD] == sent).all() and (bits[-GUARD:] == sent).all(), "%s: a store left the output region" % what
@@ -297,10 +548,20 @@ def per_channel_close(got, want, creal, tol, what):
         what, bad[:8], tol, [float(err[c] / scale[c].clamp(min=1e-300)) for c in bad[:8]])
 
 
-def channel_scales(cout, g):
-    """2^k x a non-power-of-two factor per output channel, k spread over [-12, 12]."""
-    k = torch.linspace(-12, 12, cout).round()[torch.randperm(cout, generator=g)]
+def channel_scales(cout, g, lo=-12, hi=12):
+    """2^k x a non-power-of-two factor per output channel, k spread over [lo, hi]."""
+    k = torch.linspace(lo, hi, cout).round()[torch.randperm(cout, generator=g)]
     return torch.ldexp(torch.ones(cout), k.int()) * (1.0 + 0.9 * torch.rand(cout, generator=g)) * 0.77
+
+
+def scale_range(row):
+    """Exponent range of the row's channel scales: the GRU gates saturate (sigmoid / tanh of pre-activations kept within a few
+    units), a split output must stay inside the fp16 range of its encoding (|y| < 4094)."""
+    if row.mode.startswith("gru"):
+        return -3, 0
+    if row.mode == "split" and row.opt[1] == SPLIT:
+        return -12, 4
+    return -12, 12
 
 
 @pytest.fixture
@@ -317,19 +578,27 @@ def test_routing_item_loop_accuracy_and_bounds(osb, grid_cap, row):
     g = gen(zlib.crc32(row.id.encode()) % 10000)
     b, d, h, w = row.shape
     x = torch.randn(b, row.cin, d, h, w, generator=g)
-    cs = channel_scales(row.cout, g)
+    cs = channel_scales(row.cout, g, *scale_range(row))
     wt = make_weight(row, g, cs)
     sc = torch.rand(row.cout, generator=g) + 0.5
     sh = 0.1 * cs * torch.randn(row.cout, generator=g)
-    conv = reference(row, x, wt)
-    res = 0.3 * cs.view(1, -1, 1, 1, 1) * torch.randn(conv.shape, generator=g) if has_residual(row) else None
     do, ho, wo = out_spatial(row)
+    res = 0.3 * cs.view(1, -1, 1, 1, 1) * torch.randn(b, row.cout, do, ho, wo, generator=g) if has_residual(row) else None
     gate = torch.sigmoid(torch.randn(b, ho, wo, row.cout, generator=g)) if row.gate else None
     act = ACT_RELU if len(row.id) % 2 else ACT_LEAKY
-    want = epilogue(conv, sc, sh, res, gate, act)
+    mul = blend = dcn = None
+    if row.mode.startswith("gru-sig"):                             # r * h: sigmoid, then the multiplier
+        act, mul = ACT_SIGMOID, torch.randn(b, ho, wo, row.cout, generator=g)
+    elif row.mode.startswith("gru-tanh"):                          # q = tanh(...), h' = h + z (q - h)
+        act = ACT_TANH
+        blend = (torch.sigmoid(torch.randn(b, ho, wo, row.cout, generator=g)), torch.randn(b, ho, wo, row.cout, generator=g))
+    elif row.kind == "dcn":
+        off, mask = dcn_operands(row, g)
+        dcn = (off, mask, int(row.mode == "dcn-2sig"))
     for o in layouts(row):
         what = "%s %s" % (row.id, "ndhwc" if o else "ncdhw")
-        L = Launch(osb, row, x, wt, sc, sh, res, gate, act, o)
+        L = Launch(osb, row, x, wt, sc, sh, res, gate, act, o, mul, blend, dcn)
+        want = epilogue(reference(row, *L.operands(x, wt), dcn=dcn), sc, sh, L.residual64(res), gate, act, mul, blend)
         outs = []
         for cap in (1, 7, 0, 0):
             grid_cap(cap)
@@ -343,6 +612,38 @@ def test_routing_item_loop_accuracy_and_bounds(osb, grid_cap, row):
                 per_channel_close(L.output(buf), want, row.creal, 1e-5, what)
         for cap, o_ in zip((7, 0, 0), outs[1:]):
             assert torch.equal(outs[0], o_), "%s: output at grid cap %d differs from the one-CTA run" % (what, cap)
+        if precision(row) == PREC_F16 and terms(row) == 3:         # conv3d_tc.cu keeps the 3-term product: the OSB_PREC_FP32 bits
+            L32 = Launch(osb, row, x, wt, sc, sh, res, gate, act, o, mul, blend, dcn, prec=PREC_FP32)
+            buf = L32.guarded()
+            L32.run(buf)
+            torch.cuda.synchronize()
+            assert torch.equal(L32.inner(buf).view(torch.int32), outs[0]), "%s: OSB_PREC_F16 differs from OSB_PREC_FP32" % what
+
+
+def _dcn_range_guard(osb, row, g):
+    """|x| = 3000 at one pixel, sampled at integer positions (offsets 0): under m = 2 sigmoid(10) ~ 2 the staged operand m x is past
+    the fp16 range and is reported (the output stays finite); under m = 0.5 it is not, and the output is accurate."""
+    _, ops = osb
+    b, _, h, w = row.shape
+    _, ho, wo = out_spatial(row)
+    dg = row.opt[2]
+    x = torch.randn(b, row.cin, 1, h, w, generator=g)
+    x[b - 1, row.cin - 1, 0, 2 * (h // 4), 2 * (w // 4)] = -3000.0   # even coordinates: sampled at every stride and dilation
+    x[0, 0, 0, 0, 0] = 3000.0
+    wt = make_weight(row, g)
+    off = torch.zeros(b, dg * 18, ho, wo)
+    ops.tc_overflow_count(reset=True)
+    for mask, mode, report in ((torch.full((b, dg * 9, ho, wo), 10.0), 1, True), (torch.full((b, dg * 9, ho, wo), 0.5), 0, False)):
+        L = Launch(osb, row, x, wt, out_ndhwc=0, dcn=(off, mask, mode))
+        buf = L.guarded()
+        L.run(buf)
+        n = ops.tc_overflow_count(reset=True)
+        if report:
+            assert n >= 1, "%s: |m x| = 6000 not reported" % row.id
+            assert torch.isfinite(L.inner(buf)).all(), "%s: saturated operands must keep the output finite" % row.id
+        else:
+            assert n == 0, "%s: |m x| = 1500 reported as overflow" % row.id
+            per_channel_close(L.output(buf), reference(row, x, wt, (off, mask, mode)), row.creal, 1e-5, row.id + " m = 0.5")
 
 
 @pytest.mark.timeout(120)
@@ -350,15 +651,18 @@ def test_routing_item_loop_accuracy_and_bounds(osb, grid_cap, row):
 def test_fp16_range_guard(osb, row):
     _, ops = osb
     g = gen(7 + zlib.crc32(row.id.encode()) % 10000)
+    if row.kind == "dcn":
+        return _dcn_range_guard(osb, row, g)
     b, d, h, w = row.shape
     x = torch.randn(b, row.cin, d, h, w, generator=g) * torch.logspace(-6, 3, w).view(1, 1, 1, 1, w)
     x = x.clamp(-4090, 4090)
-    wt = make_weight(row, g)
-    want = reference(row, x, wt)
+    split_out = row.mode == "split" and row.opt[1] == SPLIT
+    wt = make_weight(row, g, torch.full((row.cout,), 0.25) if split_out else None)   # a split output must stay below 4094 too
     gate = torch.ones(b, *out_spatial(row)[1:], row.cout) if row.gate else None
     o = layouts(row)[0]
     ops.tc_overflow_count(reset=True)
     L = Launch(osb, row, x, wt, gate=gate, out_ndhwc=o)
+    want = reference(row, *L.operands(x, wt))
     buf = L.guarded()
     L.run(buf)
     assert ops.tc_overflow_count() == 0, "%s: in-range activations reported as overflow" % row.id
@@ -370,6 +674,8 @@ def test_fp16_range_guard(osb, row):
     col_scale = want.abs().amax(dim=(0, 1, 2, 3))
     bad = (err > 2e-5 * col_scale + 2.0 ** -27 * wsum).nonzero().flatten().tolist()
     assert not bad, "%s: output columns %s off (err %s, scale %s)" % (row.id, bad[:8], err[bad[:8]].tolist(), col_scale[bad[:8]].tolist())
+    # a split input was range-checked where it was encoded: the layer stages its saturated bits as they are and reports nothing
+    converts = not (row.mode == "split" and row.opt[0] == SPLIT)
     for value, col in ((5000.0, w - 1), (-5000.0, 0)):          # last K chunk, last plane; an image edge / column-tile seam
         xo = x.clone()
         xo[b - 1, row.cin - 1, d - 1, h // 2, col] = value
@@ -377,19 +683,22 @@ def test_fp16_range_guard(osb, row):
         buf = L.guarded()
         L.run(buf)
         n = ops.tc_overflow_count(reset=True)
-        assert n >= 1, "%s: %g at column %d not reported" % (row.id, value, col)
-        assert torch.isfinite(L.inner(buf)[L.written_mask()]).all(), "%s: saturated operands must keep the output finite" % row.id
+        assert n >= 1 or not converts, "%s: %g at column %d not reported" % (row.id, value, col)
+        assert torch.isfinite(L.output(buf)).all(), "%s: saturated operands must keep the output finite" % row.id
     assert ops.tc_overflow_count() == 0
 
 
 def expected_mma_count(row):
     """-> {(output plane, output row parity or None): MMAs each accumulator received}, from the convolution geometry alone:
-    (kd, kh) tap rows issued x Cin/16 k-steps x 3 split products.  Rows outside the image are issued as zero operands (they count);
-    planes outside the volume are skipped (they do not)."""
+    (kd, kh) tap rows issued x Cin/16 k-steps x split terms (3, or 1 in single-term mode).  Rows outside the image are issued as zero
+    operands (they count); planes outside the volume are skipped (they do not).  The deformable gather issues Cin/16 x 9 taps x 3 at
+    every output pixel: samples outside the image are zero operands."""
     _, d, h, w = row.shape
-    steps = row.cin // 16 * 3
+    steps = row.cin // 16 * terms(row)
     out = {}
-    if row.kind in ("s1", "s1n", "2d2", "s2"):
+    if row.kind == "dcn":
+        return {(0, None): 9 * steps}
+    if row.kind in ("s1", "s1n", "2d1", "2d2", "s2"):
         st = 2 if row.kind == "s2" else 1
         for od in range(out_spatial(row)[0]):
             planes = sum(1 for kd in range(3) if 0 <= st * od + kd - 1 < d)
@@ -412,8 +721,17 @@ def test_kappa_mma_count(osb, row):
     b, d, h, w = row.shape
     x = torch.randn(b, row.cin, d, h, w, generator=g)
     wt = make_weight(row, g)
-    gate = torch.ones(b, *out_spatial(row)[1:], row.cout) if row.gate else None
-    L = Launch(osb, row, x, wt, gate=gate, out_ndhwc=layouts(row)[0])
+    _, ho, wo = out_spatial(row)
+    gate = torch.ones(b, ho, wo, row.cout) if row.gate else None
+    mul = blend = dcn = None
+    if row.mode.startswith("gru-sig"):                             # linear in the accumulator: y = conv * mul
+        mul = torch.randn(b, ho, wo, row.cout, generator=g)
+    elif row.mode.startswith("gru-tanh"):                          # h = 0: y = z * conv
+        blend = (torch.sigmoid(torch.randn(b, ho, wo, row.cout, generator=g)), torch.zeros(b, ho, wo, row.cout))
+    elif row.kind == "dcn":
+        off, mask = dcn_operands(row, g)
+        dcn = (off, mask, int(row.mode == "dcn-2sig"))
+    L = Launch(osb, row, x, wt, gate=gate, out_ndhwc=layouts(row)[0], mul=mul, blend=blend, dcn=dcn)
     ys = []
     old = ops.set_rz_kappa(0.0)
     try:
@@ -433,6 +751,62 @@ def test_kappa_mma_count(osb, row):
         got = e[big].median().item()
         assert got == n, "%s: output plane %d%s applied kappa * %d, the geometry gives %d MMAs" % (
             row.id, od, "" if ph is None else " row parity %d" % ph, got, n)
+
+
+# Widths, output / input channels and dilations of the sweep over what the 2D entry points accept
+SWEEP_W = (16, 24, 32, 40, 64, 80, 127, 128, 130, 160, 240)
+SWEEP_COUT = (16, 32, 64, 96, 128)
+SWEEP_CIN = (32, 64)
+
+
+@pytest.mark.timeout(180)
+def test_mode_sweep(osb):
+    """Every shape the 2D entry points accept over SWEEP_W x SWEEP_COUT x SWEEP_CIN x dilation 1, 2 (B = 1, H = 2), launched once
+    through osb_conv2d_k3_tc_prec_fwd (OSB_PREC_F16) and, at Cout = 128, osb_conv2d_k3_tc_gru_prec_fwd at both precisions; every
+    packed width osb_mdconv2d_k3_tc_fwd accepts: the instantiations reached are exactly MODE_VARIANTS of that mode, so each has rows."""
+    lib, ops = osb
+    s = torch.cuda.current_stream().cuda_stream
+    reached = {"f16": set(), "gru": set(), "gru-f16": set(), "dcn": set()}
+    g = gen(3)
+    for w in SWEEP_W:
+        for cin in SWEEP_CIN:
+            x = torch.randn(1, 2, w, cin, generator=g).cuda()
+            for cout in SWEEP_COUT:
+                for dil in (1, 2):
+                    kc = ops.conv2d_tc_kc(cin, cout, w, dil)
+                    if not kc:
+                        continue
+                    wt = torch.randn(cout, cin, 3, 3, 3, generator=g).cuda() * 0.05
+                    wp = ops.pack_tc_weight(wt, kc, pad_cout_to=16 if cout < 16 else None)
+                    y = torch.empty(1, cout, 2, w, device="cuda")
+                    sc = wp.eff_scale(None)
+                    lib.call("osb_conv2d_k3_tc_prec_fwd", x.data_ptr(), wp.data.data_ptr(), sc.data_ptr(), None, None, y.data_ptr(), 1,
+                             cin, cout, 2, w, dil, ACT_NONE, 0, 0, PREC_F16, s)
+                    reached["f16"].add(ops.tc_last_variant())
+                    if cout == 128 and dil == 1 and kc == 16:
+                        for prec, key in ((PREC_FP32, "gru"), (PREC_F16, "gru-f16")):
+                            lib.call("osb_conv2d_k3_tc_gru_prec_fwd", x.data_ptr(), wp.data.data_ptr(), sc.data_ptr(), None, None, None,
+                                     None, None, y.data_ptr(), 1, cin, cout, 2, w, ACT_TANH, 0, 0, 0, prec, s)
+                            reached[key].add(ops.tc_last_variant())
+    x = torch.randn(1, 6, 40, 32, generator=g).cuda()
+    om = torch.randn(1, 27, 6, 40, generator=g).cuda()
+    for cout in range(16, 257, 16):                                 # every packed width the entry point accepts
+        wp = ops.pack_tc_weight(torch.randn(cout, 32, 3, 3, 3, generator=g).cuda() * 0.05, 16)
+        y = torch.empty(1, cout, 6, 40, device="cuda")
+        rc = lib.lib.osb_mdconv2d_k3_tc_fwd(x.data_ptr(), om.data_ptr(), om.stride(0), om.data_ptr() + 4 * 18 * 240, om.stride(0), 1,
+                                            wp.data.data_ptr(), wp.eff_scale(None).data_ptr(), None, y.data_ptr(), 1, 32, cout, 6, 40, 1,
+                                            1, 1, 1, ACT_NONE, 0, s)
+        assert rc in (0, 1), lib.lib.osb_last_error()
+        if rc == 0:
+            reached["dcn"].add(ops.tc_last_variant())
+    torch.cuda.synchronize()
+    assert ops.tc_overflow_count(reset=True) == 0
+    for key, modes in (("f16", ("f16",)), ("gru", ("gru-sig", "gru-tanh")), ("gru-f16", ("gru-sig-f16", "gru-tanh-f16")),
+                       ("dcn", ("dcn", "dcn-2sig"))):
+        for m in modes:
+            assert reached[key] == MODE_VARIANTS[m], "mode %s: the entry point reaches %s, MODE_VARIANTS lists %s" % (
+                m, sorted(reached[key]), sorted(MODE_VARIANTS[m]))
+            assert {r.variant for r in REGISTRY if r.mode == m} == reached[key], "mode %s: instantiations without a row" % m
 
 
 # ------------------------------------------------------------------------------------------------ rounding bias against fp64
