@@ -29,7 +29,7 @@ class _Packed:
     __slots__ = ("w", "scale", "shift", "stride", "kernel", "transposed", "cin", "cout", "_w5", "_tc")
 
     def __init__(self, conv, bn=None):
-        self._tc = {}                                           # K-chunk -> hi/lo split weight for the wgmma kernels
+        self._tc = {}                                           # kind -> weight packed for the wgmma kernels (tc)
         self._w5 = conv.weight.detach() if conv.weight.dim() == 5 else None
         self.cin, self.cout = (conv.in_channels, conv.out_channels)
         self.transposed = isinstance(conv, (torch.nn.ConvTranspose3d, torch.nn.ConvTranspose2d))
@@ -73,7 +73,38 @@ def _packed_validate(self, conv):
                                   "groups 1; ConvTranspose k3 s2 p1 op1 or k4 s2 p1)" % (conv,))
 
 
+def _packed_tc(self, kind):
+    """This layer's weight packed for a tensor-core kernel family, packed on first use: kind 16 or 32 the stride-1 pack at that K
+    chunk (a head narrower than 16 channels zero-padded to 16), "s2" the stride-2 pack, "dc" the transposed conv's, "c1" the taps of
+    a one-channel head for conv3d_k3_c1_ndhwc, "head" a one-channel head with Cin zero-padded to a multiple of 32."""
+    if kind not in self._tc:
+        w = self._w5
+        if kind == "s2":
+            self._tc[kind] = ops.pack_tc_weight(w, 16, kw_order=(1, 0, 2))
+        elif kind == "dc":
+            self._tc[kind] = ops.pack_tc_deconv_weight(w)
+        elif kind == "c1":
+            self._tc[kind] = ops.pack_c1_weight(w)
+        elif kind == "head":
+            self._tc[kind] = ops.pack_tc_weight(_zero_padded(w, 1, _pad32(self.cin)), 32, pad_cout_to=16)
+        else:
+            self._tc[kind] = ops.pack_tc_weight(w, kind, pad_cout_to=16 if self.cout < 16 else None)
+    return self._tc[kind]
+
+
+def _zero_padded(w, n0, n1):
+    """w (n0', n1', ...) zero-padded to (n0, n1, ...)."""
+    out = w.new_zeros((n0, n1) + tuple(w.shape[2:]))
+    out[:w.shape[0], :w.shape[1]] = w
+    return out
+
+
+def _pad32(c):
+    return (c + 31) // 32 * 32
+
+
 _Packed._validate = _packed_validate
+_Packed.tc = _packed_tc
 
 
 def _conv(layer, x, act=ACT_NONE, residual=None, gate=None):
@@ -90,11 +121,7 @@ def _tc_weight(layer, width):
     if not USE_TENSOR_CORES or layer.transposed or layer.kernel != 3 or layer.stride != 1 or layer._w5 is None:
         return None
     kc = ops.conv3d_tc_kc(layer.cin, layer.cout, width)
-    if not kc:
-        return None
-    if kc not in layer._tc:
-        layer._tc[kc] = ops.pack_tc_weight(layer._w5, kc, pad_cout_to=16 if layer.cout < 16 else None)
-    return layer._tc[kc]
+    return layer.tc(kc) if kc else None
 
 
 def _tc_ok(layer, width):
@@ -127,18 +154,14 @@ def _conv_auto(layer, x, act=ACT_NONE, residual=None):
         return _conv_tc(layer, ops.to_ndhwc(x), act, residual, out_ndhwc=False, res_ndhwc=False)
     if (USE_TENSOR_CORES and layer.stride == 2 and layer.kernel == 3 and not layer.transposed and layer._w5 is not None
             and ops.conv3d_s2_tc_supported(layer.cin, layer.cout, x.shape[2], x.shape[3], x.shape[4])):
-        if "s2" not in layer._tc:
-            layer._tc["s2"] = ops.pack_tc_weight(layer._w5, 16, kw_order=(1, 0, 2))
-        return ops.conv3d_k3_s2_tc(ops.to_ndhwc(x), layer._tc["s2"], layer.scale, layer.shift, residual, act)
+        return ops.conv3d_k3_s2_tc(ops.to_ndhwc(x), layer.tc("s2"), layer.scale, layer.shift, residual, act)
     return _conv(layer, x, act, residual)
 
 
 def _deconv(layer, x, act=ACT_NONE, residual=None):
     if (USE_TENSOR_CORES and layer.transposed and layer.kernel == 3 and layer._w5 is not None
             and ops.deconv3d_tc_supported(layer.cin, layer.cout, x.shape[-1])):
-        if "dc" not in layer._tc:
-            layer._tc["dc"] = ops.pack_tc_deconv_weight(layer._w5)
-        return ops.deconv3d_k3_tc(ops.to_ndhwc(x), layer._tc["dc"], layer.scale, layer.shift, residual, act)
+        return ops.deconv3d_k3_tc(ops.to_ndhwc(x), layer.tc("dc"), layer.scale, layer.shift, residual, act)
     return ops.deconv3d(x, layer.w, layer.scale, layer.shift, residual, layer.kernel, act)
 
 
@@ -208,28 +231,16 @@ def _hg_channels_last_ok(hg, x_shape_ndhwc):
             and (hg.redir1.cin, hg.redir1.cout) in ((32, 32), (64, 64)) and (hg.redir2.cin, hg.redir2.cout) in ((32, 32), (64, 64)))
 
 
-def _s2_weight(layer):
-    if "s2" not in layer._tc:
-        layer._tc["s2"] = ops.pack_tc_weight(layer._w5, 16, kw_order=(1, 0, 2))
-    return layer._tc["s2"]
-
-
-def _dc_weight(layer):
-    if "dc" not in layer._tc:
-        layer._tc["dc"] = ops.pack_tc_deconv_weight(layer._w5)
-    return layer._tc["dc"]
-
-
 def _gwc_hourglass_channels_last(hg, x):
     """GwcNet hourglass (gwcnet/hourglass.py:46-56) with every tensor channels-last: no layout conversion between layers."""
-    c1 = ops.conv3d_k3_s2_tc(x, _s2_weight(hg.conv1), hg.conv1.scale, hg.conv1.shift, None, ACT_RELU, out_ndhwc=True)
+    c1 = ops.conv3d_k3_s2_tc(x, hg.conv1.tc("s2"), hg.conv1.scale, hg.conv1.shift, None, ACT_RELU, out_ndhwc=True)
     c2 = _conv_tc(hg.conv2, c1, ACT_RELU)
-    c3 = ops.conv3d_k3_s2_tc(c2, _s2_weight(hg.conv3), hg.conv3.scale, hg.conv3.shift, None, ACT_RELU, out_ndhwc=True)
+    c3 = ops.conv3d_k3_s2_tc(c2, hg.conv3.tc("s2"), hg.conv3.scale, hg.conv3.shift, None, ACT_RELU, out_ndhwc=True)
     c4 = _conv_tc(hg.conv4, c3, ACT_RELU)
     r2 = ops.conv1x1_ndhwc(c2, hg.redir2.w, hg.redir2.scale, hg.redir2.shift)
-    c5 = ops.deconv3d_k3_tc(c4, _dc_weight(hg.conv5), hg.conv5.scale, hg.conv5.shift, r2, ACT_RELU, out_ndhwc=True, res_ndhwc=True)
+    c5 = ops.deconv3d_k3_tc(c4, hg.conv5.tc("dc"), hg.conv5.scale, hg.conv5.shift, r2, ACT_RELU, out_ndhwc=True, res_ndhwc=True)
     r1 = ops.conv1x1_ndhwc(x, hg.redir1.w, hg.redir1.scale, hg.redir1.shift)
-    return ops.deconv3d_k3_tc(c5, _dc_weight(hg.conv6), hg.conv6.scale, hg.conv6.shift, r1, ACT_RELU, out_ndhwc=True, res_ndhwc=True)
+    return ops.deconv3d_k3_tc(c5, hg.conv6.tc("dc"), hg.conv6.scale, hg.conv6.shift, r1, ACT_RELU, out_ndhwc=True, res_ndhwc=True)
 
 
 def _classif3_channels_last(classif3, out):
@@ -241,10 +252,8 @@ def _classif3_channels_last(classif3, out):
         mid = _conv_tc(head0, out, ACT_RELU, out_split=_split_chain_ok(width, head0, cls))
         return _conv_tc(cls, mid, ACT_NONE, out_ndhwc=False, res_ndhwc=False)
     if cls.cin == 32 and cls.cout == 1 and cls._w5 is not None and cls.stride == 1:
-        if "c1" not in cls._tc:
-            cls._tc["c1"] = ops.pack_c1_weight(cls._w5)
         head = _conv_tc(head0, out, ACT_RELU)                      # stays channels-last for the 1-channel head
-        return ops.conv3d_k3_c1_ndhwc(head, cls._tc["c1"], cls.scale, cls.shift)
+        return ops.conv3d_k3_c1_ndhwc(head, cls.tc("c1"), cls.scale, cls.shift)
     head = _conv_tc(head0, out, ACT_RELU, out_ndhwc=False)
     return _conv(cls, head)
 
@@ -345,13 +354,13 @@ def _psm_hg_channels_last_ok(hg, shape_ndhwc):
 def _psm_hourglass_channels_last(hg, x, presqu, postsqu, skip):
     """PSMNet hourglass (psmnet_cost_processor.py:108-132) with every tensor channels-last: the NCDHW route converted the layout in
     front of every layer.  Returns (out + skip, pre, post) like _PSMHourglass.__call__, all NDHWC."""
-    out = ops.conv3d_k3_s2_tc(x, _s2_weight(hg.conv1), hg.conv1.scale, hg.conv1.shift, None, ACT_RELU, out_ndhwc=True)
+    out = ops.conv3d_k3_s2_tc(x, hg.conv1.tc("s2"), hg.conv1.scale, hg.conv1.shift, None, ACT_RELU, out_ndhwc=True)
     pre = _conv_tc(hg.conv2, out, ACT_RELU, residual=postsqu)
-    out = ops.conv3d_k3_s2_tc(pre, _s2_weight(hg.conv3), hg.conv3.scale, hg.conv3.shift, None, ACT_RELU, out_ndhwc=True)
+    out = ops.conv3d_k3_s2_tc(pre, hg.conv3.tc("s2"), hg.conv3.scale, hg.conv3.shift, None, ACT_RELU, out_ndhwc=True)
     out = _conv_tc(hg.conv4, out, ACT_RELU)
-    post = ops.deconv3d_k3_tc(out, _dc_weight(hg.conv5), hg.conv5.scale, hg.conv5.shift, presqu if presqu is not None else pre, ACT_RELU,
+    post = ops.deconv3d_k3_tc(out, hg.conv5.tc("dc"), hg.conv5.scale, hg.conv5.shift, presqu if presqu is not None else pre, ACT_RELU,
                               out_ndhwc=True, res_ndhwc=True)
-    out = ops.deconv3d_k3_tc(post, _dc_weight(hg.conv6), hg.conv6.scale, hg.conv6.shift, skip, ACT_NONE, out_ndhwc=True, res_ndhwc=True)
+    out = ops.deconv3d_k3_tc(post, hg.conv6.tc("dc"), hg.conv6.scale, hg.conv6.shift, skip, ACT_NONE, out_ndhwc=True, res_ndhwc=True)
     return out, pre, post
 
 
@@ -476,10 +485,6 @@ class StereoBaseAggregation(_Engine):
         return _conv(l2, _conv(l1, x, a1), a2, gate=gate)
 
     # ---- tensor-core route: channels-last, channel plan zero-padded to multiples of 32 (24 -> 32, 48 -> 64, 96) -------------------
-    @staticmethod
-    def _pad32(c):
-        return (c + 31) // 32 * 32
-
     def tc_route_ok(self, shape):
         """True when the 1/8 and 1/16 levels and the two upper transposed convs of this hourglass have wgmma variants for an
         input volume of `shape` (B, C, D', H', W'); the 1/32 level (6 % of the MACs at config 3) stays on the CUDA-core kernels."""
@@ -492,7 +497,7 @@ class StereoBaseAggregation(_Engine):
         (l20, _), (l21, _) = self.conv["conv2"]
         if (l10.cin, l10.cout, l20.cout) != (c, 2 * c, 4 * c) or any(l._w5 is None for l in (l10, l11, l20, l21)):
             return False
-        pc, p2, p4 = self._pad32(c), self._pad32(2 * c), self._pad32(4 * c)
+        pc, p2, p4 = _pad32(c), _pad32(2 * c), _pad32(4 * c)
         return bool(ops.conv3d_s2_tc_supported(pc, p2, d, h, w) and ops.conv3d_tc_kc(p2, p2, w // 2) == 16
                     and ops.conv3d_s2_tc_supported(p2, p4, d // 2, h // 2, w // 2) and ops.conv3d_tc_kc(p4, p4, w // 4) == 16
                     and ops.deconv3d_k4_tc_supported(p4, p2, w // 4) and ops.deconv3d_k4_tc_supported(p2, pc, w // 2)
@@ -503,7 +508,7 @@ class StereoBaseAggregation(_Engine):
         """Zero-padded tensor-core packs of the layers on the 1/8 and 1/16 levels (built once per _ensure stamp)."""
         if getattr(self, "_tcp_stamp", None) == self._stamp:
             return self._tcp
-        P = self._pad32
+        P = _pad32
 
         def vec(v, n, fill):
             if v is None:
@@ -512,17 +517,22 @@ class StereoBaseAggregation(_Engine):
             out[:v.numel()] = v
             return out
 
-        def conv(layer, kw_order=(0, 1, 2)):
-            w = layer._w5
-            wp = w.new_zeros((P(w.shape[0]), P(w.shape[1])) + tuple(w.shape[2:]))
-            wp[:w.shape[0], :w.shape[1]] = w
-            return (ops.pack_tc_weight(wp, 16, kw_order=kw_order), vec(layer.scale, wp.shape[0], 1.0), vec(layer.shift, wp.shape[0], 0.0))
+        def pack(layer, transposed=False, kw_order=(0, 1, 2), bounds=None):
+            """[(lo, weight, scale, shift)] per output-channel slice [lo, hi) of `bounds` (default: one slice of every channel) of the
+            layer with Cin and Cout zero-padded to multiples of 32."""
+            w = layer._w5                                                   # (Cout, Cin, 3, 3, 3); transposed (Cin, Cout, 4, 4, 4)
+            wp = _zero_padded(w, P(w.shape[0]), P(w.shape[1]))
+            n = wp.shape[1 if transposed else 0]
+            sc, sh = vec(layer.scale, n, 1.0), vec(layer.shift, n, 0.0)
+            out = []
+            for lo, hi in bounds or ((0, n),):
+                wt = (ops.pack_tc_deconv_weight(wp[:, lo:hi].contiguous()) if transposed
+                      else ops.pack_tc_weight(wp[lo:hi].contiguous(), 16, kw_order=kw_order))
+                out.append((lo, wt, None if sc is None else sc[lo:hi].contiguous(), None if sh is None else sh[lo:hi].contiguous()))
+            return out
 
-        def deconv(layer):
-            w = layer._w5                                                   # (Cin, Cout, 4, 4, 4)
-            wp = w.new_zeros((P(w.shape[0]), P(w.shape[1])) + tuple(w.shape[2:]))
-            wp[:w.shape[0], :w.shape[1]] = w
-            return (ops.pack_tc_deconv_weight(wp), vec(layer.scale, wp.shape[1], 1.0), vec(layer.shift, wp.shape[1], 0.0))
+        def whole(layer, **kw):
+            return pack(layer, **kw)[0][1:]
 
         def cat1x1(layer):
             w = layer.w                                                     # (C0 + C1, Cout), both slabs Cout channels wide
@@ -535,42 +545,25 @@ class StereoBaseAggregation(_Engine):
         t = {}
         for name in ("conv1", "conv2"):
             (l0, _), (l1, _) = self.conv[name]
-            t[name] = (conv(l0, (1, 0, 2)), conv(l1))
+            t[name] = (whole(l0, kw_order=(1, 0, 2)), whole(l1))
         for name in ("agg_0", "agg_1"):
             (l0, _), (l1, _), (l2, _) = self.conv[name]
-            t[name] = (cat1x1(l0), conv(l1), conv(l2))
+            t[name] = (cat1x1(l0), whole(l1), whole(l2))
         for name in ("conv2_up", "conv1_up"):
-            t[name] = deconv(self.up[name][0])
+            t[name] = whole(self.up[name][0], transposed=True)
         # 1/32 level: 6c = 144 runs as 160 = 96 + 64 output-channel slices (N = 3 * 160 exceeds one CTA's weight buffers), the
         # transposed conv back to 4c = 96 as 64 + 32 (N = 4 * 96 exceeds the wgmma N limit of 256): separately packed weight slices
         (l0, _), (l1, _) = self.conv["conv3"]
         lu = self.up["conv3_up"][0]
         if P(l0.cout) == 160 and P(l0.cin) == 96 and lu.kernel == 4 and all(l._w5 is not None for l in (l0, l1, lu)):
-            def slices(layer, bounds, transposed=False, kw_order=(0, 1, 2)):
-                w = layer._w5
-                if transposed:                                              # (Cin, Cout, 4, 4, 4): pad Cin, slice Cout
-                    wp = w.new_zeros((P(w.shape[0]), P(w.shape[1])) + tuple(w.shape[2:]))
-                    wp[:w.shape[0], :w.shape[1]] = w
-                    n = wp.shape[1]
-                else:
-                    wp = w.new_zeros((P(w.shape[0]), P(w.shape[1])) + tuple(w.shape[2:]))
-                    wp[:w.shape[0], :w.shape[1]] = w
-                    n = wp.shape[0]
-                sc, sh = vec(layer.scale, n, 1.0), vec(layer.shift, n, 0.0)
-                out = []
-                for lo, hi in bounds:
-                    wt = (ops.pack_tc_deconv_weight(wp[:, lo:hi].contiguous()) if transposed
-                          else ops.pack_tc_weight(wp[lo:hi].contiguous(), 16, kw_order=kw_order))
-                    out.append((lo, wt, None if sc is None else sc[lo:hi].contiguous(), None if sh is None else sh[lo:hi].contiguous()))
-                return out
-            t["conv3"] = (slices(l0, ((0, 96), (96, 160)), kw_order=(1, 0, 2)), slices(l1, ((0, 96), (96, 160))))
-            t["conv3_up"] = slices(lu, ((0, 64), (64, 96)), transposed=True)
+            t["conv3"] = (pack(l0, kw_order=(1, 0, 2), bounds=((0, 96), (96, 160))), pack(l1, bounds=((0, 96), (96, 160))))
+            t["conv3_up"] = pack(lu, transposed=True, bounds=((0, 64), (64, 96)))
         self._tcp, self._tcp_stamp = t, self._stamp
         return t
 
     def _level32_tc_ok(self, shape):
         b, c, d, h, w = shape
-        return bool(w // 8 == 16 and self._pad32(6 * c) == 160 and self._pad32(4 * c) == 96
+        return bool(w // 8 == 16 and _pad32(6 * c) == 160 and _pad32(4 * c) == 96
                     and ops.conv3d_s2_tc_supported(96, 96, d // 4, h // 4, w // 4) and ops.conv3d_s2_tc_supported(96, 64, d // 4, h // 4, w // 4)
                     and ops.conv3d_tc_kc(160, 96, 16) == 16 and ops.conv3d_tc_kc(160, 64, 16) == 16
                     and ops.deconv3d_k4_tc_supported(160, 64, 16) and ops.deconv3d_k4_tc_supported(160, 32, 16))
@@ -585,7 +578,7 @@ class StereoBaseAggregation(_Engine):
     def _call_tc(self, x, feats):
         t = self._tc_pack()
         c = x.shape[1]
-        pc, p2, p4 = self._pad32(c), self._pad32(2 * c), self._pad32(4 * c)
+        pc, p2, p4 = _pad32(c), _pad32(2 * c), _pad32(4 * c)
         act = lambda name, i: self.conv[name][i][1]                         # noqa: E731
         xc = ops.to_ndhwc(x, pad_to=pc)
         (w0, sc0, sh0), (w1, sc1, sh1) = t["conv1"]
@@ -661,17 +654,13 @@ class StereoBaseCostHead(_Engine):
         geo = self._check(geo)
         self._ensure(geo.device)
         lay = self.layer
-        cp = (lay.cin + 31) // 32 * 32
+        cp = _pad32(lay.cin)
         if (USE_TENSOR_CORES and lay.cout == 1 and lay._w5 is not None and lay.kernel == 3 and lay.stride == 1
                 and ops.conv3d_tc_kc(cp, 1, geo.shape[-1]) == 32):
             # 24 -> 1 head on the narrow tensor-core variant: channels zero-padded to 32 while the layout changes (one pass), the
             # generic CUDA-core conv is the slow path at config 3
-            if "head" not in lay._tc:
-                w = lay._w5.new_zeros((1, cp) + tuple(lay._w5.shape[2:]))
-                w[:, :lay.cin] = lay._w5
-                lay._tc["head"] = ops.pack_tc_weight(w, 32, pad_cout_to=16)
             mon = self._watch(geo.device)
-            logits = ops.conv3d_k3_tc(ops.to_ndhwc(geo, pad_to=cp), lay._tc["head"], lay.scale, lay.shift, None, ACT_NONE,
+            logits = ops.conv3d_k3_tc(ops.to_ndhwc(geo, pad_to=cp), lay.tc("head"), lay.scale, lay.shift, None, ACT_NONE,
                                       out_ndhwc=False, res_ndhwc=False)
             if mon is not None:
                 mon.poll()
@@ -837,10 +826,10 @@ class _MSNetHourglass:
         c2 = self.conv2(self.conv1(x, in_ndhwc=True, out_ndhwc=True), in_ndhwc=True, out_ndhwc=True)
         c4 = self.conv4(self.conv3(c2, in_ndhwc=True, out_ndhwc=True), in_ndhwc=True, out_ndhwc=True)
         r2 = self.redir2(c2, in_ndhwc=True, out_ndhwc=True)
-        c5 = ops.deconv3d_k3_tc(c4, _dc_weight(self.conv5), self.conv5.scale, self.conv5.shift, r2, ACT_RELU, out_ndhwc=True,
+        c5 = ops.deconv3d_k3_tc(c4, self.conv5.tc("dc"), self.conv5.scale, self.conv5.shift, r2, ACT_RELU, out_ndhwc=True,
                                 res_ndhwc=True)
         r1 = self.redir1(x, in_ndhwc=True, out_ndhwc=True)
-        return ops.deconv3d_k3_tc(c5, _dc_weight(self.conv6), self.conv6.scale, self.conv6.shift, r1, ACT_RELU, out_ndhwc=True,
+        return ops.deconv3d_k3_tc(c5, self.conv6.tc("dc"), self.conv6.scale, self.conv6.shift, r1, ACT_RELU, out_ndhwc=True,
                                   res_ndhwc=True)
 
     def channels_last_ok(self, shape):

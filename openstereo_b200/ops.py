@@ -6,6 +6,7 @@ PyTorch is plumbing here: it owns device memory (tensor.data_ptr()) and the stre
 CPU path: a non-CUDA tensor raises, exactly like the reference's own native ops
 (stereo/modeling/models/nmrf/ops/src/ms_deform_attn.h:29-38 -> "Not implemented on the CPU").
 """
+import collections
 import math
 
 import torch
@@ -766,10 +767,10 @@ class TcWeight:
     """A conv weight packed for the wgmma kernels: `data` fp16 [3 kd][Cin/kc][3 kh][3*Cout (kw-major)][kc hi | kc lo] of
     w * 2^e_c with the 16-byte chunks of every row stored in the wgmma swizzle order (pack_tc_weight), and `inv` = 2^-(e_c + TC_ACT_SCALE_LOG2) per output channel -- the exact factor the epilogue must apply.
     `cout` is the packed row count per kw slice (narrow heads are zero-padded to 16), `cout_real` the layer's channels."""
-    __slots__ = ("data", "inv", "kc", "cout", "cout_real", "ksize", "_eff")
+    __slots__ = ("data", "inv", "kc", "cout", "cout_real", "ksize", "_eff", "_shift")
 
     def __init__(self, data, inv, kc, cout, cout_real=None, ksize=3):
-        self.data, self.inv, self.kc, self.cout, self._eff = data, inv, kc, cout, None
+        self.data, self.inv, self.kc, self.cout, self._eff, self._shift = data, inv, kc, cout, None, None
         self.cout_real = cout if cout_real is None else cout_real
         self.ksize = ksize                                                  # 3, or 4 for the k4-s2 transposed conv
 
@@ -782,6 +783,15 @@ class TcWeight:
             eff = self.inv if scale is None else scale.float() * self.inv
             self._eff = (key, eff.contiguous())
         return self._eff[1]
+
+    def eff_shift(self, shift):
+        """Epilogue shift vector: folded-BN shift or bias (or None), zero-padded to the packed rows of a zero-padded head."""
+        if shift is None or shift.numel() >= self.cout:
+            return None if shift is None else shift.float().contiguous()
+        key = (shift.data_ptr(), shift._version)
+        if self._shift is None or self._shift[0] != key:
+            self._shift = (key, torch.cat((shift.float(), shift.new_zeros(self.cout - shift.numel()).float())))
+        return self._shift[1]
 
 
 def pack_tc_weight(weight, kc=None, kw_order=(0, 1, 2), pad_cout_to=None):
@@ -875,56 +885,124 @@ def from_split(x_split):
     return ((v[..., 0, :] + v[..., 1, :]) * (1.0 / 16)).reshape(*x_split.shape[:4], g * SPLIT_GRANULE).contiguous()
 
 
+def _conv_out(n, stride, padding, dilation):
+    """Output extent of a 3-tap convolution along an input axis of n."""
+    return (n + 2 * padding - 2 * dilation - 1) // stride + 1
+
+
+# The wgmma convolution families.  extent: the output (D, H, W) of an input (D, H, W) -- a 2D family's D is 1 -- and the family's own
+# C arguments e; cout: the Cout it launches, "cout_real" (the layer's channels: a zero-padded head writes only those) or "cout" (the
+# packed rows); kc: the K chunk of the kernel that serves a shape, for the wrappers that look it up.
+_TcFamily = collections.namedtuple("_TcFamily", "rank extent cout kc")
+_TC_FAMILIES = {
+    "s1": _TcFamily(5, lambda d, h, w, e: (d, h, w), "cout_real", lambda cin, cout, w, e: conv3d_tc_kc(cin, cout, w)),
+    "s2": _TcFamily(5, lambda d, h, w, e: (max(1, d // 2), h // 2, w // 2), "cout", None),
+    "dc": _TcFamily(5, lambda d, h, w, e: (2 * d, 2 * h, 2 * w), "cout", None),           # k3 s2 p1 op1 and k4 s2 p1
+    "2d": _TcFamily(4, lambda d, h, w, e: (1, h, w), "cout", lambda cin, cout, w, e: conv2d_tc_kc(cin, cout, w, e["dilation"])),
+    "md": _TcFamily(4, lambda d, h, w, e: (1,) + tuple(_conv_out(n, e["stride"], e["padding"], e["dilation"]) for n in (h, w)),
+                    "cout", None),
+}
+# The C arguments of each entry point (include/openstereo_b200.h), in order, by the names _tc_conv gives them; the stream follows.
+_TC_ENTRY = {
+    "osb_conv3d_k3_tc_fwd": "x w scale shift residual y B Cin Cout D H W act out_cl res_cl",
+    "osb_conv3d_k3_tc_ncdhw_fwd": "x w scale shift residual y B Cin Cout D H W act out_cl res_cl",
+    "osb_conv3d_k3_tc_split_fwd": "x w scale shift residual y B Cin Cout D H W act in_layout out_layout res_layout",
+    "osb_conv3d_k3_tc_gate_fwd": "x w scale shift residual gate y B Cin Cout D H W act",
+    "osb_conv3d_k3_tc_cs_fwd": "x w scale shift residual gate y B Cin Cout D H W act ystride",
+    "osb_conv3d_k3_s2_tc_fwd": "x w scale shift residual y B Cin Cout D H W act out_cl res_cl",
+    "osb_conv3d_k3_s2_tc_cs_fwd": "x w scale shift y B Cin Cout D H W act ystride",
+    "osb_deconv3d_k3_tc_fwd": "x w scale shift residual y B Cin Cout D H W act out_cl res_cl",
+    "osb_deconv3d_k4_tc_fwd": "x w scale shift residual y B Cin Cout cout_real D H W act out_cl res_cl",
+    "osb_deconv3d_k4_tc_cs_fwd": "x w scale shift y B Cin Cout D H W act ystride",
+    "osb_conv2d_k3_tc_fwd": "x w scale shift residual y B Cin Cout H W dilation act out_cl res_cl",
+    "osb_conv2d_k3_tc_prec_fwd": "x w scale shift residual y B Cin Cout H W dilation act out_cl res_cl prec",
+    "osb_conv2d_k3_tc_gru_fwd": "x w scale shift residual mul blend_z blend_h y B Cin Cout H W act out_cl res_cl res_bstride",
+    "osb_conv2d_k3_tc_gru_prec_fwd": "x w scale shift residual mul blend_z blend_h y B Cin Cout H W act out_cl res_cl res_bstride prec",
+    "osb_mdconv2d_k3_tc_fwd": "x offset offset_bstride mask mask_bstride mask_mode w scale shift y B Cin Cout H W stride padding dilation "
+                              "deformable_groups act out_cl",
+}
+
+
+def _tc_conv(family, name, x, w_split, scale, shift, residual=None, act=ACT_NONE, out_cl=True, res_cl=True, *, kc=16, in_cl=True,
+             out_split=False, res_view=False, gate=None, y=None, coff=0, cout_real=None, profile_as=None, **extra):
+    """The host side of every wgmma convolution wrapper: launches entry point `name` of `family` once and returns y.
+    x is channels-last fp32, split (the split entry point only) or NCDHW (in_cl=False).  kc: the K chunk, None to look up the
+    family's kernel for the shape, or a tuple of the chunks `name` is instantiated for.  y is allocated channels-last or channels-first
+    (out_cl), or split (out_split), or is the caller's channels-last tensor, of which the launch writes channels [coff, coff + Cout).
+    A residual has y's shape in its own layout (res_cl, split); with res_view an NCHW residual may be a channel view of a wider
+    tensor, whose batch stride goes to the kernel.  cout_real < Cout: channels-first tensors hold only the real channels.  A gate
+    is (B, H, W, C) for a y of C channels.  extra: the family's own C arguments."""
+    fam = _TC_FAMILIES[family]
+    split_ok = name == "osb_conv3d_k3_tc_split_fwd"
+    assert x.is_cuda and x.is_contiguous() and x.dim() == fam.rank and (x.dtype == torch.float32 or (split_ok and is_split(x)))
+    in_split = is_split(x)
+    if fam.rank == 4:
+        (b, h, w, cin), d = x.shape, 1
+    elif in_cl:
+        b, d, h, w, cin = x.shape
+    else:
+        b, cin, d, h, w = x.shape
+    if in_split:
+        cin = w_split.data.shape[1] * w_split.kc
+        if x.shape[4] != 2 * cin:
+            raise ValueError("conv3d_k3_tc: an fp16 input is read as split activations (ops.to_split), 2 * Cin = %d entries per "
+                             "voxel for this weight; got %d" % (2 * cin, x.shape[4]))
+    cout = getattr(w_split, fam.cout)
+    if not isinstance(kc, int):
+        found = fam.kc(cin, cout, w, extra)
+        assert found and (kc is None or found in kc)
+        kc = found
+    wptr, scale = _tc_args(w_split, cin, kc, scale)
+    shift = w_split.eff_shift(shift)
+    dims = fam.extent(d, h, w, extra)[5 - fam.rank:]
+    creal = cout if cout_real is None else int(cout_real)
+
+    def shape(cl, split):
+        return (b, *dims, 2 * cout if split else cout) if cl else (b, creal, *dims)
+    if y is None:
+        y = torch.empty(shape(out_cl, out_split), dtype=torch.float16 if out_split else torch.float32, device=x.device)
+    else:
+        assert y.is_contiguous() and y.dtype == torch.float32 and y.dim() == 5 and tuple(y.shape[:4]) == (b, *dims)
+        assert 0 <= coff and coff + cout <= y.shape[-1] and coff % 4 == 0
+    res_split, res_bstride = residual is not None and is_split(residual), 0
+    if residual is not None:
+        assert residual.is_cuda and residual.dtype == (torch.float16 if res_split else torch.float32) and (split_ok or not res_split)
+        assert tuple(residual.shape) == shape(res_cl, res_split)
+        if res_view and not res_cl:
+            assert tuple(residual.stride()[1:]) == (dims[-2] * dims[-1], dims[-1], 1)
+            res_bstride = 0 if residual.is_contiguous() else residual.stride(0)
+        else:
+            assert residual.is_contiguous()
+    if gate is not None:
+        assert tuple(gate.shape) == (b, h, w, y.shape[-1]) and gate.is_contiguous() and gate.dtype == torch.float32 and gate.is_cuda
+    layout = lambda split, cl: LAYOUT_SPLIT if split else (LAYOUT_NDHWC if cl else LAYOUT_NCDHW)     # noqa: E731
+    args = dict(x=x.data_ptr(), w=wptr, scale=_ptr(scale), shift=_ptr(shift), residual=_ptr(residual),
+                gate=None if gate is None else gate.data_ptr() + 4 * coff, y=y.data_ptr() + 4 * coff, B=b, Cin=cin, Cout=cout,
+                cout_real=creal, D=d, H=h, W=w, act=act, out_cl=1 if out_cl else 0, res_cl=1 if res_cl else 0,
+                in_layout=layout(in_split, in_cl), out_layout=layout(out_split, out_cl), res_layout=layout(res_split, res_cl),
+                ystride=y.shape[-1], res_bstride=res_bstride, **extra)
+    _call(name, *(args[k] for k in _TC_ENTRY[name].split()), _stream(y), profile_as=profile_as)
+    return y
+
+
 def conv3d_k3_tc(x_ndhwc, w_split, scale=None, shift=None, residual=None, act=ACT_NONE, out_ndhwc=True, res_ndhwc=True,
                  in_ncdhw=False, gate=None, out_split=False):
     """3x3x3 stride-1 conv + folded BN + residual + activation on the tensor cores.  x_ndhwc: (B,D,H,W,Cin), or the NCDHW
     tensor (B,Cin,D,H,W) with in_ncdhw=True (W = 128 layers only: the cost volume goes in as the volume kernel wrote it).
     W = 128 layers also take x and a channels-last residual as split activations (to_split), and out_split=True returns y as one;
     a split residual enters as (hi + lo) / 16."""
-    assert x_ndhwc.is_cuda and x_ndhwc.dtype in (torch.float32, torch.float16) and x_ndhwc.is_contiguous() and x_ndhwc.dim() == 5
-    in_split = is_split(x_ndhwc)
-    assert not (in_split and in_ncdhw)
-    if in_ncdhw:
-        b, cin, d, h, w = x_ndhwc.shape
-    else:
-        b, d, h, w, cin = x_ndhwc.shape
-        if in_split:
-            cin = w_split.data.shape[1] * w_split.kc
-            if x_ndhwc.shape[4] != 2 * cin:
-                raise ValueError("conv3d_k3_tc: an fp16 input is read as split activations (ops.to_split), 2 * Cin = %d entries per "
-                                 "voxel for this weight; got %d" % (2 * cin, x_ndhwc.shape[4]))
-    cout = w_split.cout_real
-    kc = conv3d_tc_kc(cin, cout, w)
-    assert kc
-    wptr, scale = _tc_args(w_split, cin, kc, scale)
-    if shift is not None and shift.numel() < w_split.cout:               # zero-padded head
-        shift = torch.cat((shift.float(), shift.new_zeros(w_split.cout - shift.numel()).float()))
-    res_split = residual is not None and is_split(residual)
-    if residual is not None:
-        want = (b, d, h, w, 2 * cout if res_split else cout) if res_ndhwc else (b, cout, d, h, w)
-        assert tuple(residual.shape) == want and residual.is_contiguous() and (res_split or residual.dtype == torch.float32)
-    if in_split or out_split or res_split:
-        assert gate is None and (out_ndhwc or not out_split)
-        shape = (b, d, h, w, 2 * cout if out_split else cout) if out_ndhwc else (b, cout, d, h, w)
-        y = torch.empty(shape, dtype=torch.float16 if out_split else torch.float32, device=x_ndhwc.device)
-        layout = lambda split, ndhwc: LAYOUT_SPLIT if split else (LAYOUT_NDHWC if ndhwc else LAYOUT_NCDHW)
+    args = (x_ndhwc, w_split, scale, shift, residual, act, out_ndhwc, res_ndhwc)
+    if is_split(x_ndhwc) or out_split or (residual is not None and is_split(residual)):
+        assert not (is_split(x_ndhwc) and in_ncdhw) and gate is None and (out_ndhwc or not out_split)
         # profiled as the fp32 entry point reading the same input layout would be: the same kernel and the same layers
-        _call("osb_conv3d_k3_tc_split_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), y.data_ptr(),
-              b, cin, cout, d, h, w, act, layout(in_split, not in_ncdhw), layout(out_split, out_ndhwc), layout(res_split, res_ndhwc),
-              _stream(y), profile_as="osb_conv3d_k3_tc_ncdhw_fwd" if in_ncdhw else "osb_conv3d_k3_tc_fwd")
-        return y
-    shape = (b, d, h, w, cout) if out_ndhwc else (b, cout, d, h, w)
-    y = torch.empty(shape, dtype=torch.float32, device=x_ndhwc.device)
-    assert not in_ncdhw or kc == 32
+        return _tc_conv("s1", "osb_conv3d_k3_tc_split_fwd", *args, kc=None, in_cl=not in_ncdhw, out_split=out_split,
+                        profile_as="osb_conv3d_k3_tc_ncdhw_fwd" if in_ncdhw else "osb_conv3d_k3_tc_fwd")
     if gate is not None:                                                     # FeatureAtt: (B,H,W,Cout) multiplier after the activation
-        assert kc == 16 and out_ndhwc and res_ndhwc and not in_ncdhw
-        assert tuple(gate.shape) == (b, h, w, cout) and gate.is_contiguous() and gate.dtype == torch.float32 and gate.is_cuda
-        _call("osb_conv3d_k3_tc_gate_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), gate.data_ptr(),
-              y.data_ptr(), b, cin, cout, d, h, w, act, _stream(y))
-        return y
-    _call("osb_conv3d_k3_tc_ncdhw_fwd" if in_ncdhw else "osb_conv3d_k3_tc_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual),
-          y.data_ptr(), b, cin, cout, d, h, w, act, 1 if out_ndhwc else 0, 1 if res_ndhwc else 0, _stream(y))
-    return y
+        assert out_ndhwc and res_ndhwc and not in_ncdhw
+        return _tc_conv("s1", "osb_conv3d_k3_tc_gate_fwd", *args, kc=(16,), gate=gate)
+    if in_ncdhw:
+        return _tc_conv("s1", "osb_conv3d_k3_tc_ncdhw_fwd", *args, kc=(32,), in_cl=False)
+    return _tc_conv("s1", "osb_conv3d_k3_tc_fwd", *args, kc=None)
 
 
 def conv3d_s2_tc_supported(cin, cout, d, h, w):
@@ -935,19 +1013,7 @@ def conv3d_k3_s2_tc(x_ndhwc, w_split, scale=None, shift=None, residual=None, act
     """3x3x3 STRIDE-2 conv + folded BN + residual + activation on the tensor cores.  x_ndhwc: (B,D,H,W,Cin), even D,H,W, or D = 1:
     a stride-2 3x3 Conv2d as one plane (its taps at kd = 1 of the weight, one output plane);
     w_split = pack_tc_weight(weight, 16, kw_order=(1, 0, 2))."""
-    assert x_ndhwc.is_cuda and x_ndhwc.dtype == torch.float32 and x_ndhwc.is_contiguous() and x_ndhwc.dim() == 5
-    b, d, h, w, cin = x_ndhwc.shape
-    cout = w_split.cout
-    wptr, scale = _tc_args(w_split, cin, 16, scale)
-    do, ho, wo = max(1, d // 2), h // 2, w // 2
-    shape = (b, do, ho, wo, cout) if out_ndhwc else (b, cout, do, ho, wo)
-    y = torch.empty(shape, dtype=torch.float32, device=x_ndhwc.device)
-    if residual is not None:
-        want = (b, do, ho, wo, cout) if res_ndhwc else (b, cout, do, ho, wo)
-        assert tuple(residual.shape) == want and residual.is_contiguous()
-    _call("osb_conv3d_k3_s2_tc_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual),
-          y.data_ptr(), b, cin, cout, d, h, w, act, 1 if out_ndhwc else 0, 1 if res_ndhwc else 0, _stream(y))
-    return y
+    return _tc_conv("s2", "osb_conv3d_k3_s2_tc_fwd", x_ndhwc, w_split, scale, shift, residual, act, out_ndhwc, res_ndhwc)
 
 
 def deconv3d_tc_supported(cin, cout, w):
@@ -971,50 +1037,18 @@ def deconv3d_k4_tc(x_ndhwc, w_split, scale=None, shift=None, residual=None, act=
                    cout_real=None):
     """ConvTranspose3d(k4, s2, p1) + folded BN + residual + activation on the tensor cores.  x_ndhwc: (B,D,H,W,Cin); cout_real <
     packed Cout (zero-padded channel plan) is allowed for an NCDHW output, which then holds only the real channels."""
-    assert x_ndhwc.is_cuda and x_ndhwc.dtype == torch.float32 and x_ndhwc.is_contiguous() and x_ndhwc.dim() == 5
-    b, d, h, w, cin = x_ndhwc.shape
-    cout = w_split.cout
-    creal = cout if cout_real is None else int(cout_real)
-    assert w_split.ksize == 4 and (out_ndhwc is False or creal == cout)
-    wptr, scale = _tc_args(w_split, cin, 16, scale)
-    shape = (b, 2 * d, 2 * h, 2 * w, cout) if out_ndhwc else (b, creal, 2 * d, 2 * h, 2 * w)
-    y = torch.empty(shape, dtype=torch.float32, device=x_ndhwc.device)
-    if residual is not None:
-        want = (b, 2 * d, 2 * h, 2 * w, cout) if res_ndhwc else (b, creal, 2 * d, 2 * h, 2 * w)
-        assert tuple(residual.shape) == want and residual.is_contiguous()
-    _call("osb_deconv3d_k4_tc_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual),
-          y.data_ptr(), b, cin, cout, creal, d, h, w, act, 1 if out_ndhwc else 0, 1 if res_ndhwc else 0, _stream(y))
-    return y
+    assert w_split.ksize == 4 and (not out_ndhwc or cout_real in (None, w_split.cout))
+    return _tc_conv("dc", "osb_deconv3d_k4_tc_fwd", x_ndhwc, w_split, scale, shift, residual, act, out_ndhwc, res_ndhwc,
+                    cout_real=cout_real)
 
 
 def tc_slice(kind, x_ndhwc, w_split, scale, shift, y, coff, act=ACT_NONE, gate=None):
     """One output-channel SLICE of a tensor-core conv (include/openstereo_b200.h: *_cs_fwd): channels [coff, coff + w_split.cout) of
     the preallocated channels-last `y` (..., Ctot).  kind: "s1" (3x3x3 stride 1, optional (B,H,W,Ctot) gate), "s2" (stride 2) or
     "dc4" (ConvTranspose3d k4 s2 p1).  scale / shift: this slice's folded BN."""
-    assert x_ndhwc.is_cuda and x_ndhwc.dtype == torch.float32 and x_ndhwc.is_contiguous() and x_ndhwc.dim() == 5
-    assert y.is_contiguous() and y.dtype == torch.float32 and y.dim() == 5
-    b, d, h, w, cin = x_ndhwc.shape
-    cout, ctot = w_split.cout, y.shape[-1]
-    assert 0 <= coff and coff + cout <= ctot and coff % 4 == 0
-    wptr, scale = _tc_args(w_split, cin, 16, scale)
-    yp = y.data_ptr() + 4 * coff
-    if kind == "s1":
-        assert tuple(y.shape[:4]) == (b, d, h, w)
-        gp = None
-        if gate is not None:
-            assert tuple(gate.shape) == (b, h, w, ctot) and gate.is_contiguous()
-            gp = gate.data_ptr() + 4 * coff
-        _call("osb_conv3d_k3_tc_cs_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), None, gp, yp, b, cin, cout, d, h, w, act,
-              ctot, _stream(y))
-    elif kind == "s2":
-        assert tuple(y.shape[:4]) == (b, d // 2, h // 2, w // 2) and gate is None
-        _call("osb_conv3d_k3_s2_tc_cs_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), yp, b, cin, cout, d, h, w, act, ctot,
-              _stream(y))
-    else:
-        assert kind == "dc4" and tuple(y.shape[:4]) == (b, 2 * d, 2 * h, 2 * w) and gate is None and w_split.ksize == 4
-        _call("osb_deconv3d_k4_tc_cs_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), yp, b, cin, cout, d, h, w, act, ctot,
-              _stream(y))
-    return y
+    assert kind == "s1" or (gate is None and (kind == "s2" or (kind == "dc4" and w_split.ksize == 4)))
+    name = {"s1": "osb_conv3d_k3_tc_cs_fwd", "s2": "osb_conv3d_k3_s2_tc_cs_fwd", "dc4": "osb_deconv3d_k4_tc_cs_fwd"}[kind]
+    return _tc_conv("dc" if kind == "dc4" else kind, name, x_ndhwc, w_split, scale, shift, act=act, gate=gate, y=y, coff=coff)
 
 
 def feature_att_gate(feat, w1, scale1, shift1, w2, scale2, shift2, pad_to=None, act1=ACT_LEAKY):
@@ -1046,18 +1080,7 @@ def conv1x1_ndhwc_cat(x0, x1, w_packed, scale=None, shift=None, act=ACT_NONE):
 
 def deconv3d_k3_tc(x_ndhwc, w_split, scale=None, shift=None, residual=None, act=ACT_NONE, out_ndhwc=False, res_ndhwc=False):
     """ConvTranspose3d(k3, s2, p1, op1) + folded BN + residual + activation on the tensor cores.  x_ndhwc: (B,D,H,W,Cin)."""
-    assert x_ndhwc.is_cuda and x_ndhwc.dtype == torch.float32 and x_ndhwc.is_contiguous() and x_ndhwc.dim() == 5
-    b, d, h, w, cin = x_ndhwc.shape
-    cout = w_split.cout
-    wptr, scale = _tc_args(w_split, cin, 16, scale)
-    shape = (b, 2 * d, 2 * h, 2 * w, cout) if out_ndhwc else (b, cout, 2 * d, 2 * h, 2 * w)
-    y = torch.empty(shape, dtype=torch.float32, device=x_ndhwc.device)
-    if residual is not None:
-        want = (b, 2 * d, 2 * h, 2 * w, cout) if res_ndhwc else (b, cout, 2 * d, 2 * h, 2 * w)
-        assert tuple(residual.shape) == want and residual.is_contiguous()
-    _call("osb_deconv3d_k3_tc_fwd", x_ndhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual),
-          y.data_ptr(), b, cin, cout, d, h, w, act, 1 if out_ndhwc else 0, 1 if res_ndhwc else 0, _stream(y))
-    return y
+    return _tc_conv("dc", "osb_deconv3d_k3_tc_fwd", x_ndhwc, w_split, scale, shift, residual, act, out_ndhwc, res_ndhwc)
 
 
 def conv1x1_ndhwc(x_ndhwc, w_packed, scale=None, shift=None, act=ACT_NONE):
@@ -1257,22 +1280,8 @@ def conv2d_k3_tc(x_nhwc, w_split, scale=None, shift=None, residual=None, act=ACT
     products; "f16": one fp16 MMA per product (autocast accuracy, osb_conv2d_k3_tc_prec_fwd) where a 16-channel-chunk kernel
     serves the shape -- a 32-channel-chunk shape (conv2d_tc_kc(...) == 32) keeps the fp32-accurate product.  fp32 in and out."""
     prec = _precision(precision)
-    assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float32 and x_nhwc.is_contiguous() and x_nhwc.dim() == 4
-    b, h, w, cin = x_nhwc.shape
-    cout = w_split.cout
-    kc = conv2d_tc_kc(cin, cout, w, dilation)
-    assert kc
-    wptr, scale = _tc_args(w_split, cin, kc, scale)
-    y = torch.empty((b, h, w, cout) if out_nhwc else (b, cout, h, w), dtype=torch.float32, device=x_nhwc.device)
-    if residual is not None:
-        assert residual.is_contiguous() and residual.numel() == y.numel()
-    args = (x_nhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), y.data_ptr(), b, cin, cout, h, w, dilation, act,
-            int(out_nhwc), int(res_nhwc))
-    if prec:
-        _call("osb_conv2d_k3_tc_prec_fwd", *args, prec, _stream(y))
-    else:
-        _call("osb_conv2d_k3_tc_fwd", *args, _stream(y))
-    return y
+    return _tc_conv("2d", "osb_conv2d_k3_tc_prec_fwd" if prec else "osb_conv2d_k3_tc_fwd", x_nhwc, w_split, scale, shift, residual,
+                    act, out_nhwc, res_nhwc, kc=None, dilation=dilation, prec=prec)
 
 
 # --------------------------------------------------------------------------- ConvGRU update (gru.py)
@@ -1301,29 +1310,12 @@ def conv2d_k3_tc_gru(x_nhwc, w_split, shift=None, residual=None, act=ACT_NONE, m
     split() view of a wider (B, C', H, W) tensor (its batch stride goes to the kernel, no copy).  precision: as conv2d_k3_tc
     (osb_conv2d_k3_tc_gru_prec_fwd); the epilogue is fp32 either way."""
     prec = _precision(precision)
-    assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float32 and x_nhwc.is_contiguous() and x_nhwc.dim() == 4
-    b, h, w, cin = x_nhwc.shape
-    cout = w_split.cout
-    wptr, scale = _tc_args(w_split, cin, 16, None)
-    y = torch.empty((b, h, w, cout) if out_nhwc else (b, cout, h, w), dtype=torch.float32, device=x_nhwc.device)
-    rbs = 0
-    if residual is not None:
-        assert residual.is_cuda and residual.dtype == torch.float32
-        if res_nhwc:
-            assert tuple(residual.shape) == (b, h, w, cout) and residual.is_contiguous()
-        else:
-            assert tuple(residual.shape) == (b, cout, h, w) and tuple(residual.stride()[1:]) == (h * w, w, 1)
-            rbs = 0 if residual.is_contiguous() else residual.stride(0)
     z, hh = blend if blend is not None else (None, None)
     for t in (mul, z, hh):
-        assert t is None or (tuple(t.shape) == (b, h, w, cout) and t.is_contiguous() and t.dtype == torch.float32 and t.is_cuda)
-    args = (x_nhwc.data_ptr(), wptr, _ptr(scale), _ptr(shift), _ptr(residual), _ptr(mul), _ptr(z), _ptr(hh), y.data_ptr(), b, cin,
-            cout, h, w, act, int(out_nhwc), int(res_nhwc), rbs)
-    if prec:
-        _call("osb_conv2d_k3_tc_gru_prec_fwd", *args, prec, _stream(y))
-    else:
-        _call("osb_conv2d_k3_tc_gru_fwd", *args, _stream(y))
-    return y
+        assert t is None or (tuple(t.shape) == (*x_nhwc.shape[:3], w_split.cout) and t.is_contiguous() and t.dtype == torch.float32
+                             and t.is_cuda)
+    return _tc_conv("2d", "osb_conv2d_k3_tc_gru_prec_fwd" if prec else "osb_conv2d_k3_tc_gru_fwd", x_nhwc, w_split, None, shift,
+                    residual, act, out_nhwc, res_nhwc, res_view=True, mul=_ptr(mul), blend_z=_ptr(z), blend_h=_ptr(hh), prec=prec)
 
 
 # --------------------------------------------------------------------------- modulated deformable convolution (aanet.py)
@@ -1344,23 +1336,17 @@ def mdconv2d_k3_tc(x_nhwc, offset, mask, w_split, scale=None, shift=None, stride
     logits, m = 2 * sigmoid(mask); w_split = pack_tc_weight_2d(weight, 16, pad_cout_to=32 for 16 channels); scale / shift:
     per output channel (w_split.cout_real of them).  -> (B, cout_real, Ho, Wo), or (B, Ho, Wo, cout) when out_nhwc (no zero-padded
     plan).  No backward."""
-    assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float32 and x_nhwc.is_contiguous() and x_nhwc.dim() == 4
-    b, h, w, cin = x_nhwc.shape
-    ho = (h + 2 * padding - 2 * dilation - 1) // stride + 1
-    wo = (w + 2 * padding - 2 * dilation - 1) // stride + 1
+    assert x_nhwc.dim() == 4
+    b, h, w, _ = x_nhwc.shape
+    ho, wo = (_conv_out(n, stride, padding, dilation) for n in (h, w))
     for t, n in ((offset, 18), (mask, 9)):
         assert t.is_cuda and t.dtype == torch.float32 and tuple(t.shape) == (b, deformable_groups * n, ho, wo), (tuple(t.shape), n)
         assert tuple(t.stride()[1:]) == (ho * wo, wo, 1), "offset / mask need unit strides inside each batch"
     cout, real = w_split.cout, w_split.cout_real
     assert not (out_nhwc and real != cout), "a zero-padded channel plan writes NCHW"
-    wptr, eff = _tc_args(w_split, cin, 16, scale)
-    if shift is not None and shift.numel() < cout:
-        shift = torch.cat((shift.float(), shift.new_zeros(cout - shift.numel()).float()))
-    shift = None if shift is None else shift.float().contiguous()
-    y = torch.empty((b, ho, wo, cout) if out_nhwc else (b, cout, ho, wo), dtype=torch.float32, device=x_nhwc.device)
-    _call("osb_mdconv2d_k3_tc_fwd", x_nhwc.data_ptr(), offset.data_ptr(), offset.stride(0), mask.data_ptr(), mask.stride(0),
-          int(mask_mode), wptr, _ptr(eff), _ptr(shift), y.data_ptr(), b, cin, cout, h, w, stride, padding, dilation,
-          deformable_groups, act, int(out_nhwc), _stream(y))
+    y = _tc_conv("md", "osb_mdconv2d_k3_tc_fwd", x_nhwc, w_split, scale, shift, act=act, out_cl=out_nhwc, offset=offset.data_ptr(),
+                 offset_bstride=offset.stride(0), mask=mask.data_ptr(), mask_bstride=mask.stride(0), mask_mode=int(mask_mode),
+                 stride=stride, padding=padding, dilation=dilation, deformable_groups=deformable_groups)
     return y if real == cout else y[:, :real].contiguous()
 
 
