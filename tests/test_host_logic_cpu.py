@@ -325,16 +325,23 @@ def test_kernel_contract_registry_matches_sources():
 
 
 def _struct_fields(name, struct):
-    """Field names of `struct <struct> { ... };` in csrc/<name> (member functions skipped)."""
+    """Field names of `struct <struct> { ... };` in csrc/<name> (member functions skipped, array extents dropped)."""
     import re
     body = re.search(r"struct\s+%s\s*\{(.*?)\n\};" % struct, _csrc(name), re.S).group(1)
     body = re.sub(r"[\w:<>]+\s+\w+\s*\([^()]*\)\s*(?:const\s*)?\{[^{}]*\}", "", body)      # bool slice() const { ... }
     fields = []
     for stmt in body.split(";"):
-        stmt = re.sub(r"=[^,]*", "", stmt).strip()
+        stmt = re.sub(r"=[^,]*|\[[^\]]*\]", "", stmt).strip()                                # initialisers, [GEO_MAX_LEVELS]
         if stmt:
             fields += [re.findall(r"\w+", part)[-1] for part in stmt.split(",")]
     return fields
+
+
+def _kernel_params(name, kernel):
+    """Parameter names of __global__ <kernel>(...) in csrc/<name>."""
+    import re
+    params = re.search(_GLOBAL.replace(r"(\w+)", kernel) + r"([^()]*)\)", _csrc(name)).group(1)
+    return [re.findall(r"\w+", p)[-1] for p in params.split(",")]
 
 
 def test_tc_runtime_modes_have_contract_rows():
@@ -358,6 +365,45 @@ def test_tc_runtime_modes_have_contract_rows():
     dcn = [r for r in REGISTRY if r.kind == "dcn"]
     assert {r.opt[0] for r in dcn} == {1, 2} and {r.opt[1] for r in dcn} == {1, 2, 3}
     assert {r.cin // r.opt[2] for r in dcn} >= {4, 8, 16}
+
+
+def test_nonconv_runtime_modes_have_contract_rows():
+    """Every field of struct GeoParams (geo.cu) and struct WarpParams (cascade.cu) and every parameter of ncdhw_to_ndhwc_kernel
+    (conv3d_tc.cu) is classified in tests/test_kernel_contract_gpu.py as an operand / geometry field or as the runtime mode it selects;
+    every mode is one row family whose rows reach exactly the instantiations NONCONV_MODE_VARIANTS lists for it (test_routing checks
+    each row's on the GPU); each lookup family has a row whose taps take the fallback read and a row at grid z = 65535."""
+    from test_kernel_contract_gpu import (GEO_PARAMS_FIELDS, LAYOUT_KERNEL_PARAMS, MODE_REQUIREMENTS, NONCONV_MODE_VARIANTS, REGISTRY,
+                                          WARP_PARAMS_FIELDS, grid_z)
+    classified = {}
+    for what, fields, table in (("GeoParams", _struct_fields("geo.cu", "GeoParams"), GEO_PARAMS_FIELDS),
+                                ("WarpParams", _struct_fields("cascade.cu", "WarpParams"), WARP_PARAMS_FIELDS),
+                                ("ncdhw_to_ndhwc_kernel", _kernel_params("conv3d_tc.cu", "ncdhw_to_ndhwc_kernel"), LAYOUT_KERNEL_PARAMS)):
+        assert len(fields) == len(set(fields)) and len(fields) >= 9, (what, fields)
+        assert set(fields) == set(table), "%s fields not classified: %s; classified fields that are gone: %s" % (
+            what, sorted(set(fields) - set(table)), sorted(set(table) - set(fields)))
+        classified[what] = {m for m in table.values() if m}
+    assert {"geo", "corr", "out_corr", "D2"} <= set(GEO_PARAMS_FIELDS) and {"border", "ys", "coff"} <= set(WARP_PARAMS_FIELDS) | set(
+        LAYOUT_KERNEL_PARAMS)
+    modes = set().union(*classified.values())
+    assert modes == set(NONCONV_MODE_VARIANTS), "modes without an entry in NONCONV_MODE_VARIANTS: %s; entries no field selects: %s" % (
+        sorted(modes - set(NONCONV_MODE_VARIANTS)), sorted(set(NONCONV_MODE_VARIANTS) - modes))
+    plain = {r.fam for r in REGISTRY} - modes
+    for mode, variants in NONCONV_MODE_VARIANTS.items():
+        rows = [r for r in REGISTRY if r.fam == mode]
+        assert rows, "mode %s has no row family" % mode
+        assert mode not in plain
+        got = {r.variant for r in rows}
+        assert got == variants, "mode %s: instantiations without a row: %s; rows reaching an instantiation the mode does not: %s" % (
+            mode, sorted(variants - got), sorted(got - variants))
+    for fam in ("geov", "geomr"):
+        rows = [r for r in REGISTRY if r.fam == fam]
+        assert any(r.opts.get("cross") and r.opts["radius"] == 4 for r in rows), "%s: no row whose taps take the fallback read" % fam
+        assert any(grid_z(r) == 65535 for r in rows), "%s: no row at grid z = 65535" % fam
+    assert set(MODE_REQUIREMENTS) == set(NONCONV_MODE_VARIANTS)
+    for mode, needs in MODE_REQUIREMENTS.items():
+        rows = [r for r in REGISTRY if r.fam == mode]
+        for what, met in needs.items():
+            assert any(met(r) for r in rows), "mode %s: no row with %s" % (mode, what)
 
 
 def test_instance_norm_modes_have_contract_rows():

@@ -24,6 +24,15 @@ and a small shape with partial tiles, chunks and units in every tiled dimension.
                and nearest_resize3d have totals above their SM-count-based grid caps;
   determinism  two launches are bit-identical, except epe_partial_kernel, whose float atomics add block partial sums in
                arrival order: its error sum gets the bar of the sum instead (its counts are integers and stay exact).
+Runtime modes are row families of their own (NONCONV_MODE_VARIANTS; GEO_PARAMS_FIELDS, WARP_PARAMS_FIELDS and LAYOUT_KERNEL_PARAMS
+classify every field that selects one, and MODE_REQUIREMENTS lists the edges each family's rows must cover):
+  geov         the geometry-only lookup (corr[0] == NULL): geo_model without correlation rows, a grid z of exactly 65535;
+  geomr        the multi-range lookup: four outputs, one case each, the other three written to guarded scratch; vol2's taps
+               leave both ends; D1 != D2, D1 = D2 = 2, W2 != W, a grid z of exactly 65535;
+  warp         the disparity warp (border = 1): border_roundtrip replayed in fp32, disparities past both edges, 227 KB of rows;
+  slice        the channel slice of a channels-last concatenation: exact inside the slice, the other channels still NaN;
+  split        the split NDHWC conversion: every 32-bit word of hi/lo halves exact, tc_overflow_count >= 1 after a saturating
+               row and 0 after the others.
 test_volume_item_order_0: the other work-item order, read once per process, in a child process, bit-identical to order 1.
 test_volume_input_types: fp16 / bf16 inputs through ops.*: output in the input type, equal to the rounded fp32 result.
 test_refusals: every input an entry point refuses returns OSB_EINVAL and launches nothing.
@@ -120,6 +129,19 @@ REGISTRY = [
     R("geo-r0-l2", "geo", "geo_lookup_kernel<0>", (1, 3, 16, 2, 40, 44, 2), radius=0),
     R("geo-r1-l3", "geo", "geo_lookup_kernel<0>", (2, 2, 24, 2, 33, 30, 3), radius=1),
     R("geo-r3-l4", "geo", "geo_lookup_kernel<0>", (1, 2, 32, 3, 131, 140, 4), radius=3),
+    # geometry-only mode (corr[0] == NULL, osb_geo_volume_lookup_fwd) (B, C, D, H, W, levels): output (B, L * C * (2r + 1), H, W)
+    R("geov-r4-l4", "geov", "geo_lookup_kernel<4>", (2, 3, 48, 3, 130, 4), radius=4, cross=1),
+    R("geov-r4-l1", "geov", "geo_lookup_kernel<4>", (1, 2, 8, 2, 21, 1), radius=4),
+    R("geov-r0-l2", "geov", "geo_lookup_kernel<0>", (1, 3, 16, 2, 40, 2), radius=0),
+    R("geov-r2-l3-b3", "geov", "geo_lookup_kernel<0>", (3, 2, 24, 2, 131, 3), radius=2),
+    R("geov-zmax", "geov", "geo_lookup_kernel<0>", (257, 85, 8, 1, 3, 3), radius=1),        # grid z = B * L * C = 65535
+    # multi-range mode (out_corr != NULL, osb_geo_multirange_lookup_fwd) (B, C, D0, D1, D2, H, W, W2, levels): four outputs, the
+    # geo_volume0 pyramid, vol1 at disp / 2, vol2 at disp / 4 and the correlation rows
+    R("geomr-r4-l4", "geomr", "geo_lookup_kernel<4>", (2, 3, 48, 13, 7, 2, 130, 136, 4), radius=4, cross=1),
+    R("geomr-r4-l1-d2", "geomr", "geo_lookup_kernel<4>", (1, 2, 8, 2, 2, 3, 21, 20, 1), radius=4),
+    R("geomr-r0-l2", "geomr", "geo_lookup_kernel<0>", (1, 3, 16, 6, 10, 2, 40, 44, 2), radius=0),
+    R("geomr-r3-l3", "geomr", "geo_lookup_kernel<0>", (2, 2, 24, 12, 5, 2, 131, 140, 3), radius=3),
+    R("geomr-zmax", "geomr", "geo_lookup_kernel<0>", (771, 28, 4, 3, 5, 1, 3, 6, 1), radius=1),   # B * (L * C + 2C + L) = 65535
     R("pool-small", "pool", "avgpool_pairs_kernel", (3, 7, 35)),                         # odd n: the last element is dropped
     R("pool-multipass", "pool", "avgpool_pairs_kernel", (3, 11, 0)),                     # inner from the SM count: > 2 grid passes
     # context_upsample (B, h, w, s): one thread per 4 output columns, 512 columns per block
@@ -138,6 +160,13 @@ REGISTRY = [
     R("cas-gwc-k16", "cas", "warped_volume_kernel<16>", (1, 32, 2, 10, 3, 7, 33), two=1),
     R("cas-gwc-wmax", "cas", "warped_volume_kernel<16>", (1, 16, 1, 1, 2, 2, 1816)),     # 16 x 2 rows x 1816 floats = 227 KB
     R("cas-cat-wmax", "cas", "warped_volume_kernel<8>", (1, 0, 0, 1, 2, 2, 3632), mask=1),
+    # disparity-warp mode (border = 1, osb_disp_warp_fwd) (B, C, H, W): units of 8 channels; every row coordinate is an integer at
+    # H = 2 (and 3), not at the heights below
+    R("warp-c5-h2", "warp", "warped_volume_kernel<8>", (2, 5, 2, 17), two=0),
+    R("warp-c8-w131", "warp", "warped_volume_kernel<8>", (1, 8, 7, 131), two=1),
+    R("warp-c19", "warp", "warped_volume_kernel<8>", (2, 19, 6, 40), two=1),              # three units, the last one partial
+    R("warp-wmax", "warp", "warped_volume_kernel<8>", (1, 8, 4, 3632), two=1),            # 8 x 2 rows x 3632 floats = 227 KB, all staged
+    R("warp-w2", "warp", "warped_volume_kernel<8>", (1, 1, 5, 2), two=1),
     # coex.cu regression (B, D, h, w): tiles of 16 x 32 low-resolution pixels
     R("coex-k2", "coex", "coex_regression_kernel<2>", (2, 2, 5, 9), k=2, logits=1),
     R("coex-k3", "coex", "coex_regression_kernel<3>", (1, 3, 17, 33), k=3, logits=1, ties=1),
@@ -162,8 +191,96 @@ REGISTRY = [
     R("pad-24-32", "pad", "ncdhw_to_ndhwc_kernel", (2, 24, 32, 3, 5, 7)),
     R("pad-40", "pad", "ncdhw_to_ndhwc_kernel", (1, 40, 40, 2, 3, 11)),
     R("pad-48-64", "pad", "ncdhw_to_ndhwc_kernel", (1, 48, 64, 2, 5, 9)),
+    # channel slice (osb_ncdhw_to_ndhwc_slice) (B, C, D, H, W, ystride, coff): channels coff .. coff + C - 1 of voxels of ystride
+    R("slice-96-at-150", "slice", "ncdhw_to_ndhwc_kernel", (2, 96, 1, 5, 37, 300, 150)),
+    R("slice-5-at-3", "slice", "ncdhw_to_ndhwc_kernel", (1, 5, 2, 3, 11, 13, 3)),
+    R("slice-40-whole", "slice", "ncdhw_to_ndhwc_kernel", (1, 40, 2, 3, 7, 40, 0)),
+    R("slice-33-at-37-last", "slice", "ncdhw_to_ndhwc_kernel", (2, 33, 1, 4, 9, 70, 37)),  # odd C and offset, ends at the last channel
+    # split output (osb_ncdhw_to_split) (B, C, D, H, W): split NDHWC, 2C fp16 per voxel
+    R("split-c16", "split", "ncdhw_to_ndhwc_kernel", (2, 16, 3, 5, 7)),
+    R("split-c48", "split", "ncdhw_to_ndhwc_kernel", (1, 48, 2, 3, 11)),                  # two transpose tiles of channels
+    R("split-c32-sat", "split", "ncdhw_to_ndhwc_kernel", (2, 32, 2, 3, 9), sat=1),        # |x| >= 4094 and subnormal lo halves
 ]
 BY_ID = {r.id: r for r in REGISTRY}
+
+# Runtime modes of the kernels above.  Each mode is one row family; NONCONV_MODE_VARIANTS lists the instantiations its entry point
+# reaches, and its rows must reach exactly those (tests/test_host_logic_cpu.py).
+NONCONV_MODE_VARIANTS = {
+    "geov": {"geo_lookup_kernel<4>", "geo_lookup_kernel<0>"},           # geometry-only (IGEV-RT): corr[0] == NULL
+    "geomr": {"geo_lookup_kernel<4>", "geo_lookup_kernel<0>"},          # multi-range (IGEV++): out_corr != NULL
+    "warp": {"warped_volume_kernel<8>"},                                # disparity warp (MonSter, AANet): border = 1
+    "slice": {"ncdhw_to_ndhwc_kernel"},                                 # channel slice of a channels-last concatenation
+    "split": {"ncdhw_to_ndhwc_kernel"},                                 # split NDHWC output
+}
+# Every field of struct GeoParams (csrc/geo.cu), struct WarpParams (csrc/cascade.cu) and every parameter of ncdhw_to_ndhwc_kernel
+# (csrc/conv3d_tc.cu): "" = an operand or geometry field the plain rows exercise, otherwise the mode whose rows exercise it.  A
+# field that is in neither fails tests/test_host_logic_cpu.py.
+GEO_PARAMS_FIELDS = {
+    **{f: "" for f in "geo disp coords out B C D H W W2 levels radius".split()},
+    "corr": "geov",
+    **{f: "geomr" for f in "vol1 vol2 out1 out2 out_corr D1 D2".split()},
+}
+WARP_PARAMS_FIELDS = {
+    **{f: "" for f in "xg yg xc yc disp out B Cg G K Cc D H W Ctot oc_cat n_gwc_units n_cat_units mask_left half_w half_h".split()},
+    **{f: "warp" for f in "border wm1 hm1".split()},
+}
+LAYOUT_KERNEL_PARAMS = {
+    **{f: "" for f in "x y C Cp vol".split()},
+    "ys": "split", "overflow": "split",
+    "ystride": "slice", "coff": "slice",
+}
+
+
+def grid_z(row):
+    """Grid z of a geo_lookup_kernel launch: one CTA row per (batch item, row of the output)."""
+    if row.fam == "geov":
+        B, C, D, H, W, L = row.shape
+        return B * L * C
+    B, C, D0, D1, D2, H, W, W2, L = row.shape
+    return B * (L * C + 2 * C + L)
+
+
+def _pow2(n):
+    return n & (n - 1) == 0
+
+
+# What each mode's rows must include between them (tests/test_host_logic_cpu.py): every requirement is met by at least one row.
+MODE_REQUIREMENTS = {
+    "geov": {
+        "radius 4 over 4 levels with taps that take the fallback read": lambda r: r.opts["radius"] == 4 and r.shape[5] == 4 and r.opts.get("cross"),
+        "radius 4 at one level": lambda r: r.opts["radius"] == 4 and r.shape[5] == 1,
+        "radius 0": lambda r: r.opts["radius"] == 0,
+        "a generic radius other than 0 at B = 3 and a partial 128-column block": lambda r: r.opts["radius"] not in (0, 4) and r.shape[0] == 3
+        and r.shape[4] % 128 not in (0, r.shape[4]),
+        "grid z = 65535": lambda r: grid_z(r) == 65535,
+    },
+    "geomr": {
+        "radius 4 over 4 levels with taps that take the fallback read": lambda r: r.opts["radius"] == 4 and r.shape[8] == 4 and r.opts.get("cross"),
+        "radius 4 at one level with D1 = D2 = 2": lambda r: r.opts["radius"] == 4 and r.shape[8] == 1 and r.shape[3] == r.shape[4] == 2,
+        "radius 0": lambda r: r.opts["radius"] == 0,
+        "radius 3": lambda r: r.opts["radius"] == 3,
+        "D1 != D2, neither a power of two": lambda r: r.shape[3] != r.shape[4] and not _pow2(r.shape[3]) and not _pow2(r.shape[4]),
+        "W2 != W": lambda r: r.shape[7] != r.shape[6],
+        "grid z = 65535": lambda r: grid_z(r) == 65535,
+    },
+    "warp": {
+        "a partial unit at H = 2": lambda r: r.shape[1] % 8 and r.shape[2] == 2,
+        "three units, the last one partial": lambda r: r.shape[1] > 16 and r.shape[1] % 8,
+        "227 KB of staged rows, two per channel": lambda r: r.shape[1] >= 8 and 8 * 2 * r.shape[3] * 4 == 227 * 1024 and r.opts["two"],
+        "W = 2": lambda r: r.shape[3] == 2,
+    },
+    "slice": {
+        "odd channel count and offset, ending at the voxel's last channel": lambda r: r.shape[1] % 2 and r.shape[6] % 2
+        and r.shape[6] + r.shape[1] == r.shape[5],
+        "a slice that is the whole voxel": lambda r: r.shape[6] == 0 and r.shape[1] == r.shape[5],
+        "three channel tiles in the middle of the voxel": lambda r: r.shape[1] > 64 and 0 < r.shape[6] < r.shape[5] - r.shape[1],
+    },
+    "split": {
+        "one granule": lambda r: r.shape[1] == 16,
+        "two transpose tiles of channels": lambda r: r.shape[1] > 32,
+        "saturation and subnormal lo halves": lambda r: r.opts.get("sat"),
+    },
+}
 
 
 @pytest.fixture(scope="module")
@@ -259,10 +376,74 @@ def roundtrip_geo(x, n):
     return (g + f32(1.0)) * (f32(0.5) * f32(n - 1))
 
 
+def lerp_taps(data, n, base, r):
+    """Taps k = 0 .. 2r of grid_sample's linear interpolation (align_corners=True, zero padding) of data (B, C, n, H, W) along dim
+    2 at base + (k - r), base (B, H, W) in fp32, the coordinate round-tripped as geo.cu does -> (taps (B, C, T, H, W), sum |terms|,
+    number of taps whose floor is not the first tap's floor + k: those take the kernel's fallback read)."""
+    B, Cn, _, H, W = data.shape
+    first = torch.floor(roundtrip_geo(f32(-r) + base, n))
+    taps, mags, cross = [], [], 0
+    for k in range(2 * r + 1):
+        ix = roundtrip_geo(f32(k - r) + base, n)
+        fl = torch.floor(ix)
+        cross += int((fl != first + k).sum())
+        w1, w0 = (ix - fl).double().unsqueeze(1), ((fl + f32(1.0)) - ix).double().unsqueeze(1)
+        i0 = fl.long()
+        vals = []
+        for i in (i0, i0 + 1):
+            ok = ((i >= 0) & (i < n)).unsqueeze(1)
+            idx = i.clamp(0, n - 1).view(B, 1, 1, H, W).expand(B, Cn, 1, H, W)
+            vals.append(torch.gather(data, 2, idx).squeeze(2) * ok)
+        taps.append(vals[0] * w0 + vals[1] * w1)
+        mags.append((vals[0] * w0).abs() + (vals[1] * w1).abs())
+    return torch.stack(taps, 2), torch.stack(mags, 2), cross
+
+
+def geo_model(vols, corr, disp, coords, r):
+    """fp64 model of geo_lookup_kernel.  vols: [(volume (B, C, n, H, W), shift)], each sampled at disp / 2^shift; corr: None (no
+    correlation row) or, per vols entry i, (B, H, W, W2 >> i) sampled at coords / 2^i - disp / 2^i.  -> (want (B, len(vols),
+    C [+ 1], 2r + 1, H, W), sum |terms|, taps that take the fallback read)."""
+    wants, mags, cross = [], [], 0
+    for i, (vol, shift) in enumerate(vols):
+        sc = f32(1.0 / (1 << shift))
+        dq = disp[:, 0] * sc                                                  # (B, H, W)
+        rows = [(vol.double(), vol.shape[2], dq)]
+        if corr is not None:
+            rows.append((corr[i].double().permute(0, 3, 1, 2).unsqueeze(1), corr[i].shape[3], coords * sc - dq))
+        parts = [lerp_taps(data, n, base, r) for data, n, base in rows]
+        wants.append(torch.cat([p[0] for p in parts], 1))
+        mags.append(torch.cat([p[1] for p in parts], 1))
+        cross += sum(p[2] for p in parts)
+    return torch.stack(wants, 1), torch.stack(mags, 1), cross
+
+
 def roundtrip_cas(v, half):
     """cascade.cu cas_roundtrip: grid value v/half - 1 and aten's unnormalisation (g + 1) * half, in fp32."""
     g = v / half - f32(1.0)
     return (g + f32(1.0)) * half
+
+
+def roundtrip_border(v, size):
+    """cascade.cu border_roundtrip: the grid value 2 (v / (size - 1)) - 1 in fp32, then fmaf(g + 1, size / 2, -0.5) and the clamp to
+    [0, size - 1].  The fmaf's product is exact in fp64 and so is its sum whenever the result is >= 0 (below 0 the clamp takes over),
+    so one rounding to fp32 replays it.  -> (coordinate, (clamped below anywhere, clamped above anywhere))."""
+    g = f32(2.0) * (v / f32(size - 1)) - f32(1.0)
+    u = ((g + f32(1.0)).double() * (size / 2.0) - 0.5).float()
+    return u.clamp(0.0, size - 1.0), (bool((u < 0).any()), bool((u > size - 1).any()))
+
+
+def host_split(x):
+    """(..., C) fp32 -> (..., 2C) fp16 split channels-last: per 16-channel granule [16 hi | 16 lo] of s = 16 x, hi = fp16_rn(s),
+    lo = fp16_rn(s - hi), each saturating to +-65504."""
+    def sat(v):
+        h = v.half()
+        return torch.where(torch.isinf(h), torch.sign(v).half() * 65504.0, h)
+    s = x.contiguous().float() * 16.0
+    hi = sat(s)
+    lo = sat(s - hi.float())
+    lead, C = s.shape[:-1], s.shape[-1]
+    both = torch.stack((hi.view(*lead, C // 16, 16), lo.view(*lead, C // 16, 16)), -2)              # (..., granule, hi / lo, 16)
+    return both.reshape(*lead, 2 * C)
 
 
 class Case:
@@ -315,7 +496,7 @@ class Case:
         assert (bits[:lead] == sent).all() and (bits[lead + self.numel:] == sent).all(), "%s: a store left the output region" % what
         got = buf[lead:lead + self.numel].cpu().view(self.want.shape)
         nan = torch.isnan(got)
-        assert nan[self.skip].all(), "%s: %d elements of a gradient that was not asked for were written" % (
+        assert nan[self.skip].all(), "%s: %d elements the launch must leave unwritten were written" % (
             what, int((~nan[self.skip]).sum()))
         live = ~self.skip
         assert not nan[live].any(), "%s: %d output elements never written" % (what, int(nan[live].sum()))
@@ -565,53 +746,67 @@ def cases(osb, row, g):
         fn = lambda y, P: call("osb_softargmin_bwd", P("cost"), P("gout"), y, B, D, H, W, alpha, start, step, norm, s())  # noqa: E731
         return [Case(row.id, want, scale, fn, {"cost": cost, "gout": gout}, tol=TOL_SOFT)]
 
-    if fam == "geo":
-        B, C, D, H, W, W2, L = row.shape
+    if fam in ("geo", "geov", "geomr"):
+        if fam == "geomr":
+            B, C, D, D1, D2, H, W, W2, L = row.shape
+        elif fam == "geov":
+            B, C, D, H, W, L = row.shape
+            W2 = 0
+        else:
+            B, C, D, H, W, W2, L = row.shape
         r = o["radius"]
         T = 2 * r + 1
         geo = [per(rn(B, C, D >> i, H, W), scales(C, g), 1) for i in range(L)]
-        corr = [rn(B, H, W, W2 >> i) * 3.1 for i in range(L)]
-        disp = disp_mixture(g, (B, 1, H, W), -6.0, D + 6.0)
+        corr = [rn(B, H, W, W2 >> i) * 3.1 for i in range(L)] if W2 else None
         coords = torch.arange(W, dtype=torch.float32).view(1, 1, W).expand(B, H, W).contiguous()
-        want = torch.zeros(B, L, C + 1, T, H, W, dtype=F64)
-        mag = torch.zeros_like(want)
-        fallback = 0
-        for lvl in range(L):
-            sc = f32(1.0 / (1 << lvl))
-            dq = disp[:, 0] * sc                                              # (B, H, W)
-            for c in range(C + 1):
-                if c < C:
-                    n, base = D >> lvl, dq
-                    data = geo[lvl][:, c].double()                               # (B, n, H, W): sample along dim 1
-                else:
-                    n, base = W2 >> lvl, coords * sc - dq
-                    data = corr[lvl].double().permute(0, 3, 1, 2)               # (B, n, H, W)
-                first = torch.floor(roundtrip_geo(f32(-r) + base, n))
-                for k in range(T):
-                    ix = roundtrip_geo(f32(k - r) + base, n)
-                    fl = torch.floor(ix)
-                    if r == 4:
-                        fallback += int((fl != first + k).sum())
-                    w1, w0 = (ix - fl).double(), ((fl + f32(1.0)) - ix).double()
-                    i0 = fl.long()
-                    vals = []
-                    for i in (i0, i0 + 1):
-                        ok = (i >= 0) & (i < n)
-                        vals.append(torch.gather(data, 1, i.clamp(0, n - 1).unsqueeze(1)).squeeze(1) * ok)
-                    want[:, lvl, c, k] = vals[0] * w0 + vals[1] * w1
-                    mag[:, lvl, c, k] = (vals[0] * w0).abs() + (vals[1] * w1).abs()
-        if o.get("cross"):
-            assert fallback > 0, "%s: no tap crosses an integer in the coordinate round trip" % row.id
-        want, mag = want.view(B, L * (C + 1) * T, H, W), mag.view(B, L * (C + 1) * T, H, W)
-        inputs = {"disp": disp, "coords": coords}
-        for i in range(L):
-            inputs["geo%d" % i], inputs["corr%d" % i] = geo[i], corr[i]
+        inputs = {"geo%d" % i: geo[i] for i in range(L)}
+        gp = lambda P: [P("geo%d" % i) if i < L else None for i in range(4)]           # noqa: E731
+        cp = lambda P: [P("corr%d" % i) if i < L else None for i in range(4)]          # noqa: E731
+        if corr is not None:
+            inputs.update({"corr%d" % i: corr[i] for i in range(L)}, coords=coords)
+        if fam == "geomr":                              # half the pixels reach past vol2's far end (disp / 4 > D2 + r)
+            near, far = disp_mixture(g, (B, 1, H, W), -6.0, D + 6.0), disp_mixture(g, (B, 1, H, W), -6.0, 4 * max(D, D1, D2) + 8.0)
+            disp = torch.where(torch.rand(B, 1, H, W, generator=g) < 0.5, near, far)
+        else:
+            disp = disp_mixture(g, (B, 1, H, W), -6.0, D + 6.0)
+        inputs["disp"] = disp
+        want, mag, cross = geo_model([(geo[i], i) for i in range(L)], corr, disp, coords, r)      # (B, L, C [+ 1], T, H, W)
+        if fam == "geo":
+            want, mag = want.view(B, L * (C + 1) * T, H, W), mag.view(B, L * (C + 1) * T, H, W)
 
-        def fn(y, P):
-            gp = [P("geo%d" % i) if i < L else None for i in range(4)]
-            cp = [P("corr%d" % i) if i < L else None for i in range(4)]
-            call("osb_geo_lookup_fwd", *gp, *cp, P("disp"), P("coords"), y, B, C, D, H, W, W2, L, r, s())
-        return [Case(row.id, want, mag, fn, inputs)]
+            def fn(y, P):
+                call("osb_geo_lookup_fwd", *gp(P), *cp(P), P("disp"), P("coords"), y, B, C, D, H, W, W2, L, r, s())
+            out = [Case(row.id, want, mag, fn, inputs)]
+        elif fam == "geov":
+            want, mag = want.view(B, L * C * T, H, W), mag.view(B, L * C * T, H, W)
+
+            def fn(y, P):
+                call("osb_geo_volume_lookup_fwd", *gp(P), P("disp"), y, B, C, D, H, W, L, r, s())
+            out = [Case(row.id, want, mag, fn, inputs)]
+        else:
+            vol1, vol2 = per(rn(B, C, D1, H, W), scales(C, g), 1), per(rn(B, C, D2, H, W), scales(C, g), 1)
+            inputs.update(vol1=vol1, vol2=vol2)
+            w12, m12, cross12 = geo_model([(vol1, 1), (vol2, 2)], None, disp, None, r)             # (B, 2, C, T, H, W)
+            cross += cross12
+            q = disp / 4
+            assert bool((q - r < -1).any() and (q + r > D2).any()), "%s: vol2's taps do not leave both ends" % row.id
+            # geo_feat0 (B, L * C * T, H, W), geo_feat1 and geo_feat2 (B, C * T, H, W), init_corr (B, L * T, H, W)
+            outs = [(want[:, :, :C], mag[:, :, :C]), (w12[:, 0], m12[:, 0]), (w12[:, 1], m12[:, 1]), (want[:, :, C], mag[:, :, C])]
+            outs = [(w.reshape(B, -1, H, W), m.reshape(B, -1, H, W)) for w, m in outs]
+            sizes = [w.numel() for w, _ in outs]
+            out = []
+            for j, name in enumerate(("geo_feat0", "geo_feat1", "geo_feat2", "init_corr")):
+                def fn(y, P, j=j):
+                    """Output j at y, the other three in scratch between sentinel guards (their own cases check them)."""
+                    scratch = [torch.full((2 * GUARD + n,), SENTINEL, device="cuda") for n in sizes]
+                    ys = [y if i == j else scratch[i].data_ptr() + 4 * GUARD for i in range(4)]
+                    call("osb_geo_multirange_lookup_fwd", *gp(P), P("vol1"), P("vol2"), *cp(P), P("disp"), P("coords"), *ys,
+                         B, C, D, D1, D2, H, W, W2, L, r, s())
+                    torch.cuda.synchronize()
+                out.append(Case("%s %s" % (row.id, name), outs[j][0], outs[j][1], fn, inputs))
+        if o.get("cross"):
+            assert cross > 0, "%s: no tap crosses an integer in the coordinate round trip" % row.id
+        return out
 
     if fam == "pool":
         outer, n, inner = row.shape
@@ -773,6 +968,59 @@ def cases(osb, row, g):
         fn = lambda y, P: call("osb_regression_values_fwd", P("prob"), P("values"), y, B, D, H, W, s())     # noqa: E731
         return [Case(row.id, want, mag, fn, {"prob": prob, "values": values})]
 
+    if fam == "warp":
+        B, C, H, W = row.shape
+        img = per(rn(B, C, H, W), scales(C, g), 1)
+        disp = disp_mixture(g, (B, 1, H, W), -(W // 2) - 3.0, W + W // 2 + 3.0)
+        disp[0, 0, 0, 0], disp[-1, 0, -1, -1] = W + 2.5, -W - 1.0            # column coordinates below 0 and past W - 1
+        iy, bites_y = roundtrip_border(torch.arange(H, dtype=torch.float32), H)
+        fy = torch.floor(iy)
+        ny = iy - fy
+        assert bool((ny != 0).any()) == bool(o["two"]), "%s: row coordinates do not stage the rows the row expects" % row.id
+        ix, bites = roundtrip_border(torch.arange(W, dtype=torch.float32) - disp[:, 0], W)       # (B, H, W)
+        assert bites[0] and bites[1], "%s: the border clamp does not bite on both sides" % row.id
+        fx = torch.floor(ix)
+        wx = ix - fx
+        ex, sy = f32(1.0) - wx, (f32(1.0) - ny).view(1, H, 1)
+        nyv = ny.view(1, H, 1)
+        wts = [sy * ex, sy * wx, nyv * ex, nyv * wx]                          # nw, ne, sw, se in fp32
+        want, mag = torch.zeros(B, C, H, W, dtype=F64), torch.zeros(B, C, H, W, dtype=F64)
+        for t, (dy, dx) in enumerate(((0, 0), (0, 1), (1, 0), (1, 1))):
+            yy = (fy.long() + dy).clamp(max=H - 1)                            # row H is only reached with weight 0
+            xx = fx.long() + dx                                               # (B, H, W) in [0, W]; column W reads as zero
+            rows = img.double()[:, :, yy]                                     # (B, C, H, W)
+            v = torch.gather(rows, 3, xx.clamp(max=W - 1).unsqueeze(1).expand(B, C, H, W)) * (xx < W).unsqueeze(1)
+            term = v * wts[t].double().unsqueeze(1)
+            want += term
+            mag += term.abs()
+        fn = lambda y, P: call("osb_disp_warp_fwd", P("img"), P("disp"), y, B, C, H, W, s())          # noqa: E731
+        return [Case(row.id, want, mag, fn, {"img": img, "disp": disp})]
+
+    if fam == "slice":
+        B, C, D, H, W, ys, coff = row.shape
+        x = per(rn(B, C, D, H, W), scales(C, g), 1)
+        want = torch.zeros(B, D, H, W, ys, dtype=F64)
+        want[..., coff:coff + C] = x.permute(0, 2, 3, 4, 1).double()
+        inside = torch.zeros(ys, dtype=torch.bool)
+        inside[coff:coff + C] = True
+        fn = lambda y, P: call("osb_ncdhw_to_ndhwc_slice", P("x"), y, B, C, D, H, W, ys, coff, s())   # noqa: E731
+        return [Case(row.id, want, None, fn, {"x": x}, exact=inside, skip=~inside.expand(want.shape))]
+
+    if fam == "split":
+        B, C, D, H, W = row.shape
+        sat = o.get("sat", 0)
+        x = per(rn(B, C, D, H, W), scales(C, g, -24 if sat else -12, 8), 1).clamp(-4000.0, 4000.0)
+        if sat:                                            # 16 x 4094 = 65504 is the largest fp16; the others saturate
+            x.view(-1)[:6] = torch.tensor([4094.0, -4094.0, 4094.5, -5000.0, 1e6, -1e30])
+        want = host_split(x.permute(0, 2, 3, 4, 1)).view(torch.int32).view(torch.float32).double()   # (B, D, H, W, C) words
+
+        def fn(y, P):
+            ops.tc_overflow_count(reset=True)
+            call("osb_ncdhw_to_split", P("x"), y, B, C, D, H, W, s())
+            n = ops.tc_overflow_count(reset=True)
+            assert (n >= 1) if sat else (n == 0), "%s: overflow count %d after the conversion" % (row.id, n)
+        return [Case(row.id, want, None, fn, {"x": x}, exact=torch.ones(want.shape, dtype=torch.bool))]
+
     assert fam == "pad"
     B, C, Cp, D, H, W = row.shape
     x = rn(B, C, D, H, W)
@@ -833,7 +1081,7 @@ def profiled_kernels(osb, case, what):
     dev = case.dev()
     buf = case.guarded()
     names = []
-    for _ in range(3):
+    for _ in range(10):
         torch.cuda.synchronize()
         before = lib.launch_count()
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
@@ -852,7 +1100,8 @@ def test_routing(osb, row):
     """One call is one launch (the library's launch counter) of the row's instantiation (torch.profiler).  In a few sessions per
     thousand the profiler's activity-buffer request lands inside cudaLaunchKernel (which then takes about 1 ms) and the session
     holds the launch's API record but no device record, although the kernel ran (measured on an H100 with the parent commit's
-    library as well).  Only a session with no kernel of this library recorded is repeated, at most three times; a session
+    library as well).  Such sessions can come several in a row (an H100 run of this file once had three empty sessions in a
+    row for one row), so only a session with no kernel of this library recorded is repeated, at most ten times; a session
     that records any kernel is judged as it is."""
     names = profiled_kernels(osb, cases(osb, row, seed(row, 3))[0], row.id)
     want = re.compile(r"osb::%s\(" % re.escape(row.variant))
@@ -924,7 +1173,13 @@ def refusals(P, s):
     gb, cb, sb = "osb_gwc_volume_bwd", "osb_concat_volume_bwd", "osb_softargmin_bwd"
     geo = "osb_geo_lookup_fwd"
     lv = (P,) * 8                                                       # geo0..3, corr0..3
-    cx, cg = "osb_warped_concat_volume_fwd", "osb_warped_gwc_concat_volume_fwd"
+    gv, l4 = "osb_geo_volume_lookup_fwd", (P,) * 4
+    mr = "osb_geo_multirange_lookup_fwd"
+
+    def mrp(vol1=P, out_corr=P):
+        """geo0..3, vol1, vol2, corr0..3, disp, coords, out0, out1, out2, out_corr"""
+        return (P,) * 4 + (vol1, P) + (P,) * 4 + (P, P, P, P, P, out_corr)
+    cx, cg, dw = "osb_warped_concat_volume_fwd", "osb_warped_gwc_concat_volume_fwd", "osb_disp_warp_fwd"
     co = "osb_coex_regression_fwd"
     return [
         ("gwc_volume empty W", "osb_gwc_volume_fwd", (P, P, P, 1, 8, 4, 0, 4, 2, s)),
@@ -962,6 +1217,22 @@ def refusals(P, s):
         ("geo_lookup W2 pyramid", geo, lv + (P, P, P, 1, 2, 64, 2, 8, 7, 3, 4, s)),
         ("geo_lookup null level", geo, (P, None, P, P, P, P, P, P, P, P, P, 1, 2, 64, 2, 8, 64, 2, 4, s)),
         ("geo_lookup empty", geo, lv + (P, P, P, 1, 0, 64, 2, 8, 64, 2, 4, s)),
+        ("geo_lookup B*L*(C+1) 65536", geo, lv + (P, P, P, 256, 255, 64, 2, 8, 64, 1, 4, s)),
+        ("geo_volume_lookup 0 levels", gv, l4 + (P, P, 1, 2, 16, 2, 8, 0, 4, s)),
+        ("geo_volume_lookup 5 levels", gv, l4 + (P, P, 1, 2, 64, 2, 8, 5, 4, s)),
+        ("geo_volume_lookup radius 17", gv, l4 + (P, P, 1, 2, 64, 2, 8, 2, 17, s)),
+        ("geo_volume_lookup radius -1", gv, l4 + (P, P, 1, 2, 64, 2, 8, 2, -1, s)),
+        ("geo_volume_lookup D pyramid", gv, l4 + (P, P, 1, 2, 7, 2, 8, 3, 4, s)),
+        ("geo_volume_lookup null level", gv, (P, None, P, P, P, P, 1, 2, 64, 2, 8, 2, 4, s)),
+        ("geo_volume_lookup empty", gv, l4 + (P, P, 1, 2, 64, 0, 8, 2, 4, s)),
+        ("geo_volume_lookup B*L*C 65536", gv, l4 + (P, P, 16, 1024, 16, 2, 8, 4, 4, s)),
+        ("geo_multirange D1 1", mr, mrp() + (1, 2, 64, 1, 8, 2, 8, 64, 2, 4, s)),
+        ("geo_multirange D2 1", mr, mrp() + (1, 2, 64, 8, 1, 2, 8, 64, 2, 4, s)),
+        ("geo_multirange null vol1", mr, mrp(vol1=None) + (1, 2, 64, 8, 8, 2, 8, 64, 2, 4, s)),
+        ("geo_multirange null out_corr", mr, mrp(out_corr=None) + (1, 2, 64, 8, 8, 2, 8, 64, 2, 4, s)),
+        ("geo_multirange W2 pyramid", mr, mrp() + (1, 2, 64, 8, 8, 2, 8, 7, 3, 4, s)),
+        ("geo_multirange radius 17", mr, mrp() + (1, 2, 64, 8, 8, 2, 8, 64, 2, 17, s)),
+        ("geo_multirange grid z 65536", mr, mrp() + (256, 85, 64, 8, 8, 2, 8, 64, 1, 4, s)),       # 256 x (85 + 170 + 1)
         ("avgpool_pairs n 1", "osb_avgpool_pairs_fwd", (P, P, 4, 1, 4, s)),
         ("context_upsample scale 0", "osb_context_upsample_fwd", (P, P, P, 1, 4, 4, 0, s)),
         ("warped_concat H 1", cx, (P, P, P, P, 1, 4, 2, 1, 8, 0, s)),
@@ -972,6 +1243,11 @@ def refusals(P, s):
         ("warped_gwc Cg % G", cg, (P, P, P, P, P, P, 1, 10, 3, 4, 2, 4, 8, s)),
         ("warped_gwc W 1817", cg, (P, P, P, P, P, P, 1, 16, 1, 1, 2, 2, 1817, s)),
         ("warped_gwc Cc 0", cg, (P, P, P, P, P, P, 1, 16, 2, 0, 2, 4, 8, s)),
+        ("disp_warp H 1", dw, (P, P, P, 1, 4, 1, 16, s)),
+        ("disp_warp W 1", dw, (P, P, P, 1, 4, 2, 1, s)),
+        ("disp_warp W 3633", dw, (P, P, P, 1, 1, 2, 3633, s)),
+        ("disp_warp C 0", dw, (P, P, P, 1, 0, 2, 16, s)),
+        ("disp_warp empty B", dw, (P, P, P, 0, 4, 2, 16, s)),
         ("coex top_k 1", co, (P, P, P, 1, 8, 4, 4, 1, 1, s)),
         ("coex top_k 9", co, (P, P, P, 1, 16, 4, 4, 9, 1, s)),
         ("coex top_k 5 > D 4", co, (P, P, P, 1, 4, 4, 4, 5, 1, s)),
@@ -985,6 +1261,9 @@ def refusals(P, s):
         ("sub_volume B*H 65536", "osb_sub_volume_fwd", (P, P, P, 2, 4, 32768, 8, 4, s)),
         ("regression_values empty", "osb_regression_values_fwd", (P, P, P, 1, 0, 4, 4, s)),
         ("ncdhw_to_ndhwc_pad Cpad < C", "osb_ncdhw_to_ndhwc_pad", (P, P, 1, 8, 4, 2, 2, 2, s)),
+        ("ncdhw_to_ndhwc_slice B 65536", "osb_ncdhw_to_ndhwc_slice", (P, P, 65536, 4, 1, 2, 2, 4, 0, s)),
+        ("ncdhw_to_split C 24", "osb_ncdhw_to_split", (P, P, 1, 24, 1, 2, 2, s)),
+        ("ncdhw_to_split B 65536", "osb_ncdhw_to_split", (P, P, 65536, 16, 1, 2, 2, s)),
     ]
 
 

@@ -70,13 +70,10 @@ def test_disp_warp_against_reference(osb, case):
 
 
 def test_disp_warp_refusals_launch_nothing(osb):
+    """ops.disp_warp refuses mismatched shapes; the C entry point's refusals are in test_kernel_contract_gpu.py::test_refusals."""
     lib, ops, _, _ = osb
-    img, disp = torch.zeros(1, 4, 1, 16, device="cuda"), torch.zeros(1, 1, 1, 16, device="cuda")
-    out = torch.zeros(1, 4, 1, 16, device="cuda")
+    img = torch.zeros(1, 4, 1, 16, device="cuda")
     before = lib.launch_count()
-    for b, c, h, w in ((1, 4, 1, 16), (1, 4, 2, 1), (0, 4, 2, 16), (1, 0, 2, 16)):
-        with pytest.raises(ValueError):
-            lib.call("osb_disp_warp_fwd", img.data_ptr(), disp.data_ptr(), out.data_ptr(), b, c, h, w, None)
     with pytest.raises(ValueError, match="do not match"):
         ops.disp_warp(img, torch.zeros(1, 2, 1, 16, device="cuda"))
     assert lib.launch_count() == before
