@@ -40,6 +40,10 @@ extern "C" {
 #define OSB_ACT_RELU6 3 /* nn.ReLU6 of LightStereo's MobileV2Residual; accepted by the CUDA-core 1x1, depthwise and 2D kernels */
 #define OSB_ACT_SIGMOID 4 /* the ConvGRU gates (torch.sigmoid / torch.tanh); accepted by osb_conv2d_k3_tc_gru_fwd */
 #define OSB_ACT_TANH 5
+/* CFNet's Mish, v * tanh(softplus(v)) with F.softplus's threshold 20 (cfnet/submodule.py:249-260), applied after the residual:
+ * FMish(conv(x) + redir(y)) is one launch.  Accepted by osb_conv3d_k3_bn_act_fwd, osb_deconv3d_bn_act_fwd and
+ * osb_conv3d_1x1_bn_act_fwd only; every other entry point returns OSB_EINVAL for it. */
+#define OSB_ACT_MISH 6
 
 /* Precision of the tensor-core products (osb_conv2d_k3_tc_prec_fwd, osb_conv2d_k3_tc_gru_prec_fwd) */
 #define OSB_PREC_FP32 0 /* fp32-accurate 3xFP16 split products (the default of every other entry point) */
@@ -118,6 +122,15 @@ int osb_corr_volume_fwd(const float* left, const float* right, float* out, int B
  * alpha first; normalize=0 skips the softmax (sum_d cost*value). */
 int osb_softargmin_fwd(const float* cost, float* out, int B, int D, int H, int W, float alpha,
                        float start, float step, int normalize, osb_stream_t stream);
+
+/* Soft-argmin with the candidates' values and the variance of the distribution (CFNet, cfnet/cfnet.py:526-566,
+ * cfnet/submodule.py:121-141): p = softmax over D of cost (B,D,H,W),
+ *   disp_out[b,h,w] = mu = sum_d p_d v_d,   var_out[b,h,w] = sum_d p_d (v_d - mu)^2   (disparity_variance(_confidence))
+ * with v_d = values[b,d,h,w] (CFNet's disparity samples), or v_d = d when values is NULL.  var_out may be NULL (no variance);
+ * the variance is a second pass over the cost about the mu of the same launch.  With values and var_out NULL, disp_out is
+ * osb_softargmin_fwd(cost, disp_out, B, D, H, W, 1, 0, 1, 1) bit for bit.  disp_out / var_out: (B,H,W) = (B,1,H,W). */
+int osb_softargmin_var_fwd(const float* cost, const float* values, float* disp_out, float* var_out, int B, int D, int H, int W,
+                           osb_stream_t stream);
 
 /* F.interpolate(cost,[D,H,W],'trilinear',align_corners) -> softmax(dim=1) -> expectation, fused;
  * the upsampled (B,D,H,W) tensor is never materialised.
@@ -377,6 +390,16 @@ int osb_warped_concat_volume_fwd(const float* x, const float* y, const float* di
                                  int mask_left, osb_stream_t stream);
 int osb_warped_gwc_concat_volume_fwd(const float* xg, const float* yg, const float* xc, const float* yc, const float* disp,
                                      float* out, int B, int Cg, int G, int Cc, int D, int H, int W, osb_stream_t stream);
+/* osb_warped_gwc_concat_volume_fwd with the left masking as an argument: mask_left = 1 is that entry point bit for bit;
+ * mask_left = 0 leaves x unmasked in both the correlation and the concatenation half -- CFNet's cost_volume_generator
+ * (cfnet/cfnet.py:463-486, SpatialTransformer + groupwise_correlation_4D + cat, cfnet/submodule.py:167-173, 315-361), whose
+ * right features are gathered at integer samples with zeros outside [0, W-1].  The bilinear coordinate round trip lands within
+ * 2^-23 (W - 1) of the integer column and 2^-23 (H - 1) of the integer row (rows too: at H = 64 / 128 / 256, 15 / 21 / 63 rows
+ * come back off the integer), so each warped feature differs from that exact gather by at most 2^-23 (W - 1 + H - 1) times the
+ * largest difference between the gathered feature and one of its 3x3 neighbours (DESIGN.md section 4.22). */
+int osb_warped_gwc_concat_volume_ex_fwd(const float* xg, const float* yg, const float* xc, const float* yc, const float* disp,
+                                        float* out, int B, int Cg, int G, int Cc, int D, int H, int W, int mask_left,
+                                        osb_stream_t stream);
 /* osb_disp_warp_fwd: MonSter's disp_warp(img, disp)[0] (monster/warp.py): img (B,C,H,W), disp (B,1,H,W) -> out (B,C,H,W), img
  *   sampled at column w - disp like F.grid_sample(bilinear, padding_mode='border', align_corners=False) of MonSter's
  *   normalize_coords grid, bit for bit with the reference on the CPU.  The same kernel as the two above, one launch; H >= 2, W >= 2. */

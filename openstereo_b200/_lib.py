@@ -77,6 +77,8 @@ SIGNATURES = {
     "osb_upsample_softargmin_values_fwd": [_f32p] * 3 + [_i] * 8 + [_s],
     "osb_warped_concat_volume_fwd": [_f32p] * 4 + [_i] * 6 + [_s],
     "osb_warped_gwc_concat_volume_fwd": [_f32p] * 6 + [_i] * 7 + [_s],
+    "osb_warped_gwc_concat_volume_ex_fwd": [_f32p] * 6 + [_i] * 8 + [_s],
+    "osb_softargmin_var_fwd": [_f32p] * 4 + [_i] * 4 + [_s],
     "osb_disp_warp_fwd": [_f32p] * 3 + [_i] * 4 + [_s],
     "osb_coex_regression_fwd": [_f32p] * 3 + [_i] * 6 + [_s],
     "osb_nearest_resize3d_fwd": [_f32p] * 2 + [_i] * 7 + [_s],

@@ -6,7 +6,7 @@
 // Every stage of a cascade samples the right features at a fractional, per-pixel hypothesis disp[b,d,h,w] (arbitrary per
 // (b, d, h, w): not linear in d, possibly negative or beyond either edge) through
 //   F.grid_sample(y, grid, 'bilinear', padding_mode='zeros', align_corners=True),  grid = ((w - disp)/((W-1)/2) - 1, h/((H-1)/2) - 1)
-// and CasGwcNet zeroes the left features where w < disp.  The reference materialises meshgrid repeats, the (B,D,H,W,2) grid,
+// and CasGwcNet zeroes the left features where w < disp (mask_left; CFNet's cost_volume_generator does not, cfnet/cfnet.py:463-486).  The reference materialises meshgrid repeats, the (B,D,H,W,2) grid,
 // a warped copy of the right features, a repeated copy of the left, their product and a torch.cat; here ONE launch writes
 // the final (B, Cout, D, H, W) fp32 volume, every element exactly once (masked entries as exact zeros, so no memset).
 //
@@ -49,7 +49,7 @@ struct WarpParams {
   int B, Cg, G, K, Cc, D, H, W;
   int Ctot, oc_cat;    // output channels; first concatenation channel (= G)
   int n_gwc_units, n_cat_units;
-  int mask_left;       // zero the left copy where w < disp (CasGwcNet) or not (CasPSMNet)
+  int mask_left;       // zero the left copy where w < disp (CasGwcNet) or not (CasPSMNet, CFNet)
   int border;          // disparity-warp mode: MonSter's coordinates, border padding, warped right features only
   float half_w, half_h;  // (W - 1) / 2, (H - 1) / 2
   float wm1, hm1;        // W - 1, H - 1
@@ -169,7 +169,8 @@ __global__ void __launch_bounds__(kCasThreads) warped_volume_kernel(const WarpPa
         for (int c = 0; c < KMAX; ++c)
           if (c < nch) acc = __fadd_rn(acc, __fmul_rn(xl[c], taps[c]));
         const int g = unit;
-        __stcs(p.out + (((size_t)b * p.Ctot + g) * p.D + d) * HW + (size_t)h * p.W + w, masked ? 0.f : __fdiv_rn(acc, kf));
+        __stcs(p.out + (((size_t)b * p.Ctot + g) * p.D + d) * HW + (size_t)h * p.W + w,
+               p.mask_left && masked ? 0.f : __fdiv_rn(acc, kf));
       } else {
         const bool zero_left = p.mask_left && masked;
 #pragma unroll
@@ -250,6 +251,18 @@ int osb_warped_gwc_concat_volume_fwd(const float* xg, const float* yg, const flo
   osb::WarpParams p{};
   p.xg = xg, p.yg = yg, p.xc = xc, p.yc = yc, p.disp = disp, p.out = out;
   p.B = B, p.Cg = Cg, p.G = G, p.Cc = Cc, p.D = D, p.H = H, p.W = W, p.mask_left = 1;
+  return osb::launch_warped(p, (cudaStream_t)stream);
+}
+
+int osb_warped_gwc_concat_volume_ex_fwd(const float* xg, const float* yg, const float* xc, const float* yc, const float* disp,
+                                        float* out, int B, int Cg, int G, int Cc, int D, int H, int W, int mask_left,
+                                        osb_stream_t stream) {
+  OSB_REQUIRE(xg && yg && xc && yc && disp && out, "warped_gwc_concat_volume_ex: null pointer");
+  OSB_REQUIRE(Cg > 0, "warped_gwc_concat_volume_ex: Cg=%d", Cg);
+  OSB_REQUIRE(mask_left == 0 || mask_left == 1, "warped_gwc_concat_volume_ex: mask_left=%d (0 or 1)", mask_left);
+  osb::WarpParams p{};
+  p.xg = xg, p.yg = yg, p.xc = xc, p.yc = yc, p.disp = disp, p.out = out;
+  p.B = B, p.Cg = Cg, p.G = G, p.Cc = Cc, p.D = D, p.H = H, p.W = W, p.mask_left = mask_left;
   return osb::launch_warped(p, (cudaStream_t)stream);
 }
 

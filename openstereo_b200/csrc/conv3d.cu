@@ -60,6 +60,13 @@ __device__ __forceinline__ float activate(float v, int act) {
   return v;
 }
 
+// CFNet's Mish (cfnet/submodule.py:99-106, 249-260): v * tanh(softplus(v)), softplus as F.softplus (beta 1, threshold 20), IEEE
+// expf / log1pf / tanhf.  Out of line, like tc_common.cuh's gru_act, so the instantiations that never meet it do not grow.
+static __device__ __noinline__ float mish(float v) { return v * tanhf(v > 20.f ? v : log1pf(expf(v))); }
+
+// The activation of the ConvParams epilogue: activate(), or OSB_ACT_MISH (the _bn_act_ entry points only)
+__device__ __forceinline__ float epilogue_act(float v, int act) { return act == OSB_ACT_MISH ? mish(v) : activate(v, act); }
+
 // Normalised input: leaky((v - mean) * rstd) * gate of one staged element of channel bc = b * C + c at plane offset hw.
 __device__ __forceinline__ float normalise(const float* stats, const float* gate, float v, int bc, size_t hw, size_t plane) {
   const float2 s = __ldg(reinterpret_cast<const float2*>(stats) + bc);
@@ -197,7 +204,7 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, float (&acc)[TCO][
         v[0] += r0.x, v[1] += r0.y, v[2] += r0.z, v[3] += r0.w, v[4] += r1.x, v[5] += r1.y, v[6] += r1.z, v[7] += r1.w;
       }
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = activate(v[i], p.act);
+      for (int i = 0; i < 8; ++i) v[i] = epilogue_act(v[i], p.act);
       if (grow) {
         const float4 g0 = __ldg(reinterpret_cast<const float4*>(grow));
         const float4 g1 = __ldg(reinterpret_cast<const float4*>(grow + 4));
@@ -215,7 +222,7 @@ __device__ __forceinline__ void epilogue(const ConvParams& p, float (&acc)[TCO][
         if (ow_first + i < p.Wo) {
           float t = v[i];
           if (p.residual) t += __ldg(p.residual + row + i);
-          t = activate(t, p.act);
+          t = epilogue_act(t, p.act);
           if (grow) t *= __ldg(grow + i);
           if (p.sigmoid_out) t = 1.f / (1.f + expf(-t));
           p.y[row + i] = t;
@@ -987,7 +994,7 @@ int osb_conv3d_k3_bn_act_fwd(const float* x, const float* w_packed, const float*
   OSB_REQUIRE(x && w_packed && y, "conv3d_k3: null pointer");
   OSB_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && D > 0 && H > 0 && W > 0, "conv3d_k3: empty shape");
   OSB_REQUIRE(stride == 1 || stride == 2, "conv3d_k3: stride %d not supported (1 or 2)", stride);
-  OSB_REQUIRE(act >= 0 && act <= 2, "conv3d_k3: unknown activation %d", act);
+  OSB_REQUIRE((act >= 0 && act <= 2) || act == OSB_ACT_MISH, "conv3d_k3: unknown activation %d", act);
   ConvParams p{};
   p.x = x, p.w = w_packed, p.scale = scale, p.shift = shift, p.residual = residual, p.gate = gate, p.y = y;
   p.B = B, p.Cin = Cin, p.Cin0 = Cin, p.Cout = Cout, p.D = D, p.H = H, p.W = W;
@@ -1004,7 +1011,7 @@ int osb_deconv3d_bn_act_fwd(const float* x, const float* w_packed, const float* 
   OSB_REQUIRE(x && w_packed && y, "deconv3d: null pointer");
   OSB_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && D > 0 && H > 0 && W > 0, "deconv3d: empty shape");
   OSB_REQUIRE(kernel == 3 || kernel == 4, "deconv3d: kernel %d not supported (3 or 4)", kernel);
-  OSB_REQUIRE(act >= 0 && act <= 2, "deconv3d: unknown activation %d", act);
+  OSB_REQUIRE((act >= 0 && act <= 2) || act == OSB_ACT_MISH, "deconv3d: unknown activation %d", act);
   ConvParams p{};
   p.x = x, p.w = w_packed, p.scale = scale, p.shift = shift, p.residual = residual, p.gate = nullptr, p.y = y;
   p.B = B, p.Cin = Cin, p.Cin0 = Cin, p.Cout = Cout, p.D = D, p.H = H, p.W = W;
@@ -1022,7 +1029,7 @@ int osb_conv3d_1x1_bn_act_fwd(const float* x0, const float* x1, int Cin0, const 
   OSB_REQUIRE(x0 && w_packed && y, "conv3d_1x1: null pointer");
   OSB_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && D > 0 && H > 0 && W > 0, "conv3d_1x1: empty shape");
   OSB_REQUIRE(Cin0 > 0 && Cin0 <= Cin && (Cin0 == Cin || x1 != nullptr), "conv3d_1x1: bad channel split %d of %d", Cin0, Cin);
-  OSB_REQUIRE(act >= 0 && act <= 3, "conv3d_1x1: unknown activation %d", act);
+  OSB_REQUIRE((act >= 0 && act <= 3) || act == OSB_ACT_MISH, "conv3d_1x1: unknown activation %d", act);
   ConvParams p{};
   p.x = x0, p.x1 = x1, p.w = w_packed, p.scale = scale, p.shift = shift, p.residual = residual, p.gate = gate, p.y = y;
   p.B = B, p.Cin = Cin, p.Cin0 = Cin0, p.Cout = Cout, p.D = D, p.H = H, p.W = W;

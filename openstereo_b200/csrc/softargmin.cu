@@ -15,15 +15,63 @@
 namespace osb {
 
 // ------------------------------------------------------------------------------------------------ plain soft-argmin
+// Variance mode of softargmin_kernel for one pixel: p = softmax_d(cost), mu = sum_d p_d v_d with v_d = vals[d * HW] (or d when
+// vals is NULL), then var = sum_d p_d (v_d - mu)^2, CFNet's disparity_variance / disparity_variance_confidence
+// (cfnet/submodule.py:128-141).  Pass 1 is the plain kernel's loop (alpha 1, start 0, step 1), so with vals NULL mu is its result
+// bit for bit; pass 2 re-reads the cost and sums exp(x_d - max) (v_d - mu)^2 about that mu (no E[v^2] - mu^2 cancellation).
+// Out of line: the plain instantiation's code is unchanged.
+static __device__ __noinline__ void softargmin_var(const float* __restrict__ p, const float* __restrict__ vals, float* __restrict__ mu_out,
+                                                   float* __restrict__ var_out, int D, size_t HW) {
+  float m = -INFINITY, s = 0.f, t = 0.f;
+  for (int d0 = 0; d0 < D; d0 += 8) {
+    float x[8];
+    float cm = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      x[i] = (d0 + i < D) ? __ldg(p + (size_t)(d0 + i) * HW) : -INFINITY;
+      cm = fmaxf(cm, x[i]);
+    }
+    const float nm = fmaxf(m, cm);
+    if (nm == -INFINITY) continue;
+    const float sc = expf(m - nm);
+    s *= sc, t *= sc;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float e = expf(x[i] - nm);
+      s += e;
+      const float v = vals ? (d0 + i < D ? __ldg(vals + (size_t)(d0 + i) * HW) : 0.f) : (float)(d0 + i);
+      t = fmaf(e, v, t);
+    }
+    m = nm;
+  }
+  const float mu = t / s;
+  *mu_out = mu;
+  if (!var_out) return;
+  float s2 = 0.f, q = 0.f;
+  for (int d = 0; d < D; ++d) {
+    const float e = expf(__ldg(p + (size_t)d * HW) - m);
+    const float dv = (vals ? __ldg(vals + (size_t)d * HW) : (float)d) - mu;
+    s2 += e;
+    q = fmaf(e, dv * dv, q);
+  }
+  *var_out = q / s2;
+}
+
 // cost (B,D,H,W): one pass, online softmax in chunks of 8 bins (one rescale per chunk).  Consecutive threads own
 // consecutive pixels, so every load of a warp is one 128-byte line; 8 independent loads are in flight per thread.
+// Variance mode (values or var_out non-NULL; osb_softargmin_var_fwd, always normalised): CFNet's regression tails.
 __global__ void __launch_bounds__(256) softargmin_kernel(const float* __restrict__ cost, float* __restrict__ out, int D,
                                                          size_t HW, size_t total, float alpha, float start, float step,
-                                                         int normalize) {
+                                                         int normalize, const float* __restrict__ values,
+                                                         float* __restrict__ var_out) {
   const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (pix >= total) return;
   const size_t b = pix / HW, hw = pix - b * HW;
   const float* p = cost + b * (size_t)D * HW + hw;
+  if (values || var_out) {
+    softargmin_var(p, values ? values + b * (size_t)D * HW + hw : nullptr, out + pix, var_out ? var_out + pix : nullptr, D, HW);
+    return;
+  }
   if (!normalize) {
     float t = 0.f;
     for (int d = 0; d < D; ++d) t = fmaf(__ldg(p + (size_t)d * HW) * alpha, start + step * (float)d, t);
@@ -196,7 +244,19 @@ int osb_softargmin_fwd(const float* cost, float* out, int B, int D, int H, int W
   OSB_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0, "softargmin: empty shape B=%d D=%d H=%d W=%d", B, D, H, W);
   const size_t HW = (size_t)H * W, total = HW * B;
   const unsigned blocks = (unsigned)((total + 255) / 256);
-  osb::softargmin_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(cost, out, D, HW, total, alpha, start, step, normalize);
+  osb::softargmin_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(cost, out, D, HW, total, alpha, start, step, normalize, nullptr,
+                                                                    nullptr);
+  osb::count_launch();
+  return osb::check_launch("softargmin_kernel");
+}
+
+int osb_softargmin_var_fwd(const float* cost, const float* values, float* disp_out, float* var_out, int B, int D, int H, int W,
+                           osb_stream_t stream) {
+  OSB_REQUIRE(cost && disp_out, "softargmin_var: null pointer");
+  OSB_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0, "softargmin_var: empty shape B=%d D=%d H=%d W=%d", B, D, H, W);
+  const size_t HW = (size_t)H * W, total = HW * B;
+  const unsigned blocks = (unsigned)((total + 255) / 256);
+  osb::softargmin_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(cost, disp_out, D, HW, total, 1.f, 0.f, 1.f, 1, values, var_out);
   osb::count_launch();
   return osb::check_launch("softargmin_kernel");
 }

@@ -14,6 +14,7 @@ import torch
 from . import _lib
 
 ACT_NONE, ACT_RELU, ACT_LEAKY, ACT_RELU6 = 0, 1, 2, 3
+ACT_MISH = 6        # CFNet's Mish: conv3d_k3, deconv3d and conv3d_1x1 only (OSB_ACT_MISH)
 TC_WIDTH = 128      # image width (at 1/4 resolution) handled by the tensor-core conv kernel
 TC_KC = 32          # input channels per K chunk of the tensor-core conv (128-byte K-major rows)
 
@@ -262,10 +263,13 @@ def warped_concat_volume(x, y, disp_samples, mask_left=False):
     return out.to(dt)
 
 
-def warped_gwc_concat_volume(x_gwc, y_gwc, x_cat, y_cat, disp_samples, num_groups):
+def warped_gwc_concat_volume(x_gwc, y_gwc, x_cat, y_cat, disp_samples, num_groups, mask_left=True):
     """CasGwcNet's GetCostVolume.forward (casnet/cas_gwc.py:263-329) -> (B, G + 2*Cc, D, H, W): the group-wise correlation of
     the masked left and warped right gwc features, then [masked left | warped right] concatenation features, in one launch.
-    No backward."""
+    mask_left=False leaves the left features unmasked in both halves: CFNet's cost_volume_generator (cfnet/cfnet.py:463-486)
+    at its integer disparity samples, whose gather the bilinear sampling reproduces to 2^-23 (W - 1 + H - 1) of the largest
+    difference to a 3x3-neighbouring feature: the round trip leaves the integer column and, at some heights, the integer row
+    (DESIGN.md section 4.22).  No backward."""
     _no_autograd("warped_gwc_concat_volume", x_gwc, y_gwc, x_cat, y_cat, disp_samples)
     xg, dt = _prep(x_gwc, "x_gwc")
     yg, _ = _prep(y_gwc, "y_gwc")
@@ -280,9 +284,12 @@ def warped_gwc_concat_volume(x_gwc, y_gwc, x_cat, y_cat, disp_samples, num_group
     _same_device(xg, yg, xc, yc, ds)
     d = ds.shape[1]
     out = torch.empty((b, num_groups + 2 * cc, d, h, w), dtype=torch.float32, device=xg.device)
-    if out.numel():
+    if out.numel() and mask_left:
         _call("osb_warped_gwc_concat_volume_fwd", xg.data_ptr(), yg.data_ptr(), xc.data_ptr(), yc.data_ptr(), ds.data_ptr(),
               out.data_ptr(), b, cg, num_groups, cc, d, h, w, _stream(out))
+    elif out.numel():
+        _call("osb_warped_gwc_concat_volume_ex_fwd", xg.data_ptr(), yg.data_ptr(), xc.data_ptr(), yc.data_ptr(), ds.data_ptr(),
+              out.data_ptr(), b, cg, num_groups, cc, d, h, w, 0, _stream(out))
     return out.to(dt)
 
 
@@ -322,6 +329,27 @@ def softargmin(cost, maxdisp, keepdim=True, alpha=1.0, start=0.0, step=1.0, norm
                   float(step), 1 if normalize else 0, _stream(out))
     out = out.to(dt)
     return out.unsqueeze(1) if keepdim else out
+
+
+def softargmin_var(cost, values=None, variance=True):
+    """CFNet's regression tails (cfnet/cfnet.py:526-566) in one launch: p = F.softmax(cost, 1) over D, the expectation
+    sum_d p_d v_d and, with variance=True, sum_d p_d (v_d - mean)^2 (disparity_variance / disparity_variance_confidence,
+    cfnet/submodule.py:128-141), v_d = values[:, d] or d when values is None.  cost, values: (B, D, H, W) ->
+    (mean (B, 1, H, W), variance (B, 1, H, W) or None) in cost's dtype.  No backward."""
+    _no_autograd("softargmin_var", cost, values)
+    c, dt = _prep(cost, "cost")
+    assert c.dim() == 4
+    v = None
+    if values is not None:
+        v, _ = _prep(values, "values")
+        assert v.shape == c.shape
+        _same_device(c, v)
+    b, d, h, w = c.shape
+    mean = torch.empty((b, 1, h, w), dtype=torch.float32, device=c.device)
+    var = torch.empty_like(mean) if variance else None
+    if mean.numel():
+        _call("osb_softargmin_var_fwd", c.data_ptr(), _ptr(v), mean.data_ptr(), _ptr(var), b, d, h, w, _stream(mean))
+    return mean.to(dt), None if var is None else var.to(dt)
 
 
 def disparity_regression(x, maxdisp, keepdim=True):

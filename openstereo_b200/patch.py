@@ -1,5 +1,5 @@
 """patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / IGEV-RT /
-IGEV++ / MonSter / CoEx / MSNet3D, CasStereo's CasPSMNet / CasGwcNet, and AANet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
+IGEV++ / MonSter / CoEx / MSNet3D, CasStereo's CasPSMNet / CasGwcNet, AANet and CFNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
 hot path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each needs its own
@@ -28,6 +28,8 @@ rebinding.  What each model rebinds:
               (aanet/submodule.py:748, 801-824)
 * MSNet3D     one monolithic ``forward`` (MSNet3D.py:110-161), no processor modules: ``model.forward``, which keeps the
               reference's ``feature_extraction``
+* CFNet       the same: ``model.forward`` (cfnet.py:488-668), which keeps ``feature_extraction`` and the reference's search-range
+              and sampling code between the stages
 
 "The update block" is the per-instance ``forward`` of its ``gru04 / gru08 / gru16`` (gru.py) and ``encoder / disp_head /
 mask_feat_4`` (update.py).  A module override is a per-instance ``forward`` attribute.  A reference global is rebound by giving the
@@ -536,10 +538,28 @@ def _patch_msnet3d(model, strict, backbone=True):
     return model
 
 
+def _patch_cfnet(model, strict, backbone=True):
+    """CFNet (cfnet/cfnet.py, class cfnet, built by the CFNet(d) factory): everything after the 2D features in the eval forward
+    (``model.forward``, per instance) -- the three stage-1 volumes, the warped volumes of the s3 / s2 refinements, every 3D
+    convolution with its Mish epilogue and the three soft-argmin tails with their variances (cfnet.CFNetEngine).  The Mish feature
+    extractor and the model's generate_search_range / generate_disparity_samples stay the reference's code; the bounds and
+    their up-sampling, inline in the reference's forward, are restated term for term; `backbone` has no effect.  A model built with replace_mish=True is refused here, naming the module."""
+    from .cfnet import CFNetEngine
+    engine = CFNetEngine(model)
+
+    def forward(data):
+        left, right = data["left"], data["right"]
+        fl, fr = model.feature_extraction(left), model.feature_extraction(right)
+        return {"disp_pred": engine(fl, fr, left.shape[2], left.shape[3]).to(left.dtype)}
+
+    _override(model, "CFNet", strict, forward, serves=engine.serves, operands=lambda data: (data["left"], data["right"]))
+    return model
+
+
 # Models routed by (package, module, class) of their defining module: CasStereo's classes are also named PSMNet / GwcNet, and
-# AANet's class is the bare lowercase `aanet`
+# AANet's and CFNet's classes are the bare lowercase `aanet` / `cfnet`
 _MODULE_PATCHERS = {("casnet", "cas_psm", "PSMNet"): _patch_cascade, ("casnet", "cas_gwc", "GwcNet"): _patch_cascade,
-                    ("aanet", "aanet", "aanet"): _patch_aanet}
+                    ("aanet", "aanet", "aanet"): _patch_aanet, ("cfnet", "cfnet", "cfnet"): _patch_cfnet}
 
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
              "IGEVStereo": _patch_igev, "IGEVRTtereo": _patch_igev_rt,
@@ -552,9 +572,9 @@ def patch(model, strict=True, backbone=True, aggregation=False, amp=False):
     """Rebind the hot path of a reference model instance in place and return it.  backbone=True (default) also routes the
     GwcNet / PSMNet 2D extractor's residual blocks to the wgmma conv kernels in CUDA inference calls (_patch_backbone);
     backbone=False leaves the extractor entirely to the reference's cuDNN code.  For the CasStereo models (casnet.cas_psm.PSMNet,
-    casnet.cas_gwc.GwcNet) and AANet (aanet.aanet.aanet) `backbone` has no effect: their FPN extractor always runs the reference's code.  aggregation=True
-    (IGEV++ only) also runs the three instance-normalised hourglasses on the library; off by default.  amp=True (IGEVStereo,
-    StereoBase, IGEVPPStereo, MonSter) runs the update blocks' tensor-core convolutions at autocast accuracy -- one fp16 MMA per
+    casnet.cas_gwc.GwcNet), AANet (aanet.aanet.aanet) and CFNet (cfnet.cfnet.cfnet) `backbone` has no effect: their 2D extractor
+    always runs the reference's code.  aggregation=True (IGEV++ only) also runs the three instance-normalised hourglasses on the
+    library; off by default.  amp=True (IGEVStereo, StereoBase, IGEVPPStereo, MonSter) runs the update blocks' tensor-core convolutions at autocast accuracy -- one fp16 MMA per
     product -- inside torch.autocast("cuda"), for users of the AMP YAMLs; outside autocast it changes nothing.  Off by default:
     every patched layer is then fp32-accurate under autocast too."""
     if not isinstance(model, torch.nn.Module):
@@ -567,7 +587,7 @@ def patch(model, strict=True, backbone=True, aggregation=False, amp=False):
         patcher = _PATCHERS[name]
     else:
         raise NotImplementedError("patch(): no hot-path drop-in for %s (supported: %s, CasStereo's casnet.cas_psm.PSMNet / "
-                                  "casnet.cas_gwc.GwcNet and aanet.aanet.aanet)" % (name, sorted(_PATCHERS)))
+                                  "casnet.cas_gwc.GwcNet, aanet.aanet.aanet and cfnet.cfnet.cfnet)" % (name, sorted(_PATCHERS)))
     if aggregation:
         if patcher is not _patch_igevpp:
             raise NotImplementedError("patch(%s, aggregation=True): only IGEVPPStereo has an aggregation option" % name)

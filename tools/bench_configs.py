@@ -48,6 +48,10 @@
       bottlenecks on the gather mode / unpatched in alternating rotation, ms per forward (median and range over the rounds) and in
       the deformable convolutions (CUDA events around every call), and the EPE against the unpatched model
       (python tools/bench_configs.py --only c16 > results/h100_c16_aanet.jsonl)
+  c17 CFNet (the reference's class, cfgs/cfnet/cfnet_sceneflow_part2.yaml), fp32, B=4 @512x960 (the YAML's batch and eval crop) and
+      B=8 @256x512: patch() / unpatched (cuDNN fp32, TF32 off) in alternating rounds, ms per forward and per stage (CUDA events:
+      feature extractor, volumes, stage 1, s3, s2), and the EPE against the unpatched model
+      (python tools/bench_configs.py --only c17 > results/h100_c17_cfnet.jsonl)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -1014,6 +1018,110 @@ def c16(iters, B=2, h=576, w=960, rounds=5):
     torch.cuda.empty_cache()
 
 
+def _hook_times(run, hooks):
+    """One run of `run` with CUDA events around every call of each hooked callable: hooks = [(tags, owner, attribute)], tags a
+    list naming the calls in order (the last tag names any further call).  -> {tag: ms summed over its calls}."""
+    events, restore = [], []
+    for tags, owner, attr in hooks:
+        inner = getattr(owner, attr)
+        count = [0]
+
+        def fwd(*args, _inner=inner, _tags=tags, _count=count, **kw):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            out = _inner(*args, **kw)
+            b.record()
+            events.append((_tags[min(_count[0], len(_tags) - 1)], a, b))
+            _count[0] += 1
+            return out
+        had = attr in vars(owner)
+        setattr(owner, attr, fwd)
+        restore.append(lambda owner=owner, attr=attr, inner=inner, had=had: setattr(owner, attr, inner) if had else delattr(owner, attr))
+    try:
+        run()
+        torch.cuda.synchronize()
+    finally:
+        for r in reversed(restore):
+            r()
+    out = {}
+    for tag, a, b in events:
+        out[tag] = round(out.get(tag, 0.0) + a.elapsed_time(b), 3)
+    return out
+
+
+def c17(iters, rounds=3):
+    """CFNet (cfnet/cfnet.py, the reference's class built by CFNet(cfg.MODEL) from the unchanged cfnet_sceneflow_part2.yaml), fp32,
+    TF32 off, seeded weights with the regression heads sharpened (oracle/cfnet.py), random images.  At B=4 @512x960 and B=8
+    @256x512: patch(m) and the unpatched model in alternating rounds (`rounds` x `iters` timed forwards after 2 warm-ups), ms per
+    forward (median, min, max over the rounds); then one forward of each with CUDA events per stage:
+      patched    features = feature_extraction (both images), volumes = the three stage-1 ops.gwc_concat_volume launches + the two
+                 warped volumes, stage1 = CFNetEngine.stage1 (aggregation + tail), s3 / s2 = CFNetEngine.refine (warped volume, the
+                 samples channel's torch.cat, aggregation, tail);
+      unpatched  features, volumes = build_gwc_volume / build_concat_volume calls + cost_volume_generator (the stage-1 torch.cat
+                 is not in it), stage1 / s3 / s2 = the 3D modules of each stage (dres*, combine1, dres3, classif2 / confidence*_s3 /
+                 confidence*_s2; the softmax and regression tails are not in them);
+    and the EPE of the patched disparity against the unpatched one."""
+    from oracle import cfnet as ocf
+    from openstereo_b200.cfnet import CFNetEngine
+    from openstereo_b200.patch import patch
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    mod = ocf.reference_module()
+    stage_mods = {"stage1": ["dres0", "dres1", "dres0_5", "dres1_5", "dres0_6", "dres1_6", "combine1", "dres3", "classif2"],
+                  "s3": ["confidence0_s3", "confidence1_s3", "confidence2_s3", "confidence3_s3", "confidence_classif1_s3"],
+                  "s2": ["confidence0_s2", "confidence1_s2", "confidence2_s2", "confidence3_s2", "confidence_classif1_s2"]}
+    for B, h, w in ((4, 512, 960), (8, 256, 512)):
+        variants = {"patched": patch(ocf.reference_model().to(DEV)), "reference": ocf.reference_model().to(DEV)}
+        gen = torch.Generator().manual_seed(17)
+        x = {"left": rnd(gen, B, 3, h, w), "right": rnd(gen, B, 3, h, w)}
+        ms = {k: [] for k in variants}
+        outs = {}
+        with torch.no_grad():
+            for _ in range(rounds):
+                for k, m in variants.items():
+                    t, outs[k] = timeit(lambda: m(dict(x))["disp_pred"], iters, warm=2)
+                    ms[k].append(t)
+            pm, rm = variants["patched"], variants["reference"]
+            stages = {"patched": _hook_times(lambda: pm(dict(x)), [
+                (["features"], pm.feature_extraction, "forward"), (["volumes"], ops, "gwc_concat_volume"),
+                (["volumes"], ops, "warped_gwc_concat_volume"), (["stage1"], CFNetEngine, "stage1"),
+                (["s3", "s2"], CFNetEngine, "refine")])}
+            hooks = [(["features"], rm.feature_extraction, "forward"), (["volumes"], rm, "cost_volume_generator")]
+            g = type(rm).forward.__globals__                                # the reference module's namespace
+            saved = {n: g[n] for n in ("build_gwc_volume", "build_concat_volume")}
+            events = []
+
+            def timed(fn):
+                def call(*a, **kw):
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    out = fn(*a, **kw)
+                    e1.record()
+                    events.append((e0, e1))
+                    return out
+                return call
+            g.update({n: timed(f) for n, f in saved.items()})
+            try:
+                for tag, names in stage_mods.items():
+                    hooks += [([tag], getattr(rm, n), "forward") for n in names]
+                st = _hook_times(lambda: rm(dict(x)), hooks)
+            finally:
+                g.update(saved)
+            st["volumes"] = round(st.get("volumes", 0.0) + sum(a.elapsed_time(b) for a, b in events), 3)
+            stages["reference"] = st
+        med = lambda v: sorted(v)[len(v) // 2]                               # noqa: E731
+        ref = outs["reference"]
+        emit(config="c17 CFNet, B=%d @%dx%d, %d rounds x %d forwards (reference class + patch(); unpatched: cuDNN fp32, TF32 off)"
+             % (B, h, w, rounds, iters),
+             gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+             forward_ms={k: {"median": round(med(v), 2), "min": round(min(v), 2), "max": round(max(v), 2)} for k, v in ms.items()},
+             stage_ms=stages,
+             epe_vs_reference_px=float("%.3e" % (outs["patched"] - ref).abs().mean().item()),
+             disparity_std_px=round(ref.std().item(), 2))
+        del variants, outs
+        torch.cuda.empty_cache()
+
+
 def _timed_call(events, fn, *args, **kw):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
@@ -1080,7 +1188,7 @@ if __name__ == "__main__":
     for name in a.only.split(","):
         try:
             {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11,
-             "c12": c12, "c13": c13, "c14": c14, "c15": c15, "c16": c16}[name](a.iters)
+             "c12": c12, "c13": c13, "c14": c14, "c15": c15, "c16": c16, "c17": c17}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:
