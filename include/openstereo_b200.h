@@ -112,6 +112,16 @@ int osb_gwc_concat_volume_fwd(const float* ref_gwc, const float* tgt_gwc, const 
 int osb_corr_volume_fwd(const float* left, const float* right, float* out, int B, int C, int H,
                         int W, int D, osb_stream_t stream);
 
+/* MSNet2D's per-disparity inputs (msnet/MSNet2D.py:145-159: interweave_tensors(featL[..., d:], featR[..., :-d])), cropped and
+ * channels-last, written by the concat path of the volume kernel: for d = 0 .. D-1 the image
+ *     out_d[b, h, w - d, 8j + k]     = left[b, 4j + k, h, w]
+ *     out_d[b, h, w - d, 8j + 4 + k] = right[b, 4j + k, h, w - d]        (w = d .. W-1, j < C/4, k < 4)
+ * of shape (B, H, W - d, 2C), the D images back to back (image d starts at B*H*2C*(d*W - d*(d-1)/2) floats).  Block j holds the
+ * four left and four right channels that the reference's interleave puts at depths 8j .. 8j+7, left first.  C % 4 == 0,
+ * 1 <= D <= W, out 16-byte aligned.  The columns w < d are not stored anywhere: each image is exactly the reference's crop. */
+int osb_interlaced_crops_fwd(const float* left, const float* right, float* out, int B, int C, int H, int W, int D,
+                             osb_stream_t stream);
+
 /* ------------------------------------------------------------------------ soft-argmin tails --- */
 
 /* softmax over D fused with the expectation (one pass over the cost):

@@ -20,6 +20,7 @@ SIGNATURES = {
     "osb_concat_volume_fwd": [_f32p, _f32p, _f32p, _i, _i, _i, _i, _i, _i, _s],
     "osb_gwc_concat_volume_fwd": [_f32p, _f32p, _f32p, _f32p, _f32p, _i, _i, _i, _i, _i, _i, _i, _s],
     "osb_corr_volume_fwd": [_f32p, _f32p, _f32p, _i, _i, _i, _i, _i, _s],
+    "osb_interlaced_crops_fwd": [_f32p, _f32p, _f32p, _i, _i, _i, _i, _i, _s],
     "osb_softargmin_fwd": [_f32p, _f32p, _i, _i, _i, _i, _f, _f, _f, _i, _s],
     "osb_upsample_softargmin_fwd": [_f32p, _f32p, _i, _i, _i, _i, _i, _i, _i, _i, _s],
     "osb_epe_partial_fwd": [_f32p, _f32p, _f32p, _i, _i, _f, _s],

@@ -16,6 +16,8 @@ Graphs restated (file:line of the reference forward each engine replaces):
   LightStereoAggregation lightstereo/aggregation.py:42-60 (Aggregation.forward), :94-101 (MobileV2Residual), :119-134 (AttentionModule)
   CoExAggregation       coex/coex_cost_processor.py:196-237 (Aggregation.forward), :68-80 (channelAtt)
   MSNet3DAggregation    msnet/MSNet3D.py:118-161 (eval forward after the volume), :10-46 (hourglass3D), submodule.py:136-173
+  MSNet2DVolume         msnet/MSNet2D.py:143-162 (the 48-disparity volume loop)
+  MSNet2DAggregation    msnet/MSNet2D.py:164-212 (eval forward after the volume), :10-45 (hourglass2D), submodule.py:94-133
   IGEVPPAggregation     igevpp/igevpp_stereo.py:69-94 (hourglass.forward), submodule.py:8-34 (BasicConv), :162-175 (FeatureAtt)
 """
 import torch
@@ -998,6 +1000,209 @@ class LightStereoAggregation(_Engine):
         up = ops.deconv2d_k3s2(quarter, w5, s5, b5, residual=self.redir2(half), act=ACT_RELU)
         w6, s6, b6 = self.up[1]
         return [ops.deconv2d_k3s2(up, w6, s6, b6, residual=self.redir1(x), act=ACT_RELU)]
+
+
+# ------------------------------------------------------------------------------------------------------ MSNet2D
+def msnet2d_volume_weights(conv3d):
+    """The reference's depth-strided Conv3d chain (msnet/MSNet2D.py:73-81: k(8,3,3) s8, k(4,3,3) s4, k(2,3,3) s2, each + BN +
+    ReLU) as three dense 3x3 Conv2d weights over the channel orders the library uses:
+      layer-1 input   8j + t      the crop block j of ops.interlaced_crops: t < 4 left channel 4j+t (reference depth 8j + 2t),
+                                  t >= 4 right channel 4j+t-4 (depth 8j + 2(t-4) + 1)
+      layer-1 output  16j + c     channel c of reference depth j (eight blocks of the shared 8 -> 16 weight: block diagonal)
+      layer-2 output  32e + c     channel c of depth e; input block 16(4e + k) + c' is channel c' of depth 4e + k
+      layer-3 output  c           input 32k + c' is channel c' of depth k
+    -> [(weight (Cout, Cin, 3, 3), scale, shift)] with the BN folded and the conv bias in the shift, fp32, on conv3d's device."""
+    c1, b1, _, c2, b2, _, c3, b3, _ = conv3d
+    w1, w2, w3 = (c.weight.detach().float() for c in (c1, c2, c3))
+    n1, n2, n3 = w1.shape[0], w2.shape[0], w3.shape[0]
+    depth = [2 * (t % 4) + t // 4 for t in range(8)]
+    d1 = w1.new_zeros(8 * n1, 64, 3, 3)
+    for j in range(8):
+        d1[n1 * j:n1 * (j + 1), 8 * j:8 * (j + 1)] = w1[:, 0, depth]
+    d2 = w2.new_zeros(2 * n2, 8 * n1, 3, 3)
+    for e in range(2):
+        d2[n2 * e:n2 * (e + 1), 4 * n1 * e:4 * n1 * (e + 1)] = w2.permute(0, 2, 1, 3, 4).reshape(n2, 4 * n1, 3, 3)
+    d3 = w3.permute(0, 2, 1, 3, 4).reshape(n3, 2 * n2, 3, 3).contiguous()
+    out = []
+    for wd, conv, bn, rep in ((d1, c1, b1, 8), (d2, c2, b2, 2), (d3, c3, b3, 1)):
+        if bn.training:
+            raise RuntimeError("BatchNorm folding is only valid in eval mode (call model.eval())")
+        scale, shift = ops.fold_bn(bn)
+        if conv.bias is not None:
+            shift = shift + conv.bias.detach().float() * scale
+        out.append((wd.contiguous(), scale.repeat(rep).contiguous(), shift.repeat(rep).contiguous()))
+    return out
+
+
+def _msnet2d_check(model):
+    """Refuse an MSNet2D whose volume network is not the one msnet2d_volume_weights restates, naming the module."""
+    want = [((8, 3, 3), (8, 1, 1), 1, 16), ((4, 3, 3), (4, 1, 1), 16, 32), ((2, 3, 3), (2, 1, 1), 32, 16)]
+    convs = [model.conv3d[i] for i in (0, 3, 6)] if len(model.conv3d) == 9 else []
+    ok = len(convs) == 3 and all(
+        isinstance(c, torch.nn.Conv3d) and (tuple(c.kernel_size), tuple(c.stride), c.in_channels, c.out_channels) == w
+        and tuple(c.padding) == (0, 1, 1) and tuple(c.dilation) == (1, 1, 1) and c.groups == 1 for c, w in zip(convs, want))
+    ok = ok and all(isinstance(model.conv3d[i], torch.nn.BatchNorm3d) for i in (1, 4, 7))
+    ok = ok and all(isinstance(model.conv3d[i], torch.nn.ReLU) for i in (2, 5, 8))
+    ok = ok and model.num_groups == 1 and model.volume_size == 48
+    if not ok:
+        raise NotImplementedError("openstereo_b200: MSNet2D.conv3d / num_groups / volume_size differ from the reference's "
+                                  "(msnet/MSNet2D.py:55-81); no kernel plan for them")
+
+
+class MSNet2DVolume(_Engine):
+    """MSNet2D's volume loop (msnet/MSNet2D.py:143-162): featL, featR (B, 32, H, W) after preconv11 -> volume (B, 48, H, W).
+    One osb_interlaced_crops_fwd launch writes the 48 cropped, interleaved inputs; per disparity d the three depth-strided Conv3ds
+    run as dense 3x3 Conv2ds on the crop of width W - d (so their zero padding sits at its edges, as in the reference) and
+    volume11 as a 1x1 conv, BN and ReLU folded into each epilogue.  A crop at least OSB_TC_MIN_WIDTH wide runs its 3x3 layers on
+    the general-width wgmma kernels (3xFP16, fp32-accurate), a narrower one on the fp32 CUDA-core kernels.  Each volume11 result
+    is copied into volume[:, d, :, d:] of a zeroed volume, so the columns w < d stay exactly 0."""
+
+    def __init__(self, module):
+        super().__init__(module)
+        _msnet2d_check(module)
+
+    def _pack(self):
+        m = self.module
+        self.layers = msnet2d_volume_weights(m.conv3d)
+        w3, s3, b3 = self.layers[2]
+        self.cout3 = _pad32(w3.shape[0])                        # the 16-channel layer runs zero-padded to 32 channels
+        pad = lambda v: torch.cat((v, v.new_zeros(self.cout3 - v.numel())))     # noqa: E731
+        self.cc = [ops.pack_conv_weight(self._at_kd1(w)) for w, _, _ in self.layers[:2]]
+        self.cc.append(ops.pack_conv_weight(self._at_kd1(_zero_padded(w3, self.cout3, w3.shape[1]))))
+        self.cc_affine = [(s, b) for _, s, b in self.layers[:2]] + [(pad(s3), pad(b3))]
+        conv, bn = m.volume11[0][0], m.volume11[0][1]
+        self.v11 = conv.weight.detach().float().reshape(1, -1).t()
+        self.v11 = torch.cat((self.v11, self.v11.new_zeros(self.cout3 - self.v11.shape[0], 1))).contiguous()
+        self.v11_scale, self.v11_shift = ops.fold_bn(bn)
+        self._tc = {}
+
+    @staticmethod
+    def _at_kd1(w):
+        w5 = w.new_zeros(w.shape[0], w.shape[1], 3, 3, 3)
+        w5[:, :, 1] = w
+        return w5
+
+    def _tc_weight(self, i, width):
+        w, _, _ = self.layers[i]
+        kc = ops.conv2d_tc_kc(w.shape[1], self.cout3 if i == 2 else w.shape[0], width)
+        if not kc:
+            return None
+        if (i, kc) not in self._tc:
+            self._tc[(i, kc)] = ops.pack_tc_weight_2d(w, kc, pad_cout_to=self.cout3 if i == 2 else None)
+        return self._tc[(i, kc)]
+
+    def tc_width(self, width):
+        """True when every 3x3 layer of a crop this wide runs on the tensor cores."""
+        return USE_TENSOR_CORES and all(self._tc_weight(i, width) is not None for i in range(3))
+
+    def front(self, x, width):
+        """One crop (B, H, width, 64) channels-last -> the layer-3 output (B, cout3, H, width), channels 16.. zero."""
+        if self.tc_width(width):
+            for i, (_, s, b) in enumerate(self.layers):
+                x = ops.conv2d_k3_tc(x, self._tc_weight(i, width), s, b, act=ACT_RELU, out_nhwc=i < 2)
+            return x
+        x = x.permute(0, 3, 1, 2).unsqueeze(2).contiguous()
+        for w, (s, b) in zip(self.cc, self.cc_affine):
+            x = ops.conv3d_k3(x, w, s, b, act=ACT_RELU)
+        return x.squeeze(2)
+
+    def __call__(self, feat_left, feat_right):
+        fl, fr = self._check(feat_left), self._check(feat_right)
+        self._ensure(fl.device)
+        mon = self._watch(fl.device)
+        b, _, h, w = fl.shape
+        volume = torch.zeros((b, self.module.volume_size, h, w), dtype=torch.float32, device=fl.device)
+        for d, x in enumerate(ops.interlaced_crops(fl, fr, min(self.module.volume_size, w))):
+            y = ops.conv3d_1x1(self.front(x, w - d), self.v11, self.v11_scale, self.v11_shift, act=ACT_RELU)
+            volume[:, d, :, d:].copy_(y[:, 0])
+        if mon is not None:
+            mon.poll()
+        return volume
+
+
+class _MBV2Block2D:
+    """MobileV2_Residual (msnet/submodule.py:94-133): 1x1 + BN + ReLU6 -> depthwise 3x3 (stride 1/2) + BN + ReLU6 -> 1x1 + BN
+    (+ identity when use_res_connect); `act` is applied after the identity, in the projection's epilogue."""
+
+    def __init__(self, m, name):
+        layers = list(m.conv)
+        if len(layers) != 8 or not all(isinstance(layers[i], torch.nn.Conv2d) for i in (0, 3, 6)) or layers[0].kernel_size != (1, 1):
+            raise NotImplementedError("openstereo_b200: %s is not an expanding MobileV2_Residual (1x1, depthwise 3x3, 1x1)" % name)
+        pw, dw, pl = layers[0], layers[3], layers[6]
+        if dw.groups != dw.in_channels or dw.kernel_size != (3, 3) or dw.dilation != (1, 1) or pl.kernel_size != (1, 1):
+            raise NotImplementedError("openstereo_b200: %s has a dilated or non-depthwise 3x3; only dilation 1 has a kernel" % name)
+        self.pw, self.dw, self.pl = _PW(pw, layers[1]), _DW(dw, layers[4]), _PW(pl, layers[7])
+        self.res = bool(m.use_res_connect)
+
+    def __call__(self, x, act=ACT_NONE):
+        h = ops.conv3d_1x1(x, self.pw.w, self.pw.scale, self.pw.shift, act=ACT_RELU6)
+        h = ops.dwconv2d(h, self.dw.w, self.dw.scale, self.dw.shift, stride=self.dw.stride, act=ACT_RELU6)
+        return ops.conv3d_1x1(h, self.pl.w, self.pl.scale, self.pl.shift, residual=x if self.res else None, act=act)
+
+
+class _Hourglass2D:
+    """hourglass2D (msnet/MSNet2D.py:10-45): relu(conv5(conv4) + redir2(conv2)), relu(conv6(conv5) + redir1(x)) in the
+    transposed convs' epilogues."""
+
+    def __init__(self, m, name):
+        blk = lambda attr: _MBV2Block2D(getattr(m, attr), "%s.%s" % (name, attr))          # noqa: E731
+        self.conv1, self.conv2, self.conv3, self.conv4 = blk("conv1"), blk("conv2"), blk("conv3"), blk("conv4")
+        self.redir1, self.redir2 = blk("redir1"), blk("redir2")
+        self.up = []
+        for attr in ("conv5", "conv6"):
+            up = getattr(m, attr)[0]
+            if (up.kernel_size, up.stride, up.padding, up.output_padding, up.dilation, up.groups) != ((3, 3), (2, 2), (1, 1), (1, 1),
+                                                                                                      (1, 1), 1) or up.bias is not None:
+                raise NotImplementedError("openstereo_b200: %s.%s is not ConvTranspose2d(k3, s2, p1, op1, bias=False)" % (name, attr))
+            seq = getattr(m, attr)
+            sc, sh = ops.fold_bn(seq[1])
+            self.up.append((ops.pack_deconv2d_weight(seq[0].weight), sc, sh))
+
+    def __call__(self, x):
+        c2 = self.conv2(self.conv1(x))
+        c4 = self.conv4(self.conv3(c2))
+        (w5, s5, b5), (w6, s6, b6) = self.up
+        c5 = ops.deconv2d_k3s2(c4, w5, s5, b5, residual=self.redir2(c2), act=ACT_RELU)
+        return ops.deconv2d_k3s2(c5, w6, s6, b6, residual=self.redir1(x), act=ACT_RELU)
+
+
+class MSNet2DAggregation(_Engine):
+    """Eval forward of MSNet2D after the volume (msnet/MSNet2D.py:164-212): dres0 -> dres1 (+ cost0) -> 3 x hourglass2D ->
+    classif3 -> trilinear x4 + softmax + regression (osb_upsample_softargmin_fwd, Dl = 48 -> maxdisp).  ``module`` is the MSNet2D
+    model; its parameters are read by the reference's attribute names.  The ReLUs between the dres blocks ride on the blocks'
+    projection epilogues; dres1's `+ cost0` follows its last block (that block already adds its own identity)."""
+
+    def __init__(self, module):
+        super().__init__(module)
+        self._pack_blocks()
+
+    def _pack_blocks(self):
+        m = self.module
+        self.dres0 = [_MBV2Block2D(m.dres0[i], "dres0.%d" % i) for i in (0, 2)]
+        self.dres1 = [_MBV2Block2D(m.dres1[i], "dres1.%d" % i) for i in (0, 2)]
+        self.hg = [_Hourglass2D(getattr(m, n), n) for n in ("encoder_decoder1", "encoder_decoder2", "encoder_decoder3")]
+        cls = m.classif3
+        self.classif3 = [(ops.pack_conv_weight(MSNet2DVolume._at_kd1(cls[0][0].weight.detach().float())),) + ops.fold_bn(cls[0][1]),
+                         (ops.pack_conv_weight(MSNet2DVolume._at_kd1(cls[2].weight.detach().float())), None, None)]
+
+    def _pack(self):
+        self._pack_blocks()
+
+    def logits(self, volume):
+        """volume (B, 48, H, W) -> classif3's cost (B, 48, H, W)."""
+        x = self._check(volume)
+        self._ensure(x.device)
+        cost0 = self.dres0[1](self.dres0[0](x, ACT_RELU), ACT_RELU)
+        out = self.dres1[1](self.dres1[0](cost0, ACT_RELU))
+        out += cost0
+        for hg in self.hg:
+            out = hg(out)
+        (w0, s0, b0), (w1, _, _) = self.classif3
+        out = ops.conv3d_k3(out.unsqueeze(2), w0, s0, b0, act=ACT_RELU)
+        return ops.conv3d_k3(out, w1).squeeze(2)
+
+    def __call__(self, volume, h, w):
+        return ops.upsample_softargmin(self.logits(volume).unsqueeze(1), self.module.maxdisp, h, w, align_corners=False)
 
 
 # ------------------------------------------------------------------------------------------------------ IGEV++

@@ -44,7 +44,13 @@ struct VolParams {
   int mask_left, use_tma, vec_ok;
   int order;           // work-item order: 0 = unit fastest, 1 = image row fastest (adjacent CTAs write adjacent 512-byte rows)
   float inv_k;
+  int crop;            // 1: interlaced crops (osb_interlaced_crops_fwd), concat inputs only, one unit per item
 };
+
+// Floats of the interlaced crops of disparities 0 .. d-1: images (B, H, W - d', 2C) back to back.
+__host__ __device__ __forceinline__ size_t crop_offset(const VolParams& p, int d) {
+  return (size_t)p.B * p.H * 2 * p.Cc * ((size_t)d * p.W - (size_t)d * (d - 1) / 2);
+}
 
 __device__ __forceinline__ float4 load_quad(const float* row, int w, int W, bool vec) {
   // row points at column 0 of a feature row; returns columns w..w+3 (zero beyond W).
@@ -139,7 +145,37 @@ __global__ void __launch_bounds__(256, 2) volume_kernel(const __grid_constant__ 
     const int nquads = (nd + 3) >> 2;
     const int col0 = w0 - d0 - kChunkD;                             // global column of staged column 0
 
-    if (cur.unit < p.n_gwc_units) {
+    if (p.crop) {
+      // ---------------------------------------------------------------- interlaced crops (MSNet2D's per-disparity inputs)
+      // Stage the row's left columns w0 .. w0+127 and right columns col0 .. col0+191 channel-major (pitch +1: the four channels
+      // of one float4 fall in four banks), then write every crop voxel (w, block j) = L[4j..4j+3][w], R[4j..4j+3][w-d] as
+      // contiguous streaming float4 stores: consecutive threads write consecutive 16 bytes of one image row.
+      const int C = p.Cc, nq = C / 2;                               // float4 per output voxel (2C channels)
+      constexpr int LP = kTileW + 1, RP = kRowW + 1;
+      float* ls = smem;
+      float* rs = smem + (size_t)C * LP;
+      for (int idx = threadIdx.x; idx < C * kRowW; idx += blockDim.x) {
+        const int r = idx / kRowW, c = idx - r * kRowW;
+        const size_t row = ((size_t)(b * C + r) * p.H + h) * p.W;
+        const int gw = col0 + c;
+        rs[r * RP + c] = (gw >= 0 && gw < p.W) ? __ldg(p.tgt_c + row + gw) : 0.f;
+        if (c < kTileW) ls[r * LP + c] = (w0 + c < p.W) ? __ldg(p.ref_c + row + w0 + c) : 0.f;
+      }
+      __syncthreads();
+      for (int dd = 0; dd < nd; ++dd) {
+        const int d = d0 + dd;
+        const int wa = max(w0, d), wb = min(w0 + kTileW, p.W);
+        if (wa >= wb) continue;
+        float4* img = reinterpret_cast<float4*>(p.out + crop_offset(p, d)) + ((size_t)(b * p.H + h) * (p.W - d) + (wa - d)) * nq;
+        const int n = (wb - wa) * nq;
+        for (int i = threadIdx.x; i < n; i += blockDim.x) {
+          const int wl = i / nq, q = i - wl * nq;
+          const float* s = (q & 1) ? rs + (size_t)(2 * (q - 1)) * RP + (wa + wl - d - col0) : ls + (size_t)(2 * q) * LP + (wa + wl - w0);
+          const int pitch = (q & 1) ? RP : LP;
+          st_cs_f4(reinterpret_cast<float*>(img + i), make_float4(s[0], s[pitch], s[2 * pitch], s[3 * pitch]));
+        }
+      }
+    } else if (cur.unit < p.n_gwc_units) {
       // ---------------------------------------------------------------- group-wise correlation unit
       const int g0 = cur.unit * p.GU;
       if (p.use_tma) {
@@ -273,7 +309,8 @@ __global__ void __launch_bounds__(256, 2) volume_kernel(const __grid_constant__ 
 static thread_local const char* g_volume_variant = "";   // osb_volume_last_variant
 
 static int launch_volume(const float* ref_g, const float* tgt_g, const float* ref_c, const float* tgt_c, float* out,
-                         int B, int Cg, int Cc, int H, int W, int D, int G, int mask_left, cudaStream_t stream, int reduce_sum = 0) {
+                         int B, int Cg, int Cc, int H, int W, int D, int G, int mask_left, cudaStream_t stream, int reduce_sum = 0,
+                         int crop = 0) {
   OSB_REQUIRE(B > 0 && H > 0 && W > 0 && D > 0, "volume: empty shape B=%d H=%d W=%d D=%d", B, H, W, D);
   OSB_REQUIRE(Cg >= 0 && Cc >= 0 && (Cg > 0 || Cc > 0), "volume: no channels");
   int K = 0;
@@ -295,10 +332,11 @@ static int launch_volume(const float* ref_g, const float* tgt_g, const float* re
   }
   p.GU = GU;
   p.n_gwc_units = Cg > 0 ? (G + GU - 1) / GU : 0;
-  p.n_cat_units = Cc > 0 ? (2 * Cc + GU - 1) / GU : 0;
+  p.n_cat_units = crop ? 1 : Cc > 0 ? (2 * Cc + GU - 1) / GU : 0;
   p.w_tiles = (W + kTileW - 1) / kTileW;
   p.d_chunks = (D + kChunkD - 1) / kChunkD;
   p.mask_left = mask_left;
+  p.crop = crop;
   {
     static const int order = [] {                   // OSB_VOLUME_ORDER=0 restores the round-1 item order (A/B in tools/kbench.py)
       const char* e = getenv("OSB_VOLUME_ORDER");
@@ -311,6 +349,7 @@ static int launch_volume(const float* ref_g, const float* tgt_g, const float* re
   p.vec_ok = (W % 4 == 0) && aligned16(ref_g) && aligned16(ref_c) && aligned16(out);
   const int rows = Cg > 0 ? GU * K : GU;
   size_t smem = 2 * (size_t)rows * kRowW * sizeof(float) + 16;    // two-stage ring + two mbarriers
+  if (crop) smem = (size_t)Cc * (kTileW + 1 + kRowW + 1) * sizeof(float) + 16;   // one left and one right row per channel
   CUtensorMap map{};
   p.use_tma = 0;
   if (Cg > 0 && W % 4 == 0 && aligned16(tgt_g) && rows <= 256) {
@@ -387,6 +426,15 @@ int osb_gwc_concat_volume_fwd(const float* ref_gwc, const float* tgt_gwc, const 
   OSB_REQUIRE(ref_gwc && tgt_gwc && ref_cat && tgt_cat && out, "gwc_concat_volume: null pointer");
   OSB_REQUIRE(Cg > 0 && Cc > 0, "gwc_concat_volume: Cg=%d Cc=%d", Cg, Cc);
   return osb::launch_volume(ref_gwc, tgt_gwc, ref_cat, tgt_cat, out, B, Cg, Cc, H, W, D, G, 1, (cudaStream_t)stream);
+}
+
+int osb_interlaced_crops_fwd(const float* left, const float* right, float* out, int B, int C, int H, int W, int D,
+                             osb_stream_t stream) {
+  OSB_REQUIRE(left && right && out, "interlaced_crops: null pointer");
+  OSB_REQUIRE(C > 0 && C % 4 == 0, "interlaced_crops: C=%d is not a positive multiple of 4", C);
+  OSB_REQUIRE(D > 0 && D <= W, "interlaced_crops: D=%d disparities need W >= D (W=%d)", D, W);
+  OSB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "interlaced_crops: out is not 16-byte aligned");
+  return osb::launch_volume(nullptr, nullptr, left, right, out, B, 0, C, H, W, D, 0, 0, (cudaStream_t)stream, 0, 1);
 }
 
 int osb_corr_volume_fwd(const float* left, const float* right, float* out, int B, int C, int H, int W, int D,

@@ -166,6 +166,25 @@ def correlation_volume(left_feature, right_feature, max_disp):
     return out.to(dt)
 
 
+def interlaced_crops(left, right, ndisp):
+    """MSNet2D's per-disparity inputs (msnet/MSNet2D.py:145-159), one launch: left, right (B, C, H, W) -> [x_0, .., x_{ndisp-1}],
+    x_d (B, H, W - d, 2C) the channels-last crop interweave_tensors(left[..., d:], right[..., :W - d]) with the 2C depths regrouped
+    in blocks of eight: block j holds left channels 4j..4j+3, then right channels 4j..4j+3 (osb_interlaced_crops_fwd).  The images
+    are contiguous views of one buffer.  1 <= ndisp <= W, C % 4 == 0."""
+    l, _ = _prep(left, "left")
+    r, _ = _prep(right, "right")
+    if l.dim() != 4 or l.shape != r.shape:
+        raise ValueError("interlaced_crops: left %s and right %s must be the same (B, C, H, W)" % (tuple(l.shape), tuple(r.shape)))
+    _same_device(l, r)
+    b, c, h, w = l.shape
+    if c % 4 or not 1 <= ndisp <= w:
+        raise ValueError("interlaced_crops: C=%d must be a multiple of 4 and 1 <= ndisp=%d <= W=%d" % (c, ndisp, w))
+    sizes = [b * h * (w - d) * 2 * c for d in range(ndisp)]
+    out = torch.empty(sum(sizes), dtype=torch.float32, device=l.device)
+    _call("osb_interlaced_crops_fwd", l.data_ptr(), r.data_ptr(), out.data_ptr(), b, c, h, w, ndisp, _stream(out))
+    return [t.view(b, h, w - d, 2 * c) for d, t in enumerate(torch.split(out, sizes))]
+
+
 def build_gwc_volume_normalized(refimg_fea, targetimg_fea, maxdisp, num_groups):
     """FoundationStereo's L2-normalised group-wise correlation volume (foundationstereo/core/submodule.py:422-461):
     every group's channel vector is F.normalize'd (eps 1e-12) before the dot product, which is a SUM over the group."""

@@ -1,5 +1,5 @@
 """patch(model): make an UNMODIFIED OpenStereo model instance (GwcNet / PSMNet / StereoBase / LightStereo / IGEVStereo / IGEV-RT /
-IGEV++ / MonSter / CoEx / MSNet3D, CasStereo's CasPSMNet / CasGwcNet, AANet and CFNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
+IGEV++ / MonSter / CoEx / MSNet3D / MSNet2D, CasStereo's CasPSMNet / CasGwcNet, AANet and CFNet, built by the reference's own classes from an unchanged cfg YAML) run its cost-volume
 hot path on the sm_90a kernels.
 
 The reference has no operator registry; names are bound three different ways (SURVEY.md section 8b), and each needs its own
@@ -28,6 +28,7 @@ rebinding.  What each model rebinds:
               (aanet/submodule.py:748, 801-824)
 * MSNet3D     one monolithic ``forward`` (MSNet3D.py:110-161), no processor modules: ``model.forward``, which keeps the
               reference's ``feature_extraction``
+* MSNet2D     the same: ``model.forward`` (MSNet2D.py:134-212), which keeps ``feature_extraction`` and ``preconv11``
 * CFNet       the same: ``model.forward`` (cfnet.py:488-668), which keeps ``feature_extraction`` and the reference's search-range
               and sampling code between the stages
 
@@ -538,6 +539,25 @@ def _patch_msnet3d(model, strict, backbone=True):
     return model
 
 
+def _patch_msnet2d(model, strict, backbone=True):
+    """MSNet2D (msnet/MSNet2D.py): everything after preconv11 in the eval forward (``model.forward``, per instance) -- the
+    48-disparity volume loop (aggregation.MSNet2DVolume: the interlaced crops in one launch, the three depth-strided Conv3ds as 3x3
+    Conv2ds per crop, volume11), then dres0 / dres1, the three hourglass2Ds, classif3 and the trilinear x4 + softmax + regression
+    tail (aggregation.MSNet2DAggregation).  ``feature_extraction`` and ``preconv11`` stay the reference's code; `backbone` has no
+    effect.  A volume network or block the kernels do not implement is refused here, naming it."""
+    from .aggregation import MSNet2DAggregation, MSNet2DVolume
+    volume, engine = MSNet2DVolume(model), MSNet2DAggregation(model)
+
+    def forward(data):
+        left, right = data["left"], data["right"]
+        fl = model.preconv11(model.feature_extraction(left))
+        fr = model.preconv11(model.feature_extraction(right))
+        return {"disp_pred": engine(volume(fl, fr), left.shape[2], left.shape[3]).to(left.dtype)}
+
+    _override(model, "MSNet2D", strict, forward, operands=lambda data: (data["left"], data["right"]))
+    return model
+
+
 def _patch_cfnet(model, strict, backbone=True):
     """CFNet (cfnet/cfnet.py, class cfnet, built by the CFNet(d) factory): everything after the 2D features in the eval forward
     (``model.forward``, per instance) -- the three stage-1 volumes, the warped volumes of the s3 / s2 refinements, every 3D
@@ -557,9 +577,10 @@ def _patch_cfnet(model, strict, backbone=True):
 
 
 # Models routed by (package, module, class) of their defining module: CasStereo's classes are also named PSMNet / GwcNet, and
-# AANet's and CFNet's classes are the bare lowercase `aanet` / `cfnet`
+# AANet's and CFNet's classes are the bare lowercase `aanet` / `cfnet`; MSNet2D is routed the same way
 _MODULE_PATCHERS = {("casnet", "cas_psm", "PSMNet"): _patch_cascade, ("casnet", "cas_gwc", "GwcNet"): _patch_cascade,
-                    ("aanet", "aanet", "aanet"): _patch_aanet, ("cfnet", "cfnet", "cfnet"): _patch_cfnet}
+                    ("aanet", "aanet", "aanet"): _patch_aanet, ("cfnet", "cfnet", "cfnet"): _patch_cfnet,
+                    ("msnet", "MSNet2D", "MSNet2D"): _patch_msnet2d}
 
 _PATCHERS = {"GwcNet": _patch_gwcnet, "PSMNet": _patch_psmnet, "StereoBase": _patch_stereobase, "LightStereo": _patch_lightstereo,
              "IGEVStereo": _patch_igev, "IGEVRTtereo": _patch_igev_rt,
@@ -587,7 +608,7 @@ def patch(model, strict=True, backbone=True, aggregation=False, amp=False):
         patcher = _PATCHERS[name]
     else:
         raise NotImplementedError("patch(): no hot-path drop-in for %s (supported: %s, CasStereo's casnet.cas_psm.PSMNet / "
-                                  "casnet.cas_gwc.GwcNet, aanet.aanet.aanet and cfnet.cfnet.cfnet)" % (name, sorted(_PATCHERS)))
+                                  "casnet.cas_gwc.GwcNet, aanet.aanet.aanet, cfnet.cfnet.cfnet and msnet.MSNet2D.MSNet2D)" % (name, sorted(_PATCHERS)))
     if aggregation:
         if patcher is not _patch_igevpp:
             raise NotImplementedError("patch(%s, aggregation=True): only IGEVPPStereo has an aggregation option" % name)

@@ -52,6 +52,11 @@
       B=8 @256x512: patch() / unpatched (cuDNN fp32, TF32 off) in alternating rounds, ms per forward and per stage (CUDA events:
       feature extractor, volumes, stage 1, s3, s2), and the EPE against the unpatched model
       (python tools/bench_configs.py --only c17 > results/h100_c17_cfnet.jsonl)
+  c18 MSNet2D (the reference's class, cfgs/msnet/msnet2d_sceneflow.yaml), fp32, B=8 @256x512 (the YAML's training crop) and B=4
+      @512x960 (its eval crop): patch() / unpatched (cuDNN fp32, TF32 off) in alternating rounds, ms per forward and per stage
+      (CUDA events: features, volume front end, aggregation, tail), the library's launches per forward, the cost of the 48
+      volume11 copies into the volume, and the EPE against the unpatched model
+      (python tools/bench_configs.py --only c18 > results/h100_c18_msnet2d.jsonl)
 Each line: this library (CUDA events, L2 flushed between iterations by the working set itself: every config streams > 126 MB per
 step) next to the SAME graph of the oracle modules (bit-equal restatements of the reference: identical aten calls) on this GPU with
 cuDNN fp32 (TF32 off) -- SURVEY.md section 8d's GPU comparator -- and the max abs / EPE difference between the two.
@@ -70,7 +75,7 @@ sys.path.insert(0, ROOT)
 import __graft_entry__                                  # noqa: E402
 __graft_entry__.build()
 from openstereo_b200 import aggregation as agg          # noqa: E402
-from openstereo_b200 import geo, host_models, ops       # noqa: E402
+from openstereo_b200 import _lib, geo, host_models, ops  # noqa: E402
 from oracle import aggregation as oagg                  # noqa: E402
 from oracle import cascade as ocas                      # noqa: E402
 from oracle import cost_volume as ocv                   # noqa: E402
@@ -1122,6 +1127,74 @@ def c17(iters, rounds=3):
         torch.cuda.empty_cache()
 
 
+def c18(iters, rounds=3):
+    """MSNet2D (msnet/MSNet2D.py, the reference's class built from the unchanged msnet2d_sceneflow.yaml), fp32, TF32 off, seeded
+    weights with volume11 and classif3 sharpened (oracle/msnet2d.py), random images.  At B=8 @256x512 and B=4 @512x960: patch(m)
+    and the unpatched model in alternating rounds (`rounds` x `iters` timed forwards after 2 warm-ups), ms per forward (median,
+    min, max over the rounds); then one forward of each with CUDA events per stage:
+      patched    features = feature_extraction + preconv11 (both images), volume = aggregation.MSNet2DVolume (the crops, 3 x 48
+                 convolutions, 48 volume11 convs and copies), aggregation = MSNet2DAggregation.logits, tail = ops.upsample_softargmin;
+      unpatched  the same cut of the reference's forward (oracle/msnet2d.stages' order: its volume loop, dres0 .. classif3,
+                 interpolate + softmax + regression), events between the stages;
+    the library's kernel launches in one patched forward, the ms of the 48 volume[:, d, :, d:] copies alone (the same shapes), and
+    the EPE of the patched disparity against the unpatched one."""
+    from oracle import msnet2d as om
+    from openstereo_b200.patch import patch
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    for B, h, w in ((8, 256, 512), (4, 512, 960)):
+        variants = {"patched": patch(om.reference_model().to(DEV)), "reference": om.reference_model().to(DEV)}
+        gen = torch.Generator().manual_seed(18)
+        x = {"left": rnd(gen, B, 3, h, w), "right": rnd(gen, B, 3, h, w)}
+        ms = {k: [] for k in variants}
+        outs = {}
+        with torch.no_grad():
+            for _ in range(rounds):
+                for k, m in variants.items():
+                    t, outs[k] = timeit(lambda: m(dict(x))["disp_pred"], iters, warm=2)
+                    ms[k].append(t)
+            pm, rm = variants["patched"], variants["reference"]
+            stages = {"patched": _hook_times(lambda: pm(dict(x)), [
+                (["features"], pm.feature_extraction, "forward"), (["features"], pm.preconv11, "forward"),
+                (["volume"], agg.MSNet2DVolume, "__call__"), (["aggregation"], agg.MSNet2DAggregation, "logits"),
+                (["tail"], ops, "upsample_softargmin")])}
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
+            ev[0].record()
+            fl, fr = rm.preconv11(rm.feature_extraction(x["left"])), rm.preconv11(rm.feature_extraction(x["right"]))
+            ev[1].record()
+            volume = om.volume_loop(rm, fl, fr)
+            ev[2].record()
+            cost0 = rm.dres0(volume)
+            cost0 = rm.dres1(cost0) + cost0
+            logits = rm.classif3(rm.encoder_decoder3(rm.encoder_decoder2(rm.encoder_decoder1(cost0))))
+            ev[3].record()
+            cost3 = torch.squeeze(F.interpolate(torch.unsqueeze(logits, 1), [rm.maxdisp, h, w], mode="trilinear"), 1)
+            pred3 = F.softmax(cost3, dim=1)
+            torch.sum(pred3 * torch.arange(0, rm.maxdisp, dtype=pred3.dtype, device=DEV).view(1, rm.maxdisp, 1, 1), 1)
+            ev[4].record()
+            torch.cuda.synchronize()
+            stages["reference"] = {k: round(ev[i].elapsed_time(ev[i + 1]), 3)
+                                   for i, k in enumerate(("features", "volume", "aggregation", "tail"))}
+            n0 = _lib.launch_count()
+            pm(dict(x))
+            launches = _lib.launch_count() - n0
+            hl, wl = fl.shape[2:]
+            vol = torch.zeros(B, 48, hl, wl, device=DEV)
+            ys = [torch.rand(B, hl, wl - d, device=DEV) for d in range(48)]
+            copy_ms = timeit(lambda: [vol[:, d, :, d:].copy_(y) for d, y in enumerate(ys)], iters, warm=2)[0]
+        med = lambda v: sorted(v)[len(v) // 2]                               # noqa: E731
+        ref = outs["reference"]
+        emit(config="c18 MSNet2D, B=%d @%dx%d, %d rounds x %d forwards (reference class + patch(); unpatched: cuDNN fp32, TF32 off)"
+             % (B, h, w, rounds, iters),
+             gpu="%s, %.0f W power limit" % (torch.cuda.get_device_name(DEV), _power_limit_w()),
+             forward_ms={k: {"median": round(med(v), 2), "min": round(min(v), 2), "max": round(max(v), 2)} for k, v in ms.items()},
+             stage_ms=stages, library_launches_per_forward=launches, volume11_copies_ms=round(copy_ms, 3),
+             epe_vs_reference_px=float("%.3e" % (outs["patched"] - ref).abs().mean().item()),
+             disparity_std_px=round(ref.std().item(), 2))
+        del variants, outs
+        torch.cuda.empty_cache()
+
+
 def _timed_call(events, fn, *args, **kw):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
@@ -1188,7 +1261,7 @@ if __name__ == "__main__":
     for name in a.only.split(","):
         try:
             {"c1": c1, "c3": c3, "c4": c4, "c5": c5, "gw": gw, "c6": c6, "c7": c7, "c8": c8, "c9": c9, "c10": c10, "c11": c11,
-             "c12": c12, "c13": c13, "c14": c14, "c15": c15, "c16": c16, "c17": c17}[name](a.iters)
+             "c12": c12, "c13": c13, "c14": c14, "c15": c15, "c16": c16, "c17": c17, "c18": c18}[name](a.iters)
         except Exception as exc:                                               # one config must not hide the others
             emit(config=name, error=repr(exc)[:300])
     if WORLD > 1:
