@@ -118,6 +118,7 @@ int osb_corr_volume_fwd(const float* left, const float* right, float* out, int B
  *     out_d[b, h, w - d, 8j + 4 + k] = right[b, 4j + k, h, w - d]        (w = d .. W-1, j < C/4, k < 4)
  * of shape (B, H, W - d, 2C), the D images back to back (image d starts at B*H*2C*(d*W - d*(d-1)/2) floats).  Block j holds the
  * four left and four right channels that the reference's interleave puts at depths 8j .. 8j+7, left first.  C % 4 == 0,
+ * C <= 180 (a CTA stages one left and one right row per channel, 1288 C + 16 bytes of shared memory, 227 KB at most),
  * 1 <= D <= W, out 16-byte aligned.  The columns w < d are not stored anywhere: each image is exactly the reference's crop. */
 int osb_interlaced_crops_fwd(const float* left, const float* right, float* out, int B, int C, int H, int W, int D,
                              osb_stream_t stream);

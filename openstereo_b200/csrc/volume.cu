@@ -52,6 +52,13 @@ __host__ __device__ __forceinline__ size_t crop_offset(const VolParams& p, int d
   return (size_t)p.B * p.H * 2 * p.Cc * ((size_t)d * p.W - (size_t)d * (d - 1) / 2);
 }
 
+// Dynamic shared memory of an interlaced-crops CTA: one left and one right row per channel (pitch +1) plus the ring's two
+// mbarriers (unused by crops), 1288 C + 16 bytes, so C <= 180 fits the 227 KB a CTA can opt into.
+constexpr size_t kCropSmemLimit = 227 * 1024;
+__host__ __forceinline__ size_t crop_smem_bytes(int C) {
+  return (size_t)C * (kTileW + 1 + kRowW + 1) * sizeof(float) + 16;
+}
+
 __device__ __forceinline__ float4 load_quad(const float* row, int w, int W, bool vec) {
   // row points at column 0 of a feature row; returns columns w..w+3 (zero beyond W).
   if (vec && w + 3 < W) return __ldg(reinterpret_cast<const float4*>(row + w));
@@ -349,7 +356,7 @@ static int launch_volume(const float* ref_g, const float* tgt_g, const float* re
   p.vec_ok = (W % 4 == 0) && aligned16(ref_g) && aligned16(ref_c) && aligned16(out);
   const int rows = Cg > 0 ? GU * K : GU;
   size_t smem = 2 * (size_t)rows * kRowW * sizeof(float) + 16;    // two-stage ring + two mbarriers
-  if (crop) smem = (size_t)Cc * (kTileW + 1 + kRowW + 1) * sizeof(float) + 16;   // one left and one right row per channel
+  if (crop) smem = crop_smem_bytes(Cc);                           // one left and one right row per channel
   CUtensorMap map{};
   p.use_tma = 0;
   if (Cg > 0 && W % 4 == 0 && aligned16(tgt_g) && rows <= 256) {
@@ -432,6 +439,8 @@ int osb_interlaced_crops_fwd(const float* left, const float* right, float* out, 
                              osb_stream_t stream) {
   OSB_REQUIRE(left && right && out, "interlaced_crops: null pointer");
   OSB_REQUIRE(C > 0 && C % 4 == 0, "interlaced_crops: C=%d is not a positive multiple of 4", C);
+  OSB_REQUIRE(osb::crop_smem_bytes(C) <= osb::kCropSmemLimit,
+              "interlaced_crops: C=%d stages %zu bytes of shared memory per CTA (227 KB max, C <= 180)", C, osb::crop_smem_bytes(C));
   OSB_REQUIRE(D > 0 && D <= W, "interlaced_crops: D=%d disparities need W >= D (W=%d)", D, W);
   OSB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "interlaced_crops: out is not 16-byte aligned");
   return osb::launch_volume(nullptr, nullptr, left, right, out, B, 0, C, H, W, D, 0, 0, (cudaStream_t)stream, 0, 1);

@@ -166,19 +166,24 @@ def correlation_volume(left_feature, right_feature, max_disp):
     return out.to(dt)
 
 
+CROPS_MAX_CHANNELS = 180        # osb_interlaced_crops_fwd stages 1288 C + 16 bytes of shared memory per CTA, 227 KB at most
+
+
 def interlaced_crops(left, right, ndisp):
     """MSNet2D's per-disparity inputs (msnet/MSNet2D.py:145-159), one launch: left, right (B, C, H, W) -> [x_0, .., x_{ndisp-1}],
     x_d (B, H, W - d, 2C) the channels-last crop interweave_tensors(left[..., d:], right[..., :W - d]) with the 2C depths regrouped
     in blocks of eight: block j holds left channels 4j..4j+3, then right channels 4j..4j+3 (osb_interlaced_crops_fwd).  The images
-    are contiguous views of one buffer.  1 <= ndisp <= W, C % 4 == 0."""
+    are contiguous views of one buffer.  1 <= ndisp <= W, C % 4 == 0, C <= 180 (the kernel stages one left and one right row per
+    channel in shared memory)."""
     l, _ = _prep(left, "left")
     r, _ = _prep(right, "right")
     if l.dim() != 4 or l.shape != r.shape:
         raise ValueError("interlaced_crops: left %s and right %s must be the same (B, C, H, W)" % (tuple(l.shape), tuple(r.shape)))
     _same_device(l, r)
     b, c, h, w = l.shape
-    if c % 4 or not 1 <= ndisp <= w:
-        raise ValueError("interlaced_crops: C=%d must be a multiple of 4 and 1 <= ndisp=%d <= W=%d" % (c, ndisp, w))
+    if c % 4 or c > CROPS_MAX_CHANNELS or not 1 <= ndisp <= w:
+        raise ValueError("interlaced_crops: C=%d must be a multiple of 4 and at most %d, and 1 <= ndisp=%d <= W=%d" % (
+            c, CROPS_MAX_CHANNELS, ndisp, w))
     sizes = [b * h * (w - d) * 2 * c for d in range(ndisp)]
     out = torch.empty(sum(sizes), dtype=torch.float32, device=l.device)
     _call("osb_interlaced_crops_fwd", l.data_ptr(), r.data_ptr(), out.data_ptr(), b, c, h, w, ndisp, _stream(out))

@@ -328,7 +328,7 @@ def _struct_fields(name, struct):
     """Field names of `struct <struct> { ... };` in csrc/<name> (member functions skipped, array extents dropped)."""
     import re
     body = re.search(r"struct\s+%s\s*\{(.*?)\n\};" % struct, _csrc(name), re.S).group(1)
-    body = re.sub(r"[\w:<>]+\s+\w+\s*\([^()]*\)\s*(?:const\s*)?\{[^{}]*\}", "", body)      # bool slice() const { ... }
+    body = re.sub(r"(?:\w+\s+)*[\w:<>]+\s+\w+\s*\([^()]*\)\s*(?:const\s*)?\{[^{}]*\}", "", body)   # __device__ void f() const { }
     fields = []
     for stmt in body.split(";"):
         stmt = re.sub(r"=[^,]*|\[[^\]]*\]", "", stmt).strip()                                # initialisers, [GEO_MAX_LEVELS]
@@ -338,10 +338,21 @@ def _struct_fields(name, struct):
 
 
 def _kernel_params(name, kernel):
-    """Parameter names of __global__ <kernel>(...) in csrc/<name>."""
+    """Parameter names of __global__ <kernel>(...) in csrc/<name>.  A parameter passed by value whose type is a struct defined in
+    that file is replaced by its fields, spelled as the kernel reads them ("p.crop", "ad.align")."""
     import re
-    params = re.search(_GLOBAL.replace(r"(\w+)", kernel) + r"([^()]*)\)", _csrc(name)).group(1)
-    return [re.findall(r"\w+", p)[-1] for p in params.split(",")]
+    src = _csrc(name)
+    structs = set(re.findall(r"\bstruct\s+(\w+)\s*\{", src))
+    params = re.search(_GLOBAL.replace(r"(\w+)", kernel) + r"([^()]*)\)", src).group(1)
+    names = []
+    for p in params.split(","):
+        words = re.findall(r"\w+", p)
+        struct = [w for w in words[:-1] if w in structs]
+        if struct and "*" not in p and "&" not in p:
+            names += ["%s.%s" % (words[-1], f) for f in _struct_fields(name, struct[0])]
+        else:
+            names.append(words[-1])
+    return names
 
 
 def test_tc_runtime_modes_have_contract_rows():
@@ -367,26 +378,47 @@ def test_tc_runtime_modes_have_contract_rows():
     assert {r.cin // r.opt[2] for r in dcn} >= {4, 8, 16}
 
 
+def _nonconv_kernel_params():
+    """{kernel: parameter names} for every __global__ function of the non-convolution sources, by-value structs field by field."""
+    import re
+    params = {}
+    for name in _KERNEL_CONTRACT_FILES:
+        for kernel in set(re.findall(_GLOBAL, _csrc(name))) - _CONVOLUTIONS_THERE:
+            assert kernel not in params, "%s is defined twice" % kernel
+            params[kernel] = _kernel_params(name, kernel)
+    return params
+
+
 def test_nonconv_runtime_modes_have_contract_rows():
-    """Every field of struct GeoParams (geo.cu) and struct WarpParams (cascade.cu) and every parameter of ncdhw_to_ndhwc_kernel
-    (conv3d_tc.cu) is classified in tests/test_kernel_contract_gpu.py as an operand / geometry field or as the runtime mode it selects;
-    every mode is one row family whose rows reach exactly the instantiations NONCONV_MODE_VARIANTS lists for it (test_routing checks
-    each row's on the GPU); each lookup family has a row whose taps take the fallback read and a row at grid z = 65535."""
-    from test_kernel_contract_gpu import (GEO_PARAMS_FIELDS, LAYOUT_KERNEL_PARAMS, MODE_REQUIREMENTS, NONCONV_MODE_VARIANTS, REGISTRY,
-                                          WARP_PARAMS_FIELDS, grid_z)
-    classified = {}
-    for what, fields, table in (("GeoParams", _struct_fields("geo.cu", "GeoParams"), GEO_PARAMS_FIELDS),
-                                ("WarpParams", _struct_fields("cascade.cu", "WarpParams"), WARP_PARAMS_FIELDS),
-                                ("ncdhw_to_ndhwc_kernel", _kernel_params("conv3d_tc.cu", "ncdhw_to_ndhwc_kernel"), LAYOUT_KERNEL_PARAMS)):
-        assert len(fields) == len(set(fields)) and len(fields) >= 9, (what, fields)
-        assert set(fields) == set(table), "%s fields not classified: %s; classified fields that are gone: %s" % (
-            what, sorted(set(fields) - set(table)), sorted(set(table) - set(fields)))
-        classified[what] = {m for m in table.values() if m}
-    assert {"geo", "corr", "out_corr", "D2"} <= set(GEO_PARAMS_FIELDS) and {"border", "ys", "coff"} <= set(WARP_PARAMS_FIELDS) | set(
-        LAYOUT_KERNEL_PARAMS)
-    modes = set().union(*classified.values())
+    """Every parameter of every __global__ function in the non-convolution sources (a by-value struct such as VolParams, GeoParams,
+    WarpParams, RegressionParams or Axis field by field) is classified in NONCONV_KERNEL_PARAMS (tests/test_kernel_contract_gpu.py) as
+    an operand / geometry field or as the runtime mode it selects; every mode is one row family whose rows reach exactly the
+    instantiations NONCONV_MODE_VARIANTS lists for it (test_routing checks each row's on the GPU), all of them of the kernels whose
+    parameters select the mode; each mode's rows meet MODE_REQUIREMENTS; each lookup family has a row whose taps take the fallback
+    read and a row at grid z = 65535; both warped_volume_kernel instantiations have a cas row with the left copy unmasked."""
+    from test_kernel_contract_gpu import MODE_REQUIREMENTS, NONCONV_KERNEL_PARAMS, NONCONV_MODE_VARIANTS, REGISTRY, grid_z
+    found = _nonconv_kernel_params()
+    assert set(found) == set(NONCONV_KERNEL_PARAMS), "kernels not classified: %s; classified kernels that are gone: %s" % (
+        sorted(set(found) - set(NONCONV_KERNEL_PARAMS)), sorted(set(NONCONV_KERNEL_PARAMS) - set(found)))
+    selects = {}                                                        # mode -> kernels with a parameter that selects it
+    for kernel, params in found.items():
+        table = NONCONV_KERNEL_PARAMS[kernel]
+        assert params and len(params) == len(set(params)), (kernel, params)
+        assert set(params) == set(table), "%s parameters not classified: %s; classified parameters that are gone: %s" % (
+            kernel, sorted(set(params) - set(table)), sorted(set(table) - set(params)))
+        for mode in set(table.values()) - {""}:
+            selects.setdefault(mode, set()).add(kernel)
+    assert {"p.crop", "p.mask_left", "tgt_map"} <= set(found["volume_kernel"]) and {"values", "var_out"} <= set(found["softargmin_kernel"])
+    assert {"p.corr", "p.out_corr", "p.D2"} <= set(found["geo_lookup_kernel"]) and "p.border" in found["warped_volume_kernel"]
+    assert {"ad.align", "aw.scale"} <= set(found["upsample_softargmin_kernel"]) and "p.logits" in found["coex_regression_kernel"]
+    assert {"ys", "coff"} <= set(found["ncdhw_to_ndhwc_kernel"])
+    modes = set(selects)
     assert modes == set(NONCONV_MODE_VARIANTS), "modes without an entry in NONCONV_MODE_VARIANTS: %s; entries no field selects: %s" % (
         sorted(modes - set(NONCONV_MODE_VARIANTS)), sorted(set(NONCONV_MODE_VARIANTS) - modes))
+    for mode, variants in NONCONV_MODE_VARIANTS.items():
+        kernels = {v.split("<")[0] for v in variants}
+        assert kernels == selects[mode], "mode %s lists instantiations of %s, but parameters of %s select it" % (
+            mode, sorted(kernels), sorted(selects[mode]))
     plain = {r.fam for r in REGISTRY} - modes
     for mode, variants in NONCONV_MODE_VARIANTS.items():
         rows = [r for r in REGISTRY if r.fam == mode]
@@ -404,6 +436,9 @@ def test_nonconv_runtime_modes_have_contract_rows():
         rows = [r for r in REGISTRY if r.fam == mode]
         for what, met in needs.items():
             assert any(met(r) for r in rows), "mode %s: no row with %s" % (mode, what)
+    for variant in ("warped_volume_kernel<8>", "warped_volume_kernel<16>"):      # CFNet's volume: (B, Cg, G, Cc, D, H, W)
+        assert any(r.fam == "cas" and r.variant == variant and r.shape[1] > 0 and r.opts.get("mask") == 0 for r in REGISTRY), (
+            "%s: no cas row with Cg > 0 and mask_left = 0" % variant)
 
 
 def test_instance_norm_modes_have_contract_rows():

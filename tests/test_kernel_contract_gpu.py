@@ -13,19 +13,27 @@ and a small shape with partial tiles, chunks and units in every tiled dimension.
                                      can make |want| small while the fp32 rounding stays proportional to sum |terms|); the geo,
                                      context and regression-values taps use each element's own sum |terms|, which is stricter;
                  copies and gathers  bit-exact: the concat volume and the concat halves of the fused volume, the left copies of
-                                     the warped volumes, nearest_resize3d, avgpool_pairs, the layout pass with its zero
-                                     channels, and the exact zeros of every masked triangle;
+                                     the warped volumes, the interlaced crops, nearest_resize3d, avgpool_pairs, the layout pass
+                                     with its zero channels, and the exact zeros of every masked triangle;
                  soft-argmin family  per pixel, see soft_model();
   bounds       the output region starts as NaN between 4 KB sentinel guards: every element is written and no sentinel changes;
-               a backward launch with one gradient pointer null leaves that gradient's region unwritten;
+               a backward launch with one gradient pointer null, or a variance launch with var_out null, leaves that output's
+               region unwritten;
   store paths  where a kernel picks its loads and stores by alignment (the volume's vec_ok and use_tma, context_upsample's
                vector branch) the row runs aligned and with pointers moved 4 bytes: bit-identical, and each run passes the bar;
-  item loop    volume rows run at persistent-grid caps 1, 5 and uncapped, bit-identical; the grid-stride rows of avgpool_pairs
-               and nearest_resize3d have totals above their SM-count-based grid caps;
+  item loop    volume and crop rows run at persistent-grid caps 1, 5 and uncapped, bit-identical; the grid-stride rows of
+               avgpool_pairs and nearest_resize3d have totals above their SM-count-based grid caps;
   determinism  two launches are bit-identical, except epe_partial_kernel, whose float atomics add block partial sums in
                arrival order: its error sum gets the bar of the sum instead (its counts are integers and stay exact).
-Runtime modes are row families of their own (NONCONV_MODE_VARIANTS; GEO_PARAMS_FIELDS, WARP_PARAMS_FIELDS and LAYOUT_KERNEL_PARAMS
-classify every field that selects one, and MODE_REQUIREMENTS lists the edges each family's rows must cover):
+Runtime modes are row families of their own (NONCONV_MODE_VARIANTS; NONCONV_KERNEL_PARAMS classifies every parameter of every
+kernel above, a by-value struct parameter field by field, as an operand or as the mode it selects, and MODE_REQUIREMENTS lists the
+edges each family's rows must cover):
+  crop         the interlaced crops (VolParams::crop): all D crops in one guarded buffer, bit-exact against the fp64 gather;
+               aligned, with the left or the right input moved 4 bytes (a moved left input takes volume_kernel<false,true>),
+               at grid caps 1 and 5; three column tiles and two disparity chunks, D = W, the largest C whose rows fit;
+  var          the soft-argmin variance (softargmin_kernel's values / var_out): mean and variance in one guarded buffer; the
+               variance is summed about the kernel's fp32 mean, so its bar adds the mean's bar squared; the var_out-NULL run's
+               mean equals the full run's bit for bit, and with values NULL too it is osb_softargmin_fwd's result;
   geov         the geometry-only lookup (corr[0] == NULL): geo_model without correlation rows, a grid z of exactly 65535;
   geomr        the multi-range lookup: four outputs, one case each, the other three written to guarded scratch; vol2's taps
                leave both ends; D1 != D2, D1 = D2 = 2, W2 != W, a grid z of exactly 65535;
@@ -33,9 +41,14 @@ classify every field that selects one, and MODE_REQUIREMENTS lists the edges eac
   slice        the channel slice of a channels-last concatenation: exact inside the slice, the other channels still NaN;
   split        the split NDHWC conversion: every 32-bit word of hi/lo halves exact, tc_overflow_count >= 1 after a saturating
                row and 0 after the others.
-test_volume_item_order_0: the other work-item order, read once per process, in a child process, bit-identical to order 1.
+The cas rows with mask = 0 run the fused warped volume through its _ex entry point with the left copy and the correlation
+unmasked (CFNet), at fractional samples, on both instantiations.
+test_volume_item_order_0: the other work-item order, read once per process, in a child process, bit-identical to order 1, for a
+fused volume and for interlaced crops (through ops.interlaced_crops, whose views must have the crops' shapes).
+test_warped_ex_mask_left_1: the _ex entry point with mask_left = 1 is osb_warped_gwc_concat_volume_fwd bit for bit.
 test_volume_input_types: fp16 / bf16 inputs through ops.*: output in the input type, equal to the rounded fp32 result.
-test_refusals: every input an entry point refuses returns OSB_EINVAL and launches nothing.
+test_refusals: every input an entry point refuses returns OSB_EINVAL and launches nothing, and a valid launch after them all
+returns OSB_OK (no refusal leaves a CUDA error behind for the next launch to report).
 """
 import math
 import os
@@ -52,7 +65,7 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OSB_EINVAL = 1
+OSB_OK, OSB_EINVAL = 0, 1
 GUARD = 1024                            # sentinel floats on each side of an output region (4 KB, keeps 16-byte alignment)
 SENTINEL = -1234.5
 TOL = 1e-5                              # products and sums: error / (channel max of sum |terms|)
@@ -92,6 +105,13 @@ REGISTRY = [
     R("vol-fused-k4", "vol", V(1, 1), (2, 10, 4, 6, 2, 128, 65), entry="fused"),
     R("vol-fused-k3", "vol", V(1, 0), (1, 5, 3, 5, 2, 132, 48), entry="fused"),
     R("vol-fused-k3-w129", "vol", V(0, 0), (1, 5, 3, 4, 2, 129, 20), entry="fused"),
+    # interlaced-crops mode (VolParams::crop, osb_interlaced_crops_fwd) (B, C, H, W, D): the D crops (B, H, W - d, 2C) back to back.
+    # A work item stages C left and C right rows of one 128-column tile, 1288 C + 16 bytes
+    R("crop-w260-d70", "crop", V(1, 1), (2, 8, 3, 260, 70)),           # three column tiles, the last partial; two disparity chunks
+    R("crop-d-eq-w", "crop", V(0, 1), (1, 4, 2, 131, 131)),            # the last crop is one column wide
+    R("crop-c180", "crop", V(1, 1), (1, 180, 2, 40, 9)),               # 231 856 bytes staged: the largest C that fits 227 KB
+    R("crop-msnet2d", "crop", V(1, 1), (2, 32, 3, 240, 48)),           # MSNet2D's own shape at 1/4 of 960
+    R("crop-b3-w61", "crop", V(0, 1), (3, 8, 2, 61, 17)),
     # softargmin.cu softargmin_kernel (B, D, H, W): 8-bin chunks; 185 pixels per image, not a multiple of the 256-thread block
     R("sa-d1", "sa", "softargmin_kernel", (2, 1, 5, 37)),
     R("sa-d7-alpha-1", "sa", "softargmin_kernel", (2, 7, 5, 37), alpha=-1.0),
@@ -103,6 +123,15 @@ REGISTRY = [
     R("sa-d193-inf", "sa", "softargmin_kernel", (1, 193, 3, 37), inf=1, spread=60.0),
     R("sa-d9-raw", "sa", "softargmin_kernel", (2, 9, 5, 37), norm=0),
     R("sa-d192-raw", "sa", "softargmin_kernel", (1, 192, 5, 37), norm=0, alpha=-1.0, start=2.0, step=0.5),
+    # variance mode (values / var_out, osb_softargmin_var_fwd) (B, D, H, W): the sa rows' costs; values = 1 reads sorted non-integer
+    # samples, some negative (CFNet's), values NULL the planes 0 .. D - 1.  No pixel count is a multiple of the 256-thread block
+    R("var-d1", "var", "softargmin_kernel", (2, 1, 5, 37)),                         # the variance must be exactly 0
+    R("var-d1-values", "var", "softargmin_kernel", (2, 1, 5, 37), values=1),
+    R("var-d9-inf", "var", "softargmin_kernel", (2, 9, 5, 37), inf=1),               # a one-bin last chunk with -inf bins
+    R("var-d9-inf-values", "var", "softargmin_kernel", (2, 9, 7, 37), inf=1, values=1, peak_last=1),
+    R("var-d193-inf-values", "var", "softargmin_kernel", (1, 193, 3, 37), inf=1, spread=60.0, values=1),
+    R("var-d48-spread", "var", "softargmin_kernel", (1, 48, 5, 37), spread=60.0, offset=1e4),
+    R("var-d192-spread-values", "var", "softargmin_kernel", (1, 192, 5, 37), spread=60.0, offset=1e4, values=1),
     # upsample_softargmin_kernel (B, Dl, Hl, Wl, D, H, W): 128-column tiles; shared tables of D + Dl + 1 words (48 KB)
     R("up-x4", "up", "upsample_softargmin_kernel<false>", (2, 12, 5, 40, 48, 20, 160), align=0),
     R("up-x4-align", "up", "upsample_softargmin_kernel<false>", (2, 12, 5, 40, 48, 20, 160), align=1),
@@ -160,6 +189,9 @@ REGISTRY = [
     R("cas-gwc-k16", "cas", "warped_volume_kernel<16>", (1, 32, 2, 10, 3, 7, 33), two=1),
     R("cas-gwc-wmax", "cas", "warped_volume_kernel<16>", (1, 16, 1, 1, 2, 2, 1816)),     # 16 x 2 rows x 1816 floats = 227 KB
     R("cas-cat-wmax", "cas", "warped_volume_kernel<8>", (1, 0, 0, 1, 2, 2, 3632), mask=1),
+    # the left copy and the correlation unmasked (osb_warped_gwc_concat_volume_ex_fwd, mask_left = 0: CFNet)
+    R("cas-gwc-k8-unmasked", "cas", "warped_volume_kernel<8>", (2, 24, 3, 5, 4, 10, 40), mask=0, two=1),
+    R("cas-gwc-wmax-unmasked", "cas", "warped_volume_kernel<16>", (1, 32, 2, 3, 2, 6, 1816), mask=0, two=1),   # 227 KB of rows
     # disparity-warp mode (border = 1, osb_disp_warp_fwd) (B, C, H, W): units of 8 channels; every row coordinate is an integer at
     # H = 2 (and 3), not at the heights below
     R("warp-c5-h2", "warp", "warped_volume_kernel<8>", (2, 5, 2, 17), two=0),
@@ -206,28 +238,56 @@ BY_ID = {r.id: r for r in REGISTRY}
 # Runtime modes of the kernels above.  Each mode is one row family; NONCONV_MODE_VARIANTS lists the instantiations its entry point
 # reaches, and its rows must reach exactly those (tests/test_host_logic_cpu.py).
 NONCONV_MODE_VARIANTS = {
+    "crop": {V(1, 1), V(0, 1)},                                         # interlaced crops (MSNet2D): VolParams::crop
+    "var": {"softargmin_kernel"},                                       # soft-argmin variance (CFNet): values / var_out
     "geov": {"geo_lookup_kernel<4>", "geo_lookup_kernel<0>"},           # geometry-only (IGEV-RT): corr[0] == NULL
     "geomr": {"geo_lookup_kernel<4>", "geo_lookup_kernel<0>"},          # multi-range (IGEV++): out_corr != NULL
     "warp": {"warped_volume_kernel<8>"},                                # disparity warp (MonSter, AANet): border = 1
     "slice": {"ncdhw_to_ndhwc_kernel"},                                 # channel slice of a channels-last concatenation
     "split": {"ncdhw_to_ndhwc_kernel"},                                 # split NDHWC output
 }
-# Every field of struct GeoParams (csrc/geo.cu), struct WarpParams (csrc/cascade.cu) and every parameter of ncdhw_to_ndhwc_kernel
-# (csrc/conv3d_tc.cu): "" = an operand or geometry field the plain rows exercise, otherwise the mode whose rows exercise it.  A
-# field that is in neither fails tests/test_host_logic_cpu.py.
-GEO_PARAMS_FIELDS = {
-    **{f: "" for f in "geo disp coords out B C D H W W2 levels radius".split()},
-    "corr": "geov",
-    **{f: "geomr" for f in "vol1 vol2 out1 out2 out_corr D1 D2".split()},
-}
-WARP_PARAMS_FIELDS = {
-    **{f: "" for f in "xg yg xc yc disp out B Cg G K Cc D H W Ctot oc_cat n_gwc_units n_cat_units mask_left half_w half_h".split()},
-    **{f: "warp" for f in "border wm1 hm1".split()},
-}
-LAYOUT_KERNEL_PARAMS = {
-    **{f: "" for f in "x y C Cp vol".split()},
-    "ys": "split", "overflow": "split",
-    "ystride": "slice", "coff": "slice",
+
+
+def _plain(names):
+    return {n: "" for n in names.split()}
+
+
+# Every parameter of every kernel above (the __global__ functions of the registry's sources, tests/test_host_logic_cpu.py), a
+# by-value struct parameter replaced by its fields, spelled as the kernel reads them ("p.crop", "ad.align"): "" = an operand,
+# geometry field or flag the plain rows exercise, otherwise the mode whose rows exercise it.  A parameter that is not here fails
+# tests/test_host_logic_cpu.py.  p.order is the work-item order: order 1 in every row, order 0 in test_volume_item_order_0.
+NONCONV_KERNEL_PARAMS = {
+    "volume_kernel": {
+        **_plain("tgt_map total_items"),
+        **{"p." + f: "" for f in ("ref_g tgt_g ref_c tgt_c out B Cg Cc H W D G K Ctot oc_cat GU n_gwc_units n_cat_units w_tiles "
+                                  "d_chunks mask_left use_tma vec_ok order inv_k").split()},
+        "p.crop": "crop",
+    },
+    "softargmin_kernel": {**_plain("cost out D HW total alpha start step normalize"), "values": "var", "var_out": "var"},
+    "upsample_softargmin_kernel": {**_plain("cost out Dl Hl Wl D H W values"),
+                                   **{"%s.%s" % (a, f): "" for a in ("ad", "ah", "aw") for f in ("scale", "in", "align")}},
+    "epe_partial_kernel": _plain("pred gt out HW maxdisp"),
+    "gwc_volume_bwd_kernel": _plain("gvol ref tgt gref gtgt C H W D G s"),
+    "concat_volume_bwd_kernel": _plain("gvol gref gtgt C H W D mask_left"),
+    "softargmin_bwd_kernel": _plain("cost gout gcost D hw total alpha start step normalize"),
+    "geo_lookup_kernel": {
+        **{"p." + f: "" for f in "geo disp coords out B C D H W W2 levels radius".split()},
+        "p.corr": "geov",
+        **{"p." + f: "geomr" for f in "vol1 vol2 out1 out2 out_corr D1 D2".split()},
+    },
+    "avgpool_pairs_kernel": _plain("x y outer n inner"),
+    "context_upsample_kernel": _plain("disp up out h w s"),
+    "warped_volume_kernel": {
+        **{"p." + f: "" for f in ("xg yg xc yc disp out B Cg G K Cc D H W Ctot oc_cat n_gwc_units n_cat_units mask_left half_w "
+                                  "half_h").split()},
+        **{"p." + f: "warp" for f in "border wm1 hm1".split()},
+    },
+    "coex_regression_kernel": {"p." + f: "" for f in "cost spx out B D h w logits".split()},
+    "nearest_resize3d_kernel": _plain("x y total Di Hi Wi Do Ho Wo"),
+    "group_l2_normalize_kernel": _plain("x y K hw total eps"),
+    "sub_volume_kernel": _plain("l r out C H W D"),
+    "regression_values_kernel": _plain("prob values out D hw total"),
+    "ncdhw_to_ndhwc_kernel": {**_plain("x y C Cp vol"), "ys": "split", "overflow": "split", "ystride": "slice", "coff": "slice"},
 }
 
 
@@ -244,8 +304,34 @@ def _pow2(n):
     return n & (n - 1) == 0
 
 
+def crop_smem(C):
+    """Shared memory of an interlaced-crops CTA (volume.cu crop_smem_bytes): a left row of 128 + 1 and a right row of 192 + 1
+    floats per channel, and 16 bytes of mbarriers."""
+    return C * (129 + 193) * 4 + 16
+
+
+SMEM_OPT_IN = 227 * 1024
+
+
 # What each mode's rows must include between them (tests/test_host_logic_cpu.py): every requirement is met by at least one row.
 MODE_REQUIREMENTS = {
+    "crop": {
+        "three column tiles, the last one partial, and two disparity chunks": lambda r: 256 < r.shape[3] < 384 and r.shape[3] % 128
+        and 64 < r.shape[4] <= 128,
+        "D = W with W % 4 != 0 at C = 4": lambda r: r.shape[4] == r.shape[3] and r.shape[3] % 4 and r.shape[1] == 4,
+        "the largest C whose staged rows fit": lambda r: crop_smem(r.shape[1]) <= SMEM_OPT_IN < crop_smem(r.shape[1] + 4),
+        "MSNet2D's shape at 1/4 of 960": lambda r: r.shape[1:] == (32, 3, 240, 48),
+        "B > 1 at an odd width": lambda r: r.shape[0] > 1 and r.shape[3] % 2,
+    },
+    "var": {
+        "D = 1": lambda r: r.shape[1] == 1,
+        "-inf bins with a one-bin last chunk at D = 9": lambda r: r.shape[1] == 9 and r.opts.get("inf"),
+        "-inf bins with a one-bin last chunk at D = 193": lambda r: r.shape[1] == 193 and r.opts.get("inf"),
+        "offset 1e4 with spread 60": lambda r: r.opts.get("offset") == 1e4 and r.opts.get("spread") == 60.0,
+        "values (also run with var_out NULL)": lambda r: r.opts.get("values"),
+        "values NULL": lambda r: not r.opts.get("values"),
+        "a pixel count not a multiple of 256": lambda r: (r.shape[0] * r.shape[2] * r.shape[3]) % 256,
+    },
     "geov": {
         "radius 4 over 4 levels with taps that take the fallback read": lambda r: r.opts["radius"] == 4 and r.shape[5] == 4 and r.opts.get("cross"),
         "radius 4 at one level": lambda r: r.opts["radius"] == 4 and r.shape[5] == 1,
@@ -552,6 +638,9 @@ def cat_ref(ref, tgt, D, mask):
 
 
 def volume_variant(K, W, shift=(), y_off=0, gwc=True):
+    """osb_volume_last_variant() of a volume launch: vector stores when W % 4 == 0 and the left inputs and the output are 16-byte
+    aligned; TMA staging only for correlation units (gwc) with W % 4 == 0 and an aligned right input.  Concatenation-only launches,
+    the interlaced crops among them (K = 0, gwc = False), always stage with plain loads."""
     vec = W % 4 == 0 and y_off == 0 and not {"ref", "rc"} & set(shift)
     tma = gwc and W % 4 == 0 and "tgt" not in shift
     return "volume<%d,%d,%s>" % (vec, K % 4 == 0, "tma" if tma else "ldg")
@@ -563,6 +652,20 @@ def disp_mixture(g, shape, lo, hi):
     pick = torch.rand(shape, generator=g)
     u = torch.where(pick < 0.3, u.round(), u)
     return torch.where((pick >= 0.3) & (pick < 0.45), u.floor() + 0.5, u)
+
+
+def soft_cost(o, shape, g):
+    """Costs of the soft-argmin rows (B, D, H, W): offset + spread x U(-1, 1); peak_last puts the arg-max of every other row of
+    pixels in the last bin; inf sets about 40% of the bins to -inf, every pixel keeping bin D // 2 finite."""
+    B, D, H, W = shape
+    cost = o.get("offset", 0.0) + o.get("spread", 3.0) * (2 * torch.rand(B, D, H, W, generator=g) - 1)
+    if o.get("peak_last"):
+        cost[:, D - 1, ::2] += 0.5 * o.get("spread", 3.0) + 8.0
+    if o.get("inf"):
+        hit = torch.rand(B, D, H, W, generator=g) < 0.4
+        hit[:, D // 2] = False
+        cost = cost.masked_fill(hit, -math.inf)
+    return cost
 
 
 def cases(osb, row, g):
@@ -613,16 +716,64 @@ def cases(osb, row, g):
         }
         return [Case(row.id, want, scale, fns[e], inputs, exact=ex, info=dict(K=K, W=W, gwc=Cg > 0))]
 
+    if fam == "crop":
+        from oracle.msnet2d import interlaced_crops64
+        B, C, H, W, D = row.shape
+        rc, tc = per(rn(B, C, H, W), scales(C, g), 1), per(rn(B, C, H, W), scales(C, g), 1)
+        want = torch.cat([x.reshape(-1) for x in interlaced_crops64(rc, tc, D)])
+        fn = lambda y, P: call("osb_interlaced_crops_fwd", P("rc"), P("tc"), y, B, C, H, W, D, s())     # noqa: E731
+        return [Case(row.id, want, None, fn, {"rc": rc, "tc": tc}, exact=torch.ones(want.shape, dtype=torch.bool),
+                     info=dict(K=0, W=W, gwc=False))]
+
+    if fam == "var":
+        B, D, H, W = row.shape
+        n = B * H * W
+        cost = soft_cost(o, row.shape, g)
+        inputs = {"cost": cost}
+        if o.get("values"):                                         # sorted, non-integer, some negative
+            lo = 200.0 * torch.rand(B, 1, H, W, generator=g) - 20.0
+            inputs["values"] = lo + torch.sort(3.0 * D * torch.rand(B, D, H, W, generator=g), dim=1).values
+            v = inputs["values"].double()
+        else:
+            v = torch.arange(D, dtype=F64).view(1, D, 1, 1).expand(B, D, H, W)
+        x = cost.double()                                           # the kernel reads the logits as they are: no rounding
+        p = torch.softmax(x, 1)
+        mu = (p * v).sum(1)
+        dev2 = (v - mu.unsqueeze(1)) ** 2
+        var = (p * dev2).sum(1)
+        none = torch.zeros_like(x)
+        e_mu = soft_model(p, x, v, mu, none, 0)
+        # summed about the kernel's mean m: sum p (v - m)^2 = var + (m - mu)^2, and |m - mu| <= TOL_SOFT e_mu
+        e_var = soft_model(p, x, dev2, var, none, 0) + TOL_SOFT * e_mu ** 2
+        want, scale = torch.stack([mu, var]), torch.stack([e_mu, e_var])
+        exact = torch.full(want.shape, D == 1)                      # p = 1: the mean is v_0 and the variance 0, both exact
+        no_var = torch.zeros(want.shape, dtype=torch.bool)
+        no_var[1] = True                                            # the variance region: a mean-only launch leaves it unwritten
+
+        def vals(P):
+            return P("values") if "values" in inputs else None
+
+        def full(y, P):                                             # mean at y, variance after it
+            call("osb_softargmin_var_fwd", P("cost"), vals(P), y, y + 4 * n, B, D, H, W, s())
+
+        def mean_only(y, P):
+            call("osb_softargmin_var_fwd", P("cost"), vals(P), y, None, B, D, H, W, s())
+
+        def plain(y, P):
+            call("osb_softargmin_fwd", P("cost"), y, B, D, H, W, 1.0, 0.0, 1.0, 1, s())
+        # same_as: the mean must equal the first case's mean bit for bit
+        out = [Case(row.id, want, scale, full, inputs, tol=TOL_SOFT, exact=exact),
+               Case(row.id + " var_out NULL", want, scale, mean_only, inputs, tol=TOL_SOFT, exact=exact, skip=no_var,
+                    info=dict(same_as=row.id))]
+        if "values" not in inputs:                                  # both NULL above: that is the plain kernel's launch
+            out.append(Case(row.id + " osb_softargmin_fwd", want, scale, plain, inputs, tol=TOL_SOFT, exact=exact, skip=no_var,
+                            info=dict(same_as=row.id)))
+        return out
+
     if fam == "sa":
         B, D, H, W = row.shape
         alpha, start, step, norm = o.get("alpha", 1.0), o.get("start", 0.0), o.get("step", 1.0), o.get("norm", 1)
-        cost = o.get("offset", 0.0) + o.get("spread", 3.0) * (2 * torch.rand(B, D, H, W, generator=g) - 1)
-        if o.get("peak_last"):
-            cost[:, D - 1, ::2] += 0.5 * o.get("spread", 3.0) + 8.0
-        if o.get("inf"):
-            hit = torch.rand(B, D, H, W, generator=g) < 0.4
-            hit[:, D // 2] = False                                  # every pixel keeps a finite bin
-            cost = cost.masked_fill(hit, -math.inf)
+        cost = soft_cost(o, row.shape, g)
         x = (cost * f32(alpha)).double()                            # the fp32 logits
         v = (f32(start) + f32(step) * torch.arange(D, dtype=torch.float32)).double().view(1, D, 1, 1)
         v = v.expand(B, D, H, W)
@@ -873,16 +1024,17 @@ def cases(osb, row, g):
             return taps, mg
         masked = (fw < disp).unsqueeze(1)                                    # (B, 1, D, H, W)
         parts, mags, exact, inputs = [], [], [], {"xc": xc, "yc": yc, "disp": disp}
+        mask_left = o.get("mask", 1) if Cg else o.get("mask", 0)             # with Cg > 0 it masks the correlation too
         if Cg:
             xg, yg = per(rn(B, Cg, H, W), scales(Cg, g), 1), per(rn(B, Cg, H, W), scales(Cg, g), 1)
             tg, mg = warp(yg)
             xl = xg.double().unsqueeze(2)
             vol = (xl * tg).view(B, G, K, D, H, W).sum(2) / K
             vm = (xl.abs() * mg).view(B, G, K, D, H, W).sum(2) / K
-            vol = vol.masked_fill(masked, 0.0)
-            parts.append(vol), mags.append(chanmax(vm, 1)), exact.append(masked.expand(vol.shape))
+            zeros = masked if mask_left else torch.zeros_like(masked)
+            vol = vol.masked_fill(zeros, 0.0)
+            parts.append(vol), mags.append(chanmax(vm, 1)), exact.append(zeros.expand(vol.shape))
             inputs.update(xg=xg, yg=yg)
-        mask_left = 1 if Cg else o.get("mask", 0)
         left = xc.double().unsqueeze(2).expand(B, Cc, D, H, W)
         if mask_left:
             left = left.masked_fill(masked, 0.0)
@@ -892,7 +1044,10 @@ def cases(osb, row, g):
         exact += [torch.ones(left.shape, dtype=torch.bool), torch.zeros(tc.shape, dtype=torch.bool)]
         want = torch.cat(parts, 1)
         scale = torch.cat([m.expand(1, p.shape[1], 1, 1, 1) for m, p in zip(mags, parts)], 1)
-        if Cg:
+        if Cg and "mask" in o:
+            fn = lambda y, P: call("osb_warped_gwc_concat_volume_ex_fwd", P("xg"), P("yg"), P("xc"), P("yc"), P("disp"), y, B, Cg,  # noqa
+                                   G, Cc, D, H, W, mask_left, s())
+        elif Cg:
             fn = lambda y, P: call("osb_warped_gwc_concat_volume_fwd", P("xg"), P("yg"), P("xc"), P("yc"), P("disp"), y, B, Cg, G,  # noqa
                                    Cc, D, H, W, s())
         else:
@@ -1042,6 +1197,8 @@ def runs_of(row, case):
             runs += [("out+4", {"y_off": 1}, 0), ("ref+4", {"shift": ("ref", "rc")}, 0), ("tgt+4", {"shift": ("tgt", "tc")}, 0),
                      ("ref+4 tgt+4", {"shift": ("ref", "rc", "tgt", "tc")}, 0)]
         runs += [("grid cap 1", {}, 1), ("grid cap 5", {}, 5)]
+    if row.fam == "crop":                       # a moved output is refused (test_refusals); a moved left input drops vec_ok
+        runs += [("rc+4", {"shift": ("rc",)}, 0), ("tc+4", {"shift": ("tc",)}, 0), ("grid cap 1", {}, 1), ("grid cap 5", {}, 5)]
     if row.fam == "ctx" and case.info["vec"]:
         runs += [("out+4", {"y_off": 1}, 0), ("up+4", {"shift": ("up",)}, 0)]
     return runs
@@ -1052,13 +1209,14 @@ def runs_of(row, case):
 def test_accuracy_store_paths_bounds_determinism(osb, grid_cap, row):
     _, ops = osb
     worst = 0.0
+    firsts = {}
     for case in cases(osb, row, seed(row)):
         first = None
         for label, kw, cap in runs_of(row, case):
             what = "%s, %s" % (case.name, label)
             grid_cap(cap)
             buf, lead = case.launch(**kw)
-            if row.fam == "vol":
+            if row.fam in ("vol", "crop"):
                 want_v = volume_variant(case.info["K"], case.info["W"], kw.get("shift", ()), kw.get("y_off", 0), case.info["gwc"])
                 assert ops.volume_last_variant() == want_v, "%s: ran %s, expected %s" % (what, ops.volume_last_variant(), want_v)
             worst = max(worst, case.check(buf, lead, what))
@@ -1070,7 +1228,12 @@ def test_accuracy_store_paths_bounds_determinism(osb, grid_cap, row):
             else:
                 diff = (first.double() - inner.double()).abs().view(case.want.shape)
                 assert (diff <= 2 * case.det_scale).all(), "%s: repeated launches differ beyond the bar of the sum" % what
-    print("\n%-22s %-5s worst err/scale %.2e (bar %g)" % (row.id, row.fam, worst, TOL_SOFT if row.fam in ("sa", "up", "bsa", "coex")
+        firsts[case.name] = first
+        if "same_as" in case.info:              # the written elements must equal that case's bit for bit
+            other, live = firsts[case.info["same_as"]], ~case.skip.flatten()
+            assert torch.equal(first[live].view(torch.int32), other[live].view(torch.int32)), "%s: differs bit-wise from %s" % (
+                case.name, case.info["same_as"])
+    print("\n%-22s %-5s worst err/scale %.2e (bar %g)" % (row.id, row.fam, worst, TOL_SOFT if row.fam in ("sa", "var", "up", "bsa", "coex")
                                                           else (1.0 if row.fam == "epe" else TOL)))
 
 
@@ -1110,26 +1273,56 @@ def test_routing(osb, row):
 
 @pytest.mark.timeout(300)
 def test_volume_item_order_0(osb, tmp_path):
-    """OSB_VOLUME_ORDER=0 (unit fastest) is read once per process: a child process computes a fused row in that order, and its
-    output must equal order 1's bit for bit.  subprocess.run waits for the child and kills it on timeout."""
-    row = BY_ID["vol-fused-k4"]
-    case = cases(osb, row, seed(row))[0]
-    buf, lead = case.launch()
-    case.check(buf, lead, "order 1")
-    mine = buf[lead:lead + case.numel].cpu()
-    B, G, K, Cc, H, W, D = row.shape
-    torch.save({k: v for k, v in case.inputs.items()}, str(tmp_path / "in.pt"))
+    """OSB_VOLUME_ORDER=0 (unit fastest) is read once per process: a child process computes a fused row and a crop row in that
+    order, and each output must equal order 1's bit for bit; the crops go through ops.interlaced_crops, whose views must be the
+    (B, H, W - d, 2C) images back to back.  subprocess.run waits for the child and kills it on timeout."""
+    mine = {}
+    for rid in ("vol-fused-k4", "crop-w260-d70"):
+        row = BY_ID[rid]
+        case = cases(osb, row, seed(row))[0]
+        buf, lead = case.launch()
+        case.check(buf, lead, "%s, order 1" % rid)
+        mine[rid] = buf[lead:lead + case.numel].cpu()
+        torch.save({k: v for k, v in case.inputs.items()}, str(tmp_path / ("%s.pt" % rid)))
+    B, G, K, Cc, H, W, D = BY_ID["vol-fused-k4"].shape
+    cB, cC, cH, cW, cD = BY_ID["crop-w260-d70"].shape
     script = ("import sys, torch\n"
               "from openstereo_b200 import ops\n"
-              "t = torch.load(sys.argv[1] + '/in.pt')\n"
+              "t = torch.load(sys.argv[1] + '/vol-fused-k4.pt')\n"
               "c = {k: v.cuda() for k, v in t.items()}\n"
               "out = ops.gwc_concat_volume(c['ref'], c['tgt'], c['rc'], c['tc'], %d, %d)\n"
-              "torch.save(out.cpu(), sys.argv[1] + '/out.pt')\n" % (D, G))
+              "torch.save(out.cpu(), sys.argv[1] + '/vol-fused-k4.out.pt')\n"
+              "t = torch.load(sys.argv[1] + '/crop-w260-d70.pt')\n"
+              "views = ops.interlaced_crops(t['rc'].cuda(), t['tc'].cuda(), %d)\n"
+              "torch.save([v.cpu() for v in views], sys.argv[1] + '/crop-w260-d70.out.pt')\n" % (D, G, cD))
     env = dict(os.environ, OSB_VOLUME_ORDER="0", PYTHONPATH=os.pathsep.join([ROOT] + [p for p in [os.environ.get("PYTHONPATH")] if p]))
     res = subprocess.run([sys.executable, "-c", script, str(tmp_path)], env=env, cwd=ROOT, timeout=240, capture_output=True, text=True)
     assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-2000:]
-    other = torch.load(str(tmp_path / "out.pt")).flatten()
-    assert torch.equal(other.view(torch.int32), mine.view(torch.int32)), "order 0 and order 1 differ"
+    other = torch.load(str(tmp_path / "vol-fused-k4.out.pt")).flatten()
+    assert torch.equal(other.view(torch.int32), mine["vol-fused-k4"].view(torch.int32)), "fused volume: order 0 and order 1 differ"
+    views = torch.load(str(tmp_path / "crop-w260-d70.out.pt"))
+    assert [tuple(v.shape) for v in views] == [(cB, cH, cW - d, 2 * cC) for d in range(cD)]
+    other = torch.cat([v.flatten() for v in views])
+    assert torch.equal(other.view(torch.int32), mine["crop-w260-d70"].view(torch.int32)), "crops: order 0 and order 1 differ"
+
+
+@pytest.mark.timeout(120)
+def test_warped_ex_mask_left_1(osb):
+    """osb_warped_gwc_concat_volume_ex_fwd with mask_left = 1 passes the masked cas model and is osb_warped_gwc_concat_volume_fwd
+    bit for bit, on both instantiations, with the inputs of the unmasked rows."""
+    lib, _ = osb
+    for rid in ("cas-gwc-k8-unmasked", "cas-gwc-wmax-unmasked"):
+        row = BY_ID[rid]
+        B, Cg, G, Cc, D, H, W = row.shape
+        case = cases(osb, row._replace(opts=dict(row.opts, mask=1)), seed(row))[0]      # the _ex launch, the masked model
+        ex, lead = case.launch()
+        case.check(ex, lead, "%s, mask_left = 1" % rid)
+        dev = case.dev()
+        buf = case.guarded()
+        lib.call("osb_warped_gwc_concat_volume_fwd", *(dev[k].data_ptr() for k in ("xg", "yg", "xc", "yc", "disp")),
+                 buf.data_ptr() + 4 * GUARD, B, Cg, G, Cc, D, H, W, torch.cuda.current_stream().cuda_stream)
+        torch.cuda.synchronize()
+        assert torch.equal(ex.view(torch.int32), buf.view(torch.int32)), "%s: _ex with mask_left = 1 differs from the cascade entry" % rid
 
 
 @pytest.mark.timeout(120)
@@ -1180,8 +1373,24 @@ def refusals(P, s):
         """geo0..3, vol1, vol2, corr0..3, disp, coords, out0, out1, out2, out_corr"""
         return (P,) * 4 + (vol1, P) + (P,) * 4 + (P, P, P, P, P, out_corr)
     cx, cg, dw = "osb_warped_concat_volume_fwd", "osb_warped_gwc_concat_volume_fwd", "osb_disp_warp_fwd"
+    cgx = "osb_warped_gwc_concat_volume_ex_fwd"
     co = "osb_coex_regression_fwd"
+    ic, sv = "osb_interlaced_crops_fwd", "osb_softargmin_var_fwd"
     return [
+        ("interlaced_crops C 6", ic, (P, P, P, 1, 6, 2, 16, 4, s)),
+        ("interlaced_crops C 184", ic, (P, P, P, 1, 184, 2, 16, 4, s)),            # 237 008 bytes of staged rows
+        ("interlaced_crops D 0", ic, (P, P, P, 1, 8, 2, 16, 0, s)),
+        ("interlaced_crops D 17 > W 16", ic, (P, P, P, 1, 8, 2, 16, 17, s)),
+        ("interlaced_crops out+4", ic, (P, P, mis, 1, 8, 2, 16, 4, s)),
+        ("interlaced_crops null right", ic, (P, None, P, 1, 8, 2, 16, 4, s)),
+        ("softargmin_var null cost", sv, (None, None, P, P, 1, 4, 2, 2, s)),
+        ("softargmin_var null output", sv, (P, None, None, P, 1, 4, 2, 2, s)),
+        ("softargmin_var D 0", sv, (P, None, P, P, 1, 0, 2, 2, s)),
+        ("softargmin_var empty B", sv, (P, P, P, None, 0, 4, 2, 2, s)),
+        ("warped_gwc_ex mask_left 2", cgx, (P, P, P, P, P, P, 1, 16, 2, 4, 2, 4, 8, 2, s)),
+        ("warped_gwc_ex K 17", cgx, (P, P, P, P, P, P, 1, 17, 1, 4, 2, 4, 8, 0, s)),
+        ("warped_gwc_ex W 1817", cgx, (P, P, P, P, P, P, 1, 16, 1, 1, 2, 2, 1817, 0, s)),
+
         ("gwc_volume empty W", "osb_gwc_volume_fwd", (P, P, P, 1, 8, 4, 0, 4, 2, s)),
         ("gwc_volume empty D", "osb_gwc_volume_fwd", (P, P, P, 1, 8, 4, 8, 0, 2, s)),
         ("gwc_volume C % G", "osb_gwc_volume_fwd", (P, P, P, 1, 9, 4, 8, 4, 2, s)),
@@ -1269,12 +1478,24 @@ def refusals(P, s):
 
 @pytest.mark.timeout(60)
 def test_refusals(osb):
-    lib, _ = osb
+    lib, ops = osb
     buf = torch.zeros(1 << 20, device="cuda")                   # 4 MB: every argument list above stays inside it
     torch.cuda.synchronize()
-    for what, name, args in refusals(buf.data_ptr(), torch.cuda.current_stream().cuda_stream):
+    s = torch.cuda.current_stream().cuda_stream
+    for what, name, args in refusals(buf.data_ptr(), s):
         before = lib.launch_count()
         rc = getattr(lib.lib, name)(*args)
         assert rc == OSB_EINVAL, "%s: %s returned %d, expected %d (%s)" % (what, name, rc, OSB_EINVAL, lib.lib.osb_last_error())
         assert lib.launch_count() == before, "%s: a refused call launched a kernel" % what
+    small = torch.zeros(1, 8, 2, 16, device="cuda")
+    for c, nd in ((184, 4), (6, 4), (8, 0), (8, 17)):           # ops.interlaced_crops refuses the same shapes before any launch
+        before = lib.launch_count()
+        with pytest.raises(ValueError, match="interlaced_crops"):
+            ops.interlaced_crops(small.new_zeros(1, c, 2, 16), small.new_zeros(1, c, 2, 16), nd)
+        assert lib.launch_count() == before, "ops.interlaced_crops C %d ndisp %d launched a kernel" % (c, nd)
+    # a valid launch after every refusal: OSB_OK, so no refused call left a CUDA error for the next launch's check to report
+    before = lib.launch_count()
+    rc = lib.lib.osb_interlaced_crops_fwd(small.data_ptr(), small.data_ptr(), buf.data_ptr(), 1, 8, 2, 16, 4, s)
+    assert rc == OSB_OK, "a valid launch after the refusals returned %d (%s)" % (rc, lib.lib.osb_last_error())
+    assert lib.launch_count() == before + 1
     torch.cuda.synchronize()

@@ -4,7 +4,8 @@
   imported read-only) re-run with act = OSB_ACT_MISH against fp64 conv + BN (+ residual) + Mish (+ gate) from the same fp32 inputs:
   error per output channel <= 1e-5 x the channel's max sum |terms| plus four ulp of Mish, both store paths, output inside
   NaN-filled regions between sentinels, determinism; the instance-norm, tensor-core, 2D and channels-last entry points refuse 6.
-* Variance mode of the soft-argmin (osb_softargmin_var_fwd) against fp64, bit-identical to osb_softargmin_fwd without values.
+* The variance mode of the soft-argmin (osb_softargmin_var_fwd) is a row family of tests/test_kernel_contract_gpu.py ("var"), as
+  are the unmasked warped volume at fractional samples (the cas rows with mask = 0) and both entry points' refusals.
 * The warped volume with the left copy unmasked at CFNet's integer samples against the reference's SpatialTransformer +
   groupwise_correlation_4D + cat, and bit-identical to osb_warped_gwc_concat_volume_fwd with mask_left = 1.
 * Each engine stage and the whole patched model against the reference (cuDNN fp32, TF32 off), and the guard.
@@ -146,79 +147,6 @@ def test_mish_refused_elsewhere(osb):
         with pytest.raises(ValueError, match="activation"):
             lib.call(name, *args)
         assert lib.launch_count() == before, name
-
-
-# ------------------------------------------------------------------------------------------------------- soft-argmin variance
-GUARD, SENT = cc.GUARD, cc.SENTINEL
-
-
-def _guarded(n):
-    buf = torch.full((GUARD + n + GUARD,), SENT, device="cuda")
-    buf[GUARD:GUARD + n] = float("nan")
-    return buf
-
-
-def _check_guarded(buf, n, what):
-    bits = buf.view(torch.int32)
-    sent = torch.tensor([SENT]).view(torch.int32).item()
-    assert (bits[:GUARD] == sent).all() and (bits[GUARD + n:] == sent).all(), "%s: a store left the output region" % what
-    assert not torch.isnan(buf[GUARD:GUARD + n]).any(), "%s: output elements never written" % what
-    return buf[GUARD:GUARD + n]
-
-
-@pytest.mark.parametrize("d", [6, 12, 16, 24, 48])
-@pytest.mark.parametrize("kind", ["planes", "samples", "large"])
-def test_softargmin_variance(osb, d, kind):
-    from oracle.cfnet import softargmin_var64
-    lib, _ = osb
-    g = torch.Generator().manual_seed(1000 * d + len(kind))
-    b, h, w = 2, 7, 37
-    cost = torch.randn(b, d, h, w, generator=g) * 3
-    values = None
-    if kind != "planes":                                         # CFNet's samples: sorted integers, floor / ceil at the ends
-        lo = torch.randint(0, 200, (b, 1, h, w), generator=g).float()
-        values = lo + torch.sort(torch.randint(0, 3 * d, (b, d, h, w), generator=g).float(), dim=1).values
-    if kind == "large":
-        cost = cost * 50 + 1000
-    want_mu, want_var = softargmin_var64(cost, values)
-    n = b * h * w
-    cd = cost.cuda()
-    vd = None if values is None else values.cuda()
-    mu_buf, var_buf = _guarded(n), _guarded(n)
-    lib.call("osb_softargmin_var_fwd", cd.data_ptr(), cc.ptr(vd), mu_buf.data_ptr() + 4 * GUARD, var_buf.data_ptr() + 4 * GUARD,
-             b, d, h, w, _stream())
-    torch.cuda.synchronize()
-    mu = _check_guarded(mu_buf, n, "mean").double().cpu().view(b, h, w)
-    var = _check_guarded(var_buf, n, "variance").double().cpu().view(b, h, w)
-    vmax = float(d - 1 if values is None else values.abs().max())
-    eps = 2.0 ** -24
-    assert float((mu - want_mu).abs().max()) <= 16 * eps * vmax, float((mu - want_mu).abs().max())
-    bar = 1e-5 * want_var + (16 * eps * vmax) ** 2 + 16 * eps * want_var
-    assert bool(((var - want_var).abs() <= bar).all()), float(((var - want_var).abs() / bar).max())
-    # determinism, and the mean without values is the plain kernel's bit for bit
-    mu2, var2 = torch.empty(n, device="cuda"), torch.empty(n, device="cuda")
-    lib.call("osb_softargmin_var_fwd", cd.data_ptr(), cc.ptr(vd), mu2.data_ptr(), var2.data_ptr(), b, d, h, w, _stream())
-    assert torch.equal(mu2.view(torch.int32).cpu(), mu_buf[GUARD:GUARD + n].view(torch.int32).cpu())
-    assert torch.equal(var2.view(torch.int32).cpu(), var_buf[GUARD:GUARD + n].view(torch.int32).cpu())
-    if values is None:
-        plain = torch.empty(n, device="cuda")
-        lib.call("osb_softargmin_fwd", cd.data_ptr(), plain.data_ptr(), b, d, h, w, 1.0, 0.0, 1.0, 1, _stream())
-        nul = torch.empty(n, device="cuda")
-        lib.call("osb_softargmin_var_fwd", cd.data_ptr(), None, nul.data_ptr(), None, b, d, h, w, _stream())
-        torch.cuda.synchronize()
-        assert torch.equal(plain.view(torch.int32), nul.view(torch.int32)), "both pointers NULL: not the plain kernel's bits"
-        assert torch.equal(plain.view(torch.int32), mu2.view(torch.int32)), "the mean differs from the plain kernel's"
-
-
-def test_softargmin_variance_refusals(osb):
-    lib, _ = osb
-    t = torch.zeros(64, device="cuda")
-    p = t.data_ptr()
-    for args in ((None, None, p, p, 1, 4, 2, 2), (p, None, None, p, 1, 4, 2, 2), (p, None, p, p, 1, 0, 2, 2), (p, p, p, None, 0, 4, 2, 2)):
-        before = lib.launch_count()
-        with pytest.raises(ValueError):
-            lib.call("osb_softargmin_var_fwd", *args, _stream())
-        assert lib.launch_count() == before
 
 
 # --------------------------------------------------------------------------------------------------------------- warped volume

@@ -1,8 +1,8 @@
 """GPU: MSNet2D on the library (aggregation.MSNet2DVolume / MSNet2DAggregation) and the interlaced-crop mode of the volume kernel.
 
-* osb_interlaced_crops_fwd against the fp64 gather of oracle/msnet2d.py: bit-exact (a copy), at widths whose late crops fall below
-  the tensor-core width floor, inside a NaN-guarded buffer (nothing written outside the images); the existing volume entry points
-  with the mode off still give exact copies / the oracle's correlations.
+* osb_interlaced_crops_fwd is a row family of tests/test_kernel_contract_gpu.py ("crop": bit-exact against the fp64 gather of
+  oracle/msnet2d.py in a NaN-guarded buffer, both staging instantiations, grid caps, the other item order, the refusals); here the
+  existing volume entry points with the mode off still give exact copies / the oracle's correlations.
 * The volume front end against the reference's own 48-iteration loop in fp64: per voxel the error stays below 1e-4 times the
   largest voxel plus 1e-5, and every voxel with w < d is exactly 0.  Crops below OSB_TC_MIN_WIDTH take the CUDA-core kernels.
 * The aggregation stage and the whole patched model against the unpatched model (cuDNN fp32, TF32 off): EPE <= 1e-3 px at
@@ -35,41 +35,6 @@ def _fp32_reference():
 def _feats(b, c, h, w, seed):
     g = torch.Generator().manual_seed(seed)
     return torch.randn(b, c, h, w, generator=g), torch.randn(b, c, h, w, generator=g)
-
-
-@pytest.mark.parametrize("shape", [(2, 32, 3, 40, 40), (1, 32, 5, 128, 48), (3, 8, 2, 61, 17), (1, 4, 1, 5, 5)])
-def test_crops_exact_and_guarded(osb, shape):
-    _lib, _, ops = osb
-    from oracle.msnet2d import interlaced_crops64
-    b, c, h, w, nd = shape
-    fl, fr = _feats(b, c, h, w, seed=w)
-    want = interlaced_crops64(fl, fr, nd)
-    total = sum(x.numel() for x in want)
-    guard = 256
-    buf = torch.full((guard + total + guard,), float("nan"), device="cuda")
-    flc, frc = fl.cuda(), fr.cuda()
-    rc = _lib.lib.osb_interlaced_crops_fwd(flc.data_ptr(), frc.data_ptr(), buf[guard:].data_ptr(), b, c, h, w, nd,
-                                           torch.cuda.current_stream().cuda_stream)
-    assert rc == 0
-    torch.cuda.synchronize()
-    assert torch.isnan(buf[:guard]).all() and torch.isnan(buf[guard + total:]).all(), "a store left the images"
-    got = buf[guard:guard + total].cpu()
-    assert torch.equal(got, torch.cat([x.float().reshape(-1) for x in want]))
-    views = ops.interlaced_crops(flc, frc, nd)
-    assert [tuple(v.shape) for v in views] == [(b, h, w - d, 2 * c) for d in range(nd)]
-    assert all(torch.equal(v.cpu(), x.float()) for v, x in zip(views, want))
-
-
-def test_crops_refusals(osb):
-    _lib, _, ops = osb
-    fl, fr = (t.cuda() for t in _feats(1, 32, 2, 16, seed=0))
-    s = torch.cuda.current_stream().cuda_stream
-    out = torch.empty(1 << 16, device="cuda")
-    for args in ((1, 30, 2, 16, 4), (1, 32, 2, 16, 17), (1, 32, 2, 16, 0)):
-        assert _lib.lib.osb_interlaced_crops_fwd(fl.data_ptr(), fr.data_ptr(), out.data_ptr(), *args, s) != 0
-    assert _lib.lib.osb_interlaced_crops_fwd(fl.data_ptr(), fr.data_ptr(), out.data_ptr() + 4, 1, 32, 2, 16, 4, s) != 0
-    with pytest.raises(ValueError):
-        ops.interlaced_crops(fl, fr, 17)
 
 
 def test_existing_volumes_unchanged(osb):
