@@ -3,7 +3,7 @@ MEASUREMENT INFRASTRUCTURE -- see oracle/__init__.py).
 
 * ``aanet(yaml, seed, offset_scale)``  the reference's ``aanet``, eval mode, from an unchanged YAML with seeded parameters.  Its
   submodule imports ``stereo.libs.AANet.deform_conv``, whose wrapper imports the compiled ``deform_conv_cuda`` extension as a
-  sibling module; ``load_reference`` registers the build that oracle/make_ref_aanet.py staged under oracle/_ref/ under that name
+  sibling module; ``load_reference`` registers the build that oracle/make_ref.py staged under oracle/_ref/ under that name
   first, so the import succeeds from the live reference tree and from the staged copy alike.  The seeded ``offset_conv`` weights
   and biases are multiplied by ``offset_scale``: the reference initialises them to zero, which makes every deformable layer a plain
   dilated convolution with mask 1 and would leave the gather untested.
@@ -19,18 +19,10 @@ import torch
 
 from oracle import _reference_shim as shim
 from oracle import seeded_init as si
+from oracle.make_ref import extension_path
 
 EVAL_YAML = "cfgs/aanet/aanet_sceneflow.yaml"
 _EXT = "stereo.libs.AANet.deform_conv.deform_conv_cuda"
-
-
-def extension_path():
-    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    try:
-        import make_ref_aanet
-    finally:
-        sys.path.pop(0)
-    return make_ref_aanet.extension_path()
 
 
 def extension_available():
@@ -42,7 +34,7 @@ def load_reference(dotted):
     if _EXT not in sys.modules:
         path = extension_path()
         if not os.path.exists(path):
-            raise RuntimeError("the reference's deform_conv_cuda is not built (%s): run oracle/make_ref_aanet.py" % path)
+            raise RuntimeError("the reference's deform_conv_cuda is not built (%s): run oracle/make_ref.py" % path)
         spec = importlib.util.spec_from_file_location(_EXT, path)
         mod = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(mod)
